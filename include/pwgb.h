@@ -1,5 +1,5 @@
 /*
- * pwgb.h -- C ABI of the B200-native vocoder hot path (libpwgb.so).
+ * pwgb.h -- C ABI of the H100-native vocoder hot path (libpwgb.so).
  *
  * The reference (kan-bayashi/ParallelWaveGAN) has no FFI of its own: its seam is
  * the torch.nn.Module surface (SURVEY.md 8b).  Each entry point below replaces
@@ -108,18 +108,17 @@ PWGB_API int pwgb_conv_transpose1d_forward(const pwgb_convtr1d_desc* d, const fl
                                   float* y, void* ws, size_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------------
- * tcgen05 (5th-gen tensor core) path for the wide stride-1 convolutions: same descriptor
+ * Tensor-core (Hopper wgmma) path for the wide stride-1 convolutions: same descriptor
  * and semantics as pwgb_conv1d_forward, fp32-accurate through a bf16x3 operand split with
- * fp32 TMEM accumulation.  Weights are re-laid out once per weight update by
+ * fp32 register accumulation.  Weights are re-laid out once per weight update by
  * pwgb_conv1d_tc_pack_weight into a caller-owned buffer of
  * pwgb_conv1d_tc_packed_weight_bytes().  pwgb_conv1d_tc_supported() returns 1 when the
  * configuration can run here (stride 1, cin/groups % 32 == 0, cout/groups % 16 == 0, halo fits shared
- * memory; cout/groups > 256 and groups > 1 run as several launches); everything else stays on
+ * memory; cout/groups > 128 and groups > 1 run as several column chunks of one launch); everything else stays on
  * pwgb_conv1d_forward.
  * ---------------------------------------------------------------------- */
-/* bring-up / measurement aids (not part of the product contract): set key 1 = tcgen05 descriptor variant, key 2 = timing
- * variants of the fused WaveNet kernel (bit 64: record a per-role timeline of CTA 0); get key 2 = that timeline
- * (8 roles x 32 tiles x 4 stamps, int64 SM clocks), returns bytes copied or -1. */
+/* measurement aids (not part of the product contract): set key 1 = conv variant (bit 1: stage activations with
+ * cp.async instead of TMA); get returns -1 (no read-back available). */
 PWGB_API void pwgb_debug_set(int key, int value);
 PWGB_API int pwgb_debug_get(int key, void* dst, size_t bytes);
 PWGB_API size_t pwgb_conv1d_tc_packed_weight_bytes(int cin, int cout, int kernel);
@@ -137,7 +136,7 @@ PWGB_API int pwgb_conv1d_tc_forward(const pwgb_conv1d_desc* d, const float* x, c
  *     g  = conv_{k,dilation}(x) + W_aux c (+ b_conv)
  *     z  = tanh(g[:G/2]) * sigmoid(g[G/2:])
  *     skips += W_skip z + b_skip ;   x_out = (W_out z + b_out + x) * sqrt(0.5)
- * on the tcgen05 path (bf16x3, fp32 accumulate).  `c` must be stored with `aux_channels`
+ * on the tensor-core path (bf16x3, fp32 accumulate).  `c` must be stored with `aux_channels`
  * channels, a multiple of 32 (zero-padded beyond the model's real aux_channels; the pack
  * routine zero-fills the matching weight columns).  g_ws: workspace of batch*G*t floats.
  * b_skip_out = concat(b_skip, b_out) or NULL.  pwgb_wavenet_supported() == 0 means the caller
@@ -298,7 +297,7 @@ PWGB_API int pwgb_avg_pool1d_forward(const float* x, float* y, int rows, int t_i
 
 /* ------------------------------------------------------------------------
  * Backward building blocks of the train step (bin/train.py:287-288, 327-328 `loss.backward()`).
- * Data gradients reuse the forward entry points: the dgrad of a stride-1 conv is the conv1d forward entry point (FFMA or tcgen05)
+ * Data gradients reuse the forward entry points: the dgrad of a stride-1 conv is the conv1d forward entry point (FFMA or tensor cores)
  * with the transposed, tap-flipped weight; the dgrad of a strided / grouped / period conv is
  * pwgb_conv_transpose1d_forward (groups / period fields); the dgrad of a conv-transpose is a strided
  * pwgb_conv1d_forward.  New here:
@@ -313,7 +312,7 @@ PWGB_API int pwgb_avg_pool1d_forward(const float* x, float* y, int rows, int t_i
 PWGB_API size_t pwgb_conv1d_wgrad_workspace(const pwgb_conv1d_desc* d);
 PWGB_API int pwgb_conv1d_wgrad(const pwgb_conv1d_desc* d, const float* x, const float* gy, float g_slope, float* dw,
                       int accumulate, void* ws, size_t ws_bytes, void* stream);
-/* tcgen05 variant (stride 1, groups 1, period 1, zero padding, cout % 8 == 0 (>= 32), cin % 32 == 0): the
+/* tensor-core variant (stride 1, groups 1, period 1, zero padding, cout % 8 == 0 (>= 32), cin % 32 == 0): the
  * reduction over time is the MMA K dimension, both operands MN-major; same result contract. */
 PWGB_API int pwgb_conv1d_wgrad_tc_supported(const pwgb_conv1d_desc* d);
 PWGB_API size_t pwgb_conv1d_wgrad_tc_workspace(const pwgb_conv1d_desc* d);

@@ -1,4 +1,4 @@
-"""parallelwavegan_b200 -- B200-native (sm_100a) vocoder hot path behind the
+"""parallelwavegan_b200 -- H100-native (sm_90a) vocoder hot path behind the
 ``parallel_wavegan`` model/loss API.
 
 ``models`` / ``layers`` / ``losses`` mirror the reference namespaces (classes are

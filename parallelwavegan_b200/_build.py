@@ -1,4 +1,4 @@
-"""Build libpwgb.so in-tree with nvcc for sm_100a (no torch headers: pure C ABI)."""
+"""Build libpwgb.so in-tree with nvcc for sm_90a (no torch headers: pure C ABI)."""
 import hashlib
 import os
 import subprocess
@@ -14,7 +14,7 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
 def _flags():
     return [
-        "-gencode", "arch=compute_100a,code=sm_100a",
+        "-gencode", "arch=compute_90a,code=sm_90a",
         "-O3", "-lineinfo", "-std=c++17",
         "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
         "-I", os.path.join(ROOT, "include"), "-I", CSRC,
@@ -58,7 +58,7 @@ def build(force=False, verbose=False):
             sys.stderr.write(out)
     if fail:
         raise RuntimeError("nvcc failed building libpwgb.so")
-    cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+    cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
     subprocess.check_call(cmd)
     with open(stamp, "w") as fh:
         fh.write(dig)

@@ -1,6 +1,6 @@
 """torch.autograd glue for the train step (bin/train.py:189-340): every Function's forward AND
 backward run libpwgb kernels.  Data gradients reuse the forward kernels (dgrad of a stride-1 conv =
-conv with the transposed, tap-flipped weight -> tcgen05 path; dgrad of a strided conv = poly-phase
+conv with the transposed, tap-flipped weight -> tensor-core path; dgrad of a strided conv = poly-phase
 conv-transpose); weight gradients use pwgb_conv1d_wgrad.  Weight / spectral-norm
 re-parametrisation stays in PyTorch on the (tiny) weight tensors, so its backward is PyTorch's."""
 import ctypes as C
@@ -153,7 +153,7 @@ class ConvTranspose1dFn(torch.autograd.Function):
             gw = ops.conv1d_wgrad(gy, x, (cin, cout, K), stride=stride, padding=padding, g_slope=pre_slope)
         gx = None
         if ctx.needs_input_grad[0]:
-            gx = ops.conv1d(gy, w.detach(), None, stride=stride, padding=padding)  # (cin, cout, K) read as a conv weight; strided -> space-to-depth + tcgen05
+            gx = ops.conv1d(gy, w.detach(), None, stride=stride, padding=padding)  # (cin, cout, K) read as a conv weight; strided -> space-to-depth + tensor cores
             if gx.shape[-1] != x.shape[-1]:
                 raise PwgbError("conv_transpose dgrad: length mismatch")
             if pre_slope != 1.0:

@@ -2,7 +2,7 @@
 //   * wgrad of the generic fused Conv1d (any stride / dilation / groups / period view),
 //     deterministic two-stage split reduction;
 //   * data gradients reuse the FORWARD kernels (a stride-1 dgrad is a conv with the transposed,
-//     tap-flipped weight -> tcgen05 path; a strided dgrad is the poly-phase conv-transpose), so only
+//     tap-flipped weight -> tensor-core path; a strided dgrad is the poly-phase conv-transpose), so only
 //     the elementwise chain-rule pieces live here: activation masks, bias sums, loss / pooling grads.
 #include <cooperative_groups.h>
 
@@ -556,7 +556,7 @@ __global__ void __launch_bounds__(256) upsample_fir_backward_f_tap_kernel(int ro
 
 static int grid_for(long long n) {
   long long b = (n + 255) / 256;
-  return (int)(b > 148 * 16 ? 148 * 16 : (b < 1 ? 1 : b));
+  return (int)(b > 132 * 16 ? 132 * 16 : (b < 1 ? 1 : b));
 }
 
 }  // namespace pwgb

@@ -1,7 +1,7 @@
 // Generic fused 1-D convolution, fp32 FFMA path (any channel count / stride / dilation /
 // groups / period).  This is the exact-arithmetic path: narrow layers (Cin or Cout < 16,
 // grouped and strided discriminator convs) always use it, and it is the in-library
-// cross-check for the tcgen05 path (conv1d_tc.cu) that takes the wide stride-1 layers.
+// cross-check for the tensor-core path (conv1d_tc.cu) that takes the wide stride-1 layers.
 //
 // Tiling: one CTA = CO_T output channels x TT output positions of one batch item.
 // 8 warps = WARPS_CO (channel sub-tiles of RCO channels) x WARPS_T (time sub-tiles of

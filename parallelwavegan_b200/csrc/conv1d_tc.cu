@@ -1,34 +1,35 @@
-// Stride-1 Conv1d on the 5th-gen tensor cores (tcgen05 + TMEM), fp32-accurate via a bf16x3
-// operand split:  x = xh + xl, w = wh + wl (bf16 each),  x*w ~= xh*wh + xl*wh + xh*wl  with
-// fp32 accumulation in TMEM (dropped term xl*wl ~ 2^-16 relative).  One pass of plain
-// TF32/BF16 does not meet the 1e-3 parity bar end to end (SURVEY.md 7 "hard parts").
+// Stride-1 Conv1d on the Hopper tensor cores (wgmma, fp32 accumulators in registers), fp32-accurate via a bf16x3
+// operand split:  x = xh + xl, w = wh + wl (bf16 each),  x*w ~= xh*wh + xl*wh + xh*wl  with fp32 accumulation
+// (dropped term xl*wl ~ 2^-16 relative).  One pass of plain TF32/BF16 does not meet the 1e-3 parity bar end to end
+// (SURVEY.md 7 "hard parts").
 //
 // Formulation (im2col is never materialised): TIME is the MMA M dimension.
 //   D[t, co] += sum_{ci in 16-chunk} A_k[t, ci] * B_k[co, ci]      for every tap k
 //   A_k = rows (t0 + t + k*dilation - pad) of the staged activation tile  -> a *row offset*
-//         into ONE shared-memory tile, expressed through the UMMA descriptor start address;
+//         into ONE shared-memory tile, expressed through the wgmma descriptor start address;
 //   B_k = W[:, :, k] pre-packed (hi/lo bf16) in global memory in the exact smem image.
 // Both operands are K-major, no-swizzle ("interleaved") core-matrix layouts:
 //   [ci/8][row][8 ci] bf16  -> 16 B per (row, 8 channels); 8-row core matrices are contiguous
 //   (SBO = 128 B) so any row offset is a legal 16 B-aligned descriptor start, and the K-adjacent
 //   core matrix sits LBO = rows*16 B away.
-// Warp roles (640 threads, one persistent CTA per SM; every role loops over the same tile sequence and
+// Warp roles (576 threads, one persistent CTA per SM; every role loops over the same tile sequence and
 // talks through mbarriers only):
 //   warps 0-7   A producers: convert landed raw fp32 stages (pre-activation, padding mask, bf16 hi/lo split)
 //               into the K-major operand image, 16 B st.shared.
-//   warps 8-15  epilogue: tcgen05.ld -> bias / act / residual / scale / accumulate -> coalesced stores.
+//   warps 8-15  consumers, two warpgroups: warpgroup g issues the wgmma of its 64 (MT = 2: 128) rows of the tile into
+//               registers (<= 128 columns: 64 fp32 per thread), then runs bias / act / residual / scale / accumulate
+//               and stores.
 //   warp 16     B producer: cp.async.bulk (TMA, 1-D) of one packed weight stage per (chunk, tap).
-//   warps 17-18 MMA issuers (one per 128-row m-tile; elected lane issues tcgen05.mma, tcgen05.commit frees stages).
-//   warp 19     raw activation loader: cp.async.bulk row copies into the raw fp32 ring.
+//   warp 17     raw activation loader: cp.async.bulk row copies into the raw fp32 ring.
 #include "tc_common.cuh"
 
 namespace pwgb {
 
 constexpr int NPROD = 256;  // producer threads (warps 0-7); 4 warps measured slower (conversion-bound)
-constexpr int NEPI = 256;   // epilogue threads (warps 8-15)
-// warp roles after the producers / epilogue: weight TMA, MMA issuer(s), activation TMA
-constexpr int W_EPI0 = NPROD / 32, W_TMA = (NPROD + NEPI) / 32, W_MMA = W_TMA + 1, W_LDA = W_TMA + 3;  // W_MMA + 1: second MMA issuer
-constexpr int TC_THREADS = NPROD + NEPI + 128;
+constexpr int NCONS = 256;  // consumer threads (warps 8-15: two warpgroups)
+// warp roles after the producers / consumers: weight TMA, activation TMA
+constexpr int W_CONS0 = NPROD / 32, W_TMA = (NPROD + NCONS) / 32, W_LDA = W_TMA + 1;
+constexpr int TC_THREADS = NPROD + NCONS + 64;
 constexpr int NS_MAX = 4;  // raw activation stages
 
 struct TcK {
@@ -39,18 +40,14 @@ struct TcK {
   float out_scale;
   int accumulate;
   int shuffle, shuffle_pad, shuffle_tout;
-  int MT, R, nchunks, tiles_per_seq, nb, na, nacc, total_tiles;
+  int MT, R, nchunks, tiles_per_seq, nb, na, total_tiles;
   int ns;                // raw fp32 staging buffers for the activation chunks (0 = direct register path)
   int R4, raw_bytes;     // raw stage: KC rows of R4 floats (R4 = R + alignment slack, multiple of 4)
   int tma_act;           // 1: raw stages are filled by cp.async.bulk row copies (warp W_LDA), 0: by cp.async (producers)
-  int nmma;              // MMA issuer warps: 2 = one per 128-row m-tile (MT == 2)
-  int shuffle_vec;       // pixel-shuffle epilogue may use 16-byte stores
   int nco;               // column chunks of Cout channels sharing this launch (conv-transpose: cout * stride > 256; wide / grouped convs)
   int cpg;               // column chunks per group (grouped convs: chunk cc reads the input channels of group cc / cpg)
   long long xgs;         // input offset between groups (elements): cin_per_group * T_in, 0 for dense convs
   long long xbs, ybs, rbs;
-  unsigned idesc;
-  int tmem_cols;
   int a_bytes, b_bytes;  // per buffer / per stage
   int win_mode;          // 1: one TT-row window per tap (halo too large for a contiguous tile)
   int nchunks2, C2;      // auxiliary 1x1 source (WaveNet conditioning): extra K=1 chunks
@@ -58,7 +55,7 @@ struct TcK {
   int wavenet;           // epilogue: cols < split -> y2 += v ; cols >= split -> y = (v + res) * scale
   int split;
   int co_off;            // first output channel of this launch (N-chunked callers)
-  int variant;           // debug: bit0 swaps LBO/SBO (bring-up aid, see pwgb_debug_set)
+  int variant;           // debug (pwgb_debug_set(1, v)): bit 1 stages activations with cp.async instead of TMA
 };
 
 // ------------------------------------------------------------------ weight packing
@@ -105,61 +102,48 @@ void tc_pack_rows(const float* w, void* packed, int cin_real, int cin_pad, int r
   tc_pack_weight_kernel<<<blocks, 128, 0, st>>>(w, (uint4*)packed, cin_real, cin_pad, rows, K, co_begin, cout_total, 0);
 }
 
-// Generic epilogue for W (16 or 32) accumulator columns of one row: every independent global load
-// (residual, and the accumulate read-modify-write) is issued before the TMEM load is waited for, so
-// W (2W) requests per thread are in flight.
-template <int W>
-__device__ __forceinline__ void epi_generic(const TcK& p, unsigned taddr, const float* __restrict__ bias_s, int col,
-                                            const float* rq, float* yq, long long st, bool tv) {
-  unsigned r[W];
-  {
-    unsigned (&r0)[16] = *reinterpret_cast<unsigned (*)[16]>(&r[0]);
-    tc_ld16(taddr, r0);
-    if (W == 32) {
-      unsigned (&r1)[16] = *reinterpret_cast<unsigned (*)[16]>(&r[W == 32 ? 16 : 0]);
-      tc_ld16(taddr + 16, r1);
-    }
-  }
-  float rv[W];
-  if (rq && tv) {
-    const float* q = rq;
-#pragma unroll
-    for (int j = 0; j < W; ++j, q += st) rv[j] = __ldg(q);
+// Epilogue of one accumulator element (row t, column col of the launch's column chunk starting at co_base).
+__device__ __forceinline__ void epi_store(const TcK& p, float a, int b, int t, int col, int co_base, const float* __restrict__ bias,
+                                          const float* bias_s, const float* __restrict__ res, float* __restrict__ y,
+                                          float* __restrict__ y2) {
+  const long long st = p.T_out;
+  if (p.shuffle > 1) {
+    const int co = co_base + col, cof = co / p.shuffle;
+    float v = a + (bias ? __ldg(bias + cof) : 0.f);
+    if (p.post_act == PWGB_ACT_TANH)
+      v = tanhf(v);
+    else if (p.post_act == PWGB_ACT_LRELU)
+      v = lrelu(v, p.post_slope);
+    const int of = t * p.shuffle + (co - cof * p.shuffle) - p.shuffle_pad;
+    if (of >= 0 && of < p.shuffle_tout) y[(long long)b * p.ybs + (long long)cof * p.shuffle_tout + of] = v * p.out_scale;
+  } else if (p.wavenet) {
+    // WaveNet split epilogue (residual_block.py:131-138): columns [0, split) are the skip 1x1
+    // (accumulated into y2), columns [split, Cout) the residual 1x1: y = (v + x) * sqrt(0.5)
+    const bool is_skip = col < p.split;
+    const int ch = is_skip ? col : col - p.split, nch = is_skip ? p.split : p.Cout - p.split;
+    const long long off = ((long long)b * nch + ch) * st + t;
+    const float v = a + bias_s[col];
+    if (is_skip)
+      y2[off] = v + y2[off];
+    else
+      y[off] = (v + __ldg(res + off)) * p.out_scale;
   } else {
-#pragma unroll
-    for (int j = 0; j < W; ++j) rv[j] = 0.f;
-  }
-  tc_wait_ld();
-  if (!tv) return;
-  float* q = yq;
-  if (p.accumulate) {
-    float yv[W];
-    const float* q2 = yq;
-#pragma unroll
-    for (int j = 0; j < W; ++j, q2 += st) yv[j] = *q2;
-#pragma unroll
-    for (int j = 0; j < W; ++j, q += st) {
-      float v = __uint_as_float(r[j]) + bias_s[col + j];
-      if (p.post_act != PWGB_ACT_NONE) v = p.post_act == PWGB_ACT_TANH ? tanhf(v) : lrelu(v, p.post_slope);
-      *q = (v + rv[j]) * p.out_scale + yv[j];
-    }
-  } else if (p.post_act == PWGB_ACT_NONE) {
-#pragma unroll
-    for (int j = 0; j < W; ++j, q += st) *q = (__uint_as_float(r[j]) + bias_s[col + j] + rv[j]) * p.out_scale;
-  } else {
-#pragma unroll
-    for (int j = 0; j < W; ++j, q += st) {
-      float v = __uint_as_float(r[j]) + bias_s[col + j];
-      v = p.post_act == PWGB_ACT_TANH ? tanhf(v) : lrelu(v, p.post_slope);
-      *q = (v + rv[j]) * p.out_scale;
-    }
+    // several column chunks per launch: bias_s holds the bias of every chunk
+    const long long off = (long long)(co_base + col) * st + t;
+    float v = a + bias_s[co_base - p.co_off + col];
+    if (p.post_act != PWGB_ACT_NONE) v = p.post_act == PWGB_ACT_TANH ? tanhf(v) : lrelu(v, p.post_slope);
+    if (res) v += __ldg(res + (long long)b * p.rbs + off);
+    v *= p.out_scale;
+    float* q = y + (long long)b * p.ybs + off;
+    if (p.accumulate) v += *q;
+    *q = v;
   }
 }
 
 // ------------------------------------------------------------------ main kernel
 // Persistent: one CTA per SM loops over (batch, time-tile) work items; every role runs the same
-// tile sequence and talks through mbarriers only, so the load of tile i+1, the MMAs of tile i and
-// the epilogue of tile i-1 overlap (TMEM holds two accumulator sets when they fit 512 columns).
+// tile sequence and talks through mbarriers only, so the loads of tile i+1 overlap the MMAs and the
+// epilogue of tile i.
 
 // stage one activation chunk (KC channels x R rows) into the operand layout
 __device__ __forceinline__ void fill_main_chunk(const TcK& p, const float* __restrict__ xc, int t0, int TT,
@@ -226,29 +210,26 @@ __device__ __forceinline__ void fill_main_chunk(const TcK& p, const float* __res
   }
 }
 
-// MC = 1: several column chunks / groups of a plain (non pixel-shuffle) conv share the launch -- the extra index
-// arithmetic (group input offset, per-chunk bias and output channel base) is compiled only into that instantiation
-template <int MC>
 __global__ void __launch_bounds__(TC_THREADS, 1)
     conv1d_tc_kernel(const TcK p, const float* __restrict__ x, const float* __restrict__ x2,
                      const uint4* __restrict__ wpk, const float* __restrict__ bias, const float* __restrict__ res,
                      float* __restrict__ y, float* __restrict__ y2) {
   extern __shared__ __align__(128) unsigned char smem[];
-  // layout: A[na] | B[nb] | raw staging[ns] | barriers | tmem ptr | bias
+  // layout: A[na] | B[nb] | raw staging[ns] | barriers | bias
   unsigned char* a_buf = smem;
   unsigned char* b_buf = smem + (size_t)p.na * p.a_bytes;
   unsigned char* raw_buf = b_buf + (size_t)p.nb * p.b_bytes;
   unsigned long long* bars = reinterpret_cast<unsigned long long*>(raw_buf + (size_t)p.ns * p.raw_bytes);
   const int nbar = 2 * p.na + 2 * p.nb + 4 + 2 * NS_MAX;
-  unsigned* tmem_slot = reinterpret_cast<unsigned*>(bars + nbar);
-  float* bias_s = reinterpret_cast<float*>(tmem_slot + 4);  // Cout floats (0 when bias == nullptr)
+  float* bias_s = reinterpret_cast<float*>(bars + nbar + 2);  // Cout floats (0 when bias == nullptr)
+  // several column chunks / groups of a plain (non pixel-shuffle) conv share the launch
+  const bool MC = p.nco > 1 && p.shuffle <= 1;
 
   const int tid = threadIdx.x;
   const int warp = tid >> 5;
   const int lane = tid & 31;
   const int TT = p.MT * 128;
   const int nc_total = p.nchunks + p.nchunks2;
-  const int acc_cols = p.MT * p.Cout;
   const int pct = p.B * p.tiles_per_seq;  // work items per column chunk (nco chunks share one launch)
 
   const unsigned bar0 = smem_u32(bars);
@@ -256,23 +237,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   auto A_EMPTY = [&](int i) { return bar0 + 8u * (p.na + i); };
   auto B_FULL = [&](int i) { return bar0 + 8u * (2 * p.na + i); };
   auto B_EMPTY = [&](int i) { return bar0 + 8u * (2 * p.na + p.nb + i); };
-  auto ACC_FULL = [&](int i) { return bar0 + 8u * (2 * p.na + 2 * p.nb + i); };
-  auto ACC_EMPTY = [&](int i) { return bar0 + 8u * (2 * p.na + 2 * p.nb + 2 + i); };
   auto RAW_FULL = [&](int i) { return bar0 + 8u * (2 * p.na + 2 * p.nb + 4 + i); };
   auto RAW_EMPTY = [&](int i) { return bar0 + 8u * (2 * p.na + 2 * p.nb + 4 + NS_MAX + i); };
 
   if (tid == 0) {
     for (int i = 0; i < p.na; ++i) {
       mbar_init(A_FULL(i), NPROD);
-      mbar_init(A_EMPTY(i), p.nmma);
+      mbar_init(A_EMPTY(i), NCONS / 32);
     }
     for (int i = 0; i < p.nb; ++i) {
       mbar_init(B_FULL(i), 1);
-      mbar_init(B_EMPTY(i), p.nmma);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(ACC_FULL(i), p.nmma);
-      mbar_init(ACC_EMPTY(i), NEPI);
+      mbar_init(B_EMPTY(i), NCONS / 32);
     }
     for (int i = 0; i < NS_MAX; ++i) {
       mbar_init(RAW_FULL(i), 1);
@@ -280,20 +255,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == W_MMA) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"((unsigned)p.tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   for (int i = tid; i < p.Cout * (MC ? p.nco : 1); i += TC_THREADS)
     bias_s[i] = bias ? __ldg(bias + (p.shuffle > 1 ? (p.co_off + i) / p.shuffle : p.co_off + i)) : 0.f;
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const unsigned tmem_base = *tmem_slot;
 
-  if (warp < W_EPI0 && p.tma_act) {
+  if (warp < W_CONS0 && p.tma_act) {
     // ===================== A producers, TMA-staged =====================
     // Warp W_LDA streams the raw fp32 rows of chunk q + ns - 1 into shared memory with bulk copies
     // (no LSU instructions, no registers); these 8 warps only convert landed stages to the bf16 hi/lo
@@ -338,7 +304,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         if (++buf == p.na) { buf = 0; aph ^= 1; }
       }
     }
-  } else if (warp < W_EPI0 && p.ns > 0) {
+  } else if (warp < W_CONS0 && p.ns > 0) {
     // ===================== A producers, cp.async-staged =====================
     // The raw fp32 chunk q+1 streams into shared memory (no registers held, any padding policy by
     // per-element addressing, zero-fill through src-size 0) while chunk q is converted to the bf16
@@ -427,7 +393,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       mbar_arrive(A_FULL(buf));
       producer_barrier();  // raw[q % ns] may be overwritten by issue(q + 2)
     }
-  } else if (warp < W_EPI0) {
+  } else if (warp < W_CONS0) {
     // ===================== A producers, direct register path =====================
     unsigned ca = 0;
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
@@ -464,141 +430,68 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       }
     }
   } else if (warp < W_TMA) {
-    // ===================== epilogue =====================
-    // 8 warps: lane quarter = warp % 4 (hardware TMEM access rule), column half = (warp - W_EPI0) / 4
-    const int ew = warp & 3;
-    const int ngroups = p.Cout / 16;
-    const int col_begin = ((warp - W_EPI0) >> 2) ? (ngroups / 2) * 16 : 0;
-    const int col_end = ((warp - W_EPI0) >> 2) ? p.Cout : (ngroups / 2) * 16;
-    const int m = ew * 32 + lane;
-    const bool generic = !(p.shuffle > 1) && !p.wavenet;
-    const long long st = p.T_out;
-    int as = 0, accph = 0;
+    // ===================== consumers: wgmma into registers, then the epilogue =====================
+    // warpgroup wg owns the 64-row blocks wg * MT + mb of the tile; per (chunk, tap) and 16-channel K-step the three
+    // bf16x3 products of every block, one wait per weight stage before the stage is handed back
+    const int wg = (warp - W_CONS0) >> 2, wq = warp & 3;
+    const int nb16 = p.Cout / 16;
+    const unsigned lbo_a = (unsigned)p.R * 16u, lbo_b = (unsigned)p.Cout * 16u;
+    const unsigned a_sub = (unsigned)(KC / 8) * p.R, b_sub = (unsigned)(KC / 8) * p.Cout;  // hi -> lo image (16-byte units)
+    int buf = 0, aph = 0, s = 0, bph = 0;
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      float acc[64];
+#pragma unroll
+      for (int e = 0; e < 64; ++e) acc[e] = 0.f;
+      for (int c = 0; c < nc_total; ++c) {
+        mbar_wait_spin(A_FULL(buf), aph);
+        const unsigned a_addr = smem_u32(a_buf + (size_t)buf * p.a_bytes);
+        const int ntaps = c < p.nchunks ? p.K : 1;
+        for (int k = 0; k < ntaps; ++k) {
+          mbar_wait_spin(B_FULL(s), bph);
+          __syncwarp();
+          const unsigned b_addr = smem_u32(b_buf + (size_t)s * p.b_bytes);
+          const int tap_row = c < p.nchunks ? (p.win_mode ? k * TT : k * p.D) : 0;
+          wg_fence();
+#pragma unroll
+          for (int ks = 0; ks < KC / 16; ++ks) {
+            const unsigned long long bh = gmma_desc(b_addr + (unsigned)(2 * ks) * lbo_b, lbo_b, 128);
+            const unsigned long long ah0 =
+                gmma_desc(a_addr + ((unsigned)(2 * ks) * p.R + (unsigned)(tap_row + wg * p.MT * 64)) * 16u, lbo_a, 128);
+            if (p.MT == 1) {
+              wgmma_cols<0, 0, 8>(acc, ah0, bh, nb16, 16);
+              wgmma_cols<0, 0, 8>(acc, ah0 + a_sub, bh, nb16, 16);
+              wgmma_cols<0, 0, 8>(acc, ah0, bh + b_sub, nb16, 16);
+            } else {
+              const unsigned long long ah1 = ah0 + 64;  // next 64 rows: 64 x 16 B
+              wgmma_cols<0, 0, 4>(acc, ah0, bh, nb16, 16);
+              wgmma_cols<0, 0, 4>(acc, ah0 + a_sub, bh, nb16, 16);
+              wgmma_cols<0, 0, 4>(acc, ah0, bh + b_sub, nb16, 16);
+              wgmma_cols<0, 0, 4>(acc + 32, ah1, bh, nb16, 16);
+              wgmma_cols<0, 0, 4>(acc + 32, ah1 + a_sub, bh, nb16, 16);
+              wgmma_cols<0, 0, 4>(acc + 32, ah1, bh + b_sub, nb16, 16);
+            }
+          }
+          wg_commit();
+          wg_wait<0>();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(B_EMPTY(s));  // weight stage reusable
+          if (++s == p.nb) { s = 0; bph ^= 1; }
+        }
+        if (lane == 0) mbar_arrive(A_EMPTY(buf));
+        if (++buf == p.na) { buf = 0; aph ^= 1; }
+      }
       const int tr = p.nco > 1 ? tile % pct : tile;  // tile within its column chunk
       const int b = tr / p.tiles_per_seq;
       const int t0 = (tr - b * p.tiles_per_seq) * TT;
-      // L2 prefetch of the NEXT tile's residual (and read-modify-write) lines: one 128-byte line per
-      // (m-tile, column) and warp, no registers held; the epilogue's loads then hit L2 instead of HBM
-      if (generic && (res || p.accumulate) && !(p.variant & 8)) {
-        const int ncol = col_end - col_begin;
-        for (int pass = (tile == (int)blockIdx.x ? 0 : 1); pass < 2; ++pass) {
-          const int tl = pass ? tile + (int)gridDim.x : tile;
-          if (tl >= p.total_tiles) break;
-          const int tlr = p.nco > 1 ? tl % pct : tl;
-          const int bb = tlr / p.tiles_per_seq;
-          const int tt0 = (tlr - bb * p.tiles_per_seq) * TT;
-          for (int i = lane; i < p.MT * ncol; i += 32) {
-            const int mt = i / ncol;
-            const int col = col_begin + (i - mt * ncol);
-            const int tp = tt0 + mt * 128 + ew * 32;
-            if (tp < p.T_out) {
-              const long long off = (long long)(p.co_off + (MC ? (tl / pct) * p.Cout : 0) + col) * st + tp;
-              if (res) prefetch_l2(res + (long long)bb * p.rbs + off);
-              if (p.accumulate) prefetch_l2(y + (long long)bb * p.ybs + off);
-            }
-          }
-        }
-      }
       const int co_base = p.co_off + (p.nco > 1 ? (tile / pct) * p.Cout : 0);
-      mbar_wait(ACC_FULL(as), accph);
-      tc_fence_after();
-      const unsigned tacc = tmem_base + ((unsigned)(ew * 32) << 16) + (unsigned)(as * acc_cols);
-      for (int mt = 0; mt < p.MT; ++mt) {
-        const int t = t0 + mt * 128 + m;
-        const bool tv = t < p.T_out;
-        if (p.shuffle > 1 && p.shuffle_vec) {
-          // pixel-shuffle epilogue, vector form: the `shuffle` phases of one output channel are adjacent
-          // columns AND adjacent output samples, so a thread stores 16-byte pieces (a warp: contiguous KBs)
-          for (int col = col_begin; col < col_end; col += 16) {
-            unsigned r[16];
-            tc_ld16(tacc + (unsigned)(mt * p.Cout + col), r);
-            tc_wait_ld();
-            if (tv) {
 #pragma unroll
-              for (int j0 = 0; j0 < 16; j0 += 4) {
-                const int co = co_base + col + j0;
-                const int cof = co / p.shuffle;
-                const int of = t * p.shuffle + (co - cof * p.shuffle) - p.shuffle_pad;
-                float v[4];
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  v[j] = __uint_as_float(r[j0 + j]) + (p.nco > 1 ? (bias ? __ldg(bias + cof) : 0.f) : bias_s[col + j0 + j]);
-                  if (p.post_act == PWGB_ACT_TANH)
-                    v[j] = tanhf(v[j]);
-                  else if (p.post_act == PWGB_ACT_LRELU)
-                    v[j] = lrelu(v[j], p.post_slope);
-                  v[j] *= p.out_scale;
-                }
-                if (of >= 0 && of < p.shuffle_tout)
-                  *reinterpret_cast<float4*>(y + (long long)b * p.ybs + (long long)cof * p.shuffle_tout + of) =
-                      make_float4(v[0], v[1], v[2], v[3]);
-              }
-            }
-          }
-        } else if (p.shuffle > 1) {
-          for (int col = col_begin; col < col_end; col += 16) {
-            unsigned r[16];
-            tc_ld16(tacc + (unsigned)(mt * p.Cout + col), r);
-            tc_wait_ld();
-            if (tv) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) {
-                const int co = co_base + col + j;
-                const int cof = co / p.shuffle;
-                float v = __uint_as_float(r[j]) + (p.nco > 1 ? (bias ? __ldg(bias + cof) : 0.f) : bias_s[col + j]);
-                if (p.post_act == PWGB_ACT_TANH)
-                  v = tanhf(v);
-                else if (p.post_act == PWGB_ACT_LRELU)
-                  v = lrelu(v, p.post_slope);
-                const int of = t * p.shuffle + (co - cof * p.shuffle) - p.shuffle_pad;
-                if (of >= 0 && of < p.shuffle_tout)
-                  y[(long long)b * p.ybs + (long long)cof * p.shuffle_tout + of] = v * p.out_scale;
-              }
-            }
-          }
-        } else if (p.wavenet) {
-          // WaveNet split epilogue (residual_block.py:131-138): columns [0, split) are the skip 1x1
-          // (accumulated into y2), columns [split, Cout) the residual 1x1: y = (v + x) * sqrt(0.5)
-          for (int col = col_begin; col < col_end; col += 16) {
-            unsigned r[16];
-            tc_ld16(tacc + (unsigned)(mt * p.Cout + col), r);
-            const bool is_skip = col < p.split;
-            const int ch = is_skip ? col : col - p.split;
-            const int nch = is_skip ? p.split : p.Cout - p.split;
-            const long long off = ((long long)b * nch + ch) * st + t;
-            float rv[16];
-            if (tv) {
-              const float* rq = is_skip ? y2 + off : res + off;
-#pragma unroll
-              for (int j = 0; j < 16; ++j, rq += st) rv[j] = is_skip ? *rq : __ldg(rq);
-            }
-            tc_wait_ld();
-            if (tv) {
-              float* wq = is_skip ? y2 + off : y + off;
-              const float sc = is_skip ? 1.f : p.out_scale;
-#pragma unroll
-              for (int j = 0; j < 16; ++j, wq += st) *wq = (__uint_as_float(r[j]) + bias_s[col + j] + rv[j]) * sc;
-            }
-          }
-        } else {
-          // generic: running 64-bit pointers (2 integer instructions per element instead of a full
-          // address recomputation), every independent load of a 16-column group issued before use
-          const int cb = MC ? co_base : p.co_off;
-          float* yq = y + (long long)b * p.ybs + (long long)(cb + col_begin) * st + t;
-          const float* rq = res ? res + (long long)b * p.rbs + (long long)(cb + col_begin) * st + t : nullptr;
-          // several column chunks per launch: bias_s holds the bias of every chunk
-          const float* bptr = MC ? bias_s + (co_base - p.co_off) : bias_s;
-          // (32-column groups were tried: they spill at the register budget of this block size)
-          for (int col = col_begin; col < col_end; col += 16, yq += 16 * st) {
-            epi_generic<16>(p, tacc + (unsigned)(mt * p.Cout + col), bptr, col, rq, yq, st, tv);
-            if (rq) rq += 16 * st;
-          }
-        }
+      for (int e = 0; e < 64; ++e) {
+        const int mb = p.MT == 2 ? (e >> 5) : 0;
+        const int i = p.MT == 2 ? (e & 31) : e;
+        const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+        const int t = t0 + (wg * p.MT + mb) * 64 + wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+        if (col < p.Cout && t < p.T_out) epi_store(p, acc[e], b, t, col, co_base, bias, bias_s, res, y, y2);
       }
-      tc_fence_before();
-      mbar_arrive(ACC_EMPTY(as));  // accumulator set drained: the MMA warp may overwrite it
-      if (++as == p.nacc) { as = 0; accph ^= 1; }
     }
   } else if (warp == W_TMA) {
     // ===================== B producer (TMA bulk copies of packed weight stages) =====================
@@ -657,62 +550,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         }
       }
     }
-  } else if (warp - W_MMA < p.nmma) {
-    // ===================== MMA issuer(s) (whole warp converged; one elected lane issues) =====================
-    // nmma == 2: warp W_MMA + i owns m-tile i (its own accumulator columns); both commit to the same
-    // stage barriers, whose arrival counts are nmma.
-    const int mw = warp - W_MMA;
-    const bool split2 = p.nmma == 2;
-    // descriptor = hi_const : (lo_const + (addr >> 4));  LBO/SBO/version never change in a launch
-    const unsigned long long hi_const = ((unsigned long long)((128u >> 4) | (1u << 14))) << 32;
-    const unsigned a_lo = ((((unsigned)p.R) & 0x3FFFu) << 16) + (split2 ? (unsigned)mw * 128u : 0u);  // LBO = R*16 B
-    const unsigned b_lo = (((unsigned)p.Cout) & 0x3FFFu) << 16;                                      // LBO = Cout*16 B
-    const unsigned a_sub = (unsigned)(KC / 8) * p.R;  // hi -> lo image distance (16 B units)
-    const unsigned b_sub = (unsigned)(KC / 8) * p.Cout;
-    int buf = 0, aph = 0, s = 0, bph = 0, as = 0, accph = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      mbar_wait_spin(ACC_EMPTY(as), accph ^ 1);
-      tc_fence_after();
-      const unsigned d_base = tmem_base + (unsigned)(as * acc_cols) + (split2 ? (unsigned)(mw * p.Cout) : 0u);
-      for (int c = 0; c < nc_total; ++c) {
-        mbar_wait_spin(A_FULL(buf), aph);
-        const unsigned a16 = smem_u32(a_buf + (size_t)buf * p.a_bytes) >> 4;
-        const int ntaps = c < p.nchunks ? p.K : 1;
-        for (int k = 0; k < ntaps; ++k) {
-          mbar_wait_spin(B_FULL(s), bph);
-          tc_fence_after();
-          const unsigned b16 = smem_u32(b_buf + (size_t)s * p.b_bytes) >> 4;
-          const unsigned tap_row = c < p.nchunks ? (unsigned)(p.win_mode ? k * TT : k * p.D) : 0u;
-          if (p.MT == 1 || split2) {
-            const unsigned long long b_hi = hi_const | (unsigned long long)(b_lo + b16);
-            const unsigned long long a_hi = hi_const | (unsigned long long)(a_lo + a16 + tap_row);
-            tc_mma_tap6(d_base, a_hi, b_hi, a_sub, b_sub, 2u * (unsigned)p.R, 2u * (unsigned)p.Cout, p.idesc,
-                        (c | k) != 0 ? 1u : 0u);
-          } else {
-#pragma unroll
-            for (int ks = 0; ks < KC / 16; ++ks) {
-              const unsigned bk = b16 + (unsigned)(2 * ks) * p.Cout;
-              const unsigned ak = a16 + (unsigned)(2 * ks) * p.R + tap_row;
-              const unsigned long long b_hi = hi_const | (unsigned long long)(b_lo + bk);
-              const unsigned long long a_hi = hi_const | (unsigned long long)(a_lo + ak);
-              tc_mma_x3(d_base, a_hi, b_hi, a_sub, b_sub, p.idesc, (c | k | ks) != 0 ? 1u : 0u, 1u, (unsigned)p.Cout);
-            }
-          }
-          tc_commit(B_EMPTY(s));  // weight stage reusable once these MMAs retire
-          if (++s == p.nb) { s = 0; bph ^= 1; }
-        }
-        tc_commit(A_EMPTY(buf));
-        if (++buf == p.na) { buf = 0; aph ^= 1; }
-      }
-      tc_commit(ACC_FULL(as));
-      if (++as == p.nacc) { as = 0; accph ^= 1; }
-    }
-  }
-  __syncthreads();
-  if (warp == W_MMA) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((unsigned)p.tmem_cols)
-                 : "memory");
   }
 }
 
@@ -728,7 +565,7 @@ static int tc_plan(const pwgb_conv1d_desc* d, TcK& p, size_t& smem_bytes, int au
   p.xgs = 0;
   const int P = d->period < 1 ? 1 : d->period;
   if (d->stride != 1 || d->groups != 1 || P != 1) return 0;
-  if (d->cin % KC != 0 || d->cout % 16 != 0 || d->cout < 16 || d->cout > 256) return 0;
+  if (d->cin % KC != 0 || d->cout % 16 != 0 || d->cout < 16 || d->cout > TC_NMAX) return 0;
   if (aux_c2 % KC != 0 || split % 16 != 0 || split > d->cout) return 0;
   if (d->t_valid > 0 && d->t_valid != d->t_in) return 0;
   if (d->x_batch_stride || d->y_batch_stride || d->r_batch_stride) return 0;
@@ -760,15 +597,14 @@ static int tc_plan(const pwgb_conv1d_desc* d, TcK& p, size_t& smem_bytes, int au
   p.xbs = (long long)d->cin * (d->pre_gate ? 2 : 1) * d->t_in;
   p.ybs = d->shuffle > 1 ? (long long)(d->cout / d->shuffle) * d->shuffle_tout : (long long)d->cout * d->t_out;
   p.rbs = (long long)d->cout * d->t_out;
-  // instruction descriptor: D=f32 (1<<4), A=B=bf16 (1<<7, 1<<10), K-major both, N>>3 @17, M>>4 @24
-  p.idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((unsigned)(d->cout >> 3) << 17) | ((128u >> 4) << 24);
   p.b_bytes = 2 * (KC / 8) * d->cout * 16;
   // tile shape (1 persistent CTA / SM, ~216 KB of shared memory): prefer a contiguous halo tile of
-  // 2 x 128 rows; fall back to 128 rows, then to one window per tap (very large dilation)
+  // 2 x 128 rows (Cout <= 64: the 64 accumulator registers hold both); fall back to 128 rows, then to
+  // one window per tap (very large dilation)
   const size_t budget = 216 * 1024;
   for (int attempt = 0; attempt < 4; ++attempt) {
     if (attempt == 0) {
-      p.MT = (2 * d->cout <= 256 && d->t_out > 128) ? 2 : 1;
+      p.MT = (d->cout <= TC_NMAX / 2 && d->t_out > 128) ? 2 : 1;
       p.win_mode = 0;
       p.R = p.MT * 128 + (int)halo;
     } else if (attempt == 1) {
@@ -776,7 +612,7 @@ static int tc_plan(const pwgb_conv1d_desc* d, TcK& p, size_t& smem_bytes, int au
       p.win_mode = 0;
       p.R = 128 + (int)halo;
     } else if (attempt == 2) {
-      p.MT = (2 * d->cout <= 256 && d->t_out > 128) ? 2 : 1;
+      p.MT = (d->cout <= TC_NMAX / 2 && d->t_out > 128) ? 2 : 1;
       p.win_mode = 1;
       p.R = d->kernel * p.MT * 128;
     } else {
@@ -793,12 +629,9 @@ static int tc_plan(const pwgb_conv1d_desc* d, TcK& p, size_t& smem_bytes, int au
     // 16-byte aligned rows; anything else is staged with 4-byte cp.async by the producers
     p.tma_act = !(p.variant & 2) && !d->pre_gate && !p.win_mode && d->pad_mode == PWGB_PAD_ZERO && d->t_in % 4 == 0 &&
                 (aux_c2 == 0 || d->t_out % 4 == 0);
-    p.nmma = (p.MT == 2 && !(p.variant & 4)) ? 2 : 1;
-    p.shuffle_vec = d->shuffle > 1 && d->shuffle % 4 == 0 && 16 % d->shuffle == 0 && d->shuffle_pad % 4 == 0 &&
-                    d->shuffle_tout % 4 == 0 && !(p.variant & 16);
     // shared-memory split: [na operand buffers][nb weight stages][ns raw staging buffers]
     int na = 0, nb = 0, ns = 0;
-    const size_t bias_bytes = 4 * (size_t)(nco_bias > 1 ? nco_bias * d->cout : 256);  // bias of every column chunk of the launch
+    const size_t bias_bytes = 4 * (size_t)(nco_bias > 1 ? nco_bias * d->cout : TC_NMAX);  // bias of every column chunk of the launch
     const size_t A = (size_t)p.a_bytes, Bs = (size_t)p.b_bytes, S = (size_t)p.raw_bytes, slack = 1024 + bias_bytes;
     if (p.tma_act && 2 * A + 3 * S + 3 * Bs + slack <= budget) {
       ns = 3;
@@ -824,11 +657,6 @@ static int tc_plan(const pwgb_conv1d_desc* d, TcK& p, size_t& smem_bytes, int au
     p.ns = ns;
     p.tiles_per_seq = ceil_div(d->t_out, p.MT * 128);
     p.total_tiles = p.tiles_per_seq * d->batch;
-    const int cols = p.MT * d->cout;
-    p.nacc = 2 * cols <= 512 ? 2 : 1;
-    int alloc = 32;
-    while (alloc < p.nacc * cols) alloc <<= 1;
-    p.tmem_cols = alloc;
     smem_bytes = (size_t)na * p.a_bytes + (size_t)ns * p.raw_bytes + (size_t)nb * p.b_bytes + 8 * (2 * na + 2 * nb + 4 + 2 * NS_MAX) + 16 + bias_bytes;
     return 1;
   }
@@ -841,8 +669,7 @@ static int tc_launch(TcK& p, size_t bytes, const float* x, const void* packed_w,
   if (p.B == 0 || p.T_out == 0) return PWGB_OK;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv1d_tc_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv1d_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(conv1d_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
     if (e != cudaSuccess) {
       set_error("conv1d_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
       return PWGB_CUDA_ERROR;
@@ -854,7 +681,7 @@ static int tc_launch(TcK& p, size_t bytes, const float* x, const void* packed_w,
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (num_sms <= 0) num_sms = 148;
+    if (num_sms <= 0) num_sms = 132;
   }
   if ((long long)p.B * p.tiles_per_seq > 0x7fffffffLL) {
     set_error("conv1d_tc: too many tiles");
@@ -862,12 +689,8 @@ static int tc_launch(TcK& p, size_t bytes, const float* x, const void* packed_w,
   }
   if (p.tma_act && ((reinterpret_cast<uintptr_t>(x) & 15) || (x2 && (reinterpret_cast<uintptr_t>(x2) & 15))))
     p.tma_act = 0;  // unaligned base pointer: the producers stage with cp.async instead
-  if (p.shuffle_vec && ((reinterpret_cast<uintptr_t>(y) & 15) || p.co_off % 16 != 0)) p.shuffle_vec = 0;
   const int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
-  if (p.nco > 1 && p.shuffle <= 1)
-    conv1d_tc_kernel<1><<<(unsigned)grid, TC_THREADS, bytes, st>>>(p, x, x2, (const uint4*)packed_w, bias, residual, y, y2);
-  else
-    conv1d_tc_kernel<0><<<(unsigned)grid, TC_THREADS, bytes, st>>>(p, x, x2, (const uint4*)packed_w, bias, residual, y, y2);
+  conv1d_tc_kernel<<<(unsigned)grid, TC_THREADS, bytes, st>>>(p, x, x2, (const uint4*)packed_w, bias, residual, y, y2);
   return check_launch("conv1d_tc_kernel");
 }
 
@@ -905,19 +728,13 @@ using namespace pwgb;
 
 static int tc_cout_chunk(int cout);
 
-namespace pwgb {
-extern int g_wn_variant;
-int wn_trace_read(void* dst, size_t bytes);
-}
-
 extern "C" void pwgb_debug_set(int key, int value) {
   if (key == 1) g_tc_variant = value;
-  if (key == 2) pwgb::g_wn_variant = value;  // timing experiments of the fused WaveNet kernel (results are NOT valid)
 }
 
-// key 2: timeline of CTA 0 of the last traced fused WaveNet launch (synchronises the device; see wavenet_tc.cu)
+// no debug read-back is available in this build
 extern "C" int pwgb_debug_get(int key, void* dst, size_t bytes) {
-  if (key == 2 && dst) return pwgb::wn_trace_read(dst, bytes);
+  (void)key, (void)dst, (void)bytes;
   return -1;
 }
 
@@ -948,13 +765,11 @@ extern "C" int pwgb_conv1d_tc_pack_weight(const float* w, int cin, int cout, int
   return pwgb_conv1d_tc_pack_weight_grouped(w, cin, cout, kernel, 1, packed, stream);
 }
 
-// Output channels beyond the 256 accumulator columns of one launch are processed in column chunks
-// (one launch each, re-reading x): chunk = largest multiple of 16 that is <= 256 and divides cout.
+// Output channels beyond the TC_NMAX accumulator columns of one launch are processed in column chunks
+// (work items of one launch, each re-reading x): chunk = largest multiple of 16 that is <= 128 and divides cout.
 static int tc_cout_chunk(int cout) {
-  if (cout <= 256) return cout;
-  // wide layers (discriminator towers, 512 / 1024 channels on short sequences): 128-column chunks double the number
-  // of (chunk, batch, time tile) work items of the single launch, i.e. the number of SMs that have work
-  for (int c = 128; c >= 16; c -= 16)
+  if (cout <= TC_NMAX) return cout;
+  for (int c = TC_NMAX; c >= 16; c -= 16)
     if (cout % c == 0) return c;
   return 0;
 }
@@ -980,7 +795,7 @@ extern "C" int pwgb_conv1d_tc_supported(const pwgb_conv1d_desc* d) {
 extern "C" int pwgb_conv1d_tc_forward(const pwgb_conv1d_desc* d, const float* x, const void* packed_w,
                                       const float* bias, const float* residual, float* y, void* stream) {
   PWGB_CHECK_ARG(d && x && packed_w && y, "conv1d_tc: null argument");
-  PWGB_UNSUPPORTED_IF(!pwgb_conv1d_tc_supported(d), "conv1d_tc: configuration not supported by the tcgen05 path");
+  PWGB_UNSUPPORTED_IF(!pwgb_conv1d_tc_supported(d), "conv1d_tc: configuration not supported by the tensor-core path");
   const int G = d->groups, cin_g = d->cin / G, cout_g = d->cout / G;
   const int chunk = tc_cout_chunk(cout_g);
   pwgb_conv1d_desc c = *d;
@@ -1014,8 +829,8 @@ extern "C" int pwgb_conv1d_tc_forward(const pwgb_conv1d_desc* d, const float* x,
 }
 
 // ======================================================================================
-// WaveNet residual layer (layers/residual_block.py:102-140) as two tcgen05 launches:
-//   1) g = conv_k,dil(x) + W_aux c + b        (aux 1x1 folded into the same TMEM accumulation)
+// WaveNet residual layer (layers/residual_block.py:102-140) as two tensor-core launches:
+//   1) g = conv_k,dil(x) + W_aux c + b        (aux 1x1 folded into the same accumulation)
 //   2) z = tanh(g[:G/2]) * sigmoid(g[G/2:]) in the producer;  [skip | out] 1x1 stacked as one
 //      N = S + R contraction;  epilogue: skips += s,  x' = (o + x) * sqrt(0.5)
 // ======================================================================================
@@ -1086,7 +901,7 @@ extern "C" size_t pwgb_wavenet_packed_bytes(const pwgb_wavenet_desc* d) {
 extern "C" int pwgb_wavenet_pack(const pwgb_wavenet_desc* d, const float* w_conv, const float* w_aux,
                                  int aux_channels_real, const float* w_skip, const float* w_out, void* packed,
                                  void* stream) {
-  PWGB_UNSUPPORTED_IF(!pwgb_wavenet_supported(d), "wavenet_pack: configuration not supported by the tcgen05 path");
+  PWGB_UNSUPPORTED_IF(!pwgb_wavenet_supported(d), "wavenet_pack: configuration not supported by the tensor-core path");
   PWGB_CHECK_ARG(w_conv && w_skip && w_out && packed && (w_aux || d->aux_channels == 0), "wavenet_pack: null argument");
   PWGB_CHECK_ARG(aux_channels_real <= d->aux_channels, "wavenet_pack: aux_channels_real > padded aux_channels");
   cudaStream_t st = (cudaStream_t)stream;
@@ -1111,7 +926,7 @@ extern "C" int pwgb_wavenet_pack(const pwgb_wavenet_desc* d, const float* w_conv
 extern "C" int pwgb_wavenet_layer_forward(const pwgb_wavenet_desc* d, const float* x, const float* c,
                                           const void* packed, const float* b_conv, const float* b_skip_out,
                                           float* x_out, float* skips, float* g_ws, void* stream) {
-  PWGB_UNSUPPORTED_IF(!pwgb_wavenet_supported(d), "wavenet_layer: configuration not supported by the tcgen05 path");
+  PWGB_UNSUPPORTED_IF(!pwgb_wavenet_supported(d), "wavenet_layer: configuration not supported by the tensor-core path");
   PWGB_CHECK_ARG(x && packed && x_out && skips && g_ws && (c || d->aux_channels == 0), "wavenet_layer: null argument");
   PWGB_CHECK_ARG(x != x_out, "wavenet_layer: x_out must not alias x (halo reads)");
   cudaStream_t st = (cudaStream_t)stream;
@@ -1128,43 +943,128 @@ extern "C" int pwgb_wavenet_layer_forward(const pwgb_wavenet_desc* d, const floa
 }
 
 // ======================================================================================
-// Weight gradient on tcgen05:  dW[co, ci, k] = sum_{b,t} G[b,co,t] * X~[b,ci,t + k*D - pad]
+// Weight gradient on the tensor cores:  dW[co, ci, k] = sum_{b,t} G[b,co,t] * X~[b,ci,t + k*D - pad]
 // is a GEMM whose reduction (MMA K) dimension is TIME.  Both operands are used MN-major: the same
 // [channel/8][time row][8 channels] shared-memory tile as the forward activation tile, read with the
-// roles of the two axes swapped (instruction descriptor a_major = b_major = MN), so a tap is again a
-// row offset in the descriptor.  M = 128 output channels (TMEM lanes), N = 32 input channels, one
-// accumulator column block per tap (<= 8 taps = 256 columns, 2 CTAs / SM), bf16x3 split, fp32
-// accumulation over the CTA's (batch, time-chunk) items; split partials are reduced deterministically.
+// roles of the two axes swapped (wgmma transpose flags), so a tap is again a row offset in the descriptor.
+// M = 128 output channels (two warpgroups of 64), N = 32 or 64 input channels, one accumulator block per tap
+// (taps x N <= 128 columns: 64 fp32 registers per thread), bf16x3 split, fp32 accumulation over the CTA's
+// (batch, time-chunk) items; split partials are reduced deterministically.  The operand images are double
+// buffered: the 256 threads convert item n + 1 while the wgmma of item n run.
 // ======================================================================================
 namespace pwgb {
 
-constexpr int WT_NC = 32;    // input channels per CTA (MMA N); 64 for <= 4 taps (TMEM: taps x NC <= 256 columns)
+constexpr int WT_NC = 32;    // input channels per CTA (MMA N); 64 for <= 2 taps (taps x NC <= 128 columns)
 constexpr int WT_TK = 128;   // time steps per item (8 MMA k-steps)
-constexpr int WT_TG = 8;     // taps per CTA
-constexpr int WT_THREADS = 160;
+constexpr int WT_THREADS = 256;
 
 struct WtK {
   int B, Cin, Cout, T_in, T_out, K, D, padL;
   int G, Cin_g, Cout_g;  // groups: an M tile never straddles two groups (rows beyond the group's channels are zero)
   float x_slope, g_slope;
-  int chunks_per_seq, nsplit, RX, ntg, tg;  // tg = taps per CTA (<= WT_TG), ntg = tap groups
+  int chunks_per_seq, nsplit, RX, ntg, tg;  // tg = taps per CTA, ntg = tap groups
   int nc;                                   // input channels per CTA (32 or 64)
-  unsigned idesc;
 };
+
+// gradient tile (row = time, 8 output channels per 16 B) and activation tile (rows t0 + k0*D - pad ... + RX) of one
+// item, converted to the bf16 hi/lo operand images
+template <int NC>
+__device__ __forceinline__ void wt_fill(const WtK& p, const float* __restrict__ x, const float* __restrict__ gy, int b, int t0,
+                                        int co0, int co_end, int grp, int ci0, int k0, bool vec_a, bool vec_b,
+                                        unsigned char* a_buf, int a_img, unsigned char* b_buf, int b_img, int tid) {
+  const float* gb = gy + ((long long)b * p.Cout + co0) * p.T_out;
+  if (vec_a) {
+    // a task = (8-channel group, 4 consecutive rows); consecutive lanes take consecutive row quads of one group
+    for (int task = tid; task < 16 * (WT_TK / 4); task += WT_THREADS) {
+      const int g = task / (WT_TK / 4), rq = task - g * (WT_TK / 4);
+      const int t = t0 + 4 * rq;
+      const bool cok = t < p.T_out && (co0 + g * 8 < co_end);  // Cout_g % 8 == 0: whole 8-channel groups are in or out
+      float4 v[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        v[j] = cok ? __ldg(reinterpret_cast<const float4*>(gb + (long long)(g * 8 + j) * p.T_out + t)) : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+      for (int rr = 0; rr < 4; ++rr) {
+        float u[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float e = rr == 0 ? v[j].x : (rr == 1 ? v[j].y : (rr == 2 ? v[j].z : v[j].w));
+          u[j] = lrelu(e, p.g_slope);
+        }
+        uint4 hi, lo;
+        split8(u, hi, lo);
+        const int r = 4 * rq + rr;
+        *reinterpret_cast<uint4*>(a_buf + ((size_t)g * WT_TK + r) * 16) = hi;
+        *reinterpret_cast<uint4*>(a_buf + a_img + ((size_t)g * WT_TK + r) * 16) = lo;
+      }
+    }
+  } else {
+    for (int task = tid; task < 16 * WT_TK; task += WT_THREADS) {
+      const int g = task / WT_TK, r = task - g * WT_TK;
+      const int t = t0 + r;
+      const bool cok = t < p.T_out && (co0 + g * 8 < co_end);
+      float u[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) u[j] = cok ? lrelu(__ldg(gb + (long long)(g * 8 + j) * p.T_out + t), p.g_slope) : 0.f;
+      uint4 hi, lo;
+      split8(u, hi, lo);
+      *reinterpret_cast<uint4*>(a_buf + ((size_t)g * WT_TK + r) * 16) = hi;
+      *reinterpret_cast<uint4*>(a_buf + a_img + ((size_t)g * WT_TK + r) * 16) = lo;
+    }
+  }
+  const float* xb = x + ((long long)b * p.Cin + grp * p.Cin_g + ci0) * p.T_in;
+  const long long ts0 = (long long)t0 + (long long)k0 * p.D - p.padL;
+  if (vec_b) {
+    for (int task = tid; task < (NC / 8) * (p.RX / 4); task += WT_THREADS) {
+      const int g = task / (p.RX / 4), rq = task - g * (p.RX / 4);
+      const long long ts = ts0 + 4 * rq;
+      const bool ok = ts >= 0 && ts + 3 < p.T_in;  // T_in % 4 == 0 and ts % 4 == 0: a quad is entirely in or out
+      float4 v[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        v[j] = ok ? __ldg(reinterpret_cast<const float4*>(xb + (long long)(g * 8 + j) * p.T_in + ts)) : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+      for (int rr = 0; rr < 4; ++rr) {
+        float u[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float e = rr == 0 ? v[j].x : (rr == 1 ? v[j].y : (rr == 2 ? v[j].z : v[j].w));
+          u[j] = lrelu(e, p.x_slope);
+        }
+        uint4 hi, lo;
+        split8(u, hi, lo);
+        const int r = 4 * rq + rr;
+        *reinterpret_cast<uint4*>(b_buf + ((size_t)g * p.RX + r) * 16) = hi;
+        *reinterpret_cast<uint4*>(b_buf + b_img + ((size_t)g * p.RX + r) * 16) = lo;
+      }
+    }
+  } else {
+    for (int task = tid; task < (NC / 8) * p.RX; task += WT_THREADS) {
+      const int g = task / p.RX, r = task - g * p.RX;
+      const long long ts = ts0 + r;
+      const bool ok = ts >= 0 && ts < p.T_in;
+      float u[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) u[j] = ok ? lrelu(__ldg(xb + (long long)(g * 8 + j) * p.T_in + ts), p.x_slope) : 0.f;
+      uint4 hi, lo;
+      split8(u, hi, lo);
+      *reinterpret_cast<uint4*>(b_buf + ((size_t)g * p.RX + r) * 16) = hi;
+      *reinterpret_cast<uint4*>(b_buf + b_img + ((size_t)g * p.RX + r) * 16) = lo;
+    }
+  }
+}
 
 // NC = input channels per CTA (MMA N): 64 halves the number of CTAs that re-read and re-convert the gradient tile
 template <int NC>
-__global__ void __launch_bounds__(WT_THREADS, 2)
+__global__ void __launch_bounds__(WT_THREADS, 1)
     wgrad_tc_kernel(const WtK p, const float* __restrict__ x, const float* __restrict__ gy, float* __restrict__ part) {
   extern __shared__ __align__(128) unsigned char smem[];
-  // A (gradient) image: [hi|lo][16 co8][WT_TK rows][16 B];  B (activation) image: [hi|lo][4 ci8][RX rows][16 B]
-  unsigned char* a_buf = smem;
+  // per buffer: A (gradient) image [hi|lo][16 co8][WT_TK rows][16 B];  B (activation) image [hi|lo][NC/8 ci8][RX rows][16 B]
   const int a_img = 16 * WT_TK * 16;
-  unsigned char* b_buf = smem + 2 * a_img;
   const int b_img = (NC / 8) * p.RX * 16;
-  unsigned long long* bars = reinterpret_cast<unsigned long long*>(b_buf + 2 * b_img);
-  unsigned* tmem_slot = reinterpret_cast<unsigned*>(bars + 3);
+  const int buf_bytes = 2 * a_img + 2 * b_img;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = warp >> 2, wq = warp & 3;
   const int tpg = (p.Cout_g + 127) / 128;  // M tiles per group
   const int grp = blockIdx.x / tpg;
   const int co0 = grp * p.Cout_g + (blockIdx.x - grp * tpg) * 128;
@@ -1173,181 +1073,67 @@ __global__ void __launch_bounds__(WT_THREADS, 2)
   const int k0 = (blockIdx.y % p.ntg) * p.tg;
   const int ntap = min(p.tg, p.K - k0);
   const int split = blockIdx.z;
-  const unsigned bar0 = smem_u32(bars);
-  const unsigned FULL = bar0, EMPTY = bar0 + 8, ACC = bar0 + 16;
-  if (tid == 0) {
-    mbar_init(FULL, 128);
-    mbar_init(EMPTY, 1);
-    mbar_init(ACC, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 4) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(256u)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const unsigned tmem_base = *tmem_slot;
   const int total_items = p.B * p.chunks_per_seq;
-
-  if (warp < 4) {
-    unsigned n = 0;
-    // 16-byte loads need 16-byte aligned rows: row pitch and window offset multiples of 4 samples
-    const bool vec_a = p.T_out % 4 == 0 && (reinterpret_cast<uintptr_t>(gy) & 15) == 0;
-    const bool vec_b = p.T_in % 4 == 0 && p.RX % 4 == 0 && ((long long)k0 * p.D - p.padL) % 4 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0;
-    for (int item = split; item < total_items; item += p.nsplit, ++n) {
-      const int b = item / p.chunks_per_seq;
-      const int t0 = (item - b * p.chunks_per_seq) * WT_TK;
-      mbar_wait(EMPTY, (n & 1) ^ 1);
-      // gradient tile: row = time, 8 output channels per 16 B
-      const float* gb = gy + ((long long)b * p.Cout + co0) * p.T_out;
-      if (vec_a) {
-        // 16-byte loads along time: a task = (8-channel group, 4 consecutive rows); a warp's lanes take consecutive row
-        // quads of one group (512 contiguous bytes per channel).  Two tasks (16 LDG.128) are in flight per thread: the
-        // scalar version kept 16 KB per CTA in flight and paid four DRAM round trips per item.
+  // 16-byte loads need 16-byte aligned rows: row pitch and window offset multiples of 4 samples
+  const bool vec_a = p.T_out % 4 == 0 && (reinterpret_cast<uintptr_t>(gy) & 15) == 0;
+  const bool vec_b = p.T_in % 4 == 0 && p.RX % 4 == 0 && ((long long)k0 * p.D - p.padL) % 4 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0;
+  constexpr int TGMAX = 128 / NC;  // accumulator blocks of NC columns
+  float acc[64];
 #pragma unroll
-        for (int it = 0; it < 4; it += 2) {
-          float4 v[2][8];
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int g = (it + h) * 4 + warp;
-            const int t = t0 + 4 * lane;
-            const bool cok = t < p.T_out && (co0 + g * 8 < co_end);
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              v[h][j] = cok ? __ldg(reinterpret_cast<const float4*>(gb + (long long)(g * 8 + j) * p.T_out + t)) : make_float4(0.f, 0.f, 0.f, 0.f);
-          }
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int g = (it + h) * 4 + warp;
-#pragma unroll
-            for (int rr = 0; rr < 4; ++rr) {
-              float u[8];
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const float e = rr == 0 ? v[h][j].x : (rr == 1 ? v[h][j].y : (rr == 2 ? v[h][j].z : v[h][j].w));
-                u[j] = lrelu(e, p.g_slope);
-              }
-              uint4 hi, lo;
-              split8(u, hi, lo);
-              const int r = 4 * lane + rr;
-              *reinterpret_cast<uint4*>(a_buf + ((size_t)g * WT_TK + r) * 16) = hi;
-              *reinterpret_cast<uint4*>(a_buf + a_img + ((size_t)g * WT_TK + r) * 16) = lo;
-            }
-          }
-        }
-      } else {
-        for (int r = tid; r < WT_TK; r += 128) {
-          const int t = t0 + r;
-          const bool ok = t < p.T_out;
-#pragma unroll 4
-          for (int g = 0; g < 16; ++g) {
-            float u[8];
-            const bool cok = ok && (co0 + g * 8 < co_end);  // Cout_g % 8 == 0: whole 8-channel groups are in or out
-#pragma unroll
-            for (int j = 0; j < 8; ++j) u[j] = cok ? lrelu(__ldg(gb + (long long)(g * 8 + j) * p.T_out + t), p.g_slope) : 0.f;
-            uint4 hi, lo;
-            split8(u, hi, lo);
-            *reinterpret_cast<uint4*>(a_buf + ((size_t)g * WT_TK + r) * 16) = hi;
-            *reinterpret_cast<uint4*>(a_buf + a_img + ((size_t)g * WT_TK + r) * 16) = lo;
-          }
-        }
-      }
-      // activation tile: rows t0 + k0*D - pad ... (+ RX)
-      const float* xb = x + ((long long)b * p.Cin + grp * p.Cin_g + ci0) * p.T_in;
-      const long long ts0 = (long long)t0 + (long long)k0 * p.D - p.padL;
-      if (vec_b) {
-        for (int task = tid; task < (NC / 8) * (p.RX / 4); task += 128) {
-          const int g = task / (p.RX / 4), rq = task - g * (p.RX / 4);
-          const long long ts = ts0 + 4 * rq;
-          const bool ok = ts >= 0 && ts + 3 < p.T_in;  // T_in % 4 == 0 and ts % 4 == 0: a quad is entirely in or out
-          float4 v[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            v[j] = ok ? __ldg(reinterpret_cast<const float4*>(xb + (long long)(g * 8 + j) * p.T_in + ts)) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-          for (int rr = 0; rr < 4; ++rr) {
-            float u[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float e = rr == 0 ? v[j].x : (rr == 1 ? v[j].y : (rr == 2 ? v[j].z : v[j].w));
-              u[j] = lrelu(e, p.x_slope);
-            }
-            uint4 hi, lo;
-            split8(u, hi, lo);
-            const int r = 4 * rq + rr;
-            *reinterpret_cast<uint4*>(b_buf + ((size_t)g * p.RX + r) * 16) = hi;
-            *reinterpret_cast<uint4*>(b_buf + b_img + ((size_t)g * p.RX + r) * 16) = lo;
-          }
-        }
-      } else {
-        for (int r = tid; r < p.RX; r += 128) {
-          const long long ts = ts0 + r;
-          const bool ok = ts >= 0 && ts < p.T_in;
-#pragma unroll
-          for (int g = 0; g < NC / 8; ++g) {
-            float u[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) u[j] = ok ? lrelu(__ldg(xb + (long long)(g * 8 + j) * p.T_in + ts), p.x_slope) : 0.f;
-            uint4 hi, lo;
-            split8(u, hi, lo);
-            *reinterpret_cast<uint4*>(b_buf + ((size_t)g * p.RX + r) * 16) = hi;
-            *reinterpret_cast<uint4*>(b_buf + b_img + ((size_t)g * p.RX + r) * 16) = lo;
-          }
-        }
-      }
-      fence_proxy_async();
-      mbar_arrive(FULL);
-    }
-    // ---- epilogue: lane = output channel, column = tap * NC + ci
-    mbar_wait(ACC, 0);
-    tc_fence_after();
-    const int co = co0 + warp * 32 + lane;
-    const bool co_ok = co < co_end;
-    float* dst = part + (((long long)split * p.Cout + (co_ok ? co : 0)) * p.Cin_g + ci0) * p.K + k0;
-    for (int tp = 0; tp < ntap; ++tp) {
-      for (int c16 = 0; c16 < NC; c16 += 16) {
-        unsigned r[16];
-        tc_ld16(tmem_base + ((unsigned)(warp * 32) << 16) + (unsigned)(tp * NC + c16), r);
-        tc_wait_ld();
-        if (co_ok) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) dst[(long long)(c16 + j) * p.K + tp] = __uint_as_float(r[j]);
-        }
-      }
-    }
-    tc_fence_before();
-  } else {
-    // ---- MMA issuer (converged warp, elected lane)
-    const unsigned long long hi_const = ((unsigned long long)(1u << 14)) << 32;  // version = 1; SBO goes in per operand
-    const unsigned a16 = smem_u32(a_buf) >> 4, b16 = smem_u32(b_buf) >> 4;
-    // MN-major no-swizzle: LBO = 8-row K group stride (128 B = 8 units), SBO = MN 16 B-chunk stride (rows * 16 B)
-    const unsigned long long a_hi = ((unsigned long long)((unsigned)WT_TK & 0x3FFFu) << 32) | hi_const;
-    const unsigned long long b_hi = ((unsigned long long)((unsigned)p.RX & 0x3FFFu) << 32) | hi_const;
-    const unsigned lbo = 8u << 16;
-    const unsigned a_sub = (unsigned)(a_img >> 4), b_sub = (unsigned)(b_img >> 4);
-    unsigned n = 0;
-    for (int item = split; item < total_items; item += p.nsplit, ++n) {
-      mbar_wait_spin(FULL, n & 1);
-      tc_fence_after();
-      for (int ks = 0; ks < WT_TK / 16; ++ks) {
-        const unsigned long long ad = a_hi | (unsigned long long)(lbo + a16 + (unsigned)(ks * 16));
-        for (int tp = 0; tp < ntap; ++tp) {
-          const unsigned long long bd = b_hi | (unsigned long long)(lbo + b16 + (unsigned)(tp * p.D + ks * 16));
-          const unsigned acc = (n | (unsigned)ks) != 0 ? 1u : 0u;
-          tc_mma_x3_single(tmem_base + (unsigned)(tp * NC), ad, bd, a_sub, b_sub, p.idesc, acc);
-        }
-      }
-      tc_commit(EMPTY);
-    }
-    tc_commit(ACC);
+  for (int e = 0; e < 64; ++e) acc[e] = 0.f;
+  // MN-major no-swizzle: LBO = next 8 time rows (128 B), SBO = next 8 channels (rows * 16 B)
+  const unsigned a_sbo = WT_TK * 16, b_sbo = (unsigned)p.RX * 16;
+  int buf = 0;
+  if (split < total_items) {
+    const int b = split / p.chunks_per_seq;
+    wt_fill<NC>(p, x, gy, b, (split - b * p.chunks_per_seq) * WT_TK, co0, co_end, grp, ci0, k0, vec_a, vec_b, smem, a_img,
+                smem + 2 * a_img, b_img, tid);
   }
+  fence_proxy_async();
   __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256u) : "memory");
+  for (int item = split; item < total_items; item += p.nsplit) {
+    unsigned char* a_buf = smem + (size_t)buf * buf_bytes;
+    const unsigned a_addr = smem_u32(a_buf) + (unsigned)(wg * 8) * a_sbo;  // this warpgroup's 64 output channels
+    const unsigned b_addr = smem_u32(a_buf + 2 * a_img);
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < WT_TK / 16; ++ks) {
+      const unsigned long long ah = gmma_desc(a_addr + (unsigned)(ks * 16 * 16), 128, a_sbo);
+      const unsigned long long al = ah + (unsigned)(a_img >> 4);
+#pragma unroll
+      for (int tp = 0; tp < TGMAX; ++tp) {
+        if (tp < ntap) {
+          const unsigned long long bh = gmma_desc(b_addr + (unsigned)((tp * p.D + ks * 16) * 16), 128, b_sbo);
+          const unsigned long long bl = bh + (unsigned)(b_img >> 4);
+          float* d = acc + tp * (NC / 2);
+          Wgmma<NC, 1, 1>::run(d, ah, bh);
+          Wgmma<NC, 1, 1>::run(d, al, bh);
+          Wgmma<NC, 1, 1>::run(d, ah, bl);
+        }
+      }
+    }
+    wg_commit();
+    // convert the next item into the other buffer while the MMAs run
+    const int next = item + p.nsplit;
+    if (next < total_items) {
+      unsigned char* nb = smem + (size_t)(buf ^ 1) * buf_bytes;
+      const int b = next / p.chunks_per_seq;
+      wt_fill<NC>(p, x, gy, b, (next - b * p.chunks_per_seq) * WT_TK, co0, co_end, grp, ci0, k0, vec_a, vec_b, nb, a_img,
+                  nb + 2 * a_img, b_img, tid);
+      fence_proxy_async();
+    }
+    wg_wait<0>();
+    __syncthreads();
+    buf ^= 1;
+  }
+  // ---- epilogue: row = output channel, column = tap * NC + ci
+#pragma unroll
+  for (int e = 0; e < 64; ++e) {
+    const int tp = e / (NC / 2), i = e % (NC / 2);
+    const int n = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+    const int co = co0 + wg * 64 + wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+    if (tp < ntap && co < co_end)
+      part[(((long long)split * p.Cout + co) * p.Cin_g + ci0 + n) * p.K + k0 + tp] = acc[e];
   }
 }
 
@@ -1379,28 +1165,27 @@ static int wt_plan(const pwgb_conv1d_desc* d, WtK& p) {
   p.x_slope = d->pre_slope;
   p.g_slope = 1.f;
   p.chunks_per_seq = ceil_div(d->t_out, WT_TK);
-  // 64 input channels per CTA when the taps fit the accumulator (taps x 64 <= 256 TMEM columns): the (dominant)
+  // 64 input channels per CTA when the taps fit the accumulator (taps x 64 <= 128 columns): the (dominant)
   // gradient tile is then read and converted once per 64 instead of once per 32 input channels
-  p.nc = (cin_g % 64 == 0 && d->kernel <= 4) ? 64 : WT_NC;
+  p.nc = (cin_g % 64 == 0 && d->kernel <= 2) ? 64 : WT_NC;
   // taps per CTA: as many as fit (the activation window grows with (taps - 1) * dilation)
-  int tg = d->kernel < WT_TG ? d->kernel : WT_TG;
+  const int tg_max = 128 / p.nc;
+  int tg = d->kernel < tg_max ? d->kernel : tg_max;
   for (;; tg = (tg + 1) / 2) {
     p.RX = WT_TK + (tg - 1) * d->dilation;
-    if ((size_t)2 * 16 * WT_TK * 16 + (size_t)2 * (p.nc / 8) * p.RX * 16 + 64 <= 110 * 1024) break;
+    if (2 * ((size_t)2 * 16 * WT_TK * 16 + (size_t)2 * (p.nc / 8) * p.RX * 16) <= 220 * 1024) break;
     if (tg == 1) return 0;
   }
   p.tg = tg;
   p.ntg = ceil_div(d->kernel, tg);
   const long long items = (long long)p.B * p.chunks_per_seq;
   const long long gxy = (long long)d->groups * ceil_div(cout_g, 128) * (cin_g / p.nc) * p.ntg;
-  // enough (tile, split) CTAs for two per SM on 148 SMs; a split keeps at least 8 items (1024 time steps) of work
-  long long ns = (2 * 296 + gxy - 1) / gxy;
+  // enough (tile, split) CTAs for two waves over 132 SMs; a split keeps at least 8 items (1024 time steps) of work
+  long long ns = (2 * 132 + gxy - 1) / gxy;
   if (ns > items / 8) ns = items / 8;
   if (ns > 512) ns = 512;
   if (ns < 1) ns = 1;
   p.nsplit = (int)ns;
-  // D = f32, A = B = bf16, both MN-major (bits 15, 16), N >> 3 @ 17, M >> 4 @ 24
-  p.idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((unsigned)(p.nc >> 3) << 17) | ((128u >> 4) << 24);
   return 1;
 }
 
@@ -1422,7 +1207,7 @@ extern "C" int pwgb_conv1d_wgrad_tc(const pwgb_conv1d_desc* d, const float* x, c
   using namespace pwgb;
   PWGB_CHECK_ARG(d && x && gy && dw && ws, "conv1d_wgrad_tc: null argument");
   WtK p;
-  PWGB_UNSUPPORTED_IF(!wt_plan(d, p), "conv1d_wgrad_tc: configuration not supported by the tcgen05 path");
+  PWGB_UNSUPPORTED_IF(!wt_plan(d, p), "conv1d_wgrad_tc: configuration not supported by the tensor-core path");
   p.g_slope = g_slope;
   const size_t need = pwgb_conv1d_wgrad_tc_workspace(d);
   PWGB_CHECK_ARG(ws_bytes >= need, "conv1d_wgrad_tc: workspace too small (%zu < %zu)", ws_bytes, need);
@@ -1432,11 +1217,11 @@ extern "C" int pwgb_conv1d_wgrad_tc(const pwgb_conv1d_desc* d, const float* x, c
     cudaMemsetAsync(dw, 0, n * sizeof(float), st);
     return PWGB_OK;
   }
-  const size_t smem = (size_t)2 * 16 * WT_TK * 16 + (size_t)2 * (p.nc / 8) * p.RX * 16 + 64;
+  const size_t smem = 2 * ((size_t)2 * 16 * WT_TK * 16 + (size_t)2 * (p.nc / 8) * p.RX * 16);
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(wgrad_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(wgrad_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
     if (e != cudaSuccess) {
       set_error("conv1d_wgrad_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
       return PWGB_CUDA_ERROR;

@@ -3,6 +3,7 @@
 // re-laid out on device to the virtual conv  (cout*s, cin, M)  and the generic conv kernel
 // writes through a pixel-shuffle epilogue  o = i*s + phase - padding.
 #include "common.cuh"
+#include "tc_common.cuh"
 
 namespace pwgb {
 
@@ -38,7 +39,7 @@ using namespace pwgb;
 extern "C" size_t pwgb_conv_transpose1d_workspace(const pwgb_convtr1d_desc* d) {
   if (!d || d->stride <= 0) return 0;
   const int M = ceil_div(d->kernel, d->stride);
-  // [virtual-conv fp32 weights][bf16 hi/lo operand image of the same weights for the tcgen05 path]
+  // [virtual-conv fp32 weights][bf16 hi/lo operand image of the same weights for the tensor-core path]
   const int G = d->groups > 1 ? d->groups : 1;
   return 2 * (size_t)d->cout * d->stride * (d->cin / G) * M * sizeof(float);
 }
@@ -85,11 +86,11 @@ extern "C" int pwgb_conv_transpose1d_forward(const pwgb_convtr1d_desc* d, const 
   c.shuffle = s;
   c.shuffle_pad = d->padding;
   c.shuffle_tout = d->t_out;
-  // tcgen05 path: N (= cout*s virtual channels) in chunks of <= 256 accumulator columns
+  // tensor-core path: N (= cout*s virtual channels) in chunks of <= TC_NMAX accumulator columns
   if (G == 1 && P == 1 && d->cin % 32 == 0 && c.cout % 16 == 0) {
     int chunk = c.cout;
-    if (chunk > 256) {
-      chunk = 256;
+    if (chunk > TC_NMAX) {
+      chunk = TC_NMAX;
       while (c.cout % chunk) chunk -= 16;
     }
     pwgb_conv1d_desc cc = c;

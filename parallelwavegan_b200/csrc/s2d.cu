@@ -1,6 +1,6 @@
 // Space-to-depth along time: turns a stride-s Conv1d (or the (k,1)-strided Conv2d of the period
 // discriminators, hifigan.py:354-381) into a stride-1 conv with s x the input channels and ceil(K/s) taps
-// -- the shape the tcgen05 kernels take.  With k = s*j + r:
+// -- the shape the tensor-core kernels take.  With k = s*j + r:
 //   y[t] = sum_k w[k] x[s*t + k - pad] = sum_r sum_j w[s*j + r] xs_r[t + j],   xs_r[u] = x[s*u + r - pad].
 // One HBM-bound gather pass (and its adjoint, also a gather: (row + pad) <-> (u, r) is a bijection).
 #include "common.cuh"
@@ -67,7 +67,7 @@ extern "C" int pwgb_s2d_forward(const float* x, float* y, int batch, int channel
   PWGB_CHECK_ARG(cgo >= channels / groups * stride, "s2d_forward: group_channels_out smaller than stride * channels per group");
   const long long total = (long long)batch * groups * cgo * rows_out * period;
   if (total == 0) return PWGB_OK;
-  int blocks = (int)((total + 255) / 256 > 148 * 16 ? 148 * 16 : (total + 255) / 256);
+  int blocks = (int)((total + 255) / 256 > 132 * 16 ? 132 * 16 : (total + 255) / 256);
   s2d_forward_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(x, y, channels, channels / groups, cgo, rows_in, period, stride, pad_left,
                                                              rows_out, total);
   return check_launch("s2d_forward_kernel");
@@ -80,7 +80,7 @@ extern "C" int pwgb_s2d_backward(const float* gy, float* gx, int batch, int chan
   PWGB_CHECK_ARG(cgo >= channels / groups * stride, "s2d_backward: group_channels_out smaller than stride * channels per group");
   const long long total = (long long)batch * channels * rows_in * period;
   if (total == 0) return PWGB_OK;
-  int blocks = (int)((total + 255) / 256 > 148 * 16 ? 148 * 16 : (total + 255) / 256);
+  int blocks = (int)((total + 255) / 256 > 132 * 16 ? 132 * 16 : (total + 255) / 256);
   s2d_backward_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(gy, gx, channels, channels / groups, cgo, rows_in, period, stride, pad_left,
                                                               rows_out, total);
   return check_launch("s2d_backward_kernel");

@@ -8,7 +8,7 @@ namespace pwgb {
 
 static int grid_for(long long n) {
   long long b = (n + 255) / 256;
-  if (b > 148LL * 16) b = 148LL * 16;
+  if (b > 132LL * 16) b = 132LL * 16;
   return b < 1 ? 1 : (int)b;
 }
 

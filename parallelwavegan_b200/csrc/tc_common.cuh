@@ -1,13 +1,14 @@
-// tcgen05 / TMEM / mbarrier / bulk-copy PTX helpers shared by the tensor-core kernels (sm_100a).
+// mbarrier / bulk-copy PTX helpers and the bf16 hi/lo split shared by the tensor-core kernels (sm_90a).
 #pragma once
 #include <cuda_bf16.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace pwgb {
 
-constexpr int KC = 32;  // input channels per activation chunk / weight stage (2 UMMA K-steps).  KC = 16 was
-                        // measured slower (22.3 vs 18.5 ms / step): the per-stage barrier round trip dominates
+constexpr int KC = 32;  // input channels per activation chunk / weight stage (2 MMA K-steps)
+constexpr int TC_NMAX = 128;  // accumulator columns of one launch: 64 rows x 128 fp32 = 64 registers per consumer thread
 constexpr unsigned SPIN_LIMIT = 1u << 22;
 #ifndef PWGB_NPROD
 #define PWGB_NPROD 256
@@ -96,11 +97,7 @@ __device__ __forceinline__ void cp_async_wait() {
 }
 __device__ __forceinline__ void producer_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(PWGB_NPROD) : "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// One elected lane of a converged warp (all 32 lanes must call this).  Keeping the issuing warp
-// converged lets the compiler hold descriptors in uniform registers; a `lane == 0` branch instead
-// forces R2UR moves + an ELECT retry loop around every UTCHMMA (~150 cycles per MMA, measured).
+// One elected lane of a converged warp (all 32 lanes must call this).
 __device__ __forceinline__ unsigned elect_one() {
   unsigned pred;
   asm volatile(
@@ -110,125 +107,8 @@ __device__ __forceinline__ unsigned elect_one() {
       : "=r"(pred));
   return pred;
 }
-__device__ __forceinline__ void tc_commit(unsigned bar) {
-  if (elect_one())
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_mma(unsigned d_tmem, unsigned long long adesc, unsigned long long bdesc,
-                                       unsigned idesc, unsigned accumulate) {
-  if (elect_one())
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// All bf16x3 passes of one (k-step, tap) for up to two 128-row m-tiles in ONE asm block: a single
-// elect.sync and descriptor arithmetic in PTX (u64 adds on the 14-bit start-address field) instead of
-// one elect + register->uniform moves per MMA.  d1 = d0 + dcol, a(mt=1) = a0 + 128 rows (8 units... 128
-// 16-byte units), lo images at +a_sub / +b_sub.
-__device__ __forceinline__ void tc_mma_x3(unsigned d0, unsigned long long a_hi, unsigned long long b_hi,
-                                          unsigned a_sub, unsigned b_sub, unsigned idesc, unsigned accumulate,
-                                          unsigned two_tiles, unsigned dcol) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred pe, pacc, p2;\n\t"
-      ".reg .b64 a_lo, b_lo, a1_hi, a1_lo, t64;\n\t"
-      ".reg .b32 d1;\n\t"
-      "elect.sync _|pe, 0xffffffff;\n\t"
-      "setp.ne.b32 pacc, %6, 0;\n\t"
-      "setp.ne.b32 p2, %7, 0;\n\t"
-      "and.pred p2, p2, pe;\n\t"
-      "cvt.u64.u32 t64, %3;\n\t"
-      "add.u64 a_lo, %1, t64;\n\t"
-      "cvt.u64.u32 t64, %4;\n\t"
-      "add.u64 b_lo, %2, t64;\n\t"
-      "add.u64 a1_hi, %1, 128;\n\t"
-      "add.u64 a1_lo, a_lo, 128;\n\t"
-      "add.u32 d1, %0, %8;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %5, pacc;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], a_lo, %2, %5, 1;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], %1, b_lo, %5, 1;\n\t"
-      "@p2 tcgen05.mma.cta_group::1.kind::f16 [d1], a1_hi, %2, %5, pacc;\n\t"
-      "@p2 tcgen05.mma.cta_group::1.kind::f16 [d1], a1_lo, %2, %5, 1;\n\t"
-      "@p2 tcgen05.mma.cta_group::1.kind::f16 [d1], a1_hi, b_lo, %5, 1;\n\t"
-      "}" ::"r"(d0),
-      "l"(a_hi), "l"(b_hi), "r"(a_sub), "r"(b_sub), "r"(idesc), "r"(accumulate), "r"(two_tiles), "r"(dcol)
-      : "memory");
-}
-// single m-tile variant (Cout > 128: one 128-row tile per CTA item)
-__device__ __forceinline__ void tc_mma_x3_single(unsigned d0, unsigned long long a_hi, unsigned long long b_hi,
-                                                 unsigned a_sub, unsigned b_sub, unsigned idesc, unsigned accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred pe, pacc;\n\t"
-      ".reg .b64 a_lo, b_lo, t64;\n\t"
-      "elect.sync _|pe, 0xffffffff;\n\t"
-      "setp.ne.b32 pacc, %6, 0;\n\t"
-      "cvt.u64.u32 t64, %3;\n\t"
-      "add.u64 a_lo, %1, t64;\n\t"
-      "cvt.u64.u32 t64, %4;\n\t"
-      "add.u64 b_lo, %2, t64;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %5, pacc;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], a_lo, %2, %5, 1;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], %1, b_lo, %5, 1;\n\t"
-      "}" ::"r"(d0),
-      "l"(a_hi), "l"(b_hi), "r"(a_sub), "r"(b_sub), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Both K-steps of one (chunk, tap) for one m-tile: 6 MMAs from two base descriptors.  Everything that
-// differs between the six instructions is added in the uniform datapath inside the block, so the
-// issuing thread pays the register->uniform moves once per tap instead of once per MMA.
-// a_step / b_step: descriptor distance of the second 16-channel K-step (16-byte units).
-__device__ __forceinline__ void tc_mma_tap6(unsigned d0, unsigned long long a_hi, unsigned long long b_hi, unsigned a_sub,
-                                            unsigned b_sub, unsigned a_step, unsigned b_step, unsigned idesc,
-                                            unsigned accumulate) {
-  static_assert(KC == 32, "tc_mma_tap6 issues exactly two K-steps");
-  asm volatile(
-      "{\n\t"
-      ".reg .pred pe, pacc;\n\t"
-      ".reg .b64 a_lo, b_lo, a1, b1, a1_lo, b1_lo, t64;\n\t"
-      "elect.sync _|pe, 0xffffffff;\n\t"
-      "setp.ne.b32 pacc, %8, 0;\n\t"
-      "cvt.u64.u32 t64, %3;\n\t"
-      "add.u64 a_lo, %1, t64;\n\t"
-      "cvt.u64.u32 t64, %4;\n\t"
-      "add.u64 b_lo, %2, t64;\n\t"
-      "cvt.u64.u32 t64, %5;\n\t"
-      "add.u64 a1, %1, t64;\n\t"
-      "add.u64 a1_lo, a_lo, t64;\n\t"
-      "cvt.u64.u32 t64, %6;\n\t"
-      "add.u64 b1, %2, t64;\n\t"
-      "add.u64 b1_lo, b_lo, t64;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %7, pacc;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], a_lo, %2, %7, 1;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], %1, b_lo, %7, 1;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], a1, b1, %7, 1;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], a1_lo, b1, %7, 1;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], a1, b1_lo, %7, 1;\n\t"
-      "}" ::"r"(d0),
-      "l"(a_hi), "l"(b_hi), "r"(a_sub), "r"(b_sub), "r"(a_step), "r"(b_step), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tc_ld16(unsigned taddr, unsigned (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void prefetch_l2(const void* ptr) { asm volatile("prefetch.global.L2 [%0];" ::"l"(ptr)); }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major, no-swizzle UMMA shared-memory descriptor (cute::UMMA::SmemDescriptor bit layout):
-// [0,14) start>>4, [16,30) LBO>>4 (K-adjacent core matrix), [32,46) SBO>>4 (8-row group stride),
-// [46,48) version = 1 (Blackwell), [61,64) layout = 0 (SWIZZLE_NONE).
-__device__ __forceinline__ unsigned long long make_desc(unsigned addr, unsigned lbo, unsigned sbo) {
-  return (unsigned long long)((addr >> 4) & 0x3FFF) | ((unsigned long long)((lbo >> 4) & 0x3FFF) << 16) |
-         ((unsigned long long)((sbo >> 4) & 0x3FFF) << 32) | (1ull << 46);
-}
+// named barrier of the 128 threads of warpgroup `wg` (ids 2.. ; id 1 is the conv producers' barrier)
+__device__ __forceinline__ void wg_barrier(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory"); }
 
 __device__ __forceinline__ void split8(const float (&v)[8], uint4& hi, uint4& lo) {
   unsigned h[4], l[4];
@@ -244,7 +124,7 @@ __device__ __forceinline__ void split8(const float (&v)[8], uint4& hi, uint4& lo
   lo = make_uint4(l[0], l[1], l[2], l[3]);
 }
 
-// w (rows, cin_real, K) fp32 -> rows [co_begin, co_begin + rows) of the tcgen05 weight operand image
+// w (rows, cin_real, K) fp32 -> rows [co_begin, co_begin + rows) of the tensor-core weight operand image
 // [chunk][tap][hi|lo][ci8][co (cout_total)][8] bf16 (defined in conv1d_tc.cu)
 void tc_pack_rows(const float* w, void* packed, int cin_real, int cin_pad, int rows, int K, int co_begin, int cout_total,
                   cudaStream_t st);

@@ -47,7 +47,7 @@ def activation_slope(name, params):
         return float((params or {}).get("negative_slope", 0.01))
     if name == "ReLU":
         return 0.0
-    raise PwgbError(f"nonlinear_activation={name!r} has no sm_100a kernel (supported: LeakyReLU, ReLU)")
+    raise PwgbError(f"nonlinear_activation={name!r} has no sm_90a kernel (supported: LeakyReLU, ReLU)")
 
 
 class Conv1d(torch.nn.Conv1d):
@@ -94,7 +94,7 @@ class CausalConvTranspose1d(torch.nn.Module):
                  pad="ReplicationPad1d", pad_params={}):
         super().__init__()
         if pad not in ("ReplicationPad1d", "ConstantPad1d", "ReflectionPad1d"):
-            raise PwgbError(f"CausalConvTranspose1d: pad={pad!r} has no sm_100a kernel")
+            raise PwgbError(f"CausalConvTranspose1d: pad={pad!r} has no sm_90a kernel")
         self.pad = getattr(torch.nn, pad)((1, 0), **pad_params)
         self.deconv = torch.nn.ConvTranspose1d(in_channels, out_channels, kernel_size, stride, bias=bias)
         self.stride = stride
@@ -229,7 +229,7 @@ def pad_mode_of(pad, pad_params):
         return "replicate"
     if pad == "ConstantPad1d" and float((pad_params or {}).get("value", 0.0)) == 0.0:
         return "zero"
-    raise PwgbError(f"pad={pad!r} {pad_params!r} has no sm_100a kernel (supported: ReflectionPad1d, ReplicationPad1d, zero ConstantPad1d)")
+    raise PwgbError(f"pad={pad!r} {pad_params!r} has no sm_90a kernel (supported: ReflectionPad1d, ReplicationPad1d, zero ConstantPad1d)")
 
 
 def design_prototype_filter(taps=62, cutoff_ratio=0.142, beta=9.0):
@@ -308,9 +308,9 @@ class WaveNetResidualBlock(torch.nn.Module):
     ):
         super().__init__()
         if use_causal_conv:
-            raise PwgbError("WaveNetResidualBlock(use_causal_conv=True) has no sm_100a kernel yet")
+            raise PwgbError("WaveNetResidualBlock(use_causal_conv=True) has no sm_90a kernel yet")
         if dropout != 0.0:
-            raise PwgbError("WaveNetResidualBlock(dropout>0) has no sm_100a kernel (all reference configs use 0.0)")
+            raise PwgbError("WaveNetResidualBlock(dropout>0) has no sm_90a kernel (all reference configs use 0.0)")
         assert (kernel_size - 1) % 2 == 0, "Not support even number kernel size."
         self.dropout = dropout
         self.dilation = dilation
@@ -374,7 +374,7 @@ class Stretch2d(torch.nn.Module):
     def __init__(self, x_scale, y_scale, mode="nearest"):
         super().__init__()
         if mode != "nearest" or y_scale != 1:
-            raise PwgbError("Stretch2d: only nearest time-axis stretching has an sm_100a kernel")
+            raise PwgbError("Stretch2d: only nearest time-axis stretching has an sm_90a kernel")
         self.x_scale, self.y_scale, self.mode = x_scale, y_scale, mode
 
 
@@ -394,7 +394,7 @@ class UpsampleNetwork(torch.nn.Module):
                  interpolate_mode="nearest", freq_axis_kernel_size=1, use_causal_conv=False):
         super().__init__()
         if use_causal_conv or nonlinear_activation is not None or freq_axis_kernel_size != 1:
-            raise PwgbError("UpsampleNetwork: causal / nonlinear / freq-axis-kernel variants have no sm_100a kernel yet")
+            raise PwgbError("UpsampleNetwork: causal / nonlinear / freq-axis-kernel variants have no sm_90a kernel yet")
         self.use_causal_conv = use_causal_conv
         self.upsample_scales = list(upsample_scales)
         self.up_layers = torch.nn.ModuleList()
@@ -425,7 +425,7 @@ class ConvInUpsampleNetwork(torch.nn.Module):
                  use_causal_conv=False):
         super().__init__()
         if use_causal_conv:
-            raise PwgbError("ConvInUpsampleNetwork(use_causal_conv=True) has no sm_100a kernel yet")
+            raise PwgbError("ConvInUpsampleNetwork(use_causal_conv=True) has no sm_90a kernel yet")
         self.aux_context_window = aux_context_window
         self.use_causal_conv = False
         kernel_size = 2 * aux_context_window + 1
@@ -449,7 +449,7 @@ class TADELayer(torch.nn.Module):
     def __init__(self, in_channels=64, aux_channels=80, kernel_size=9, bias=True, upsample_factor=2, upsample_mode="nearest"):
         super().__init__()
         if upsample_mode != "nearest":
-            raise PwgbError(f"TADELayer: upsample_mode={upsample_mode!r} has no sm_100a kernel (nearest only)")
+            raise PwgbError(f"TADELayer: upsample_mode={upsample_mode!r} has no sm_90a kernel (nearest only)")
         self.norm = torch.nn.InstanceNorm1d(in_channels)  # parameter-free container (eps read from it)
         self.aux_conv = torch.nn.Sequential(
             torch.nn.Conv1d(aux_channels, in_channels, kernel_size, 1, bias=bias, padding=(kernel_size - 1) // 2))

@@ -1,6 +1,6 @@
 """Host-side mirror of ``parallel_wavegan.losses`` (class names, ctor kwargs, return values).
 
-Forward values are produced by fused sm_100a kernels (``libpwgb.so``): the STFT losses
+Forward values are produced by fused sm_90a kernels (``libpwgb.so``): the STFT losses
 never materialise framed / complex / magnitude tensors, the GAN losses are deterministic
 two-stage reductions.  Every loss returns 0-dim CUDA tensors like the reference.
 Backward: the overlap-add of the STFT adjoint (``pwgb_stft_amplitude_backward``) scatters frames with fp32
@@ -149,7 +149,7 @@ class MelSpectrogram(torch.nn.Module):
                  fmax=7600, center=True, normalized=False, onesided=True, eps=1e-10, log_base=10.0):
         super().__init__()
         if not center or normalized or not onesided:
-            raise PwgbError("MelSpectrogram: only center=True, normalized=False, onesided=True has an sm_100a kernel")
+            raise PwgbError("MelSpectrogram: only center=True, normalized=False, onesided=True has an sm_90a kernel")
         self.fft_size = fft_size
         self.win_length = fft_size if win_length is None else win_length
         self.hop_size = hop_size

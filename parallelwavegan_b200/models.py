@@ -431,7 +431,7 @@ class ParallelWaveGANGenerator(_GeneratorBase):
         from . import layers as L
 
         if use_causal_conv:
-            raise PwgbError("ParallelWaveGANGenerator(use_causal_conv=True) has no sm_100a kernel yet")
+            raise PwgbError("ParallelWaveGANGenerator(use_causal_conv=True) has no sm_90a kernel yet")
         self.in_channels = in_channels
         self.out_channels = out_channels
         self.aux_channels = aux_channels
@@ -855,7 +855,7 @@ class HiFiGANMultiScaleDiscriminator(torch.nn.Module):
                  }, follow_official_norm=False):
         super().__init__()
         if downsample_pooling != "AvgPool1d":
-            raise PwgbError(f"downsample_pooling={downsample_pooling!r} has no sm_100a kernel (AvgPool1d only)")
+            raise PwgbError(f"downsample_pooling={downsample_pooling!r} has no sm_90a kernel (AvgPool1d only)")
         self.discriminators = torch.nn.ModuleList()
         for i in range(scales):
             params = copy.deepcopy(discriminator_params)
@@ -987,7 +987,7 @@ class MelGANMultiScaleDiscriminator(torch.nn.Module, _NormMixin):
                  use_weight_norm=True):
         super().__init__()
         if downsample_pooling != "AvgPool1d":
-            raise PwgbError(f"downsample_pooling={downsample_pooling!r} has no sm_100a kernel (AvgPool1d only)")
+            raise PwgbError(f"downsample_pooling={downsample_pooling!r} has no sm_90a kernel (AvgPool1d only)")
         self.discriminators = torch.nn.ModuleList()
         for _ in range(scales):
             self.discriminators += [

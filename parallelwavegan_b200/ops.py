@@ -35,13 +35,13 @@ class _Prof:
             PROFILE.append((self.name, self.flops, self.bytes, self.e0, e1, self.desc))
 
 
-# Engine selection: "auto" = tcgen05 path whenever pwgb_conv1d_tc_supported() says so, else the
+# Engine selection: "auto" = tensor-core path whenever pwgb_conv1d_tc_supported() says so, else the
 # FFMA kernel; "simt" forces the FFMA kernel (used by tests to cross-check the two paths).
 ENGINE = os.environ.get("PWGB_ENGINE", "auto")
 
 
 def packed_weight(w, groups=1):
-    """bf16 hi/lo operand image of a conv weight for the tcgen05 path, cached on the tensor
+    """bf16 hi/lo operand image of a conv weight for the tensor-core path, cached on the tensor
     object and invalidated by its version counter (in-place updates) -- a temporary such as a
     weight-norm product is simply re-packed every forward."""
     cache = getattr(w, "_pwgb_packed", None)
@@ -131,7 +131,7 @@ def conv1d_raw(
     if P > 1 and stride == 1 and L % P == 0 and out is None and residual is None:
         # a (k,1) Conv2d with stride 1 over the (rows, P) view IS a 1-D conv over the flat axis with
         # dilation P and zero padding pad*P (rows outside [0, R) are flat indices outside [0, R*P)):
-        # this puts the wide 1024-channel period layers on the tcgen05 path
+        # this puts the wide 1024-channel period layers on the tensor-core path
         y = conv1d_raw(x.reshape(B, cin_x, L), w, bias, stride=1, padding=(pl * P, pr * P), dilation=dilation * P, groups=groups,
                        pad_mode=pad_mode, pre_slope=pre_slope, pre_gate=pre_gate, post_act=post_act, post_slope=post_slope,
                        out_scale=out_scale)
@@ -223,7 +223,7 @@ def upsample_fir(x, fir, scale, out=None, out_channels=None):
     nearest repeat x`scale` + (2*scale+1)-tap FIR, zero padded -- pwgb_upsample_fir_forward.
     x: (B, C, T) -> (B, C, T*scale); with ``out_channels`` > C the result is written into the
     first C channels of a zero-initialised (B, out_channels, T*scale) tensor (channel padding
-    for the tcgen05 conditioning contraction)."""
+    for the tensor-core conditioning contraction)."""
     x = _dev(x, "x")
     fir = _dev(fir, "fir").reshape(-1)
     B, Cc, T = x.shape
@@ -277,7 +277,7 @@ def invalidate_caches(module):
 def wavenet_layer(x, c, w_conv, b_conv, w_aux, w_skip, b_skip, w_out, b_out, dilation, skips, aux_real, cache=None, key=None):
     """WaveNetResidualBlock.forward (layers/residual_block.py:102-140), in place on ``skips``:
     returns x_out.  ``c``: (B, aux_pad, T) conditioning, zero-padded to a multiple of 32 channels
-    (or None).  Uses the fused tcgen05 layer when pwgb_wavenet_supported(), otherwise composes the
+    (or None).  Uses the fused tensor-core layer when pwgb_wavenet_supported(), otherwise composes the
     layer from the generic fused conv (gate pre-op, accumulate, residual epilogue)."""
     x = _dev(x, "x")
     B, R, T = x.shape
@@ -333,7 +333,7 @@ class WnStack:
                                      kernel=K, halo=(K - 1) // 2 * int(max_dilation))
         L = capi.lib()
         if not L.pwgb_wnstack_supported(C.byref(self.desc)):
-            raise PwgbError("wnstack: configuration not supported by the fused tcgen05 layer")
+            raise PwgbError("wnstack: configuration not supported by the fused tensor-core layer")
         nx = L.pwgb_wnstack_x_bytes(C.byref(self.desc))
         nc = L.pwgb_wnstack_c_bytes(C.byref(self.desc))
         self.x = [torch.zeros(nx // 4, device=device, dtype=torch.int32) for _ in range(2)]  # zero halos: written once
@@ -787,7 +787,7 @@ def _conv1d_s2d(x, w, bias, kw):
 def _conv1d_padcin(x, w, bias, kw):
     """Input convs on mel features (80 -> 512 k7 of HiFi-GAN, 80 -> 384 of MelGAN): 80 input channels are not a
     multiple of the tensor cores' 32-channel chunk, so the features and the weight are zero-padded to 96 channels (a
-    copy of the small (B, 80, frames) tensor) and the conv runs on the tcgen05 path instead of the FFMA kernel
+    copy of the small (B, 80, frames) tensor) and the conv runs on the tensor-core path instead of the FFMA kernel
     (0.06 vs 0.26 ms at the C2 batch).  Zero channels contribute exact zeros; reflect / replicate padding, activations
     and gradients are unaffected (the pad is torch indexing, differentiable by autograd)."""
     cout, cin_g = w.shape[0], w.shape[1]

@@ -126,7 +126,7 @@ class FusedAdam(_FusedBase):
 
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, amsgrad=False):
         if amsgrad:
-            raise PwgbError("FusedAdam: amsgrad has no sm_100a kernel")
+            raise PwgbError("FusedAdam: amsgrad has no sm_90a kernel")
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, amsgrad=False))
 
     def _init_state(self, p):

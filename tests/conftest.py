@@ -9,8 +9,8 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
-    config.addinivalue_line("markers", "gpu_unverified: CUDA test of a component that has not had its first run on a B200 yet; "
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu)")
+    config.addinivalue_line("markers", "gpu_unverified: CUDA test of a component that has not had its first run on the GPU yet; "
                                        "NOT part of `-m gpu` (skips itself without CUDA) -- promote to `gpu` after the first green run (none parked at the moment)")
 
 

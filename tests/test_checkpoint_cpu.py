@@ -1,7 +1,7 @@
 """Checkpoint boundary (CPU, no kernels): ``utils.load_model`` (utils/utils.py:294-360) and the
-``Trainer.save_checkpoint`` dict layout (bin/train.py:112-186) round-trip through the mirror modules; when the
-reference tree is present (build container) checkpoints written by the REAL reference load into the mirror and
-checkpoints written by the mirror load strictly into the reference modules."""
+``Trainer.save_checkpoint`` dict layout (bin/train.py:112-186) round-trip through the mirror modules; a checkpoint
+written by the REAL reference (stored golden) loads into the mirror, and checkpoints written by the mirror have the
+reference modules' exact state-dict layout."""
 import os
 import sys
 
@@ -91,44 +91,46 @@ def test_load_model_from_checkpoint_dir(tmp_path):
     assert isinstance(mh, models.HiFiGANGenerator)
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/parallel_wavegan"), reason="reference tree only exists in the build container")
-def test_checkpoints_interchange_with_the_real_reference(tmp_path):
-    from oracle.make_golden import import_reference
-
-    import_reference()
-    import parallel_wavegan.models as rm
-    from parallel_wavegan.optimizers import RAdam as RefRAdam
+def test_checkpoints_interchange_with_the_real_reference(tmp_path, golden_dir):
+    """tests/golden/checkpoint_ref.npz (oracle/make_golden_checkpoint.py): a checkpoint the real reference wrote after one
+    RAdam step, and the reference modules' state-dict layout."""
+    import json
 
     from parallelwavegan_b200 import models, optimizers, utils
 
+    z = np.load(os.path.join(golden_dir, "checkpoint_ref.npz"))
+    meta = json.loads(str(z["meta"]))
+    gp = meta["generator_params"]
+    g_sd = {k: torch.from_numpy(z[f"g/{k}"]) for k, _ in meta["g_spec"]}
+    d_sd = synth.synth_state_dict([(k, tuple(s)) for k, s in meta["d_spec"]], 12, 1.0)
+    groups = meta["param_groups"]
+    state = {i: {"step": torch.tensor(float(z[f"step/{i}"])), "exp_avg": torch.from_numpy(z[f"exp_avg/{i}"]),
+                 "exp_avg_sq": torch.from_numpy(z[f"exp_avg_sq/{i}"])} for i in groups[0]["params"]}
+    d_tmp = models.HiFiGANMultiScaleMultiPeriodDiscriminator()
+    d_tmp.load_state_dict(d_sd)
     # reference -> mirror
-    rg, rd = rm.HiFiGANGenerator(**HIFI_SMALL), rm.HiFiGANMultiScaleMultiPeriodDiscriminator()
-    _fill(rg, 11)
-    _fill(rd, 12)
-    ro = RefRAdam(rg.parameters(), lr=1e-3)
-    for p in rg.parameters():
-        p.grad = torch.randn_like(p) * 0.01
-    ro.step()
     path = str(tmp_path / "ref.pkl")
-    torch.save({"model": {"generator": rg.state_dict(), "discriminator": rd.state_dict()},
-                "optimizer": {"generator": ro.state_dict(), "discriminator": torch.optim.Adam(rd.parameters()).state_dict()},
+    torch.save({"model": {"generator": g_sd, "discriminator": d_sd},
+                "optimizer": {"generator": {"state": state, "param_groups": groups},
+                              "discriminator": torch.optim.Adam(d_tmp.parameters()).state_dict()},
                 "scheduler": {"generator": {}, "discriminator": {}}, "steps": 1, "epochs": 0}, path)
-    m = utils.load_model(path, config={"generator_type": "HiFiGANGenerator", "generator_params": HIFI_SMALL, "format": "npy"})
-    for (k, a), (k2, b) in zip(rg.state_dict().items(), m.state_dict().items()):
-        assert k == k2 and torch.equal(a, b)
-    g2, d2 = models.HiFiGANGenerator(**HIFI_SMALL), models.HiFiGANMultiScaleMultiPeriodDiscriminator()
+    m = utils.load_model(path, config={"generator_type": "HiFiGANGenerator", "generator_params": gp, "format": "npy"})
+    assert list(m.state_dict()) == list(g_sd)
+    for k, v in m.state_dict().items():
+        assert torch.equal(v, g_sd[k])
+    g2, d2 = models.HiFiGANGenerator(**gp), models.HiFiGANMultiScaleMultiPeriodDiscriminator()
     o2 = optimizers.RAdam(g2.parameters(), lr=1.0)
     utils.load_checkpoint(path, {"generator": g2, "discriminator": d2}, {"generator": o2, "discriminator": optimizers.FusedAdam(d2.parameters())})
-    p_ref, p_new = next(iter(rg.parameters())), next(iter(g2.parameters()))
-    assert torch.equal(ro.state[p_ref]["exp_avg"], o2.state[p_new]["exp_avg"]) and o2.state[p_new]["step"] == 1
+    p_new = next(iter(g2.parameters()))
+    assert torch.equal(state[groups[0]["params"][0]]["exp_avg"], o2.state[p_new]["exp_avg"]) and o2.state[p_new]["step"] == 1
     assert o2.param_groups[0]["lr"] == 1e-3
-    # mirror -> reference (strict)
+    # mirror -> reference (strict): the written state dicts have exactly the reference modules' keys and shapes, and the
+    # optimizer state has the reference optimizer's parameter-group structure
     utils.save_checkpoint(str(tmp_path / "ours.pkl"), {"generator": g2, "discriminator": d2},
                           {"generator": o2, "discriminator": optimizers.FusedAdam(d2.parameters())})
     ck = torch.load(str(tmp_path / "ours.pkl"), map_location="cpu")
-    rg2, rd2 = rm.HiFiGANGenerator(**HIFI_SMALL), rm.HiFiGANMultiScaleMultiPeriodDiscriminator()
-    rg2.load_state_dict(ck["model"]["generator"], strict=True)
-    rd2.load_state_dict(ck["model"]["discriminator"], strict=True)
-    ro2 = RefRAdam(rg2.parameters(), lr=5.0)
-    ro2.load_state_dict(ck["optimizer"]["generator"])
-    assert ro2.param_groups[0]["lr"] == 1e-3
+    assert [[k, list(v.shape)] for k, v in ck["model"]["generator"].items()] == meta["g_spec"]
+    assert [[k, list(v.shape)] for k, v in ck["model"]["discriminator"].items()] == meta["d_spec"]
+    og = ck["optimizer"]["generator"]
+    assert len(og["param_groups"]) == len(groups) and len(og["param_groups"][0]["params"]) == len(groups[0]["params"])
+    assert og["param_groups"][0]["lr"] == 1e-3

@@ -32,13 +32,13 @@ def dev():
         (16, 16, 41, 4, 1, 4, 20, 515, 2, 1.0, "lrelu"),
         (16, 32, 41, 2, 1, 16, 20, 300, 2, 1.0, "lrelu"),
         (32, 1, 3, 1, 1, 1, 1, 64, 2, 1.0, None),
-        (64, 128, 7, 1, 3, 1, 9, 300, 2, 0.1, None),       # tcgen05 wgrad (cout % 128 == 0)
+        (64, 128, 7, 1, 3, 1, 9, 300, 2, 0.1, None),       # tensor-core wgrad (cout % 128 == 0)
         (128, 256, 11, 1, 5, 1, 25, 517, 3, 0.1, None),    # two tap groups, several splits
-        (1024, 1024, 5, 1, 1, 1, 2, 40, 2, 1.0, "lrelu"),  # discriminator tail: column chunks + tcgen05 wgrad
-        (128, 128, 41, 1, 1, 4, 20, 200, 2, 1.0, "lrelu"), # grouped stride-1 conv on the tcgen05 path
-        (64, 64, 3, 1, 2, 1, 2, 1000, 2, 0.2, None),       # tcgen05 wgrad with a half-filled 128-row M tile
+        (1024, 1024, 5, 1, 1, 1, 2, 40, 2, 1.0, "lrelu"),  # discriminator tail: column chunks + tensor-core wgrad
+        (128, 128, 41, 1, 1, 4, 20, 200, 2, 1.0, "lrelu"), # grouped stride-1 conv on the tensor-core path
+        (64, 64, 3, 1, 2, 1, 2, 1000, 2, 0.2, None),       # tensor-core wgrad with a half-filled 128-row M tile
         (32, 160, 1, 1, 1, 1, 0, 300, 2, 1.0, None),       # cout = 128 + 32
-        (64, 128, 3, 1, 512, 1, 512, 1500, 1, 1.0, None),  # WaveNet-size dilation: one tap per CTA in the tcgen05 wgrad
+        (64, 128, 3, 1, 512, 1, 512, 1500, 1, 1.0, None),  # WaveNet-size dilation: one tap per CTA in the tensor-core wgrad
     ],
 )
 def test_conv1d_gradients(dev, cin, cout, k, stride, dil, groups, pad, T, B, pre, post):
@@ -108,7 +108,7 @@ def test_period_conv_gradients(dev, period):
 
 
 def test_period_stride1_wide_gradients(dev):
-    """MPD tail layer (1024 -> 1024, (5,1), stride 1) as a dilated 1-D conv on the tcgen05 paths."""
+    """MPD tail layer (1024 -> 1024, (5,1), stride 1) as a dilated 1-D conv on the tensor-core paths."""
     from parallelwavegan_b200 import ops
 
     B, R, P = 2, 9, 3

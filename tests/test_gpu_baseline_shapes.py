@@ -1,5 +1,5 @@
 """GPU parity at the BASELINE.json shapes (C2 / C3 / C4 / C5) and at tile counts that make every
-persistent CTA of the tcgen05 kernels loop many times (running ring counters, accumulator-set and
+persistent CTA of the tensor-core kernels loop many times (running ring counters, accumulator-set and
 mbarrier-parity wraps).  The GPU computes the full batch; the CPU oracle re-computes a few batch
 items (the ops are batch-independent), so the whole file costs seconds of host time.
 Tolerance: rel-L2 <= 1e-3 and max-abs <= 1e-3 of peak (north_star), far tighter where noted."""

@@ -237,7 +237,7 @@ TC_TOL = 1e-4  # bf16x3 split: ~2^-16 per product, fp32 accumulation
     ],
 )
 def test_conv1d_tcgen05_path(dev, cin, cout, k, dil, T, B, mode):
-    """tcgen05 bf16x3 path vs the oracle (ATen fp32 on CPU) and vs the FFMA kernel."""
+    """tensor-core bf16x3 path vs the oracle (ATen fp32 on CPU) and vs the FFMA kernel."""
     import ctypes as C
 
     from parallelwavegan_b200 import capi, ops
@@ -301,7 +301,7 @@ def test_pwg_generator_vs_reference(dev, name):
 @pytest.mark.parametrize("engine", ["auto", "simt"])
 def test_wavenet_layer(dev, dilation, T, B, engine):
     """One WaveNetResidualBlock (PWG v1 sizes) vs the oracle, both engines; dilation 128/512
-    exercise the per-tap window mode of the tcgen05 kernel."""
+    exercise the per-tap window mode of the tensor-core kernel."""
     from parallelwavegan_b200 import layers, ops
 
     blk = layers.WaveNetResidualBlock(dilation=dilation)
@@ -341,7 +341,7 @@ def test_wavenet_fused_layer_packed(dev, dilation, T, B, skips_init, write_x):
     """The ONE-kernel fused layer on the packed (bf16 hi/lo operand layout) residual stream vs the oracle:
     pack -> pwgb_wnstack_layer_forward -> unpack.  Covers ragged tails (T % 128 != 0), every tap window
     reaching into the zero halo, skip initialisation and the last-layer form (no residual output);
-    the last case gives every CTA several tiles (all 4 TMEM accumulator sets and both ring phases wrap)."""
+    the last case gives every CTA several tiles (both ring phases wrap)."""
     from parallelwavegan_b200 import layers, ops
 
     blk = layers.WaveNetResidualBlock(dilation=dilation)

@@ -1,4 +1,4 @@
-"""Strided discriminator convs on the tensor-core path (space-to-depth + stride-1 tcgen05 conv):
+"""Strided discriminator convs on the tensor-core path (space-to-depth + stride-1 tensor-core conv):
 forward, data gradient and weight gradient vs torch autograd on the CPU (fp32 oracle of the same op),
 at the HiFi-GAN MSD / MPD layer shapes (hifigan.py:354-381, 586-601) and the C5 batch."""
 import pytest
@@ -74,7 +74,7 @@ def test_strided_conv_s2d_forward_backward(dev, cin, cout, K, stride, groups, pa
 
 @pytest.mark.parametrize("P,rows,B", [(1, 128, 16), (3, 37, 4)])
 def test_logit_conv_on_tensor_cores(dev, P, rows, B):
-    """1024 -> 1 logit convs (MSD k3, MPD (3,1)): zero-padded to 16 output channels for the tcgen05 path; forward and
+    """1024 -> 1 logit convs (MSD k3, MPD (3,1)): zero-padded to 16 output channels for the tensor-core path; forward and
     gradients vs torch autograd."""
     from parallelwavegan_b200 import ops
 
@@ -153,7 +153,7 @@ def test_grouped_strided_conv_padded_groups_inference(dev):
 
 @pytest.mark.parametrize("mode", ["zero", "reflect"])
 def test_mel_input_conv_padded_channels(dev, mode):
-    """80 -> 512 k7 input conv (hifigan.py:80-91 / melgan.py:70-72): channels zero-padded to 96 for the tcgen05 path;
+    """80 -> 512 k7 input conv (hifigan.py:80-91 / melgan.py:70-72): channels zero-padded to 96 for the tensor-core path;
     forward and gradients vs torch autograd."""
     from parallelwavegan_b200 import ops
 

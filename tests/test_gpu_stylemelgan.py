@@ -4,8 +4,8 @@ the travelling oracle.
 Tolerances.  The bar is 1e-3 relative L2.  The 9-block instance-normalised, softmax-gated stack is ill-conditioned
 with the synthetic weights: on the CPU, in pure fp32, a 1e-6 relative perturbation of the conditioning moves the
 reference output by 9e-5 rel-L2 and 1.9e-3 of peak at the worst sample, and the oracle differs from the reference
-by 2.4e-5 / 5.3e-4 just through the order of fp32 sums.  Emulating the bf16x3 operand split of the tcgen05 convs on
-the CPU gives 2.5e-4 / 3.5e-3; the B200 measured 4.5e-4 / 9.1e-3 (profiles/gpu_tests_r1_stylemelgan_first_run.log).
+by 2.4e-5 / 5.3e-4 just through the order of fp32 sums.  Emulating the bf16x3 operand split of the tensor-core convs on
+the CPU gives 2.5e-4 / 3.5e-3.
 So the full-depth model is held to the 1e-3 rel-L2 bar and to 2e-2 of peak pointwise; single blocks and the small
 model are held to 1e-3 on both."""
 import json
@@ -151,7 +151,7 @@ def test_tade_glue_gradients(dev, scale):
 
 def test_style_melgan_generator_gradients(dev):
     """StyleMelGAN generator training (row a11b): parameter and input gradients of the small golden model through the TADE
-    adjoints, the tcgen05 conv data / weight gradients and the transposed-conv noise path vs torch autograd through the
+    adjoints, the tensor-core conv data / weight gradients and the transposed-conv noise path vs torch autograd through the
     CPU oracle, with the conditioning-aware bound (instance norm + softmax gates amplify fp32 rounding, see the header)."""
     from helpers import conditioning_tolerances
     from parallelwavegan_b200 import models

@@ -1,4 +1,4 @@
-import sys; sys.path.insert(0,'/root/repo/tests'); sys.path.insert(0,'/root/repo')
+import os, sys; _R = os.path.join(os.path.dirname(os.path.abspath(__file__)), '..', '..'); sys.path.insert(0, os.path.join(_R, 'tests')); sys.path.insert(0, _R)
 import torch, torch.nn.functional as F
 from helpers import rel_l2
 from oracle import ref_ops, synth

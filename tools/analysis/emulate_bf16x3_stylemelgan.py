@@ -1,4 +1,4 @@
-import sys; sys.path.insert(0,'/root/repo/tests'); sys.path.insert(0,'/root/repo')
+import os, sys; _R = os.path.join(os.path.dirname(os.path.abspath(__file__)), '..', '..'); sys.path.insert(0, os.path.join(_R, 'tests')); sys.path.insert(0, _R)
 import torch, torch.nn.functional as F
 from helpers import golden_effective_weights, load_golden, rel_l2, max_abs_over_peak
 from oracle import ref_ops, synth
@@ -15,7 +15,7 @@ def split(t):
 orig_conv=F.conv1d
 def conv3(x, wt, b=None, **k):
     cin=wt.shape[1]; cout=wt.shape[0]
-    if cin % 32 == 0 and cout % 16 == 0:   # tcgen05 path condition
+    if cin % 32 == 0 and cout % 16 == 0:   # tensor-core path condition
         xh,xl=split(x); wh,wl=split(wt)
         y=orig_conv(xh,wh,None,**k)+orig_conv(xl,wh,None,**k)+orig_conv(xh,wl,None,**k)
         return y if b is None else y+b[None,:,None]

@@ -1,4 +1,4 @@
-"""Bring-up probe for the tcgen05 conv path: prints error statistics for several shapes and
+"""Bring-up probe for the tensor-core conv path: prints error statistics for several shapes and
 descriptor variants, never asserts (diagnostics for a box without interactive access)."""
 import ctypes as C
 import os
