@@ -21,6 +21,8 @@
 //               and stores.
 //   warp 16     B producer: cp.async.bulk (TMA, 1-D) of one packed weight stage per (chunk, tap).
 //   warp 17     raw activation loader: cp.async.bulk row copies into the raw fp32 ring.
+#include <type_traits>
+
 #include "tc_common.cuh"
 
 namespace pwgb {
@@ -102,12 +104,16 @@ void tc_pack_rows(const float* w, void* packed, int cin_real, int cin_pad, int r
   tc_pack_weight_kernel<<<blocks, 128, 0, st>>>(w, (uint4*)packed, cin_real, cin_pad, rows, K, co_begin, cout_total, 0);
 }
 
-// Epilogue of one accumulator element (row t, column col of the launch's column chunk starting at co_base).
+// Epilogue of one accumulator element (row t, column col of the launch's column chunk starting at co_base).  The mode
+// (EPI_SHUFFLE: p.shuffle > 1, EPI_WAVENET: p.wavenet, else EPI_PLAIN) is a template argument so the consumers branch on
+// it once per 64-row block, not per element.
+enum { EPI_PLAIN, EPI_SHUFFLE, EPI_WAVENET };
+template <int MODE>
 __device__ __forceinline__ void epi_store(const TcK& p, float a, int b, int t, int col, int co_base, const float* __restrict__ bias,
                                           const float* bias_s, const float* __restrict__ res, float* __restrict__ y,
                                           float* __restrict__ y2) {
   const long long st = p.T_out;
-  if (p.shuffle > 1) {
+  if constexpr (MODE == EPI_SHUFFLE) {
     const int co = co_base + col, cof = co / p.shuffle;
     float v = a + (bias ? __ldg(bias + cof) : 0.f);
     if (p.post_act == PWGB_ACT_TANH)
@@ -116,7 +122,7 @@ __device__ __forceinline__ void epi_store(const TcK& p, float a, int b, int t, i
       v = lrelu(v, p.post_slope);
     const int of = t * p.shuffle + (co - cof * p.shuffle) - p.shuffle_pad;
     if (of >= 0 && of < p.shuffle_tout) y[(long long)b * p.ybs + (long long)cof * p.shuffle_tout + of] = v * p.out_scale;
-  } else if (p.wavenet) {
+  } else if constexpr (MODE == EPI_WAVENET) {
     // WaveNet split epilogue (residual_block.py:131-138): columns [0, split) are the skip 1x1
     // (accumulated into y2), columns [split, Cout) the residual 1x1: y = (v + x) * sqrt(0.5)
     const bool is_skip = col < p.split;
@@ -210,6 +216,9 @@ __device__ __forceinline__ void fill_main_chunk(const TcK& p, const float* __res
   }
 }
 
+// MT (64-row blocks per warpgroup) and NB16 (16-column blocks, Cout = 16 * NB16) are compile-time constants, so the
+// consumers issue a fixed wgmma sequence into fixed accumulator registers (tc_launch picks the instantiation).
+template <int MT, int NB16>
 __global__ void __launch_bounds__(TC_THREADS, 1)
     conv1d_tc_kernel(const TcK p, const float* __restrict__ x, const float* __restrict__ x2,
                      const uint4* __restrict__ wpk, const float* __restrict__ bias, const float* __restrict__ res,
@@ -228,7 +237,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   const int tid = threadIdx.x;
   const int warp = tid >> 5;
   const int lane = tid & 31;
-  const int TT = p.MT * 128;
+  constexpr int TT = MT * 128;
   const int nc_total = p.nchunks + p.nchunks2;
   const int pct = p.B * p.tiles_per_seq;  // work items per column chunk (nco chunks share one launch)
 
@@ -431,23 +440,26 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     }
   } else if (warp < W_TMA) {
     // ===================== consumers: wgmma into registers, then the epilogue =====================
-    // warpgroup wg owns the 64-row blocks wg * MT + mb of the tile; per (chunk, tap) and 16-channel K-step the three
-    // bf16x3 products of every block, one wait per weight stage before the stage is handed back
+    // warpgroup wg owns the 64-row blocks wg * MT + mb of the tile.  One wgmma group per (chunk, tap): the three bf16x3
+    // products of every block and 16-channel K-step.  A group stays in flight while the next one is issued; the wait that
+    // retires it hands its weight stage (and, after a chunk's last tap, its A buffer) back to the producers.  The order
+    // of the MMAs into each accumulator is the issue order, so the overlap does not change the result.
     const int wg = (warp - W_CONS0) >> 2, wq = warp & 3;
-    const int nb16 = p.Cout / 16;
-    const unsigned lbo_a = (unsigned)p.R * 16u, lbo_b = (unsigned)p.Cout * 16u;
-    const unsigned a_sub = (unsigned)(KC / 8) * p.R, b_sub = (unsigned)(KC / 8) * p.Cout;  // hi -> lo image (16-byte units)
+    constexpr int NACC = 8 * NB16;  // fp32 accumulators per thread and 64-row block
+    const unsigned lbo_a = (unsigned)p.R * 16u, lbo_b = NB16 * 256u;
+    const unsigned a_sub = (unsigned)(KC / 8) * p.R, b_sub = (KC / 8) * NB16 * 16u;  // hi -> lo image (16-byte units)
     int buf = 0, aph = 0, s = 0, bph = 0;
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      float acc[64];
+      float acc[MT * NACC];
 #pragma unroll
-      for (int e = 0; e < 64; ++e) acc[e] = 0.f;
+      for (int e = 0; e < MT * NACC; ++e) acc[e] = 0.f;
+      int held_s = -1, held_a = -1;  // weight stage / A buffer read by the group in flight
       for (int c = 0; c < nc_total; ++c) {
-        mbar_wait_spin(A_FULL(buf), aph);
+        mbar_wait_trap(A_FULL(buf), aph);
         const unsigned a_addr = smem_u32(a_buf + (size_t)buf * p.a_bytes);
         const int ntaps = c < p.nchunks ? p.K : 1;
         for (int k = 0; k < ntaps; ++k) {
-          mbar_wait_spin(B_FULL(s), bph);
+          mbar_wait_trap(B_FULL(s), bph);
           __syncwarp();
           const unsigned b_addr = smem_u32(b_buf + (size_t)s * p.b_bytes);
           const int tap_row = c < p.nchunks ? (p.win_mode ? k * TT : k * p.D) : 0;
@@ -456,41 +468,56 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
           for (int ks = 0; ks < KC / 16; ++ks) {
             const unsigned long long bh = gmma_desc(b_addr + (unsigned)(2 * ks) * lbo_b, lbo_b, 128);
             const unsigned long long ah0 =
-                gmma_desc(a_addr + ((unsigned)(2 * ks) * p.R + (unsigned)(tap_row + wg * p.MT * 64)) * 16u, lbo_a, 128);
-            if (p.MT == 1) {
-              wgmma_cols<0, 0, 8>(acc, ah0, bh, nb16, 16);
-              wgmma_cols<0, 0, 8>(acc, ah0 + a_sub, bh, nb16, 16);
-              wgmma_cols<0, 0, 8>(acc, ah0, bh + b_sub, nb16, 16);
-            } else {
-              const unsigned long long ah1 = ah0 + 64;  // next 64 rows: 64 x 16 B
-              wgmma_cols<0, 0, 4>(acc, ah0, bh, nb16, 16);
-              wgmma_cols<0, 0, 4>(acc, ah0 + a_sub, bh, nb16, 16);
-              wgmma_cols<0, 0, 4>(acc, ah0, bh + b_sub, nb16, 16);
-              wgmma_cols<0, 0, 4>(acc + 32, ah1, bh, nb16, 16);
-              wgmma_cols<0, 0, 4>(acc + 32, ah1 + a_sub, bh, nb16, 16);
-              wgmma_cols<0, 0, 4>(acc + 32, ah1, bh + b_sub, nb16, 16);
+                gmma_desc(a_addr + ((unsigned)(2 * ks) * p.R + (unsigned)(tap_row + wg * MT * 64)) * 16u, lbo_a, 128);
+#pragma unroll
+            for (int mb = 0; mb < MT; ++mb) {
+              const unsigned long long ah = ah0 + 64 * mb;  // next 64 rows: 64 x 16 B
+              wgmma_n<0, 0, NB16>(acc + mb * NACC, ah, bh, 16);
+              wgmma_n<0, 0, NB16>(acc + mb * NACC, ah + a_sub, bh, 16);
+              wgmma_n<0, 0, NB16>(acc + mb * NACC, ah, bh + b_sub, 16);
             }
           }
           wg_commit();
-          wg_wait<0>();
+          wg_wait<1>();  // the previous group has retired: its stage and, at a chunk boundary, its A buffer are free
           __syncwarp();
-          if (lane == 0) mbar_arrive(B_EMPTY(s));  // weight stage reusable
+          if (lane == 0) {
+            if (held_s >= 0) mbar_arrive(B_EMPTY(held_s));
+            if (held_a >= 0) mbar_arrive(A_EMPTY(held_a));
+          }
+          held_s = s;
+          held_a = k == ntaps - 1 ? buf : -1;
           if (++s == p.nb) { s = 0; bph ^= 1; }
         }
-        if (lane == 0) mbar_arrive(A_EMPTY(buf));
         if (++buf == p.na) { buf = 0; aph ^= 1; }
+      }
+      wg_wait<0>();
+      __syncwarp();
+      if (lane == 0) {
+        if (held_s >= 0) mbar_arrive(B_EMPTY(held_s));
+        if (held_a >= 0) mbar_arrive(A_EMPTY(held_a));
       }
       const int tr = p.nco > 1 ? tile % pct : tile;  // tile within its column chunk
       const int b = tr / p.tiles_per_seq;
       const int t0 = (tr - b * p.tiles_per_seq) * TT;
       const int co_base = p.co_off + (p.nco > 1 ? (tile / pct) * p.Cout : 0);
+      // one 64-row block at a time, the mode chosen once per block (branching per element, or once for both blocks,
+      // made ptxas spill at MT = 2)
+      auto store_block = [&](auto mode, const float* ab, int mb) {
 #pragma unroll
-      for (int e = 0; e < 64; ++e) {
-        const int mb = p.MT == 2 ? (e >> 5) : 0;
-        const int i = p.MT == 2 ? (e & 31) : e;
-        const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
-        const int t = t0 + (wg * p.MT + mb) * 64 + wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
-        if (col < p.Cout && t < p.T_out) epi_store(p, acc[e], b, t, col, co_base, bias, bias_s, res, y, y2);
+        for (int i = 0; i < NACC; ++i) {
+          const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+          const int t = t0 + (wg * MT + mb) * 64 + wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+          if (t < p.T_out) epi_store<decltype(mode)::value>(p, ab[i], b, t, col, co_base, bias, bias_s, res, y, y2);
+        }
+      };
+#pragma unroll
+      for (int mb = 0; mb < MT; ++mb) {
+        if (p.shuffle > 1)
+          store_block(std::integral_constant<int, EPI_SHUFFLE>{}, acc + mb * NACC, mb);
+        else if (p.wavenet)
+          store_block(std::integral_constant<int, EPI_WAVENET>{}, acc + mb * NACC, mb);
+        else
+          store_block(std::integral_constant<int, EPI_PLAIN>{}, acc + mb * NACC, mb);
       }
     }
   } else if (warp == W_TMA) {
@@ -501,7 +528,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       const unsigned char* srcc = src + (p.nco > 1 ? (size_t)(tile / pct) * per_tile * p.b_bytes : 0);
       for (int j = 0; j < per_tile; ++j) {
-        mbar_wait_spin(B_EMPTY(s), ph ^ 1);
+        mbar_wait_trap(B_EMPTY(s), ph ^ 1);
         if (elect_one()) {
           mbar_expect_tx(B_FULL(s), (unsigned)p.b_bytes);
           bulk_g2s(smem_u32(b_buf + (size_t)s * p.b_bytes), srcc + (size_t)j * p.b_bytes, (unsigned)p.b_bytes, B_FULL(s));
@@ -663,17 +690,41 @@ static int tc_plan(const pwgb_conv1d_desc* d, TcK& p, size_t& smem_bytes, int au
   return 0;
 }
 
+using TcKernel = void (*)(const TcK, const float*, const float*, const uint4*, const float*, const float*, float*, float*);
+
+// Every tile shape tc_plan produces: MT = 1 at any width of 16 .. TC_NMAX columns, MT = 2 up to TC_NMAX / 2.
+static TcKernel tc_kernel_for(int mt, int cout) {
+  static const TcKernel mt1[8] = {conv1d_tc_kernel<1, 1>, conv1d_tc_kernel<1, 2>, conv1d_tc_kernel<1, 3>,
+                                  conv1d_tc_kernel<1, 4>, conv1d_tc_kernel<1, 5>, conv1d_tc_kernel<1, 6>,
+                                  conv1d_tc_kernel<1, 7>, conv1d_tc_kernel<1, 8>};
+  static const TcKernel mt2[4] = {conv1d_tc_kernel<2, 1>, conv1d_tc_kernel<2, 2>, conv1d_tc_kernel<2, 3>,
+                                  conv1d_tc_kernel<2, 4>};
+  if (cout % 16 != 0) return nullptr;
+  const int nb16 = cout / 16;
+  if (mt == 1 && nb16 >= 1 && nb16 <= 8) return mt1[nb16 - 1];
+  if (mt == 2 && nb16 >= 1 && nb16 <= 4) return mt2[nb16 - 1];
+  return nullptr;
+}
+
 static int tc_launch(TcK& p, size_t bytes, const float* x, const void* packed_w, const float* bias,
                      const float* residual, float* y, cudaStream_t st, const float* x2 = nullptr,
                      float* y2 = nullptr) {
   if (p.B == 0 || p.T_out == 0) return PWGB_OK;
+  const TcKernel kernel = tc_kernel_for(p.MT, p.Cout);
+  if (!kernel) {
+    set_error("conv1d_tc: no kernel instantiation for MT = %d, Cout = %d", p.MT, p.Cout);
+    return PWGB_UNSUPPORTED;
+  }
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv1d_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-    if (e != cudaSuccess) {
-      set_error("conv1d_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-      return PWGB_CUDA_ERROR;
-    }
+    for (int mt = 1; mt <= 2; ++mt)
+      for (int cout = 16; cout <= TC_NMAX / mt; cout += 16) {
+        cudaError_t e = cudaFuncSetAttribute(tc_kernel_for(mt, cout), cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+        if (e != cudaSuccess) {
+          set_error("conv1d_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+          return PWGB_CUDA_ERROR;
+        }
+      }
     attr_set = true;
   }
   static int num_sms = 0;
@@ -690,7 +741,7 @@ static int tc_launch(TcK& p, size_t bytes, const float* x, const void* packed_w,
   if (p.tma_act && ((reinterpret_cast<uintptr_t>(x) & 15) || (x2 && (reinterpret_cast<uintptr_t>(x2) & 15))))
     p.tma_act = 0;  // unaligned base pointer: the producers stage with cp.async instead
   const int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
-  conv1d_tc_kernel<<<(unsigned)grid, TC_THREADS, bytes, st>>>(p, x, x2, (const uint4*)packed_w, bias, residual, y, y2);
+  kernel<<<(unsigned)grid, TC_THREADS, bytes, st>>>(p, x, x2, (const uint4*)packed_w, bias, residual, y, y2);
   return check_launch("conv1d_tc_kernel");
 }
 

@@ -48,6 +48,12 @@ __device__ __forceinline__ void mbar_wait_spin(unsigned bar, unsigned parity) {
     }
   }
 }
+// The same bound without the diagnostic, for kernels that pipeline their wgmma groups: a call (printf) anywhere in the
+// kernel, in any warp role, makes ptxas serialize every wgmma of it (C7510).
+__device__ __forceinline__ void mbar_wait_trap(unsigned bar, unsigned parity) {
+  for (unsigned n = 0; !mbar_try(bar, parity);)
+    if (++n > SPIN_LIMIT) __trap();
+}
 // Long waits of the wide roles: the thread is suspended in hardware until the phase completes (or `hint_ns` passed), so a
 // waiting warp issues almost nothing -- plain try_wait loops were 35-40 % of the executed instructions of the fused
 // WaveNet kernel's gate / epilogue warps.
@@ -70,16 +76,12 @@ __device__ __forceinline__ void mbar_wait_hint(unsigned bar, unsigned parity, un
   }
 }
 // Same with a sleep back-off: waiting warps must not steal issue slots from the working ones
-// (spin loops were 17% of all executed instructions in the first persistent version).
+// (spin loops were 17% of all executed instructions in the first persistent version).  Trap only, like mbar_wait_trap.
 __device__ __forceinline__ void mbar_wait(unsigned bar, unsigned parity) {
   unsigned n = 0;
   while (!mbar_try(bar, parity)) {
     if (n > 4) __nanosleep(n > 64 ? 200 : 40);
-    if (++n > SPIN_LIMIT) {
-      printf("pwgb conv1d_tc: mbarrier timeout (block %d thread %d bar %u parity %u)\n", blockIdx.x, threadIdx.x, bar,
-             parity);
-      __trap();
-    }
+    if (++n > SPIN_LIMIT) __trap();
   }
 }
 __device__ __forceinline__ void bulk_g2s(unsigned dst, const void* src, unsigned bytes, unsigned bar) {

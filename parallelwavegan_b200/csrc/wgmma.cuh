@@ -72,6 +72,22 @@ struct Wgmma<128, TA, TB> {
   }
 };
 
+// N = 16 * NB16 (compile time, 1 <= NB16 <= 8) as one instruction of 128 columns or at most three of 64 / 32 / 16 columns,
+// each into a fixed slice of d.  With the width fixed at compile time ptxas can keep consecutive commit groups in flight;
+// the run-time selection below makes it serialize every wgmma.  b_col16: as below.
+template <int TA, int TB, int NB16>
+__device__ __forceinline__ void wgmma_n(float* d, unsigned long long a, unsigned long long b, unsigned b_col16) {
+  static_assert(NB16 >= 1 && NB16 <= 8, "NB16");
+  if constexpr (NB16 == 8) {
+    Wgmma<128, TA, TB>::run(d, a, b);
+  } else {
+    constexpr int c32 = NB16 & 4, c16 = NB16 & 6;  // first 16-column block of the 32- and of the 16-column instruction
+    if constexpr ((NB16 & 4) != 0) Wgmma<64, TA, TB>::run(d, a, b);
+    if constexpr ((NB16 & 2) != 0) Wgmma<32, TA, TB>::run(d + 8 * c32, a, b + (unsigned long long)c32 * b_col16);
+    if constexpr ((NB16 & 1) != 0) Wgmma<16, TA, TB>::run(d + 8 * c16, a, b + (unsigned long long)c16 * b_col16);
+  }
+}
+
 // N = 16 * nb16 (1 <= nb16 <= NBMAX, run time; NBMAX = 4 or 8) as at most three instructions of 64 / 32 / 16 columns
 // (or one of 128); d holds the fragment of the whole width.  b_col16: descriptor distance (16-byte units) of the B
 // operand's next 16 columns.
