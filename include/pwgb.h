@@ -117,8 +117,9 @@ PWGB_API int pwgb_conv_transpose1d_forward(const pwgb_convtr1d_desc* d, const fl
  * memory; cout/groups > 128 and groups > 1 run as several column chunks of one launch); everything else stays on
  * pwgb_conv1d_forward.
  * ---------------------------------------------------------------------- */
-/* measurement aids (not part of the product contract): set key 1 = conv variant (bit 1: stage activations with
- * cp.async instead of TMA); get returns -1 (no read-back available). */
+/* measurement aids (not part of the product contract): set key 1 = conv variant (value 2: stage activations with
+ * cp.async instead of TMA; value 4: register epilogue instead of the staged one); get key 1 copies the plan of the last
+ * tensor-core conv launch, 5 ints {MT, na, nb, ns, staged}, and returns 0 (-1 for any other key or a short buffer). */
 PWGB_API void pwgb_debug_set(int key, int value);
 PWGB_API int pwgb_debug_get(int key, void* dst, size_t bytes);
 PWGB_API size_t pwgb_conv1d_tc_packed_weight_bytes(int cin, int cout, int kernel);

@@ -18,9 +18,11 @@
 //               into the K-major operand image, 16 B st.shared.
 //   warps 8-15  consumers, two warpgroups: warpgroup g issues the wgmma of its 64 (MT = 2: 128) rows of the tile into
 //               registers (<= 128 columns: 64 fp32 per thread), then runs bias / act / residual / scale / accumulate
-//               and stores.
+//               and stores.  A plain conv with a residual or an accumulate does that in a shared-memory tile: its
+//               residual rows arrive by bulk copy while the MMAs run, its rows leave by bulk store (or bulk fp32 add).
 //   warp 16     B producer: cp.async.bulk (TMA, 1-D) of one packed weight stage per (chunk, tap).
 //   warp 17     raw activation loader: cp.async.bulk row copies into the raw fp32 ring.
+#include <cstring>
 #include <type_traits>
 
 #include "tc_common.cuh"
@@ -33,6 +35,7 @@ constexpr int NCONS = 256;  // consumer threads (warps 8-15: two warpgroups)
 constexpr int W_CONS0 = NPROD / 32, W_TMA = (NPROD + NCONS) / 32, W_LDA = W_TMA + 1;
 constexpr int TC_THREADS = NPROD + NCONS + 64;
 constexpr int NS_MAX = 4;  // raw activation stages
+constexpr size_t TC_SMEM_STAGED = 227 * 1024;  // H100 opt-in limit of dynamic shared memory per block: staged-epilogue plans
 
 struct TcK {
   int B, Cin, Cout, T_in, T_out, K, D, padL, pad_mode;
@@ -57,8 +60,18 @@ struct TcK {
   int wavenet;           // epilogue: cols < split -> y2 += v ; cols >= split -> y = (v + res) * scale
   int split;
   int co_off;            // first output channel of this launch (N-chunked callers)
-  int variant;           // debug (pwgb_debug_set(1, v)): bit 1 stages activations with cp.async instead of TMA
+  int variant;           // debug (pwgb_debug_set(1, v)): bit 1 stages activations with cp.async instead of TMA,
+                         // bit 2 keeps the register epilogue
+  int staged;            // plain epilogue through a shared-memory tile per consumer warpgroup (tc_plan)
 };
+
+// Staged epilogue tile of one consumer warpgroup: fp32 [col][64 * MT + 4].  Rows of a channel are contiguous, so one
+// bulk copy moves a channel's residual in and its outputs out; the 16-byte pad keeps the rows 16-byte aligned and puts
+// the 8 rows x 4 columns of an accumulator-fragment write in 32 distinct banks.
+__host__ __device__ constexpr int stage_ld(int mt) { return 64 * mt + 4; }
+// Tile shapes compiled with the staged epilogue: at MT = 2 and more than 32 columns it made ptxas spill, and its tiles
+// would not fit beside the pipeline there anyway.
+__host__ __device__ constexpr bool stage_shape(int mt, int cout) { return mt == 1 || cout <= 32; }
 
 // ------------------------------------------------------------------ weight packing
 // w (rows, cin_real, K) fp32 -> rows [co_begin, co_begin + rows) of the operand image
@@ -224,12 +237,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
                      const uint4* __restrict__ wpk, const float* __restrict__ bias, const float* __restrict__ res,
                      float* __restrict__ y, float* __restrict__ y2) {
   extern __shared__ __align__(128) unsigned char smem[];
-  // layout: A[na] | B[nb] | raw staging[ns] | barriers | bias
+  // layout: A[na] | B[nb] | raw staging[ns] | epilogue tiles[2 if staged] | barriers | bias
+  constexpr int SLD = stage_ld(MT);
+  const bool staged = stage_shape(MT, NB16 * 16) && p.staged;
   unsigned char* a_buf = smem;
   unsigned char* b_buf = smem + (size_t)p.na * p.a_bytes;
   unsigned char* raw_buf = b_buf + (size_t)p.nb * p.b_bytes;
-  unsigned long long* bars = reinterpret_cast<unsigned long long*>(raw_buf + (size_t)p.ns * p.raw_bytes);
-  const int nbar = 2 * p.na + 2 * p.nb + 4 + 2 * NS_MAX;
+  float* stage_buf = reinterpret_cast<float*>(raw_buf + (size_t)p.ns * p.raw_bytes);
+  unsigned long long* bars = reinterpret_cast<unsigned long long*>(stage_buf + (staged ? 2 * p.Cout * SLD : 0));
+  const int nbar = 2 * p.na + 2 * p.nb + 4 + 2 * NS_MAX + 2;
   float* bias_s = reinterpret_cast<float*>(bars + nbar + 2);  // Cout floats (0 when bias == nullptr)
   // several column chunks / groups of a plain (non pixel-shuffle) conv share the launch
   const bool MC = p.nco > 1 && p.shuffle <= 1;
@@ -248,6 +264,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   auto B_EMPTY = [&](int i) { return bar0 + 8u * (2 * p.na + p.nb + i); };
   auto RAW_FULL = [&](int i) { return bar0 + 8u * (2 * p.na + 2 * p.nb + 4 + i); };
   auto RAW_EMPTY = [&](int i) { return bar0 + 8u * (2 * p.na + 2 * p.nb + 4 + NS_MAX + i); };
+  auto RES_FULL = [&](int wg) { return bar0 + 8u * (2 * p.na + 2 * p.nb + 4 + 2 * NS_MAX + wg); };  // staged residual
 
   if (tid == 0) {
     for (int i = 0; i < p.na; ++i) {
@@ -262,6 +279,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       mbar_init(RAW_FULL(i), 1);
       mbar_init(RAW_EMPTY(i), NPROD);
     }
+    // one arrival per channel row: each issuing thread of the warpgroup arrives with its row's byte count
+    for (int i = 0; i < 2; ++i) mbar_init(RES_FULL(i), p.Cout);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   for (int i = tid; i < p.Cout * (MC ? p.nco : 1); i += TC_THREADS)
@@ -448,7 +467,43 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     constexpr int NACC = 8 * NB16;  // fp32 accumulators per thread and 64-row block
     const unsigned lbo_a = (unsigned)p.R * 16u, lbo_b = NB16 * 256u;
     const unsigned a_sub = (unsigned)(KC / 8) * p.R, b_sub = (KC / 8) * NB16 * 16u;  // hi -> lo image (16-byte units)
+    // Staged epilogue: thread wt of the warpgroup owns channel row wt of the warpgroup's tile.  It issues that row's
+    // residual load and its store (or add), so its own bulk-group wait is the only guard the row needs before reuse.
+    const int wt = tid - NPROD - wg * 128;
+    float* stg = stage_buf + (size_t)wg * p.Cout * SLD;
+    const bool row_owner = staged && wt < p.Cout;
     int buf = 0, aph = 0, s = 0, bph = 0;
+    // (batch, first time step, first channel) of a tile
+    auto tile_pos = [&](int tile, int& b, int& t0, int& co_base) {
+      const int tr = p.nco > 1 ? tile % pct : tile;  // tile within its column chunk
+      b = tr / p.tiles_per_seq;
+      t0 = (tr - b * p.tiles_per_seq) * TT;
+      co_base = p.co_off + (p.nco > 1 ? (tile / pct) * p.Cout : 0);
+    };
+    // channel row wt of this warpgroup's rows [tw0, tw0 + MT * 64) of a tile: its first element within the batch item
+    // (y / residual layout) and its bytes below T_out
+    auto row_pos = [&](int t0, int co_base, unsigned& row_bytes) -> long long {
+      const int tw0 = t0 + wg * MT * 64;
+      const int nrow = p.T_out - tw0 < MT * 64 ? p.T_out - tw0 : MT * 64;
+      row_bytes = nrow > 0 ? 4u * (unsigned)nrow : 0u;
+      return (long long)(co_base + wt) * p.T_out + tw0;
+    };
+    // Residual row of a tile, issued before the tile's MMAs (at the end of the previous tile's epilogue, once its store
+    // has read the row), so that it streams in while they run.  Nothing of it is live across the MMA loop.
+    auto load_res = [&](int tile) {
+      int b, t0, co_base;
+      unsigned row_bytes;
+      tile_pos(tile, b, t0, co_base);
+      const long long row_off = row_pos(t0, co_base, row_bytes);
+      bulk_wait_read();
+      if (row_bytes) {
+        mbar_expect_tx(RES_FULL(wg), row_bytes);
+        bulk_g2s(smem_u32(stg + wt * SLD), res + (long long)b * p.rbs + row_off, row_bytes, RES_FULL(wg));
+      } else {
+        mbar_arrive(RES_FULL(wg));
+      }
+    };
+    if (row_owner && res && (int)blockIdx.x < p.total_tiles) load_res(blockIdx.x);
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       float acc[MT * NACC];
 #pragma unroll
@@ -496,10 +551,29 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         if (held_s >= 0) mbar_arrive(B_EMPTY(held_s));
         if (held_a >= 0) mbar_arrive(A_EMPTY(held_a));
       }
-      const int tr = p.nco > 1 ? tile % pct : tile;  // tile within its column chunk
-      const int b = tr / p.tiles_per_seq;
-      const int t0 = (tr - b * p.tiles_per_seq) * TT;
-      const int co_base = p.co_off + (p.nco > 1 ? (tile / pct) * p.Cout : 0);
+      int b, t0, co_base;
+      tile_pos(tile, b, t0, co_base);
+      // Staged (plain mode): v = (act(a + bias) + res) * out_scale in the register epilogue's order, written over the
+      // residual in the warpgroup's tile, then one bulk store (accumulate: bulk fp32 add, y + v) per channel row.
+      if (staged) {
+        if (res) {
+          mbar_wait_trap(RES_FULL(wg), ((tile - blockIdx.x) / gridDim.x) & 1);  // one phase per tile
+        } else {
+          if (row_owner) bulk_wait_read();  // the last tile's store has read the tile
+          wg_barrier(wg);
+        }
+      }
+      auto stage_block = [&](const float* ab, int mb) {
+#pragma unroll
+        for (int i = 0; i < NACC; ++i) {
+          const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+          float* sv = stg + col * SLD + mb * 64 + wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+          float v = ab[i] + bias_s[co_base - p.co_off + col];
+          if (p.post_act != PWGB_ACT_NONE) v = p.post_act == PWGB_ACT_TANH ? tanhf(v) : lrelu(v, p.post_slope);
+          if (res) v += *sv;
+          *sv = v * p.out_scale;
+        }
+      };
       // one 64-row block at a time, the mode chosen once per block (branching per element, or once for both blocks,
       // made ptxas spill at MT = 2)
       auto store_block = [&](auto mode, const float* ab, int mb) {
@@ -512,14 +586,32 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       };
 #pragma unroll
       for (int mb = 0; mb < MT; ++mb) {
-        if (p.shuffle > 1)
+        if (staged)
+          stage_block(acc + mb * NACC, mb);
+        else if (p.shuffle > 1)
           store_block(std::integral_constant<int, EPI_SHUFFLE>{}, acc + mb * NACC, mb);
         else if (p.wavenet)
           store_block(std::integral_constant<int, EPI_WAVENET>{}, acc + mb * NACC, mb);
         else
           store_block(std::integral_constant<int, EPI_PLAIN>{}, acc + mb * NACC, mb);
       }
+      if (staged) {
+        fence_proxy_async();  // generic-proxy writes -> visible to the bulk copies
+        wg_barrier(wg);
+        unsigned row_bytes;
+        const long long row_off = row_pos(t0, co_base, row_bytes);
+        if (row_owner && row_bytes) {
+          float* q = y + (long long)b * p.ybs + row_off;
+          if (p.accumulate)
+            bulk_s2g_add(q, smem_u32(stg + wt * SLD), row_bytes);
+          else
+            bulk_s2g(q, smem_u32(stg + wt * SLD), row_bytes);
+          bulk_commit();
+        }
+        if (row_owner && res && tile + (int)gridDim.x < p.total_tiles) load_res(tile + gridDim.x);
+      }
     }
+    if (row_owner) bulk_wait();  // the shared-memory source must outlive the CTA's last stores
   } else if (warp == W_TMA) {
     // ===================== B producer (TMA bulk copies of packed weight stages) =====================
     const int per_tile = p.nchunks * p.K + p.nchunks2;
@@ -581,10 +673,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 }
 
 static int g_tc_variant = 0;
+// the plan of the last conv1d_tc_kernel launch, for pwgb_debug_get(1, ...)
+struct TcPlanInfo {
+  int MT, na, nb, ns, staged;
+};
+static TcPlanInfo g_tc_last = {};
 
 // aux_c2: channels of the auxiliary 1x1 source (0 = none, else multiple of KC); split > 0 selects the
 // WaveNet epilogue.  pre_gate: d->cin is the number of gated channels, x holds 2*cin channels.
-static int tc_plan(const pwgb_conv1d_desc* d, TcK& p, size_t& smem_bytes, int aux_c2 = 0, int split = 0, int nco_bias = 1) {
+// has_res: the launch adds a residual (selects the staged epilogue like an accumulate does).
+static int tc_plan(const pwgb_conv1d_desc* d, TcK& p, size_t& smem_bytes, int aux_c2 = 0, int split = 0, int nco_bias = 1,
+                   int has_res = 0) {
   p.variant = g_tc_variant;
   p.co_off = 0;
   p.nco = 1;
@@ -625,67 +724,84 @@ static int tc_plan(const pwgb_conv1d_desc* d, TcK& p, size_t& smem_bytes, int au
   p.ybs = d->shuffle > 1 ? (long long)(d->cout / d->shuffle) * d->shuffle_tout : (long long)d->cout * d->t_out;
   p.rbs = (long long)d->cout * d->t_out;
   p.b_bytes = 2 * (KC / 8) * d->cout * 16;
-  // tile shape (1 persistent CTA / SM, ~216 KB of shared memory): prefer a contiguous halo tile of
-  // 2 x 128 rows (Cout <= 64: the 64 accumulator registers hold both); fall back to 128 rows, then to
-  // one window per tap (very large dilation)
-  const size_t budget = 216 * 1024;
-  for (int attempt = 0; attempt < 4; ++attempt) {
-    if (attempt == 0) {
-      p.MT = (d->cout <= TC_NMAX / 2 && d->t_out > 128) ? 2 : 1;
-      p.win_mode = 0;
-      p.R = p.MT * 128 + (int)halo;
-    } else if (attempt == 1) {
-      p.MT = 1;
-      p.win_mode = 0;
-      p.R = 128 + (int)halo;
-    } else if (attempt == 2) {
-      p.MT = (d->cout <= TC_NMAX / 2 && d->t_out > 128) ? 2 : 1;
-      p.win_mode = 1;
-      p.R = d->kernel * p.MT * 128;
-    } else {
-      p.MT = 1;
-      p.win_mode = 1;
-      p.R = d->kernel * 128;
+  // Staged epilogue (see conv1d_tc_kernel): plain mode with a residual or an accumulate, 16-byte rows (T_out % 4 == 0;
+  // tc_launch also checks the y and residual base pointers).  Its two tiles must fit beside the raw-staged pipeline
+  // (three raw stages with TMA activations, else two; two operand buffers) and at least four weight stages, within the
+  // opt-in limit TC_SMEM_STAGED instead of the 216 KB of the other plans; a tile shape that cannot gets the next
+  // attempt (64 channels: MT = 1 instead of 2), and without any such plan the conv keeps the register epilogue.
+  const bool want_stage = !(p.variant & 4) && d->shuffle <= 1 && split == 0 && !d->pre_gate && (has_res || d->accumulate) &&
+                          d->t_out % 4 == 0;
+  for (int staged = want_stage ? 1 : 0; staged >= 0; --staged) {
+    // tile shape (1 persistent CTA / SM, ~216 KB of shared memory): prefer a contiguous halo tile of
+    // 2 x 128 rows (Cout <= 64: the 64 accumulator registers hold both); fall back to 128 rows, then to
+    // one window per tap (very large dilation)
+    const size_t budget = staged ? TC_SMEM_STAGED : 216 * 1024;
+    for (int attempt = 0; attempt < 4; ++attempt) {
+      if (attempt == 0) {
+        p.MT = (d->cout <= TC_NMAX / 2 && d->t_out > 128) ? 2 : 1;
+        p.win_mode = 0;
+        p.R = p.MT * 128 + (int)halo;
+      } else if (attempt == 1) {
+        p.MT = 1;
+        p.win_mode = 0;
+        p.R = 128 + (int)halo;
+      } else if (attempt == 2) {
+        p.MT = (d->cout <= TC_NMAX / 2 && d->t_out > 128) ? 2 : 1;
+        p.win_mode = 1;
+        p.R = d->kernel * p.MT * 128;
+      } else {
+        p.MT = 1;
+        p.win_mode = 1;
+        p.R = d->kernel * 128;
+      }
+      if (!p.win_mode && halo > 2048) continue;
+      if (p.win_mode && halo <= p.MT * 128) continue;  // a contiguous tile is never larger in that case
+      p.a_bytes = 2 * (KC / 8) * p.R * 16;
+      p.R4 = (p.R + 6) & ~3;
+      p.raw_bytes = KC * p.R4 * 4;
+      // activation rows by TMA: zero padding only (out-of-range samples are masked, never copied) and
+      // 16-byte aligned rows; anything else is staged with 4-byte cp.async by the producers
+      p.tma_act = !(p.variant & 2) && !d->pre_gate && !p.win_mode && d->pad_mode == PWGB_PAD_ZERO && d->t_in % 4 == 0 &&
+                  (aux_c2 == 0 || d->t_out % 4 == 0);
+      // shared-memory split: [na operand buffers][nb weight stages][ns raw staging buffers][epilogue tiles]
+      int na = 0, nb = 0, ns = 0;
+      const size_t bias_bytes = 4 * (size_t)(nco_bias > 1 ? nco_bias * d->cout : TC_NMAX);  // bias of every column chunk of the launch
+      const size_t A = (size_t)p.a_bytes, Bs = (size_t)p.b_bytes, S = (size_t)p.raw_bytes, slack = 1024 + bias_bytes;
+      const size_t E = staged ? 2 * (size_t)d->cout * stage_ld(p.MT) * 4 : 0;
+      if (staged) {
+        if (!stage_shape(p.MT, d->cout)) continue;
+        ns = p.tma_act ? 3 : 2;
+        na = 2;
+        if (na * A + ns * S + 4 * Bs + E + slack > budget) continue;
+      } else if (p.tma_act && 2 * A + 3 * S + 3 * Bs + slack <= budget) {
+        ns = 3;
+        na = 2;
+      } else if (!d->pre_gate && 3 * A + 2 * S + 3 * Bs + slack <= budget) {
+        ns = 2;
+        na = 3;
+      } else if (!d->pre_gate && 2 * A + 2 * S + 2 * Bs + slack <= budget) {
+        ns = 2;
+        na = 2;
+      } else if (3 * A + 2 * Bs + slack <= budget) {
+        na = 3;
+      } else if (2 * A + 2 * Bs + slack <= budget) {
+        na = 2;
+      } else {
+        continue;
+      }
+      if (ns == 0) p.tma_act = 0;
+      nb = (int)((budget - slack - (size_t)na * A - (size_t)ns * S - E) / Bs);
+      if (nb > 24) nb = 24;
+      p.na = na;
+      p.nb = nb;
+      p.ns = ns;
+      p.staged = staged;
+      p.tiles_per_seq = ceil_div(d->t_out, p.MT * 128);
+      p.total_tiles = p.tiles_per_seq * d->batch;
+      smem_bytes = (size_t)na * p.a_bytes + (size_t)ns * p.raw_bytes + (size_t)nb * p.b_bytes + E +
+                   8 * (2 * na + 2 * nb + 4 + 2 * NS_MAX + 2) + 16 + bias_bytes;
+      return 1;
     }
-    if (!p.win_mode && halo > 2048) continue;
-    if (p.win_mode && halo <= p.MT * 128) continue;  // a contiguous tile is never larger in that case
-    p.a_bytes = 2 * (KC / 8) * p.R * 16;
-    p.R4 = (p.R + 6) & ~3;
-    p.raw_bytes = KC * p.R4 * 4;
-    // activation rows by TMA: zero padding only (out-of-range samples are masked, never copied) and
-    // 16-byte aligned rows; anything else is staged with 4-byte cp.async by the producers
-    p.tma_act = !(p.variant & 2) && !d->pre_gate && !p.win_mode && d->pad_mode == PWGB_PAD_ZERO && d->t_in % 4 == 0 &&
-                (aux_c2 == 0 || d->t_out % 4 == 0);
-    // shared-memory split: [na operand buffers][nb weight stages][ns raw staging buffers]
-    int na = 0, nb = 0, ns = 0;
-    const size_t bias_bytes = 4 * (size_t)(nco_bias > 1 ? nco_bias * d->cout : TC_NMAX);  // bias of every column chunk of the launch
-    const size_t A = (size_t)p.a_bytes, Bs = (size_t)p.b_bytes, S = (size_t)p.raw_bytes, slack = 1024 + bias_bytes;
-    if (p.tma_act && 2 * A + 3 * S + 3 * Bs + slack <= budget) {
-      ns = 3;
-      na = 2;
-    } else if (!d->pre_gate && 3 * A + 2 * S + 3 * Bs + slack <= budget) {
-      ns = 2;
-      na = 3;
-    } else if (!d->pre_gate && 2 * A + 2 * S + 2 * Bs + slack <= budget) {
-      ns = 2;
-      na = 2;
-    } else if (3 * A + 2 * Bs + slack <= budget) {
-      na = 3;
-    } else if (2 * A + 2 * Bs + slack <= budget) {
-      na = 2;
-    } else {
-      continue;
-    }
-    if (ns == 0) p.tma_act = 0;
-    nb = (int)((budget - slack - (size_t)na * A - (size_t)ns * S) / Bs);
-    if (nb > 24) nb = 24;
-    p.na = na;
-    p.nb = nb;
-    p.ns = ns;
-    p.tiles_per_seq = ceil_div(d->t_out, p.MT * 128);
-    p.total_tiles = p.tiles_per_seq * d->batch;
-    smem_bytes = (size_t)na * p.a_bytes + (size_t)ns * p.raw_bytes + (size_t)nb * p.b_bytes + 8 * (2 * na + 2 * nb + 4 + 2 * NS_MAX) + 16 + bias_bytes;
-    return 1;
   }
   return 0;
 }
@@ -719,7 +835,7 @@ static int tc_launch(TcK& p, size_t bytes, const float* x, const void* packed_w,
   if (!attr_set) {
     for (int mt = 1; mt <= 2; ++mt)
       for (int cout = 16; cout <= TC_NMAX / mt; cout += 16) {
-        cudaError_t e = cudaFuncSetAttribute(tc_kernel_for(mt, cout), cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+        cudaError_t e = cudaFuncSetAttribute(tc_kernel_for(mt, cout), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM_STAGED);
         if (e != cudaSuccess) {
           set_error("conv1d_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
           return PWGB_CUDA_ERROR;
@@ -740,6 +856,9 @@ static int tc_launch(TcK& p, size_t bytes, const float* x, const void* packed_w,
   }
   if (p.tma_act && ((reinterpret_cast<uintptr_t>(x) & 15) || (x2 && (reinterpret_cast<uintptr_t>(x2) & 15))))
     p.tma_act = 0;  // unaligned base pointer: the producers stage with cp.async instead
+  if (p.staged && ((reinterpret_cast<uintptr_t>(y) & 15) || (reinterpret_cast<uintptr_t>(residual) & 15)))
+    p.staged = 0;  // bulk copies need 16-byte aligned rows: the register epilogue (the plan's tiles stay unused)
+  g_tc_last = TcPlanInfo{p.MT, p.na, p.nb, p.ns, p.staged};
   const int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
   kernel<<<(unsigned)grid, TC_THREADS, bytes, st>>>(p, x, x2, (const uint4*)packed_w, bias, residual, y, y2);
   return check_launch("conv1d_tc_kernel");
@@ -783,10 +902,11 @@ extern "C" void pwgb_debug_set(int key, int value) {
   if (key == 1) g_tc_variant = value;
 }
 
-// no debug read-back is available in this build
+// key 1: the plan of the last conv1d_tc launch as 5 ints {MT, na, nb, ns, staged}
 extern "C" int pwgb_debug_get(int key, void* dst, size_t bytes) {
-  (void)key, (void)dst, (void)bytes;
-  return -1;
+  if (key != 1 || !dst || bytes < sizeof(TcPlanInfo)) return -1;
+  memcpy(dst, &g_tc_last, sizeof(TcPlanInfo));
+  return 0;
 }
 
 extern "C" size_t pwgb_conv1d_tc_packed_weight_bytes(int cin, int cout, int kernel) {
@@ -859,7 +979,7 @@ extern "C" int pwgb_conv1d_tc_forward(const pwgb_conv1d_desc* d, const float* x,
   TcK p;
   size_t bytes = 0;
   const int nco = G * (cout_g / chunk);
-  if (!tc_plan(&c, p, bytes, 0, 0, nco)) {
+  if (!tc_plan(&c, p, bytes, 0, 0, nco, residual != nullptr)) {
     set_error("conv1d_tc: no tile plan for this configuration");
     return PWGB_UNSUPPORTED;
   }

@@ -89,6 +89,20 @@ __device__ __forceinline__ void bulk_g2s(unsigned dst, const void* src, unsigned
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
+// shared -> global bulk copy, and the same as an fp32 add into global memory (y = y + smem, round to nearest); both
+// belong to the issuing thread's bulk group
+__device__ __forceinline__ void bulk_s2g(void* dst, unsigned src, unsigned bytes) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_s2g_add(float* dst, unsigned src, unsigned bytes) {
+  asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;" ::"l"(dst), "r"(src), "r"(bytes)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// this thread's bulk groups have finished reading their shared-memory source
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// this thread's bulk groups are complete (writes performed)
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void cp_async4(unsigned dst, const float* src, unsigned src_bytes) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
 }

@@ -1,4 +1,7 @@
-"""Per-launch table of the HiFi-GAN v1 C2 forward (CUDA events on the launching stream)."""
+"""Per-launch table of the HiFi-GAN v1 C2 forward (CUDA events on the launching stream).  For conv1d_tc launches the
+last column is the tile plan: MT (64-row blocks per warpgroup), na / nb / ns (operand buffers, weight stages, raw
+activation stages) and whether the epilogue went through the shared-memory tile (staged) or registers."""
+import ctypes as C
 import os
 import sys
 
@@ -6,12 +9,26 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 
 import bench
-from parallelwavegan_b200 import ops
+from parallelwavegan_b200 import capi, ops
 
 model, _ = bench.synth_weights()
 dev = torch.device("cuda:0")
 model = model.to(dev)
 mel = torch.randn(bench.BATCH, 80, bench.FRAMES, device=dev)
+
+plans = {}
+_done = ops._Prof.done
+
+
+def _done_with_plan(self):
+    _done(self)
+    if ops.PROFILE is not None and self.name == "conv1d_tc":
+        v = (C.c_int * 5)()
+        if capi.lib().pwgb_debug_get(1, C.cast(v, C.c_void_p), C.sizeof(v)) == 0:
+            plans[len(ops.PROFILE) - 1] = f"MT{v[0]} na{v[1]} nb{v[2]} ns{v[3]} {'staged' if v[4] else 'reg'}"
+
+
+ops._Prof.done = _done_with_plan
 with torch.no_grad():
     for _ in range(3):
         model(mel)
@@ -21,9 +38,9 @@ with torch.no_grad():
     torch.cuda.synchronize()
 prof, ops.PROFILE = ops.PROFILE, None
 tot = 0.0
-print(f"{'kernel':18s} {'shape':46s} {'ms':>8s} {'TFLOP/s':>8s} {'algGB/s':>8s}")
-for name, fl, by, a, b, desc in prof:
+print(f"{'kernel':18s} {'shape':46s} {'ms':>8s} {'TFLOP/s':>8s} {'algGB/s':>8s}  plan")
+for i, (name, fl, by, a, b, desc) in enumerate(prof):
     ms = a.elapsed_time(b)
     tot += ms
-    print(f"{name:18s} {desc:46s} {ms:8.3f} {fl / ms / 1e9:8.1f} {by / ms / 1e6:8.0f}")
+    print(f"{name:18s} {desc:46s} {ms:8.3f} {fl / ms / 1e9:8.1f} {by / ms / 1e6:8.0f}  {plans.get(i, '')}")
 print("total ms", tot)

@@ -11,7 +11,8 @@ dev = torch.device("cuda:0")
 if os.environ.get("PWGB_TC_VARIANT"):
     from parallelwavegan_b200 import capi
 
-    capi.lib().pwgb_debug_set(1, int(os.environ["PWGB_TC_VARIANT"]))  # bit1: no TMA activations, bit2: one MMA issuer
+    # value 2: activations staged with cp.async instead of TMA, value 4: register epilogue instead of the staged one
+    capi.lib().pwgb_debug_set(1, int(os.environ["PWGB_TC_VARIANT"]))
 for spec in sys.argv[1:]:
     c, k, d, T, B = [int(v) for v in spec.split(",")]
     x = torch.randn(B, c, T, device=dev)
