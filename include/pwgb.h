@@ -132,6 +132,30 @@ PWGB_API int pwgb_conv1d_tc_forward(const pwgb_conv1d_desc* d, const float* x, c
                            const float* residual, float* y, void* stream);
 
 /* ------------------------------------------------------------------------
+ * One HiFi-GAN ResBlock conv pair (layers/residual_block.py:243-258, non-causal, additional convs) in one
+ * tensor-core launch; the intermediate stays in shared memory:
+ *     h = conv_{kernel,dilation}(lrelu(x)) + b1 ;  x' = conv_{kernel,1}(lrelu(h)) + b2 + x
+ *     y = out_scale * x'   (accumulate: y += out_scale * x')
+ * x, y: (batch, channels, t), 16-byte aligned, y must not alias x.  Both convs pad with zeros ("same" length).
+ * w1_packed / w2_packed: pwgb_conv1d_tc_pack_weight images of the two (channels, channels, kernel) weights; b1 / b2
+ * may be NULL.  The result is bit-identical to the two pwgb_conv1d_tc_forward calls it replaces.
+ * pwgb_resblock_pair_supported() == 0 (channels other than 32 / 64, t % 4 != 0, or no shared-memory plan): use
+ * those two calls instead.  pwgb_resblock_pair_plan() fills 5 ints {output rows per tile, conv rows per tile,
+ * conv1 operand buffers, weight stages, raw activation stages} and returns 1, or returns 0 when unsupported.
+ * ---------------------------------------------------------------------- */
+typedef struct pwgb_resblock_desc {
+  int32_t batch, channels, t;
+  int32_t kernel, dilation; /* conv1: (kernel, dilation); conv2: (kernel, 1) */
+  float slope;              /* LeakyReLU negative slope before each conv */
+  float out_scale;
+  int32_t accumulate;
+} pwgb_resblock_desc;
+PWGB_API int pwgb_resblock_pair_supported(const pwgb_resblock_desc* d);
+PWGB_API int pwgb_resblock_pair_plan(const pwgb_resblock_desc* d, int* info);
+PWGB_API int pwgb_resblock_pair_forward(const pwgb_resblock_desc* d, const float* x, const void* w1_packed, const float* b1,
+                               const void* w2_packed, const float* b2, float* y, void* stream);
+
+/* ------------------------------------------------------------------------
  * Fused WaveNet residual layer of ParallelWaveGANGenerator (layers/residual_block.py:102-140,
  * called 30x from models/parallel_wavegan.py:161-166):
  *     g  = conv_{k,dilation}(x) + W_aux c (+ b_conv)

@@ -40,6 +40,13 @@ class WaveNetDesc(C.Structure):
     ]
 
 
+class ResBlockDesc(C.Structure):
+    _fields_ = [
+        ("batch", C.c_int32), ("channels", C.c_int32), ("t", C.c_int32), ("kernel", C.c_int32), ("dilation", C.c_int32),
+        ("slope", C.c_float), ("out_scale", C.c_float), ("accumulate", C.c_int32),
+    ]
+
+
 class WnStackDesc(C.Structure):
     _fields_ = [
         ("batch", C.c_int32), ("t", C.c_int32), ("residual_channels", C.c_int32), ("gate_channels", C.c_int32),
@@ -92,6 +99,12 @@ def lib():
     L.pwgb_debug_set.argtypes = [C.c_int, C.c_int]
     L.pwgb_debug_get.restype = C.c_int
     L.pwgb_debug_get.argtypes = [C.c_int, vp, C.c_size_t]
+    L.pwgb_resblock_pair_supported.restype = C.c_int
+    L.pwgb_resblock_pair_supported.argtypes = [C.POINTER(ResBlockDesc)]
+    L.pwgb_resblock_pair_plan.restype = C.c_int
+    L.pwgb_resblock_pair_plan.argtypes = [C.POINTER(ResBlockDesc), C.POINTER(C.c_int)]
+    L.pwgb_resblock_pair_forward.restype = C.c_int
+    L.pwgb_resblock_pair_forward.argtypes = [C.POINTER(ResBlockDesc), vp, vp, vp, vp, vp, vp, vp]
     L.pwgb_wavenet_supported.restype = C.c_int
     L.pwgb_wavenet_supported.argtypes = [C.POINTER(WaveNetDesc)]
     L.pwgb_wavenet_packed_bytes.restype = C.c_size_t
@@ -222,7 +235,9 @@ EXPORTED_SYMBOLS = [
     "pwgb_conv1d_forward", "pwgb_conv_transpose1d_workspace", "pwgb_conv_transpose1d_forward",
     "pwgb_conv1d_tc_packed_weight_bytes", "pwgb_conv1d_tc_pack_weight", "pwgb_conv1d_tc_pack_weight_grouped",
     "pwgb_conv1d_tc_supported",
-    "pwgb_conv1d_tc_forward", "pwgb_debug_set", "pwgb_debug_get", "pwgb_wavenet_supported", "pwgb_wavenet_packed_bytes",
+    "pwgb_conv1d_tc_forward", "pwgb_debug_set", "pwgb_debug_get",
+    "pwgb_resblock_pair_supported", "pwgb_resblock_pair_plan", "pwgb_resblock_pair_forward",
+    "pwgb_wavenet_supported", "pwgb_wavenet_packed_bytes",
     "pwgb_wavenet_pack", "pwgb_wavenet_layer_forward", "pwgb_upsample_fir_forward",
     "pwgb_s2d_forward", "pwgb_s2d_backward", "pwgb_mt_clip_coef", "pwgb_mt_adam_step", "pwgb_prep_features", "pwgb_pcm16_forward", "pwgb_collate_crop",
     "pwgb_wnstack_supported", "pwgb_wnstack_x_bytes", "pwgb_wnstack_c_bytes", "pwgb_wnstack_pack_x", "pwgb_wnstack_unpack_x",

@@ -1,0 +1,462 @@
+// One HiFi-GAN ResBlock conv pair (layers/residual_block.py:243-258, non-causal, with the additional convs) in one
+// tensor-core kernel:
+//   h  = conv_{k,d}(lrelu(x)) + b1                       (zero padding (k-1)/2 * d)
+//   x' = conv_{k,1}(lrelu(h)) + b2 + x                   (zero padding (k-1)/2)
+//   y  = x' * out_scale,  or  y += x' * out_scale       (the last pair of a block writes the MRF sum)
+// The intermediate h never leaves the SM: conv1's accumulators are written, as lrelu(h) split into bf16 hi/lo, straight
+// into the K-major operand image that conv2's wgmma reads.  Everything else is the stride-1 conv of conv1d_tc.cu: the
+// same weight images (pwgb_conv1d_tc_pack_weight), bf16x3 products, and MMA order into every accumulator (32-channel
+// chunk, tap, k16 step, hi*hi, lo*hi, hi*lo), so the result is bit-identical to the two conv1d_tc launches.
+//
+// Tiling: a tile produces M2 output rows [t0, t0 + M2).  Conv2 needs h rows [t0 - p2, t0 + M2 + p2), p2 = (k-1)/2;
+// conv1 computes the TT = 128 MT rows [t0 - p2, t0 - p2 + TT) (two warpgroups of MT 64-row blocks) from
+// R1 = TT + (k-1) d input rows, so M2 = TT - (k-1) rounded down to a multiple of 4 (16-byte output rows).  Halo rows of
+// h are recomputed by the neighbouring tile.  Conv2 also runs TT rows per tile; rows >= M2 read beyond the computed h
+// rows and are dropped.
+// Warp roles (576 threads, one persistent CTA per SM), as in conv1d_tc_kernel with TMA-staged activations:
+//   warps 0-7   convert landed raw fp32 rows of x (pre-activation, padding mask, hi/lo split) into conv1's operand image
+//   warps 8-15  two consumer warpgroups: conv1 wgmma, h image, conv2 wgmma on it, staged epilogue (bulk copies)
+//   warp 16     weight stages (conv1's then conv2's of every tile) by cp.async.bulk
+//   warp 17     raw activation rows by cp.async.bulk
+#include <cstring>
+
+#include "tc_common.cuh"
+
+namespace pwgb {
+
+namespace {
+
+constexpr int RB_NPROD = 256;  // producer threads (warps 0-7)
+constexpr int RB_NCONS = 256;  // consumer threads (warps 8-15)
+constexpr int RB_W_CONS0 = RB_NPROD / 32, RB_W_TMA = (RB_NPROD + RB_NCONS) / 32, RB_W_LDA = RB_W_TMA + 1;
+constexpr int RB_THREADS = RB_NPROD + RB_NCONS + 64;
+__host__ __device__ constexpr int rb_sld(int mt) { return 64 * mt + 4; }  // staged epilogue row pitch, as in conv1d_tc.cu
+constexpr size_t RB_SMEM = 227 * 1024;      // H100 opt-in limit of dynamic shared memory per block
+constexpr int RB_MIN_STAGES = 4;            // weight stages a plan must keep
+
+struct RbK {
+  int B, C, T, K, D;
+  float slope, out_scale;
+  int accumulate;
+  int MT, M2;              // 64-row blocks per consumer warpgroup (conv rows per tile: 128 MT), output rows per tile
+  int p1, p2;              // left padding of conv1 ((k-1)/2 * d) and conv2 ((k-1)/2)
+  int R1, R4, Rh;          // conv1 operand rows, raw stage row pitch (floats), h image rows (128 MT + k - 1)
+  int nchunks, tiles_per_seq, total_tiles;
+  int na, nb, ns;          // conv1 operand buffers, weight stages, raw stages
+  int a_bytes, b_bytes, raw_bytes, h_bytes;  // per buffer / stage; h_bytes: one 32-channel chunk of the h image
+};
+
+// consumers of both warpgroups (named barrier 4; 1 = conv producers, 2-3 = per-warpgroup barriers)
+__device__ __forceinline__ void consumer_barrier() { asm volatile("bar.sync 4, %0;" ::"n"(RB_NCONS) : "memory"); }
+
+// MT: 64-row blocks per consumer warpgroup; NB16: channels / 16 (the MMA width; the weight images are the conv1d_tc
+// images of a Cout = C conv)
+template <int MT, int NB16>
+__global__ void __launch_bounds__(RB_THREADS, 1)
+    resblock_pair_kernel(const RbK p, const float* __restrict__ x, const unsigned char* __restrict__ w1,
+                         const float* __restrict__ b1, const unsigned char* __restrict__ w2, const float* __restrict__ b2,
+                         float* __restrict__ y) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  constexpr int C = 16 * NB16, NCH = C / KC, NACC = 8 * NB16, SLD = rb_sld(MT), WR = 64 * MT;  // WR: rows per warpgroup
+  // layout: A[na] | B[nb] | raw staging[ns] | h image[NCH chunks] | epilogue tiles[2] | barriers | bias1 | bias2
+  unsigned char* a_buf = smem;
+  unsigned char* b_buf = a_buf + (size_t)p.na * p.a_bytes;
+  unsigned char* raw_buf = b_buf + (size_t)p.nb * p.b_bytes;
+  unsigned char* h_buf = raw_buf + (size_t)p.ns * p.raw_bytes;
+  float* stage_buf = reinterpret_cast<float*>(h_buf + (size_t)NCH * p.h_bytes);
+  unsigned long long* bars = reinterpret_cast<unsigned long long*>(stage_buf + 2 * C * SLD);
+  const int nbar = 2 * p.na + 2 * p.nb + 2 * p.ns + 2;
+  float* bias_s = reinterpret_cast<float*>(bars + nbar);  // b1 | b2 (zeros for a missing bias)
+
+  const int tid = threadIdx.x;
+  const int warp = tid >> 5;
+  const int lane = tid & 31;
+
+  const unsigned bar0 = smem_u32(bars);
+  auto A_FULL = [&](int i) { return bar0 + 8u * i; };
+  auto A_EMPTY = [&](int i) { return bar0 + 8u * (p.na + i); };
+  auto B_FULL = [&](int i) { return bar0 + 8u * (2 * p.na + i); };
+  auto B_EMPTY = [&](int i) { return bar0 + 8u * (2 * p.na + p.nb + i); };
+  auto RAW_FULL = [&](int i) { return bar0 + 8u * (2 * p.na + 2 * p.nb + i); };
+  auto RAW_EMPTY = [&](int i) { return bar0 + 8u * (2 * p.na + 2 * p.nb + p.ns + i); };
+  auto RES_FULL = [&](int wg) { return bar0 + 8u * (2 * p.na + 2 * p.nb + 2 * p.ns + wg); };
+
+  if (tid == 0) {
+    for (int i = 0; i < p.na; ++i) {
+      mbar_init(A_FULL(i), RB_NPROD);
+      mbar_init(A_EMPTY(i), RB_NCONS / 32);
+    }
+    for (int i = 0; i < p.nb; ++i) {
+      mbar_init(B_FULL(i), 1);
+      mbar_init(B_EMPTY(i), RB_NCONS / 32);
+    }
+    for (int i = 0; i < p.ns; ++i) {
+      mbar_init(RAW_FULL(i), 1);
+      mbar_init(RAW_EMPTY(i), RB_NPROD);
+    }
+    for (int i = 0; i < 2; ++i) mbar_init(RES_FULL(i), C);  // one arrival per channel row of the warpgroup's tile
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  for (int i = tid; i < 2 * C; i += RB_THREADS) {
+    const float* bb = i < C ? b1 : b2;
+    bias_s[i] = bb ? __ldg(bb + (i < C ? i : i - C)) : 0.f;
+  }
+  // conv2 rows >= M2 read the h rows [128 MT, Rh) that no tile writes: keep them zero
+  for (int i = tid; i < NCH * p.h_bytes / 16; i += RB_THREADS) reinterpret_cast<uint4*>(h_buf)[i] = make_uint4(0, 0, 0, 0);
+  fence_proxy_async();
+  __syncthreads();
+
+  if (warp < RB_W_CONS0) {
+    // ===================== A producers: raw fp32 rows -> conv1 operand image =====================
+    int s = 0, sph = 0, buf = 0, aph = 0;
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      const int b = tile / p.tiles_per_seq;
+      const int t0 = (tile - b * p.tiles_per_seq) * p.M2;
+      const int ts_first = t0 - p.p2 - p.p1;
+      const int shift = ts_first - (ts_first & ~3);
+      for (int c = 0; c < NCH; ++c) {
+        mbar_wait(RAW_FULL(s), sph);
+        mbar_wait(A_EMPTY(buf), aph ^ 1);
+        unsigned char* dst = a_buf + (size_t)buf * p.a_bytes;
+        const float* raw = reinterpret_cast<const float*>(raw_buf + (size_t)s * p.raw_bytes);
+        for (int r = tid; r < p.R1; r += RB_NPROD) {
+          const bool ok = (unsigned)(ts_first + r) < (unsigned)p.T;
+          const float* rr = raw + r + shift;
+#pragma unroll
+          for (int g = 0; g < KC / 8; ++g) {
+            float u[8];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) u[j] = ok ? lrelu(rr[(g * 8 + j) * p.R4], p.slope) : 0.f;
+            uint4 hi, lo;
+            split8(u, hi, lo);
+            *reinterpret_cast<uint4*>(dst + ((size_t)g * p.R1 + r) * 16) = hi;
+            *reinterpret_cast<uint4*>(dst + ((size_t)(KC / 8 + g) * p.R1 + r) * 16) = lo;
+          }
+        }
+        fence_proxy_async();
+        mbar_arrive(A_FULL(buf));
+        mbar_arrive(RAW_EMPTY(s));
+        if (++s == p.ns) { s = 0; sph ^= 1; }
+        if (++buf == p.na) { buf = 0; aph ^= 1; }
+      }
+    }
+  } else if (warp < RB_W_TMA) {
+    // ===================== consumers =====================
+    // warpgroup wg owns conv rows [WR wg, WR wg + WR) of both convs.  One wgmma group per (chunk, tap), kept in flight
+    // while the next is issued, as in conv1d_tc_kernel.
+    const int wg = (warp - RB_W_CONS0) >> 2, wq = warp & 3;
+    const unsigned lbo_b = NB16 * 256u, b_sub = (KC / 8) * NB16 * 16u;
+    const unsigned lbo_a = (unsigned)p.R1 * 16u, a_sub = (unsigned)(KC / 8) * p.R1;
+    const unsigned lbo_h = (unsigned)p.Rh * 16u, h_sub = (unsigned)(KC / 8) * p.Rh;
+    // staged epilogue: thread wt of the warpgroup owns channel row wt of the warpgroup's tile (residual in, result out)
+    const int wt = tid - RB_NPROD - wg * 128;
+    float* stg = stage_buf + (size_t)wg * C * SLD;
+    const bool row_owner = wt < C;
+    int buf = 0, aph = 0, s = 0, bph = 0;
+    // channel row wt of this warpgroup's output rows of a tile: first element and bytes (below M2 and T)
+    auto row_pos = [&](int tile, unsigned& row_bytes) -> long long {
+      const int b = tile / p.tiles_per_seq;
+      const int t0 = (tile - b * p.tiles_per_seq) * p.M2;
+      int nrow = p.M2 - wg * WR;
+      if (nrow > WR) nrow = WR;
+      if (nrow > p.T - (t0 + wg * WR)) nrow = p.T - (t0 + wg * WR);
+      row_bytes = nrow > 0 ? 4u * (unsigned)nrow : 0u;
+      return ((long long)b * C + wt) * p.T + t0 + wg * WR;
+    };
+    // the residual (x itself) of a tile, issued at the end of the previous tile's epilogue so that it streams in while
+    // this tile's MMAs run
+    auto load_res = [&](int tile) {
+      unsigned row_bytes;
+      const long long off = row_pos(tile, row_bytes);
+      bulk_wait_read();  // the previous store has read the row
+      if (row_bytes) {
+        mbar_expect_tx(RES_FULL(wg), row_bytes);
+        bulk_g2s(smem_u32(stg + wt * SLD), x + off, row_bytes, RES_FULL(wg));
+      } else {
+        mbar_arrive(RES_FULL(wg));
+      }
+    };
+    // one weight stage of wgmma on the operand image at `a_img` (rows `row0` ..): per k16 step and 64-row block, the
+    // three bf16x3 products
+    auto mma_stage = [&](float* acc, unsigned a_img, unsigned lbo, unsigned sub, int row0, unsigned b_addr) {
+      wg_fence();
+#pragma unroll
+      for (int ks = 0; ks < KC / 16; ++ks) {
+        const unsigned long long bh = gmma_desc(b_addr + (unsigned)(2 * ks) * lbo_b, lbo_b, 128);
+        const unsigned long long ah0 = gmma_desc(a_img + ((unsigned)(2 * ks) * (lbo / 16u) + (unsigned)row0) * 16u, lbo, 128);
+#pragma unroll
+        for (int mb = 0; mb < MT; ++mb) {
+          const unsigned long long ah = ah0 + 64 * mb;  // next 64 rows: 64 x 16 B
+          wgmma_n<0, 0, NB16>(acc + mb * NACC, ah, bh, 16);
+          wgmma_n<0, 0, NB16>(acc + mb * NACC, ah + sub, bh, 16);
+          wgmma_n<0, 0, NB16>(acc + mb * NACC, ah, bh + b_sub, 16);
+        }
+      }
+      wg_commit();
+    };
+    auto release = [&](int held_s, int held_a) {
+      __syncwarp();
+      if (lane == 0) {
+        if (held_s >= 0) mbar_arrive(B_EMPTY(held_s));
+        if (held_a >= 0) mbar_arrive(A_EMPTY(held_a));
+      }
+    };
+    if (row_owner && (int)blockIdx.x < p.total_tiles) load_res(blockIdx.x);
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      const int b = tile / p.tiles_per_seq;
+      const int t0 = (tile - b * p.tiles_per_seq) * p.M2;
+      float acc[MT * NACC];
+      // ---- conv1 over the staged x rows
+#pragma unroll
+      for (int e = 0; e < MT * NACC; ++e) acc[e] = 0.f;
+      int held_s = -1, held_a = -1;  // weight stage / A buffer read by the group in flight
+      for (int c = 0; c < NCH; ++c) {
+        mbar_wait_trap(A_FULL(buf), aph);
+        const unsigned a_addr = smem_u32(a_buf + (size_t)buf * p.a_bytes);
+        for (int k = 0; k < p.K; ++k) {
+          mbar_wait_trap(B_FULL(s), bph);
+          __syncwarp();
+          mma_stage(acc, a_addr, lbo_a, a_sub, k * p.D + wg * WR, smem_u32(b_buf + (size_t)s * p.b_bytes));
+          wg_wait<1>();  // the previous group has retired: its stage and, at a chunk boundary, its A buffer are free
+          release(held_s, held_a);
+          held_s = s;
+          held_a = k == p.K - 1 ? buf : -1;
+          if (++s == p.nb) { s = 0; bph ^= 1; }
+        }
+        if (++buf == p.na) { buf = 0; aph ^= 1; }
+      }
+      wg_wait<0>();
+      release(held_s, held_a);
+      // ---- h = lrelu(acc + b1) as conv2's operand image; rows outside [0, T) are conv2's zero padding.  Both
+      // warpgroups' conv2 MMAs of the previous tile must have read the image first.
+      consumer_barrier();
+      const int th0 = t0 - p.p2 + wg * WR;
+#pragma unroll
+      for (int e = 0; e < MT * NACC; e += 2) {
+        const int i = e % NACC;
+        const int col = 8 * (i >> 2) + 2 * (lane & 3);
+        const int r = (e / NACC) * 64 + wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+        const bool ok = (unsigned)(th0 + r) < (unsigned)p.T;
+        const float h0 = acc[e] + bias_s[col], h1 = acc[e + 1] + bias_s[col + 1];
+        unsigned hi, lo;
+        split2(ok ? lrelu(h0, p.slope) : 0.f, ok ? lrelu(h1, p.slope) : 0.f, hi, lo);
+        unsigned char* hc = h_buf + (size_t)(col >> 5) * p.h_bytes;
+        const size_t off = ((size_t)((col & 31) >> 3) * p.Rh + wg * WR + r) * 16 + (col & 7) * 2;
+        *reinterpret_cast<unsigned*>(hc + off) = hi;
+        *reinterpret_cast<unsigned*>(hc + (size_t)(KC / 8) * p.Rh * 16 + off) = lo;
+      }
+      fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor core
+      consumer_barrier();
+      // ---- conv2 over the h image (resident for the whole tile)
+#pragma unroll
+      for (int e = 0; e < MT * NACC; ++e) acc[e] = 0.f;
+      held_s = -1;
+      for (int c = 0; c < NCH; ++c) {
+        const unsigned h_addr = smem_u32(h_buf + (size_t)c * p.h_bytes);
+        for (int k = 0; k < p.K; ++k) {
+          mbar_wait_trap(B_FULL(s), bph);
+          __syncwarp();
+          mma_stage(acc, h_addr, lbo_h, h_sub, k + wg * WR, smem_u32(b_buf + (size_t)s * p.b_bytes));
+          wg_wait<1>();
+          release(held_s, -1);
+          held_s = s;
+          if (++s == p.nb) { s = 0; bph ^= 1; }
+        }
+      }
+      wg_wait<0>();
+      release(held_s, -1);
+      // ---- staged epilogue: v = (a + b2 + x) * out_scale over the residual row, one bulk store (or fp32 add) per row
+      mbar_wait_trap(RES_FULL(wg), ((tile - blockIdx.x) / gridDim.x) & 1);  // one phase per tile
+#pragma unroll
+      for (int e = 0; e < MT * NACC; ++e) {
+        const int i = e % NACC;
+        const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+        float* sv = stg + col * SLD + (e / NACC) * 64 + wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+        float v = acc[e] + bias_s[C + col];
+        v += *sv;
+        *sv = v * p.out_scale;
+      }
+      fence_proxy_async();  // generic-proxy writes -> visible to the bulk copies
+      wg_barrier(wg);
+      if (row_owner) {
+        unsigned row_bytes;
+        const long long off = row_pos(tile, row_bytes);
+        if (row_bytes) {
+          if (p.accumulate)
+            bulk_s2g_add(y + off, smem_u32(stg + wt * SLD), row_bytes);
+          else
+            bulk_s2g(y + off, smem_u32(stg + wt * SLD), row_bytes);
+          bulk_commit();
+        }
+        if (tile + (int)gridDim.x < p.total_tiles) load_res(tile + gridDim.x);
+      }
+    }
+    if (row_owner) bulk_wait();  // the shared-memory source must outlive the CTA's last stores
+  } else if (warp == RB_W_TMA) {
+    // ===================== weight stages: conv1's NCH * K, then conv2's, per tile =====================
+    const int per = NCH * p.K;
+    int s = 0, ph = 0;
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      for (int j = 0; j < 2 * per; ++j) {
+        mbar_wait_trap(B_EMPTY(s), ph ^ 1);
+        if (elect_one()) {
+          const unsigned char* src = j < per ? w1 + (size_t)j * p.b_bytes : w2 + (size_t)(j - per) * p.b_bytes;
+          mbar_expect_tx(B_FULL(s), (unsigned)p.b_bytes);
+          bulk_g2s(smem_u32(b_buf + (size_t)s * p.b_bytes), src, (unsigned)p.b_bytes, B_FULL(s));
+        }
+        __syncwarp();
+        if (++s == p.nb) { s = 0; ph ^= 1; }
+      }
+    }
+  } else if (warp == RB_W_LDA) {
+    // ===================== raw activation rows of x (one channel per lane) =====================
+    int s = 0, ph = 0;
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      const int b = tile / p.tiles_per_seq;
+      const int t0 = (tile - b * p.tiles_per_seq) * p.M2;
+      const int ts0 = (t0 - p.p2 - p.p1) & ~3;
+      const int start = ts0 < 0 ? 0 : ts0;
+      const int end = ts0 + p.R4 < p.T ? ts0 + p.R4 : p.T;
+      const int nbytes = (end - start) * 4;
+      for (int c = 0; c < NCH; ++c) {
+        mbar_wait(RAW_EMPTY(s), ph ^ 1);
+        if (nbytes > 0) {
+          if (lane == 0) mbar_expect_tx(RAW_FULL(s), (unsigned)nbytes * KC);
+          __syncwarp();
+          bulk_g2s(smem_u32(raw_buf + (size_t)s * p.raw_bytes) + (unsigned)(lane * p.R4 + start - ts0) * 4u,
+                   x + ((long long)b * C + c * KC + lane) * p.T + start, (unsigned)nbytes, RAW_FULL(s));
+        } else if (lane == 0) {
+          mbar_arrive(RAW_FULL(s));
+        }
+        __syncwarp();
+        if (++s == p.ns) { s = 0; ph ^= 1; }
+      }
+    }
+  }
+}
+
+using RbKernel = void (*)(const RbK, const float*, const unsigned char*, const float*, const unsigned char*, const float*,
+                          float*);
+
+// Instantiations: 32 and 64 channels at MT = 1, and 32 channels at MT = 2 (at 64 channels a 256-row tile's h image and
+// epilogue tiles alone would take 135 KB).
+RbKernel rb_kernel_for(int mt, int channels) {
+  if (mt == 1 && channels == 32) return resblock_pair_kernel<1, 2>;
+  if (mt == 1 && channels == 64) return resblock_pair_kernel<1, 4>;
+  if (mt == 2 && channels == 32) return resblock_pair_kernel<2, 2>;
+  return nullptr;
+}
+
+// Plan of one pair.  A warpgroup's 64-row blocks are independent accumulator chains, so the planner tries MT = 2 first
+// (the wgmma of one chain wait for each other: at MT = 1 and 32 channels the tensor cores idle between them), then
+// MT = 1.  Per tile shape: two conv1 operand buffers with three, then two raw stages; then, with one 32-channel chunk,
+// one operand buffer (the producers then convert the next tile while conv2 runs).  A plan must keep RB_MIN_STAGES
+// weight stages within the opt-in shared-memory limit.
+int rb_plan(const pwgb_resblock_desc* d, RbK& p, size_t& smem_bytes) {
+  if (!d || d->batch < 0 || d->t <= 0 || d->kernel < 1 || d->kernel % 2 == 0 || d->dilation < 1) return 0;
+  if (!rb_kernel_for(1, d->channels)) return 0;
+  if (d->t % 4 != 0) return 0;  // 16-byte rows for the bulk copies of x and y
+  const long long halo1 = (long long)(d->kernel - 1) * d->dilation;
+  if (d->kernel - 1 > 64 || halo1 > 2048) return 0;
+  p.B = d->batch;
+  p.C = d->channels;
+  p.T = d->t;
+  p.K = d->kernel;
+  p.D = d->dilation;
+  p.slope = d->slope;
+  p.out_scale = d->out_scale;
+  p.accumulate = d->accumulate;
+  p.p1 = (d->kernel - 1) / 2 * d->dilation;
+  p.p2 = (d->kernel - 1) / 2;
+  p.nchunks = d->channels / KC;
+  p.b_bytes = 2 * (KC / 8) * d->channels * 16;
+  static const int bufs[3][2] = {{2, 3}, {2, 2}, {1, 2}};  // (na, ns)
+  for (int mt = 2; mt >= 1; --mt) {
+    if (!rb_kernel_for(mt, d->channels)) continue;
+    const int tt = 128 * mt;
+    p.MT = mt;
+    p.M2 = (tt - (d->kernel - 1)) & ~3;
+    p.R1 = tt + (int)halo1;
+    p.R4 = (p.R1 + 6) & ~3;
+    p.Rh = tt + d->kernel - 1;
+    p.a_bytes = 2 * (KC / 8) * p.R1 * 16;
+    p.raw_bytes = KC * p.R4 * 4;
+    p.h_bytes = 2 * (KC / 8) * p.Rh * 16;
+    const size_t epi = 2 * (size_t)d->channels * rb_sld(mt) * 4;
+    const size_t fixed = (size_t)p.nchunks * p.h_bytes + epi + 2 * (size_t)d->channels * 4 + 1024;
+    for (const auto& nn : bufs) {
+      const int na = nn[0], ns = nn[1];
+      if (na < p.nchunks) continue;  // one operand buffer only for a single chunk
+      const size_t used = fixed + (size_t)na * p.a_bytes + (size_t)ns * p.raw_bytes;
+      if (used + (size_t)RB_MIN_STAGES * p.b_bytes > RB_SMEM) continue;
+      int nb = (int)((RB_SMEM - used) / p.b_bytes);
+      if (nb > 24) nb = 24;
+      p.na = na;
+      p.nb = nb;
+      p.ns = ns;
+      p.tiles_per_seq = ceil_div(d->t, p.M2);
+      if ((long long)p.tiles_per_seq * d->batch > 0x7fffffffLL) return 0;
+      p.total_tiles = p.tiles_per_seq * d->batch;
+      smem_bytes = (size_t)na * p.a_bytes + (size_t)nb * p.b_bytes + (size_t)ns * p.raw_bytes + (size_t)p.nchunks * p.h_bytes +
+                   epi + 8 * (size_t)(2 * na + 2 * nb + 2 * ns + 2) + 2 * (size_t)d->channels * 4;
+      return 1;
+    }
+  }
+  return 0;
+}
+
+}  // namespace
+
+}  // namespace pwgb
+
+using namespace pwgb;
+
+extern "C" int pwgb_resblock_pair_supported(const pwgb_resblock_desc* d) {
+  RbK p;
+  size_t bytes;
+  return rb_plan(d, p, bytes);
+}
+
+extern "C" int pwgb_resblock_pair_plan(const pwgb_resblock_desc* d, int* info) {
+  RbK p;
+  size_t bytes;
+  if (!info || !rb_plan(d, p, bytes)) return 0;
+  const int v[5] = {p.M2, 128 * p.MT, p.na, p.nb, p.ns};
+  memcpy(info, v, sizeof(v));
+  return 1;
+}
+
+extern "C" int pwgb_resblock_pair_forward(const pwgb_resblock_desc* d, const float* x, const void* w1_packed,
+                                          const float* b1, const void* w2_packed, const float* b2, float* y,
+                                          void* stream) {
+  PWGB_CHECK_ARG(d && x && w1_packed && w2_packed && y, "resblock_pair: null argument");
+  RbK p;
+  size_t bytes = 0;
+  PWGB_UNSUPPORTED_IF(!rb_plan(d, p, bytes), "resblock_pair: configuration not supported by the fused kernel");
+  PWGB_CHECK_ARG(x != y, "resblock_pair: y must not alias x (halo reads)");
+  PWGB_UNSUPPORTED_IF((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(y) & 15),
+                      "resblock_pair: x and y must be 16-byte aligned");
+  if (p.B == 0) return PWGB_OK;
+  static bool attr_set = false;
+  if (!attr_set) {
+    for (const RbKernel k : {rb_kernel_for(1, 32), rb_kernel_for(1, 64), rb_kernel_for(2, 32)}) {
+      cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RB_SMEM);
+      if (e != cudaSuccess) {
+        set_error("resblock_pair: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+        return PWGB_CUDA_ERROR;
+      }
+    }
+    attr_set = true;
+  }
+  static int num_sms = 0;
+  if (!num_sms) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
+    if (num_sms <= 0) num_sms = 132;
+  }
+  const int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
+  rb_kernel_for(p.MT, p.C)<<<(unsigned)grid, RB_THREADS, bytes, (cudaStream_t)stream>>>(
+      p, x, (const unsigned char*)w1_packed, b1, (const unsigned char*)w2_packed, b2, y);
+  return check_launch("resblock_pair_kernel");
+}

@@ -139,6 +139,14 @@ __device__ __forceinline__ void split8(const float (&v)[8], uint4& hi, uint4& lo
   hi = make_uint4(h[0], h[1], h[2], h[3]);
   lo = make_uint4(l[0], l[1], l[2], l[3]);
 }
+// two floats -> packed bf16 hi pair and lo pair (the residual of the hi rounding); the same values as split8
+__device__ __forceinline__ void split2(float a, float b, unsigned& hi, unsigned& lo) {
+  __nv_bfloat162 hh = __floats2bfloat162_rn(a, b);
+  const float2 hf = __bfloat1622float2(hh);
+  __nv_bfloat162 ll = __floats2bfloat162_rn(a - hf.x, b - hf.y);
+  hi = *reinterpret_cast<unsigned*>(&hh);
+  lo = *reinterpret_cast<unsigned*>(&ll);
+}
 
 // w (rows, cin_real, K) fp32 -> rows [co_begin, co_begin + rows) of the tensor-core weight operand image
 // [chunk][tap][hi|lo][ci8][co (cout_total)][8] bf16 (defined in conv1d_tc.cu)

@@ -73,14 +73,6 @@ __device__ __forceinline__ void bf16x8_to_float(const uint4& v, float (&f)[8]) {
     f[2 * i + 1] = __uint_as_float(u[i] & 0xFFFF0000u);
   }
 }
-// two floats -> packed bf16 hi pair and lo pair (the residual of the hi rounding)
-__device__ __forceinline__ void split2(float a, float b, unsigned& hi, unsigned& lo) {
-  __nv_bfloat162 hh = __floats2bfloat162_rn(a, b);
-  const float2 hf = __bfloat1622float2(hh);
-  __nv_bfloat162 ll = __floats2bfloat162_rn(a - hf.x, b - hf.y);
-  hi = *reinterpret_cast<unsigned*>(&hh);
-  lo = *reinterpret_cast<unsigned*>(&ll);
-}
 
 // z = gate(g) of this thread's accumulator fragment into the warpgroup's z image [hi|lo][H/8][64 rows][8] bf16.
 // HH = H / 2 registers separate gate column c from its partner c + H (H is a multiple of 32).

@@ -160,9 +160,14 @@ class HiFiGANResidualBlock(torch.nn.Module):
                 else:
                     x = c1(x, pre_slope=self.slope, residual=x, **tail)
             elif self.use_additional_convs:
-                xt = ops.conv1d(x, effective_weight(c1), c1.bias, dilation=d, padding=(k - 1) // 2 * d, pre_slope=self.slope)
                 c2 = self.convs2[idx][1]
-                x = ops.conv1d(xt, effective_weight(c2), c2.bias, padding=(k - 1) // 2, pre_slope=self.slope, residual=x, **tail)
+                w1, w2 = effective_weight(c1), effective_weight(c2)
+                # inference at 32 / 64 channels: both convs in one launch, the intermediate never leaves the SM
+                y = ops.resblock_pair(x, w1, c1.bias, w2, c2.bias, kernel_size=k, dilation=d, slope=self.slope, **tail)
+                if y is None:
+                    xt = ops.conv1d(x, w1, c1.bias, dilation=d, padding=(k - 1) // 2 * d, pre_slope=self.slope)
+                    y = ops.conv1d(xt, w2, c2.bias, padding=(k - 1) // 2, pre_slope=self.slope, residual=x, **tail)
+                x = y
             else:
                 x = ops.conv1d(x, effective_weight(c1), c1.bias, dilation=d, padding=(k - 1) // 2 * d, pre_slope=self.slope, residual=x, **tail)
         return x

@@ -188,6 +188,61 @@ def conv1d_raw(
     return out
 
 
+def resblock_pair(x, w1, b1, w2, b2, *, kernel_size, dilation, slope, out=None, accumulate=False, out_scale=1.0):
+    """One HiFi-GAN ResBlock conv pair in one launch (pwgb_resblock_pair_forward), inference only:
+        x' = conv_{k,1}(lrelu(conv_{k,d}(lrelu(x)) + b1)) + b2 + x     ("same" zero padding, LeakyReLU ``slope``)
+    returned as ``out_scale * x'``, or written / added into ``out``.  Bit-identical to the two conv1d calls it replaces.
+    Returns None when the fused kernel does not serve the call (autograd, the FFMA engine, channel counts other than
+    32 / 64, t % 4 != 0, unaligned tensors): the caller then runs the two convs."""
+    if ENGINE == "simt" or _needs_grad(x, w1, b1, w2, b2):
+        return None
+    if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 3 and x.is_contiguous()):
+        return None
+    B, Cc, T = x.shape
+    K = int(kernel_size)
+    if tuple(w1.shape) != (Cc, Cc, K) or tuple(w2.shape) != (Cc, Cc, K) or x.data_ptr() % 16:
+        return None
+    if out is not None and (tuple(out.shape) != tuple(x.shape) or not out.is_contiguous() or out.dtype != torch.float32
+                            or out.data_ptr() % 16 or out.data_ptr() == x.data_ptr()):
+        return None
+    if accumulate and out is None:
+        raise PwgbError("resblock_pair: accumulate needs `out`")
+    dkey = ("resblock", B, Cc, T, K, int(dilation), float(slope), float(out_scale), bool(accumulate))
+    d = _DESC_CACHE.get(dkey)
+    if d is None:
+        if len(_DESC_CACHE) > 4096:
+            _DESC_CACHE.clear()
+        d = _DESC_CACHE[dkey] = capi.ResBlockDesc(batch=B, channels=Cc, t=T, kernel=K, dilation=int(dilation), slope=float(slope),
+                                                  out_scale=float(out_scale), accumulate=int(bool(accumulate)))
+    L = capi.lib()
+    if not L.pwgb_resblock_pair_supported(C.byref(d)):
+        return None
+    w1, w2 = _dev(w1, "w1"), _dev(w2, "w2")
+    b1 = _dev(b1, "b1") if b1 is not None else None
+    b2 = _dev(b2, "b2") if b2 is not None else None
+    if out is None:
+        out = torch.empty_like(x)
+    pk1, pk2 = packed_weight(w1), packed_weight(w2)
+    # FLOPs of both convs; bytes: x once, out written (and read too when accumulating), the intermediate stays on chip
+    prof = _Prof("resblock_pair_tc", 2 * 2.0 * B * Cc * T * Cc * K, 4.0 * (x.numel() + out.numel() * (2 if accumulate else 1)),
+                 f"B{B} C{Cc} k{K} d{dilation} T{T}" if PROFILE is not None else "")
+    rc = L.pwgb_resblock_pair_forward(C.byref(d), _p(x), _p(pk1), _p(b1), _p(pk2), _p(b2), _p(out), _stream())
+    capi.check(rc, "pwgb_resblock_pair_forward")
+    prof.done()
+    return out
+
+
+def resblock_pair_plan(channels, t, kernel_size, dilation, batch=1):
+    """The fused pair's tile plan as a dict (output rows per tile, conv rows per tile, conv1 operand buffers, weight
+    stages, raw activation stages), or None when the pair keeps the two-launch path."""
+    d = capi.ResBlockDesc(batch=batch, channels=channels, t=t, kernel=kernel_size, dilation=dilation, slope=0.1, out_scale=1.0,
+                          accumulate=0)
+    v = (C.c_int * 5)()
+    if not capi.lib().pwgb_resblock_pair_plan(C.byref(d), v):
+        return None
+    return dict(zip(("M2", "TT", "na", "nb", "ns"), list(v)))
+
+
 def conv_transpose1d_raw(x, w, bias=None, *, stride, padding=0, output_padding=0, pre_slope=1.0, groups=1, period=1):
     """ConvTranspose1d with fused pre-LeakyReLU -- pwgb_conv_transpose1d_forward.
     w is the reference layout (cin, cout, k)."""

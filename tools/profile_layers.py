@@ -1,6 +1,7 @@
 """Per-launch table of the HiFi-GAN v1 C2 forward (CUDA events on the launching stream).  For conv1d_tc launches the
 last column is the tile plan: MT (64-row blocks per warpgroup), na / nb / ns (operand buffers, weight stages, raw
-activation stages) and whether the epilogue went through the shared-memory tile (staged) or registers."""
+activation stages) and whether the epilogue went through the shared-memory tile (staged) or registers.  For fused ResBlock
+pairs (resblock_pair_tc) it is the output / conv rows per tile, conv1 operand buffers, weight stages and raw stages."""
 import ctypes as C
 import os
 import sys
@@ -26,6 +27,11 @@ def _done_with_plan(self):
         v = (C.c_int * 5)()
         if capi.lib().pwgb_debug_get(1, C.cast(v, C.c_void_p), C.sizeof(v)) == 0:
             plans[len(ops.PROFILE) - 1] = f"MT{v[0]} na{v[1]} nb{v[2]} ns{v[3]} {'staged' if v[4] else 'reg'}"
+    elif ops.PROFILE is not None and self.name == "resblock_pair_tc":
+        # desc "B.. C.. k.. d.. T..": the plan is a function of the shape
+        f = {s[0]: int(s[1:]) for s in self.desc.split()}
+        pl = ops.resblock_pair_plan(f["C"], f["T"], f["k"], f["d"], batch=f["B"])
+        plans[len(ops.PROFILE) - 1] = f"rows {pl['M2']}/{pl['TT']} na{pl['na']} nb{pl['nb']} ns{pl['ns']}"
 
 
 ops._Prof.done = _done_with_plan
