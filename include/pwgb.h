@@ -119,7 +119,9 @@ PWGB_API int pwgb_conv_transpose1d_forward(const pwgb_convtr1d_desc* d, const fl
  * ---------------------------------------------------------------------- */
 /* measurement aids (not part of the product contract): set key 1 = conv variant (value 2: stage activations with
  * cp.async instead of TMA; value 4: register epilogue instead of the staged one); get key 1 copies the plan of the last
- * tensor-core conv launch, 5 ints {MT, na, nb, ns, staged}, and returns 0 (-1 for any other key or a short buffer). */
+ * tensor-core conv launch, 8 ints {MT, na, nb, ns, staged, tma_act, win_mode, nco} (a buffer of at least 5 ints gets
+ * the leading min(bytes, 32) bytes); get key 2 copies the plan of the last tensor-core weight-gradient launch, 4 ints
+ * {nc, tg, ntg, nsplit}.  Returns 0, or -1 for any other key or a short buffer. */
 PWGB_API void pwgb_debug_set(int key, int value);
 PWGB_API int pwgb_debug_get(int key, void* dst, size_t bytes);
 PWGB_API size_t pwgb_conv1d_tc_packed_weight_bytes(int cin, int cout, int kernel);

@@ -673,11 +673,18 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 }
 
 static int g_tc_variant = 0;
-// the plan of the last conv1d_tc_kernel launch, for pwgb_debug_get(1, ...)
+// the plan of the last conv1d_tc_kernel launch, for pwgb_debug_get(1, ...); the first five fields are the original
+// readout, so a caller that asks for five ints keeps working
 struct TcPlanInfo {
   int MT, na, nb, ns, staged;
+  int tma_act, win_mode, nco;
 };
 static TcPlanInfo g_tc_last = {};
+// the plan of the last wgrad_tc_kernel launch, for pwgb_debug_get(2, ...)
+struct WtPlanInfo {
+  int nc, tg, ntg, nsplit;
+};
+static WtPlanInfo g_wt_last = {};
 
 // aux_c2: channels of the auxiliary 1x1 source (0 = none, else multiple of KC); split > 0 selects the
 // WaveNet epilogue.  pre_gate: d->cin is the number of gated channels, x holds 2*cin channels.
@@ -858,7 +865,7 @@ static int tc_launch(TcK& p, size_t bytes, const float* x, const void* packed_w,
     p.tma_act = 0;  // unaligned base pointer: the producers stage with cp.async instead
   if (p.staged && ((reinterpret_cast<uintptr_t>(y) & 15) || (reinterpret_cast<uintptr_t>(residual) & 15)))
     p.staged = 0;  // bulk copies need 16-byte aligned rows: the register epilogue (the plan's tiles stay unused)
-  g_tc_last = TcPlanInfo{p.MT, p.na, p.nb, p.ns, p.staged};
+  g_tc_last = TcPlanInfo{p.MT, p.na, p.nb, p.ns, p.staged, p.tma_act, p.win_mode, p.nco};
   const int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
   kernel<<<(unsigned)grid, TC_THREADS, bytes, st>>>(p, x, x2, (const uint4*)packed_w, bias, residual, y, y2);
   return check_launch("conv1d_tc_kernel");
@@ -902,10 +909,16 @@ extern "C" void pwgb_debug_set(int key, int value) {
   if (key == 1) g_tc_variant = value;
 }
 
-// key 1: the plan of the last conv1d_tc launch as 5 ints {MT, na, nb, ns, staged}
+// key 1: the plan of the last conv1d_tc launch, {MT, na, nb, ns, staged, tma_act, win_mode, nco};
+// key 2: the plan of the last conv1d_wgrad_tc launch, {nc, tg, ntg, nsplit}.
+// Copies min(bytes, size of the record); a buffer of at least 5 (key 1) or 4 (key 2) ints is required.
 extern "C" int pwgb_debug_get(int key, void* dst, size_t bytes) {
-  if (key != 1 || !dst || bytes < sizeof(TcPlanInfo)) return -1;
-  memcpy(dst, &g_tc_last, sizeof(TcPlanInfo));
+  if (!dst) return -1;
+  const void* src = key == 1 ? (const void*)&g_tc_last : key == 2 ? (const void*)&g_wt_last : nullptr;
+  const size_t size = key == 1 ? sizeof(TcPlanInfo) : sizeof(WtPlanInfo);
+  const size_t need = key == 1 ? 5 * sizeof(int) : sizeof(WtPlanInfo);
+  if (!src || bytes < need) return -1;
+  memcpy(dst, src, bytes < size ? bytes : size);
   return 0;
 }
 
@@ -1399,6 +1412,7 @@ extern "C" int pwgb_conv1d_wgrad_tc(const pwgb_conv1d_desc* d, const float* x, c
     }
     attr_set = true;
   }
+  g_wt_last = WtPlanInfo{p.nc, p.tg, p.ntg, p.nsplit};
   dim3 grid(p.G * ceil_div(p.Cout_g, 128), (p.Cin_g / p.nc) * p.ntg, p.nsplit);
   if (p.nc == 64)
     wgrad_tc_kernel<64><<<grid, WT_THREADS, smem, st>>>(p, x, gy, (float*)ws);

@@ -5,6 +5,7 @@ checks that its tensors live on a CUDA device and raises otherwise -- there is n
 CPU path in this package.
 """
 import ctypes as C
+import math
 import os
 
 import torch
@@ -121,7 +122,7 @@ def conv1d_raw(
     if w.dim() == 4:  # Conv2d (k, 1) weights of the period discriminators
         w = w.reshape(w.shape[0], w.shape[1], w.shape[2])
     B, cin_x = x.shape[0], x.shape[1]
-    L = x.numel() // max(B * cin_x, 1)
+    L = math.prod(x.shape[2:])  # from the shape, so that an empty batch keeps its length
     cout, cin_g, K = w.shape
     cin = cin_g * groups
     if cin_x != cin * (2 if pre_gate else 1):
@@ -153,8 +154,10 @@ def conv1d_raw(
         residual = _dev(residual, "residual")
         if residual.numel() != out.numel():
             raise PwgbError("conv1d: residual shape mismatch")
-        if residual.data_ptr() == out.data_ptr():
+        if out.numel() and residual.data_ptr() == out.data_ptr():
             raise PwgbError("conv1d: residual must not alias out")
+    if out.numel() == 0:
+        return out  # an empty batch: nothing to compute (and no device pointers to pass)
     if bias is not None:
         bias = _dev(bias, "bias")
     # descriptors are immutable on the C side: one ctypes object per distinct configuration (building a 25-field
@@ -252,7 +255,7 @@ def conv_transpose1d_raw(x, w, bias=None, *, stride, padding=0, output_padding=0
         w = w.reshape(w.shape[0], w.shape[1], w.shape[2])
     B, cin = x.shape[0], x.shape[1]
     P = int(period)
-    t_in = x.numel() // max(B * cin * P, 1)
+    t_in = math.prod(x.shape[2:]) // P
     if w.shape[0] != cin:
         raise PwgbError(f"conv_transpose1d: x has {cin} channels, weight expects {w.shape[0]}")
     cout, K = w.shape[1] * groups, w.shape[2]
@@ -265,6 +268,8 @@ def conv_transpose1d_raw(x, w, bias=None, *, stride, padding=0, output_padding=0
     nbytes = L.pwgb_conv_transpose1d_workspace(C.byref(d))
     ws = torch.empty((nbytes + 3) // 4, device=x.device, dtype=torch.float32)
     y = torch.empty((B, cout, t_out) if P == 1 else (B, cout, t_out, P), device=x.device, dtype=torch.float32)
+    if y.numel() == 0:
+        return y  # an empty batch: nothing to compute
     prof = _Prof("conv_transpose1d", 2.0 * B * cout * t_out * cin * ((K + stride - 1) // stride), 4.0 * (x.numel() + y.numel()),
                  f"B{B} cin{cin} cout{cout} k{K} s{stride} T{t_out}")
     rc = L.pwgb_conv_transpose1d_forward(C.byref(d), _p(x), _p(w), _p(bias), _p(y), _p(ws), C.c_size_t(nbytes), _stream())
