@@ -199,3 +199,350 @@ def resblock_pair(x, w1, b1, w2, b2, *, kernel_size, dilation, slope, out_scale=
     h, ex1 = conv1d(x, w1, b1, padding=(k - 1) // 2 * d, dilation=d, pre_slope=slope)
     y, ex2 = conv1d(h, w2, b2, padding=(k - 1) // 2, pre_slope=slope, residual=x, out_scale=out_scale, prev=prev)
     return y, ex1 & ex2
+
+
+# ---------------------------------------------------------------------------------------------------- WaveNet layer
+# Both tensor-core forms of the WaveNet residual layer (residual_block.py:102-140):
+#   g  = conv_{K,d}(x) + W_aux c [+ b]    bf16x3, one fp32 accumulation (the aux 1x1 is extra K chunks)
+#   z  = tanh(g[:H]) * sigmoid(g[H:])     the only inexact step: ex2.approx / div.approx (fused form, gate_fast) or
+#                                         tanhf / __expf (two-launch form, the pre_gate producer)
+#   so = bf16x3(split(z)) . [W_skip ; W_out]
+#   skips (+)= so[:S] + b_skip ;  x' = (so[S:] + b_out + x) * fl32(sqrt(1/2))
+# The fused form adds the conv bias inside the gate (one fma into the ex2 argument), reads x as its packed x_hi + x_lo
+# and writes x' split into packed hi / lo words.
+SQRT_HALF = float(np.float32(math.sqrt(0.5)))     # `rs` / `out_scale` of both forms
+LOG2E2 = float(np.float32(2.8853900817779268))    # gate_fast: a-half factor 2 log2(e) in fp32
+NLOG2E = float(np.float32(-1.4426950408889634))   # gate_fast: b-half factor -log2(e) in fp32
+CLAMP_A = float(np.float32(43.28))                # gate_fast: clamp of the a-half ex2 argument
+U32 = 2.0 ** -24                                   # unit roundoff of fp32 round to nearest
+U_BF16 = 2.0 ** -8                                 # unit roundoff of bf16 round to nearest
+
+
+def gate_fp64(a, b):
+    """tanh(a) * sigmoid(b) in fp64"""
+    a, b = a.double(), b.double()
+    return torch.tanh(a) * torch.sigmoid(b)
+
+
+# Gate inputs on which the device gate is exactly known (the identities that tests/test_gpu_wavenet_exact.py reads back
+# on the device).  fused: gate_fast(0, .) = 0, gate_fast(-64, 128) = -1, gate_fast(-64, 0) = -0.5;
+# two-launch: tanhf(0) = 0, tanhf(+-20) = +-1, sigmoidf_(20) = 1, sigmoidf_(0) = 0.5, sigmoidf_(-100) = 0.
+EXACT_TANH = {"fused": {0.0: 0.0, -64.0: -1.0}, "two": {0.0: 0.0, 20.0: 1.0, -20.0: -1.0}}
+EXACT_SIGMOID = {"fused": {0.0: 0.5, 128.0: 1.0}, "two": {20.0: 1.0, 0.0: 0.5, -100.0: 0.0}}
+
+
+def gate_table(form):
+    """The gate of ``form`` ("fused" / "two") on its exact classes: a function (a, b) -> z (fp64) that raises when an
+    element is outside the table.  In the fused form a = 0 gives z = 0 for any b (ex2(0) - 1 = 0)."""
+    ta, sg = EXACT_TANH[form], EXACT_SIGMOID[form]
+
+    def gate(a, b):
+        a, b = a.double(), b.double()
+        za = torch.full_like(a, math.nan)
+        sb = torch.full_like(b, math.nan)
+        for k, v in ta.items():
+            za[a == k] = v
+        for k, v in sg.items():
+            sb[b == k] = v
+        z = za * sb
+        if form == "fused":
+            z[a == 0] = 0.0
+        assert not torch.isnan(z).any(), f"gate input outside the exact {form} classes"
+        return z
+
+    return gate
+
+
+def _same_pad(k, d):
+    p = (k - 1) // 2 * d
+    return (p, p)
+
+
+def _bf16x3_acc(a, w, kw, drop_lo_hi=False, lolo=False):
+    """fp64 sum of a_hi w_hi + a_lo w_hi + a_hi w_lo (F.conv1d with ``kw``), its magnitude bound and grid;
+    ``drop_lo_hi`` leaves out a_lo w_hi, ``lolo`` adds a_lo w_lo"""
+    ah, al = (t.double() for t in split(a))
+    wh, wl = (t.double() for t in split(w))
+    acc = F.conv1d(ah, wh, **kw) + F.conv1d(ah, wl, **kw)
+    if not drop_lo_hi:
+        acc = acc + F.conv1d(al, wh, **kw)
+    if lolo:
+        acc = acc + F.conv1d(al, wl, **kw)
+    bound = F.conv1d(ah.abs() + al.abs(), wh.abs() + wl.abs(), **kw)
+    return acc, bound, _term_grid(ah, al, wh, wl)
+
+
+@dataclass
+class WaveNetResult:
+    """One emulated layer: fp32 g (two-launch: with the conv bias; fused: the accumulator, without it), z (fp64, the
+    gate's value before the split), skips, x' and, for the fused form, xw = x' split as the kernel writes it (hi + lo
+    values, fp32); an Exactness record per stage: ex_g (conv + aux [+ bias]), ex_skip, ex_x."""
+
+    g: torch.Tensor
+    z: torch.Tensor
+    skips: torch.Tensor
+    x: torch.Tensor
+    xw: torch.Tensor
+    ex_g: Exactness
+    ex_skip: Exactness
+    ex_x: Exactness
+
+    @property
+    def ex(self):
+        return self.ex_g & self.ex_skip & self.ex_x
+
+
+def wavenet_layer(x, c, w_conv, b_conv, w_aux, w_skip, b_skip, w_out, b_out, *, dilation, form, gate=None, skips=None,
+                  skips_init=False, drop=(), lolo=False):
+    """fp64 emulation of one WaveNet layer in the kernels' order, ``form`` "two" (pwgb_wavenet_layer_forward: two
+    conv1d_tc launches) or "fused" (pwgb_wnstack_layer_forward).  Shapes: x (B, R, T), c (B, A, T) or None, w_conv
+    (G, R, K), w_aux (G, A[, 1]), w_skip (S, H[, 1]), w_out (R, H[, 1]), biases 1-D or None, skips (B, S, T) or None
+    (zeros).  ``gate(a, b)`` -> z in fp64 (default: tanh * sigmoid in fp64, rounded to fp32 as the kernels hold z);
+    a and b include the conv bias.  The two-launch form always accumulates into skips; the fused form overwrites them
+    when ``skips_init``.  ``drop`` names terms to leave out, to emulate broken kernels: "x_lo_w_hi" (conv),
+    "z_lo_w_hi" (skip / out), "x_lo" (the fused residual reads x_hi only).  ``lolo`` adds both dropped lo*lo terms."""
+    assert form in ("two", "fused")
+    B, R, T = x.shape
+    G, _, K = w_conv.shape
+    H = G // 2
+    S = w_skip.shape[0]
+    acc, bound, g_grid = _bf16x3_acc(x, w_conv, dict(padding=_same_pad(K, dilation)[0], dilation=dilation),
+                                     "x_lo_w_hi" in drop, lolo)
+    if c is not None:
+        a2, b2, gg2 = _bf16x3_acc(c, w_aux.reshape(G, -1, 1), {}, False, lolo)
+        acc, bound, g_grid = acc + a2, bound + b2, min(g_grid, gg2)
+    if form == "two":
+        g32, ex_g = _epilogue(acc, bound, g_grid, b_conv, None, 1.0, None, 1.0, None)
+        a, b = g32[:, :H].double(), g32[:, H:].double()
+    else:
+        g32, ex_g = _epilogue(acc, bound, g_grid, None, None, 1.0, None, 1.0, None)
+        bc = torch.zeros(G, dtype=torch.float64) if b_conv is None else b_conv.double()
+        a = g32[:, :H].double() + bc[:H].reshape(1, -1, 1)
+        b = g32[:, H:].double() + bc[H:].reshape(1, -1, 1)
+    z = gate_fp64(a, b).float().double() if gate is None else gate(a, b)
+    w_so = torch.cat([w_skip.reshape(S, H), w_out.reshape(R, H)]).reshape(S + R, H, 1)
+    so, so_bound, so_grid = _bf16x3_acc(z.float(), w_so, {}, "z_lo_w_hi" in drop, lolo)
+    bso = None if b_skip is None else torch.cat([b_skip.reshape(-1), b_out.reshape(-1)])
+    b_s, b_o = (None, None) if bso is None else (bso[:S], bso[S:])
+    prev = None if (form == "fused" and skips_init) else (torch.zeros(B, S, T) if skips is None else skips)
+    sk, ex_skip = _epilogue(so[:, :S], so_bound[:, :S], so_grid, b_s, None, 1.0, None, 1.0, prev)
+    if form == "fused":
+        xh, xl = split(x)
+        res = xh.double() if "x_lo" in drop else xh.double() + xl.double()
+    else:
+        res = x
+    xo, ex_x = _epilogue(so[:, S:], so_bound[:, S:], so_grid, b_o, None, 1.0, res, SQRT_HALF, None)
+    hi, lo = split(xo)
+    return WaveNetResult(g32, z, sk, xo, hi + lo, ex_g, ex_skip, ex_x)
+
+
+def pack_words(x, halo, t_pad):
+    """The packed hi / lo image of fp32 x (B, C, T) that wn_pack_kernel / wn_first_conv_kernel write: int32 words of
+    [B][hi|lo][ceil(C/8)][t_pad][8 ch] bf16 (two channels per word, the even one in the low half), samples in rows
+    [halo, halo + T), every other row and every channel >= C zero.  Returned flat, as the device buffer."""
+    B, Cc, T = x.shape
+    ng = (Cc + 7) // 8
+    if B == 0:
+        return torch.zeros(0, dtype=torch.int32)
+    hi, lo = split(x)
+    img = torch.zeros(B, 2, ng * 8, t_pad, dtype=torch.bfloat16)
+    img[:, 0, :Cc, halo:halo + T] = hi.to(torch.bfloat16)
+    img[:, 1, :Cc, halo:halo + T] = lo.to(torch.bfloat16)
+    img = img.reshape(B, 2, ng, 8, t_pad).permute(0, 1, 2, 4, 3).contiguous()
+    return img.view(torch.int16).view(torch.int32).reshape(-1)
+
+
+def unpack_words(words, B, Cc, halo, t_pad, T):
+    """inverse of pack_words: hi + lo of rows [halo, halo + T) as fp32 (B, Cc, T)"""
+    ng = (Cc + 7) // 8
+    if B == 0:
+        return torch.zeros(0, Cc, T)
+    img = words.reshape(-1).view(torch.int16).view(torch.bfloat16).reshape(B, 2, ng, t_pad, 8).float()
+    v = img[:, 0] + img[:, 1]
+    return v.permute(0, 1, 3, 2).reshape(B, ng * 8, t_pad)[:, :Cc, halo:halo + T].contiguous()
+
+
+def fits_split(t):
+    """every value survives the hi / lo split: hi + lo == t"""
+    hi, lo = split(t)
+    return bool(torch.equal(hi + lo, t.float()))
+
+
+def zero_target_data(gen, B, R, G, S, T, K, dilation, *, lo_on="x", scale_w=2.0 ** -3, max_tries=64):
+    """Data on which g == 0 exactly: W_aux = -I (A = G) and c = the bf16x3 conv of x, so the conditioning 1x1 cancels
+    the conv at every element.  x and W_conv are grid values with lo parts on ``lo_on`` ("x" or "w") only; b_conv = 0
+    (the fused kernel folds it into the ex2 argument); W_skip / W_out / b_skip / b_out / prior skips are grid values.
+    Every c must survive the hi / lo split (c is fed through it); data that do not are redrawn from the same generator.
+    Returns a dict of the layer's inputs."""
+    for _ in range(max_tries):
+        x = grid_values((B, R, T), gen, 1.0, hmax=1, lo=lo_on == "x")
+        w = grid_values((G, R, K), gen, scale_w, hmax=1, lo=lo_on == "w")
+        acc, bound, g = _bf16x3_acc(x, w, dict(padding=_same_pad(K, dilation)[0], dilation=dilation))
+        c = acc.float()
+        if not (torch.equal(c.double(), acc) and fits_split(c) and Exactness(float(bound.max()), g).ok):
+            continue
+        return dict(x=x, c=c, w_conv=w, b_conv=None, w_aux=-torch.eye(G), **_so_data(gen, R, G, S, B, T))
+    raise AssertionError("zero_target_data: no draw survives the split")
+
+
+def _so_data(gen, R, G, S, B, T):
+    H = G // 2
+    return dict(w_skip=grid_values((S, H), gen, 2.0 ** -2, hmax=3), w_out=grid_values((R, H), gen, 2.0 ** -2, hmax=3),
+                b_skip=grid_values((S,), gen, 2.0 ** -1, hmax=3), b_out=grid_values((R,), gen, 2.0 ** -1, hmax=3),
+                skips=grid_values((B, S, T), gen, 1.0, hmax=3))
+
+
+def saturated_data(gen, B, R, G, S, T, form):
+    """Data on which every gate input is in an exact class of ``form`` (EXACT_TANH / EXACT_SIGMOID): W_conv = 0,
+    W_aux = I (A = G), b_conv = 0 and c drawn from the classes, so z is exactly 0, +-0.5 or +-1 (fused: 0, -0.5, -1).
+    x, W_skip / W_out, the biases and prior skips are grid values.  Returns a dict of the layer's inputs."""
+    H = G // 2
+    ka = torch.tensor(sorted(EXACT_TANH[form]))
+    kb = torch.tensor(sorted(EXACT_SIGMOID[form]))
+    c = torch.cat([ka[torch.randint(0, len(ka), (B, H, T), generator=gen)],
+                   kb[torch.randint(0, len(kb), (B, H, T), generator=gen)]], 1).float()
+    assert fits_split(c)
+    x = grid_values((B, R, T), gen, 1.0, hmax=3)
+    return dict(x=x, c=c, w_conv=torch.zeros(G, R, 3), b_conv=None, w_aux=torch.eye(G), **_so_data(gen, R, G, S, B, T))
+
+
+def bound_data(gen, B, R, G, S, A, T, K=3, hmax=2):
+    """Bound-regime data (fused form): grid x, c, W_conv, W_aux and a nonzero grid conv bias, so that g is exact and
+    spreads over the whole gate range, saturation included.  W_skip / W_out are readout weights: one nonzero power of
+    two per row, so that the skip / out contraction is exact for any z and gate_bound isolates the gate."""
+    H = G // 2
+
+    def readout(n):
+        w = torch.zeros(n, H)
+        h = torch.randint(0, H, (n,), generator=gen)
+        s = torch.randint(0, 2, (n,), generator=gen) * 2 - 1
+        e = torch.randint(0, 4, (n,), generator=gen)
+        w[torch.arange(n), h] = s.float() * torch.exp2(e.float())
+        return w
+
+    x = grid_values((B, R, T), gen, 1.0, hmax=hmax)
+    c = grid_values((B, A, T), gen, 1.0, hmax=hmax)
+    return dict(x=x, c=c, w_conv=grid_values((G, R, K), gen, 2.0 ** -3, hmax=hmax),
+                b_conv=grid_values((G,), gen, 2.0 ** -1, hmax=3), w_aux=grid_values((G, A), gen, 2.0 ** -3, hmax=hmax),
+                w_skip=readout(S), w_out=readout(R), b_skip=grid_values((S,), gen, 2.0 ** -3, hmax=1, zero_frac=0.5),
+                b_out=grid_values((R,), gen, 2.0 ** -1, hmax=3),
+                skips=grid_values((B, S, T), gen, 2.0 ** -3, hmax=1, zero_frac=0.5))
+
+
+EPS_EX2 = 2.0 ** -22   # ex2.approx.ftz.f32: relative error budget
+EPS_DIV = 2.0 ** -22   # __fdividef (div.approx): 2 ulp for 2^-126 <= |d| <= 2^126
+
+
+def gate_fast_bound(ga, gb, ba, bb):
+    """Per-element bound on |gate_fast(ga, gb) - tanh(ga + ba) sigmoid(gb + bb)| for the fused kernel's gate
+    (wavenet_tc.cu: z = (Ea - 1) / ((Ea + 1)(1 + Eb)), Ea = ex2(min(pa, 43.28)), Eb = ex2(pb)), from these per-step
+    budgets:
+      - the ex2 arguments pa = RN(fma(ga, fl(2 log2 e), RN(ba fl(2 log2 e)))) (pb the same with -log2 e) differ from
+        the exact 2 log2(e) a by (|ga| + |ba|) |fl(2 log2 e) - 2 log2 e|, plus one fp32 rounding of the bias product and
+        one of the fma (2^-24 of their magnitudes);
+      - ex2.approx has relative error EPS_EX2 and an argument error dp scales its result by 2^dp, so the device's Ea lies
+        in Ea (1 +- rho_a), rho_a = (2^(|dp|) - 1) + EPS_EX2 (times 1.01 for the product of the two), Eb likewise;
+      - t = (Ea - 1) / (Ea + 1) and s = 1 / (1 + Eb) are monotone in Ea and Eb, so the exact t s over those intervals
+        is bounded by the corner values (this keeps the correlated error of Ea in numerator and denominator exact);
+      - N = Ea - 1, D1 = Ea + 1, D2 = 1 + Eb and D = D1 D2 round once each to fp32.  A rounding is at most 2^-24 of
+        its result, and at most the distance to an fp32 candidate: Ea (or 1) is one, so N and D1 move by at most 1 and
+        D2 by at most Eb.  Relative: min(2^-24, 1 / |N|) + min(2^-24, 1 / D1) + min(2^-24, Eb / D2) + 2^-24, and the
+        quotient costs EPS_DIV;
+      - the clamp at 43.28 replaces tanh by t(2^43.28): that difference is computed exactly;
+      - ftz: an ex2 result below 2^-126 is 0 (an absolute 2^-118 where pa < -120);
+      - where D may exceed 2^125, __fdividef may return 0 (and ex2 may overflow): there the bound is |z| + 2^-100.
+    Inputs: fp64 tensors of the accumulator halves (ga, gb, without bias) and the conv bias halves (ba, bb) broadcast
+    to them."""
+    ga, gb, ba, bb = (t.double() for t in (ga, gb, ba, bb))
+    a, b = ga + ba, gb + bb
+    z = gate_fp64(a, b)
+    ln2 = math.log(2.0)
+
+    def arg_err(g, bias, cf, c):
+        pb_ = bias * cf
+        return (g.abs() + bias.abs()) * abs(cf - c) + U32 * pb_.abs() + U32 * (g * cf + pb_).abs()
+
+    c1, c2 = 2.0 / ln2, -1.0 / ln2
+    pa = torch.clamp(c1 * a, max=CLAMP_A)
+    pb = c2 * b
+    ea, eb = torch.exp2(pa), torch.exp2(torch.clamp(pb, max=1000.0))
+    ra = (torch.exp2(arg_err(ga, ba, LOG2E2, c1)) - 1 + EPS_EX2) * 1.01
+    rb = (torch.exp2(arg_err(gb, bb, NLOG2E, c2)) - 1 + EPS_EX2) * 1.01
+
+    def t_of(e):
+        return (e - 1) / (e + 1)
+
+    def s_of(e):
+        return 1 / (1 + e)
+
+    ts = [t_of(ea * (1 - ra)), t_of(ea * (1 + ra))]
+    ss = [s_of(eb * (1 - rb)), s_of(eb * (1 + rb))]
+    ideal = t_of(ea) * s_of(eb)
+    corner = torch.stack([(t * s - ideal).abs() for t in ts for s in ss]).amax(0)
+    mag = torch.stack([(t * s).abs() for t in ts for s in ss]).amax(0)
+    ea_lo = ea * (1 - ra)
+    rnd = (torch.clamp(1 / (ea_lo - 1).abs(), max=U32) + torch.clamp(1 / (ea_lo + 1), max=U32)
+           + torch.clamp(eb * (1 + rb) / (1 + eb), max=U32) + U32 + EPS_DIV)
+    e = corner + mag * rnd * 1.01 + (z - ideal).abs() + 2.0 ** -50 * z.abs() + 2.0 ** -100
+    e = e + torch.where(pa < -120, torch.full_like(e, 2.0 ** -118), torch.zeros_like(e))
+    huge = ((ea + 1) * (1 + eb) > 2.0 ** 125) | (pb > 125)
+    return torch.where(huge, z.abs() + 2.0 ** -100, e)
+
+
+def split_bound(v, e):
+    """bound on |hi(w) + lo(w) - v| for any fp32 w with |w - v| <= e: |w - hi(w)| <= |v - hi(v)| + e (hi(w) is the
+    bf16 nearest to w), lo rounds that remainder to 8 bits"""
+    v = v.double()
+    vh = v.float().to(torch.bfloat16).double()
+    return e + U_BF16 * ((v - vh).abs() + e)
+
+
+def gate_bound(d, dilation):
+    """Per-element bounds (skips, x') of the fused layer on bound_data ``d`` (readout W_skip / W_out, skips_init False)
+    against the fp64 layer with exact gate: skips_ref = w z + b_skip + skips, x'_ref = ((w z + b_out) + x) fl(sqrt 1/2).
+    Derivation, per element:
+      - g is exact (guarded), so the gate input error is the gate's own: e_z = gate_fast_bound;
+      - the kernel contracts split(z_dev): |hi + lo - z| <= e_S = split_bound(z, e_z);
+      - one nonzero power-of-two weight per row: so = w (hi + lo) exactly, error |w| e_S;
+      - every later fp32 operation (+ b, + prior skips / + x_hi, + x_lo, * rs) adds at most 2^-24 of its result's
+        magnitude (reference magnitude plus the error so far), an addition also at most its exact addend (zero biases
+        and prior skips, which bound_data draws often, add nothing);
+      - x' is written split: compare hi + lo of the words, split_bound again.
+    Returns (bound_skips, bound_x, ref_skips, ref_x) as fp64 tensors."""
+    x, c, w_conv, b_conv, w_aux = d["x"], d["c"], d["w_conv"], d["b_conv"], d["w_aux"]
+    G, R, K = w_conv.shape
+    H = G // 2
+    S = d["w_skip"].shape[0]
+    emu = wavenet_layer(x, c, w_conv, b_conv, w_aux, d["w_skip"], d["b_skip"], d["w_out"], d["b_out"], dilation=dilation,
+                        form="fused", gate=gate_fp64, skips=d["skips"])
+    emu.ex_g.check("gate_bound: g")
+    for w in (d["w_skip"], d["w_out"]):
+        nz = (w != 0).sum(1)
+        assert bool((nz == 1).all()), "gate_bound needs one nonzero weight per row"
+        m, _ = torch.frexp(w[w != 0])
+        assert bool((m.abs() == 0.5).all()), "gate_bound needs power-of-two readout weights"
+    g = emu.g.double()
+    bc = b_conv.double().reshape(1, -1, 1)
+    e_z = gate_fast_bound(g[:, :H], g[:, H:], bc[:, :H].expand_as(g[:, :H]), bc[:, H:].expand_as(g[:, H:]))
+    z = emu.z
+    e_s = split_bound(z, e_z)
+    W = torch.cat([d["w_skip"], d["w_out"]]).double()
+    so = torch.einsum("nh,bht->bnt", W, z)
+    e_so = torch.einsum("nh,bht->bnt", W.abs(), e_s)
+
+    def add(v, e, t):
+        """v + t in fp32 (v an fp32 value within e of the reference, t exact): value, error.  The rounding is at most
+        2^-24 of the result and at most |t| (v itself is a candidate)."""
+        r = v + t
+        return r, e + torch.minimum(U32 * (r.abs() + e), t.abs().expand_as(r))
+
+    bs, bo = d["b_skip"].double().reshape(1, -1, 1), d["b_out"].double().reshape(1, -1, 1)
+    v, e = add(so[:, :S], e_so[:, :S], bs)
+    sk, e_sk = add(v, e, d["skips"].double())
+    xh, xl = (t.double() for t in split(x))
+    v, e = add(so[:, S:], e_so[:, S:], bo)
+    v, e = add(v, e, xh)
+    v, e = add(v, e, xl)
+    xo = v * SQRT_HALF
+    e = e * SQRT_HALF + U32 * (xo.abs() + e * SQRT_HALF)
+    return e_sk, split_bound(xo, e), sk, xo

@@ -1111,6 +1111,7 @@ extern "C" int pwgb_wavenet_layer_forward(const pwgb_wavenet_desc* d, const floa
                                           const void* packed, const float* b_conv, const float* b_skip_out,
                                           float* x_out, float* skips, float* g_ws, void* stream) {
   PWGB_UNSUPPORTED_IF(!pwgb_wavenet_supported(d), "wavenet_layer: configuration not supported by the tensor-core path");
+  if (d->batch == 0) return PWGB_OK;  // an empty batch: no launch (and the empty tensors have no storage)
   PWGB_CHECK_ARG(x && packed && x_out && skips && g_ws && (c || d->aux_channels == 0), "wavenet_layer: null argument");
   PWGB_CHECK_ARG(x != x_out, "wavenet_layer: x_out must not alias x (halo reads)");
   cudaStream_t st = (cudaStream_t)stream;

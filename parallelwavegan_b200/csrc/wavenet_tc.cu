@@ -408,8 +408,8 @@ extern "C" int pwgb_wnstack_pack_x(const pwgb_wnstack_desc* d, const float* x, v
   WnK p;
   size_t bytes;
   PWGB_UNSUPPORTED_IF(!wn_plan(d, p, bytes), "wnstack: configuration not supported");
+  if (p.B == 0) return PWGB_OK;  // an empty batch: nothing to pack (and the empty tensors have no storage)
   PWGB_CHECK_ARG(x && xpk, "wnstack_pack_x: null argument");
-  if (p.B == 0) return PWGB_OK;
   wn_pack_kernel<<<wn_grid(p.T, p.ngx, p.B), 256, 0, (cudaStream_t)stream>>>(x, (long long)p.R * p.T, p.R, p.T, (uint4*)xpk, p.ngx, p.Tp,
                                                                             p.halo, 0);
   return check_launch("wn_pack_kernel");
@@ -419,8 +419,8 @@ extern "C" int pwgb_wnstack_pack_c(const pwgb_wnstack_desc* d, const float* c, l
   WnK p;
   size_t bytes;
   PWGB_UNSUPPORTED_IF(!wn_plan(d, p, bytes), "wnstack: configuration not supported");
-  PWGB_CHECK_ARG(c && cpk && c_batch_stride >= (long long)p.A * p.T, "wnstack_pack_c: bad argument");
   if (p.B == 0) return PWGB_OK;
+  PWGB_CHECK_ARG(c && cpk && c_batch_stride >= (long long)p.A * p.T, "wnstack_pack_c: bad argument");
   wn_pack_kernel<<<wn_grid(p.Tc, p.ngc, p.B), 256, 0, (cudaStream_t)stream>>>(c, c_batch_stride, p.A, p.T, (uint4*)cpk, p.ngc, p.Tc, 0, 1);
   return check_launch("wn_pack_kernel");
 }
@@ -429,8 +429,8 @@ extern "C" int pwgb_wnstack_unpack_x(const pwgb_wnstack_desc* d, const void* xpk
   WnK p;
   size_t bytes;
   PWGB_UNSUPPORTED_IF(!wn_plan(d, p, bytes), "wnstack: configuration not supported");
-  PWGB_CHECK_ARG(x && xpk, "wnstack_unpack_x: null argument");
   if (p.B == 0) return PWGB_OK;
+  PWGB_CHECK_ARG(x && xpk, "wnstack_unpack_x: null argument");
   wn_unpack_kernel<<<wn_grid(p.T, p.ngx, p.B), 256, 0, (cudaStream_t)stream>>>((const uint4*)xpk, p.ngx, p.Tp, p.halo, x, p.R, p.T);
   return check_launch("wn_unpack_kernel");
 }
@@ -440,8 +440,9 @@ extern "C" int pwgb_wnstack_first_conv(const pwgb_wnstack_desc* d, const float* 
   WnK p;
   size_t bytes;
   PWGB_UNSUPPORTED_IF(!wn_plan(d, p, bytes), "wnstack: configuration not supported");
-  PWGB_CHECK_ARG(z && w && xpk && in_channels > 0, "wnstack_first_conv: bad argument");
+  PWGB_CHECK_ARG(in_channels > 0, "wnstack_first_conv: bad argument");
   if (p.B == 0) return PWGB_OK;
+  PWGB_CHECK_ARG(z && w && xpk, "wnstack_first_conv: bad argument");
   wn_first_conv_kernel<<<wn_grid(p.T, p.ngx, p.B), 256, 0, (cudaStream_t)stream>>>(z, in_channels, w, bias, p.T, (uint4*)xpk, p.ngx, p.Tp,
                                                                                   p.halo);
   return check_launch("wn_first_conv_kernel");
@@ -453,14 +454,14 @@ extern "C" int pwgb_wnstack_layer_forward(const pwgb_wnstack_desc* d, int dilati
   WnK p;
   size_t bytes = 0;
   PWGB_UNSUPPORTED_IF(!wn_plan(d, p, bytes), "wnstack: configuration not supported by the fused tensor-core layer");
-  PWGB_CHECK_ARG(xpk_in && cpk && packed_w && skips, "wnstack_layer: null argument");
   PWGB_CHECK_ARG(dilation > 0 && (long long)(d->kernel / 2) * dilation <= d->halo, "wnstack_layer: dilation %d exceeds the halo %d of the packed stream",
                  dilation, d->halo);
+  if (p.B == 0) return PWGB_OK;  // an empty batch: no launch (and the empty buffers have no storage)
+  PWGB_CHECK_ARG(xpk_in && cpk && packed_w && skips, "wnstack_layer: null argument");
   PWGB_CHECK_ARG(xpk_in != xpk_out, "wnstack_layer: xpk_out must not alias xpk_in (other tiles read the halo)");
   PWGB_CHECK_ARG(!((reinterpret_cast<uintptr_t>(xpk_in) | reinterpret_cast<uintptr_t>(cpk) | reinterpret_cast<uintptr_t>(packed_w) |
                     reinterpret_cast<uintptr_t>(xpk_out)) & 15),
                  "wnstack_layer: packed buffers must be 16-byte aligned");
-  if (p.B == 0) return PWGB_OK;
   p.D = dilation;
   p.write_x = xpk_out != nullptr;
   p.skip_init = skips_init != 0;
