@@ -106,6 +106,26 @@ typedef struct pwgb_convtr1d_desc {
 PWGB_API size_t pwgb_conv_transpose1d_workspace(const pwgb_convtr1d_desc* d);
 PWGB_API int pwgb_conv_transpose1d_forward(const pwgb_convtr1d_desc* d, const float* x, const float* w, const float* bias,
                                   float* y, void* ws, size_t ws_bytes, void* stream);
+/* Two-source input (the skip concatenation of UHiFiGAN's decoder, models/uhifigan.py:289-291): the same conv-transpose
+ * on cat(x1, x2) along channels without materialising the concatenation.  d->cin = cin1 + cin2; x1 is
+ * (batch, cin1, t_in), x2 is (batch, cin2, t_in); w, bias, y, ws and the fused pre-LeakyReLU are those of
+ * pwgb_conv_transpose1d_forward on the concatenated input, and the result is bit-identical to it.
+ * pwgb_conv_transpose1d_cat_supported() returns 1 when the conv-transpose takes the tensor-core path and
+ * cin1 % 32 == 0 (dense, plain); otherwise concatenate and call pwgb_conv_transpose1d_forward. */
+PWGB_API int pwgb_conv_transpose1d_cat_supported(const pwgb_convtr1d_desc* d, int cin1);
+PWGB_API int pwgb_conv_transpose1d_cat_forward(const pwgb_convtr1d_desc* d, int cin1, const float* x1, const float* x2,
+                                      const float* w, const float* bias, float* y, void* ws, size_t ws_bytes, void* stream);
+
+/* ------------------------------------------------------------------------
+ * Dropout in training mode (torch.nn.Dropout(p); models/uhifigan.py input / downsample convs) over n elements.
+ * Element e is kept when word e % 4 of Philox4x32-10(counter = (e / 4, offset), key = seed), as a 24-bit uniform in
+ * [0, 1), is >= p; kept elements are multiplied by 1 / (1 - p) computed in fp32, the others are 0.  p == 0 is the
+ * identity.  The backward recomputes the same mask from (seed, offset): gx = mask * gy / (1 - p).
+ * ---------------------------------------------------------------------- */
+PWGB_API int pwgb_dropout_forward(const float* x, float* y, long long n, float p, unsigned long long seed,
+                                  unsigned long long offset, void* stream);
+PWGB_API int pwgb_dropout_backward(const float* gy, float* gx, long long n, float p, unsigned long long seed,
+                                   unsigned long long offset, void* stream);
 
 /* ------------------------------------------------------------------------
  * Tensor-core (Hopper wgmma) path for the wide stride-1 convolutions: same descriptor

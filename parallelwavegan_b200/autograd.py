@@ -167,6 +167,64 @@ def conv_transpose1d(x, w, bias=None, *, stride, padding=0, output_padding=0, pr
     return ConvTranspose1dFn.apply(x, w, bias, stride, padding, output_padding, float(pre_slope))
 
 
+class ConvTransposeCat1dFn(torch.autograd.Function):
+    """ConvTranspose1d on cat(x1, x2) along channels (UHiFiGAN's decoder skip path) without the concatenation in either
+    direction: the weight rows [0, cin1) only ever meet x1 and rows [cin1, cin) only x2, so each source gets its own
+    data gradient (the dgrad conv with its slice of the weight) and its own weight-gradient rows (the wgrad kernels on
+    that source alone); only the two small weight-gradient blocks are concatenated."""
+
+    @staticmethod
+    def forward(ctx, x1, x2, w, bias, stride, padding, output_padding, pre_slope):
+        y = ops.conv_transpose1d_cat_raw(x1, x2, w, bias, stride=stride, padding=padding, output_padding=output_padding,
+                                         pre_slope=pre_slope)
+        ctx.cfg = (stride, padding, pre_slope)
+        ctx.has_bias = bias is not None
+        ctx.save_for_backward(x1, x2, w)
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        x1, x2, w = ctx.saved_tensors
+        stride, padding, pre_slope = ctx.cfg
+        gy = gy.contiguous()
+        cin1 = x1.shape[1]
+        cin, cout, K = w.shape
+        gb = ops.bias_grad(gy, cout) if (ctx.has_bias and ctx.needs_input_grad[3]) else None
+        gw = None
+        if ctx.needs_input_grad[2]:
+            gw = torch.cat([ops.conv1d_wgrad(gy, x, (x.shape[1], cout, K), stride=stride, padding=padding, g_slope=pre_slope)
+                            for x in (x1, x2)])
+        gxs = []
+        for i, (x, wi) in enumerate(((x1, w[:cin1]), (x2, w[cin1:]))):
+            gx = None
+            if ctx.needs_input_grad[i]:
+                gx = ops.conv1d(gy, wi.detach(), None, stride=stride, padding=padding)
+                if gx.shape[-1] != x.shape[-1]:
+                    raise PwgbError("conv_transpose dgrad: length mismatch")
+                if pre_slope != 1.0:
+                    ops.act_backward("lrelu", gx, x, slope=pre_slope, out=gx)
+            gxs.append(gx)
+        return gxs[0], gxs[1], gw, gb, None, None, None, None
+
+
+def conv_transpose1d_cat(x1, x2, w, bias=None, *, stride, padding=0, output_padding=0, pre_slope=1.0):
+    return ConvTransposeCat1dFn.apply(x1, x2, w, bias, stride, padding, output_padding, float(pre_slope))
+
+
+class DropoutFn(torch.autograd.Function):
+    """Training-mode dropout; the backward recomputes the mask from the seed (pwgb_dropout_backward)."""
+
+    @staticmethod
+    def forward(ctx, x, p, seed):
+        ctx.cfg = (p, seed)
+        return ops.dropout_raw(x, p, seed)
+
+    @staticmethod
+    def backward(ctx, gy):
+        p, seed = ctx.cfg
+        return ops.dropout_raw(gy.contiguous(), p, seed, backward=True), None, None
+
+
 class S2DFn(torch.autograd.Function):
     """Space-to-depth along time (strided convs on the tensor-core path); backward = the adjoint gather."""
 

@@ -85,6 +85,14 @@ def lib():
     L.pwgb_conv_transpose1d_workspace.argtypes = [C.POINTER(ConvTr1dDesc)]
     L.pwgb_conv_transpose1d_forward.restype = C.c_int
     L.pwgb_conv_transpose1d_forward.argtypes = [C.POINTER(ConvTr1dDesc), vp, vp, vp, vp, vp, C.c_size_t, vp]
+    L.pwgb_conv_transpose1d_cat_supported.restype = C.c_int
+    L.pwgb_conv_transpose1d_cat_supported.argtypes = [C.POINTER(ConvTr1dDesc), C.c_int]
+    L.pwgb_conv_transpose1d_cat_forward.restype = C.c_int
+    L.pwgb_conv_transpose1d_cat_forward.argtypes = [C.POINTER(ConvTr1dDesc), C.c_int, vp, vp, vp, vp, vp, vp, C.c_size_t, vp]
+    L.pwgb_dropout_forward.restype = C.c_int
+    L.pwgb_dropout_forward.argtypes = [vp, vp, C.c_longlong, C.c_float, C.c_ulonglong, C.c_ulonglong, vp]
+    L.pwgb_dropout_backward.restype = C.c_int
+    L.pwgb_dropout_backward.argtypes = [vp, vp, C.c_longlong, C.c_float, C.c_ulonglong, C.c_ulonglong, vp]
     L.pwgb_conv1d_tc_packed_weight_bytes.restype = C.c_size_t
     L.pwgb_conv1d_tc_packed_weight_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
     L.pwgb_conv1d_tc_pack_weight.restype = C.c_int
@@ -233,6 +241,7 @@ def reset_launch_count():
 EXPORTED_SYMBOLS = [
     "pwgb_last_error", "pwgb_version", "pwgb_compiled_arch", "pwgb_launch_count", "pwgb_reset_launch_count",
     "pwgb_conv1d_forward", "pwgb_conv_transpose1d_workspace", "pwgb_conv_transpose1d_forward",
+    "pwgb_conv_transpose1d_cat_supported", "pwgb_conv_transpose1d_cat_forward", "pwgb_dropout_forward", "pwgb_dropout_backward",
     "pwgb_conv1d_tc_packed_weight_bytes", "pwgb_conv1d_tc_pack_weight", "pwgb_conv1d_tc_pack_weight_grouped",
     "pwgb_conv1d_tc_supported",
     "pwgb_conv1d_tc_forward", "pwgb_debug_set", "pwgb_debug_get",

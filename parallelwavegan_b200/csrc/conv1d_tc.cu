@@ -55,7 +55,8 @@ struct TcK {
   long long xbs, ybs, rbs;
   int a_bytes, b_bytes;  // per buffer / per stage
   int win_mode;          // 1: one TT-row window per tap (halo too large for a contiguous tile)
-  int nchunks2, C2;      // auxiliary 1x1 source (WaveNet conditioning): extra K=1 chunks
+  int nchunks2, C2;      // channels of x2: the auxiliary 1x1 source (WaveNet conditioning) of nchunks2 extra K=1 chunks, or,
+                         // with nchunks2 == 0, the last C2 of the Cin main input channels (two-source input; 0: x holds all)
   int pre_gate;          // producer computes tanh(x[c]) * sigmoid(x[c + Cin])
   int wavenet;           // epilogue: cols < split -> y2 += v ; cols >= split -> y = (v + res) * scale
   int split;
@@ -163,6 +164,15 @@ __device__ __forceinline__ void epi_store(const TcK& p, float a, int b, int t, i
 // Persistent: one CTA per SM loops over (batch, time-tile) work items; every role runs the same
 // tile sequence and talks through mbarriers only, so the loads of tile i+1 overlap the MMAs and the
 // epilogue of tile i.
+
+// First sample of main chunk c (input channels c*KC .. c*KC + KC) of batch item b.  A two-source conv (nchunks2 == 0,
+// C2 > 0) reads channels [0, Cin - C2) from x (B, Cin - C2, T_in) and [Cin - C2, Cin) from x2 (B, C2, T_in): the input
+// is cat(x, x2) without the copy.  KC divides C2, so a chunk never straddles the two.  goff: group offset.
+__device__ __forceinline__ const float* main_src(const TcK& p, const float* x, const float* x2, int b, int c, long long goff) {
+  const int ch = c * KC, c1 = p.Cin - p.C2;
+  if (p.nchunks2 == 0 && ch >= c1) return x2 + ((long long)b * p.C2 + (ch - c1)) * p.T_in;
+  return x + (long long)b * p.xbs + (long long)ch * p.T_in + goff;
+}
 
 // stage one activation chunk (KC channels x R rows) into the operand layout
 __device__ __forceinline__ void fill_main_chunk(const TcK& p, const float* __restrict__ xc, int t0, int TT,
@@ -347,7 +357,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       const int t0 = (tr - b * p.tiles_per_seq) * TT;
       const unsigned raw = smem_u32(raw_buf + (size_t)(q % p.ns) * p.raw_bytes);
       if (c < p.nchunks) {
-        const float* xc = x + (long long)b * p.xbs + (long long)(c * KC) * p.T_in + (MC ? (long long)((tile / pct) / p.cpg) * p.xgs : 0);
+        const float* xc = main_src(p, x, x2, b, c, MC ? (long long)((tile / pct) / p.cpg) * p.xgs : 0);
         for (int r = tid; r < p.R; r += NPROD) {
           long long ts;
           if (p.win_mode) {
@@ -423,6 +433,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     }
   } else if (warp < W_CONS0) {
     // ===================== A producers, direct register path =====================
+    // (one source only: conv1d_tc_chunk gives two-source inputs raw-staged plans)
     unsigned ca = 0;
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       const int tr = p.nco > 1 ? tile % pct : tile;  // tile within its column chunk
@@ -647,7 +658,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
             end = ts0 + p.R4 < p.T_in ? ts0 + p.R4 : p.T_in;
             rowstride = p.T_in;
             dst_off = start - ts0;
-            src = x + (long long)b * p.xbs + (long long)(c * KC) * p.T_in + (MC ? (long long)((tile / pct) / p.cpg) * p.xgs : 0);
+            src = main_src(p, x, x2, b, c, MC ? (long long)((tile / pct) / p.cpg) * p.xgs : 0);
           } else {
             start = t0;
             end = t0 + TT < p.T_out ? t0 + TT : p.T_out;
@@ -872,12 +883,19 @@ static int tc_launch(TcK& p, size_t bytes, const float* x, const void* packed_w,
 }
 
 // Internal entry for N-chunked callers (conv_transpose): runs output channels
-// [co_off, co_off + d->cout) of a conv whose full output has cout_total channels.
+// [co_off, co_off + d->cout) of a conv whose full output has cout_total channels.  cin1 > 0: the input is
+// cat(x (B, cin1, T), x2 (B, d->cin - cin1, T)) along channels (cin1 a multiple of KC).
 int conv1d_tc_chunk(const pwgb_conv1d_desc* d, int co_off, int cout_total, const float* x, const void* packed_w,
-                    const float* bias, float* y, cudaStream_t st, int nco) {
+                    const float* bias, float* y, cudaStream_t st, int nco, const float* x2, int cin1) {
   TcK p;
   size_t bytes = 0;
   if (!tc_plan(d, p, bytes)) return PWGB_UNSUPPORTED;
+  if (cin1 > 0) {
+    // the direct register path (ns == 0) reads one source
+    if (!x2 || cin1 % KC || cin1 >= d->cin || p.ns == 0) return PWGB_UNSUPPORTED;
+    p.C2 = d->cin - cin1;
+    p.xbs = (long long)cin1 * d->t_in;
+  }
   p.co_off = co_off;
   p.ybs = d->shuffle > 1 ? (long long)(cout_total / d->shuffle) * d->shuffle_tout : (long long)cout_total * d->t_out;
   if (nco > 1) {
@@ -886,13 +904,17 @@ int conv1d_tc_chunk(const pwgb_conv1d_desc* d, int co_off, int cout_total, const
     p.nco = nco;
     p.total_tiles *= nco;
   }
-  return tc_launch(p, bytes, x, packed_w, bias, nullptr, y, st);
+  return tc_launch(p, bytes, x, packed_w, bias, nullptr, y, st, cin1 > 0 ? x2 : nullptr);
 }
 
-int conv1d_tc_plan_ok(const pwgb_conv1d_desc* d) {
+// raw_staged: set to 1 when the plan stages activations through shared memory (TMA or cp.async), as a two-source
+// input requires
+int conv1d_tc_plan_ok(const pwgb_conv1d_desc* d, int* raw_staged) {
   TcK p;
   size_t bytes;
-  return tc_plan(d, p, bytes);
+  const int ok = tc_plan(d, p, bytes);
+  if (raw_staged) *raw_staged = ok && p.ns > 0;
+  return ok;
 }
 
 void tc_pack_weight(const float* w, int cin, int cout, int kernel, void* packed, cudaStream_t st) {

@@ -10,8 +10,8 @@ namespace pwgb {
 int conv1d_forward_simt(const pwgb_conv1d_desc* d, const float* x, const float* w, const float* bias,
                         const float* residual, float* y, cudaStream_t st);
 int conv1d_tc_chunk(const pwgb_conv1d_desc* d, int co_off, int cout_total, const float* x, const void* packed_w,
-                    const float* bias, float* y, cudaStream_t st, int nco);
-int conv1d_tc_plan_ok(const pwgb_conv1d_desc* d);
+                    const float* bias, float* y, cudaStream_t st, int nco, const float* x2 = nullptr, int cin1 = 0);
+int conv1d_tc_plan_ok(const pwgb_conv1d_desc* d, int* raw_staged = nullptr);
 void tc_pack_weight(const float* w, int cin, int cout, int kernel, void* packed, cudaStream_t st);
 
 // w: (cin, cout/groups, K) -> wv: (cout*s, cin/groups, M),
@@ -44,28 +44,22 @@ extern "C" size_t pwgb_conv_transpose1d_workspace(const pwgb_convtr1d_desc* d) {
   return 2 * (size_t)d->cout * d->stride * (d->cin / G) * M * sizeof(float);
 }
 
-extern "C" int pwgb_conv_transpose1d_forward(const pwgb_convtr1d_desc* d, const float* x, const float* w,
-                                             const float* bias, float* y, void* ws, size_t ws_bytes, void* stream) {
-  PWGB_CHECK_ARG(d && x && w && y, "conv_transpose1d: null argument");
+static int convtr_desc_ok(const pwgb_convtr1d_desc* d) {
   PWGB_CHECK_ARG(d->batch >= 0 && d->cin > 0 && d->cout > 0 && d->t_in > 0 && d->kernel > 0 && d->stride > 0 &&
                      d->padding >= 0,
                  "conv_transpose1d: bad descriptor");
-  const int s = d->stride, K = d->kernel, M = ceil_div(K, s);
-  const int G = d->groups > 1 ? d->groups : 1, P = d->period > 1 ? d->period : 1;
+  const int G = d->groups > 1 ? d->groups : 1;
   PWGB_CHECK_ARG(d->cin % G == 0 && d->cout % G == 0, "conv_transpose1d: channels not divisible by groups");
-  const int op = d->t_out - ((d->t_in - 1) * s - 2 * d->padding + K);
-  PWGB_CHECK_ARG(op >= 0 && op < s, "conv_transpose1d: t_out=%d inconsistent with t_in=%d k=%d s=%d p=%d", d->t_out,
-                 d->t_in, K, s, d->padding);
-  const size_t need = pwgb_conv_transpose1d_workspace(d);
-  PWGB_CHECK_ARG(ws && ws_bytes >= need, "conv_transpose1d: workspace too small (%zu < %zu)", ws_bytes, need);
-  cudaStream_t st = (cudaStream_t)stream;
-  float* wv = (float*)ws;
-  const long long n = (long long)d->cout * s * (d->cin / G) * M;
-  int blocks = (int)((n + 255) / 256);
-  if (blocks > 4096) blocks = 4096;
-  convtr_weight_kernel<<<blocks, 256, 0, st>>>(w, wv, d->cin, d->cout, K, s, M, G);
-  int rc = check_launch("convtr_weight_kernel");
-  if (rc) return rc;
+  const int op = d->t_out - ((d->t_in - 1) * d->stride - 2 * d->padding + d->kernel);
+  PWGB_CHECK_ARG(op >= 0 && op < d->stride, "conv_transpose1d: t_out=%d inconsistent with t_in=%d k=%d s=%d p=%d", d->t_out,
+                 d->t_in, d->kernel, d->stride, d->padding);
+  return PWGB_OK;
+}
+
+// The virtual stride-1 conv (cout*s channels, ceil(K/s) taps) that the conv-transpose lowers to
+static pwgb_conv1d_desc convtr_virtual_desc(const pwgb_convtr1d_desc* d) {
+  const int s = d->stride, M = ceil_div(d->kernel, s);
+  const int P = d->period > 1 ? d->period : 1;
   pwgb_conv1d_desc c = {};
   c.batch = d->batch;
   c.cin = d->cin;
@@ -75,7 +69,7 @@ extern "C" int pwgb_conv_transpose1d_forward(const pwgb_convtr1d_desc* d, const 
   c.kernel = M;
   c.stride = 1;
   c.dilation = 1;
-  c.groups = G;
+  c.groups = d->groups > 1 ? d->groups : 1;
   c.pad_left = M - 1;
   c.pad_mode = PWGB_PAD_ZERO;
   c.period = P;
@@ -86,27 +80,85 @@ extern "C" int pwgb_conv_transpose1d_forward(const pwgb_convtr1d_desc* d, const 
   c.shuffle = s;
   c.shuffle_pad = d->padding;
   c.shuffle_tout = d->t_out;
-  // tensor-core path: N (= cout*s virtual channels) in chunks of <= TC_NMAX accumulator columns
-  if (G == 1 && P == 1 && d->cin % 32 == 0 && c.cout % 16 == 0) {
-    int chunk = c.cout;
-    if (chunk > TC_NMAX) {
-      chunk = TC_NMAX;
-      while (c.cout % chunk) chunk -= 16;
-    }
+  return c;
+}
+
+// Tensor-core path: N (= cout*s virtual channels) in chunks of <= TC_NMAX accumulator columns.  Returns the chunk
+// width, or 0 when the conv-transpose runs on the FFMA kernel (or, for a two-source input, cannot take it).
+static int convtr_tc_chunk(const pwgb_conv1d_desc& c, bool two_source) {
+  if (c.groups != 1 || c.period != 1 || c.cin % 32 != 0 || c.cout % 16 != 0) return 0;
+  int chunk = c.cout;
+  if (chunk > TC_NMAX) {
+    chunk = TC_NMAX;
+    while (c.cout % chunk) chunk -= 16;
+  }
+  pwgb_conv1d_desc cc = c;
+  cc.cout = chunk;
+  int raw_staged = 0;
+  if (!conv1d_tc_plan_ok(&cc, &raw_staged) || (two_source && !raw_staged)) return 0;
+  return chunk;
+}
+
+// x2 / cin1: the second source of a two-source input (cin1 > 0 only on the tensor-core path)
+static int convtr_forward(const pwgb_convtr1d_desc* d, const float* x, const float* x2, int cin1, const float* w,
+                          const float* bias, float* y, void* ws, size_t ws_bytes, void* stream) {
+  const int s = d->stride, K = d->kernel, M = ceil_div(K, s);
+  const int G = d->groups > 1 ? d->groups : 1;
+  const size_t need = pwgb_conv_transpose1d_workspace(d);
+  PWGB_CHECK_ARG(ws && ws_bytes >= need, "conv_transpose1d: workspace too small (%zu < %zu)", ws_bytes, need);
+  cudaStream_t st = (cudaStream_t)stream;
+  float* wv = (float*)ws;
+  const long long n = (long long)d->cout * s * (d->cin / G) * M;
+  int blocks = (int)((n + 255) / 256);
+  if (blocks > 4096) blocks = 4096;
+  convtr_weight_kernel<<<blocks, 256, 0, st>>>(w, wv, d->cin, d->cout, K, s, M, G);
+  int rc = check_launch("convtr_weight_kernel");
+  if (rc) return rc;
+  const pwgb_conv1d_desc c = convtr_virtual_desc(d);
+  const int chunk = convtr_tc_chunk(c, cin1 > 0);
+  if (chunk) {
     pwgb_conv1d_desc cc = c;
     cc.cout = chunk;
-    if (conv1d_tc_plan_ok(&cc)) {
-      unsigned char* pk = (unsigned char*)ws + need / 2;
-      // the operand image is laid out per (32-channel chunk, tap) over the rows of ONE launch, so
-      // each column chunk gets its own image
-      for (int co = 0; co < c.cout; co += chunk) {
-        unsigned char* pkc = pk + (size_t)co * d->cin * M * sizeof(float);
-        tc_pack_weight(wv + (size_t)co * d->cin * M, d->cin, chunk, M, pkc, st);
-        rc = check_launch("tc_pack_weight_kernel");
-        if (rc) return rc;
-      }
-      return conv1d_tc_chunk(&cc, 0, c.cout, x, pk, bias, y, st, c.cout / chunk);
+    unsigned char* pk = (unsigned char*)ws + need / 2;
+    // the operand image is laid out per (32-channel chunk, tap) over the rows of ONE launch, so
+    // each column chunk gets its own image
+    for (int co = 0; co < c.cout; co += chunk) {
+      unsigned char* pkc = pk + (size_t)co * d->cin * M * sizeof(float);
+      tc_pack_weight(wv + (size_t)co * d->cin * M, d->cin, chunk, M, pkc, st);
+      rc = check_launch("tc_pack_weight_kernel");
+      if (rc) return rc;
     }
+    return conv1d_tc_chunk(&cc, 0, c.cout, x, pk, bias, y, st, c.cout / chunk, x2, cin1);
+  }
+  if (cin1 > 0) {
+    set_error("conv_transpose1d_cat: configuration not supported by the tensor-core path");
+    return PWGB_UNSUPPORTED;
   }
   return conv1d_forward_simt(&c, x, wv, bias, nullptr, y, st);
+}
+
+extern "C" int pwgb_conv_transpose1d_forward(const pwgb_convtr1d_desc* d, const float* x, const float* w,
+                                             const float* bias, float* y, void* ws, size_t ws_bytes, void* stream) {
+  PWGB_CHECK_ARG(d && x && w && y, "conv_transpose1d: null argument");
+  const int rc = convtr_desc_ok(d);
+  if (rc) return rc;
+  return convtr_forward(d, x, nullptr, 0, w, bias, y, ws, ws_bytes, stream);
+}
+
+extern "C" int pwgb_conv_transpose1d_cat_supported(const pwgb_convtr1d_desc* d, int cin1) {
+  if (!d || d->batch < 0 || d->cin <= 0 || d->cout <= 0 || d->t_in <= 0 || d->kernel <= 0 || d->stride <= 0 || d->padding < 0)
+    return 0;
+  if (cin1 <= 0 || cin1 >= d->cin || cin1 % 32 != 0) return 0;
+  const int op = d->t_out - ((d->t_in - 1) * d->stride - 2 * d->padding + d->kernel);
+  if (op < 0 || op >= d->stride) return 0;
+  return convtr_tc_chunk(convtr_virtual_desc(d), true) > 0;
+}
+
+extern "C" int pwgb_conv_transpose1d_cat_forward(const pwgb_convtr1d_desc* d, int cin1, const float* x1, const float* x2,
+                                                 const float* w, const float* bias, float* y, void* ws, size_t ws_bytes,
+                                                 void* stream) {
+  PWGB_CHECK_ARG(d && x1 && x2 && w && y, "conv_transpose1d_cat: null argument");
+  PWGB_UNSUPPORTED_IF(!pwgb_conv_transpose1d_cat_supported(d, cin1),
+                      "conv_transpose1d_cat: configuration not supported by the two-source tensor-core path");
+  return convtr_forward(d, x1, x2, cin1, w, bias, y, ws, ws_bytes, stream);
 }

@@ -16,19 +16,37 @@ from .capi import PwgbError
 
 
 class DeviceCorpus:
-    """items: list of (audio (T,), feats (frames, C)) numpy arrays / tensors [mel2wav case] or of audio arrays
-    [audio-only case].  ``hop_size`` applies ``Collater._adjust_length`` (train.py:868-893): audio shorter than
-    ``frames * hop_size`` is edge-padded; any other mismatch is an error, like the reference's assert."""
+    """items: list of (audio (T,), feats (frames, C)) numpy arrays / tensors [mel2wav case], of
+    (audio, feats, f0 (frames,), excitation (frames, E)) [UHiFiGAN recipes], or of audio arrays [audio-only case].
+    ``hop_size`` applies ``Collater._adjust_length`` (train.py:868-893): audio shorter than ``frames * hop_size`` is
+    edge-padded; any other mismatch is an error, like the reference's assert.  f0 is kept as a 1-channel feature
+    matrix whose rows line up with the features', excitation flattened like audio (E samples per frame)."""
 
     def __init__(self, items, device, hop_size=None):
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise PwgbError("DeviceCorpus lives on a CUDA device (no CPU fallback)")
         auds, fts, self.x_start, self.c_start, self.x_len, self.c_len = [], [], [], [], [], []
-        xo = co = 0
+        f0s, exs, self.e_start = [], [], []
+        xo = co = eo = 0
         self.has_feats = len(items) > 0 and isinstance(items[0], (tuple, list))
+        self.has_f0 = self.has_feats and len(items[0]) == 4
+        self.excitation_width = 0
         for it in items:
             x, c = (it[0], it[1]) if self.has_feats else (it, None)
+            if self.has_f0:
+                f0 = np.asarray(it[2], dtype=np.float32).reshape(-1, 1)
+                ex = np.asarray(it[3], dtype=np.float32)
+                ex = ex.reshape(len(ex), -1)
+                if len(f0) != len(c) or len(ex) != len(c):
+                    raise PwgbError(f"f0 / excitation have {len(f0)} / {len(ex)} frames, features {len(c)}")
+                if self.excitation_width and ex.shape[1] != self.excitation_width:
+                    raise PwgbError("excitation frames of different widths")
+                self.excitation_width = ex.shape[1]
+                f0s.append(torch.from_numpy(f0))
+                exs.append(torch.from_numpy(ex.reshape(-1)))
+                self.e_start.append(eo)
+                eo += ex.size
             x = np.asarray(x, dtype=np.float32).reshape(-1)
             if c is not None:
                 c = np.asarray(c, dtype=np.float32)
@@ -48,6 +66,8 @@ class DeviceCorpus:
         self.audio = torch.cat(auds).to(self.device) if auds else torch.empty(0, device=self.device)
         self.feats = torch.cat(fts).contiguous().to(self.device) if fts else None
         self.channels = self.feats.shape[1] if self.feats is not None else 0
+        self.f0 = torch.cat(f0s).contiguous().to(self.device) if f0s else None
+        self.excitation = torch.cat(exs).to(self.device) if exs else None
 
     def __len__(self):
         return len(self.x_start)
@@ -56,7 +76,8 @@ class DeviceCorpus:
 class Collater:
     """``Collater`` of bin/train.py:646-925 for the mel2wav and audio-only cases, on the device."""
 
-    def __init__(self, batch_max_steps=20480, hop_size=256, aux_context_window=2, use_noise_input=False, use_aux_input=True):
+    def __init__(self, batch_max_steps=20480, hop_size=256, aux_context_window=2, use_noise_input=False, use_aux_input=True,
+                 use_f0_and_excitation=False):
         if hop_size is not None:
             if batch_max_steps % hop_size != 0:
                 batch_max_steps += -(batch_max_steps % hop_size)
@@ -67,6 +88,7 @@ class Collater:
         self.aux_context_window = aux_context_window
         self.use_noise_input = use_noise_input
         self.use_aux_input = use_aux_input
+        self.use_f0_and_excitation = use_f0_and_excitation
         if not use_aux_input:
             assert not use_noise_input, "Not supported."
         if use_aux_input:
@@ -81,7 +103,9 @@ class Collater:
 
     def __call__(self, corpus, indices):
         """indices: the utterance ids of this batch (what the sampler yields).  Returns ``(inputs, y)`` exactly like
-        the reference: inputs = (z, c) / (c,) [mel2wav] with c (B, C, frames + 2*ctx) and y (B, 1, T)."""
+        the reference: inputs = (z, c) / (c,) [mel2wav] with c (B, C, frames + 2*ctx) and y (B, 1, T); with
+        ``use_f0_and_excitation`` (train.py:758-797) f0 (B, 1, F) and excitation (B, 1, F * E) follow, cropped at the
+        feature rows of c (F = frames + 2*ctx), each gathered by one more pwgb_collate_crop launch."""
         dev = corpus.device
         if self.use_aux_input:
             if not corpus.has_feats:
@@ -108,10 +132,26 @@ class Collater:
                                           vp(co.data_ptr()) if co is not None else None, vp(y.data_ptr()), vp(c.data_ptr()) if c is not None else None,
                                           B, T, corpus.channels, F, vp(torch.cuda.current_stream().cuda_stream))
         capi.check(rc, "pwgb_collate_crop")
+        f0 = e = None
+        if self.use_aux_input and self.use_f0_and_excitation:
+            if not corpus.has_f0:
+                raise PwgbError("Collater(use_f0_and_excitation=True) needs a corpus with f0 and excitation")
+            E = corpus.excitation_width
+            e_off = np.array([corpus.e_start[i] for i in keep], dtype=np.int64) + (starts - self.aux_context_window) * E
+            eo = torch.from_numpy(e_off).pin_memory().to(dev, non_blocking=True)
+            f0 = torch.empty((B, 1, F), device=dev, dtype=torch.float32)
+            e = torch.empty((B, 1, F * E), device=dev, dtype=torch.float32)
+            # excitation as the "audio" of the gather, f0 as a 1-channel feature matrix at the rows of c
+            rc = capi.lib().pwgb_collate_crop(vp(corpus.excitation.data_ptr()), vp(eo.data_ptr()), vp(corpus.f0.data_ptr()),
+                                              vp(co.data_ptr()), vp(e.data_ptr()), vp(f0.data_ptr()), B, F * E, 1, F,
+                                              vp(torch.cuda.current_stream().cuda_stream))
+            capi.check(rc, "pwgb_collate_crop")
         if not self.use_aux_input:
             return (None, None), y  # the reference returns (l_batch, g_batch) = (None, None) here (train.py:861-876)
         inputs = (c,)
         if self.use_noise_input:
             z = torch.randn(y.shape, device=dev, generator=self.generator)  # train.py:790-792, drawn on the device
             inputs = (z,) + inputs
+        if f0 is not None:
+            inputs = inputs + (f0, e)
         return inputs, y

@@ -174,6 +174,186 @@ class HiFiGANGenerator(_GeneratorBase):
         return c.squeeze(0).transpose(1, 0)
 
 
+def _mrf_average(blocks, first, nb, h, differentiable):
+    """sum_j blocks[first + j](h) / nb: ScaledSumFn under autograd, else fused into each block's last conv."""
+    if differentiable:
+        from .autograd import ScaledSumFn
+
+        return ScaledSumFn.apply(1.0 / nb, *[blocks[first + j](h) for j in range(nb)])
+    cs = torch.empty_like(h)
+    for j in range(nb):
+        blocks[first + j](h, out=cs, accumulate=j > 0, out_scale=1.0 / nb)
+    return cs
+
+
+class UHiFiGANGenerator(_GeneratorBase):
+    """models/uhifigan.py:19-343: a U-Net over the excitation signal.  The encoder (input conv, then per level the MRF
+    and a strided conv) keeps each level's output; the decoder starts from the mel features (hidden_conv) and on every
+    level runs LeakyReLU -> ConvTranspose1d over cat(decoder state, encoder output), then the MRF.  The concatenation
+    is never materialised: the conv-transpose reads its input channels from the two tensors."""
+
+    def __init__(
+        self,
+        in_channels=80,
+        out_channels=1,
+        channels=512,
+        kernel_size=7,
+        downsample_scales=(8, 8, 2, 2),
+        downsample_kernel_sizes=(16, 16, 4, 4),
+        upsample_scales=(8, 8, 2, 2),
+        upsample_kernel_sizes=(16, 16, 4, 4),
+        resblock_kernel_sizes=(3, 7, 11),
+        resblock_dilations=[(1, 3, 5), (1, 3, 5), (1, 3, 5)],
+        dropout=0.3,
+        use_additional_convs=True,
+        bias=True,
+        nonlinear_activation="LeakyReLU",
+        nonlinear_activation_params={"negative_slope": 0.1},
+        use_causal_conv=False,
+        use_weight_norm=True,
+    ):
+        super().__init__()
+        assert kernel_size % 2 == 1, "Kernel size must be odd number."
+        assert len(upsample_scales) == len(upsample_kernel_sizes)
+        assert len(resblock_dilations) == len(resblock_kernel_sizes)
+        self.num_upsamples = len(upsample_kernel_sizes)
+        self.num_blocks = len(resblock_kernel_sizes)
+        self.use_causal_conv = use_causal_conv
+        self.kernel_size = kernel_size
+        self.downsample_scales = tuple(downsample_scales)
+        self.upsample_scales = tuple(upsample_scales)
+        self.slope = activation_slope(nonlinear_activation, nonlinear_activation_params)
+        act = getattr(torch.nn, nonlinear_activation)
+        self.downsamples = torch.nn.ModuleList()
+        self.downsamples_mrf = torch.nn.ModuleList()
+        self.upsamples = torch.nn.ModuleList()
+        self.upsamples_mrf = torch.nn.ModuleList()
+        # the reference passes padding= to CausalConv1d, which has no such argument: use_causal_conv=True raises
+        # TypeError here as it does there (uhifigan.py:91-101)
+        conv = CausalConv1d if use_causal_conv else torch.nn.Conv1d
+        self.input_conv = torch.nn.Sequential(
+            conv(out_channels, channels, kernel_size=kernel_size, bias=bias, padding=(kernel_size - 1) // 2),
+            act(**nonlinear_activation_params),
+            torch.nn.Dropout(dropout),
+        )
+        for i in range(len(downsample_scales)):
+            for j in range(len(resblock_kernel_sizes)):
+                self.downsamples_mrf += [
+                    ResidualBlock(
+                        kernel_size=resblock_kernel_sizes[j],
+                        channels=channels,
+                        dilations=resblock_dilations[j],
+                        bias=bias,
+                        use_additional_convs=use_additional_convs,
+                        nonlinear_activation=nonlinear_activation,
+                        nonlinear_activation_params=nonlinear_activation_params,
+                        use_causal_conv=use_causal_conv,
+                    )
+                ]
+            s = downsample_scales[i]
+            self.downsamples += [
+                torch.nn.Sequential(
+                    torch.nn.Conv1d(channels, channels * 2, kernel_size=downsample_kernel_sizes[i], stride=s, bias=bias,
+                                    padding=s // 2 + s % 2),
+                    act(**nonlinear_activation_params),
+                    torch.nn.Dropout(dropout),
+                )
+            ]
+            channels = channels * 2
+        self.hidden_conv = torch.nn.Conv1d(in_channels, channels, kernel_size=kernel_size, bias=bias, padding=(kernel_size - 1) // 2)
+        for i in range(len(upsample_kernel_sizes)):
+            s = upsample_scales[i]
+            self.upsamples += [
+                torch.nn.Sequential(
+                    act(**nonlinear_activation_params),
+                    torch.nn.ConvTranspose1d(channels * 2, channels // 2, upsample_kernel_sizes[i], s, padding=s // 2 + s % 2,
+                                             output_padding=s % 2, bias=bias),
+                )
+            ]
+            for j in range(len(resblock_kernel_sizes)):
+                self.upsamples_mrf += [
+                    ResidualBlock(
+                        kernel_size=resblock_kernel_sizes[j],
+                        channels=channels // 2,
+                        dilations=resblock_dilations[j],
+                        bias=bias,
+                        use_additional_convs=use_additional_convs,
+                        nonlinear_activation=nonlinear_activation,
+                        nonlinear_activation_params=nonlinear_activation_params,
+                        use_causal_conv=use_causal_conv,
+                    )
+                ]
+            channels = channels // 2
+        self.output_conv = torch.nn.Sequential(
+            torch.nn.LeakyReLU(),  # default slope 0.01 (uhifigan.py:222-235)
+            torch.nn.Conv1d(channels, out_channels, kernel_size, bias=bias, padding=(kernel_size - 1) // 2),
+            torch.nn.Tanh(),
+        )
+        if use_weight_norm:
+            self.apply_weight_norm()
+        self.reset_parameters()
+
+    def forward(self, c=None, f0=None, excitation=None):
+        """c (B, in_channels, T'), excitation (B, 1, T' * hop) -> (B, out_channels, T' * hop)  (uhifigan.py:262-301).
+        ``f0`` is accepted and unused, as in the reference."""
+        pad = (self.kernel_size - 1) // 2
+        nb = self.num_blocks
+        slope = self.slope
+        grad = torch.is_grad_enabled() and next(self.parameters()).requires_grad  # autograd: ScaledSumFn for the MRF average
+        ic = self.input_conv[0]
+        h = ops.conv1d(excitation, effective_weight(ic), ic.bias, padding=pad, post_act="lrelu", post_slope=slope)
+        h = ops.dropout(h, self.input_conv[2].p, self.training)
+        skips = []
+        for i, ds in enumerate(self.downsamples):
+            h = _mrf_average(self.downsamples_mrf, i * nb, nb, h, grad or h.requires_grad)
+            s = self.downsample_scales[i]
+            h = ops.conv1d(h, effective_weight(ds[0]), ds[0].bias, stride=s, padding=s // 2 + s % 2, post_act="lrelu",
+                           post_slope=slope)
+            h = ops.dropout(h, ds[2].p, self.training)
+            skips.append(h)
+        hc = self.hidden_conv
+        h = ops.conv1d(c, effective_weight(hc), hc.bias, padding=pad)
+        for i in range(self.num_upsamples):
+            up = self.upsamples[i][1]
+            s = self.upsample_scales[i]
+            h = ops.conv_transpose1d_cat(h, skips[-1 - i], effective_weight(up), up.bias, stride=s, padding=s // 2 + s % 2,
+                                         output_padding=s % 2, pre_slope=slope)
+            h = _mrf_average(self.upsamples_mrf, i * nb, nb, h, grad or h.requires_grad)
+        oc = self.output_conv[1]
+        return ops.conv1d(h, effective_weight(oc), oc.bias, padding=pad, pre_slope=0.01, post_act="tanh")
+
+    def reset_parameters(self):
+        def _reset_parameters(m):
+            if isinstance(m, (torch.nn.Conv1d, torch.nn.ConvTranspose1d)):
+                m.weight.data.normal_(0.0, 0.01)
+
+        self.apply(_reset_parameters)
+
+    def apply_weight_norm(self):
+        def _apply_weight_norm(m):
+            if isinstance(m, (torch.nn.Conv1d, torch.nn.ConvTranspose1d)):
+                torch.nn.utils.weight_norm(m)
+
+        self.apply(_apply_weight_norm)
+
+    def inference(self, excitation=None, f0=None, c=None, normalize_before=False):
+        """excitation (T' * hop,) or (T', hop), c (T', in_channels) -> (T' * hop, out_channels)  (uhifigan.py:317-343).
+        ``normalize_before`` is ignored, as in the reference."""
+        dev = next(self.parameters()).device
+        if c is not None and not isinstance(c, torch.Tensor):
+            c = torch.tensor(c, dtype=torch.float).to(dev)
+        if excitation is not None and not isinstance(excitation, torch.Tensor):
+            excitation = torch.tensor(excitation, dtype=torch.float).to(dev)
+        if f0 is not None and not isinstance(f0, torch.Tensor):
+            f0 = torch.tensor(f0, dtype=torch.float).to(dev)
+        y = self.forward(
+            c.transpose(1, 0).unsqueeze(0).contiguous(),
+            f0.unsqueeze(1).transpose(1, 0).unsqueeze(0) if f0 is not None else None,
+            excitation.reshape(1, 1, -1).contiguous(),
+        )
+        return y.squeeze(0).transpose(1, 0)
+
+
 class MelGANGenerator(_GeneratorBase):
     """models/melgan.py:17-257 (also the multi-band generator with out_channels=4)."""
 

@@ -278,6 +278,67 @@ def conv_transpose1d_raw(x, w, bias=None, *, stride, padding=0, output_padding=0
     return y
 
 
+def conv_transpose1d_cat_raw(x1, x2, w, bias=None, *, stride, padding=0, output_padding=0, pre_slope=1.0):
+    """conv_transpose1d_raw on torch.cat((x1, x2), dim=1) -- pwgb_conv_transpose1d_cat_forward, which reads the two
+    sources in place, bit-identical to the single-source entry on the concatenation.  Configurations it does not serve
+    (x1's channels not a multiple of 32, the FFMA conv-transpose) concatenate and call the single-source entry."""
+    x1, x2, w = _dev(x1, "x1"), _dev(x2, "x2"), _dev(w, "w")
+    B, cin1, t_in = x1.shape
+    if x2.dim() != 3 or x2.shape[0] != B or x2.shape[2] != t_in:
+        raise PwgbError(f"conv_transpose1d_cat: x1 {tuple(x1.shape)} and x2 {tuple(x2.shape)} do not concatenate along channels")
+    cin = cin1 + x2.shape[1]
+    if w.shape[0] != cin:
+        raise PwgbError(f"conv_transpose1d_cat: inputs have {cin} channels, weight expects {w.shape[0]}")
+    cout, K = w.shape[1], w.shape[2]
+    t_out = (t_in - 1) * stride - 2 * padding + K + output_padding
+    d = capi.ConvTr1dDesc(batch=B, cin=cin, cout=cout, t_in=t_in, t_out=t_out, kernel=K, stride=stride, padding=padding,
+                          pre_slope=float(pre_slope), groups=1, period=1)
+    L = capi.lib()
+    if ENGINE == "simt" or not L.pwgb_conv_transpose1d_cat_supported(C.byref(d), cin1):
+        return conv_transpose1d_raw(torch.cat((x1, x2), dim=1), w, bias, stride=stride, padding=padding,
+                                    output_padding=output_padding, pre_slope=pre_slope)
+    if bias is not None:
+        bias = _dev(bias, "bias")
+    nbytes = L.pwgb_conv_transpose1d_workspace(C.byref(d))
+    ws = torch.empty((nbytes + 3) // 4, device=x1.device, dtype=torch.float32)
+    y = torch.empty((B, cout, t_out), device=x1.device, dtype=torch.float32)
+    if y.numel() == 0:
+        return y  # an empty batch: nothing to compute
+    prof = _Prof("conv_transpose1d_cat", 2.0 * B * cout * t_out * cin * ((K + stride - 1) // stride),
+                 4.0 * (x1.numel() + x2.numel() + y.numel()), f"B{B} cin{cin1}+{cin - cin1} cout{cout} k{K} s{stride} T{t_out}")
+    rc = L.pwgb_conv_transpose1d_cat_forward(C.byref(d), cin1, _p(x1), _p(x2), _p(w), _p(bias), _p(y), _p(ws),
+                                             C.c_size_t(nbytes), _stream())
+    capi.check(rc, "pwgb_conv_transpose1d_cat_forward")
+    prof.done()
+    return y
+
+
+def dropout_raw(x, p, seed, offset=0, backward=False):
+    """Training-mode dropout with the counter-based mask of (seed, offset) -- pwgb_dropout_forward; ``backward``
+    applies the same mask and scale to a gradient (pwgb_dropout_backward)."""
+    x = _dev(x, "x")
+    y = torch.empty_like(x)
+    fn = capi.lib().pwgb_dropout_backward if backward else capi.lib().pwgb_dropout_forward
+    rc = fn(_p(x) if x.numel() else None, _p(y) if y.numel() else None, x.numel(), float(p), int(seed), int(offset), _stream())
+    capi.check(rc, "pwgb_dropout_backward" if backward else "pwgb_dropout_forward")
+    return y
+
+
+def dropout(x, p, training):
+    """torch.nn.Dropout(p) semantics: identity (no launch) in eval mode or at p == 0, else a fresh mask per call whose
+    seed is drawn from torch's default CPU generator -- no device sync, and ``torch.manual_seed`` makes it
+    reproducible.  Applied in training mode also under ``no_grad`` (the discriminator phase regenerates the
+    generator's output under no_grad with the generator still in train())."""
+    if not training or p == 0:
+        return x
+    seed = int(torch.randint(0, 2**63 - 1, (), dtype=torch.int64))
+    if _needs_grad(x):
+        from . import autograd as ag
+
+        return ag.DropoutFn.apply(x, float(p), seed)
+    return dropout_raw(x, p, seed)
+
+
 def upsample_fir(x, fir, scale, out=None, out_channels=None):
     """One stage of the PWG conditioning upsampler (layers/upsample.py:112-128):
     nearest repeat x`scale` + (2*scale+1)-tap FIR, zero padded -- pwgb_upsample_fir_forward.
@@ -904,6 +965,15 @@ def conv_transpose1d(x, w, bias=None, **kw):
 
         return ag.conv_transpose1d(x, w, bias, **kw)
     return conv_transpose1d_raw(x, w, bias, **kw)
+
+
+def conv_transpose1d_cat(x1, x2, w, bias=None, **kw):
+    """conv_transpose1d on torch.cat((x1, x2), dim=1) without the concatenation (see conv_transpose1d_cat_raw)."""
+    if _needs_grad(x1, x2, w, bias):
+        from . import autograd as ag
+
+        return ag.conv_transpose1d_cat(x1, x2, w, bias, **kw)
+    return conv_transpose1d_cat_raw(x1, x2, w, bias, **kw)
 
 
 def avg_pool1d(x, kernel_size, stride, padding=0, count_include_pad=True):
