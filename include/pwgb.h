@@ -435,6 +435,59 @@ PWGB_API int pwgb_tade_combine_backward(const float* cg, const float* xn, const 
 PWGB_API int pwgb_tade_gate_backward(const float* x, const float* gy, float* gx, int batch, int channels, long long t, int softmax,
                             void* stream);
 
+/* ------------------------------------------------------------------------
+ * Discrete-symbol HiFi-GAN front end (models/hifigan.py:867-1289, layers/duration_predictor.py,
+ * layers/length_regulator.py, layers/layer_norm.py, losses/duration_prediction_loss.py, bin/train.py:768-783).
+ * Deterministic throughout: no float atomics, every reduction in a fixed order.
+ *
+ *   symbol_embed_forward: y (B, C, t_out) = table[idx[b, 0, j]] (+ spk_table[idx[b, 1, 0]]) -- the channel-major input
+ *     of input_conv in one launch.  idx is read in place as int64 (idx_int64 = 1) or float32 truncated toward zero
+ *     (torch's c.long()), with element strides for batch / channel / time (the speaker id is channel 1, frame 0).
+ *     durations (B, len) int64 or null: length regulation -- frame t of row b takes the symbol j with
+ *     prefix[j] <= t < prefix[j] + ds[b, j] (exclusive prefix sums per row); frames past a row's total are 0.  Without
+ *     durations t_out == len.  An index outside its table is never read: the column (or, for the speaker, the item)
+ *     is written as NaN.
+ *   symbol_embed_backward: d_emb (num_embs, C) [and d_spk (num_spk, C)] from the frame-level gradient gy (B, C, t_out)
+ *     (after regulation) and / or the symbol-level gradient gsym (B, C, len); either may be null.  Each symbol's frames
+ *     are summed in time order, gsym added, and the (b, j) positions are counting-sorted by index (stable) and summed
+ *     per (index, channel) in position order.  Rows no position uses get 0; there is no padding_idx.
+ *     num_embs <= 8192.  Workspace: pwgb_symbol_embed_backward_workspace bytes.
+ *   channel_layernorm_forward / _backward: LayerNorm over C at every (b, t) of (B, C, T) with biased variance, affine
+ *     gamma / beta and eps; the forward optionally stores mean / rstd (B, T) for the backward, which writes dx and the
+ *     two-level fixed-order dgamma / dbeta (workspace: pwgb_channel_layernorm_backward_workspace bytes).
+ *   duration_loss_forward / _backward: out[0] = mean_i (x_i - log(d_i + offset))^2 with int64 d (MSELoss(mean) against
+ *     log-domain targets); backward gx = gout[0] * 2 (x - log(d + offset)) / n.
+ *   duration_round: with x: ds = max(0, rint(exp(x) - offset)) as int64 (rint: half to even, like torch.round); with
+ *     x == null ds is the input.  totals[b] = sum_j ds[b, j].  zero_rule != 0 applies the length regulator's rule in
+ *     place: when the whole batch sums to 0, rows that sum to 0 become all ones.  One launch.
+ *   collate_runlength: run-length encoding of the cropped feature rows feats[(c_offsets[b] + f) * C + ch], f < frames,
+ *     read as int64 by truncation (torch.unique_consecutive(dim=0, return_counts=True) per item).  codes == null: pass 1
+ *     writes runs[b], the number of runs.  Else pass 2 writes codes (B, C, max_runs) and counts (B, max_runs), padded
+ *     with pad_value / 0 past each item's runs.
+ * ---------------------------------------------------------------------- */
+PWGB_API int pwgb_symbol_embed_forward(const void* idx, int idx_int64, long long idx_batch_stride, long long idx_chan_stride,
+                                       long long idx_time_stride, const float* table, int num_embs, const float* spk_table,
+                                       int num_spk, const long long* durations, int batch, int len, int channels, int t_out,
+                                       float* y, void* stream);
+PWGB_API size_t pwgb_symbol_embed_backward_workspace(int batch, int len, int channels, int num_embs);
+PWGB_API int pwgb_symbol_embed_backward(const float* gy, const float* gsym, const void* idx, int idx_int64, long long idx_batch_stride,
+                                        long long idx_chan_stride, long long idx_time_stride, const long long* durations, int batch,
+                                        int len, int channels, int t_out, int num_embs, float* d_emb, int num_spk, float* d_spk,
+                                        void* ws, size_t ws_bytes, void* stream);
+PWGB_API int pwgb_channel_layernorm_forward(const float* x, const float* gamma, const float* beta, int batch, int channels, long long t,
+                                            float eps, float* y, float* mean, float* rstd, void* stream);
+PWGB_API size_t pwgb_channel_layernorm_backward_workspace(int batch, int channels, long long t);
+PWGB_API int pwgb_channel_layernorm_backward(const float* x, const float* gy, const float* gamma, const float* mean, const float* rstd,
+                                             int batch, int channels, long long t, float* dx, float* dgamma, float* dbeta, void* ws,
+                                             size_t ws_bytes, void* stream);
+PWGB_API int pwgb_duration_loss_forward(const float* x, const long long* d, long long n, float offset, float* out, void* stream);
+PWGB_API int pwgb_duration_loss_backward(const float* x, const long long* d, long long n, float offset, const float* gout, float* gx,
+                                         void* stream);
+PWGB_API int pwgb_duration_round(const float* x, long long* ds, long long* totals, int batch, int len, float offset, int zero_rule,
+                                 void* stream);
+PWGB_API int pwgb_collate_runlength(const float* feats, const long long* c_offsets, int batch, int channels, int frames, long long* runs,
+                                    long long* codes, long long* counts, int max_runs, long long pad_value, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -553,3 +553,82 @@ class TadeGateFn(torch.autograd.Function):
         capi.check(rc, "pwgb_tade_gate_backward")
         gres = _nearest_backward(gy, ctx.scale) if ctx.has_res and ctx.needs_input_grad[1] else None
         return gx, gres, None, None
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Discrete-symbol generator front end (models/hifigan.py:867-1289 under autograd)
+# ---------------------------------------------------------------------------------------------------------------
+class SymbolEmbedFn(torch.autograd.Function):
+    """Embedding (+ speaker) with optional length regulation.  With ``symbol_level`` it returns both the regulated
+    (B, C, t_out) and the unregulated (B, C, S) embedding; the backward takes both gradients (either may be absent)
+    and scatters them into the tables in one deterministic pass (pwgb_symbol_embed_backward)."""
+
+    @staticmethod
+    def forward(ctx, table, spk_table, c, ds, t_out, symbol_level):
+        y = ops.symbol_embed_raw(c, table, spk_table, ds, t_out)
+        ctx.set_materialize_grads(False)
+        ctx.cfg = (table.shape[0], spk_table.shape[0] if spk_table is not None else 0, y.shape[2])
+        ctx.save_for_backward(c, ds)
+        if symbol_level:
+            return y, ops.symbol_embed_raw(c, table, spk_table)
+        return y
+
+    @staticmethod
+    def backward(ctx, *grads):
+        c, ds = ctx.saved_tensors
+        num_embs, num_spk, t_out = ctx.cfg
+        gy = grads[0].contiguous() if grads[0] is not None else None
+        gsym = grads[1].contiguous() if len(grads) > 1 and grads[1] is not None else None
+        if gy is None and gsym is None:
+            return None, None, None, None, None, None
+        d_emb, d_spk = ops.symbol_embed_backward_raw(gy, gsym, c, ds, t_out, num_embs, num_spk if ctx.needs_input_grad[1] else 0)
+        return d_emb, d_spk, None, None, None, None
+
+
+class ChannelLayerNormFn(torch.autograd.Function):
+    """LayerNorm over C of (B, C, T) (layers/layer_norm.py with dim=1); the forward keeps mean / rstd for the backward."""
+
+    @staticmethod
+    def forward(ctx, x, gamma, beta, eps):
+        y, mean, rstd = ops.channel_layer_norm_raw(x, gamma, beta, eps, stats=True)
+        ctx.save_for_backward(x.contiguous(), gamma, mean, rstd)
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        x, gamma, mean, rstd = ctx.saved_tensors
+        B, C_, T = x.shape
+        gy = gy.contiguous()
+        dx = torch.empty_like(x)
+        dgamma = torch.empty(C_, device=x.device, dtype=torch.float32)
+        dbeta = torch.empty(C_, device=x.device, dtype=torch.float32)
+        L = capi.lib()
+        nbytes = L.pwgb_channel_layernorm_backward_workspace(B, C_, T)
+        ws = torch.empty((nbytes + 3) // 4, device=x.device, dtype=torch.float32)
+        nz = x.numel() > 0
+        rc = L.pwgb_channel_layernorm_backward(ops._p(x) if nz else None, ops._p(gy) if nz else None, ops._p(gamma.detach().contiguous()),
+                                               ops._p(mean) if nz else None, ops._p(rstd) if nz else None, B, C_, T,
+                                               ops._p(dx) if nz else None, ops._p(dgamma), ops._p(dbeta), ops._p(ws), C.c_size_t(nbytes),
+                                               ops._stream())
+        capi.check(rc, "pwgb_channel_layernorm_backward")
+        return dx, dgamma, dbeta, None
+
+
+class DurationLossFn(torch.autograd.Function):
+    """DurationPredictorLoss (losses/duration_prediction_loss.py:34-52): gradient w.r.t. the log-domain prediction."""
+
+    @staticmethod
+    def forward(ctx, x, ds, offset):
+        ctx.offset = offset
+        ctx.save_for_backward(x, ds)
+        return ops.duration_loss_raw(x, ds, offset)
+
+    @staticmethod
+    def backward(ctx, gout):
+        x, ds = ctx.saved_tensors
+        x = x.contiguous()
+        gx = torch.empty_like(x)
+        rc = capi.lib().pwgb_duration_loss_backward(ops._p(x), ops._p(ds), x.numel(), ctx.offset, ops._p(gout.contiguous().reshape(1)),
+                                                    ops._p(gx), ops._stream())
+        capi.check(rc, "pwgb_duration_loss_backward")
+        return gx, None, None

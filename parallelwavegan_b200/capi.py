@@ -220,6 +220,28 @@ def lib():
     L.pwgb_stft_loss_terms.argtypes = [vp, vp, C.c_longlong, C.c_float, C.c_int, vp, vp, vp, C.c_int, vp]
     L.pwgb_stft_loss_dmag.restype = C.c_int
     L.pwgb_stft_loss_dmag.argtypes = [vp, vp, C.c_longlong, vp, vp, C.c_float, vp, vp]
+    ll = C.c_longlong
+    L.pwgb_symbol_embed_forward.restype = C.c_int
+    L.pwgb_symbol_embed_forward.argtypes = [vp, C.c_int, ll, ll, ll, vp, C.c_int, vp, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]
+    L.pwgb_symbol_embed_backward_workspace.restype = C.c_size_t
+    L.pwgb_symbol_embed_backward_workspace.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
+    L.pwgb_symbol_embed_backward.restype = C.c_int
+    L.pwgb_symbol_embed_backward.argtypes = [vp, vp, vp, C.c_int, ll, ll, ll, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_int,
+                                             vp, vp, C.c_size_t, vp]
+    L.pwgb_channel_layernorm_forward.restype = C.c_int
+    L.pwgb_channel_layernorm_forward.argtypes = [vp, vp, vp, C.c_int, C.c_int, ll, C.c_float, vp, vp, vp, vp]
+    L.pwgb_channel_layernorm_backward_workspace.restype = C.c_size_t
+    L.pwgb_channel_layernorm_backward_workspace.argtypes = [C.c_int, C.c_int, ll]
+    L.pwgb_channel_layernorm_backward.restype = C.c_int
+    L.pwgb_channel_layernorm_backward.argtypes = [vp, vp, vp, vp, vp, C.c_int, C.c_int, ll, vp, vp, vp, vp, C.c_size_t, vp]
+    L.pwgb_duration_loss_forward.restype = C.c_int
+    L.pwgb_duration_loss_forward.argtypes = [vp, vp, ll, C.c_float, vp, vp]
+    L.pwgb_duration_loss_backward.restype = C.c_int
+    L.pwgb_duration_loss_backward.argtypes = [vp, vp, ll, C.c_float, vp, vp, vp]
+    L.pwgb_duration_round.restype = C.c_int
+    L.pwgb_duration_round.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_float, C.c_int, vp]
+    L.pwgb_collate_runlength.restype = C.c_int
+    L.pwgb_collate_runlength.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_int, ll, vp]
     _lib = L
     return L
 
@@ -261,4 +283,7 @@ EXPORTED_SYMBOLS = [
     "pwgb_tade_gate_backward",
     "pwgb_stft_amplitude_backward", "pwgb_mel_project_backward", "pwgb_gate_forward", "pwgb_gate_backward",
     "pwgb_upsample_fir_backward", "pwgb_stft_loss_terms", "pwgb_stft_loss_dmag",
+    "pwgb_symbol_embed_forward", "pwgb_symbol_embed_backward_workspace", "pwgb_symbol_embed_backward",
+    "pwgb_channel_layernorm_forward", "pwgb_channel_layernorm_backward_workspace", "pwgb_channel_layernorm_backward",
+    "pwgb_duration_loss_forward", "pwgb_duration_loss_backward", "pwgb_duration_round", "pwgb_collate_runlength",
 ]

@@ -77,7 +77,7 @@ class Collater:
     """``Collater`` of bin/train.py:646-925 for the mel2wav and audio-only cases, on the device."""
 
     def __init__(self, batch_max_steps=20480, hop_size=256, aux_context_window=2, use_noise_input=False, use_aux_input=True,
-                 use_f0_and_excitation=False):
+                 use_f0_and_excitation=False, use_duration=False, pad_value=0):
         if hop_size is not None:
             if batch_max_steps % hop_size != 0:
                 batch_max_steps += -(batch_max_steps % hop_size)
@@ -89,6 +89,10 @@ class Collater:
         self.use_noise_input = use_noise_input
         self.use_aux_input = use_aux_input
         self.use_f0_and_excitation = use_f0_and_excitation
+        self.use_duration = use_duration
+        self.pad_value = pad_value  # the duration collater pads codes with it: generator_params["num_embs"] (train.py:1321-1323)
+        if use_duration and (not use_aux_input or use_noise_input):
+            raise PwgbError("Collater(use_duration=True) needs use_aux_input=True and use_noise_input=False (train.py:691-695)")
         if not use_aux_input:
             assert not use_noise_input, "Not supported."
         if use_aux_input:
@@ -105,7 +109,11 @@ class Collater:
         """indices: the utterance ids of this batch (what the sampler yields).  Returns ``(inputs, y)`` exactly like
         the reference: inputs = (z, c) / (c,) [mel2wav] with c (B, C, frames + 2*ctx) and y (B, 1, T); with
         ``use_f0_and_excitation`` (train.py:758-797) f0 (B, 1, F) and excitation (B, 1, F * E) follow, cropped at the
-        feature rows of c (F = frames + 2*ctx), each gathered by one more pwgb_collate_crop launch."""
+        feature rows of c (F = frames + 2*ctx), each gathered by one more pwgb_collate_crop launch.  With ``use_duration``
+        (train.py:768-783) it returns ``(c, y, ds)``: the cropped (F, C) symbol rows, truncated to int64, run-length encoded
+        per item (torch.unique_consecutive(dim=0)); c (B, C, S) int64 padded with ``pad_value``, ds (B, S) int64 run
+        lengths padded with 0.  pwgb_collate_runlength counts the runs at the crop offsets, the host reads the B counts
+        to size S (one device-to-host copy), and a second pass writes codes and lengths."""
         dev = corpus.device
         if self.use_aux_input:
             if not corpus.has_feats:
@@ -126,12 +134,15 @@ class Collater:
         c = co = None
         if c_off is not None:
             co = torch.from_numpy(c_off).pin_memory().to(dev, non_blocking=True)
-            c = torch.empty((B, corpus.channels, F), device=dev, dtype=torch.float32)
+            if not self.use_duration:
+                c = torch.empty((B, corpus.channels, F), device=dev, dtype=torch.float32)
         vp = C.c_void_p
         rc = capi.lib().pwgb_collate_crop(vp(corpus.audio.data_ptr()), vp(xo.data_ptr()), vp(corpus.feats.data_ptr()) if c is not None else None,
                                           vp(co.data_ptr()) if co is not None else None, vp(y.data_ptr()), vp(c.data_ptr()) if c is not None else None,
                                           B, T, corpus.channels, F, vp(torch.cuda.current_stream().cuda_stream))
         capi.check(rc, "pwgb_collate_crop")
+        if self.use_aux_input and self.use_duration:
+            return self._runlength(corpus, co, B, F, y)
         f0 = e = None
         if self.use_aux_input and self.use_f0_and_excitation:
             if not corpus.has_f0:
@@ -155,3 +166,19 @@ class Collater:
         if f0 is not None:
             inputs = inputs + (f0, e)
         return inputs, y
+
+    def _runlength(self, corpus, co, B, F, y):
+        L, vp, st = capi.lib(), C.c_void_p, C.c_void_p(torch.cuda.current_stream().cuda_stream)
+        Cc, dev = corpus.channels, corpus.device
+        runs = torch.empty(B, device=dev, dtype=torch.int64)
+        rc = L.pwgb_collate_runlength(vp(corpus.feats.data_ptr()), vp(co.data_ptr()) if B else None, B, Cc, F,
+                                      vp(runs.data_ptr()) if B else None, None, None, 0, 0, st)
+        capi.check(rc, "pwgb_collate_runlength")
+        S = int(runs.cpu().max()) if B else 0  # sizes the padded batch: one device-to-host copy of B int64
+        c = torch.empty((B, Cc, S), device=dev, dtype=torch.int64)
+        ds = torch.empty((B, S), device=dev, dtype=torch.int64)
+        rc = L.pwgb_collate_runlength(vp(corpus.feats.data_ptr()), vp(co.data_ptr()) if B else None, B, Cc, F, None,
+                                      vp(c.data_ptr()) if c.numel() else None, vp(ds.data_ptr()) if ds.numel() else None, S,
+                                      int(self.pad_value), st)
+        capi.check(rc, "pwgb_collate_runlength")
+        return c, y, ds

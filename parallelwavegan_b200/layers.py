@@ -505,3 +505,107 @@ class TADEResBlock(torch.nn.Module):
         x = ops.conv1d(x, effective_weight(g2), g2.bias, dilation=self.dilation, padding=self.pad * self.dilation)
         # gate + nearest-upsampled residual in one pass
         return ops.tade_gate(x, residual, self.upsample_factor, self.gated_function_name), c
+
+
+# --------------------------------------------------------------------------
+# layers/layer_norm.py, layers/duration_predictor.py, layers/length_regulator.py
+# --------------------------------------------------------------------------
+class LayerNorm(torch.nn.LayerNorm):
+    """layers/layer_norm.py:10-40: torch.nn.LayerNorm(nout, eps=1e-12) over dimension ``dim``.  dim = 1 of a
+    (B, C, T) tensor is pwgb_channel_layernorm_forward on the channel-major layout; dim = -1 of (N, C) is the same
+    kernel on the (N, C, 1) view."""
+
+    def __init__(self, nout, dim=-1):
+        super().__init__(nout, eps=1e-12)
+        self.dim = dim
+
+    def forward(self, x):
+        if self.dim == 1 and x.dim() == 3:
+            return ops.channel_layer_norm(x, self.weight, self.bias, self.eps)
+        if self.dim in (-1, x.dim() - 1):
+            shape = x.shape
+            y = ops.channel_layer_norm(x.reshape(-1, shape[-1], 1), self.weight, self.bias, self.eps)
+            return y.reshape(shape)
+        raise PwgbError(f"LayerNorm(dim={self.dim}) of a {x.dim()}-D tensor has no sm_90a kernel (dim=1 of (B, C, T) or the last dim)")
+
+
+class DurationPredictor(torch.nn.Module):
+    """layers/duration_predictor.py:17-116 (FastSpeech duration predictor).  Each layer is Conv1d (k, "same" padding)
+    with the ReLU fused into its epilogue, LayerNorm over channels (its own kernel: it spans the conv's 128-column
+    chunks) and dropout; the final Linear(n_chans, 1) runs as a k = 1 conv with one output channel.  ``forward`` takes
+    (B, Tmax, idim) like the reference; the channel-major (B, idim, Tmax) tensor the generators hold, transposed, is
+    read in place."""
+
+    def __init__(self, idim, n_layers=2, n_chans=384, kernel_size=3, dropout_rate=0.1, offset=1.0):
+        super().__init__()
+        self.offset = offset
+        self.conv = torch.nn.ModuleList()
+        for idx in range(n_layers):
+            in_chans = idim if idx == 0 else n_chans
+            self.conv += [
+                torch.nn.Sequential(
+                    torch.nn.Conv1d(in_chans, n_chans, kernel_size, stride=1, padding=(kernel_size - 1) // 2),
+                    torch.nn.ReLU(),
+                    LayerNorm(n_chans, dim=1),
+                    torch.nn.Dropout(dropout_rate),
+                )
+            ]
+        self.linear = torch.nn.Linear(n_chans, 1)
+
+    def _log_durations(self, xs, x_masks):
+        """(B, Tmax, idim) -> (B, Tmax) log-domain durations (duration_predictor.py:71-77)."""
+        if x_masks is not None:
+            raise PwgbError("DurationPredictor: x_masks has no sm_90a kernel (the generators never pass one)")
+        h = xs.transpose(1, -1)  # (B, idim, Tmax)
+        for f in self.conv:
+            conv, ln, drop = f[0], f[2], f[3]
+            if h.shape[1] != conv.in_channels:
+                raise PwgbError(f"DurationPredictor: input has {h.shape[1]} channels, the first conv expects {conv.in_channels}")
+            h = ops.conv1d(h, effective_weight(conv), conv.bias, padding=conv.padding[0], post_act="lrelu", post_slope=0.0)
+            h = ln(h)
+            h = ops.dropout(h, drop.p, self.training)
+        lin = self.linear
+        w = lin.weight.reshape(1, lin.in_features, 1)
+        if ops._needs_grad(h, w, lin.bias):
+            from .autograd import conv1d as conv1d_grad
+
+            y = conv1d_grad(h, w, lin.bias)
+        else:
+            y = ops.conv1d_raw(h, w, lin.bias)
+        return y.reshape(y.shape[0], y.shape[2])
+
+    def forward(self, xs, x_masks=None):
+        """Log-domain durations (B, Tmax) (duration_predictor.py:90-102)."""
+        return self._log_durations(xs, x_masks)
+
+    def inference(self, xs, x_masks=None):
+        """int64 durations clamp(round(exp(x) - offset), min=0) (B, Tmax) (duration_predictor.py:104-116)."""
+        ds, _ = ops.duration_round(self._log_durations(xs, x_masks), self.offset, zero_rule=False)
+        return ds
+
+
+class LengthRegulator(torch.nn.Module):
+    """layers/length_regulator.py:47-98: row b repeats xs[b, j] ds[b, j] times and the rows are zero-padded to the
+    largest total.  When the whole batch sums to zero, rows summing to zero are set to all ones first, in place on
+    ``ds`` (length_regulator.py:87-95).  The repeat is the embed kernel with xs as the table (row b * Tmax + j); sizing
+    the output reads the row totals on the host (see ``ops.regulated_length``).  Under autograd the table gradient goes
+    through pwgb_symbol_embed_backward, which serves at most 8192 table rows: B * Tmax <= 8192 (larger raises
+    PwgbError).  The generators regulate their embedding tables directly and do not go through this module."""
+
+    def __init__(self, pad_value=0.0):
+        super().__init__()
+        self.pad_value = pad_value
+
+    def forward(self, xs, ds, alpha=1.0):
+        """xs (B, Tmax, D), ds (B, Tmax) int64 -> (B, T*, D)."""
+        if alpha != 1.0:
+            raise PwgbError("LengthRegulator: alpha != 1.0 has no sm_90a kernel (the generators never pass it)")
+        if self.pad_value != 0.0:
+            raise PwgbError("LengthRegulator: pad_value != 0 has no sm_90a kernel")
+        B, S, D = xs.shape
+        _, totals = ops.duration_round(None, ds=ds)
+        if B * S == 0:
+            return xs.new_zeros((B, 0, D))
+        idx = torch.arange(B * S, device=xs.device, dtype=torch.int64).reshape(B, 1, S)
+        y = ops.symbol_embed(idx, xs.reshape(B * S, D), ds=ds, t_out=ops.regulated_length(totals))
+        return y.transpose(1, 2)

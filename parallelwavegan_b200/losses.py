@@ -298,3 +298,20 @@ class FeatureMatchLoss(torch.nn.Module):
                 out = ops.reduce_mean("l1", a, b.detach(), weight=wd * wl, out=out, accumulate=not first)
                 first = False
         return out[0]
+
+
+# --------------------------------------------------------------------------
+# losses/duration_prediction_loss.py
+# --------------------------------------------------------------------------
+class DurationPredictorLoss(torch.nn.Module):
+    """losses/duration_prediction_loss.py:15-52: MSELoss between the log-domain prediction and log(targets + offset)
+    over all (B, T), padding included (pwgb_duration_loss_forward)."""
+
+    def __init__(self, offset=1.0, reduction="mean"):
+        super().__init__()
+        if reduction != "mean":
+            raise PwgbError(f"DurationPredictorLoss(reduction={reduction!r}) has no sm_90a kernel (mean only)")
+        self.offset = offset
+
+    def forward(self, outputs, targets):
+        return ops.duration_loss(outputs, targets, self.offset)[0]

@@ -53,6 +53,38 @@ class _GeneratorBase(torch.nn.Module):
         return c.transpose(1, 0).unsqueeze(0).contiguous()
 
 
+def _mrf_average(blocks, first, nb, h, differentiable):
+    """sum_j blocks[first + j](h) / nb: ScaledSumFn under autograd, else fused into each block's last conv."""
+    if differentiable:
+        from .autograd import ScaledSumFn
+
+        return ScaledSumFn.apply(1.0 / nb, *[blocks[first + j](h) for j in range(nb)])
+    cs = torch.empty_like(h)
+    for j in range(nb):
+        blocks[first + j](h, out=cs, accumulate=j > 0, out_scale=1.0 / nb)
+    return cs
+
+
+def _hifigan_body(g, c):
+    """The HiFi-GAN body after input_conv (hifigan.py:182-192, 1023-1029, 1215-1221, 1281-1287): per level LeakyReLU ->
+    ConvTranspose1d (fused pre-activation) and the MRF average, then LeakyReLU(0.01) -> output conv -> tanh.  Shared by
+    HiFiGANGenerator and the discrete-symbol generators; the conv-transpose padding is read from each module, which
+    is where the two differ.  Inference runs the fused ResBlock pairs, autograd ScaledSumFn."""
+    nb = g.num_blocks
+    for i in range(g.num_upsamples):
+        up = g.upsamples[i][1]
+        if g.use_causal_conv:
+            c = up(c, pre_slope=g.slope)
+        else:
+            c = ops.conv_transpose1d(c, effective_weight(up), up.bias, stride=up.stride[0], padding=up.padding[0],
+                                     output_padding=up.output_padding[0], pre_slope=g.slope)
+        c = _mrf_average(g.blocks, i * nb, nb, c, torch.is_grad_enabled() and (c.requires_grad or next(g.parameters()).requires_grad))
+    oc = g.output_conv[1]
+    if g.use_causal_conv:
+        return oc(c, pre_slope=0.01, post_act="tanh")
+    return ops.conv1d(c, effective_weight(oc), oc.bias, padding=(g.kernel_size - 1) // 2, pre_slope=0.01, post_act="tanh")
+
+
 class HiFiGANGenerator(_GeneratorBase):
     """models/hifigan.py:23-267."""
 
@@ -127,32 +159,9 @@ class HiFiGANGenerator(_GeneratorBase):
 
     def forward(self, c):
         """(B, in_channels, T) -> (B, out_channels, T * prod(upsample_scales))  (hifigan.py:173-192)."""
-        pad = (self.kernel_size - 1) // 2
         ic = self.input_conv
-        causal = self.use_causal_conv
-        c = ic(c) if causal else ops.conv1d(c, effective_weight(ic), ic.bias, padding=pad)
-        nb = self.num_blocks
-        for i in range(self.num_upsamples):
-            up = self.upsamples[i][1]
-            s = self.upsample_scales[i]
-            if causal:
-                c = up(c, pre_slope=self.slope)
-            else:
-                c = ops.conv_transpose1d(c, effective_weight(up), up.bias, stride=s, padding=s // 2 + s % 2,
-                                         output_padding=s % 2, pre_slope=self.slope)
-            if torch.is_grad_enabled() and (c.requires_grad or next(self.parameters()).requires_grad):
-                from .autograd import ScaledSumFn  # training: differentiable MRF average
-
-                c = ScaledSumFn.apply(1.0 / nb, *[self.blocks[i * nb + j](c) for j in range(nb)])
-            else:
-                cs = torch.empty_like(c)
-                for j in range(nb):  # cs = sum_j block_j(c) / nb, fused into each block's last conv
-                    self.blocks[i * nb + j](c, out=cs, accumulate=j > 0, out_scale=1.0 / nb)
-                c = cs
-        oc = self.output_conv[1]
-        if causal:
-            return oc(c, pre_slope=0.01, post_act="tanh")
-        return ops.conv1d(c, effective_weight(oc), oc.bias, padding=pad, pre_slope=0.01, post_act="tanh")
+        c = ic(c) if self.use_causal_conv else ops.conv1d(c, effective_weight(ic), ic.bias, padding=(self.kernel_size - 1) // 2)
+        return _hifigan_body(self, c)
 
     def reset_parameters(self):
         def _reset_parameters(m):
@@ -174,16 +183,219 @@ class HiFiGANGenerator(_GeneratorBase):
         return c.squeeze(0).transpose(1, 0)
 
 
-def _mrf_average(blocks, first, nb, h, differentiable):
-    """sum_j blocks[first + j](h) / nb: ScaledSumFn under autograd, else fused into each block's last conv."""
-    if differentiable:
-        from .autograd import ScaledSumFn
+class DiscreteSymbolHiFiGANGenerator(torch.nn.Module):
+    """models/hifigan.py:867-1091: HiFi-GAN over discrete units (HuBERT codes).  The symbol embedding (+ the speaker
+    embedding of each item's first frame) is written channel-major by one embed launch (pwgb_symbol_embed_forward),
+    reading the index tensor in place; the body is HiFiGANGenerator's (``_hifigan_body``).  The upsampling
+    ConvTranspose1d uses padding (k - s) // 2 and no output_padding (hifigan.py:953-959).  There is no
+    ``register_stats``, as in the reference."""
 
-        return ScaledSumFn.apply(1.0 / nb, *[blocks[first + j](h) for j in range(nb)])
-    cs = torch.empty_like(h)
-    for j in range(nb):
-        blocks[first + j](h, out=cs, accumulate=j > 0, out_scale=1.0 / nb)
-    return cs
+    def __init__(
+        self,
+        in_channels=512,
+        out_channels=1,
+        channels=512,
+        num_embs=100,
+        num_spk_embs=128,
+        spk_emb_dim=128,
+        concat_spk_emb=False,
+        kernel_size=7,
+        upsample_scales=(8, 8, 2, 2),
+        upsample_kernel_sizes=(16, 16, 4, 4),
+        resblock_kernel_sizes=(3, 7, 11),
+        resblock_dilations=[(1, 3, 5), (1, 3, 5), (1, 3, 5)],
+        use_additional_convs=True,
+        bias=True,
+        nonlinear_activation="LeakyReLU",
+        nonlinear_activation_params={"negative_slope": 0.1},
+        use_weight_norm=True,
+    ):
+        super().__init__()
+        self.num_spk_embs = num_spk_embs
+        self.emb = torch.nn.Embedding(num_embeddings=num_embs, embedding_dim=in_channels)
+        if self.num_spk_embs > 0:
+            self.spk_emb = torch.nn.Embedding(num_embeddings=num_spk_embs, embedding_dim=spk_emb_dim)
+            self.concat_spk_emb = concat_spk_emb
+            if not concat_spk_emb:
+                assert in_channels == spk_emb_dim
+            else:
+                in_channels = in_channels + spk_emb_dim
+        assert kernel_size % 2 == 1, "Kernal size must be odd number."
+        assert len(upsample_scales) == len(upsample_kernel_sizes)
+        assert len(resblock_dilations) == len(resblock_kernel_sizes)
+        self.num_upsamples = len(upsample_kernel_sizes)
+        self.num_blocks = len(resblock_kernel_sizes)
+        self.use_causal_conv = False
+        self.kernel_size = kernel_size
+        self.slope = activation_slope(nonlinear_activation, nonlinear_activation_params)
+        act = getattr(torch.nn, nonlinear_activation)
+        # input / upsampling / output convs always have a bias; ``bias`` reaches the residual blocks only (hifigan.py:938-986)
+        self.input_conv = torch.nn.Conv1d(in_channels, channels, kernel_size, 1, padding=(kernel_size - 1) // 2)
+        self.upsamples = torch.nn.ModuleList()
+        self.blocks = torch.nn.ModuleList()
+        for i in range(len(upsample_kernel_sizes)):
+            self.upsamples += [
+                torch.nn.Sequential(
+                    act(**nonlinear_activation_params),
+                    torch.nn.ConvTranspose1d(channels // (2**i), channels // (2 ** (i + 1)), upsample_kernel_sizes[i], upsample_scales[i],
+                                             padding=(upsample_kernel_sizes[i] - upsample_scales[i]) // 2),
+                )
+            ]
+            for j in range(len(resblock_kernel_sizes)):
+                self.blocks += [
+                    ResidualBlock(
+                        kernel_size=resblock_kernel_sizes[j],
+                        channels=channels // (2 ** (i + 1)),
+                        dilations=resblock_dilations[j],
+                        bias=bias,
+                        use_additional_convs=use_additional_convs,
+                        nonlinear_activation=nonlinear_activation,
+                        nonlinear_activation_params=nonlinear_activation_params,
+                    )
+                ]
+        self.output_conv = torch.nn.Sequential(
+            torch.nn.LeakyReLU(),  # default slope 0.01 (hifigan.py:974-986)
+            torch.nn.Conv1d(channels // (2 ** (i + 1)), out_channels, kernel_size, 1, padding=(kernel_size - 1) // 2),
+            torch.nn.Tanh(),
+        )
+        if use_weight_norm:
+            self.apply_weight_norm()
+        self.reset_parameters()
+
+    remove_weight_norm = _GeneratorBase.remove_weight_norm
+    reset_parameters = HiFiGANGenerator.reset_parameters
+    apply_weight_norm = HiFiGANGenerator.apply_weight_norm
+
+    def _check_input(self, c):
+        if self.num_spk_embs > 0:
+            assert c.size(1) == 2
+            if self.concat_spk_emb:
+                # hifigan.py:1015-1017 concatenates the speaker embedding along time, so input_conv, built for
+                # in_channels + spk_emb_dim, receives in_channels: the reference fails there; so does the mirror
+                raise PwgbError(f"concat_spk_emb=True: input_conv expects {self.input_conv.in_channels} channels, the embedding "
+                                f"has {self.emb.embedding_dim} (the reference concatenates the speaker embedding along time)")
+        else:
+            assert c.size(1) == 1
+
+    def _embed(self, c, ds=None, t_out=None, symbol_level=False):
+        """(B, 1 or 2, S) symbol (, speaker) indices of any dtype -> channel-major embedding (see ops.symbol_embed)."""
+        self._check_input(c)
+        spk = self.spk_emb.weight if self.num_spk_embs > 0 else None
+        return ops.symbol_embed(c, self.emb.weight, spk, ds=ds, t_out=t_out, symbol_level=symbol_level)
+
+    def _body(self, c):
+        ic = self.input_conv
+        return _hifigan_body(self, ops.conv1d(c, effective_weight(ic), ic.bias, padding=(self.kernel_size - 1) // 2))
+
+    def forward(self, c):
+        """c (B, 2, T) (symbol, speaker id) or (B, 1, T) -> (B, out_channels, T * prod(upsample_scales))  (hifigan.py:995-1031)."""
+        return self._body(self._embed(c))
+
+    def _prep_symbols(self, c, g):
+        """inference input plumbing (hifigan.py:1082-1090): (T, 2) or (T, 1) -> (1, K, T) view."""
+        if not isinstance(c, torch.Tensor):
+            c = torch.tensor(c, dtype=torch.long).to(next(self.parameters()).device)
+        if g is not None:
+            c = c[:, 0:1]
+            c = torch.cat([c, c.new_zeros(*c.size()).fill_(g).to(c.device)], dim=1)
+        if self.num_spk_embs <= 0:
+            c = c[:, 0:1]
+        return c.transpose(1, 0).unsqueeze(0)
+
+    def inference(self, c, g=None, normalize_before=False):
+        """(T, 2) or (T, 1) indices [, speaker id g] -> (T * prod(upsample_scales), out_channels)  (hifigan.py:1072-1091)."""
+        assert not normalize_before, "No statistics are used."
+        c = self.forward(self._prep_symbols(c, g))
+        return c.squeeze(0).transpose(1, 0)
+
+
+class DiscreteSymbolDurationGenerator(DiscreteSymbolHiFiGANGenerator):
+    """models/hifigan.py:1094-1289: the discrete-symbol generator with a FastSpeech duration predictor and a length
+    regulator.  ``forward(c, ds)`` regulates by the given durations, ``synthesis`` by the predicted ones.  The embedding
+    is gathered twice from the table by one autograd Function: per symbol for the predictor and length-regulated for
+    input_conv.  Sizing the regulated tensor reads the B row totals on the host (one small device-to-host copy per
+    forward with durations, where the reference synchronises too).  The duration predictor is built after weight
+    norm, so its convs are plain (hifigan.py:1170-1182)."""
+
+    def __init__(
+        self,
+        in_channels=512,
+        out_channels=1,
+        channels=512,
+        num_embs=100,
+        num_spk_embs=128,
+        spk_emb_dim=128,
+        concat_spk_emb=False,
+        duration_layers=2,
+        duration_chans=384,
+        duration_kernel_size=3,
+        duration_offset=1.0,
+        duration_dropout_rate=0.5,
+        kernel_size=7,
+        upsample_scales=(8, 8, 2, 2),
+        upsample_kernel_sizes=(16, 16, 4, 4),
+        resblock_kernel_sizes=(3, 7, 11),
+        resblock_dilations=[(1, 3, 5), (1, 3, 5), (1, 3, 5)],
+        use_additional_convs=True,
+        bias=True,
+        nonlinear_activation="LeakyReLU",
+        nonlinear_activation_params={"negative_slope": 0.1},
+        use_weight_norm=True,
+    ):
+        from .layers import DurationPredictor, LengthRegulator
+
+        super().__init__(
+            in_channels=in_channels, out_channels=out_channels, channels=channels, num_embs=num_embs + 1,  # + the padding symbol
+            num_spk_embs=num_spk_embs, spk_emb_dim=spk_emb_dim, concat_spk_emb=concat_spk_emb, kernel_size=kernel_size,
+            upsample_scales=upsample_scales, upsample_kernel_sizes=upsample_kernel_sizes, resblock_kernel_sizes=resblock_kernel_sizes,
+            resblock_dilations=resblock_dilations, use_additional_convs=use_additional_convs, bias=bias,
+            nonlinear_activation=nonlinear_activation, nonlinear_activation_params=nonlinear_activation_params,
+            use_weight_norm=use_weight_norm,
+        )
+        if self.num_spk_embs > 0:
+            # built for in_channels + spk_emb_dim inputs but fed in_channels: forward raises, as in the reference
+            in_channels = in_channels + spk_emb_dim
+        self.duration_predictor = DurationPredictor(in_channels, n_layers=duration_layers, n_chans=duration_chans,
+                                                    kernel_size=duration_kernel_size, dropout_rate=duration_dropout_rate,
+                                                    offset=duration_offset)
+        self.length_regulator = LengthRegulator()
+
+    def _check_input(self, c):
+        super()._check_input(c)
+        if self.duration_predictor.conv[0][0].in_channels != self.emb.embedding_dim:
+            # num_spk_embs > 0: the predictor is built for in_channels + spk_emb_dim inputs and receives in_channels
+            # (hifigan.py:1170-1180, 1211); the reference fails at its first conv, the mirror before any launch
+            raise PwgbError(f"duration predictor expects {self.duration_predictor.conv[0][0].in_channels} channels, the embedding "
+                            f"has {self.emb.embedding_dim} (the reference builds it for in_channels + spk_emb_dim)")
+
+    def forward(self, c, ds):
+        """c (B, 2 or 1, S), ds (B, S) int64 -> (y (B, out_channels, max_b sum(ds[b]) * prod(upsample_scales)), ds_out (B, S)
+        log-domain predicted durations)  (hifigan.py:1184-1223).  ``ds`` gets the length regulator's all-zero rule in
+        place, as in the reference."""
+        self._check_input(c)
+        _, totals = ops.duration_round(None, ds=ds)
+        e, e_sym = self._embed(c, ds=ds, t_out=ops.regulated_length(totals), symbol_level=True)
+        ds_out = self.duration_predictor(e_sym.transpose(1, 2))
+        return self._body(e), ds_out
+
+    def synthesis(self, c):
+        """c (B, 2 or 1, S) -> (y, ds_out (B, S) int64 predicted durations after the all-zero rule)  (hifigan.py:1250-1289)."""
+        e_sym = self._embed(c)
+        x = self.duration_predictor._log_durations(e_sym.transpose(1, 2), None)
+        ds, totals = ops.duration_round(x, self.duration_predictor.offset)  # rounding and the regulator's rule: one launch
+        e = self._embed(c, ds=ds, t_out=ops.regulated_length(totals))
+        return self._body(e), ds
+
+    def inference(self, c, g=None, ds=None, normalize_before=False):
+        """(T, 2) or (T, 1) indices [, speaker id g] [, durations ds (T,)] -> (sum(ds) * prod(upsample_scales), out_channels)
+        (hifigan.py:1225-1248)."""
+        assert not normalize_before, "No statistics are used."
+        c = self._prep_symbols(c, g)
+        if ds is None:
+            y, _ = self.synthesis(c)
+        else:
+            y, _ = self.forward(c, ds.unsqueeze(0))
+        return y.squeeze(0).transpose(1, 0)
 
 
 class UHiFiGANGenerator(_GeneratorBase):

@@ -991,3 +991,157 @@ def reduce_mean(mode, x, y=None, c=0.0, s=1.0, weight=1.0, out=None, accumulate=
         term = ag.ReduceMeanFn.apply(x, y, mode, float(c), float(s), float(weight))
         return term if (out is None or not accumulate) else out + term
     return reduce_mean_raw(mode, x, y, c, s, weight, out, accumulate)
+
+
+# ---- discrete-symbol front end (models/hifigan.py:867-1289): embedding + length regulation, LayerNorm over channels,
+# duration loss and rounding -- pwgb_symbol_embed_* / pwgb_channel_layernorm_* / pwgb_duration_* ----
+def _index_tensor(c, name="c"):
+    """A (B, K, S) symbol-index tensor read in place by the embed kernels: float32 (the mel2wav collater's features) or
+    int64 (the duration collater's codes); any other dtype is cast with ``.long()``, as the reference reads ``c.long()``."""
+    if not isinstance(c, torch.Tensor) or not c.is_cuda:
+        raise PwgbError(f"{name}: expected a CUDA tensor; parallelwavegan_b200 only runs on CUDA (no CPU fallback)")
+    if c.dim() != 3:
+        raise PwgbError(f"{name}: expected (B, K, S) indices, got shape {tuple(c.shape)}")
+    if c.dtype not in (torch.float32, torch.int64):
+        c = c.long()
+    return c, int(c.dtype == torch.int64)
+
+
+def _durations(ds, B, S):
+    if not isinstance(ds, torch.Tensor) or not ds.is_cuda or ds.dtype != torch.int64 or tuple(ds.shape) != (B, S):
+        raise PwgbError(f"durations: expected a CUDA int64 tensor of shape {(B, S)}")
+    if not ds.is_contiguous():
+        raise PwgbError("durations: expected a contiguous tensor")
+    return ds
+
+
+def symbol_embed_raw(c, table, spk_table=None, ds=None, t_out=None):
+    """(B, C, t_out) = table[c[:, 0]] (+ spk_table[c[:, 1, 0]]), regulated by the int64 durations ``ds`` (B, S) when
+    given (t_out: the largest row total) -- pwgb_symbol_embed_forward.  Indices outside a table give NaN columns."""
+    c, is64 = _index_tensor(c)
+    table = _dev(table, "table")
+    B, K, S = c.shape
+    if spk_table is not None:
+        spk_table = _dev(spk_table, "spk_table")
+        if K < 2:
+            raise PwgbError("symbol_embed: a speaker table needs (B, 2, S) indices")
+    if ds is None:
+        t_out = S
+    else:
+        ds = _durations(ds, B, S)
+    C_ = table.shape[1]
+    y = torch.empty((B, C_, int(t_out)), device=table.device, dtype=torch.float32)
+    sb, sc, st = c.stride()
+    prof = _Prof("symbol_embed", 0.0, 4.0 * y.numel() + c.element_size() * B * S, f"B{B} C{C_} S{S} T{t_out}")
+    rc = capi.lib().pwgb_symbol_embed_forward(_p(c) if c.numel() else None, is64, sb, sc, st, _p(table), table.shape[0],
+                                              _p(spk_table), spk_table.shape[0] if spk_table is not None else 0,
+                                              _p(ds) if ds is not None and ds.numel() else None, B, S, C_, int(t_out),
+                                              _p(y) if y.numel() else None, _stream())
+    capi.check(rc, "pwgb_symbol_embed_forward")
+    prof.done()
+    return y
+
+
+def symbol_embed_backward_raw(gy, gsym, c, ds, t_out, num_embs, num_spk=0):
+    """(d_table, d_spk_table or None) of symbol_embed_raw -- pwgb_symbol_embed_backward (deterministic)."""
+    c, is64 = _index_tensor(c)
+    B, _, S = c.shape
+    gy = _dev(gy, "gy") if gy is not None else None
+    gsym = _dev(gsym, "gsym") if gsym is not None else None
+    dev = (gy if gy is not None else gsym).device
+    C_ = (gy if gy is not None else gsym).shape[1]
+    d_emb = torch.empty((num_embs, C_), device=dev, dtype=torch.float32)
+    d_spk = torch.empty((num_spk, C_), device=dev, dtype=torch.float32) if num_spk else None
+    L = capi.lib()
+    nbytes = L.pwgb_symbol_embed_backward_workspace(B, S, C_, num_embs)
+    ws = torch.empty((nbytes + 3) // 4, device=dev, dtype=torch.float32)
+    sb, sc, st = c.stride()
+    rc = L.pwgb_symbol_embed_backward(_p(gy) if gy is not None and gy.numel() else None,
+                                      _p(gsym) if gsym is not None and gsym.numel() else None, _p(c) if c.numel() else None, is64,
+                                      sb, sc, st, _p(ds) if ds is not None and ds.numel() else None, B, S, C_, int(t_out), num_embs,
+                                      _p(d_emb), num_spk, _p(d_spk), _p(ws), C.c_size_t(nbytes), _stream())
+    capi.check(rc, "pwgb_symbol_embed_backward")
+    return d_emb, d_spk
+
+
+def symbol_embed(c, table, spk_table=None, ds=None, t_out=None, symbol_level=False):
+    """Embedding (+ speaker) of the symbol indices ``c`` (B, 1 or 2, S), channel-major.  With durations ``ds`` the
+    result is length-regulated to (B, C, t_out); ``symbol_level`` also returns the unregulated (B, C, S) embedding (the
+    duration predictor's input).  Differentiable w.r.t. the tables through SymbolEmbedFn, whose backward takes the
+    gradients of both outputs in one pass."""
+    if _needs_grad(table, spk_table):
+        from . import autograd as ag
+
+        return ag.SymbolEmbedFn.apply(table, spk_table, c, ds, t_out, bool(symbol_level and ds is not None))
+    y = symbol_embed_raw(c, table, spk_table, ds, t_out)
+    if symbol_level and ds is not None:
+        return y, symbol_embed_raw(c, table, spk_table)
+    return y
+
+
+def duration_round(x, offset=1.0, ds=None, zero_rule=True):
+    """(ds, totals): ds = clamp(round(exp(x) - offset), min=0) as int64 (layers/duration_predictor.py:79-83), or the
+    given int64 ``ds`` (B, S) with x None; totals (B,) the row sums.  ``zero_rule`` applies the length regulator's
+    rule in place (layers/length_regulator.py:87-95): when the whole batch sums to zero, rows summing to zero become
+    all ones.  One launch -- pwgb_duration_round."""
+    if x is not None:
+        x = _dev(x, "x")
+        B, S = x.shape
+        ds = torch.empty((B, S), device=x.device, dtype=torch.int64)
+    else:
+        B, S = ds.shape
+        ds = _durations(ds, B, S)
+    totals = torch.empty(B, device=ds.device, dtype=torch.int64)
+    rc = capi.lib().pwgb_duration_round(_p(x) if x is not None and x.numel() else None, _p(ds) if ds.numel() else None,
+                                        _p(totals) if B else None, B, S, float(offset), int(bool(zero_rule)), _stream())
+    capi.check(rc, "pwgb_duration_round")
+    return ds, totals
+
+
+def regulated_length(totals):
+    """The largest row total: the time length of the length-regulated tensor.  Sizing that tensor needs it on the host,
+    so this is one device-to-host copy of B int64 (and a synchronisation) per forward with durations -- the reference
+    synchronises at the same point (``ds.sum() == 0`` and ``repeat_interleave``, layers/length_regulator.py:87-97)."""
+    return int(totals.cpu().max()) if totals.numel() else 0
+
+
+def channel_layer_norm_raw(x, gamma, beta, eps, stats=False):
+    """LayerNorm over the channels of (B, C, T) at every (b, t) -- pwgb_channel_layernorm_forward; with ``stats`` also
+    returns the per-(b, t) mean and 1 / std."""
+    x = _dev(x, "x")
+    B, C_, T = x.shape
+    y = torch.empty_like(x)
+    mean = torch.empty((B, T), device=x.device, dtype=torch.float32) if stats else None
+    rstd = torch.empty((B, T), device=x.device, dtype=torch.float32) if stats else None
+    rc = capi.lib().pwgb_channel_layernorm_forward(_p(x) if x.numel() else None, _p(_dev(gamma, "gamma")), _p(_dev(beta, "beta")), B, C_, T,
+                                                   float(eps), _p(y) if y.numel() else None,
+                                                   _p(mean) if stats and mean.numel() else None,
+                                                   _p(rstd) if stats and rstd.numel() else None, _stream())
+    capi.check(rc, "pwgb_channel_layernorm_forward")
+    return (y, mean, rstd) if stats else y
+
+
+def channel_layer_norm(x, gamma, beta, eps):
+    if _needs_grad(x, gamma, beta):
+        from . import autograd as ag
+
+        return ag.ChannelLayerNormFn.apply(x, gamma, beta, float(eps))
+    return channel_layer_norm_raw(x, gamma, beta, eps)
+
+
+def duration_loss_raw(x, ds, offset):
+    """mean((x - log(ds + offset))^2) over all (B, S) as a 1-element tensor -- pwgb_duration_loss_forward."""
+    x = _dev(x, "x")
+    ds = _durations(ds, *x.shape)
+    out = torch.empty(1, device=x.device, dtype=torch.float32)
+    rc = capi.lib().pwgb_duration_loss_forward(_p(x), _p(ds), x.numel(), float(offset), _p(out), _stream())
+    capi.check(rc, "pwgb_duration_loss_forward")
+    return out
+
+
+def duration_loss(x, ds, offset=1.0):
+    if _needs_grad(x):
+        from . import autograd as ag
+
+        return ag.DurationLossFn.apply(x, ds, float(offset))
+    return duration_loss_raw(x, ds, offset)

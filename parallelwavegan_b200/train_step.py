@@ -19,8 +19,9 @@ class GanTrainStep:
                  lambda_feat_match=2.0, grad_norm_g=-1, grad_norm_d=-1, generator_train_start_steps=0,
                  discriminator_train_start_steps=0, update_prediction_after_generator_update=True, sched_g=None, sched_d=None, steps=0):
         """criterion: dict with any of ``stft`` (MultiResolutionSTFTLoss), ``sub_stft``, ``mel``, ``pqmf``, and
-        ``gen_adv`` / ``dis_adv`` / ``feat_match`` -- the keys of ``Trainer.criterion`` (train.py:1384-1451);
-        a key that is present is used (the reference's ``use_*_loss`` switches)."""
+        ``gen_adv`` / ``dis_adv`` / ``feat_match`` and ``duration`` (DurationPredictorLoss) -- the keys of
+        ``Trainer.criterion`` (train.py:1384-1451); a key that is present is used (the reference's ``use_*_loss``
+        switches).  With ``duration`` the generator is a duration model called as ``G(x, ds)`` (train.py:208-213)."""
         self.g, self.d = generator, discriminator
         self.crit = criterion
         self.opt_g, self.opt_d = opt_g, opt_d
@@ -45,24 +46,34 @@ class GanTrainStep:
         if sched is not None:
             sched.step()
 
-    def _generate(self, x):
-        y_ = self.g(*x) if isinstance(x, (tuple, list)) else self.g(x)
+    def _generate(self, x, ds=None):
+        ds_ = None
+        if "duration" in self.crit:
+            y_, ds_ = self.g(x, ds)  # train.py:208-213
+        else:
+            y_ = self.g(*x) if isinstance(x, (tuple, list)) else self.g(x)
         y_mb_ = None
         if "pqmf" in self.crit and y_.shape[1] > 1:  # multi-band: reconstruct the full-band signal (train.py:225-227)
             y_mb_ = y_
             y_ = self.crit["pqmf"].synthesis(y_mb_)
-        return y_, y_mb_
+        return y_, y_mb_, ds_
 
-    def __call__(self, x, y):
-        """x: conditioning (B, mels, frames) or the tuple (z, c) of the Parallel WaveGAN recipes; y: (B, 1, T).
+    def __call__(self, x, y, ds=None):
+        """x: conditioning (B, mels, frames), the tuple (z, c) of the Parallel WaveGAN recipes, or the (B, C, S) symbol
+        codes of the duration recipes with their run lengths ``ds`` (B, S); y: (B, 1, T).
         Returns a dict of loss tensors (device scalars; nothing is synchronised with the host)."""
         stats = {}
         adv_on = self.steps > self.d_start
         y_ = None
         # ---------------- generator phase (train.py:200-295)
         if self.steps > self.g_start:
-            y_, y_mb_ = self._generate(x)
+            y_, y_mb_, ds_ = self._generate(x, ds)
             gen_loss = 0.0
+            if ds_ is not None:
+                # gen_loss starts from the duration loss, so lambda_aux (and the sub-band 0.5) scale it too (train.py:213-262)
+                dur = self.crit["duration"](ds_, ds)
+                stats["duration_loss"] = dur.detach()
+                gen_loss = gen_loss + dur
             if "stft" in self.crit:
                 sc, mag = self.crit["stft"](y_, y)
                 stats["spectral_convergence_loss"], stats["log_stft_magnitude_loss"] = sc.detach(), mag.detach()
@@ -102,7 +113,7 @@ class GanTrainStep:
         if adv_on:
             if self.update_prediction or y_ is None:
                 with torch.no_grad():
-                    y_, _ = self._generate(x)
+                    y_, _, _ = self._generate(x, ds)
             p = self.d(y)
             p_ = self.d(y_.detach())
             real, fake = self.crit["dis_adv"](p_, p)
