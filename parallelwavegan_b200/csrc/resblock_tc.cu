@@ -9,15 +9,19 @@
 // chunk, tap, k16 step, hi*hi, lo*hi, hi*lo), so the result is bit-identical to the two conv1d_tc launches.
 //
 // Tiling: a tile produces M2 output rows [t0, t0 + M2).  Conv2 needs h rows [t0 - p2, t0 + M2 + p2), p2 = (k-1)/2;
-// conv1 computes the TT = 128 MT rows [t0 - p2, t0 - p2 + TT) (two warpgroups of MT 64-row blocks) from
-// R1 = TT + (k-1) d input rows, so M2 = TT - (k-1) rounded down to a multiple of 4 (16-byte output rows).  Halo rows of
-// h are recomputed by the neighbouring tile.  Conv2 also runs TT rows per tile; rows >= M2 read beyond the computed h
-// rows and are dropped.
-// Warp roles (576 threads, one persistent CTA per SM), as in conv1d_tc_kernel with TMA-staged activations:
-//   warps 0-7   convert landed raw fp32 rows of x (pre-activation, padding mask, hi/lo split) into conv1's operand image
-//   warps 8-15  two consumer warpgroups: conv1 wgmma, h image, conv2 wgmma on it, staged epilogue (bulk copies)
-//   warp 16     weight stages (conv1's then conv2's of every tile) by cp.async.bulk
-//   warp 17     raw activation rows by cp.async.bulk
+// conv1 computes the TT conv rows [t0 - p2, t0 - p2 + TT) from R1 = TT + (k-1) d input rows, so M2 = TT - (k-1)
+// rounded down to a multiple of 4 (16-byte output rows).  Halo rows of h are recomputed by the neighbouring tile.  Conv2
+// also runs TT rows per tile; rows >= M2 read beyond the computed h rows and are dropped.
+//
+// Two kernels, one persistent CTA per SM each, with the producers and loaders of conv1d_tc_kernel with TMA-staged
+// activations: producer warps convert landed raw fp32 rows of x (pre-activation, padding mask, hi/lo split) into conv1's
+// operand image, two consumer warpgroups run the MMAs, one warp loads weight stages and one raw activation rows, both by
+// cp.async.bulk.
+// rb_pair_split_kernel (the default, 512 threads): warpgroup 0 runs conv1 of every tile and writes the h image,
+// warpgroup 1 runs conv2 on it and the staged epilogue, so that one warpgroup's drain, h write or epilogue overlaps the
+// other's MMAs.  Each conv owns a weight ring.  resblock_pair_kernel (lockstep, 576 threads): both warpgroups split a
+// tile by rows and run conv1, the h write, conv2 and the epilogue one after another; it is kept for the plans the split
+// kernel cannot fit (wide conv1 halos) and for A/B timing (pwgb_debug_set(3, 1)).
 #include <cstring>
 
 #include "tc_common.cuh"
@@ -32,22 +36,153 @@ constexpr int RB_W_CONS0 = RB_NPROD / 32, RB_W_TMA = (RB_NPROD + RB_NCONS) / 32,
 constexpr int RB_THREADS = RB_NPROD + RB_NCONS + 64;
 __host__ __device__ constexpr int rb_sld(int mt) { return 64 * mt + 4; }  // staged epilogue row pitch, as in conv1d_tc.cu
 constexpr size_t RB_SMEM = 227 * 1024;      // H100 opt-in limit of dynamic shared memory per block
-constexpr int RB_MIN_STAGES = 4;            // weight stages a plan must keep
+constexpr int RB_MIN_STAGES = 4;            // weight stages a plan must keep (per ring)
+
+int g_rb_lockstep = 0;  // pwgb_debug_set(3, 1): plan every pair for the lockstep kernel
 
 struct RbK {
   int B, C, T, K, D;
   float slope, out_scale;
   int accumulate;
-  int MT, M2;              // 64-row blocks per consumer warpgroup (conv rows per tile: 128 MT), output rows per tile
+  int split;               // 1: rb_pair_split_kernel, 0: resblock_pair_kernel
+  int MT, M2;              // 64-row blocks per consumer warpgroup, output rows per tile
   int p1, p2;              // left padding of conv1 ((k-1)/2 * d) and conv2 ((k-1)/2)
-  int R1, R4, Rh;          // conv1 operand rows, raw stage row pitch (floats), h image rows (128 MT + k - 1)
+  int R1, R4, Rh;          // conv1 operand rows, raw stage row pitch (floats), h image rows (TT + k - 1)
   int nchunks, tiles_per_seq, total_tiles;
-  int na, nb, ns;          // conv1 operand buffers, weight stages, raw stages
+  int na, nb, ns;          // conv1 operand buffers, weight stages (both rings of the split kernel), raw stages
   int a_bytes, b_bytes, raw_bytes, h_bytes;  // per buffer / stage; h_bytes: one 32-channel chunk of the h image
 };
 
 // consumers of both warpgroups (named barrier 4; 1 = conv producers, 2-3 = per-warpgroup barriers)
 __device__ __forceinline__ void consumer_barrier() { asm volatile("bar.sync 4, %0;" ::"n"(RB_NCONS) : "memory"); }
+
+// ===================== A producers: raw fp32 rows -> conv1 operand image =====================
+// NPROD producer threads, this one `tid` of them.  Barrier arguments are the first of each array of 8-byte mbarriers.
+template <int NCH, int NPROD>
+__device__ __forceinline__ void rb_convert_x(const RbK& p, unsigned char* a_buf, const unsigned char* raw_buf, unsigned a_full,
+                                             unsigned a_empty, unsigned raw_full, unsigned raw_empty, int tid) {
+  int s = 0, sph = 0, buf = 0, aph = 0;
+  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    const int b = tile / p.tiles_per_seq;
+    const int t0 = (tile - b * p.tiles_per_seq) * p.M2;
+    const int ts_first = t0 - p.p2 - p.p1;
+    const int shift = ts_first - (ts_first & ~3);
+    for (int c = 0; c < NCH; ++c) {
+      mbar_wait(raw_full + 8u * s, sph);
+      mbar_wait(a_empty + 8u * buf, aph ^ 1);
+      unsigned char* dst = a_buf + (size_t)buf * p.a_bytes;
+      const float* raw = reinterpret_cast<const float*>(raw_buf + (size_t)s * p.raw_bytes);
+      for (int r = tid; r < p.R1; r += NPROD) {
+        const bool ok = (unsigned)(ts_first + r) < (unsigned)p.T;
+        const float* rr = raw + r + shift;
+#pragma unroll
+        for (int g = 0; g < KC / 8; ++g) {
+          float u[8];
+#pragma unroll
+          for (int j = 0; j < 8; ++j) u[j] = ok ? lrelu(rr[(g * 8 + j) * p.R4], p.slope) : 0.f;
+          uint4 hi, lo;
+          split8(u, hi, lo);
+          *reinterpret_cast<uint4*>(dst + ((size_t)g * p.R1 + r) * 16) = hi;
+          *reinterpret_cast<uint4*>(dst + ((size_t)(KC / 8 + g) * p.R1 + r) * 16) = lo;
+        }
+      }
+      fence_proxy_async();
+      mbar_arrive(a_full + 8u * buf);
+      mbar_arrive(raw_empty + 8u * s);
+      if (++s == p.ns) { s = 0; sph ^= 1; }
+      if (++buf == p.na) { buf = 0; aph ^= 1; }
+    }
+  }
+}
+
+// ===================== raw activation rows of x (one channel per lane) =====================
+template <int NCH>
+__device__ __forceinline__ void rb_load_raw(const RbK& p, const float* __restrict__ x, unsigned char* raw_buf, unsigned raw_full,
+                                            unsigned raw_empty, int lane) {
+  constexpr int C = NCH * KC;
+  int s = 0, ph = 0;
+  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    const int b = tile / p.tiles_per_seq;
+    const int t0 = (tile - b * p.tiles_per_seq) * p.M2;
+    const int ts0 = (t0 - p.p2 - p.p1) & ~3;
+    const int start = ts0 < 0 ? 0 : ts0;
+    const int end = ts0 + p.R4 < p.T ? ts0 + p.R4 : p.T;
+    const int nbytes = (end - start) * 4;
+    for (int c = 0; c < NCH; ++c) {
+      mbar_wait(raw_empty + 8u * s, ph ^ 1);
+      if (nbytes > 0) {
+        if (lane == 0) mbar_expect_tx(raw_full + 8u * s, (unsigned)nbytes * KC);
+        __syncwarp();
+        bulk_g2s(smem_u32(raw_buf + (size_t)s * p.raw_bytes) + (unsigned)(lane * p.R4 + start - ts0) * 4u,
+                 x + ((long long)b * C + c * KC + lane) * p.T + start, (unsigned)nbytes, raw_full + 8u * s);
+      } else if (lane == 0) {
+        mbar_arrive(raw_full + 8u * s);
+      }
+      __syncwarp();
+      if (++s == p.ns) { s = 0; ph ^= 1; }
+    }
+  }
+}
+
+// One weight stage of wgmma on the operand image at `a_img` (rows `row0` ..): per k16 step and 64-row block, the three
+// bf16x3 products.  One commit group per call.
+template <int MT, int NB16>
+__device__ __forceinline__ void rb_mma_stage(float* acc, unsigned a_img, unsigned lbo, unsigned sub, int row0, unsigned b_addr) {
+  constexpr int NACC = 8 * NB16;
+  constexpr unsigned lbo_b = NB16 * 256u, b_sub = (KC / 8) * NB16 * 16u;
+  wg_fence();
+#pragma unroll
+  for (int ks = 0; ks < KC / 16; ++ks) {
+    const unsigned long long bh = gmma_desc(b_addr + (unsigned)(2 * ks) * lbo_b, lbo_b, 128);
+    const unsigned long long ah0 = gmma_desc(a_img + ((unsigned)(2 * ks) * (lbo / 16u) + (unsigned)row0) * 16u, lbo, 128);
+#pragma unroll
+    for (int mb = 0; mb < MT; ++mb) {
+      const unsigned long long ah = ah0 + 64 * mb;  // next 64 rows: 64 x 16 B
+      wgmma_n<0, 0, NB16>(acc + mb * NACC, ah, bh, 16);
+      wgmma_n<0, 0, NB16>(acc + mb * NACC, ah + sub, bh, 16);
+      wgmma_n<0, 0, NB16>(acc + mb * NACC, ah, bh + b_sub, 16);
+    }
+  }
+  wg_commit();
+}
+
+// h = lrelu(acc + b1) of the warpgroup's conv rows [row_base, row_base + 64 MT) (time th0 + r for fragment row r) as
+// conv2's operand image; rows outside [0, T) are conv2's zero padding
+template <int MT, int NB16>
+__device__ __forceinline__ void rb_write_h(const float* acc, unsigned char* h_buf, const RbK& p, int row_base, int th0,
+                                           const float* bias1, int lane, int wq) {
+  constexpr int NACC = 8 * NB16;
+#pragma unroll
+  for (int e = 0; e < MT * NACC; e += 2) {
+    const int i = e % NACC;
+    const int col = 8 * (i >> 2) + 2 * (lane & 3);
+    const int r = (e / NACC) * 64 + wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+    const bool ok = (unsigned)(th0 + r) < (unsigned)p.T;
+    const float h0 = acc[e] + bias1[col], h1 = acc[e + 1] + bias1[col + 1];
+    unsigned hi, lo;
+    split2(ok ? lrelu(h0, p.slope) : 0.f, ok ? lrelu(h1, p.slope) : 0.f, hi, lo);
+    unsigned char* hc = h_buf + (size_t)(col >> 5) * p.h_bytes;
+    const size_t off = ((size_t)((col & 31) >> 3) * p.Rh + row_base + r) * 16 + (col & 7) * 2;
+    *reinterpret_cast<unsigned*>(hc + off) = hi;
+    *reinterpret_cast<unsigned*>(hc + (size_t)(KC / 8) * p.Rh * 16 + off) = lo;
+  }
+}
+
+// staged epilogue in place over the residual rows of the tile `stg` ([channel][rb_sld(MT)]): v = (a + b2 + x) * out_scale
+template <int MT, int NB16>
+__device__ __forceinline__ void rb_stage_result(const float* acc, float* stg, const float* bias2, float out_scale, int lane,
+                                                int wq) {
+  constexpr int NACC = 8 * NB16, SLD = rb_sld(MT);
+#pragma unroll
+  for (int e = 0; e < MT * NACC; ++e) {
+    const int i = e % NACC;
+    const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+    float* sv = stg + col * SLD + (e / NACC) * 64 + wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+    float v = acc[e] + bias2[col];
+    v += *sv;
+    *sv = v * out_scale;
+  }
+}
 
 // MT: 64-row blocks per consumer warpgroup; NB16: channels / 16 (the MMA width; the weight images are the conv1d_tc
 // images of a Cout = C conv)
@@ -107,45 +242,12 @@ __global__ void __launch_bounds__(RB_THREADS, 1)
   __syncthreads();
 
   if (warp < RB_W_CONS0) {
-    // ===================== A producers: raw fp32 rows -> conv1 operand image =====================
-    int s = 0, sph = 0, buf = 0, aph = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      const int b = tile / p.tiles_per_seq;
-      const int t0 = (tile - b * p.tiles_per_seq) * p.M2;
-      const int ts_first = t0 - p.p2 - p.p1;
-      const int shift = ts_first - (ts_first & ~3);
-      for (int c = 0; c < NCH; ++c) {
-        mbar_wait(RAW_FULL(s), sph);
-        mbar_wait(A_EMPTY(buf), aph ^ 1);
-        unsigned char* dst = a_buf + (size_t)buf * p.a_bytes;
-        const float* raw = reinterpret_cast<const float*>(raw_buf + (size_t)s * p.raw_bytes);
-        for (int r = tid; r < p.R1; r += RB_NPROD) {
-          const bool ok = (unsigned)(ts_first + r) < (unsigned)p.T;
-          const float* rr = raw + r + shift;
-#pragma unroll
-          for (int g = 0; g < KC / 8; ++g) {
-            float u[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) u[j] = ok ? lrelu(rr[(g * 8 + j) * p.R4], p.slope) : 0.f;
-            uint4 hi, lo;
-            split8(u, hi, lo);
-            *reinterpret_cast<uint4*>(dst + ((size_t)g * p.R1 + r) * 16) = hi;
-            *reinterpret_cast<uint4*>(dst + ((size_t)(KC / 8 + g) * p.R1 + r) * 16) = lo;
-          }
-        }
-        fence_proxy_async();
-        mbar_arrive(A_FULL(buf));
-        mbar_arrive(RAW_EMPTY(s));
-        if (++s == p.ns) { s = 0; sph ^= 1; }
-        if (++buf == p.na) { buf = 0; aph ^= 1; }
-      }
-    }
+    rb_convert_x<NCH, RB_NPROD>(p, a_buf, raw_buf, A_FULL(0), A_EMPTY(0), RAW_FULL(0), RAW_EMPTY(0), tid);
   } else if (warp < RB_W_TMA) {
     // ===================== consumers =====================
     // warpgroup wg owns conv rows [WR wg, WR wg + WR) of both convs.  One wgmma group per (chunk, tap), kept in flight
     // while the next is issued, as in conv1d_tc_kernel.
     const int wg = (warp - RB_W_CONS0) >> 2, wq = warp & 3;
-    const unsigned lbo_b = NB16 * 256u, b_sub = (KC / 8) * NB16 * 16u;
     const unsigned lbo_a = (unsigned)p.R1 * 16u, a_sub = (unsigned)(KC / 8) * p.R1;
     const unsigned lbo_h = (unsigned)p.Rh * 16u, h_sub = (unsigned)(KC / 8) * p.Rh;
     // staged epilogue: thread wt of the warpgroup owns channel row wt of the warpgroup's tile (residual in, result out)
@@ -176,24 +278,6 @@ __global__ void __launch_bounds__(RB_THREADS, 1)
         mbar_arrive(RES_FULL(wg));
       }
     };
-    // one weight stage of wgmma on the operand image at `a_img` (rows `row0` ..): per k16 step and 64-row block, the
-    // three bf16x3 products
-    auto mma_stage = [&](float* acc, unsigned a_img, unsigned lbo, unsigned sub, int row0, unsigned b_addr) {
-      wg_fence();
-#pragma unroll
-      for (int ks = 0; ks < KC / 16; ++ks) {
-        const unsigned long long bh = gmma_desc(b_addr + (unsigned)(2 * ks) * lbo_b, lbo_b, 128);
-        const unsigned long long ah0 = gmma_desc(a_img + ((unsigned)(2 * ks) * (lbo / 16u) + (unsigned)row0) * 16u, lbo, 128);
-#pragma unroll
-        for (int mb = 0; mb < MT; ++mb) {
-          const unsigned long long ah = ah0 + 64 * mb;  // next 64 rows: 64 x 16 B
-          wgmma_n<0, 0, NB16>(acc + mb * NACC, ah, bh, 16);
-          wgmma_n<0, 0, NB16>(acc + mb * NACC, ah + sub, bh, 16);
-          wgmma_n<0, 0, NB16>(acc + mb * NACC, ah, bh + b_sub, 16);
-        }
-      }
-      wg_commit();
-    };
     auto release = [&](int held_s, int held_a) {
       __syncwarp();
       if (lane == 0) {
@@ -216,7 +300,7 @@ __global__ void __launch_bounds__(RB_THREADS, 1)
         for (int k = 0; k < p.K; ++k) {
           mbar_wait_trap(B_FULL(s), bph);
           __syncwarp();
-          mma_stage(acc, a_addr, lbo_a, a_sub, k * p.D + wg * WR, smem_u32(b_buf + (size_t)s * p.b_bytes));
+          rb_mma_stage<MT, NB16>(acc, a_addr, lbo_a, a_sub, k * p.D + wg * WR, smem_u32(b_buf + (size_t)s * p.b_bytes));
           wg_wait<1>();  // the previous group has retired: its stage and, at a chunk boundary, its A buffer are free
           release(held_s, held_a);
           held_s = s;
@@ -227,24 +311,9 @@ __global__ void __launch_bounds__(RB_THREADS, 1)
       }
       wg_wait<0>();
       release(held_s, held_a);
-      // ---- h = lrelu(acc + b1) as conv2's operand image; rows outside [0, T) are conv2's zero padding.  Both
-      // warpgroups' conv2 MMAs of the previous tile must have read the image first.
+      // ---- h image.  Both warpgroups' conv2 MMAs of the previous tile must have read the image first.
       consumer_barrier();
-      const int th0 = t0 - p.p2 + wg * WR;
-#pragma unroll
-      for (int e = 0; e < MT * NACC; e += 2) {
-        const int i = e % NACC;
-        const int col = 8 * (i >> 2) + 2 * (lane & 3);
-        const int r = (e / NACC) * 64 + wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
-        const bool ok = (unsigned)(th0 + r) < (unsigned)p.T;
-        const float h0 = acc[e] + bias_s[col], h1 = acc[e + 1] + bias_s[col + 1];
-        unsigned hi, lo;
-        split2(ok ? lrelu(h0, p.slope) : 0.f, ok ? lrelu(h1, p.slope) : 0.f, hi, lo);
-        unsigned char* hc = h_buf + (size_t)(col >> 5) * p.h_bytes;
-        const size_t off = ((size_t)((col & 31) >> 3) * p.Rh + wg * WR + r) * 16 + (col & 7) * 2;
-        *reinterpret_cast<unsigned*>(hc + off) = hi;
-        *reinterpret_cast<unsigned*>(hc + (size_t)(KC / 8) * p.Rh * 16 + off) = lo;
-      }
+      rb_write_h<MT, NB16>(acc, h_buf, p, wg * WR, t0 - p.p2 + wg * WR, bias_s, lane, wq);
       fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor core
       consumer_barrier();
       // ---- conv2 over the h image (resident for the whole tile)
@@ -256,7 +325,7 @@ __global__ void __launch_bounds__(RB_THREADS, 1)
         for (int k = 0; k < p.K; ++k) {
           mbar_wait_trap(B_FULL(s), bph);
           __syncwarp();
-          mma_stage(acc, h_addr, lbo_h, h_sub, k + wg * WR, smem_u32(b_buf + (size_t)s * p.b_bytes));
+          rb_mma_stage<MT, NB16>(acc, h_addr, lbo_h, h_sub, k + wg * WR, smem_u32(b_buf + (size_t)s * p.b_bytes));
           wg_wait<1>();
           release(held_s, -1);
           held_s = s;
@@ -265,17 +334,9 @@ __global__ void __launch_bounds__(RB_THREADS, 1)
       }
       wg_wait<0>();
       release(held_s, -1);
-      // ---- staged epilogue: v = (a + b2 + x) * out_scale over the residual row, one bulk store (or fp32 add) per row
+      // ---- staged epilogue over the residual row, one bulk store (or fp32 add) per row
       mbar_wait_trap(RES_FULL(wg), ((tile - blockIdx.x) / gridDim.x) & 1);  // one phase per tile
-#pragma unroll
-      for (int e = 0; e < MT * NACC; ++e) {
-        const int i = e % NACC;
-        const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
-        float* sv = stg + col * SLD + (e / NACC) * 64 + wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
-        float v = acc[e] + bias_s[C + col];
-        v += *sv;
-        *sv = v * p.out_scale;
-      }
+      rb_stage_result<MT, NB16>(acc, stg, bias_s + C, p.out_scale, lane, wq);
       fence_proxy_async();  // generic-proxy writes -> visible to the bulk copies
       wg_barrier(wg);
       if (row_owner) {
@@ -309,37 +370,236 @@ __global__ void __launch_bounds__(RB_THREADS, 1)
       }
     }
   } else if (warp == RB_W_LDA) {
-    // ===================== raw activation rows of x (one channel per lane) =====================
-    int s = 0, ph = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    rb_load_raw<NCH>(p, x, raw_buf, RAW_FULL(0), RAW_EMPTY(0), lane);
+  }
+}
+
+// Conv split by warpgroup.  MT = TT / 64: the 64-row blocks of a whole tile, run by one warpgroup (independent
+// accumulator chains: 2 at 64 channels, 4 at 32, 64 accumulator registers either way).  Warpgroup 0 runs conv1 of tile
+// i + 1 while warpgroup 1 runs conv2 and the epilogue of tile i; they hand the single h image over through two
+// mbarriers (H_FULL: written, H_FREE: conv2's MMAs have retired).  Weights come in two rings of nb / 2 stages, conv1's
+// and conv2's, both filled by the weight warp.  The residual rows belong to conv2's warpgroup.
+// 512 threads, so that a thread may hold 128 registers (warps are allocated in fours: at 18 warps the limit is 96, and
+// the 64 accumulator registers spill): warps 0-3 conv1, warps 4-7 conv2 and the epilogue, warps 8-13 the producers
+// (a chunk has at most TT + 50 conv1 rows), warp 14 the weight rings, warp 15 the raw activation rows.
+constexpr int RBS_NPROD = 192;
+constexpr int RBS_W_PROD0 = 8, RBS_W_TMA = RBS_W_PROD0 + RBS_NPROD / 32, RBS_W_LDA = RBS_W_TMA + 1;
+constexpr int RBS_THREADS = 32 * (RBS_W_LDA + 1);
+
+template <int MT, int NB16>
+__global__ void __launch_bounds__(RBS_THREADS, 1)
+    rb_pair_split_kernel(const RbK p, const float* __restrict__ x, const unsigned char* __restrict__ w1,
+                         const float* __restrict__ b1, const unsigned char* __restrict__ w2, const float* __restrict__ b2,
+                         float* __restrict__ y) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  constexpr int C = 16 * NB16, NCH = C / KC, NACC = 8 * NB16, SLD = rb_sld(MT);
+  const int nr = p.nb / 2;  // stages per weight ring
+  // layout: A[na] | B1[nr] | B2[nr] | raw staging[ns] | h image[NCH chunks] | epilogue tile | barriers | bias1 | bias2
+  unsigned char* a_buf = smem;
+  unsigned char* b1_buf = a_buf + (size_t)p.na * p.a_bytes;
+  unsigned char* b2_buf = b1_buf + (size_t)nr * p.b_bytes;
+  unsigned char* raw_buf = b2_buf + (size_t)nr * p.b_bytes;
+  unsigned char* h_buf = raw_buf + (size_t)p.ns * p.raw_bytes;
+  float* stg = reinterpret_cast<float*>(h_buf + (size_t)NCH * p.h_bytes);
+  unsigned long long* bars = reinterpret_cast<unsigned long long*>(stg + C * SLD);
+  const int nbar = 2 * p.na + 2 * p.nb + 2 * p.ns + 3;
+  float* bias_s = reinterpret_cast<float*>(bars + nbar);  // b1 | b2 (zeros for a missing bias)
+
+  const int tid = threadIdx.x;
+  const int warp = tid >> 5;
+  const int lane = tid & 31;
+
+  const unsigned bar0 = smem_u32(bars);
+  const unsigned A_FULL = bar0, A_EMPTY = A_FULL + 8u * p.na;
+  const unsigned B1_FULL = A_EMPTY + 8u * p.na, B1_EMPTY = B1_FULL + 8u * nr;
+  const unsigned B2_FULL = B1_EMPTY + 8u * nr, B2_EMPTY = B2_FULL + 8u * nr;
+  const unsigned RAW_FULL = B2_EMPTY + 8u * nr, RAW_EMPTY = RAW_FULL + 8u * p.ns;
+  const unsigned RES_FULL = RAW_EMPTY + 8u * p.ns, H_FULL = RES_FULL + 8u, H_FREE = H_FULL + 8u;
+
+  if (tid == 0) {
+    for (int i = 0; i < p.na; ++i) {
+      mbar_init(A_FULL + 8u * i, RBS_NPROD);
+      mbar_init(A_EMPTY + 8u * i, 4);  // the warps of conv1's warpgroup
+    }
+    for (int i = 0; i < nr; ++i) {
+      mbar_init(B1_FULL + 8u * i, 1);
+      mbar_init(B1_EMPTY + 8u * i, 4);
+      mbar_init(B2_FULL + 8u * i, 1);
+      mbar_init(B2_EMPTY + 8u * i, 4);
+    }
+    for (int i = 0; i < p.ns; ++i) {
+      mbar_init(RAW_FULL + 8u * i, 1);
+      mbar_init(RAW_EMPTY + 8u * i, RBS_NPROD);
+    }
+    mbar_init(RES_FULL, C);  // one arrival per channel row of the tile
+    mbar_init(H_FULL, 128);
+    mbar_init(H_FREE, 128);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  for (int i = tid; i < 2 * C; i += RBS_THREADS) {
+    const float* bb = i < C ? b1 : b2;
+    bias_s[i] = bb ? __ldg(bb + (i < C ? i : i - C)) : 0.f;
+  }
+  // conv2 rows >= M2 read the h rows [64 MT, Rh) that no tile writes: keep them zero
+  for (int i = tid; i < NCH * p.h_bytes / 16; i += RBS_THREADS) reinterpret_cast<uint4*>(h_buf)[i] = make_uint4(0, 0, 0, 0);
+  fence_proxy_async();
+  __syncthreads();
+
+  if (warp < 4) {
+    // ===================== conv1: staged x rows -> h image =====================
+    // One wgmma group per (chunk, tap), kept in flight while the next is issued, as in conv1d_tc_kernel.
+    const int wq = warp & 3;
+    const unsigned lbo_a = (unsigned)p.R1 * 16u, a_sub = (unsigned)(KC / 8) * p.R1;
+    int buf = 0, aph = 0, s = 0, bph = 0, n = 0;
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++n) {
+      float acc[MT * NACC];
+#pragma unroll
+      for (int e = 0; e < MT * NACC; ++e) acc[e] = 0.f;
+      int held_s = -1, held_a = -1;  // weight stage / A buffer read by the group in flight
+      auto release = [&]() {
+        __syncwarp();
+        if (lane == 0) {
+          if (held_s >= 0) mbar_arrive(B1_EMPTY + 8u * held_s);
+          if (held_a >= 0) mbar_arrive(A_EMPTY + 8u * held_a);
+        }
+      };
+      for (int c = 0; c < NCH; ++c) {
+        mbar_wait_trap(A_FULL + 8u * buf, aph);
+        const unsigned a_addr = smem_u32(a_buf + (size_t)buf * p.a_bytes);
+        for (int k = 0; k < p.K; ++k) {
+          mbar_wait_trap(B1_FULL + 8u * s, bph);
+          __syncwarp();
+          rb_mma_stage<MT, NB16>(acc, a_addr, lbo_a, a_sub, k * p.D, smem_u32(b1_buf + (size_t)s * p.b_bytes));
+          wg_wait<1>();  // the previous group has retired: its stage and, at a chunk boundary, its A buffer are free
+          release();
+          held_s = s;
+          held_a = k == p.K - 1 ? buf : -1;
+          if (++s == nr) { s = 0; bph ^= 1; }
+        }
+        if (++buf == p.na) { buf = 0; aph ^= 1; }
+      }
+      wg_wait<0>();
+      release();
+      mbar_wait_trap(H_FREE, (n & 1) ^ 1);  // conv2 of the previous tile has read the image
+      const int t0 = (tile % p.tiles_per_seq) * p.M2;
+      rb_write_h<MT, NB16>(acc, h_buf, p, 0, t0 - p.p2, bias_s, lane, wq);
+      fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor core
+      mbar_arrive(H_FULL);
+    }
+  } else if (warp < 8) {
+    // ===================== conv2 on the h image, staged epilogue =====================
+    const int wq = warp & 3;
+    const unsigned lbo_h = (unsigned)p.Rh * 16u, h_sub = (unsigned)(KC / 8) * p.Rh;
+    // thread wt of the warpgroup owns channel row wt of the tile (residual in, result out)
+    const int wt = tid - 128;
+    const bool row_owner = wt < C;
+    // channel row wt of a tile's output rows: first element and bytes (below M2 and T)
+    auto row_pos = [&](int tile, unsigned& row_bytes) -> long long {
       const int b = tile / p.tiles_per_seq;
       const int t0 = (tile - b * p.tiles_per_seq) * p.M2;
-      const int ts0 = (t0 - p.p2 - p.p1) & ~3;
-      const int start = ts0 < 0 ? 0 : ts0;
-      const int end = ts0 + p.R4 < p.T ? ts0 + p.R4 : p.T;
-      const int nbytes = (end - start) * 4;
-      for (int c = 0; c < NCH; ++c) {
-        mbar_wait(RAW_EMPTY(s), ph ^ 1);
-        if (nbytes > 0) {
-          if (lane == 0) mbar_expect_tx(RAW_FULL(s), (unsigned)nbytes * KC);
-          __syncwarp();
-          bulk_g2s(smem_u32(raw_buf + (size_t)s * p.raw_bytes) + (unsigned)(lane * p.R4 + start - ts0) * 4u,
-                   x + ((long long)b * C + c * KC + lane) * p.T + start, (unsigned)nbytes, RAW_FULL(s));
-        } else if (lane == 0) {
-          mbar_arrive(RAW_FULL(s));
-        }
+      const int nrow = p.M2 < p.T - t0 ? p.M2 : p.T - t0;
+      row_bytes = nrow > 0 ? 4u * (unsigned)nrow : 0u;
+      return ((long long)b * C + wt) * p.T + t0;
+    };
+    // the residual (x itself) of a tile, issued at the end of the previous tile's epilogue so that it streams in while
+    // this tile's MMAs run
+    auto load_res = [&](int tile) {
+      unsigned row_bytes;
+      const long long off = row_pos(tile, row_bytes);
+      bulk_wait_read();  // the previous store has read the row
+      if (row_bytes) {
+        mbar_expect_tx(RES_FULL, row_bytes);
+        bulk_g2s(smem_u32(stg + wt * SLD), x + off, row_bytes, RES_FULL);
+      } else {
+        mbar_arrive(RES_FULL);
+      }
+    };
+    if (row_owner && (int)blockIdx.x < p.total_tiles) load_res(blockIdx.x);
+    int s = 0, bph = 0, n = 0;
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++n) {
+      float acc[MT * NACC];
+#pragma unroll
+      for (int e = 0; e < MT * NACC; ++e) acc[e] = 0.f;
+      int held_s = -1;
+      auto release = [&]() {
         __syncwarp();
-        if (++s == p.ns) { s = 0; ph ^= 1; }
+        if (lane == 0 && held_s >= 0) mbar_arrive(B2_EMPTY + 8u * held_s);
+      };
+      mbar_wait_trap(H_FULL, n & 1);
+      for (int c = 0; c < NCH; ++c) {
+        const unsigned h_addr = smem_u32(h_buf + (size_t)c * p.h_bytes);
+        for (int k = 0; k < p.K; ++k) {
+          mbar_wait_trap(B2_FULL + 8u * s, bph);
+          __syncwarp();
+          rb_mma_stage<MT, NB16>(acc, h_addr, lbo_h, h_sub, k, smem_u32(b2_buf + (size_t)s * p.b_bytes));
+          wg_wait<1>();
+          release();
+          held_s = s;
+          if (++s == nr) { s = 0; bph ^= 1; }
+        }
+      }
+      wg_wait<0>();
+      release();
+      mbar_arrive(H_FREE);
+      // ---- staged epilogue over the residual row, one bulk store (or fp32 add) per row
+      mbar_wait_trap(RES_FULL, n & 1);  // one phase per tile
+      rb_stage_result<MT, NB16>(acc, stg, bias_s + C, p.out_scale, lane, wq);
+      fence_proxy_async();  // generic-proxy writes -> visible to the bulk copies
+      wg_barrier(1);
+      if (row_owner) {
+        unsigned row_bytes;
+        const long long off = row_pos(tile, row_bytes);
+        if (row_bytes) {
+          if (p.accumulate)
+            bulk_s2g_add(y + off, smem_u32(stg + wt * SLD), row_bytes);
+          else
+            bulk_s2g(y + off, smem_u32(stg + wt * SLD), row_bytes);
+          bulk_commit();
+        }
+        if (tile + (int)gridDim.x < p.total_tiles) load_res(tile + gridDim.x);
       }
     }
+    if (row_owner) bulk_wait();  // the shared-memory source must outlive the CTA's last stores
+  } else if (warp < RBS_W_TMA) {
+    rb_convert_x<NCH, RBS_NPROD>(p, a_buf, raw_buf, A_FULL, A_EMPTY, RAW_FULL, RAW_EMPTY, tid - 32 * RBS_W_PROD0);
+  } else if (warp == RBS_W_TMA) {
+    // ===================== weight stages: both rings, NCH * K stages per tile each =====================
+    // The two convs run different tiles, so one lane polls both rings and fills whichever has a free stage.
+    if (lane == 0) {
+      const int per = NCH * p.K;
+      const int ntiles = (int)blockIdx.x < p.total_tiles ? (p.total_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+      int n1 = 0, j1 = 0, s1 = 0, ph1 = 0, n2 = 0, j2 = 0, s2 = 0, ph2 = 0;
+      unsigned idle = 0;
+      while (n1 < ntiles || n2 < ntiles) {
+        bool moved = false;
+        if (n1 < ntiles && mbar_try(B1_EMPTY + 8u * s1, ph1 ^ 1)) {
+          mbar_expect_tx(B1_FULL + 8u * s1, (unsigned)p.b_bytes);
+          bulk_g2s(smem_u32(b1_buf + (size_t)s1 * p.b_bytes), w1 + (size_t)j1 * p.b_bytes, (unsigned)p.b_bytes, B1_FULL + 8u * s1);
+          if (++j1 == per) { j1 = 0; ++n1; }
+          if (++s1 == nr) { s1 = 0; ph1 ^= 1; }
+          moved = true;
+        }
+        if (n2 < ntiles && mbar_try(B2_EMPTY + 8u * s2, ph2 ^ 1)) {
+          mbar_expect_tx(B2_FULL + 8u * s2, (unsigned)p.b_bytes);
+          bulk_g2s(smem_u32(b2_buf + (size_t)s2 * p.b_bytes), w2 + (size_t)j2 * p.b_bytes, (unsigned)p.b_bytes, B2_FULL + 8u * s2);
+          if (++j2 == per) { j2 = 0; ++n2; }
+          if (++s2 == nr) { s2 = 0; ph2 ^= 1; }
+          moved = true;
+        }
+        if (moved) idle = 0;
+        else if (++idle > SPIN_LIMIT) __trap();
+      }
+    }
+  } else if (warp == RBS_W_LDA) {
+    rb_load_raw<NCH>(p, x, raw_buf, RAW_FULL, RAW_EMPTY, lane);
   }
 }
 
 using RbKernel = void (*)(const RbK, const float*, const unsigned char*, const float*, const unsigned char*, const float*,
                           float*);
 
-// Instantiations: 32 and 64 channels at MT = 1, and 32 channels at MT = 2 (at 64 channels a 256-row tile's h image and
-// epilogue tiles alone would take 135 KB).
+// Lockstep instantiations: 32 and 64 channels at MT = 1, and 32 channels at MT = 2 (at 64 channels a 256-row tile's h
+// image and epilogue tiles alone would take 135 KB).
 RbKernel rb_kernel_for(int mt, int channels) {
   if (mt == 1 && channels == 32) return resblock_pair_kernel<1, 2>;
   if (mt == 1 && channels == 64) return resblock_pair_kernel<1, 4>;
@@ -347,11 +607,57 @@ RbKernel rb_kernel_for(int mt, int channels) {
   return nullptr;
 }
 
-// Plan of one pair.  A warpgroup's 64-row blocks are independent accumulator chains, so the planner tries MT = 2 first
-// (the wgmma of one chain wait for each other: at MT = 1 and 32 channels the tensor cores idle between them), then
-// MT = 1.  Per tile shape: two conv1 operand buffers with three, then two raw stages; then, with one 32-channel chunk,
-// one operand buffer (the producers then convert the next tile while conv2 runs).  A plan must keep RB_MIN_STAGES
-// weight stages within the opt-in shared-memory limit.
+// Split instantiations: 256-row tiles at 32 channels, 128-row tiles at 64 channels (mt: 64-row blocks of a tile)
+RbKernel rb_split_kernel_for(int channels, int* mt) {
+  *mt = channels == 32 ? 4 : 2;
+  if (channels == 32) return rb_pair_split_kernel<4, 2>;
+  if (channels == 64) return rb_pair_split_kernel<2, 4>;
+  return nullptr;
+}
+
+// Tile geometry of one kernel at `mt` and the first (na, ns) that leaves RB_MIN_STAGES weight stages per ring: two
+// conv1 operand buffers with three, then two raw stages; then, with one 32-channel chunk, one operand buffer (the
+// producers then convert the next tile while conv2 runs).
+int rb_fit(const pwgb_resblock_desc* d, RbK& p, size_t& smem_bytes, int split, int mt) {
+  const int tt = (split ? 64 : 128) * mt, rings = split ? 2 : 1, epi_tiles = split ? 1 : 2;
+  const long long halo1 = (long long)(d->kernel - 1) * d->dilation;
+  p.split = split;
+  p.MT = mt;
+  p.M2 = (tt - (d->kernel - 1)) & ~3;
+  p.R1 = tt + (int)halo1;
+  p.R4 = (p.R1 + 6) & ~3;
+  p.Rh = tt + d->kernel - 1;
+  p.a_bytes = 2 * (KC / 8) * p.R1 * 16;
+  p.raw_bytes = KC * p.R4 * 4;
+  p.h_bytes = 2 * (KC / 8) * p.Rh * 16;
+  const size_t epi = epi_tiles * (size_t)d->channels * rb_sld(mt) * 4;
+  const size_t fixed = (size_t)p.nchunks * p.h_bytes + epi + 2 * (size_t)d->channels * 4 + 1024;
+  static const int bufs[3][2] = {{2, 3}, {2, 2}, {1, 2}};  // (na, ns)
+  for (const auto& nn : bufs) {
+    const int na = nn[0], ns = nn[1];
+    if (na < p.nchunks) continue;  // one operand buffer only for a single chunk
+    const size_t used = fixed + (size_t)na * p.a_bytes + (size_t)ns * p.raw_bytes;
+    if (used + (size_t)rings * RB_MIN_STAGES * p.b_bytes > RB_SMEM) continue;
+    int nb = (int)((RB_SMEM - used) / p.b_bytes);
+    if (nb > 24) nb = 24;
+    nb -= nb % rings;
+    p.na = na;
+    p.nb = nb;
+    p.ns = ns;
+    p.tiles_per_seq = ceil_div(d->t, p.M2);
+    if ((long long)p.tiles_per_seq * d->batch > 0x7fffffffLL) return 0;
+    p.total_tiles = p.tiles_per_seq * d->batch;
+    smem_bytes = (size_t)na * p.a_bytes + (size_t)nb * p.b_bytes + (size_t)ns * p.raw_bytes + (size_t)p.nchunks * p.h_bytes +
+                 epi + 8 * (size_t)(2 * na + 2 * nb + 2 * ns + 2 + split) + 2 * (size_t)d->channels * 4;
+    return 1;
+  }
+  return 0;
+}
+
+// Plan of one pair: the split kernel where it fits (unless pwgb_debug_set(3, 1) forces lockstep), else the lockstep
+// kernel.  For the lockstep kernel a warpgroup's 64-row blocks are independent accumulator chains, so the planner tries
+// MT = 2 first (the wgmma of one chain wait for each other: at MT = 1 and 32 channels the tensor cores idle between
+// them), then MT = 1.
 int rb_plan(const pwgb_resblock_desc* d, RbK& p, size_t& smem_bytes) {
   if (!d || d->batch < 0 || d->t <= 0 || d->kernel < 1 || d->kernel % 2 == 0 || d->dilation < 1) return 0;
   if (!rb_kernel_for(1, d->channels)) return 0;
@@ -370,42 +676,16 @@ int rb_plan(const pwgb_resblock_desc* d, RbK& p, size_t& smem_bytes) {
   p.p2 = (d->kernel - 1) / 2;
   p.nchunks = d->channels / KC;
   p.b_bytes = 2 * (KC / 8) * d->channels * 16;
-  static const int bufs[3][2] = {{2, 3}, {2, 2}, {1, 2}};  // (na, ns)
-  for (int mt = 2; mt >= 1; --mt) {
-    if (!rb_kernel_for(mt, d->channels)) continue;
-    const int tt = 128 * mt;
-    p.MT = mt;
-    p.M2 = (tt - (d->kernel - 1)) & ~3;
-    p.R1 = tt + (int)halo1;
-    p.R4 = (p.R1 + 6) & ~3;
-    p.Rh = tt + d->kernel - 1;
-    p.a_bytes = 2 * (KC / 8) * p.R1 * 16;
-    p.raw_bytes = KC * p.R4 * 4;
-    p.h_bytes = 2 * (KC / 8) * p.Rh * 16;
-    const size_t epi = 2 * (size_t)d->channels * rb_sld(mt) * 4;
-    const size_t fixed = (size_t)p.nchunks * p.h_bytes + epi + 2 * (size_t)d->channels * 4 + 1024;
-    for (const auto& nn : bufs) {
-      const int na = nn[0], ns = nn[1];
-      if (na < p.nchunks) continue;  // one operand buffer only for a single chunk
-      const size_t used = fixed + (size_t)na * p.a_bytes + (size_t)ns * p.raw_bytes;
-      if (used + (size_t)RB_MIN_STAGES * p.b_bytes > RB_SMEM) continue;
-      int nb = (int)((RB_SMEM - used) / p.b_bytes);
-      if (nb > 24) nb = 24;
-      p.na = na;
-      p.nb = nb;
-      p.ns = ns;
-      p.tiles_per_seq = ceil_div(d->t, p.M2);
-      if ((long long)p.tiles_per_seq * d->batch > 0x7fffffffLL) return 0;
-      p.total_tiles = p.tiles_per_seq * d->batch;
-      smem_bytes = (size_t)na * p.a_bytes + (size_t)nb * p.b_bytes + (size_t)ns * p.raw_bytes + (size_t)p.nchunks * p.h_bytes +
-                   epi + 8 * (size_t)(2 * na + 2 * nb + 2 * ns + 2) + 2 * (size_t)d->channels * 4;
-      return 1;
-    }
-  }
+  int split_mt = 0;
+  if (!g_rb_lockstep && rb_split_kernel_for(d->channels, &split_mt) && rb_fit(d, p, smem_bytes, 1, split_mt)) return 1;
+  for (int mt = 2; mt >= 1; --mt)
+    if (rb_kernel_for(mt, d->channels) && rb_fit(d, p, smem_bytes, 0, mt)) return 1;
   return 0;
 }
 
 }  // namespace
+
+void rb_debug_lockstep(int on) { g_rb_lockstep = on; }
 
 }  // namespace pwgb
 
@@ -421,9 +701,16 @@ extern "C" int pwgb_resblock_pair_plan(const pwgb_resblock_desc* d, int* info) {
   RbK p;
   size_t bytes;
   if (!info || !rb_plan(d, p, bytes)) return 0;
-  const int v[5] = {p.M2, 128 * p.MT, p.na, p.nb, p.ns};
+  const int v[5] = {p.M2, (p.split ? 64 : 128) * p.MT, p.na, p.nb, p.ns};
   memcpy(info, v, sizeof(v));
   return 1;
+}
+
+extern "C" int pwgb_resblock_pair_variant(const pwgb_resblock_desc* d) {
+  RbK p;
+  size_t bytes;
+  if (!rb_plan(d, p, bytes)) return 0;
+  return p.split ? 2 : 1;
 }
 
 extern "C" int pwgb_resblock_pair_forward(const pwgb_resblock_desc* d, const float* x, const void* w1_packed,
@@ -439,7 +726,9 @@ extern "C" int pwgb_resblock_pair_forward(const pwgb_resblock_desc* d, const flo
   if (p.B == 0) return PWGB_OK;
   static bool attr_set = false;
   if (!attr_set) {
-    for (const RbKernel k : {rb_kernel_for(1, 32), rb_kernel_for(1, 64), rb_kernel_for(2, 32)}) {
+    int mt;
+    for (const RbKernel k : {rb_kernel_for(1, 32), rb_kernel_for(1, 64), rb_kernel_for(2, 32), rb_split_kernel_for(32, &mt),
+                             rb_split_kernel_for(64, &mt)}) {
       cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RB_SMEM);
       if (e != cudaSuccess) {
         set_error("resblock_pair: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
@@ -456,7 +745,9 @@ extern "C" int pwgb_resblock_pair_forward(const pwgb_resblock_desc* d, const flo
     if (num_sms <= 0) num_sms = 132;
   }
   const int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
-  rb_kernel_for(p.MT, p.C)<<<(unsigned)grid, RB_THREADS, bytes, (cudaStream_t)stream>>>(
-      p, x, (const unsigned char*)w1_packed, b1, (const unsigned char*)w2_packed, b2, y);
-  return check_launch("resblock_pair_kernel");
+  int mt = p.MT;
+  const RbKernel k = p.split ? rb_split_kernel_for(p.C, &mt) : rb_kernel_for(p.MT, p.C);
+  k<<<(unsigned)grid, p.split ? RBS_THREADS : RB_THREADS, bytes, (cudaStream_t)stream>>>(p, x, (const unsigned char*)w1_packed, b1,
+                                                               (const unsigned char*)w2_packed, b2, y);
+  return check_launch(p.split ? "rb_pair_split_kernel" : "resblock_pair_kernel");
 }

@@ -225,6 +225,8 @@ def resblock_pair(x, w1, b1, w2, b2, *, kernel_size, dilation, slope, out=None, 
     b2 = _dev(b2, "b2") if b2 is not None else None
     if out is None:
         out = torch.empty_like(x)
+    if out.numel() == 0:
+        return out  # an empty batch: nothing to compute (and no device pointers to pass)
     pk1, pk2 = packed_weight(w1), packed_weight(w2)
     # FLOPs of both convs; bytes: x once, out written (and read too when accumulating), the intermediate stays on chip
     prof = _Prof("resblock_pair_tc", 2 * 2.0 * B * Cc * T * Cc * K, 4.0 * (x.numel() + out.numel() * (2 if accumulate else 1)),
@@ -237,13 +239,17 @@ def resblock_pair(x, w1, b1, w2, b2, *, kernel_size, dilation, slope, out=None, 
 
 def resblock_pair_plan(channels, t, kernel_size, dilation, batch=1):
     """The fused pair's tile plan as a dict (output rows per tile, conv rows per tile, conv1 operand buffers, weight
-    stages, raw activation stages), or None when the pair keeps the two-launch path."""
+    stages of both rings, raw activation stages, and the kernel: "split" = one consumer warpgroup per conv, "lockstep" =
+    both warpgroups through both convs), or None when the pair keeps the two-launch path."""
     d = capi.ResBlockDesc(batch=batch, channels=channels, t=t, kernel=kernel_size, dilation=dilation, slope=0.1, out_scale=1.0,
                           accumulate=0)
+    L = capi.lib()
     v = (C.c_int * 5)()
-    if not capi.lib().pwgb_resblock_pair_plan(C.byref(d), v):
+    if not L.pwgb_resblock_pair_plan(C.byref(d), v):
         return None
-    return dict(zip(("M2", "TT", "na", "nb", "ns"), list(v)))
+    plan = dict(zip(("M2", "TT", "na", "nb", "ns"), list(v)))
+    plan["variant"] = {1: "lockstep", 2: "split"}[L.pwgb_resblock_pair_variant(C.byref(d))]
+    return plan
 
 
 def conv_transpose1d_raw(x, w, bias=None, *, stride, padding=0, output_padding=0, pre_slope=1.0, groups=1, period=1):
