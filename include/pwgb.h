@@ -337,7 +337,7 @@ PWGB_API int pwgb_mel_project_forward(int batch, int frames, int bins, int n_mel
 /* ------------------------------------------------------------------------
  * Deterministic mean reductions for the GAN losses (losses/adversarial_loss.py:29-123,
  * losses/feat_match_loss.py:27-54): out[0] (+)= weight * mean_i f(x_i [, y_i]) with
- * mode 0: (x-c)^2, 1: |x-y|, 2: max(0, c - s*x), 3: s*x.  ws: >= 1 float of scratch
+ * mode 0: (x-c)^2, 1: |x-y|, 2: max(0, c - s*x), 3: s*x, 4: (x-y)^2.  ws: >= 1 float of scratch
  * (more = more parallel partials, up to 1024).
  * AvgPool1d between discriminator scales (hifigan.py:758-775, melgan.py:478-493).
  * ---------------------------------------------------------------------- */
@@ -491,6 +491,28 @@ PWGB_API int pwgb_duration_round(const float* x, long long* ds, long long* total
                                  void* stream);
 PWGB_API int pwgb_collate_runlength(const float* feats, const long long* c_offsets, int batch, int channels, int frames, long long* runs,
                                     long long* codes, long long* counts, int max_runs, long long pad_value, void* stream);
+
+/* ------------------------------------------------------------------------
+ * VQ-VAE bottleneck (models/vqvae.py, layers/vector_quantize_codebook.py, functions/vector_quantizer.py).
+ *
+ *   vq_forward: with z_e (B, D, T) fp32 channel-major (read in place), the nearest code of every frame,
+ *     d_k = fl(fl(c_sqr[k] + x_sqr) - 2 dot(x, c_k)) with dot, x_sqr and c_sqr accumulated by FFMA over d = 0 .. D-1,
+ *     argmin as torch.min(dim): ties to the lower index, a NaN distance wins and the first NaN is taken; written to
+ *     indices (B, T) int64.  With z_e == null the search is skipped and indices is read (VQVAE.decode).  Then, for
+ *     every frame, z_q (B, D, T) = codebook[index] if z_q is given, and the decoder input dec (B, D + Cl + Cg, T) if
+ *     given: channels [0, D) the gathered codes, [D, D + Cl) copied from l (B, Cl, T), [D + Cl, D + Cl + Cg)
+ *     global_table[g[b]] broadcast over time.  An index outside [0, K) or a g[b] outside the table is never read: the
+ *     frame's (or the item's) z_q / dec columns are NaN.  One launch.  D <= 768.
+ *   vq_backward: from the gradient of dec, gz_e (+)= gdec[:, :D] (the straight-through gradient of z_e) and
+ *     d_global_table (num_global, Cg) = per table row, in item order, the per-item sums over time of gdec[:, D + Cl:]
+ *     (rows no item uses get 0).  Either output may be null.  The codebook gradient is pwgb_symbol_embed_backward on
+ *     the indices; the local slice belongs to the local embedding's conv backward.
+ * ---------------------------------------------------------------------- */
+PWGB_API int pwgb_vq_forward(const float* z_e, const float* codebook, int num_codes, long long* indices, float* z_q, float* dec,
+                             const float* l, int local_channels, const float* global_table, const long long* g, int num_global,
+                             int global_channels, int batch, int dim, int t, void* stream);
+PWGB_API int pwgb_vq_backward(const float* gdec, int batch, int dim, int local_channels, int global_channels, int t, float* gz_e,
+                              int accumulate, const long long* g, int num_global, float* d_global_table, void* stream);
 
 #ifdef __cplusplus
 }

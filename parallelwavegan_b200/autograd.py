@@ -632,3 +632,43 @@ class DurationLossFn(torch.autograd.Function):
                                                     ops._p(gx), ops._stream())
         capi.check(rc, "pwgb_duration_loss_backward")
         return gx, None, None
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# VQ-VAE bottleneck (models/vqvae.py:80-110, layers/vector_quantize_codebook.py:44-75, functions/vector_quantizer.py)
+# ---------------------------------------------------------------------------------------------------------------
+class VQFn(torch.autograd.Function):
+    """Nearest-code search, gather and decoder-input assembly in one launch (ops.vq_raw) -> (dec, z_q, indices).
+    Backward: dec's code channels are the straight-through gradient of z_e (vector_quantizer.py:107-108), its local
+    slice goes to l and its global slice to the global table (pwgb_vq_backward); z_q's gradient (or, with
+    ``st_codebook``, dec's code channels) is the codebook's index_add adjoint, pwgb_symbol_embed_backward on the
+    indices (a deterministic per-row sum)."""
+
+    @staticmethod
+    def forward(ctx, z_e, codebook, l, global_table, g, want_zq, st_codebook):
+        indices, zq, dec = ops.vq_raw(z_e, codebook, z_q=want_zq, dec=True, l=l, global_table=global_table, g=g)
+        ctx.set_materialize_grads(False)
+        ctx.mark_non_differentiable(indices)
+        ctx.cfg = (codebook.shape[0], codebook.shape[1], l.shape[1] if l is not None else 0,
+                   global_table.shape[0] if global_table is not None else 0, bool(st_codebook))
+        ctx.save_for_backward(indices, g)
+        return dec, zq, indices
+
+    @staticmethod
+    def backward(ctx, gdec, gzq, _gidx):
+        indices, g = ctx.saved_tensors
+        K, D, Cl, ng, st_codebook = ctx.cfg
+        gz = gl = dgt = dcb = None
+        if gdec is not None:
+            gdec = gdec.contiguous()
+            need_gt = ctx.needs_input_grad[3] and g is not None
+            if ctx.needs_input_grad[0] or need_gt:
+                gz, dgt = ops.vq_backward_raw(gdec, D, Cl, g if need_gt else None, ng, want_gz=ctx.needs_input_grad[0])
+            if ctx.needs_input_grad[2]:
+                gl = gdec[:, D : D + Cl].contiguous()
+            if st_codebook:
+                gzq = gdec[:, :D].contiguous()
+        if ctx.needs_input_grad[1] and gzq is not None:
+            B, T = indices.shape
+            dcb, _ = ops.symbol_embed_backward_raw(gzq.contiguous(), None, indices.view(B, 1, T), None, T, K)
+        return gz, dcb, gl, dgt, None, None, None

@@ -244,6 +244,10 @@ def lib():
     L.pwgb_duration_round.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_float, C.c_int, vp]
     L.pwgb_collate_runlength.restype = C.c_int
     L.pwgb_collate_runlength.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_int, ll, vp]
+    L.pwgb_vq_forward.restype = C.c_int
+    L.pwgb_vq_forward.argtypes = [vp, vp, C.c_int, vp, vp, vp, vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp]
+    L.pwgb_vq_backward.restype = C.c_int
+    L.pwgb_vq_backward.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, C.c_int, vp, vp]
     _lib = L
     return L
 
@@ -288,4 +292,5 @@ EXPORTED_SYMBOLS = [
     "pwgb_symbol_embed_forward", "pwgb_symbol_embed_backward_workspace", "pwgb_symbol_embed_backward",
     "pwgb_channel_layernorm_forward", "pwgb_channel_layernorm_backward_workspace", "pwgb_channel_layernorm_backward",
     "pwgb_duration_loss_forward", "pwgb_duration_loss_backward", "pwgb_duration_round", "pwgb_collate_runlength",
+    "pwgb_vq_forward", "pwgb_vq_backward",
 ]

@@ -276,6 +276,8 @@ __global__ void reduce_mean_backward_kernel(int mode, const float* __restrict__ 
       d = v > y[i] ? 1.f : (v < y[i] ? -1.f : 0.f);
     else if (mode == 2)
       d = (c - s * v) > 0.f ? -s : 0.f;
+    else if (mode == 4)
+      d = 2.f * (v - y[i]);
     else
       d = s;
     gx[i] = (accumulate ? gx[i] : 0.f) + go * d;
@@ -681,7 +683,7 @@ extern "C" int pwgb_bias_grad(const float* g, float* db, int batch, int channels
 
 extern "C" int pwgb_reduce_mean_backward(int mode, const float* x, const float* y, long long n, float c, float s,
                                          float weight, const float* gout, float* gx, int accumulate, void* stream) {
-  PWGB_CHECK_ARG(x && gout && gx && n > 0 && mode >= 0 && mode <= 3 && (mode != 1 || y), "reduce_mean_backward: bad arguments");
+  PWGB_CHECK_ARG(x && gout && gx && n > 0 && mode >= 0 && mode <= 4 && ((mode != 1 && mode != 4) || y), "reduce_mean_backward: bad arguments");
   reduce_mean_backward_kernel<<<grid_for(n), 256, 0, (cudaStream_t)stream>>>(mode, x, y, n, c, s, weight, gout, gx, accumulate);
   return check_launch("reduce_mean_backward_kernel");
 }

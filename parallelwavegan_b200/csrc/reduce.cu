@@ -4,6 +4,7 @@
 //   mode 1: |x - y|          (feature matching L1)
 //   mode 2: max(0, c - s*x)  (hinge terms: real: c=1,s=+1 ; fake: c=1,s=-1)
 //   mode 3: s * x            (hinge generator loss: -mean(x))
+//   mode 4: (x - y)^2        (MSELoss between two tensors: the VQ-VAE quantisation / commitment losses)
 // out[0] (+)= weight * mean.  Two-stage, fixed order: bit-reproducible.
 #include "common.cuh"
 
@@ -21,6 +22,9 @@ __global__ void __launch_bounds__(256) reduce_partial_kernel(int mode, const flo
       t = (v - c) * (v - c);
     } else if (mode == 1) {
       t = fabsf(v - y[i]);
+    } else if (mode == 4) {
+      const float e = v - y[i];
+      t = e * e;
     } else if (mode == 2) {
       t = fmaxf(0.f, c - s * v);
     } else {
@@ -86,8 +90,8 @@ using namespace pwgb;
 extern "C" int pwgb_reduce_mean_forward(int mode, const float* x, const float* y, long long n, float c, float s,
                                         float weight, int accumulate, float* out, float* ws, int ws_floats,
                                         void* stream) {
-  PWGB_CHECK_ARG(x && out && ws && (mode != 1 || y), "reduce_mean: null argument");
-  PWGB_CHECK_ARG(mode >= 0 && mode <= 3 && n > 0 && ws_floats >= 1, "reduce_mean: bad arguments");
+  PWGB_CHECK_ARG(x && out && ws && ((mode != 1 && mode != 4) || y), "reduce_mean: null argument");
+  PWGB_CHECK_ARG(mode >= 0 && mode <= 4 && n > 0 && ws_floats >= 1, "reduce_mean: bad arguments");
   long long blocks = (n + 2047) / 2048;
   if (blocks > ws_floats) blocks = ws_floats;
   if (blocks > 1024) blocks = 1024;

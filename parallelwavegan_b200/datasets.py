@@ -18,14 +18,20 @@ from .capi import PwgbError
 class DeviceCorpus:
     """items: list of (audio (T,), feats (frames, C)) numpy arrays / tensors [mel2wav case], of
     (audio, feats, f0 (frames,), excitation (frames, E)) [UHiFiGAN recipes], or of audio arrays [audio-only case].
+    With ``global_condition`` (VQ-VAE recipes, bin/train.py:801-876) every item ends in its global id (speaker), and
+    the rest is (audio,) or (audio, local feats); the ids are kept on the host in ``global_ids``.
     ``hop_size`` applies ``Collater._adjust_length`` (train.py:868-893): audio shorter than ``frames * hop_size`` is
     edge-padded; any other mismatch is an error, like the reference's assert.  f0 is kept as a 1-channel feature
     matrix whose rows line up with the features', excitation flattened like audio (E samples per frame)."""
 
-    def __init__(self, items, device, hop_size=None):
+    def __init__(self, items, device, hop_size=None, global_condition=False):
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise PwgbError("DeviceCorpus lives on a CUDA device (no CPU fallback)")
+        self.global_ids = None
+        if global_condition:
+            self.global_ids = np.array([int(np.asarray(it[-1]).reshape(-1)[0]) for it in items], dtype=np.int64)
+            items = [tuple(it[:-1]) if len(it) > 2 else it[0] for it in items]
         auds, fts, self.x_start, self.c_start, self.x_len, self.c_len = [], [], [], [], [], []
         f0s, exs, self.e_start = [], [], []
         xo = co = eo = 0
@@ -74,10 +80,10 @@ class DeviceCorpus:
 
 
 class Collater:
-    """``Collater`` of bin/train.py:646-925 for the mel2wav and audio-only cases, on the device."""
+    """``Collater`` of bin/train.py:646-925 for the mel2wav, audio-only and VQ-wav2wav cases, on the device."""
 
     def __init__(self, batch_max_steps=20480, hop_size=256, aux_context_window=2, use_noise_input=False, use_aux_input=True,
-                 use_f0_and_excitation=False, use_duration=False, pad_value=0):
+                 use_f0_and_excitation=False, use_duration=False, use_global_condition=False, use_local_condition=False, pad_value=0):
         if hop_size is not None:
             if batch_max_steps % hop_size != 0:
                 batch_max_steps += -(batch_max_steps % hop_size)
@@ -95,7 +101,13 @@ class Collater:
             raise PwgbError("Collater(use_duration=True) needs use_aux_input=True and use_noise_input=False (train.py:691-695)")
         if not use_aux_input:
             assert not use_noise_input, "Not supported."
-        if use_aux_input:
+        if use_local_condition:
+            assert not use_aux_input and not use_duration, "Not supported."  # train.py:696-699
+        if use_global_condition:
+            assert not use_aux_input and not use_duration, "Not supported."
+        self.use_global_condition = use_global_condition
+        self.use_local_condition = use_local_condition
+        if use_aux_input or use_local_condition:
             self.start_offset = aux_context_window
             self.end_offset = -(self.batch_max_frames + aux_context_window)
             self.mel_threshold = self.batch_max_frames + 2 * aux_context_window
@@ -113,7 +125,10 @@ class Collater:
         (train.py:768-783) it returns ``(c, y, ds)``: the cropped (F, C) symbol rows, truncated to int64, run-length encoded
         per item (torch.unique_consecutive(dim=0)); c (B, C, S) int64 padded with ``pad_value``, ds (B, S) int64 run
         lengths padded with 0.  pwgb_collate_runlength counts the runs at the crop offsets, the host reads the B counts
-        to size S (one device-to-host copy), and a second pass writes codes and lengths."""
+        to size S (one device-to-host copy), and a second pass writes codes and lengths.  Without aux input (the
+        VQ-wav2wav case, train.py:799-876) it returns ``(l, g), y``: l (B, C, frames) the local features cropped at
+        ``hop_size`` (items with at least ``frames + 2 * aux_context_window`` rows) with use_local_condition, g (B,)
+        int64 the items' global ids with use_global_condition, each None otherwise."""
         dev = corpus.device
         if self.use_aux_input:
             if not corpus.has_feats:
@@ -123,6 +138,14 @@ class Collater:
             x_off = np.array([corpus.x_start[i] for i in keep], dtype=np.int64) + starts * self.hop_size
             c_off = np.array([corpus.c_start[i] for i in keep], dtype=np.int64) + starts - self.aux_context_window
             F = self.batch_max_frames + 2 * self.aux_context_window
+        elif self.use_local_condition:
+            if not corpus.has_feats:
+                raise PwgbError("Collater(use_local_condition=True) needs a corpus with local features")
+            keep = [i for i in indices if corpus.c_len[i] >= self.mel_threshold]  # train.py:804-809
+            starts = np.array([np.random.randint(self.start_offset, corpus.c_len[i] + self.end_offset) for i in keep], dtype=np.int64)
+            x_off = np.array([corpus.x_start[i] for i in keep], dtype=np.int64) + starts * self.hop_size
+            c_off = np.array([corpus.c_start[i] for i in keep], dtype=np.int64) + starts  # no context rows (train.py:825-833)
+            F = self.batch_max_frames
         else:
             keep = [i for i in indices if corpus.x_len[i] >= self.audio_threshold]  # train.py:840-843
             starts = np.array([np.random.randint(self.start_offset, corpus.x_len[i] + self.end_offset) for i in keep], dtype=np.int64)
@@ -136,6 +159,11 @@ class Collater:
             co = torch.from_numpy(c_off).pin_memory().to(dev, non_blocking=True)
             if not self.use_duration:
                 c = torch.empty((B, corpus.channels, F), device=dev, dtype=torch.float32)
+        g = None
+        if self.use_global_condition:
+            if corpus.global_ids is None:
+                raise PwgbError("Collater(use_global_condition=True) needs a corpus built with global_condition=True")
+            g = torch.from_numpy(corpus.global_ids[keep]).pin_memory().to(dev, non_blocking=True)
         vp = C.c_void_p
         rc = capi.lib().pwgb_collate_crop(vp(corpus.audio.data_ptr()), vp(xo.data_ptr()), vp(corpus.feats.data_ptr()) if c is not None else None,
                                           vp(co.data_ptr()) if co is not None else None, vp(y.data_ptr()), vp(c.data_ptr()) if c is not None else None,
@@ -158,7 +186,7 @@ class Collater:
                                               vp(torch.cuda.current_stream().cuda_stream))
             capi.check(rc, "pwgb_collate_crop")
         if not self.use_aux_input:
-            return (None, None), y  # the reference returns (l_batch, g_batch) = (None, None) here (train.py:861-876)
+            return (c, g), y  # (l_batch, g_batch), either None when its condition is off (train.py:861-876)
         inputs = (c,)
         if self.use_noise_input:
             z = torch.randn(y.shape, device=dev, generator=self.generator)  # train.py:790-792, drawn on the device

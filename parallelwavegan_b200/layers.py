@@ -609,3 +609,25 @@ class LengthRegulator(torch.nn.Module):
         idx = torch.arange(B * S, device=xs.device, dtype=torch.int64).reshape(B, 1, S)
         y = ops.symbol_embed(idx, xs.reshape(B * S, D), ds=ds, t_out=ops.regulated_length(totals))
         return y.transpose(1, 2)
+
+
+class VQCodebook(torch.nn.Module):
+    """layers/vector_quantize_codebook.py:17-75: the (num_embeds, embed_dim) codebook ``embedding.weight``, initialised
+    U(-1 / num_embeds, 1 / num_embeds).  The search reads the channel-major z_e in place (pwgb_vq_forward)."""
+
+    def __init__(self, num_embeds, embed_dim):
+        super().__init__()
+        self.embedding = torch.nn.Embedding(num_embeds, embed_dim)
+        self.embedding.weight.data.uniform_(-1.0 / num_embeds, 1.0 / num_embeds)
+
+    def forward(self, z_e):
+        """z_e (B, embed_dim, T) -> nearest-code indices (B, T)."""
+        from .functions import vector_quantize
+
+        return vector_quantize(z_e.transpose(2, 1), self.embedding.weight)
+
+    def straight_through(self, z_e):
+        """z_e (B, embed_dim, T) -> (z_q_st, z_q), both (B, embed_dim, T): the codes for the decoder, whose gradient goes
+        straight through to z_e, and the same codes for the quantisation loss, whose gradient goes to the codebook."""
+        z_q_st, z_q, _ = ops.vq(z_e, self.embedding.weight)
+        return z_q_st, z_q

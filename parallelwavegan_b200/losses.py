@@ -315,3 +315,16 @@ class DurationPredictorLoss(torch.nn.Module):
 
     def forward(self, outputs, targets):
         return ops.duration_loss(outputs, targets, self.offset)[0]
+
+
+# --------------------------------------------------------------------------
+# criterion["mse"] of the VQ-VAE recipes (bin/train.py:1384-1451, 210-211)
+# --------------------------------------------------------------------------
+class MSELoss(torch.nn.Module):
+    """torch.nn.MSELoss() (mean reduction) between two tensors of the same size -- pwgb_reduce_mean_forward mode 4,
+    with gradients to both operands."""
+
+    def forward(self, x, y):
+        if x.shape != y.shape:
+            raise PwgbError(f"MSELoss: shapes {tuple(x.shape)} and {tuple(y.shape)} differ")
+        return ops.reduce_mean("mse", x, y)[0]

@@ -12,7 +12,7 @@ import torch
 from . import ops
 from .capi import PwgbError
 from .layers import HiFiGANResidualBlock as ResidualBlock
-from .layers import CausalConv1d, CausalConvTranspose1d, ResidualStack, TADEResBlock, activation_slope, effective_weight, pad_mode_of
+from .layers import CausalConv1d, CausalConvTranspose1d, ResidualStack, TADEResBlock, VQCodebook, activation_slope, effective_weight, pad_mode_of
 
 
 def _read_stats(stats):
@@ -1484,3 +1484,96 @@ class StyleMelGANDiscriminator(torch.nn.Module, _NormMixin):
                 m.weight.data.normal_(0.0, 0.02)
 
         self.apply(_reset_parameters)
+
+
+class VQVAE(torch.nn.Module):
+    """models/vqvae.py:16-185: wav2wav VQ-VAE.  The encoder (a MelGANDiscriminator in every recipe) gives z_e, its last
+    output; one pwgb_vq_forward launch finds the nearest codes and writes both the quantised z_q and the decoder input
+    -- the codes, the (embedded) local conditioning and the global embedding broadcast over time -- so neither
+    ``torch.cat`` of the reference is built; the decoder is a MelGANGenerator.  State-dict keys follow the reference,
+    including its quirks: ``local_embed`` is weight-normed like every Conv1d, ``global_embed`` is not, and with
+    ``use_weight_norm=False`` the decoder keeps the weight norm MelGANGenerator applies by default."""
+
+    def __init__(
+        self,
+        in_channels=1,
+        out_channels=1,
+        num_embeds=512,
+        embed_dim=256,
+        num_local_embeds=None,
+        local_embed_dim=None,
+        num_global_embeds=None,
+        global_embed_dim=None,
+        encoder_type="MelGANDiscriminator",
+        decoder_type="MelGANGenerator",
+        encoder_conf={"out_channels": 256, "downsample_scales": [4, 4, 2, 2], "max_downsample_channels": 1024},
+        decoder_conf={"in_channels": 256, "upsample_scales": [4, 4, 2, 2], "channels": 512, "stacks": 3},
+        use_weight_norm=True,
+    ):
+        super().__init__()
+        import sys
+
+        mod = sys.modules[__name__]
+        if not hasattr(mod, encoder_type) or not hasattr(mod, decoder_type):
+            raise PwgbError(f"VQVAE: encoder_type={encoder_type!r} / decoder_type={decoder_type!r} are not mirrored")
+        encoder_class = getattr(mod, encoder_type)
+        decoder_class = getattr(mod, decoder_type)
+        encoder_conf = dict(encoder_conf, in_channels=in_channels)
+        decoder_conf = dict(decoder_conf, out_channels=out_channels)
+        if not issubclass(decoder_class, MelGANGenerator):
+            raise NotImplementedError(f"{decoder_class} is not supported yet.")
+        self.in_channels = in_channels
+        if num_local_embeds is not None:
+            self.local_embed = torch.nn.Conv1d(num_local_embeds, local_embed_dim, 1) if local_embed_dim is not None else None
+        if num_global_embeds is not None:
+            self.global_embed = torch.nn.Embedding(num_global_embeds, global_embed_dim)
+        self.encoder = encoder_class(**encoder_conf)
+        self.codebook = VQCodebook(num_embeds=num_embeds, embed_dim=embed_dim)
+        self.decoder = decoder_class(**decoder_conf)
+        if use_weight_norm:
+            self.remove_weight_norm()  # the decoder's own weight norm, as in the reference
+            self.apply_weight_norm()
+
+    def _local(self, l):
+        if self.local_embed is None:
+            return l
+        m = self.local_embed
+        return ops.conv1d(l, effective_weight(m), m.bias)
+
+    def _global(self, g):
+        return (self.global_embed.weight, g) if g is not None else (None, None)
+
+    def _encode(self, x):
+        z_e = self.encoder(x)
+        return z_e[-1] if isinstance(z_e, list) else z_e
+
+    def forward(self, x, l=None, g=None):
+        """x (B, in_channels, T), l (B, num_local_embeds, T') or None, g (B,) int64 or None ->
+        (x_bar (B, out_channels, T), z_e, z_q (B, embed_dim, T'))  (vqvae.py:80-110)."""
+        z_e = self._encode(x)
+        if l is not None:
+            l = self._local(l)
+        gt, g = self._global(g)
+        dec, z_q, _ = ops.vq(z_e, self.codebook.embedding.weight, l=l, global_table=gt, g=g)
+        return self.decoder(dec), z_e, z_q
+
+    def encode(self, x):
+        """x (B, in_channels, T) -> codebook indices (B, T')  (vqvae.py:112-125)."""
+        return self.codebook(self._encode(x))
+
+    def decode(self, indices, l=None, g=None):
+        """indices (B, T') int64 -> (B, out_channels, T)  (vqvae.py:127-147): gather and assembly only."""
+        if l is not None:
+            l = self._local(l)
+        gt, g = self._global(g)
+        _, _, dec = ops.vq_raw(None, self.codebook.embedding.weight, indices=indices, z_q=False, dec=True, l=l, global_table=gt, g=g)
+        return self.decoder(dec)
+
+    def apply_weight_norm(self):
+        def _apply_weight_norm(m):
+            if isinstance(m, (torch.nn.Conv1d, torch.nn.ConvTranspose1d)):
+                torch.nn.utils.weight_norm(m)
+
+        self.apply(_apply_weight_norm)
+
+    remove_weight_norm = _GeneratorBase.remove_weight_norm

@@ -616,7 +616,7 @@ def mel_project(ax, ay, melmat, eps, log_scale, want_mel=True, want_loss=False):
     return mel, loss
 
 
-_REDUCE = {"mse_const": 0, "l1": 1, "hinge": 2, "linear": 3}
+_REDUCE = {"mse_const": 0, "l1": 1, "hinge": 2, "linear": 3, "mse": 4}
 
 
 def reduce_mean_raw(mode, x, y=None, c=0.0, s=1.0, weight=1.0, out=None, accumulate=False):
@@ -1151,3 +1151,86 @@ def duration_loss(x, ds, offset=1.0):
 
         return ag.DurationLossFn.apply(x, ds, float(offset))
     return duration_loss_raw(x, ds, offset)
+
+
+# ---- VQ-VAE bottleneck (models/vqvae.py, layers/vector_quantize_codebook.py): nearest-code search, gather and the
+# decoder-input assembly -- pwgb_vq_forward / pwgb_vq_backward ----
+def _long_tensor(t, shape, name):
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.int64 or tuple(t.shape) != tuple(shape):
+        raise PwgbError(f"{name}: expected a CUDA int64 tensor of shape {tuple(shape)}")
+    return t.contiguous()
+
+
+def vq_raw(z_e, codebook, *, indices=None, z_q=True, dec=True, l=None, global_table=None, g=None):
+    """One pwgb_vq_forward launch -> (indices (B, T) int64, z_q (B, D, T) or None, dec (B, D + Cl + Cg, T) or None).
+    ``z_e`` (B, D, T) is searched for its nearest codes (fp32, fixed-order sums, ties to the lower index, NaN first as
+    torch.min); with ``indices`` given instead the search is skipped (VQVAE.decode).  ``dec`` is the decoder input:
+    the gathered codes, then ``l`` (B, Cl, T), then ``global_table[g]`` broadcast over time.  An index outside the
+    codebook or a ``g`` outside its table gives NaN columns."""
+    codebook = _dev(codebook, "codebook")
+    K, D = codebook.shape
+    if z_e is not None:
+        z_e = _dev(z_e, "z_e")
+        if z_e.dim() != 3 or z_e.shape[1] != D:
+            raise PwgbError(f"vq: z_e has shape {tuple(z_e.shape)}, the codebook {D} channels")
+        B, _, T = z_e.shape
+        indices = torch.empty((B, T), device=z_e.device, dtype=torch.int64)
+    else:
+        if not isinstance(indices, torch.Tensor) or indices.dim() != 2:
+            raise PwgbError("vq: expected (B, T) indices")
+        B, T = indices.shape
+        indices = _long_tensor(indices, (B, T), "indices")
+    dev = codebook.device
+    Cl = Cg = ng = 0
+    if l is not None:
+        l = _dev(l, "l")
+        if l.dim() != 3 or l.shape[0] != B or l.shape[2] != T:
+            raise PwgbError(f"vq: local conditioning {tuple(l.shape)} does not match the codes' (B, T) = {(B, T)}")
+        Cl = l.shape[1]
+    if g is not None:
+        if global_table is None:
+            raise PwgbError("vq: global ids without a global table")
+        global_table = _dev(global_table, "global_table")
+        g = _long_tensor(g, (B,), "g")
+        ng, Cg = global_table.shape
+    if l is not None or g is not None:
+        dec = True
+    zq = torch.empty((B, D, T), device=dev, dtype=torch.float32) if z_q else None
+    dc = torch.empty((B, D + Cl + Cg, T), device=dev, dtype=torch.float32) if dec else None
+    if B * T == 0:
+        return indices, zq, dc
+    prof = _Prof("vq_forward", 2.0 * B * T * K * D if z_e is not None else 0.0,
+                 4.0 * (B * T * D * (z_e is not None) + K * D + (zq.numel() if z_q else 0) + (dc.numel() if dec else 0)),
+                 f"B{B} D{D} K{K} T{T} Cl{Cl} Cg{Cg}")
+    rc = capi.lib().pwgb_vq_forward(_p(z_e), _p(codebook), K, _p(indices), _p(zq), _p(dc), _p(l) if Cl else None, Cl,
+                                    _p(global_table) if g is not None else None, _p(g), ng, Cg, B, D, T, _stream())
+    capi.check(rc, "pwgb_vq_forward")
+    prof.done()
+    return indices, zq, dc
+
+
+def vq_backward_raw(gdec, dim, local_channels, g=None, num_global=0, want_gz=True):
+    """(gz_e (B, D, T) or None, d_global_table (num_global, Cg) or None) from the decoder-input gradient
+    (B, D + Cl + Cg, T) -- pwgb_vq_backward (deterministic)."""
+    gdec = _dev(gdec, "gdec")
+    B, Ct, T = gdec.shape
+    Cg = Ct - dim - local_channels
+    gz = torch.empty((B, dim, T), device=gdec.device, dtype=torch.float32) if want_gz else None
+    dgt = torch.empty((num_global, Cg), device=gdec.device, dtype=torch.float32) if (g is not None and Cg > 0) else None
+    nz = gdec.numel() > 0
+    rc = capi.lib().pwgb_vq_backward(_p(gdec) if nz else None, B, dim, local_channels, Cg, T, _p(gz) if want_gz and nz else None, 0,
+                                     _p(g) if dgt is not None else None, num_global, _p(dgt), _stream())
+    capi.check(rc, "pwgb_vq_backward")
+    return gz, dgt
+
+
+def vq(z_e, codebook, *, l=None, global_table=None, g=None, z_q=True, st_codebook=False):
+    """(dec, z_q, indices): the straight-through decoder input and the quantised codes of ``z_e`` (see vq_raw).  Under
+    autograd ``dec`` carries the straight-through gradient to ``z_e``, to ``l`` and to ``global_table``; ``z_q`` the
+    codebook gradient (``st_codebook``: ``dec``'s code channels carry it instead, functions.vector_quantize_straight_through)."""
+    if _needs_grad(z_e, codebook, l, global_table):
+        from . import autograd as ag
+
+        return ag.VQFn.apply(z_e, codebook, l, global_table, g, bool(z_q), bool(st_codebook))
+    indices, zq, dc = vq_raw(z_e, codebook, z_q=z_q, dec=True, l=l, global_table=global_table, g=g)
+    return dc, zq, indices

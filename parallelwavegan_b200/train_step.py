@@ -11,17 +11,33 @@ With the fused optimizers of ``parallelwavegan_b200.optimizers`` the clip + upda
 launches right after the all-reduce."""
 import torch
 
+from .capi import PwgbError
 from .optimizers import _FusedBase
 
 
 class GanTrainStep:
     def __init__(self, generator, discriminator, criterion, opt_g, opt_d, lambda_aux=45.0, lambda_adv=1.0,
                  lambda_feat_match=2.0, grad_norm_g=-1, grad_norm_d=-1, generator_train_start_steps=0,
-                 discriminator_train_start_steps=0, update_prediction_after_generator_update=True, sched_g=None, sched_d=None, steps=0):
+                 discriminator_train_start_steps=0, update_prediction_after_generator_update=True, sched_g=None, sched_d=None, steps=0,
+                 lambda_commit=0.25):
         """criterion: dict with any of ``stft`` (MultiResolutionSTFTLoss), ``sub_stft``, ``mel``, ``pqmf``, and
-        ``gen_adv`` / ``dis_adv`` / ``feat_match`` and ``duration`` (DurationPredictorLoss) -- the keys of
-        ``Trainer.criterion`` (train.py:1384-1451); a key that is present is used (the reference's ``use_*_loss``
-        switches).  With ``duration`` the generator is a duration model called as ``G(x, ds)`` (train.py:208-213)."""
+        ``gen_adv`` / ``dis_adv`` / ``feat_match``, ``duration`` (DurationPredictorLoss) and ``mse`` (MSELoss) -- the keys
+        of ``Trainer.criterion`` (train.py:1384-1451); a key that is present is used (the reference's ``use_*_loss``
+        switches).  With ``duration`` the generator is a duration model called as ``G(x, ds)`` (train.py:208-213).
+        A ``VQVAE`` generator selects the VQ branch, as the reference's ``generator_type`` does (train.py:93, 204-219):
+        it is called as ``G(y, l, g)`` on the real audio, and ``criterion["mse"]`` gives the quantisation and
+        commitment losses, the latter weighted by ``lambda_commit``."""
+        from .models import VQVAE
+
+        g = generator.module if hasattr(generator, "module") else generator
+        self.is_vq = isinstance(g, VQVAE)
+        if self.is_vq:
+            if "mse" not in criterion:
+                raise PwgbError("a VQVAE generator needs criterion['mse'] (losses.MSELoss) for its VQ losses")
+            if g.in_channels != 1:
+                # the reference feeds a PQMF analysis of y to such an encoder (train.py:206-209); no recipe uses it
+                raise PwgbError("VQVAE with in_channels > 1 (a PQMF-analysed input) is not supported")
+        self.lambda_commit = lambda_commit
         self.g, self.d = generator, discriminator
         self.crit = criterion
         self.opt_g, self.opt_d = opt_g, opt_d
@@ -46,32 +62,42 @@ class GanTrainStep:
         if sched is not None:
             sched.step()
 
-    def _generate(self, x, ds=None):
-        ds_ = None
-        if "duration" in self.crit:
-            y_, ds_ = self.g(x, ds)  # train.py:208-213
+    def _generate(self, x, y, ds=None):
+        aux = None  # the duration model's ds_, or the VQ-VAE's (z_e, z_q)
+        if self.is_vq:
+            y_, z_e, z_q = self.g(y, *x)  # train.py:205-207
+            aux = (z_e, z_q)
+        elif "duration" in self.crit:
+            y_, aux = self.g(x, ds)  # train.py:208-213
         else:
             y_ = self.g(*x) if isinstance(x, (tuple, list)) else self.g(x)
         y_mb_ = None
         if "pqmf" in self.crit and y_.shape[1] > 1:  # multi-band: reconstruct the full-band signal (train.py:225-227)
             y_mb_ = y_
             y_ = self.crit["pqmf"].synthesis(y_mb_)
-        return y_, y_mb_, ds_
+        return y_, y_mb_, aux
 
     def __call__(self, x, y, ds=None):
-        """x: conditioning (B, mels, frames), the tuple (z, c) of the Parallel WaveGAN recipes, or the (B, C, S) symbol
-        codes of the duration recipes with their run lengths ``ds`` (B, S); y: (B, 1, T).
+        """x: conditioning (B, mels, frames), the tuple (z, c) of the Parallel WaveGAN recipes, the (B, C, S) symbol
+        codes of the duration recipes with their run lengths ``ds`` (B, S), or the VQ-VAE's (l, g); y: (B, 1, T).
         Returns a dict of loss tensors (device scalars; nothing is synchronised with the host)."""
         stats = {}
         adv_on = self.steps > self.d_start
         y_ = None
         # ---------------- generator phase (train.py:200-295)
         if self.steps > self.g_start:
-            y_, y_mb_, ds_ = self._generate(x, ds)
+            y_, y_mb_, aux = self._generate(x, y, ds)
             gen_loss = 0.0
-            if ds_ is not None:
+            if self.is_vq:
+                # gen_loss starts from the VQ losses, so lambda_aux scales them too (train.py:210-215, 262)
+                z_e, z_q = aux
+                quant = self.crit["mse"](z_q, z_e.detach())
+                commit = self.crit["mse"](z_e, z_q.detach())
+                stats["quantization_loss"], stats["commitment_loss"] = quant.detach(), commit.detach()
+                gen_loss = gen_loss + quant + self.lambda_commit * commit
+            elif aux is not None:
                 # gen_loss starts from the duration loss, so lambda_aux (and the sub-band 0.5) scale it too (train.py:213-262)
-                dur = self.crit["duration"](ds_, ds)
+                dur = self.crit["duration"](aux, ds)
                 stats["duration_loss"] = dur.detach()
                 gen_loss = gen_loss + dur
             if "stft" in self.crit:
@@ -113,7 +139,7 @@ class GanTrainStep:
         if adv_on:
             if self.update_prediction or y_ is None:
                 with torch.no_grad():
-                    y_, _, _ = self._generate(x, ds)
+                    y_, _, _ = self._generate(x, y, ds)
             p = self.d(y)
             p_ = self.d(y_.detach())
             real, fake = self.crit["dis_adv"](p_, p)
