@@ -495,11 +495,11 @@ def hann_window(n):
     return 0.5 - 0.5 * torch.cos(2.0 * math.pi * torch.arange(n, dtype=torch.float64) / n)
 
 
-def stft_power(x, fft_size, hop_size, win_length):
-    """|STFT|^2 exactly as ``torch.stft(center=True, pad_mode='reflect')`` frames it
-    (losses/stft_loss.py:31-33): reflect-pad n_fft/2, frame t = padded[t*hop : t*hop+n_fft],
-    periodic Hann of win_length centred inside n_fft, rFFT.  x: (B, T) -> (B, frames, bins).
-    Restated with explicit framing + torch.fft.rfft (fp32)."""
+def windowed_frames(x, fft_size, hop_size, win_length, window="hann"):
+    """The frames ``torch.stft(center=True, pad_mode='reflect')`` transforms (losses/stft_loss.py:31-33):
+    reflect-pad n_fft/2, frame t = padded[t*hop : t*hop+n_fft], times a window of win_length centred inside n_fft:
+    periodic Hann (``window="hann"``), all ones (``window=None``) or the given (win_length,) tensor.
+    x: (B, T) -> (B, frames, n_fft) in x's dtype (the window is taken to float64, then rounded to it)."""
     B, T = x.shape
     pad = fft_size // 2
     xp = F.pad(x.unsqueeze(1), (pad, pad), mode="reflect").squeeze(1)
@@ -508,26 +508,37 @@ def stft_power(x, fft_size, hop_size, win_length):
     frames = xp[:, idx]  # (B, frames, n_fft)
     win = torch.zeros(fft_size, dtype=torch.float64)
     left = (fft_size - win_length) // 2
-    win[left : left + win_length] = hann_window(win_length)
-    spec = torch.fft.rfft(frames * win.float(), dim=-1)
+    if isinstance(window, torch.Tensor):
+        win[left : left + win_length] = window.detach().cpu().double()
+    else:
+        win[left : left + win_length] = hann_window(win_length) if window == "hann" else 1.0
+    return frames * win.to(x.dtype)
+
+
+def stft_power(x, fft_size, hop_size, win_length, window="hann"):
+    """|STFT|^2: rFFT of :func:`windowed_frames`.  x: (B, T) -> (B, frames, bins), in x's dtype (fp32 for
+    parity with the reference, float64 as the exact oracle of the fp32 kernels)."""
+    spec = torch.fft.rfft(windowed_frames(x, fft_size, hop_size, win_length, window), dim=-1)
     return spec.real**2 + spec.imag**2
 
 
-def stft_mag(x, fft_size, hop_size, win_length):
+def stft_mag(x, fft_size, hop_size, win_length, window="hann"):
     """stft() of losses/stft_loss.py:16-40: sqrt(clamp(re^2+im^2, 1e-7))."""
-    return torch.sqrt(torch.clamp(stft_power(x, fft_size, hop_size, win_length), min=1e-7))
+    return torch.sqrt(torch.clamp(stft_power(x, fft_size, hop_size, win_length, window), min=1e-7))
 
 
-def mr_stft_loss(x, y, fft_sizes=(1024, 2048, 512), hop_sizes=(120, 240, 50), win_lengths=(600, 1200, 240)):
-    """MultiResolutionSTFTLoss.forward (losses/stft_loss.py:146-170) -> (sc, mag)."""
+def mr_stft_loss(x, y, fft_sizes=(1024, 2048, 512), hop_sizes=(120, 240, 50), win_lengths=(600, 1200, 240), windows=None):
+    """MultiResolutionSTFTLoss.forward (losses/stft_loss.py:146-170) -> (sc, mag).  ``windows``: one window per
+    resolution as :func:`windowed_frames` takes it (default Hann)."""
     if x.dim() == 3:
         x = x.reshape(-1, x.shape[2])
         y = y.reshape(-1, y.shape[2])
     sc = 0.0
     mag = 0.0
-    for n, h, wl in zip(fft_sizes, hop_sizes, win_lengths):
-        xm = stft_mag(x, n, h, wl)
-        ym = stft_mag(y, n, h, wl)
+    windows = ["hann"] * len(fft_sizes) if windows is None else windows
+    for n, h, wl, w in zip(fft_sizes, hop_sizes, win_lengths, windows):
+        xm = stft_mag(x, n, h, wl, w)
+        ym = stft_mag(y, n, h, wl, w)
         sc = sc + torch.norm(ym - xm, p="fro") / torch.norm(ym, p="fro")  # stft_loss.py:61
         mag = mag + F.l1_loss(torch.log(ym), torch.log(xm))  # stft_loss.py:82
     return sc / len(fft_sizes), mag / len(fft_sizes)
@@ -578,12 +589,12 @@ def slaney_mel_filterbank(sr, n_fft, n_mels=80, fmin=0.0, fmax=None):
     return weights.astype(np.float32)
 
 
-def mel_spectrogram(x, melmat, fft_size=1024, hop_size=256, win_length=None, eps=1e-10, log_base=10.0):
-    """MelSpectrogram.forward (losses/mel_loss.py:81-110).  melmat: (bins, n_mels)."""
+def mel_spectrogram(x, melmat, fft_size=1024, hop_size=256, win_length=None, eps=1e-10, log_base=10.0, window="hann"):
+    """MelSpectrogram.forward (losses/mel_loss.py:81-110).  melmat: (bins, n_mels), in x's dtype."""
     if x.dim() == 3:
         x = x.reshape(-1, x.shape[2])
     win_length = fft_size if win_length is None else win_length
-    amp = torch.sqrt(torch.clamp(stft_power(x, fft_size, hop_size, win_length), min=eps))
+    amp = torch.sqrt(torch.clamp(stft_power(x, fft_size, hop_size, win_length, window), min=eps))
     mel = torch.clamp(torch.matmul(amp, melmat), min=eps)
     if log_base is None:
         out = torch.log(mel)

@@ -386,6 +386,23 @@ __global__ void stft_loss_dmag_kernel(const float* __restrict__ xm, const float*
   }
 }
 
+// A kernel may use 48 KB of shared memory, static and dynamic together, unless it opts in to more.  The FFT kernels
+// reach that at n_fft = 4096 (stft_pair_kernel<0>: 48 KB dynamic + 96 B static), so they opt in whenever their total
+// would pass 48 KB.
+template <typename Kernel>
+static int allow_dynamic_smem(Kernel kernel, size_t dyn, const char* what) {
+  if (dyn <= 32 * 1024) return PWGB_OK;  // far below the limit: skip the attribute query
+  cudaFuncAttributes a;
+  cudaError_t e = cudaFuncGetAttributes(&a, kernel);
+  if (e == cudaSuccess && dyn + a.sharedSizeBytes > 48 * 1024)
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
+  if (e != cudaSuccess) {
+    set_error("%s: shared memory opt-in: %s", what, cudaGetErrorString(e));
+    return PWGB_CUDA_ERROR;
+  }
+  return PWGB_OK;
+}
+
 static int fill(const pwgb_stft_desc* d, StftK& p) {
   if (!d || d->batch < 0 || d->t <= 0 || d->n_fft < 16 || d->n_fft > 4096 || (d->n_fft & (d->n_fft - 1)) ||
       d->hop <= 0 || d->win_length <= 0 || d->win_length > d->n_fft || d->t <= d->n_fft / 2)
@@ -440,8 +457,10 @@ extern "C" int pwgb_mr_stft_loss_forward(const pwgb_stft_desc* descs, int n_res,
     nelem[r] = (long long)p.B * p.frames * p.bins;
     const size_t smem = (size_t)(p.n + p.n / 2) * sizeof(float2);
     if (p.B > 0) {
+      int rc = allow_dynamic_smem(stft_pair_kernel<0>, smem, "stft_pair_kernel");
+      if (rc) return rc;
       stft_pair_kernel<0><<<dim3(p.frames, p.B), 256, smem, st>>>(p, x, y, windows[r], part + off, nullptr);
-      int rc = check_launch("stft_pair_kernel");
+      rc = check_launch("stft_pair_kernel");
       if (rc) return rc;
     }
     off += (size_t)counts[r] * 3;
@@ -457,6 +476,8 @@ extern "C" int pwgb_stft_amplitude_forward(const pwgb_stft_desc* d, const float*
   PWGB_CHECK_ARG(fill(d, p), "stft_amplitude: bad descriptor (n_fft must be a power of two <= 4096, t > n_fft/2)");
   if (p.B == 0) return PWGB_OK;
   const size_t smem = (size_t)(p.n + p.n / 2) * sizeof(float2);
+  const int rc = allow_dynamic_smem(stft_pair_kernel<1>, smem, "stft_pair_kernel");
+  if (rc) return rc;
   stft_pair_kernel<1><<<dim3(p.frames, p.B), 256, smem, (cudaStream_t)stream>>>(p, x, y, window, amp_x, amp_y);
   return check_launch("stft_pair_kernel");
 }
@@ -485,13 +506,8 @@ extern "C" int pwgb_stft_amplitude_backward(const pwgb_stft_desc* d, const float
   PWGB_CHECK_ARG(fill(d, p), "stft_amplitude_backward: bad descriptor");
   if (p.B == 0) return PWGB_OK;
   const size_t smem = (size_t)(2 * p.n + p.n / 2) * sizeof(float2);
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(stft_amp_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) {
-      set_error("stft_amplitude_backward: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-      return PWGB_CUDA_ERROR;
-    }
-  }
+  const int rc = allow_dynamic_smem(stft_amp_backward_kernel, smem, "stft_amplitude_backward");
+  if (rc) return rc;
   stft_amp_backward_kernel<<<dim3(p.frames, p.B), 256, smem, (cudaStream_t)stream>>>(p, x, window, amp, damp, dx);
   return check_launch("stft_amp_backward_kernel");
 }

@@ -72,8 +72,31 @@ class STFTLoss(torch.nn.Module):
         self.register_buffer("window", getattr(torch, window)(win_length))
 
     def forward(self, x, y):
-        out = ops.mr_stft_loss(x, y, [self.fft_size], [self.shift_size], [self.win_length], [self.window])
+        return _mr_stft_loss([self], x, y)
+
+
+def _check_target(y):
+    if torch.is_grad_enabled() and y.requires_grad:
+        raise PwgbError("spectral losses differentiate the generated signal only: the target must not require grad "
+                        "(detach it)")
+
+
+def _mr_stft_loss(resolutions, x, y):
+    """[STFTLoss] -> (sc, mag): the fused no-grad kernels, or MrStftLossFn when x requires grad."""
+    _check_target(y)
+    if torch.is_grad_enabled() and x.requires_grad:
+        from .autograd import MrStftLossFn
+
+        if x.dim() == 3:
+            x = x.reshape(-1, x.size(2))
+            y = y.reshape(-1, y.size(2))
+        out = MrStftLossFn.apply(x.contiguous(), y.contiguous(), [f.fft_size for f in resolutions],
+                                 [f.shift_size for f in resolutions], [f.win_length for f in resolutions],
+                                 *[f.window for f in resolutions])
         return out[0], out[1]
+    out = ops.mr_stft_loss(x, y, [f.fft_size for f in resolutions], [f.shift_size for f in resolutions],
+                           [f.win_length for f in resolutions], [f.window for f in resolutions])
+    return out[0], out[1]
 
 
 class MultiResolutionSTFTLoss(torch.nn.Module):
@@ -88,24 +111,7 @@ class MultiResolutionSTFTLoss(torch.nn.Module):
 
     def forward(self, x, y):
         """x, y: (B, T) or (B, #subband, T) -> (sc_loss, mag_loss)."""
-        if torch.is_grad_enabled() and x.requires_grad:
-            from .autograd import MrStftLossFn
-
-            if x.dim() == 3:
-                x = x.reshape(-1, x.size(2))
-                y = y.reshape(-1, y.size(2))
-            out = MrStftLossFn.apply(x.contiguous(), y.contiguous(), [f.fft_size for f in self.stft_losses],
-                                     [f.shift_size for f in self.stft_losses], [f.win_length for f in self.stft_losses],
-                                     *[f.window for f in self.stft_losses])
-            return out[0], out[1]
-        out = ops.mr_stft_loss(
-            x, y,
-            [f.fft_size for f in self.stft_losses],
-            [f.shift_size for f in self.stft_losses],
-            [f.win_length for f in self.stft_losses],
-            [f.window for f in self.stft_losses],
-        )
-        return out[0], out[1]
+        return _mr_stft_loss(self.stft_losses, x, y)
 
 
 # --------------------------------------------------------------------------
@@ -198,6 +204,7 @@ class MelSpectrogramLoss(torch.nn.Module):
 
     def forward(self, y_hat, y):
         m = self.mel_spectrogram
+        _check_target(y)
         if y_hat.dim() == 3:
             y_hat = y_hat.reshape(-1, y_hat.size(2))
             y = y.reshape(-1, y.size(2))

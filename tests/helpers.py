@@ -1,11 +1,12 @@
 """Shared helpers for parity tests (tolerances are stated here once)."""
 import json
+import math
 import os
 
 import numpy as np
 import torch
 
-from oracle import synth
+from oracle import ref_ops, synth
 from oracle.ref_ops import fold_weight_norm
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -74,6 +75,34 @@ def check_fingerprint(outs, meta, g, tol):
         assert abs(float(v.sum()) - ssum) <= tol * max(snorm * v.numel() ** 0.5, 1e-12), (n, float(v.sum()), ssum)
         assert rel_l2(t.reshape(-1)[:96], g[n + "_head"]) < tol, n
         assert rel_l2(t.reshape(-1)[-96:], g[n + "_tail"]) < tol, n
+
+
+# STFT geometries (n_fft, hop, win_length, T) where framing and FFT kernels go wrong: the shortest admitted T = n/2 + 1,
+# odd n - win, hops that do not divide T or exceed n, fewer bins than a warp (n = 16) and the largest n (4096).
+SPECTRAL_GEOMS = [
+    (16, 4, 16, 9),
+    (32, 7, 25, 100),
+    (64, 80, 41, 300),
+    (512, 50, 240, 2000),
+    (1024, 120, 600, 8192),
+    (1024, 256, 1024, 8192),
+    (2048, 300, 1200, 8193),
+    (4096, 480, 2400, 9000),
+]
+
+
+def stft_frame_bound(x, y, n_fft, hop, win_length, window="hann", kappa=1.0):
+    """Per-frame bound on the fp32 STFT amplitude error: over the bins of frame f,
+    ||a - a64||_2 <= kappa * log2(n) * 2^-24 * sqrt(n) * (||w x_f||_2 + ||w y_f||_2),
+    the forward error of a radix-2 FFT of length n on z = w (x + i y).  ``y`` is the signal that shares x's FFT
+    (None when x runs alone): in the pair transform each signal's rounding error scales with both energies.
+    x, y: (B, T) -> (B, frames) float64."""
+
+    def energy(s):
+        return ref_ops.windowed_frames(s.double(), n_fft, hop, win_length, window).norm(dim=-1)
+
+    e = energy(x) + (energy(y) if y is not None else 0.0)
+    return kappa * math.log2(n_fft) * 2.0**-24 * math.sqrt(n_fft) * e
 
 
 def conditioning_tolerances(grad_fn, leaves, rel_eps=1e-6, k=4.0, floor=1e-3, seed=1234):
