@@ -138,8 +138,7 @@ PWGB_API int pwgb_dropout_backward(const float* gy, float* gx, long long n, floa
  * pwgb_conv1d_forward.
  * ---------------------------------------------------------------------- */
 /* measurement aids (not part of the product contract): set key 1 = conv variant (value 2: stage activations with
- * cp.async instead of TMA; value 4: register epilogue instead of the staged one); set key 3 = 1 runs every fused
- * ResBlock pair on the lockstep kernel (pwgb_resblock_pair_variant() == 1), 0 restores the default; get key 1 copies the plan of the last
+ * cp.async instead of TMA; value 4: register epilogue instead of the staged one); get key 1 copies the plan of the last
  * tensor-core conv launch, 8 ints {MT, na, nb, ns, staged, tma_act, win_mode, nco} (a buffer of at least 5 ints gets
  * the leading min(bytes, 32) bytes); get key 2 copies the plan of the last tensor-core weight-gradient launch, 4 ints
  * {nc, tg, ntg, nsplit}.  Returns 0, or -1 for any other key or a short buffer. */
@@ -162,11 +161,10 @@ PWGB_API int pwgb_conv1d_tc_forward(const pwgb_conv1d_desc* d, const float* x, c
  * x, y: (batch, channels, t), 16-byte aligned, y must not alias x.  Both convs pad with zeros ("same" length).
  * w1_packed / w2_packed: pwgb_conv1d_tc_pack_weight images of the two (channels, channels, kernel) weights; b1 / b2
  * may be NULL.  The result is bit-identical to the two pwgb_conv1d_tc_forward calls it replaces.
- * pwgb_resblock_pair_supported() == 0 (channels other than 32 / 64, t % 4 != 0, or no shared-memory plan): use
- * those two calls instead.  pwgb_resblock_pair_plan() fills 5 ints {output rows per tile, conv rows per tile,
- * conv1 operand buffers, weight stages, raw activation stages} and returns 1, or returns 0 when unsupported.
- * pwgb_resblock_pair_variant() returns the kernel a call would run: 2 = one consumer warpgroup per conv (the default),
- * 1 = both warpgroups through both convs in lockstep (plans the split kernel cannot fit), 0 = unsupported.
+ * pwgb_resblock_pair_supported() == 0 (channels other than 32 / 64, t % 4 != 0, or no shared-memory plan, as for a
+ * wide conv1 halo): use those two calls instead.  pwgb_resblock_pair_plan() fills 5 ints {output rows per tile, conv
+ * rows per tile, conv1 operand buffers, weight stages of both rings, raw activation stages} and returns 1, or returns 0
+ * when unsupported.
  * ---------------------------------------------------------------------- */
 typedef struct pwgb_resblock_desc {
   int32_t batch, channels, t;
@@ -177,7 +175,6 @@ typedef struct pwgb_resblock_desc {
 } pwgb_resblock_desc;
 PWGB_API int pwgb_resblock_pair_supported(const pwgb_resblock_desc* d);
 PWGB_API int pwgb_resblock_pair_plan(const pwgb_resblock_desc* d, int* info);
-PWGB_API int pwgb_resblock_pair_variant(const pwgb_resblock_desc* d);
 PWGB_API int pwgb_resblock_pair_forward(const pwgb_resblock_desc* d, const float* x, const void* w1_packed, const float* b1,
                                const void* w2_packed, const float* b2, float* y, void* stream);
 

@@ -111,8 +111,6 @@ def lib():
     L.pwgb_resblock_pair_supported.argtypes = [C.POINTER(ResBlockDesc)]
     L.pwgb_resblock_pair_plan.restype = C.c_int
     L.pwgb_resblock_pair_plan.argtypes = [C.POINTER(ResBlockDesc), C.POINTER(C.c_int)]
-    L.pwgb_resblock_pair_variant.restype = C.c_int
-    L.pwgb_resblock_pair_variant.argtypes = [C.POINTER(ResBlockDesc)]
     L.pwgb_resblock_pair_forward.restype = C.c_int
     L.pwgb_resblock_pair_forward.argtypes = [C.POINTER(ResBlockDesc), vp, vp, vp, vp, vp, vp, vp]
     L.pwgb_wavenet_supported.restype = C.c_int
@@ -273,7 +271,7 @@ EXPORTED_SYMBOLS = [
     "pwgb_conv1d_tc_packed_weight_bytes", "pwgb_conv1d_tc_pack_weight", "pwgb_conv1d_tc_pack_weight_grouped",
     "pwgb_conv1d_tc_supported",
     "pwgb_conv1d_tc_forward", "pwgb_debug_set", "pwgb_debug_get",
-    "pwgb_resblock_pair_supported", "pwgb_resblock_pair_plan", "pwgb_resblock_pair_variant", "pwgb_resblock_pair_forward",
+    "pwgb_resblock_pair_supported", "pwgb_resblock_pair_plan", "pwgb_resblock_pair_forward",
     "pwgb_wavenet_supported", "pwgb_wavenet_packed_bytes",
     "pwgb_wavenet_pack", "pwgb_wavenet_layer_forward", "pwgb_upsample_fir_forward",
     "pwgb_s2d_forward", "pwgb_s2d_backward", "pwgb_mt_clip_coef", "pwgb_mt_adam_step", "pwgb_prep_features", "pwgb_pcm16_forward", "pwgb_collate_crop",

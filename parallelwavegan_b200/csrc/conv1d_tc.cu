@@ -929,7 +929,6 @@ static int tc_cout_chunk(int cout);
 
 extern "C" void pwgb_debug_set(int key, int value) {
   if (key == 1) g_tc_variant = value;
-  if (key == 3) rb_debug_lockstep(value);
 }
 
 // key 1: the plan of the last conv1d_tc launch, {MT, na, nb, ns, staged, tma_act, win_mode, nco};

@@ -13,15 +13,13 @@
 // rounded down to a multiple of 4 (16-byte output rows).  Halo rows of h are recomputed by the neighbouring tile.  Conv2
 // also runs TT rows per tile; rows >= M2 read beyond the computed h rows and are dropped.
 //
-// Two kernels, one persistent CTA per SM each, with the producers and loaders of conv1d_tc_kernel with TMA-staged
-// activations: producer warps convert landed raw fp32 rows of x (pre-activation, padding mask, hi/lo split) into conv1's
-// operand image, two consumer warpgroups run the MMAs, one warp loads weight stages and one raw activation rows, both by
-// cp.async.bulk.
-// rb_pair_split_kernel (the default, 512 threads): warpgroup 0 runs conv1 of every tile and writes the h image,
-// warpgroup 1 runs conv2 on it and the staged epilogue, so that one warpgroup's drain, h write or epilogue overlaps the
-// other's MMAs.  Each conv owns a weight ring.  resblock_pair_kernel (lockstep, 576 threads): both warpgroups split a
-// tile by rows and run conv1, the h write, conv2 and the epilogue one after another; it is kept for the plans the split
-// kernel cannot fit (wide conv1 halos) and for A/B timing (pwgb_debug_set(3, 1)).
+// One kernel, rb_pair_split_kernel, one persistent CTA per SM, with the producers and loaders of conv1d_tc_kernel with
+// TMA-staged activations: producer warps convert landed raw fp32 rows of x (pre-activation, padding mask, hi/lo split)
+// into conv1's operand image, one warp loads weight stages and one raw activation rows, both by cp.async.bulk.  The two
+// consumer warpgroups are split by conv: warpgroup 0 runs conv1 of every tile and writes the h image, warpgroup 1 runs
+// conv2 on it and the staged epilogue, so that one warpgroup's drain, h write or epilogue overlaps the other's MMAs.
+// Each conv owns a weight ring.  A pair whose conv1 halo leaves no room for two rings of RB_MIN_STAGES stages has no
+// plan and runs as the two conv1d_tc launches.
 #include <cstring>
 
 #include "tc_common.cuh"
@@ -30,35 +28,31 @@ namespace pwgb {
 
 namespace {
 
-constexpr int RB_NPROD = 256;  // producer threads (warps 0-7)
-constexpr int RB_NCONS = 256;  // consumer threads (warps 8-15)
-constexpr int RB_W_CONS0 = RB_NPROD / 32, RB_W_TMA = (RB_NPROD + RB_NCONS) / 32, RB_W_LDA = RB_W_TMA + 1;
-constexpr int RB_THREADS = RB_NPROD + RB_NCONS + 64;
+// 512 threads, so that a thread may hold 128 registers (warps are allocated in fours: at 18 warps the limit is 96, and
+// the 64 accumulator registers spill): warps 0-3 conv1, warps 4-7 conv2 and the epilogue, warps 8-13 the producers
+// (a chunk has at most TT + 50 conv1 rows), warp 14 the weight rings, warp 15 the raw activation rows.
+constexpr int RB_NPROD = 192;
+constexpr int RB_W_PROD0 = 8, RB_W_TMA = RB_W_PROD0 + RB_NPROD / 32, RB_W_LDA = RB_W_TMA + 1;
+constexpr int RB_THREADS = 32 * (RB_W_LDA + 1);
 __host__ __device__ constexpr int rb_sld(int mt) { return 64 * mt + 4; }  // staged epilogue row pitch, as in conv1d_tc.cu
 constexpr size_t RB_SMEM = 227 * 1024;      // H100 opt-in limit of dynamic shared memory per block
-constexpr int RB_MIN_STAGES = 4;            // weight stages a plan must keep (per ring)
-
-int g_rb_lockstep = 0;  // pwgb_debug_set(3, 1): plan every pair for the lockstep kernel
+constexpr int RB_MIN_STAGES = 4;            // weight stages a plan must keep per ring
 
 struct RbK {
   int B, C, T, K, D;
   float slope, out_scale;
   int accumulate;
-  int split;               // 1: rb_pair_split_kernel, 0: resblock_pair_kernel
-  int MT, M2;              // 64-row blocks per consumer warpgroup, output rows per tile
+  int MT, M2;              // 64-row blocks per tile, output rows per tile
   int p1, p2;              // left padding of conv1 ((k-1)/2 * d) and conv2 ((k-1)/2)
   int R1, R4, Rh;          // conv1 operand rows, raw stage row pitch (floats), h image rows (TT + k - 1)
   int nchunks, tiles_per_seq, total_tiles;
-  int na, nb, ns;          // conv1 operand buffers, weight stages (both rings of the split kernel), raw stages
+  int na, nb, ns;          // conv1 operand buffers, weight stages (both rings), raw stages
   int a_bytes, b_bytes, raw_bytes, h_bytes;  // per buffer / stage; h_bytes: one 32-channel chunk of the h image
 };
 
-// consumers of both warpgroups (named barrier 4; 1 = conv producers, 2-3 = per-warpgroup barriers)
-__device__ __forceinline__ void consumer_barrier() { asm volatile("bar.sync 4, %0;" ::"n"(RB_NCONS) : "memory"); }
-
 // ===================== A producers: raw fp32 rows -> conv1 operand image =====================
-// NPROD producer threads, this one `tid` of them.  Barrier arguments are the first of each array of 8-byte mbarriers.
-template <int NCH, int NPROD>
+// RB_NPROD producer threads, this one `tid` of them.  Barrier arguments are the first of each array of 8-byte mbarriers.
+template <int NCH>
 __device__ __forceinline__ void rb_convert_x(const RbK& p, unsigned char* a_buf, const unsigned char* raw_buf, unsigned a_full,
                                              unsigned a_empty, unsigned raw_full, unsigned raw_empty, int tid) {
   int s = 0, sph = 0, buf = 0, aph = 0;
@@ -72,7 +66,7 @@ __device__ __forceinline__ void rb_convert_x(const RbK& p, unsigned char* a_buf,
       mbar_wait(a_empty + 8u * buf, aph ^ 1);
       unsigned char* dst = a_buf + (size_t)buf * p.a_bytes;
       const float* raw = reinterpret_cast<const float*>(raw_buf + (size_t)s * p.raw_bytes);
-      for (int r = tid; r < p.R1; r += NPROD) {
+      for (int r = tid; r < p.R1; r += RB_NPROD) {
         const bool ok = (unsigned)(ts_first + r) < (unsigned)p.T;
         const float* rr = raw + r + shift;
 #pragma unroll
@@ -184,210 +178,13 @@ __device__ __forceinline__ void rb_stage_result(const float* acc, float* stg, co
   }
 }
 
-// MT: 64-row blocks per consumer warpgroup; NB16: channels / 16 (the MMA width; the weight images are the conv1d_tc
-// images of a Cout = C conv)
-template <int MT, int NB16>
-__global__ void __launch_bounds__(RB_THREADS, 1)
-    resblock_pair_kernel(const RbK p, const float* __restrict__ x, const unsigned char* __restrict__ w1,
-                         const float* __restrict__ b1, const unsigned char* __restrict__ w2, const float* __restrict__ b2,
-                         float* __restrict__ y) {
-  extern __shared__ __align__(128) unsigned char smem[];
-  constexpr int C = 16 * NB16, NCH = C / KC, NACC = 8 * NB16, SLD = rb_sld(MT), WR = 64 * MT;  // WR: rows per warpgroup
-  // layout: A[na] | B[nb] | raw staging[ns] | h image[NCH chunks] | epilogue tiles[2] | barriers | bias1 | bias2
-  unsigned char* a_buf = smem;
-  unsigned char* b_buf = a_buf + (size_t)p.na * p.a_bytes;
-  unsigned char* raw_buf = b_buf + (size_t)p.nb * p.b_bytes;
-  unsigned char* h_buf = raw_buf + (size_t)p.ns * p.raw_bytes;
-  float* stage_buf = reinterpret_cast<float*>(h_buf + (size_t)NCH * p.h_bytes);
-  unsigned long long* bars = reinterpret_cast<unsigned long long*>(stage_buf + 2 * C * SLD);
-  const int nbar = 2 * p.na + 2 * p.nb + 2 * p.ns + 2;
-  float* bias_s = reinterpret_cast<float*>(bars + nbar);  // b1 | b2 (zeros for a missing bias)
-
-  const int tid = threadIdx.x;
-  const int warp = tid >> 5;
-  const int lane = tid & 31;
-
-  const unsigned bar0 = smem_u32(bars);
-  auto A_FULL = [&](int i) { return bar0 + 8u * i; };
-  auto A_EMPTY = [&](int i) { return bar0 + 8u * (p.na + i); };
-  auto B_FULL = [&](int i) { return bar0 + 8u * (2 * p.na + i); };
-  auto B_EMPTY = [&](int i) { return bar0 + 8u * (2 * p.na + p.nb + i); };
-  auto RAW_FULL = [&](int i) { return bar0 + 8u * (2 * p.na + 2 * p.nb + i); };
-  auto RAW_EMPTY = [&](int i) { return bar0 + 8u * (2 * p.na + 2 * p.nb + p.ns + i); };
-  auto RES_FULL = [&](int wg) { return bar0 + 8u * (2 * p.na + 2 * p.nb + 2 * p.ns + wg); };
-
-  if (tid == 0) {
-    for (int i = 0; i < p.na; ++i) {
-      mbar_init(A_FULL(i), RB_NPROD);
-      mbar_init(A_EMPTY(i), RB_NCONS / 32);
-    }
-    for (int i = 0; i < p.nb; ++i) {
-      mbar_init(B_FULL(i), 1);
-      mbar_init(B_EMPTY(i), RB_NCONS / 32);
-    }
-    for (int i = 0; i < p.ns; ++i) {
-      mbar_init(RAW_FULL(i), 1);
-      mbar_init(RAW_EMPTY(i), RB_NPROD);
-    }
-    for (int i = 0; i < 2; ++i) mbar_init(RES_FULL(i), C);  // one arrival per channel row of the warpgroup's tile
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  for (int i = tid; i < 2 * C; i += RB_THREADS) {
-    const float* bb = i < C ? b1 : b2;
-    bias_s[i] = bb ? __ldg(bb + (i < C ? i : i - C)) : 0.f;
-  }
-  // conv2 rows >= M2 read the h rows [128 MT, Rh) that no tile writes: keep them zero
-  for (int i = tid; i < NCH * p.h_bytes / 16; i += RB_THREADS) reinterpret_cast<uint4*>(h_buf)[i] = make_uint4(0, 0, 0, 0);
-  fence_proxy_async();
-  __syncthreads();
-
-  if (warp < RB_W_CONS0) {
-    rb_convert_x<NCH, RB_NPROD>(p, a_buf, raw_buf, A_FULL(0), A_EMPTY(0), RAW_FULL(0), RAW_EMPTY(0), tid);
-  } else if (warp < RB_W_TMA) {
-    // ===================== consumers =====================
-    // warpgroup wg owns conv rows [WR wg, WR wg + WR) of both convs.  One wgmma group per (chunk, tap), kept in flight
-    // while the next is issued, as in conv1d_tc_kernel.
-    const int wg = (warp - RB_W_CONS0) >> 2, wq = warp & 3;
-    const unsigned lbo_a = (unsigned)p.R1 * 16u, a_sub = (unsigned)(KC / 8) * p.R1;
-    const unsigned lbo_h = (unsigned)p.Rh * 16u, h_sub = (unsigned)(KC / 8) * p.Rh;
-    // staged epilogue: thread wt of the warpgroup owns channel row wt of the warpgroup's tile (residual in, result out)
-    const int wt = tid - RB_NPROD - wg * 128;
-    float* stg = stage_buf + (size_t)wg * C * SLD;
-    const bool row_owner = wt < C;
-    int buf = 0, aph = 0, s = 0, bph = 0;
-    // channel row wt of this warpgroup's output rows of a tile: first element and bytes (below M2 and T)
-    auto row_pos = [&](int tile, unsigned& row_bytes) -> long long {
-      const int b = tile / p.tiles_per_seq;
-      const int t0 = (tile - b * p.tiles_per_seq) * p.M2;
-      int nrow = p.M2 - wg * WR;
-      if (nrow > WR) nrow = WR;
-      if (nrow > p.T - (t0 + wg * WR)) nrow = p.T - (t0 + wg * WR);
-      row_bytes = nrow > 0 ? 4u * (unsigned)nrow : 0u;
-      return ((long long)b * C + wt) * p.T + t0 + wg * WR;
-    };
-    // the residual (x itself) of a tile, issued at the end of the previous tile's epilogue so that it streams in while
-    // this tile's MMAs run
-    auto load_res = [&](int tile) {
-      unsigned row_bytes;
-      const long long off = row_pos(tile, row_bytes);
-      bulk_wait_read();  // the previous store has read the row
-      if (row_bytes) {
-        mbar_expect_tx(RES_FULL(wg), row_bytes);
-        bulk_g2s(smem_u32(stg + wt * SLD), x + off, row_bytes, RES_FULL(wg));
-      } else {
-        mbar_arrive(RES_FULL(wg));
-      }
-    };
-    auto release = [&](int held_s, int held_a) {
-      __syncwarp();
-      if (lane == 0) {
-        if (held_s >= 0) mbar_arrive(B_EMPTY(held_s));
-        if (held_a >= 0) mbar_arrive(A_EMPTY(held_a));
-      }
-    };
-    if (row_owner && (int)blockIdx.x < p.total_tiles) load_res(blockIdx.x);
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      const int b = tile / p.tiles_per_seq;
-      const int t0 = (tile - b * p.tiles_per_seq) * p.M2;
-      float acc[MT * NACC];
-      // ---- conv1 over the staged x rows
-#pragma unroll
-      for (int e = 0; e < MT * NACC; ++e) acc[e] = 0.f;
-      int held_s = -1, held_a = -1;  // weight stage / A buffer read by the group in flight
-      for (int c = 0; c < NCH; ++c) {
-        mbar_wait_trap(A_FULL(buf), aph);
-        const unsigned a_addr = smem_u32(a_buf + (size_t)buf * p.a_bytes);
-        for (int k = 0; k < p.K; ++k) {
-          mbar_wait_trap(B_FULL(s), bph);
-          __syncwarp();
-          rb_mma_stage<MT, NB16>(acc, a_addr, lbo_a, a_sub, k * p.D + wg * WR, smem_u32(b_buf + (size_t)s * p.b_bytes));
-          wg_wait<1>();  // the previous group has retired: its stage and, at a chunk boundary, its A buffer are free
-          release(held_s, held_a);
-          held_s = s;
-          held_a = k == p.K - 1 ? buf : -1;
-          if (++s == p.nb) { s = 0; bph ^= 1; }
-        }
-        if (++buf == p.na) { buf = 0; aph ^= 1; }
-      }
-      wg_wait<0>();
-      release(held_s, held_a);
-      // ---- h image.  Both warpgroups' conv2 MMAs of the previous tile must have read the image first.
-      consumer_barrier();
-      rb_write_h<MT, NB16>(acc, h_buf, p, wg * WR, t0 - p.p2 + wg * WR, bias_s, lane, wq);
-      fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor core
-      consumer_barrier();
-      // ---- conv2 over the h image (resident for the whole tile)
-#pragma unroll
-      for (int e = 0; e < MT * NACC; ++e) acc[e] = 0.f;
-      held_s = -1;
-      for (int c = 0; c < NCH; ++c) {
-        const unsigned h_addr = smem_u32(h_buf + (size_t)c * p.h_bytes);
-        for (int k = 0; k < p.K; ++k) {
-          mbar_wait_trap(B_FULL(s), bph);
-          __syncwarp();
-          rb_mma_stage<MT, NB16>(acc, h_addr, lbo_h, h_sub, k + wg * WR, smem_u32(b_buf + (size_t)s * p.b_bytes));
-          wg_wait<1>();
-          release(held_s, -1);
-          held_s = s;
-          if (++s == p.nb) { s = 0; bph ^= 1; }
-        }
-      }
-      wg_wait<0>();
-      release(held_s, -1);
-      // ---- staged epilogue over the residual row, one bulk store (or fp32 add) per row
-      mbar_wait_trap(RES_FULL(wg), ((tile - blockIdx.x) / gridDim.x) & 1);  // one phase per tile
-      rb_stage_result<MT, NB16>(acc, stg, bias_s + C, p.out_scale, lane, wq);
-      fence_proxy_async();  // generic-proxy writes -> visible to the bulk copies
-      wg_barrier(wg);
-      if (row_owner) {
-        unsigned row_bytes;
-        const long long off = row_pos(tile, row_bytes);
-        if (row_bytes) {
-          if (p.accumulate)
-            bulk_s2g_add(y + off, smem_u32(stg + wt * SLD), row_bytes);
-          else
-            bulk_s2g(y + off, smem_u32(stg + wt * SLD), row_bytes);
-          bulk_commit();
-        }
-        if (tile + (int)gridDim.x < p.total_tiles) load_res(tile + gridDim.x);
-      }
-    }
-    if (row_owner) bulk_wait();  // the shared-memory source must outlive the CTA's last stores
-  } else if (warp == RB_W_TMA) {
-    // ===================== weight stages: conv1's NCH * K, then conv2's, per tile =====================
-    const int per = NCH * p.K;
-    int s = 0, ph = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      for (int j = 0; j < 2 * per; ++j) {
-        mbar_wait_trap(B_EMPTY(s), ph ^ 1);
-        if (elect_one()) {
-          const unsigned char* src = j < per ? w1 + (size_t)j * p.b_bytes : w2 + (size_t)(j - per) * p.b_bytes;
-          mbar_expect_tx(B_FULL(s), (unsigned)p.b_bytes);
-          bulk_g2s(smem_u32(b_buf + (size_t)s * p.b_bytes), src, (unsigned)p.b_bytes, B_FULL(s));
-        }
-        __syncwarp();
-        if (++s == p.nb) { s = 0; ph ^= 1; }
-      }
-    }
-  } else if (warp == RB_W_LDA) {
-    rb_load_raw<NCH>(p, x, raw_buf, RAW_FULL(0), RAW_EMPTY(0), lane);
-  }
-}
-
 // Conv split by warpgroup.  MT = TT / 64: the 64-row blocks of a whole tile, run by one warpgroup (independent
 // accumulator chains: 2 at 64 channels, 4 at 32, 64 accumulator registers either way).  Warpgroup 0 runs conv1 of tile
 // i + 1 while warpgroup 1 runs conv2 and the epilogue of tile i; they hand the single h image over through two
 // mbarriers (H_FULL: written, H_FREE: conv2's MMAs have retired).  Weights come in two rings of nb / 2 stages, conv1's
 // and conv2's, both filled by the weight warp.  The residual rows belong to conv2's warpgroup.
-// 512 threads, so that a thread may hold 128 registers (warps are allocated in fours: at 18 warps the limit is 96, and
-// the 64 accumulator registers spill): warps 0-3 conv1, warps 4-7 conv2 and the epilogue, warps 8-13 the producers
-// (a chunk has at most TT + 50 conv1 rows), warp 14 the weight rings, warp 15 the raw activation rows.
-constexpr int RBS_NPROD = 192;
-constexpr int RBS_W_PROD0 = 8, RBS_W_TMA = RBS_W_PROD0 + RBS_NPROD / 32, RBS_W_LDA = RBS_W_TMA + 1;
-constexpr int RBS_THREADS = 32 * (RBS_W_LDA + 1);
-
 template <int MT, int NB16>
-__global__ void __launch_bounds__(RBS_THREADS, 1)
+__global__ void __launch_bounds__(RB_THREADS, 1)
     rb_pair_split_kernel(const RbK p, const float* __restrict__ x, const unsigned char* __restrict__ w1,
                          const float* __restrict__ b1, const unsigned char* __restrict__ w2, const float* __restrict__ b2,
                          float* __restrict__ y) {
@@ -418,7 +215,7 @@ __global__ void __launch_bounds__(RBS_THREADS, 1)
 
   if (tid == 0) {
     for (int i = 0; i < p.na; ++i) {
-      mbar_init(A_FULL + 8u * i, RBS_NPROD);
+      mbar_init(A_FULL + 8u * i, RB_NPROD);
       mbar_init(A_EMPTY + 8u * i, 4);  // the warps of conv1's warpgroup
     }
     for (int i = 0; i < nr; ++i) {
@@ -429,19 +226,19 @@ __global__ void __launch_bounds__(RBS_THREADS, 1)
     }
     for (int i = 0; i < p.ns; ++i) {
       mbar_init(RAW_FULL + 8u * i, 1);
-      mbar_init(RAW_EMPTY + 8u * i, RBS_NPROD);
+      mbar_init(RAW_EMPTY + 8u * i, RB_NPROD);
     }
     mbar_init(RES_FULL, C);  // one arrival per channel row of the tile
     mbar_init(H_FULL, 128);
     mbar_init(H_FREE, 128);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  for (int i = tid; i < 2 * C; i += RBS_THREADS) {
+  for (int i = tid; i < 2 * C; i += RB_THREADS) {
     const float* bb = i < C ? b1 : b2;
     bias_s[i] = bb ? __ldg(bb + (i < C ? i : i - C)) : 0.f;
   }
   // conv2 rows >= M2 read the h rows [64 MT, Rh) that no tile writes: keep them zero
-  for (int i = tid; i < NCH * p.h_bytes / 16; i += RBS_THREADS) reinterpret_cast<uint4*>(h_buf)[i] = make_uint4(0, 0, 0, 0);
+  for (int i = tid; i < NCH * p.h_bytes / 16; i += RB_THREADS) reinterpret_cast<uint4*>(h_buf)[i] = make_uint4(0, 0, 0, 0);
   fence_proxy_async();
   __syncthreads();
 
@@ -560,9 +357,9 @@ __global__ void __launch_bounds__(RBS_THREADS, 1)
       }
     }
     if (row_owner) bulk_wait();  // the shared-memory source must outlive the CTA's last stores
-  } else if (warp < RBS_W_TMA) {
-    rb_convert_x<NCH, RBS_NPROD>(p, a_buf, raw_buf, A_FULL, A_EMPTY, RAW_FULL, RAW_EMPTY, tid - 32 * RBS_W_PROD0);
-  } else if (warp == RBS_W_TMA) {
+  } else if (warp < RB_W_TMA) {
+    rb_convert_x<NCH>(p, a_buf, raw_buf, A_FULL, A_EMPTY, RAW_FULL, RAW_EMPTY, tid - 32 * RB_W_PROD0);
+  } else if (warp == RB_W_TMA) {
     // ===================== weight stages: both rings, NCH * K stages per tile each =====================
     // The two convs run different tiles, so one lane polls both rings and fills whichever has a free stage.
     if (lane == 0) {
@@ -590,7 +387,7 @@ __global__ void __launch_bounds__(RBS_THREADS, 1)
         else if (++idle > SPIN_LIMIT) __trap();
       }
     }
-  } else if (warp == RBS_W_LDA) {
+  } else if (warp == RB_W_LDA) {
     rb_load_raw<NCH>(p, x, raw_buf, RAW_FULL, RAW_EMPTY, lane);
   }
 }
@@ -598,16 +395,7 @@ __global__ void __launch_bounds__(RBS_THREADS, 1)
 using RbKernel = void (*)(const RbK, const float*, const unsigned char*, const float*, const unsigned char*, const float*,
                           float*);
 
-// Lockstep instantiations: 32 and 64 channels at MT = 1, and 32 channels at MT = 2 (at 64 channels a 256-row tile's h
-// image and epilogue tiles alone would take 135 KB).
-RbKernel rb_kernel_for(int mt, int channels) {
-  if (mt == 1 && channels == 32) return resblock_pair_kernel<1, 2>;
-  if (mt == 1 && channels == 64) return resblock_pair_kernel<1, 4>;
-  if (mt == 2 && channels == 32) return resblock_pair_kernel<2, 2>;
-  return nullptr;
-}
-
-// Split instantiations: 256-row tiles at 32 channels, 128-row tiles at 64 channels (mt: 64-row blocks of a tile)
+// Instantiations: 256-row tiles at 32 channels, 128-row tiles at 64 channels (mt: 64-row blocks of a tile)
 RbKernel rb_split_kernel_for(int channels, int* mt) {
   *mt = channels == 32 ? 4 : 2;
   if (channels == 32) return rb_pair_split_kernel<4, 2>;
@@ -615,13 +403,12 @@ RbKernel rb_split_kernel_for(int channels, int* mt) {
   return nullptr;
 }
 
-// Tile geometry of one kernel at `mt` and the first (na, ns) that leaves RB_MIN_STAGES weight stages per ring: two
+// Tile geometry at `mt` and the first (na, ns) that leaves RB_MIN_STAGES weight stages in each of the two rings: two
 // conv1 operand buffers with three, then two raw stages; then, with one 32-channel chunk, one operand buffer (the
 // producers then convert the next tile while conv2 runs).
-int rb_fit(const pwgb_resblock_desc* d, RbK& p, size_t& smem_bytes, int split, int mt) {
-  const int tt = (split ? 64 : 128) * mt, rings = split ? 2 : 1, epi_tiles = split ? 1 : 2;
+int rb_fit(const pwgb_resblock_desc* d, RbK& p, size_t& smem_bytes, int mt) {
+  const int tt = 64 * mt;
   const long long halo1 = (long long)(d->kernel - 1) * d->dilation;
-  p.split = split;
   p.MT = mt;
   p.M2 = (tt - (d->kernel - 1)) & ~3;
   p.R1 = tt + (int)halo1;
@@ -630,17 +417,17 @@ int rb_fit(const pwgb_resblock_desc* d, RbK& p, size_t& smem_bytes, int split, i
   p.a_bytes = 2 * (KC / 8) * p.R1 * 16;
   p.raw_bytes = KC * p.R4 * 4;
   p.h_bytes = 2 * (KC / 8) * p.Rh * 16;
-  const size_t epi = epi_tiles * (size_t)d->channels * rb_sld(mt) * 4;
+  const size_t epi = (size_t)d->channels * rb_sld(mt) * 4;
   const size_t fixed = (size_t)p.nchunks * p.h_bytes + epi + 2 * (size_t)d->channels * 4 + 1024;
   static const int bufs[3][2] = {{2, 3}, {2, 2}, {1, 2}};  // (na, ns)
   for (const auto& nn : bufs) {
     const int na = nn[0], ns = nn[1];
     if (na < p.nchunks) continue;  // one operand buffer only for a single chunk
     const size_t used = fixed + (size_t)na * p.a_bytes + (size_t)ns * p.raw_bytes;
-    if (used + (size_t)rings * RB_MIN_STAGES * p.b_bytes > RB_SMEM) continue;
+    if (used + (size_t)2 * RB_MIN_STAGES * p.b_bytes > RB_SMEM) continue;
     int nb = (int)((RB_SMEM - used) / p.b_bytes);
     if (nb > 24) nb = 24;
-    nb -= nb % rings;
+    nb -= nb % 2;  // two rings of nb / 2 stages
     p.na = na;
     p.nb = nb;
     p.ns = ns;
@@ -648,19 +435,18 @@ int rb_fit(const pwgb_resblock_desc* d, RbK& p, size_t& smem_bytes, int split, i
     if ((long long)p.tiles_per_seq * d->batch > 0x7fffffffLL) return 0;
     p.total_tiles = p.tiles_per_seq * d->batch;
     smem_bytes = (size_t)na * p.a_bytes + (size_t)nb * p.b_bytes + (size_t)ns * p.raw_bytes + (size_t)p.nchunks * p.h_bytes +
-                 epi + 8 * (size_t)(2 * na + 2 * nb + 2 * ns + 2 + split) + 2 * (size_t)d->channels * 4;
+                 epi + 8 * (size_t)(2 * na + 2 * nb + 2 * ns + 3) + 2 * (size_t)d->channels * 4;
     return 1;
   }
   return 0;
 }
 
-// Plan of one pair: the split kernel where it fits (unless pwgb_debug_set(3, 1) forces lockstep), else the lockstep
-// kernel.  For the lockstep kernel a warpgroup's 64-row blocks are independent accumulator chains, so the planner tries
-// MT = 2 first (the wgmma of one chain wait for each other: at MT = 1 and 32 channels the tensor cores idle between
-// them), then MT = 1.
+// Plan of one pair, or 0 when the pair has none (other channel counts, ragged T, a conv1 halo too wide for rb_fit): the
+// caller then runs the two conv1d_tc launches.
 int rb_plan(const pwgb_resblock_desc* d, RbK& p, size_t& smem_bytes) {
   if (!d || d->batch < 0 || d->t <= 0 || d->kernel < 1 || d->kernel % 2 == 0 || d->dilation < 1) return 0;
-  if (!rb_kernel_for(1, d->channels)) return 0;
+  int mt = 0;
+  if (!rb_split_kernel_for(d->channels, &mt)) return 0;
   if (d->t % 4 != 0) return 0;  // 16-byte rows for the bulk copies of x and y
   const long long halo1 = (long long)(d->kernel - 1) * d->dilation;
   if (d->kernel - 1 > 64 || halo1 > 2048) return 0;
@@ -676,16 +462,10 @@ int rb_plan(const pwgb_resblock_desc* d, RbK& p, size_t& smem_bytes) {
   p.p2 = (d->kernel - 1) / 2;
   p.nchunks = d->channels / KC;
   p.b_bytes = 2 * (KC / 8) * d->channels * 16;
-  int split_mt = 0;
-  if (!g_rb_lockstep && rb_split_kernel_for(d->channels, &split_mt) && rb_fit(d, p, smem_bytes, 1, split_mt)) return 1;
-  for (int mt = 2; mt >= 1; --mt)
-    if (rb_kernel_for(mt, d->channels) && rb_fit(d, p, smem_bytes, 0, mt)) return 1;
-  return 0;
+  return rb_fit(d, p, smem_bytes, mt);
 }
 
 }  // namespace
-
-void rb_debug_lockstep(int on) { g_rb_lockstep = on; }
 
 }  // namespace pwgb
 
@@ -701,16 +481,9 @@ extern "C" int pwgb_resblock_pair_plan(const pwgb_resblock_desc* d, int* info) {
   RbK p;
   size_t bytes;
   if (!info || !rb_plan(d, p, bytes)) return 0;
-  const int v[5] = {p.M2, (p.split ? 64 : 128) * p.MT, p.na, p.nb, p.ns};
+  const int v[5] = {p.M2, 64 * p.MT, p.na, p.nb, p.ns};
   memcpy(info, v, sizeof(v));
   return 1;
-}
-
-extern "C" int pwgb_resblock_pair_variant(const pwgb_resblock_desc* d) {
-  RbK p;
-  size_t bytes;
-  if (!rb_plan(d, p, bytes)) return 0;
-  return p.split ? 2 : 1;
 }
 
 extern "C" int pwgb_resblock_pair_forward(const pwgb_resblock_desc* d, const float* x, const void* w1_packed,
@@ -727,8 +500,7 @@ extern "C" int pwgb_resblock_pair_forward(const pwgb_resblock_desc* d, const flo
   static bool attr_set = false;
   if (!attr_set) {
     int mt;
-    for (const RbKernel k : {rb_kernel_for(1, 32), rb_kernel_for(1, 64), rb_kernel_for(2, 32), rb_split_kernel_for(32, &mt),
-                             rb_split_kernel_for(64, &mt)}) {
+    for (const RbKernel k : {rb_split_kernel_for(32, &mt), rb_split_kernel_for(64, &mt)}) {
       cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RB_SMEM);
       if (e != cudaSuccess) {
         set_error("resblock_pair: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
@@ -745,9 +517,9 @@ extern "C" int pwgb_resblock_pair_forward(const pwgb_resblock_desc* d, const flo
     if (num_sms <= 0) num_sms = 132;
   }
   const int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
-  int mt = p.MT;
-  const RbKernel k = p.split ? rb_split_kernel_for(p.C, &mt) : rb_kernel_for(p.MT, p.C);
-  k<<<(unsigned)grid, p.split ? RBS_THREADS : RB_THREADS, bytes, (cudaStream_t)stream>>>(p, x, (const unsigned char*)w1_packed, b1,
-                                                               (const unsigned char*)w2_packed, b2, y);
-  return check_launch(p.split ? "rb_pair_split_kernel" : "resblock_pair_kernel");
+  int mt;
+  const RbKernel k = rb_split_kernel_for(p.C, &mt);
+  k<<<(unsigned)grid, RB_THREADS, bytes, (cudaStream_t)stream>>>(p, x, (const unsigned char*)w1_packed, b1,
+                                                                 (const unsigned char*)w2_packed, b2, y);
+  return check_launch("rb_pair_split_kernel");
 }

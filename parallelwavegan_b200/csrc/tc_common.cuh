@@ -153,7 +153,4 @@ __device__ __forceinline__ void split2(float a, float b, unsigned& hi, unsigned&
 void tc_pack_rows(const float* w, void* packed, int cin_real, int cin_pad, int rows, int K, int co_begin, int cout_total,
                   cudaStream_t st);
 
-// nonzero: plan every fused ResBlock pair for the lockstep kernel (defined in resblock_tc.cu)
-void rb_debug_lockstep(int on);
-
 }  // namespace pwgb

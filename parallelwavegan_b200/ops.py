@@ -196,7 +196,8 @@ def resblock_pair(x, w1, b1, w2, b2, *, kernel_size, dilation, slope, out=None, 
         x' = conv_{k,1}(lrelu(conv_{k,d}(lrelu(x)) + b1)) + b2 + x     ("same" zero padding, LeakyReLU ``slope``)
     returned as ``out_scale * x'``, or written / added into ``out``.  Bit-identical to the two conv1d calls it replaces.
     Returns None when the fused kernel does not serve the call (autograd, the FFMA engine, channel counts other than
-    32 / 64, t % 4 != 0, unaligned tensors): the caller then runs the two convs."""
+    32 / 64, t % 4 != 0, a conv1 halo too wide for the shared-memory plan, unaligned tensors): the caller then runs the
+    two convs."""
     if ENGINE == "simt" or _needs_grad(x, w1, b1, w2, b2):
         return None
     if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 3 and x.is_contiguous()):
@@ -239,17 +240,14 @@ def resblock_pair(x, w1, b1, w2, b2, *, kernel_size, dilation, slope, out=None, 
 
 def resblock_pair_plan(channels, t, kernel_size, dilation, batch=1):
     """The fused pair's tile plan as a dict (output rows per tile, conv rows per tile, conv1 operand buffers, weight
-    stages of both rings, raw activation stages, and the kernel: "split" = one consumer warpgroup per conv, "lockstep" =
-    both warpgroups through both convs), or None when the pair keeps the two-launch path."""
+    stages of both rings, raw activation stages), or None when the pair keeps the two-launch path."""
     d = capi.ResBlockDesc(batch=batch, channels=channels, t=t, kernel=kernel_size, dilation=dilation, slope=0.1, out_scale=1.0,
                           accumulate=0)
     L = capi.lib()
     v = (C.c_int * 5)()
     if not L.pwgb_resblock_pair_plan(C.byref(d), v):
         return None
-    plan = dict(zip(("M2", "TT", "na", "nb", "ns"), list(v)))
-    plan["variant"] = {1: "lockstep", 2: "split"}[L.pwgb_resblock_pair_variant(C.byref(d))]
-    return plan
+    return dict(zip(("M2", "TT", "na", "nb", "ns"), list(v)))
 
 
 def conv_transpose1d_raw(x, w, bias=None, *, stride, padding=0, output_padding=0, pre_slope=1.0, groups=1, period=1):

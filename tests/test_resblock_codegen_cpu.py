@@ -1,9 +1,10 @@
-"""Codegen guard and plan rule of the fused ResBlock conv pair (csrc/resblock_tc.cu); no GPU needed.
+"""Codegen guard and plan rule of the fused ResBlock conv pair (rb_pair_split_kernel, csrc/resblock_tc.cu); no GPU needed.
 
-Like the stride-1 conv (tests/test_tc_codegen_cpu.py), the fused kernel keeps its wgmma groups in flight only when ptxas
-does not serialize them, and ptxas reports that only as an info message: compile the file for sm_90a with -Xptxas -v and
-fail on any such message and on any spill in a resblock_pair_kernel instantiation.  The plan rule (which pairs take the
-fused kernel) is host code and is checked through the library."""
+Each consumer warpgroup of the kernel keeps 64 accumulator registers and its wgmma groups in flight, which holds only
+when ptxas neither serializes the wgmma nor spills, and ptxas reports serialization only as an info message (as for the
+stride-1 conv, tests/test_tc_codegen_cpu.py): compile the file for sm_90a with -Xptxas -v and fail on any such message
+and on any stack or spill in an rb_pair_split_kernel instantiation.  The plan rule (which pairs take the fused kernel,
+its tile and its two weight rings) is host code and is checked through the library."""
 import os
 import re
 import shutil
@@ -34,24 +35,24 @@ def ptxas_log(tmp_path_factory):
 
 
 def _kernel_properties(log):
-    """{mangled resblock_pair_kernel name: (stack, spill stores, spill loads)}"""
+    """{mangled rb_pair_split_kernel name: (stack, spill stores, spill loads)}"""
     out = {}
-    for m in re.finditer(r"Function properties for (\S*resblock_pair_kernel\S*)\s*\n\s*(\d+) bytes stack frame, (\d+) bytes "
+    for m in re.finditer(r"Function properties for (\S*rb_pair_split_kernel\S*)\s*\n\s*(\d+) bytes stack frame, (\d+) bytes "
                          r"spill stores, (\d+) bytes spill loads", log):
         out[m.group(1)] = tuple(int(g) for g in m.group(2, 3, 4))
     return out
 
 
-def test_resblock_pair_wgmma_not_serialized(ptxas_log):
-    assert _kernel_properties(ptxas_log), "no resblock_pair_kernel in the ptxas report"
+def test_split_kernel_wgmma_not_serialized(ptxas_log):
+    assert _kernel_properties(ptxas_log), "no rb_pair_split_kernel in the ptxas report"
     bad = [line for line in ptxas_log.splitlines() if re.search(r"\(C75\d\d\)|serialized", line)]
     assert not bad, "\n".join(bad[:10])
 
 
-def test_resblock_pair_no_spills(ptxas_log):
+def test_split_kernel_no_spills(ptxas_log):
     props = _kernel_properties(ptxas_log)
-    assert len(props) == 3, sorted(props)  # 32 and 64 channels at MT = 1, 32 channels at MT = 2
-    spilling = {k: v for k, v in props.items() if v[1] or v[2]}
+    assert len(props) == 2, sorted(props)  # 32 channels (256-row tiles) and 64 channels (128-row tiles)
+    spilling = {k: v for k, v in props.items() if any(v)}
     assert not spilling, spilling
 
 
@@ -74,7 +75,9 @@ def test_v1_pairs_at_32_and_64_channels_are_fused(ops, channels, t, k, dilations
         # a 256-row (32 channels) or 128-row (64 channels) conv tile minus the conv2 halo, in 16-byte output rows
         tt = 256 if channels == 32 else 128
         assert plan["TT"] == tt and plan["M2"] == (tt - (k - 1)) // 4 * 4, plan
-        assert plan["na"] >= 1 and plan["ns"] >= 2 and plan["nb"] >= 4, plan
+        # two weight rings of at least four stages each
+        assert plan["nb"] % 2 == 0 and 8 <= plan["nb"] <= 24, plan
+        assert plan["na"] >= 1 and plan["ns"] >= 2, plan
 
 
 @pytest.mark.parametrize("channels,t", [(128, 25600), (256, 3200), (48, 4096)])
@@ -85,3 +88,13 @@ def test_other_channel_counts_keep_two_launches(ops, channels, t):
 def test_ragged_length_keeps_two_launches(ops):
     assert ops.resblock_pair_plan(32, 2049, 3, 1) is None
     assert ops.resblock_pair_plan(32, 2052, 3, 1) is not None
+
+
+def test_wide_halo_keeps_two_launches(ops):
+    """a conv1 halo whose operand buffers leave no room for two weight rings of four stages each has no plan"""
+    # (channels, k, the first dilation without a plan)
+    for channels, k, d in [(64, 11, 6), (64, 7, 11), (64, 3, 31), (32, 11, 9), (32, 7, 15), (32, 3, 43)]:
+        t = 102400 if channels == 32 else 51200
+        assert ops.resblock_pair_plan(channels, t, k, d - 1, batch=16) is not None, (channels, k, d - 1)
+        wider = [dd for dd in range(d, 2 * d) if ops.resblock_pair_plan(channels, t, k, dd, batch=16) is not None]
+        assert not wider, (channels, k, wider)

@@ -1,8 +1,8 @@
 """Per-launch table of the HiFi-GAN v1 C2 forward (CUDA events on the launching stream).  For conv1d_tc launches the
 last column is the tile plan: MT (64-row blocks per warpgroup), na / nb / ns (operand buffers, weight stages, raw
 activation stages) and whether the epilogue went through the shared-memory tile (staged) or registers.  For fused ResBlock
-pairs (resblock_pair_tc) it is the kernel (split or lockstep), the output / conv rows per tile, conv1 operand buffers,
-weight stages and raw stages."""
+pairs (resblock_pair_tc) it is the output / conv rows per tile, conv1 operand buffers, weight stages of both rings and
+raw stages."""
 import ctypes as C
 import os
 import sys
@@ -32,7 +32,7 @@ def _done_with_plan(self):
         # desc "B.. C.. k.. d.. T..": the plan is a function of the shape
         f = {s[0]: int(s[1:]) for s in self.desc.split()}
         pl = ops.resblock_pair_plan(f["C"], f["T"], f["k"], f["d"], batch=f["B"])
-        plans[len(ops.PROFILE) - 1] = f"{pl['variant']} rows {pl['M2']}/{pl['TT']} na{pl['na']} nb{pl['nb']} ns{pl['ns']}"
+        plans[len(ops.PROFILE) - 1] = f"rows {pl['M2']}/{pl['TT']} na{pl['na']} nb{pl['nb']} ns{pl['ns']}"
 
 
 ops._Prof.done = _done_with_plan
