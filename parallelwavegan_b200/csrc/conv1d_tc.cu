@@ -36,6 +36,8 @@ constexpr int W_CONS0 = NPROD / 32, W_TMA = (NPROD + NCONS) / 32, W_LDA = W_TMA 
 constexpr int TC_THREADS = NPROD + NCONS + 64;
 constexpr int NS_MAX = 4;  // raw activation stages
 constexpr size_t TC_SMEM_STAGED = 227 * 1024;  // H100 opt-in limit of dynamic shared memory per block: staged-epilogue plans
+// named barrier 1 of the NPROD producer threads (ids 2 and 3 are the consumer warpgroups', wg_barrier)
+__device__ __forceinline__ void producer_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(NPROD) : "memory"); }
 
 struct TcK {
   int B, Cin, Cout, T_in, T_out, K, D, padL, pad_mode;
@@ -66,12 +68,8 @@ struct TcK {
   int staged;            // plain epilogue through a shared-memory tile per consumer warpgroup (tc_plan)
 };
 
-// Staged epilogue tile of one consumer warpgroup: fp32 [col][64 * MT + 4].  Rows of a channel are contiguous, so one
-// bulk copy moves a channel's residual in and its outputs out; the 16-byte pad keeps the rows 16-byte aligned and puts
-// the 8 rows x 4 columns of an accumulator-fragment write in 32 distinct banks.
-__host__ __device__ constexpr int stage_ld(int mt) { return 64 * mt + 4; }
-// Tile shapes compiled with the staged epilogue: at MT = 2 and more than 32 columns it made ptxas spill, and its tiles
-// would not fit beside the pipeline there anyway.
+// Staged epilogue: one tile (fp32 [col][stage_ld(MT)], tc_common.cuh) per consumer warpgroup.  Tile shapes compiled with
+// it: at MT = 2 and more than 32 columns it made ptxas spill, and its tiles would not fit beside the pipeline there anyway.
 __host__ __device__ constexpr bool stage_shape(int mt, int cout) { return mt == 1 || cout <= 32; }
 
 // ------------------------------------------------------------------ weight packing
@@ -174,47 +172,55 @@ __device__ __forceinline__ const float* main_src(const TcK& p, const float* x, c
   return x + (long long)b * p.xbs + (long long)ch * p.T_in + goff;
 }
 
+// Batch item and first time step of work item `tile` (TT time steps per tile; the items of the nco column chunks of a
+// launch follow one another).
+__device__ __forceinline__ void tile_origin(const TcK& p, int tile, int TT, int& b, int& t0) {
+  const int tr = p.nco > 1 ? tile % (p.B * p.tiles_per_seq) : tile;  // tile within its column chunk
+  b = tr / p.tiles_per_seq;
+  t0 = (tr - b * p.tiles_per_seq) * TT;
+}
+
+// Input sample of operand row r of a main chunk in the tile starting at t0: the row's window and tap (win_mode) or its
+// place in the contiguous halo tile, then the padding policy.  ok = false: a zero-padding row.
+__device__ __forceinline__ long long src_sample(const TcK& p, int t0, int TT, int r, bool& ok) {
+  long long ts;
+  if (p.win_mode) {
+    const int k = r / TT;
+    ts = (long long)t0 - p.padL + (long long)k * p.D + (r - k * TT);
+  } else {
+    ts = (long long)t0 - p.padL + r;
+  }
+  ok = true;
+  if (ts < 0 || ts >= p.T_in) {
+    if (p.pad_mode == PWGB_PAD_ZERO) {
+      ok = false;
+    } else if (p.pad_mode == PWGB_PAD_REFLECT) {
+      ts = ts < 0 ? -ts : 2LL * (p.T_in - 1) - ts;
+      ok = ts >= 0 && ts < p.T_in;
+    } else {
+      ts = ts < 0 ? 0 : p.T_in - 1;
+    }
+  }
+  return ts;
+}
+
 // stage one activation chunk (KC channels x R rows) into the operand layout
 __device__ __forceinline__ void fill_main_chunk(const TcK& p, const float* __restrict__ xc, int t0, int TT,
                                                 unsigned char* dst, int tid) {
-  auto src_of = [&](int r, bool& ok) -> long long {
-    long long ts;
-    if (p.win_mode) {
-      const int k = r / TT;
-      ts = (long long)t0 - p.padL + (long long)k * p.D + (r - k * TT);
-    } else {
-      ts = (long long)t0 - p.padL + r;
-    }
-    ok = true;
-    if (ts < 0 || ts >= p.T_in) {
-      if (p.pad_mode == PWGB_PAD_ZERO) {
-        ok = false;
-      } else if (p.pad_mode == PWGB_PAD_REFLECT) {
-        ts = ts < 0 ? -ts : 2LL * (p.T_in - 1) - ts;
-        ok = ts >= 0 && ts < p.T_in;
-      } else {
-        ts = ts < 0 ? 0 : p.T_in - 1;
-      }
-    }
-    return ts;
-  };
   auto store_row = [&](const float (&v)[KC], int r) {
 #pragma unroll
     for (int g = 0; g < KC / 8; ++g) {
       float u[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) u[j] = v[g * 8 + j];
-      uint4 hi, lo;
-      split8(u, hi, lo);
-      *reinterpret_cast<uint4*>(dst + ((size_t)g * p.R + r) * 16) = hi;
-      *reinterpret_cast<uint4*>(dst + ((size_t)(KC / 8 + g) * p.R + r) * 16) = lo;
+      store_split8(dst, p.R, r, g, u);
     }
   };
   if (p.pre_gate) {
     const float* xg = xc + (long long)p.Cin * p.T_in;
     for (int r = tid; r < p.R; r += NPROD) {
       bool ok;
-      const long long ts = src_of(r, ok);
+      const long long ts = src_sample(p, t0, TT, r, ok);
       float v[KC], sg[KC];
 #pragma unroll
       for (int j = 0; j < KC; ++j) {
@@ -229,7 +235,7 @@ __device__ __forceinline__ void fill_main_chunk(const TcK& p, const float* __res
   }
   for (int r = tid; r < p.R; r += NPROD) {
     bool ok;
-    const long long ts = src_of(r, ok);
+    const long long ts = src_sample(p, t0, TT, r, ok);
     float v[KC];
 #pragma unroll
     for (int j = 0; j < KC; ++j) v[j] = ok ? __ldg(xc + (long long)j * p.T_in + ts) : 0.f;
@@ -305,7 +311,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     // outside [0, T) are never copied and are masked here (zero padding).
     int s = 0, sph = 0, buf = 0, aph = 0;
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      const int tr = p.nco > 1 ? tile % pct : tile;  // tile within its column chunk
+      // tile_origin written out: through the helper here, ptxas spilled conv1d_tc_kernel<2, 4> at its 96 registers
+      const int tr = p.nco > 1 ? tile % pct : tile;
       const int b = tr / p.tiles_per_seq;
       const int t0 = (tr - b * p.tiles_per_seq) * TT;
       const int ts_first = t0 - p.padL;
@@ -313,28 +320,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       for (int c = 0; c < nc_total; ++c) {
         mbar_wait(RAW_FULL(s), sph);
         mbar_wait(A_EMPTY(buf), aph ^ 1);
-        unsigned char* dst = a_buf + (size_t)buf * p.a_bytes;
         const float* raw = reinterpret_cast<const float*>(raw_buf + (size_t)s * p.raw_bytes);
         const bool main_chunk = c < p.nchunks;
-        const int rows = main_chunk ? p.R : TT;
-        const int sh = main_chunk ? shift : 0;
-        const int tbase = main_chunk ? ts_first : t0;
-        const unsigned tlim = (unsigned)(main_chunk ? p.T_in : p.T_out);
-        const float slope = main_chunk ? p.pre_slope : 1.f;
-        for (int r = tid; r < rows; r += NPROD) {
-          const bool ok = (unsigned)(tbase + r) < tlim;
-          const float* rr = raw + r + sh;
-#pragma unroll
-          for (int g = 0; g < KC / 8; ++g) {
-            float u[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) u[j] = ok ? lrelu(rr[(g * 8 + j) * p.R4], slope) : 0.f;
-            uint4 hi, lo;
-            split8(u, hi, lo);
-            *reinterpret_cast<uint4*>(dst + ((size_t)g * p.R + r) * 16) = hi;
-            *reinterpret_cast<uint4*>(dst + ((size_t)(KC / 8 + g) * p.R + r) * 16) = lo;
-          }
-        }
+        convert_raw_stage<NPROD, true>(a_buf + (size_t)buf * p.a_bytes, p.R, raw, main_chunk ? shift : 0, p.R4,
+                                       main_chunk ? p.R : TT, main_chunk ? ts_first : t0,
+                                       (unsigned)(main_chunk ? p.T_in : p.T_out), main_chunk ? p.pre_slope : 1.f, tid);
         fence_proxy_async();
         mbar_arrive(A_FULL(buf));
         mbar_arrive(RAW_EMPTY(s));
@@ -352,31 +342,14 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     auto issue = [&](int q) {
       const int tile = blockIdx.x + (q / nc_total) * gridDim.x;
       const int c = q % nc_total;
-      const int tr = p.nco > 1 ? tile % pct : tile;  // tile within its column chunk
-      const int b = tr / p.tiles_per_seq;
-      const int t0 = (tr - b * p.tiles_per_seq) * TT;
+      int b, t0;
+      tile_origin(p, tile, TT, b, t0);
       const unsigned raw = smem_u32(raw_buf + (size_t)(q % p.ns) * p.raw_bytes);
       if (c < p.nchunks) {
         const float* xc = main_src(p, x, x2, b, c, MC ? (long long)((tile / pct) / p.cpg) * p.xgs : 0);
         for (int r = tid; r < p.R; r += NPROD) {
-          long long ts;
-          if (p.win_mode) {
-            const int k = r / TT;
-            ts = (long long)t0 - p.padL + (long long)k * p.D + (r - k * TT);
-          } else {
-            ts = (long long)t0 - p.padL + r;
-          }
-          bool ok = true;
-          if (ts < 0 || ts >= p.T_in) {
-            if (p.pad_mode == PWGB_PAD_ZERO) {
-              ok = false;
-            } else if (p.pad_mode == PWGB_PAD_REFLECT) {
-              ts = ts < 0 ? -ts : 2LL * (p.T_in - 1) - ts;
-              ok = ts >= 0 && ts < p.T_in;
-            } else {
-              ts = ts < 0 ? 0 : p.T_in - 1;
-            }
-          }
+          bool ok;
+          const long long ts = src_sample(p, t0, TT, r, ok);
           const float* src = ok ? xc + ts : xc;
           const unsigned nbytes = ok ? 4u : 0u;
           unsigned dq = raw + (unsigned)r * 4u;
@@ -411,22 +384,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       const int c = q % nc_total;
       const int buf = q % p.na;
       mbar_wait(A_EMPTY(buf), ((q / p.na) & 1) ^ 1);
-      unsigned char* dst = a_buf + (size_t)buf * p.a_bytes;
       const float* raw = reinterpret_cast<const float*>(raw_buf + (size_t)(q % p.ns) * p.raw_bytes);
-      const int rows = c < p.nchunks ? p.R : TT;
-      const float slope = c < p.nchunks ? p.pre_slope : 1.f;
-      for (int r = tid; r < rows; r += NPROD) {
-#pragma unroll
-        for (int g = 0; g < KC / 8; ++g) {
-          float u[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) u[j] = lrelu(raw[(g * 8 + j) * p.R + r], slope);
-          uint4 hi, lo;
-          split8(u, hi, lo);
-          *reinterpret_cast<uint4*>(dst + ((size_t)g * p.R + r) * 16) = hi;
-          *reinterpret_cast<uint4*>(dst + ((size_t)(KC / 8 + g) * p.R + r) * 16) = lo;
-        }
-      }
+      // the padding is in the stage (cp.async zero fill, reflected / replicated samples)
+      convert_raw_stage<NPROD, false>(a_buf + (size_t)buf * p.a_bytes, p.R, raw, 0, p.R, c < p.nchunks ? p.R : TT, 0, 0u,
+                                      c < p.nchunks ? p.pre_slope : 1.f, tid);
       fence_proxy_async();
       mbar_arrive(A_FULL(buf));
       producer_barrier();  // raw[q % ns] may be overwritten by issue(q + 2)
@@ -436,9 +397,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     // (one source only: conv1d_tc_chunk gives two-source inputs raw-staged plans)
     unsigned ca = 0;
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      const int tr = p.nco > 1 ? tile % pct : tile;  // tile within its column chunk
-      const int b = tr / p.tiles_per_seq;
-      const int t0 = (tr - b * p.tiles_per_seq) * TT;
+      int b, t0;
+      tile_origin(p, tile, TT, b, t0);
       const float* xb = x + (long long)b * p.xbs + (MC ? (long long)((tile / pct) / p.cpg) * p.xgs : 0);
       for (int c = 0; c < nc_total; ++c, ++ca) {
         const int buf = ca % p.na;
@@ -457,10 +417,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
               float u[8];
 #pragma unroll
               for (int j = 0; j < 8; ++j) u[j] = ok ? __ldg(xc + (long long)(g * 8 + j) * p.T_out + ts) : 0.f;
-              uint4 hi, lo;
-              split8(u, hi, lo);
-              *reinterpret_cast<uint4*>(dst + ((size_t)g * p.R + r) * 16) = hi;
-              *reinterpret_cast<uint4*>(dst + ((size_t)(KC / 8 + g) * p.R + r) * 16) = lo;
+              store_split8(dst, p.R, r, g, u);
             }
           }
         }
@@ -476,8 +433,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     // of the MMAs into each accumulator is the issue order, so the overlap does not change the result.
     const int wg = (warp - W_CONS0) >> 2, wq = warp & 3;
     constexpr int NACC = 8 * NB16;  // fp32 accumulators per thread and 64-row block
-    const unsigned lbo_a = (unsigned)p.R * 16u, lbo_b = NB16 * 256u;
-    const unsigned a_sub = (unsigned)(KC / 8) * p.R, b_sub = (KC / 8) * NB16 * 16u;  // hi -> lo image (16-byte units)
+    const unsigned lbo_a = (unsigned)p.R * 16u, a_sub = (unsigned)(KC / 8) * p.R;  // a_sub: hi -> lo image (16-byte units)
     // Staged epilogue: thread wt of the warpgroup owns channel row wt of the warpgroup's tile.  It issues that row's
     // residual load and its store (or add), so its own bulk-group wait is the only guard the row needs before reuse.
     const int wt = tid - NPROD - wg * 128;
@@ -486,9 +442,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     int buf = 0, aph = 0, s = 0, bph = 0;
     // (batch, first time step, first channel) of a tile
     auto tile_pos = [&](int tile, int& b, int& t0, int& co_base) {
-      const int tr = p.nco > 1 ? tile % pct : tile;  // tile within its column chunk
-      b = tr / p.tiles_per_seq;
-      t0 = (tr - b * p.tiles_per_seq) * TT;
+      tile_origin(p, tile, TT, b, t0);
       co_base = p.co_off + (p.nco > 1 ? (tile / pct) * p.Cout : 0);
     };
     // channel row wt of this warpgroup's rows [tw0, tw0 + MT * 64) of a tile: its first element within the batch item
@@ -506,13 +460,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       unsigned row_bytes;
       tile_pos(tile, b, t0, co_base);
       const long long row_off = row_pos(t0, co_base, row_bytes);
-      bulk_wait_read();
-      if (row_bytes) {
-        mbar_expect_tx(RES_FULL(wg), row_bytes);
-        bulk_g2s(smem_u32(stg + wt * SLD), res + (long long)b * p.rbs + row_off, row_bytes, RES_FULL(wg));
-      } else {
-        mbar_arrive(RES_FULL(wg));
-      }
+      stage_load_row(smem_u32(stg + wt * SLD), res + (long long)b * p.rbs + row_off, row_bytes, RES_FULL(wg));
     };
     if (row_owner && res && (int)blockIdx.x < p.total_tiles) load_res(blockIdx.x);
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
@@ -527,23 +475,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         for (int k = 0; k < ntaps; ++k) {
           mbar_wait_trap(B_FULL(s), bph);
           __syncwarp();
-          const unsigned b_addr = smem_u32(b_buf + (size_t)s * p.b_bytes);
           const int tap_row = c < p.nchunks ? (p.win_mode ? k * TT : k * p.D) : 0;
-          wg_fence();
-#pragma unroll
-          for (int ks = 0; ks < KC / 16; ++ks) {
-            const unsigned long long bh = gmma_desc(b_addr + (unsigned)(2 * ks) * lbo_b, lbo_b, 128);
-            const unsigned long long ah0 =
-                gmma_desc(a_addr + ((unsigned)(2 * ks) * p.R + (unsigned)(tap_row + wg * MT * 64)) * 16u, lbo_a, 128);
-#pragma unroll
-            for (int mb = 0; mb < MT; ++mb) {
-              const unsigned long long ah = ah0 + 64 * mb;  // next 64 rows: 64 x 16 B
-              wgmma_n<0, 0, NB16>(acc + mb * NACC, ah, bh, 16);
-              wgmma_n<0, 0, NB16>(acc + mb * NACC, ah + a_sub, bh, 16);
-              wgmma_n<0, 0, NB16>(acc + mb * NACC, ah, bh + b_sub, 16);
-            }
-          }
-          wg_commit();
+          mma_stage<MT, NB16>(acc, a_addr, lbo_a, a_sub, tap_row + wg * MT * 64, smem_u32(b_buf + (size_t)s * p.b_bytes));
           wg_wait<1>();  // the previous group has retired: its stage and, at a chunk boundary, its A buffer are free
           __syncwarp();
           if (lane == 0) {
@@ -611,14 +544,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         wg_barrier(wg);
         unsigned row_bytes;
         const long long row_off = row_pos(t0, co_base, row_bytes);
-        if (row_owner && row_bytes) {
-          float* q = y + (long long)b * p.ybs + row_off;
-          if (p.accumulate)
-            bulk_s2g_add(q, smem_u32(stg + wt * SLD), row_bytes);
-          else
-            bulk_s2g(q, smem_u32(stg + wt * SLD), row_bytes);
-          bulk_commit();
-        }
+        if (row_owner) stage_store_row(y + (long long)b * p.ybs + row_off, smem_u32(stg + wt * SLD), row_bytes, p.accumulate);
         if (row_owner && res && tile + (int)gridDim.x < p.total_tiles) load_res(tile + gridDim.x);
       }
     }
@@ -645,9 +571,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     if (p.tma_act) {
       int s = 0, ph = 0;
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        const int tr = p.nco > 1 ? tile % pct : tile;  // tile within its column chunk
-      const int b = tr / p.tiles_per_seq;
-        const int t0 = (tr - b * p.tiles_per_seq) * TT;
+        int b, t0;
+        tile_origin(p, tile, TT, b, t0);
         const int ts0 = (t0 - p.padL) & ~3;
         for (int c = 0; c < nc_total; ++c) {
           mbar_wait(RAW_EMPTY(s), ph ^ 1);
@@ -666,15 +591,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
             dst_off = 0;
             src = x2 + ((long long)b * p.C2 + (long long)(c - p.nchunks) * KC) * p.T_out;
           }
-          const int nbytes = (end - start) * 4;
-          if (nbytes > 0) {
-            if (lane == 0) mbar_expect_tx(RAW_FULL(s), (unsigned)nbytes * KC);
-            __syncwarp();
-            bulk_g2s(smem_u32(raw_buf + (size_t)s * p.raw_bytes) + (unsigned)(lane * p.R4 + dst_off) * 4u,
-                     src + (long long)lane * rowstride + start, (unsigned)nbytes, RAW_FULL(s));
-          } else if (lane == 0) {
-            mbar_arrive(RAW_FULL(s));
-          }
+          load_raw_stage(smem_u32(raw_buf + (size_t)s * p.raw_bytes), p.R4, src, rowstride, start, end, dst_off, RAW_FULL(s),
+                         lane);
           __syncwarp();
           if (++s == p.ns) { s = 0; ph ^= 1; }
         }
@@ -826,17 +744,17 @@ static int tc_plan(const pwgb_conv1d_desc* d, TcK& p, size_t& smem_bytes, int au
 
 using TcKernel = void (*)(const TcK, const float*, const float*, const uint4*, const float*, const float*, float*, float*);
 
-// Every tile shape tc_plan produces: MT = 1 at any width of 16 .. TC_NMAX columns, MT = 2 up to TC_NMAX / 2.
+// Every tile shape tc_plan produces: MT = 1 at any width of 16 .. TC_NMAX columns (the first 8), MT = 2 up to
+// TC_NMAX / 2 (the last 4).
+static const TcKernel tc_kernels[12] = {conv1d_tc_kernel<1, 1>, conv1d_tc_kernel<1, 2>, conv1d_tc_kernel<1, 3>,
+                                        conv1d_tc_kernel<1, 4>, conv1d_tc_kernel<1, 5>, conv1d_tc_kernel<1, 6>,
+                                        conv1d_tc_kernel<1, 7>, conv1d_tc_kernel<1, 8>, conv1d_tc_kernel<2, 1>,
+                                        conv1d_tc_kernel<2, 2>, conv1d_tc_kernel<2, 3>, conv1d_tc_kernel<2, 4>};
 static TcKernel tc_kernel_for(int mt, int cout) {
-  static const TcKernel mt1[8] = {conv1d_tc_kernel<1, 1>, conv1d_tc_kernel<1, 2>, conv1d_tc_kernel<1, 3>,
-                                  conv1d_tc_kernel<1, 4>, conv1d_tc_kernel<1, 5>, conv1d_tc_kernel<1, 6>,
-                                  conv1d_tc_kernel<1, 7>, conv1d_tc_kernel<1, 8>};
-  static const TcKernel mt2[4] = {conv1d_tc_kernel<2, 1>, conv1d_tc_kernel<2, 2>, conv1d_tc_kernel<2, 3>,
-                                  conv1d_tc_kernel<2, 4>};
   if (cout % 16 != 0) return nullptr;
   const int nb16 = cout / 16;
-  if (mt == 1 && nb16 >= 1 && nb16 <= 8) return mt1[nb16 - 1];
-  if (mt == 2 && nb16 >= 1 && nb16 <= 4) return mt2[nb16 - 1];
+  if (mt == 1 && nb16 >= 1 && nb16 <= 8) return tc_kernels[nb16 - 1];
+  if (mt == 2 && nb16 >= 1 && nb16 <= 4) return tc_kernels[8 + nb16 - 1];
   return nullptr;
 }
 
@@ -849,25 +767,9 @@ static int tc_launch(TcK& p, size_t bytes, const float* x, const void* packed_w,
     set_error("conv1d_tc: no kernel instantiation for MT = %d, Cout = %d", p.MT, p.Cout);
     return PWGB_UNSUPPORTED;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    for (int mt = 1; mt <= 2; ++mt)
-      for (int cout = 16; cout <= TC_NMAX / mt; cout += 16) {
-        cudaError_t e = cudaFuncSetAttribute(tc_kernel_for(mt, cout), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM_STAGED);
-        if (e != cudaSuccess) {
-          set_error("conv1d_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-          return PWGB_CUDA_ERROR;
-        }
-      }
-    attr_set = true;
-  }
-  static int num_sms = 0;
-  if (!num_sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (num_sms <= 0) num_sms = 132;
-  }
+  static bool smem_set = false;
+  if (const int rc = smem_opt_in(smem_set, tc_kernels, (int)TC_SMEM_STAGED, "conv1d_tc")) return rc;
+  const int num_sms = tc_num_sms();
   if ((long long)p.B * p.tiles_per_seq > 0x7fffffffLL) {
     set_error("conv1d_tc: too many tiles");
     return PWGB_UNSUPPORTED;
@@ -1425,16 +1327,11 @@ extern "C" int pwgb_conv1d_wgrad_tc(const pwgb_conv1d_desc* d, const float* x, c
     return PWGB_OK;
   }
   const size_t smem = 2 * ((size_t)2 * 16 * WT_TK * 16 + (size_t)2 * (p.nc / 8) * p.RX * 16);
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(wgrad_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-    if (e != cudaSuccess) {
-      set_error("conv1d_wgrad_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-      return PWGB_CUDA_ERROR;
-    }
-    attr_set = true;
-  }
+  using WtKernel = void (*)(const WtK, const float*, const float*, float*);
+  static bool smem_set = false;
+  if (const int rc = smem_opt_in(smem_set, {WtKernel(wgrad_tc_kernel<32>), WtKernel(wgrad_tc_kernel<64>)}, 220 * 1024,
+                                 "conv1d_wgrad_tc"))
+    return rc;
   g_wt_last = WtPlanInfo{p.nc, p.tg, p.ntg, p.nsplit};
   dim3 grid(p.G * ceil_div(p.Cout_g, 128), (p.Cin_g / p.nc) * p.ntg, p.nsplit);
   if (p.nc == 64)

@@ -6,15 +6,17 @@
 // The intermediate h never leaves the SM: conv1's accumulators are written, as lrelu(h) split into bf16 hi/lo, straight
 // into the K-major operand image that conv2's wgmma reads.  Everything else is the stride-1 conv of conv1d_tc.cu: the
 // same weight images (pwgb_conv1d_tc_pack_weight), bf16x3 products, and MMA order into every accumulator (32-channel
-// chunk, tap, k16 step, hi*hi, lo*hi, hi*lo), so the result is bit-identical to the two conv1d_tc launches.
+// chunk, tap, k16 step, hi*hi, lo*hi, hi*lo), so the result is bit-identical to the two conv1d_tc launches.  The pieces
+// of that pipeline (raw-row loader, raw stage conversion, MMA of a weight stage, staged-epilogue row load and store) are
+// the ones conv1d_tc_kernel calls, from tc_common.cuh.
 //
 // Tiling: a tile produces M2 output rows [t0, t0 + M2).  Conv2 needs h rows [t0 - p2, t0 + M2 + p2), p2 = (k-1)/2;
 // conv1 computes the TT conv rows [t0 - p2, t0 - p2 + TT) from R1 = TT + (k-1) d input rows, so M2 = TT - (k-1)
 // rounded down to a multiple of 4 (16-byte output rows).  Halo rows of h are recomputed by the neighbouring tile.  Conv2
 // also runs TT rows per tile; rows >= M2 read beyond the computed h rows and are dropped.
 //
-// One kernel, rb_pair_split_kernel, one persistent CTA per SM, with the producers and loaders of conv1d_tc_kernel with
-// TMA-staged activations: producer warps convert landed raw fp32 rows of x (pre-activation, padding mask, hi/lo split)
+// One kernel, rb_pair_split_kernel, one persistent CTA per SM, with the warp roles of conv1d_tc_kernel with TMA-staged
+// activations: producer warps convert landed raw fp32 rows of x (pre-activation, padding mask, hi/lo split)
 // into conv1's operand image, one warp loads weight stages and one raw activation rows, both by cp.async.bulk.  The two
 // consumer warpgroups are split by conv: warpgroup 0 runs conv1 of every tile and writes the h image, warpgroup 1 runs
 // conv2 on it and the staged epilogue, so that one warpgroup's drain, h write or epilogue overlaps the other's MMAs.
@@ -34,7 +36,6 @@ namespace {
 constexpr int RB_NPROD = 192;
 constexpr int RB_W_PROD0 = 8, RB_W_TMA = RB_W_PROD0 + RB_NPROD / 32, RB_W_LDA = RB_W_TMA + 1;
 constexpr int RB_THREADS = 32 * (RB_W_LDA + 1);
-__host__ __device__ constexpr int rb_sld(int mt) { return 64 * mt + 4; }  // staged epilogue row pitch, as in conv1d_tc.cu
 constexpr size_t RB_SMEM = 227 * 1024;      // H100 opt-in limit of dynamic shared memory per block
 constexpr int RB_MIN_STAGES = 4;            // weight stages a plan must keep per ring
 
@@ -64,22 +65,9 @@ __device__ __forceinline__ void rb_convert_x(const RbK& p, unsigned char* a_buf,
     for (int c = 0; c < NCH; ++c) {
       mbar_wait(raw_full + 8u * s, sph);
       mbar_wait(a_empty + 8u * buf, aph ^ 1);
-      unsigned char* dst = a_buf + (size_t)buf * p.a_bytes;
       const float* raw = reinterpret_cast<const float*>(raw_buf + (size_t)s * p.raw_bytes);
-      for (int r = tid; r < p.R1; r += RB_NPROD) {
-        const bool ok = (unsigned)(ts_first + r) < (unsigned)p.T;
-        const float* rr = raw + r + shift;
-#pragma unroll
-        for (int g = 0; g < KC / 8; ++g) {
-          float u[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) u[j] = ok ? lrelu(rr[(g * 8 + j) * p.R4], p.slope) : 0.f;
-          uint4 hi, lo;
-          split8(u, hi, lo);
-          *reinterpret_cast<uint4*>(dst + ((size_t)g * p.R1 + r) * 16) = hi;
-          *reinterpret_cast<uint4*>(dst + ((size_t)(KC / 8 + g) * p.R1 + r) * 16) = lo;
-        }
-      }
+      convert_raw_stage<RB_NPROD, true>(a_buf + (size_t)buf * p.a_bytes, p.R1, raw, shift, p.R4, p.R1, ts_first,
+                                        (unsigned)p.T, p.slope, tid);
       fence_proxy_async();
       mbar_arrive(a_full + 8u * buf);
       mbar_arrive(raw_empty + 8u * s);
@@ -101,43 +89,14 @@ __device__ __forceinline__ void rb_load_raw(const RbK& p, const float* __restric
     const int ts0 = (t0 - p.p2 - p.p1) & ~3;
     const int start = ts0 < 0 ? 0 : ts0;
     const int end = ts0 + p.R4 < p.T ? ts0 + p.R4 : p.T;
-    const int nbytes = (end - start) * 4;
     for (int c = 0; c < NCH; ++c) {
       mbar_wait(raw_empty + 8u * s, ph ^ 1);
-      if (nbytes > 0) {
-        if (lane == 0) mbar_expect_tx(raw_full + 8u * s, (unsigned)nbytes * KC);
-        __syncwarp();
-        bulk_g2s(smem_u32(raw_buf + (size_t)s * p.raw_bytes) + (unsigned)(lane * p.R4 + start - ts0) * 4u,
-                 x + ((long long)b * C + c * KC + lane) * p.T + start, (unsigned)nbytes, raw_full + 8u * s);
-      } else if (lane == 0) {
-        mbar_arrive(raw_full + 8u * s);
-      }
+      load_raw_stage(smem_u32(raw_buf + (size_t)s * p.raw_bytes), p.R4, x + ((long long)b * C + c * KC) * p.T, p.T, start, end,
+                     start - ts0, raw_full + 8u * s, lane);
       __syncwarp();
       if (++s == p.ns) { s = 0; ph ^= 1; }
     }
   }
-}
-
-// One weight stage of wgmma on the operand image at `a_img` (rows `row0` ..): per k16 step and 64-row block, the three
-// bf16x3 products.  One commit group per call.
-template <int MT, int NB16>
-__device__ __forceinline__ void rb_mma_stage(float* acc, unsigned a_img, unsigned lbo, unsigned sub, int row0, unsigned b_addr) {
-  constexpr int NACC = 8 * NB16;
-  constexpr unsigned lbo_b = NB16 * 256u, b_sub = (KC / 8) * NB16 * 16u;
-  wg_fence();
-#pragma unroll
-  for (int ks = 0; ks < KC / 16; ++ks) {
-    const unsigned long long bh = gmma_desc(b_addr + (unsigned)(2 * ks) * lbo_b, lbo_b, 128);
-    const unsigned long long ah0 = gmma_desc(a_img + ((unsigned)(2 * ks) * (lbo / 16u) + (unsigned)row0) * 16u, lbo, 128);
-#pragma unroll
-    for (int mb = 0; mb < MT; ++mb) {
-      const unsigned long long ah = ah0 + 64 * mb;  // next 64 rows: 64 x 16 B
-      wgmma_n<0, 0, NB16>(acc + mb * NACC, ah, bh, 16);
-      wgmma_n<0, 0, NB16>(acc + mb * NACC, ah + sub, bh, 16);
-      wgmma_n<0, 0, NB16>(acc + mb * NACC, ah, bh + b_sub, 16);
-    }
-  }
-  wg_commit();
 }
 
 // h = lrelu(acc + b1) of the warpgroup's conv rows [row_base, row_base + 64 MT) (time th0 + r for fragment row r) as
@@ -162,11 +121,11 @@ __device__ __forceinline__ void rb_write_h(const float* acc, unsigned char* h_bu
   }
 }
 
-// staged epilogue in place over the residual rows of the tile `stg` ([channel][rb_sld(MT)]): v = (a + b2 + x) * out_scale
+// staged epilogue in place over the residual rows of the tile `stg` ([channel][stage_ld(MT)]): v = (a + b2 + x) * out_scale
 template <int MT, int NB16>
 __device__ __forceinline__ void rb_stage_result(const float* acc, float* stg, const float* bias2, float out_scale, int lane,
                                                 int wq) {
-  constexpr int NACC = 8 * NB16, SLD = rb_sld(MT);
+  constexpr int NACC = 8 * NB16, SLD = stage_ld(MT);
 #pragma unroll
   for (int e = 0; e < MT * NACC; ++e) {
     const int i = e % NACC;
@@ -189,7 +148,7 @@ __global__ void __launch_bounds__(RB_THREADS, 1)
                          const float* __restrict__ b1, const unsigned char* __restrict__ w2, const float* __restrict__ b2,
                          float* __restrict__ y) {
   extern __shared__ __align__(128) unsigned char smem[];
-  constexpr int C = 16 * NB16, NCH = C / KC, NACC = 8 * NB16, SLD = rb_sld(MT);
+  constexpr int C = 16 * NB16, NCH = C / KC, NACC = 8 * NB16, SLD = stage_ld(MT);
   const int nr = p.nb / 2;  // stages per weight ring
   // layout: A[na] | B1[nr] | B2[nr] | raw staging[ns] | h image[NCH chunks] | epilogue tile | barriers | bias1 | bias2
   unsigned char* a_buf = smem;
@@ -266,7 +225,7 @@ __global__ void __launch_bounds__(RB_THREADS, 1)
         for (int k = 0; k < p.K; ++k) {
           mbar_wait_trap(B1_FULL + 8u * s, bph);
           __syncwarp();
-          rb_mma_stage<MT, NB16>(acc, a_addr, lbo_a, a_sub, k * p.D, smem_u32(b1_buf + (size_t)s * p.b_bytes));
+          mma_stage<MT, NB16>(acc, a_addr, lbo_a, a_sub, k * p.D, smem_u32(b1_buf + (size_t)s * p.b_bytes));
           wg_wait<1>();  // the previous group has retired: its stage and, at a chunk boundary, its A buffer are free
           release();
           held_s = s;
@@ -303,13 +262,7 @@ __global__ void __launch_bounds__(RB_THREADS, 1)
     auto load_res = [&](int tile) {
       unsigned row_bytes;
       const long long off = row_pos(tile, row_bytes);
-      bulk_wait_read();  // the previous store has read the row
-      if (row_bytes) {
-        mbar_expect_tx(RES_FULL, row_bytes);
-        bulk_g2s(smem_u32(stg + wt * SLD), x + off, row_bytes, RES_FULL);
-      } else {
-        mbar_arrive(RES_FULL);
-      }
+      stage_load_row(smem_u32(stg + wt * SLD), x + off, row_bytes, RES_FULL);
     };
     if (row_owner && (int)blockIdx.x < p.total_tiles) load_res(blockIdx.x);
     int s = 0, bph = 0, n = 0;
@@ -328,7 +281,7 @@ __global__ void __launch_bounds__(RB_THREADS, 1)
         for (int k = 0; k < p.K; ++k) {
           mbar_wait_trap(B2_FULL + 8u * s, bph);
           __syncwarp();
-          rb_mma_stage<MT, NB16>(acc, h_addr, lbo_h, h_sub, k, smem_u32(b2_buf + (size_t)s * p.b_bytes));
+          mma_stage<MT, NB16>(acc, h_addr, lbo_h, h_sub, k, smem_u32(b2_buf + (size_t)s * p.b_bytes));
           wg_wait<1>();
           release();
           held_s = s;
@@ -346,13 +299,7 @@ __global__ void __launch_bounds__(RB_THREADS, 1)
       if (row_owner) {
         unsigned row_bytes;
         const long long off = row_pos(tile, row_bytes);
-        if (row_bytes) {
-          if (p.accumulate)
-            bulk_s2g_add(y + off, smem_u32(stg + wt * SLD), row_bytes);
-          else
-            bulk_s2g(y + off, smem_u32(stg + wt * SLD), row_bytes);
-          bulk_commit();
-        }
+        stage_store_row(y + off, smem_u32(stg + wt * SLD), row_bytes, p.accumulate);
         if (tile + (int)gridDim.x < p.total_tiles) load_res(tile + gridDim.x);
       }
     }
@@ -417,7 +364,7 @@ int rb_fit(const pwgb_resblock_desc* d, RbK& p, size_t& smem_bytes, int mt) {
   p.a_bytes = 2 * (KC / 8) * p.R1 * 16;
   p.raw_bytes = KC * p.R4 * 4;
   p.h_bytes = 2 * (KC / 8) * p.Rh * 16;
-  const size_t epi = (size_t)d->channels * rb_sld(mt) * 4;
+  const size_t epi = (size_t)d->channels * stage_ld(mt) * 4;
   const size_t fixed = (size_t)p.nchunks * p.h_bytes + epi + 2 * (size_t)d->channels * 4 + 1024;
   static const int bufs[3][2] = {{2, 3}, {2, 2}, {1, 2}};  // (na, ns)
   for (const auto& nn : bufs) {
@@ -497,27 +444,13 @@ extern "C" int pwgb_resblock_pair_forward(const pwgb_resblock_desc* d, const flo
   PWGB_UNSUPPORTED_IF((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(y) & 15),
                       "resblock_pair: x and y must be 16-byte aligned");
   if (p.B == 0) return PWGB_OK;
-  static bool attr_set = false;
-  if (!attr_set) {
-    int mt;
-    for (const RbKernel k : {rb_split_kernel_for(32, &mt), rb_split_kernel_for(64, &mt)}) {
-      cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RB_SMEM);
-      if (e != cudaSuccess) {
-        set_error("resblock_pair: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-        return PWGB_CUDA_ERROR;
-      }
-    }
-    attr_set = true;
-  }
-  static int num_sms = 0;
-  if (!num_sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (num_sms <= 0) num_sms = 132;
-  }
-  const int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
   int mt;
+  static bool smem_set = false;
+  if (const int rc = smem_opt_in(smem_set, {rb_split_kernel_for(32, &mt), rb_split_kernel_for(64, &mt)}, (int)RB_SMEM,
+                                 "resblock_pair"))
+    return rc;
+  const int num_sms = tc_num_sms();
+  const int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
   const RbKernel k = rb_split_kernel_for(p.C, &mt);
   k<<<(unsigned)grid, RB_THREADS, bytes, (cudaStream_t)stream>>>(p, x, (const unsigned char*)w1_packed, b1,
                                                                  (const unsigned char*)w2_packed, b2, y);

@@ -465,22 +465,9 @@ extern "C" int pwgb_wnstack_layer_forward(const pwgb_wnstack_desc* d, int dilati
   p.D = dilation;
   p.write_x = xpk_out != nullptr;
   p.skip_init = skips_init != 0;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(wavenet_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e != cudaSuccess) {
-      set_error("wnstack_layer: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-      return PWGB_CUDA_ERROR;
-    }
-    attr_set = true;
-  }
-  static int num_sms = 0;
-  if (!num_sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (num_sms <= 0) num_sms = 132;
-  }
+  static bool smem_set = false;
+  if (const int rc = smem_opt_in(smem_set, {wavenet_fused_kernel}, 227 * 1024, "wnstack_layer")) return rc;
+  const int num_sms = tc_num_sms();
   const int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
   // tensor maps of the packed streams.  A plane ([rows][8 ch] bf16) is contiguous, so it is described as a vector of
   // 8-byte elements (2 per row): dims (2 * rows, 8-channel groups, batch x hi|lo), box (256, 4, 2) = one 16 KB operand
