@@ -141,7 +141,13 @@ PWGB_API int pwgb_dropout_backward(const float* gy, float* gx, long long n, floa
  * cp.async instead of TMA; value 4: register epilogue instead of the staged one); get key 1 copies the plan of the last
  * tensor-core conv launch, 8 ints {MT, na, nb, ns, staged, tma_act, win_mode, nco} (a buffer of at least 5 ints gets
  * the leading min(bytes, 32) bytes); get key 2 copies the plan of the last tensor-core weight-gradient launch, 4 ints
- * {nc, tg, ntg, nsplit}.  Returns 0, or -1 for any other key or a short buffer. */
+ * {nc, tg, ntg, nsplit}; get key 3 copies the last dispatch of the FFMA conv (pwgb_conv1d_forward, and the FFMA
+ * conv-transpose), 6 ints {kernel: 0 generic conv1d_fwd_kernel, 1 small_cout, 2 fewcout_long; RCO, WARPS_CO, RT, CI_T
+ * of the generic kernel (0 otherwise); CO: its CO_T, the small_cout kernel's cout, the fewcout_long template width};
+ * get key 4 copies the last pwgb_conv1d_wgrad launch, 4 ints {path: 0 tiled, 1 narrow; narrow_fast: 1 when the narrow
+ * kernel takes its stride-1 no-period loop; nsplit of the tiled kernel or the narrow kernel's blocks; ci_tiles of the
+ * tiled kernel (0 narrow)}.  Keys 3 and 4 are recorded on the host at launch (a call that launches nothing, B = 0,
+ * leaves them unchanged).  Returns 0, or -1 for any other key or a short buffer. */
 PWGB_API void pwgb_debug_set(int key, int value);
 PWGB_API int pwgb_debug_get(int key, void* dst, size_t bytes);
 PWGB_API size_t pwgb_conv1d_tc_packed_weight_bytes(int cin, int cout, int kernel);

@@ -5,6 +5,7 @@
 //     tap-flipped weight -> tensor-core path; a strided dgrad is the poly-phase conv-transpose), so only
 //     the elementwise chain-rule pieces live here: activation masks, bias sums, loss / pooling grads.
 #include <cooperative_groups.h>
+#include <string.h>
 
 #include "common.cuh"
 
@@ -22,6 +23,10 @@ struct WgK {
 };
 
 constexpr int WG_CO = 32, WG_CI = 8, WG_K = 8, WG_T = 128;
+
+// the last pwgb_conv1d_wgrad launch, for pwgb_debug_get(4, ...):
+// {path (0 tiled, 1 narrow), narrow_fast (the stride-1 no-period loop), nsplit (tiled) or narrow blocks, ci_tiles}
+int g_wgs_last[4] = {};
 
 // partial[split][co][ci_g][k] += sum over this split's (batch, chunk) items of g[co,o] * x~[ci, src(o,k)]
 __global__ void __launch_bounds__(256) conv1d_wgrad_kernel(const WgK p, const float* __restrict__ x,
@@ -638,6 +643,8 @@ extern "C" int pwgb_conv1d_wgrad(const pwgb_conv1d_desc* d, const float* x, cons
     if (ws_bytes_narrow(d) <= ws_bytes && blocks <= 65535) {
       p.chunks_per_seq = chunks;
       dim3 ngrid((unsigned)ceil_div(p.Cout * p.Cin_g, 8), (unsigned)blocks);
+      const int plan[4] = {1, p.P == 1 && p.S == 1 && p.t_valid >= p.t_in, (int)blocks, 0};
+      memcpy(g_wgs_last, plan, sizeof(plan));
       conv1d_wgrad_narrow_kernel<<<ngrid, 256, 0, st>>>(p, x, gy, (float*)ws);
       int rc = check_launch("conv1d_wgrad_narrow_kernel");
       if (rc) return rc;
@@ -655,6 +662,8 @@ extern "C" int pwgb_conv1d_wgrad(const pwgb_conv1d_desc* d, const float* x, cons
     }
   }
   dim3 grid(p.groups * ceil_div(p.Cout_g, WG_CO) * p.ci_tiles, ceil_div(p.K, WG_K), p.nsplit);
+  const int plan[4] = {0, 0, p.nsplit, p.ci_tiles};
+  memcpy(g_wgs_last, plan, sizeof(plan));
   conv1d_wgrad_kernel<<<grid, 256, smem, st>>>(p, x, gy, (float*)ws);
   int rc = check_launch("conv1d_wgrad_kernel");
   if (rc) return rc;

@@ -10,10 +10,16 @@
 // (with halo, padding policy and pre-activation already applied) and the weight slice
 // are staged in shared memory per CI_T input channels; im2col is never materialised.
 #include <stdarg.h>
+#include <string.h>
 
 #include "common.cuh"
 
 namespace pwgb {
+
+// the last conv1d_forward_simt dispatch, for pwgb_debug_get(3, ...):
+// {kernel (0 conv1d_fwd_kernel, 1 small_cout, 2 fewcout_long), RCO, WARPS_CO, RT, CI_T, CO}
+// (CO: CO_T of the generic kernel, Cout of small_cout, the template width of fewcout_long)
+int g_simt_last[6] = {};
 
 struct ConvK {
   int B, Cin, Cout, Cin_g, Cout_g, groups;
@@ -227,6 +233,8 @@ static int launch_conv_rt(ConvK p, const float* x, const float* w, const float* 
     set_error("conv1d: grid too large");
     return PWGB_UNSUPPORTED;
   }
+  const int plan[6] = {0, RCO, WARPS_CO, RT, ci_t, CO_T};
+  memcpy(g_simt_last, plan, sizeof(plan));
   kern<<<grid, 256, bytes, st>>>(p, x, w, bias, res, y);
   return check_launch("conv1d_fwd_kernel");
 }
@@ -418,12 +426,16 @@ int conv1d_forward_simt(const pwgb_conv1d_desc* d, const float* x, const float* 
   if (p.B == 0 || p.Lout == 0) return PWGB_OK;
   if (p.Cout <= 4 && p.groups == 1 && p.Cin >= 64 && p.pad_mode == PWGB_PAD_ZERO && !p.pre_gate && !residual &&
       !p.accumulate && p.shuffle <= 1 && (long long)p.Lout * p.B <= 65536 && p.B <= 65535) {
+    const int plan[6] = {1, 0, 0, 0, 0, p.Cout};
+    memcpy(g_simt_last, plan, sizeof(plan));
     conv1d_small_cout_kernel<<<dim3(ceil_div(p.Lout, 32), p.B), 256, 0, st>>>(p, x, w, bias, y);
     return check_launch("conv1d_small_cout_kernel");
   }
   if (p.Cout <= 4 && p.groups == 1 && p.P == 1 && p.t_valid == p.Lin && !p.pre_gate && !residual && !p.accumulate &&
       p.shuffle <= 1 && p.t_out >= 4096 && p.B <= 65535 && (size_t)p.Cin * p.K * 4 * sizeof(float) <= 40 * 1024) {
     const dim3 grid(ceil_div(p.t_out, 1024), p.B);
+    const int plan[6] = {2, 0, 0, 0, 0, p.Cout <= 2 ? p.Cout : 4};
+    memcpy(g_simt_last, plan, sizeof(plan));
     if (p.Cout == 1) {
       conv1d_fewcout_long_kernel<1><<<grid, 256, (size_t)p.Cin * p.K * sizeof(float), st>>>(p, x, w, bias, y);
     } else if (p.Cout == 2) {

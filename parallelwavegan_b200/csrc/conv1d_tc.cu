@@ -833,14 +833,25 @@ extern "C" void pwgb_debug_set(int key, int value) {
   if (key == 1) g_tc_variant = value;
 }
 
+namespace pwgb {
+extern int g_simt_last[6];  // conv1d_simt.cu
+extern int g_wgs_last[4];   // backward.cu
+}  // namespace pwgb
+
 // key 1: the plan of the last conv1d_tc launch, {MT, na, nb, ns, staged, tma_act, win_mode, nco};
-// key 2: the plan of the last conv1d_wgrad_tc launch, {nc, tg, ntg, nsplit}.
-// Copies min(bytes, size of the record); a buffer of at least 5 (key 1) or 4 (key 2) ints is required.
+// key 2: the plan of the last conv1d_wgrad_tc launch, {nc, tg, ntg, nsplit};
+// key 3: the last FFMA conv dispatch, {kernel, RCO, WARPS_CO, RT, CI_T, CO};
+// key 4: the last FFMA weight-gradient launch, {path, narrow_fast, nsplit or narrow blocks, ci_tiles}.
+// Copies min(bytes, size of the record); a buffer of at least 5 (key 1) or the whole record (keys 2-4) is required.
 extern "C" int pwgb_debug_get(int key, void* dst, size_t bytes) {
   if (!dst) return -1;
-  const void* src = key == 1 ? (const void*)&g_tc_last : key == 2 ? (const void*)&g_wt_last : nullptr;
-  const size_t size = key == 1 ? sizeof(TcPlanInfo) : sizeof(WtPlanInfo);
-  const size_t need = key == 1 ? 5 * sizeof(int) : sizeof(WtPlanInfo);
+  const void* src = key == 1   ? (const void*)&g_tc_last
+                    : key == 2 ? (const void*)&g_wt_last
+                    : key == 3 ? (const void*)g_simt_last
+                    : key == 4 ? (const void*)g_wgs_last
+                               : nullptr;
+  const size_t size = key == 1 ? sizeof(TcPlanInfo) : key == 2 ? sizeof(WtPlanInfo) : key == 3 ? sizeof(g_simt_last) : sizeof(g_wgs_last);
+  const size_t need = key == 1 ? 5 * sizeof(int) : size;
   if (!src || bytes < need) return -1;
   memcpy(dst, src, bytes < size ? bytes : size);
   return 0;
