@@ -201,6 +201,7 @@ typedef struct pwgb_wavenet_desc {
   int32_t residual_channels, gate_channels, skip_channels;
   int32_t aux_channels; /* as stored, padded to a multiple of 32 (0 = no conditioning) */
   int32_t kernel, dilation;
+  int32_t causal; /* 0: centred taps (odd kernel); 1: causal taps t - (kernel-1-j)*dilation (any kernel) */
 } pwgb_wavenet_desc;
 PWGB_API int pwgb_wavenet_supported(const pwgb_wavenet_desc* d);
 PWGB_API size_t pwgb_wavenet_packed_bytes(const pwgb_wavenet_desc* d);
@@ -275,7 +276,8 @@ PWGB_API int pwgb_s2d_backward(const float* gy, float* gx, int batch, int channe
  *       [halo, halo+t) hold the samples; every other row MUST be zero (allocate zero-filled once; the
  *       kernels only ever write rows [halo, halo+t));
  *   cpk [batch][hi|lo][ceil(aux_channels/8)][round_up(t,256)][8] bf16 (written completely by pack_c).
- * halo >= (kernel-1)/2 * (largest dilation of the stack).  Weights: the image written by
+ * halo >= (kernel-1)/2 * (largest dilation of the stack), or (kernel-1) * (largest dilation) when causal
+ * (the layout stays symmetric; a causal layer only reads the left halo).  Weights: the image written by
  * pwgb_wavenet_pack() for the same channel counts with the aux weight padded to a multiple of 32
  * channels (desc.aux_channels there = round_up(aux_channels, 32)).  b_skip_out = concat(b_skip, b_out).
  * layer_forward:  skips (fp32, (batch, skip_channels, t)) = [skips_init ? 0 : skips] + s;
@@ -287,6 +289,7 @@ typedef struct pwgb_wnstack_desc {
   int32_t residual_channels, gate_channels, skip_channels;
   int32_t aux_channels; /* real conditioning channels (multiple of 16) */
   int32_t kernel, halo;
+  int32_t causal; /* 0: centred taps (odd kernel); 1: causal taps t - (kernel-1-j)*dilation (any kernel) */
 } pwgb_wnstack_desc;
 PWGB_API int pwgb_wnstack_supported(const pwgb_wnstack_desc* d);
 PWGB_API size_t pwgb_wnstack_x_bytes(const pwgb_wnstack_desc* d);
@@ -312,6 +315,14 @@ PWGB_API int pwgb_wnstack_layer_forward(const pwgb_wnstack_desc* d, int dilation
  * ---------------------------------------------------------------------- */
 PWGB_API int pwgb_upsample_fir_forward(int rows, int rows_per_batch, int t_in, int scale, const float* x, const float* fir,
                               float* y, long long y_batch_stride, void* stream);
+/* Causal stage (layers/upsample.py:98-125 with use_causal_conv: the FIR pads 2*scale on the left and the tail is
+ * cropped): the tap origin moves from scale to 2*scale,
+ *   y[r, o] = sum_k f[k] * x[r, (o + k - 2*scale) / scale]   for 0 <= o + k - 2*scale < t_in*scale,
+ * so output frame j only meets input frames j-2, j-1, j.  Same arguments and layout as the centred pair. */
+PWGB_API int pwgb_upsample_fir_causal_forward(int rows, int rows_per_batch, int t_in, int scale, const float* x, const float* fir,
+                                     float* y, long long y_batch_stride, void* stream);
+PWGB_API int pwgb_upsample_fir_causal_backward(int rows, int rows_per_batch, int t_in, int scale, const float* x, const float* fir,
+                                      const float* gy, long long gy_batch_stride, float* gx, float* dfir, void* stream);
 
 /* ------------------------------------------------------------------------
  * Spectral losses.  stft(): losses/stft_loss.py:16-40 (center=True, reflect pad n_fft/2, window of

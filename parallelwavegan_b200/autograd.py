@@ -379,9 +379,10 @@ class UpsampleFirFn(torch.autograd.Function):
     """One stage of the conditioning upsampler (layers/upsample.py:122-128) with both adjoints."""
 
     @staticmethod
-    def forward(ctx, x, fir, scale, out_channels):
-        y = ops.upsample_fir(x, fir, scale, out_channels=out_channels)
+    def forward(ctx, x, fir, scale, out_channels, causal=False):
+        y = ops.upsample_fir(x, fir, scale, out_channels=out_channels, causal=causal)
         ctx.scale = scale
+        ctx.causal = causal
         ctx.fir_shape = tuple(fir.shape)
         ctx.save_for_backward(x, fir)
         return y
@@ -396,10 +397,12 @@ class UpsampleFirFn(torch.autograd.Function):
         gx = torch.empty_like(x) if need_x else None
         df = torch.empty(2 * ctx.scale + 1, device=x.device, dtype=torch.float32) if need_f else None
         f1 = fir.detach().reshape(-1).contiguous()
-        rc = capi.lib().pwgb_upsample_fir_backward(B * Cc, Cc, T, int(ctx.scale), ops._p(x), ops._p(f1), ops._p(gy),
-                                                   oc * T * ctx.scale, ops._p(gx), ops._p(df), ops._stream())
-        capi.check(rc, "pwgb_upsample_fir_backward")
-        return gx, (df.reshape(ctx.fir_shape) if need_f else None), None, None
+        L = capi.lib()
+        fn = L.pwgb_upsample_fir_causal_backward if ctx.causal else L.pwgb_upsample_fir_backward
+        rc = fn(B * Cc, Cc, T, int(ctx.scale), ops._p(x), ops._p(f1), ops._p(gy), oc * T * ctx.scale, ops._p(gx), ops._p(df),
+                ops._stream())
+        capi.check(rc, "pwgb_upsample_fir_causal_backward" if ctx.causal else "pwgb_upsample_fir_backward")
+        return gx, (df.reshape(ctx.fir_shape) if need_f else None), None, None, None
 
 
 class MrStftLossFn(torch.autograd.Function):

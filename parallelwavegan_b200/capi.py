@@ -37,6 +37,7 @@ class WaveNetDesc(C.Structure):
     _fields_ = [
         ("batch", C.c_int32), ("t", C.c_int32), ("residual_channels", C.c_int32), ("gate_channels", C.c_int32),
         ("skip_channels", C.c_int32), ("aux_channels", C.c_int32), ("kernel", C.c_int32), ("dilation", C.c_int32),
+        ("causal", C.c_int32),
     ]
 
 
@@ -51,6 +52,7 @@ class WnStackDesc(C.Structure):
     _fields_ = [
         ("batch", C.c_int32), ("t", C.c_int32), ("residual_channels", C.c_int32), ("gate_channels", C.c_int32),
         ("skip_channels", C.c_int32), ("aux_channels", C.c_int32), ("kernel", C.c_int32), ("halo", C.c_int32),
+        ("causal", C.c_int32),
     ]
 
 
@@ -149,8 +151,9 @@ def lib():
     for fn in (L.pwgb_s2d_forward, L.pwgb_s2d_backward):
         fn.restype = C.c_int
         fn.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_longlong, C.c_int, vp]
-    L.pwgb_upsample_fir_forward.restype = C.c_int
-    L.pwgb_upsample_fir_forward.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_longlong, vp]
+    for fn in (L.pwgb_upsample_fir_forward, L.pwgb_upsample_fir_causal_forward):
+        fn.restype = C.c_int
+        fn.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_longlong, vp]
     L.pwgb_mr_stft_loss_workspace.restype = C.c_size_t
     L.pwgb_mr_stft_loss_workspace.argtypes = [C.POINTER(StftDesc), C.c_int]
     L.pwgb_mr_stft_loss_forward.restype = C.c_int
@@ -214,8 +217,9 @@ def lib():
     L.pwgb_tade_combine_backward.argtypes = [vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_longlong, C.c_int, vp]
     L.pwgb_tade_gate_backward.restype = C.c_int
     L.pwgb_tade_gate_backward.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_longlong, C.c_int, vp]
-    L.pwgb_upsample_fir_backward.restype = C.c_int
-    L.pwgb_upsample_fir_backward.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_longlong, vp, vp, vp]
+    for fn in (L.pwgb_upsample_fir_backward, L.pwgb_upsample_fir_causal_backward):
+        fn.restype = C.c_int
+        fn.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_longlong, vp, vp, vp]
     L.pwgb_stft_loss_terms.restype = C.c_int
     L.pwgb_stft_loss_terms.argtypes = [vp, vp, C.c_longlong, C.c_float, C.c_int, vp, vp, vp, C.c_int, vp]
     L.pwgb_stft_loss_dmag.restype = C.c_int
@@ -273,7 +277,7 @@ EXPORTED_SYMBOLS = [
     "pwgb_conv1d_tc_forward", "pwgb_debug_set", "pwgb_debug_get",
     "pwgb_resblock_pair_supported", "pwgb_resblock_pair_plan", "pwgb_resblock_pair_forward",
     "pwgb_wavenet_supported", "pwgb_wavenet_packed_bytes",
-    "pwgb_wavenet_pack", "pwgb_wavenet_layer_forward", "pwgb_upsample_fir_forward",
+    "pwgb_wavenet_pack", "pwgb_wavenet_layer_forward", "pwgb_upsample_fir_forward", "pwgb_upsample_fir_causal_forward",
     "pwgb_s2d_forward", "pwgb_s2d_backward", "pwgb_mt_clip_coef", "pwgb_mt_adam_step", "pwgb_prep_features", "pwgb_pcm16_forward", "pwgb_collate_crop",
     "pwgb_wnstack_supported", "pwgb_wnstack_x_bytes", "pwgb_wnstack_c_bytes", "pwgb_wnstack_pack_x", "pwgb_wnstack_unpack_x",
     "pwgb_wnstack_pack_c", "pwgb_wnstack_first_conv", "pwgb_wnstack_layer_forward",
@@ -286,7 +290,7 @@ EXPORTED_SYMBOLS = [
     "pwgb_tade_gate_forward", "pwgb_instance_norm_backward", "pwgb_upsample_nearest_backward", "pwgb_tade_combine_backward",
     "pwgb_tade_gate_backward",
     "pwgb_stft_amplitude_backward", "pwgb_mel_project_backward", "pwgb_gate_forward", "pwgb_gate_backward",
-    "pwgb_upsample_fir_backward", "pwgb_stft_loss_terms", "pwgb_stft_loss_dmag",
+    "pwgb_upsample_fir_backward", "pwgb_upsample_fir_causal_backward", "pwgb_stft_loss_terms", "pwgb_stft_loss_dmag",
     "pwgb_symbol_embed_forward", "pwgb_symbol_embed_backward_workspace", "pwgb_symbol_embed_backward",
     "pwgb_channel_layernorm_forward", "pwgb_channel_layernorm_backward_workspace", "pwgb_channel_layernorm_backward",
     "pwgb_duration_loss_forward", "pwgb_duration_loss_backward", "pwgb_duration_round", "pwgb_collate_runlength",

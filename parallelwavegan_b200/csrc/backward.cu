@@ -439,36 +439,36 @@ __global__ void gate_backward_kernel(const float* __restrict__ g, const float* _
   }
 }
 
-// adjoints of upsample_fir_kernel: y[r,o] = sum_k f[k] x[r, (o+k-s)/s]
-__global__ void upsample_fir_backward_x_kernel(int t_in, int s, const float* __restrict__ gy, const float* __restrict__ fir,
+// adjoints of upsample_fir_kernel: y[r,o] = sum_k f[k] x[r, (o+k-origin)/s], tap origin (1 + lag) s (lag 1: causal)
+__global__ void upsample_fir_backward_x_kernel(int t_in, int s, int lag, const float* __restrict__ gy, const float* __restrict__ fir,
                                                float* __restrict__ gx, int rows_per_batch, long long gybs) {
   extern __shared__ float f[];
   for (int i = threadIdx.x; i < 2 * s + 1; i += blockDim.x) f[i] = fir[i];
   __syncthreads();
   const int r = blockIdx.y;
-  const int t_out = t_in * s;
+  const int t_out = t_in * s, origin = (1 + lag) * s;
   const float* gr = gy + (long long)(r / rows_per_batch) * gybs + (long long)(r % rows_per_batch) * t_out;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < t_in; i += gridDim.x * blockDim.x) {
     float acc = 0.f;
-    // positions q = o + k - s with q / s == i  <=>  q in [i*s, i*s + s)
+    // positions q = o + k - origin with q / s == i  <=>  q in [i*s, i*s + s)
     for (int q = i * s; q < i * s + s; ++q)
       for (int k = 0; k <= 2 * s; ++k) {
-        const int o = q - k + s;
+        const int o = q - k + origin;
         if (o >= 0 && o < t_out) acc = fmaf(f[k], gr[o], acc);
       }
     gx[(long long)r * t_in + i] = acc;
   }
 }
-// df[k] = sum_{r,o} gy[r,o] * x[r,(o+k-s)/s]: ONE pass over gy for all 2s+1 taps (the one-CTA-per-tap version read gy
+// df[k] = sum_{r,o} gy[r,o] * x[r,(o+k-origin)/s]: ONE pass over gy for all 2s+1 taps (the one-CTA-per-tap version read gy
 // 2s+1 times on 2s+1 SMs: 100 ms per call, 40 % of the Parallel WaveGAN training step).  Output o = j*s + ph only meets
-// the input frames j-1, j, j+1, so the kernel accumulates the 3 s sums S[w][ph] = sum gy[j*s+ph] * x[j + w - 1] (three FMAs
+// the input frames j-1, j, j+1 (minus lag), so the kernel accumulates the 3 s sums S[w][ph] = sum gy[j*s+ph] * x[j + w - 1] (three FMAs
 // per element, float within a row, double across rows) and folds them into the taps at the end:
 // df[k] = sum_ph S[w(ph, k)][ph], w = 0 / 1 / 2 for ph + k - s < 0 / < s / >= s.  A cluster of 8 CTAs splits the rows;
 // partials are combined through distributed shared memory in rank order (deterministic, no workspace).
 constexpr int UF_CLUSTER = 8, UF_MAXS = 8, UF_MAXT = 2 * UF_MAXS + 1, UF_THREADS = 512;
 template <int MAXS>
 __global__ void __cluster_dims__(UF_CLUSTER, 1, 1) __launch_bounds__(UF_THREADS)
-    upsample_fir_backward_f_kernel(int rows, int t_in, int s, const float* __restrict__ x, const float* __restrict__ gy,
+    upsample_fir_backward_f_kernel(int rows, int t_in, int s, int lag, const float* __restrict__ x, const float* __restrict__ gy,
                                    float* __restrict__ df, int rows_per_batch, long long gybs) {
   namespace cg = cooperative_groups;
   cg::cluster_group cl = cg::this_cluster();
@@ -491,7 +491,8 @@ __global__ void __cluster_dims__(UF_CLUSTER, 1, 1) __launch_bounds__(UF_THREADS)
 #pragma unroll
       for (int ph = 0; ph < MAXS; ++ph) f[w][ph] = 0.f;
     for (int j = threadIdx.x; j < t_in; j += UF_THREADS) {
-      const float xm = j > 0 ? xr[j - 1] : 0.f, x0 = xr[j], xp = j + 1 < t_in ? xr[j + 1] : 0.f;
+      const int jc = j - lag;
+      const float xm = jc > 0 ? xr[jc - 1] : 0.f, x0 = jc >= 0 ? xr[jc] : 0.f, xp = jc + 1 < t_in ? xr[jc + 1] : 0.f;
       const float* g = gr + (long long)j * s;
 #pragma unroll
       for (int ph = 0; ph < MAXS; ++ph) {
@@ -537,18 +538,18 @@ __global__ void __cluster_dims__(UF_CLUSTER, 1, 1) __launch_bounds__(UF_THREADS)
   cl.sync();
 }
 // scales beyond UF_MAXT taps: one CTA per tap, fixed order
-__global__ void __launch_bounds__(256) upsample_fir_backward_f_tap_kernel(int rows, int t_in, int s, const float* __restrict__ x,
+__global__ void __launch_bounds__(256) upsample_fir_backward_f_tap_kernel(int rows, int t_in, int s, int lag, const float* __restrict__ x,
                                                                            const float* __restrict__ gy, float* __restrict__ df,
                                                                            int rows_per_batch, long long gybs) {
   __shared__ double red[256];
   const int k = blockIdx.x;
-  const int t_out = t_in * s;
+  const int t_out = t_in * s, origin = (1 + lag) * s;
   double a = 0;
   for (int r = 0; r < rows; ++r) {
     const float* gr = gy + (long long)(r / rows_per_batch) * gybs + (long long)(r % rows_per_batch) * t_out;
     const float* xr = x + (long long)r * t_in;
     for (int o = threadIdx.x; o < t_out; o += 256) {
-      const int q = o + k - s;
+      const int q = o + k - origin;
       if (q >= 0 && q < t_out) a += (double)gr[o] * xr[q / s];
     }
   }
@@ -773,8 +774,8 @@ extern "C" int pwgb_gate_backward(const float* g, const float* gz, float* gg, in
   return check_launch("gate_backward_kernel");
 }
 
-extern "C" int pwgb_upsample_fir_backward(int rows, int rows_per_batch, int t_in, int scale, const float* x, const float* fir,
-                                          const float* gy, long long gy_batch_stride, float* gx, float* dfir, void* stream) {
+static int upsample_fir_backward(int rows, int rows_per_batch, int t_in, int scale, int lag, const float* x, const float* fir,
+                                 const float* gy, long long gy_batch_stride, float* gx, float* dfir, void* stream) {
   PWGB_CHECK_ARG(fir && gy && (gx || (dfir && x)), "upsample_fir_backward: null argument");
   PWGB_CHECK_ARG(rows >= 0 && rows_per_batch > 0 && t_in > 0 && scale > 0 && rows % rows_per_batch == 0, "upsample_fir_backward: bad sizes");
   PWGB_UNSUPPORTED_IF(rows > 65535, "upsample_fir_backward: too many rows");
@@ -783,20 +784,30 @@ extern "C" int pwgb_upsample_fir_backward(int rows, int rows_per_batch, int t_in
   const long long gybs = gy_batch_stride ? gy_batch_stride : (long long)rows_per_batch * t_in * scale;
   if (gx) {
     dim3 grid(ceil_div(t_in, 256) < 64 ? ceil_div(t_in, 256) : 64, rows);
-    upsample_fir_backward_x_kernel<<<grid, 256, (2 * scale + 1) * sizeof(float), st>>>(t_in, scale, gy, fir, gx, rows_per_batch, gybs);
+    upsample_fir_backward_x_kernel<<<grid, 256, (2 * scale + 1) * sizeof(float), st>>>(t_in, scale, lag, gy, fir, gx, rows_per_batch, gybs);
     int rc = check_launch("upsample_fir_backward_x_kernel");
     if (rc) return rc;
   }
   if (dfir) {
     if (2 * scale + 1 <= UF_MAXT) {
       if (scale <= 4)
-        upsample_fir_backward_f_kernel<4><<<UF_CLUSTER, UF_THREADS, 0, st>>>(rows, t_in, scale, x, gy, dfir, rows_per_batch, gybs);
+        upsample_fir_backward_f_kernel<4><<<UF_CLUSTER, UF_THREADS, 0, st>>>(rows, t_in, scale, lag, x, gy, dfir, rows_per_batch, gybs);
       else
-        upsample_fir_backward_f_kernel<UF_MAXS><<<UF_CLUSTER, UF_THREADS, 0, st>>>(rows, t_in, scale, x, gy, dfir, rows_per_batch, gybs);
+        upsample_fir_backward_f_kernel<UF_MAXS><<<UF_CLUSTER, UF_THREADS, 0, st>>>(rows, t_in, scale, lag, x, gy, dfir, rows_per_batch, gybs);
       return check_launch("upsample_fir_backward_f_kernel");
     }
-    upsample_fir_backward_f_tap_kernel<<<2 * scale + 1, 256, 0, st>>>(rows, t_in, scale, x, gy, dfir, rows_per_batch, gybs);
+    upsample_fir_backward_f_tap_kernel<<<2 * scale + 1, 256, 0, st>>>(rows, t_in, scale, lag, x, gy, dfir, rows_per_batch, gybs);
     return check_launch("upsample_fir_backward_f_tap_kernel");
   }
   return PWGB_OK;
+}
+
+extern "C" int pwgb_upsample_fir_backward(int rows, int rows_per_batch, int t_in, int scale, const float* x, const float* fir,
+                                          const float* gy, long long gy_batch_stride, float* gx, float* dfir, void* stream) {
+  return upsample_fir_backward(rows, rows_per_batch, t_in, scale, 0, x, fir, gy, gy_batch_stride, gx, dfir, stream);
+}
+
+extern "C" int pwgb_upsample_fir_causal_backward(int rows, int rows_per_batch, int t_in, int scale, const float* x, const float* fir,
+                                                 const float* gy, long long gy_batch_stride, float* gx, float* dfir, void* stream) {
+  return upsample_fir_backward(rows, rows_per_batch, t_in, scale, 1, x, fir, gy, gy_batch_stride, gx, dfir, stream);
 }

@@ -973,7 +973,7 @@ static void wn_descs(const pwgb_wavenet_desc* d, pwgb_conv1d_desc& c1, pwgb_conv
   c1.stride = 1;
   c1.dilation = d->dilation;
   c1.groups = 1;
-  c1.pad_left = (d->kernel - 1) / 2 * d->dilation;
+  c1.pad_left = (d->causal ? d->kernel - 1 : (d->kernel - 1) / 2) * d->dilation;
   c1.pad_mode = PWGB_PAD_ZERO;
   c1.period = 1;
   c1.t_valid = d->t;
@@ -997,7 +997,7 @@ static void wn_descs(const pwgb_wavenet_desc* d, pwgb_conv1d_desc& c1, pwgb_conv
 }
 
 static int wn_valid(const pwgb_wavenet_desc* d) {
-  return d && d->batch >= 0 && d->t > 0 && d->kernel > 0 && d->kernel % 2 == 1 && d->dilation > 0 &&
+  return d && d->batch >= 0 && d->t > 0 && d->kernel > 0 && (d->causal || d->kernel % 2 == 1) && d->dilation > 0 &&
          d->residual_channels > 0 && d->gate_channels > 0 && d->gate_channels % 2 == 0 && d->skip_channels > 0 &&
          d->aux_channels >= 0;
 }

@@ -1,14 +1,17 @@
 // PWG conditioning upsampler stage: nearest repeat x s + (2s+1)-tap FIR (layers/upsample.py:112-128),
 // evaluated poly-phase: output o only touches input frames (o-s)/s .. (o+s)/s, no stretched tensor.
+// The causal stage (use_causal_conv: the FIR pads 2s on the left and the tail is cropped, upsample.py:98-125) is the
+// same FIR with its tap origin at 2s instead of s: every output meets the input frames one frame earlier.  `lag` is
+// that shift in frames (0 centred, 1 causal); the per-phase coefficients do not depend on it.
 #include "common.cuh"
 
 namespace pwgb {
 
-// Output o = j*s + ph only touches the input frames j-1, j, j+1: y[o] = A[ph] x[j-1] + B[ph] x[j] + C[ph] x[j+1] with the
+// Output o = j*s + ph only touches the input frames j-1, j, j+1 (minus lag): y[o] = A[ph] x[j-1] + B[ph] x[j] + C[ph] x[j+1] with the
 // taps pre-summed per phase (A: taps that land in frame j-1, ...).  One thread per input frame writes its s outputs
 // (one 16-byte store per 4): 3 FMAs per output instead of 2s+1 taps with an integer division each (the tap loop ran
 // at 1/12 of the HBM rate: 13 % of the Parallel WaveGAN forward).
-__global__ void upsample_fir_kernel(int rows, int rows_per_batch, int t_in, int s, const float* __restrict__ x,
+__global__ void upsample_fir_kernel(int rows, int rows_per_batch, int t_in, int s, int lag, const float* __restrict__ x,
                                     const float* __restrict__ fir, float* __restrict__ y, long long ybs) {
   extern __shared__ float coef[];  // [3][s]
   for (int ph = threadIdx.x; ph < s; ph += blockDim.x) {
@@ -34,7 +37,8 @@ __global__ void upsample_fir_kernel(int rows, int rows_per_batch, int t_in, int 
   float* yr = y + (long long)(r / rows_per_batch) * ybs + (long long)(r % rows_per_batch) * t_out;
   const bool vec = (s % 4 == 0) && ((reinterpret_cast<uintptr_t>(yr) & 15) == 0);
   for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < t_in; j += gridDim.x * blockDim.x) {
-    const float xm = j > 0 ? __ldg(xr + j - 1) : 0.f, x0 = __ldg(xr + j), xp = j + 1 < t_in ? __ldg(xr + j + 1) : 0.f;
+    const int jc = j - lag;
+    const float xm = jc > 0 ? __ldg(xr + jc - 1) : 0.f, x0 = jc >= 0 ? __ldg(xr + jc) : 0.f, xp = jc + 1 < t_in ? __ldg(xr + jc + 1) : 0.f;
     float* dst = yr + (long long)j * s;
     if (vec) {
       for (int ph = 0; ph < s; ph += 4) {
@@ -55,8 +59,8 @@ __global__ void upsample_fir_kernel(int rows, int rows_per_batch, int t_in, int 
 
 using namespace pwgb;
 
-extern "C" int pwgb_upsample_fir_forward(int rows, int rows_per_batch, int t_in, int scale, const float* x,
-                                         const float* fir, float* y, long long y_batch_stride, void* stream) {
+static int upsample_fir_forward(int rows, int rows_per_batch, int t_in, int scale, int lag, const float* x, const float* fir,
+                                float* y, long long y_batch_stride, void* stream) {
   PWGB_CHECK_ARG(x && fir && y, "upsample_fir: null argument");
   PWGB_CHECK_ARG(rows >= 0 && rows_per_batch > 0 && t_in > 0 && scale > 0 && rows % rows_per_batch == 0,
                  "upsample_fir: bad sizes");
@@ -65,6 +69,16 @@ extern "C" int pwgb_upsample_fir_forward(int rows, int rows_per_batch, int t_in,
   const int t_out = t_in * scale;
   dim3 grid(ceil_div(t_in, 256) < 64 ? ceil_div(t_in, 256) : 64, rows);
   upsample_fir_kernel<<<grid, 256, 3 * scale * sizeof(float), (cudaStream_t)stream>>>(
-      rows, rows_per_batch, t_in, scale, x, fir, y, y_batch_stride ? y_batch_stride : (long long)rows_per_batch * t_out);
+      rows, rows_per_batch, t_in, scale, lag, x, fir, y, y_batch_stride ? y_batch_stride : (long long)rows_per_batch * t_out);
   return check_launch("upsample_fir_kernel");
+}
+
+extern "C" int pwgb_upsample_fir_forward(int rows, int rows_per_batch, int t_in, int scale, const float* x,
+                                         const float* fir, float* y, long long y_batch_stride, void* stream) {
+  return upsample_fir_forward(rows, rows_per_batch, t_in, scale, 0, x, fir, y, y_batch_stride, stream);
+}
+
+extern "C" int pwgb_upsample_fir_causal_forward(int rows, int rows_per_batch, int t_in, int scale, const float* x,
+                                                const float* fir, float* y, long long y_batch_stride, void* stream) {
+  return upsample_fir_forward(rows, rows_per_batch, t_in, scale, 1, x, fir, y, y_batch_stride, stream);
 }

@@ -39,6 +39,7 @@ constexpr int WN_BLK = WN_TT * 16;         // one (8 channel, 128 row) operand b
 
 struct WnK {
   int B, T, R, G, S, A, K, D, halo;
+  int tap0;              // tap sitting on the output row: K/2 centred, K-1 causal
   int H;                 // gate output channels = G / 2
   int Tp, Tc;            // rows per plane of xpk / cpk
   int ngx, ngc;          // 8-channel groups of x / c
@@ -158,7 +159,7 @@ __global__ void __launch_bounds__(WN_THREADS, 1)
           const unsigned full = FULL(s);
           mbar_expect_tx(full, (unsigned)(p.a_bytes + p.b_bytes));
           if (is_x)
-            tma_load_3d(dstA, &tm_x, 2 * (p.halo + t0 + (tap - p.K / 2) * p.D), chunk * 4, 2 * b, full);
+            tma_load_3d(dstA, &tm_x, 2 * (p.halo + t0 + (tap - p.tap0) * p.D), chunk * 4, 2 * b, full);
           else
             tma_load_3d(dstA, &tm_c, 2 * t0, chunk * 4, 2 * b, full);
           const unsigned char* wsrc = is_x ? wpk + (size_t)j * p.b_bytes : w_aux + (size_t)chunk * p.b_bytes;
@@ -333,7 +334,8 @@ __global__ void wn_first_conv_kernel(const float* __restrict__ z, int cin, const
 
 
 static int wn_plan(const pwgb_wnstack_desc* d, WnK& p, size_t& smem_bytes) {
-  if (!d || d->batch < 0 || d->t <= 0 || d->kernel <= 0 || d->kernel % 2 == 0 || d->halo < 0) return 0;
+  if (!d || d->batch < 0 || d->t <= 0 || d->kernel <= 0 || d->halo < 0) return 0;
+  if (!d->causal && d->kernel % 2 == 0) return 0;  // even kernels only as causal convs (layers/residual_block.py:73-77)
   const int R = d->residual_channels, G = d->gate_channels, S = d->skip_channels, A = d->aux_channels;
   if (R <= 0 || R % KC || G <= 0 || G % 2 || (G / 2) % KC || G % 16 || S <= 0 || S % 16 || A <= 0 || A % 16) return 0;
   const int N2 = S + R;
@@ -347,6 +349,7 @@ static int wn_plan(const pwgb_wnstack_desc* d, WnK& p, size_t& smem_bytes) {
   p.A = A;
   p.K = d->kernel;
   p.halo = d->halo;
+  p.tap0 = d->causal ? d->kernel - 1 : d->kernel / 2;
   p.H = G / 2;
   p.D = 1;
   const int tr = ceil_div(d->t, 2 * WN_TT) * (2 * WN_TT);  // packed planes are whole 256-sample blocks
@@ -454,7 +457,7 @@ extern "C" int pwgb_wnstack_layer_forward(const pwgb_wnstack_desc* d, int dilati
   WnK p;
   size_t bytes = 0;
   PWGB_UNSUPPORTED_IF(!wn_plan(d, p, bytes), "wnstack: configuration not supported by the fused tensor-core layer");
-  PWGB_CHECK_ARG(dilation > 0 && (long long)(d->kernel / 2) * dilation <= d->halo, "wnstack_layer: dilation %d exceeds the halo %d of the packed stream",
+  PWGB_CHECK_ARG(dilation > 0 && (long long)p.tap0 * dilation <= d->halo, "wnstack_layer: dilation %d exceeds the halo %d of the packed stream",
                  dilation, d->halo);
   if (p.B == 0) return PWGB_OK;  // an empty batch: no launch (and the empty buffers have no storage)
   PWGB_CHECK_ARG(xpk_in && cpk && packed_w && skips, "wnstack_layer: null argument");

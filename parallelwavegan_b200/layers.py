@@ -297,7 +297,8 @@ class PQMF(torch.nn.Module):
 
 class WaveNetResidualBlock(torch.nn.Module):
     """layers/residual_block.py:43-140.  ``forward(x, c, skips)`` runs the fused layer and
-    accumulates the skip branch in place; it returns the new residual stream."""
+    accumulates the skip branch in place; it returns the new residual stream.  ``dropout`` acts on the conv input
+    only (the residual add takes the un-dropped x, residual_block.py:114-116), in train mode also under no_grad."""
 
     def __init__(
         self,
@@ -313,15 +314,14 @@ class WaveNetResidualBlock(torch.nn.Module):
     ):
         super().__init__()
         if use_causal_conv:
-            raise PwgbError("WaveNetResidualBlock(use_causal_conv=True) has no sm_90a kernel yet")
-        if dropout != 0.0:
-            raise PwgbError("WaveNetResidualBlock(dropout>0) has no sm_90a kernel (all reference configs use 0.0)")
-        assert (kernel_size - 1) % 2 == 0, "Not support even number kernel size."
+            padding = (kernel_size - 1) * dilation  # the container's padding; the kernels pad the left side only
+        else:
+            assert (kernel_size - 1) % 2 == 0, "Not support even number kernel size."
+            padding = (kernel_size - 1) // 2 * dilation
         self.dropout = dropout
         self.dilation = dilation
         self.aux_channels = aux_channels
         self.use_causal_conv = use_causal_conv
-        padding = (kernel_size - 1) // 2 * dilation
         self.conv = Conv1d(residual_channels, gate_channels, kernel_size, padding=padding, dilation=dilation, bias=bias)
         self.conv1x1_aux = Conv1d1x1(aux_channels, gate_channels, bias=False) if aux_channels > 0 else None
         gate_out_channels = gate_channels // 2
@@ -338,6 +338,9 @@ class WaveNetResidualBlock(torch.nn.Module):
             if skips is not None:
                 raise PwgbError("in-place skip accumulation is inference-only; use the returned skip tensor under autograd")
             return self._forward_train(x, c)  # (x_out, s): the reference's pair, differentiable
+        if self.training and self.dropout > 0:  # the conv reads the dropped x, the residual add the original
+            x_out, s = self._forward_train(x, c)
+            return (x_out, s) if skips is None else (x_out, ops.axpby(1.0, s, 1.0, skips))
         if skips is None:
             skips = torch.zeros((x.shape[0], self.conv1x1_skip.out_channels, x.shape[2]), device=x.device, dtype=x.dtype)
         x_out = ops.wavenet_layer(
@@ -347,18 +350,20 @@ class WaveNetResidualBlock(torch.nn.Module):
             effective_weight(self.conv1x1_skip), self.conv1x1_skip.bias,
             effective_weight(self.conv1x1_out), self.conv1x1_out.bias,
             self.dilation, skips, self.aux_channels, cache=self._cache,
-            key=ops.param_key(self.conv, aux, self.conv1x1_skip, self.conv1x1_out),
+            key=ops.param_key(self.conv, aux, self.conv1x1_skip, self.conv1x1_out), causal=self.use_causal_conv,
         )
         return x_out, skips
 
 
 def _wn_train(self, x, c):
     """Differentiable composition of the layer (every op's forward and backward is a libpwgb kernel):
-    g = conv_dil(x) + W_aux c ; z = gate(g) ; s = W_skip z ; x' = (W_out z + x) * sqrt(0.5)."""
+    g = conv_dil(dropout(x)) + W_aux c ; z = gate(g) ; s = W_skip z ; x' = (W_out z + x) * sqrt(0.5)."""
     from .autograd import GateFn
 
     k = self.conv.kernel_size[0]
-    g = ops.conv1d(x, effective_weight(self.conv), self.conv.bias, dilation=self.dilation, padding=(k - 1) // 2 * self.dilation)
+    xd = ops.dropout(x, self.dropout, self.training)
+    g = ops.conv1d(xd, effective_weight(self.conv), self.conv.bias, dilation=self.dilation,
+                   padding=ops.wavenet_padding(k, self.dilation, self.use_causal_conv))
     if c is not None:
         wa = effective_weight(self.conv1x1_aux)
         if c.shape[1] != wa.shape[1]:  # conditioning stored channel-padded (zeros): pad the weight columns
@@ -393,19 +398,21 @@ class Conv2d(torch.nn.Conv2d):
 
 
 class UpsampleNetwork(torch.nn.Module):
-    """layers/upsample.py:62-128."""
+    """layers/upsample.py:62-128.  Causal: each FIR pads 2*scale on the left and the tail is cropped
+    (upsample.py:98-125), one launch per stage as in the centred form."""
 
     def __init__(self, upsample_scales, nonlinear_activation=None, nonlinear_activation_params={},
                  interpolate_mode="nearest", freq_axis_kernel_size=1, use_causal_conv=False):
         super().__init__()
-        if use_causal_conv or nonlinear_activation is not None or freq_axis_kernel_size != 1:
-            raise PwgbError("UpsampleNetwork: causal / nonlinear / freq-axis-kernel variants have no sm_90a kernel yet")
+        if nonlinear_activation is not None or freq_axis_kernel_size != 1:
+            raise PwgbError("UpsampleNetwork: nonlinear / freq-axis-kernel variants have no sm_90a kernel yet")
         self.use_causal_conv = use_causal_conv
         self.upsample_scales = list(upsample_scales)
         self.up_layers = torch.nn.ModuleList()
         for scale in upsample_scales:
             self.up_layers += [Stretch2d(scale, 1, interpolate_mode)]
-            self.up_layers += [Conv2d(1, 1, kernel_size=(1, scale * 2 + 1), padding=(0, scale), bias=False)]
+            padding = (0, scale * 2) if use_causal_conv else (0, scale)
+            self.up_layers += [Conv2d(1, 1, kernel_size=(1, scale * 2 + 1), padding=padding, bias=False)]
 
     def forward(self, c, out_channels=None):
         """(B, C, T') -> (B, C [padded to out_channels], T' * prod(scales))."""
@@ -416,30 +423,32 @@ class UpsampleNetwork(torch.nn.Module):
             if torch.is_grad_enabled() and (c.requires_grad or fir.requires_grad):
                 from .autograd import UpsampleFirFn
 
-                c = UpsampleFirFn.apply(c, fir, s, oc)
+                c = UpsampleFirFn.apply(c, fir, s, oc, self.use_causal_conv)
             else:
-                c = ops.upsample_fir(c, fir, s, out_channels=oc)
+                c = ops.upsample_fir(c, fir, s, out_channels=oc, causal=self.use_causal_conv)
         return c
 
 
 class ConvInUpsampleNetwork(torch.nn.Module):
-    """layers/upsample.py:131-194."""
+    """layers/upsample.py:131-194.  Causal: conv_in has aux_context_window + 1 taps and its last
+    aux_context_window frames are cropped when that is > 0; the FIR stages are causal whenever use_causal_conv is set
+    (with aux_context_window = 0 too, as in the reference, upsample.py:160,193)."""
 
     def __init__(self, upsample_scales, nonlinear_activation=None, nonlinear_activation_params={},
                  interpolate_mode="nearest", freq_axis_kernel_size=1, aux_channels=80, aux_context_window=0,
                  use_causal_conv=False):
         super().__init__()
-        if use_causal_conv:
-            raise PwgbError("ConvInUpsampleNetwork(use_causal_conv=True) has no sm_90a kernel yet")
         self.aux_context_window = aux_context_window
-        self.use_causal_conv = False
-        kernel_size = 2 * aux_context_window + 1
+        self.use_causal_conv = use_causal_conv and aux_context_window > 0  # crop conv_in's tail (the reference's flag)
+        kernel_size = aux_context_window + 1 if use_causal_conv else 2 * aux_context_window + 1
         self.conv_in = Conv1d(aux_channels, aux_channels, kernel_size=kernel_size, bias=False)
         self.upsample = UpsampleNetwork(upsample_scales, nonlinear_activation, nonlinear_activation_params,
                                         interpolate_mode, freq_axis_kernel_size, use_causal_conv)
 
     def forward(self, c, out_channels=None):
         c_ = ops.conv1d(c, effective_weight(self.conv_in), None)  # no padding: input already carries the context
+        if self.use_causal_conv:
+            c_ = c_[:, :, : -self.aux_context_window].contiguous()
         return self.upsample(c_, out_channels=out_channels)
 
 

@@ -822,8 +822,6 @@ class ParallelWaveGANGenerator(_GeneratorBase):
 
         from . import layers as L
 
-        if use_causal_conv:
-            raise PwgbError("ParallelWaveGANGenerator(use_causal_conv=True) has no sm_90a kernel yet")
         self.in_channels = in_channels
         self.out_channels = out_channels
         self.aux_channels = aux_channels
@@ -831,6 +829,8 @@ class ParallelWaveGANGenerator(_GeneratorBase):
         self.layers = layers
         self.stacks = stacks
         self.kernel_size = kernel_size
+        self.dropout = dropout
+        self.use_causal_conv = use_causal_conv
         assert layers % stacks == 0
         layers_per_stack = layers // stacks
         self.first_conv = L.Conv1d1x1(in_channels, residual_channels, bias=True)
@@ -912,8 +912,9 @@ class ParallelWaveGANGenerator(_GeneratorBase):
     def _forward_packed(self, z, c):
         """Inference fast path: the residual stack as fused one-kernel layers on the packed (bf16 hi/lo operand
         layout) residual stream -- pwgb_wnstack_*.  Returns the skip sum (B, S, T) or None when the configuration
-        has no fused kernel (the caller then runs the per-layer fp32 path)."""
-        if c is None:
+        has no fused kernel or dropout applies (train mode, also under no_grad): the caller then runs the per-layer
+        fp32 path."""
+        if c is None or (self.training and self.dropout > 0):
             return None
         l0 = self.conv_layers[0]
         G, R, K = l0.conv.out_channels, l0.conv.in_channels, l0.conv.kernel_size[0]
@@ -921,7 +922,8 @@ class ParallelWaveGANGenerator(_GeneratorBase):
         A = self.aux_channels
         B, _, T = z.shape
         dmax = max(f.dilation for f in self.conv_layers)
-        if c.shape[1] < A or not ops.WnStack.supported(B, T, R, G, S, A, K, dmax):
+        causal = self.use_causal_conv
+        if c.shape[1] < A or not ops.WnStack.supported(B, T, R, G, S, A, K, dmax, causal):
             return None
         cache = self.__dict__.setdefault("_wn_stacks", {})
         key = (B, T, str(z.device))
@@ -929,7 +931,7 @@ class ParallelWaveGANGenerator(_GeneratorBase):
         if st is None:
             if len(cache) >= 4:
                 cache.clear()
-            st = cache[key] = ops.WnStack(B, T, R, G, S, A, K, dmax, z.device)
+            st = cache[key] = ops.WnStack(B, T, R, G, S, A, K, dmax, z.device, causal)
         st.cur = 0
         st.pack_c(c)
         fc = self.first_conv
@@ -942,7 +944,7 @@ class ParallelWaveGANGenerator(_GeneratorBase):
             if ent is None or ent[0] != k:
                 packed, bso = ops.wavenet_packed_weights(effective_weight(f.conv), effective_weight(f.conv1x1_aux), effective_weight(f.conv1x1_skip),
                                                          effective_weight(f.conv1x1_out), f.conv1x1_skip.bias, f.conv1x1_out.bias, A,
-                                                         cache=f._cache, key=k)
+                                                         cache=f._cache, key=k, causal=causal)
             else:
                 packed, bso = ent[1], ent[2]
             st.layer(packed, f.conv.bias, bso, f.dilation, skips, skips_init=(i == 0), write_x=(i < n - 1))
@@ -1054,6 +1056,82 @@ class ParallelWaveGANDiscriminator(torch.nn.Module, _NormMixin):
                 x = ops.conv1d(x, effective_weight(m), m.bias, padding=m.padding[0], dilation=m.dilation[0],
                                post_act="lrelu" if act else None, post_slope=self.slope)
         return x
+
+    def apply_weight_norm(self):
+        def _apply_weight_norm(m):
+            if isinstance(m, (torch.nn.Conv1d, torch.nn.Conv2d)):
+                torch.nn.utils.weight_norm(m)
+
+        self.apply(_apply_weight_norm)
+
+
+class ResidualParallelWaveGANDiscriminator(torch.nn.Module, _NormMixin):
+    """models/parallel_wavegan.py:374-513: LReLU(1x1) -> WaveNet blocks without conditioning -> skip sum * sqrt(1/L)
+    -> LReLU -> 1x1 -> LReLU -> 1x1.  The LeakyReLU after first_conv runs in its epilogue; sqrt(1/L) is folded into
+    the first tail conv (LeakyReLU is positively homogeneous: lrelu(a s) = a lrelu(s) for a > 0)."""
+
+    def __init__(self, in_channels=1, out_channels=1, kernel_size=3, layers=30, stacks=3, residual_channels=64,
+                 gate_channels=128, skip_channels=64, dropout=0.0, bias=True, use_weight_norm=True, use_causal_conv=False,
+                 nonlinear_activation="LeakyReLU", nonlinear_activation_params={"negative_slope": 0.2}):
+        super().__init__()
+        import math
+
+        from . import layers as L
+
+        assert (kernel_size - 1) % 2 == 0, "Not support even number kernel size."
+        self.in_channels = in_channels
+        self.out_channels = out_channels
+        self.layers = layers
+        self.stacks = stacks
+        self.kernel_size = kernel_size
+        assert layers % stacks == 0
+        layers_per_stack = layers // stacks
+        self.slope = activation_slope(nonlinear_activation, nonlinear_activation_params)
+        self.first_conv = torch.nn.Sequential(
+            L.Conv1d1x1(in_channels, residual_channels, bias=True),
+            getattr(torch.nn, nonlinear_activation)(inplace=True, **nonlinear_activation_params),
+        )
+        self.conv_layers = torch.nn.ModuleList()
+        for layer in range(layers):
+            self.conv_layers += [
+                L.WaveNetResidualBlock(
+                    kernel_size=kernel_size, residual_channels=residual_channels, gate_channels=gate_channels,
+                    skip_channels=skip_channels, aux_channels=-1, dilation=2 ** (layer % layers_per_stack), dropout=dropout,
+                    bias=bias, use_causal_conv=use_causal_conv,
+                )
+            ]
+        self.last_conv_layers = torch.nn.ModuleList(
+            [
+                getattr(torch.nn, nonlinear_activation)(inplace=True, **nonlinear_activation_params),
+                L.Conv1d1x1(skip_channels, skip_channels, bias=True),
+                getattr(torch.nn, nonlinear_activation)(inplace=True, **nonlinear_activation_params),
+                L.Conv1d1x1(skip_channels, out_channels, bias=True),
+            ]
+        )
+        self._skip_scale = math.sqrt(1.0 / layers)
+        if use_weight_norm:
+            self.apply_weight_norm()
+
+    def forward(self, x):
+        """(B, in_channels, T) -> (B, out_channels, T)."""
+        fc = self.first_conv[0]
+        x = ops.conv1d(x, effective_weight(fc), fc.bias, post_act="lrelu", post_slope=self.slope)
+        l1, l3 = self.last_conv_layers[1], self.last_conv_layers[3]
+        if torch.is_grad_enabled() and (x.requires_grad or next(self.parameters()).requires_grad):
+            from .autograd import ScaledSumFn
+
+            hs = []
+            for f in self.conv_layers:
+                x, h = f._forward_train(x, None)
+                hs.append(h)
+            h = ops.conv1d(ScaledSumFn.apply(self._skip_scale, *hs), effective_weight(l1), l1.bias, pre_slope=self.slope)
+        else:
+            skips = torch.zeros((x.shape[0], self.conv_layers[0].conv1x1_skip.out_channels, x.shape[2]), device=x.device,
+                                dtype=torch.float32)
+            for f in self.conv_layers:
+                x, _ = f(x, None, skips)
+            h = ops.conv1d(skips, effective_weight(l1) * self._skip_scale, l1.bias, pre_slope=self.slope)
+        return ops.conv1d(h, effective_weight(l3), l3.bias, pre_slope=self.slope)
 
     def apply_weight_norm(self):
         def _apply_weight_norm(m):

@@ -343,9 +343,10 @@ def dropout(x, p, training):
     return dropout_raw(x, p, seed)
 
 
-def upsample_fir(x, fir, scale, out=None, out_channels=None):
+def upsample_fir(x, fir, scale, out=None, out_channels=None, causal=False):
     """One stage of the PWG conditioning upsampler (layers/upsample.py:112-128):
-    nearest repeat x`scale` + (2*scale+1)-tap FIR, zero padded -- pwgb_upsample_fir_forward.
+    nearest repeat x`scale` + (2*scale+1)-tap FIR, zero padded -- pwgb_upsample_fir_forward; ``causal``: the FIR
+    pads 2*scale on the left and the tail is cropped (upsample.py:98-125) -- pwgb_upsample_fir_causal_forward.
     x: (B, C, T) -> (B, C, T*scale); with ``out_channels`` > C the result is written into the
     first C channels of a zero-initialised (B, out_channels, T*scale) tensor (channel padding
     for the tensor-core conditioning contraction)."""
@@ -358,8 +359,10 @@ def upsample_fir(x, fir, scale, out=None, out_channels=None):
     if out is None:
         out = (torch.zeros if oc != Cc else torch.empty)((B, oc, T * scale), device=x.device, dtype=torch.float32)
     prof = _Prof("upsample_fir", 2.0 * B * Cc * T * scale * (2 * scale + 1), 4.0 * (x.numel() + B * Cc * T * scale), f"B{B} C{Cc} T{T} s{scale}")
-    rc = capi.lib().pwgb_upsample_fir_forward(B * Cc, Cc, T, int(scale), _p(x), _p(fir), _p(out), oc * T * scale, _stream())
-    capi.check(rc, "pwgb_upsample_fir_forward")
+    L = capi.lib()
+    fn = L.pwgb_upsample_fir_causal_forward if causal else L.pwgb_upsample_fir_forward
+    rc = fn(B * Cc, Cc, T, int(scale), _p(x), _p(fir), _p(out), oc * T * scale, _stream())
+    capi.check(rc, "pwgb_upsample_fir_causal_forward" if causal else "pwgb_upsample_fir_forward")
     prof.done()
     return out
 
@@ -399,9 +402,10 @@ def invalidate_caches(module):
                     pass
 
 
-def wavenet_layer(x, c, w_conv, b_conv, w_aux, w_skip, b_skip, w_out, b_out, dilation, skips, aux_real, cache=None, key=None):
+def wavenet_layer(x, c, w_conv, b_conv, w_aux, w_skip, b_skip, w_out, b_out, dilation, skips, aux_real, cache=None, key=None,
+                  causal=False):
     """WaveNetResidualBlock.forward (layers/residual_block.py:102-140), in place on ``skips``:
-    returns x_out.  ``c``: (B, aux_pad, T) conditioning, zero-padded to a multiple of 32 channels
+    returns x_out.  ``causal``: the dilated conv only sees samples t - (K-1-j)*dilation (residual_block.py:73-77).  ``c``: (B, aux_pad, T) conditioning, zero-padded to a multiple of 32 channels
     (or None).  Uses the fused tensor-core layer when pwgb_wavenet_supported(), otherwise composes the
     layer from the generic fused conv (gate pre-op, accumulate, residual epilogue)."""
     x = _dev(x, "x")
@@ -411,7 +415,7 @@ def wavenet_layer(x, c, w_conv, b_conv, w_aux, w_skip, b_skip, w_out, b_out, dil
     L = capi.lib()
     aux_pad = 0 if c is None else c.shape[1]
     d = capi.WaveNetDesc(batch=B, t=T, residual_channels=R, gate_channels=G, skip_channels=S, aux_channels=aux_pad,
-                         kernel=K, dilation=int(dilation))
+                         kernel=K, dilation=int(dilation), causal=int(bool(causal)))
     if ENGINE != "simt" and L.pwgb_wavenet_supported(C.byref(d)):
         # ``key`` identifies the leaf parameters the effective weights were derived from (param_key); without
         # it nothing is cached (effective weights are temporaries whose address / version say nothing)
@@ -438,7 +442,7 @@ def wavenet_layer(x, c, w_conv, b_conv, w_aux, w_skip, b_skip, w_out, b_out, dil
         prof.done()
         return x_out
     # generic composition (any channel counts): 4 launches
-    g = conv1d(x, w_conv, b_conv, dilation=dilation, padding=(K - 1) // 2 * dilation)
+    g = conv1d(x, w_conv, b_conv, dilation=dilation, padding=wavenet_padding(K, dilation, causal))
     if c is not None:
         wa = w_aux
         if c.shape[1] != w_aux.shape[1]:  # conditioning stored channel-padded
@@ -448,14 +452,23 @@ def wavenet_layer(x, c, w_conv, b_conv, w_aux, w_skip, b_skip, w_out, b_out, dil
     return conv1d(g, w_out, b_out, pre_gate=True, residual=x, out_scale=0.7071067811865476)
 
 
+def wavenet_padding(K, dilation, causal):
+    """(left, right) zero padding of a WaveNet layer's dilated conv: centred, or all on the left when causal"""
+    return ((K - 1) * dilation, 0) if causal else (K - 1) // 2 * dilation
+
+
+def _wn_halo(K, max_dilation, causal):
+    return (K - 1 if causal else (K - 1) // 2) * int(max_dilation)
+
+
 class WnStack:
     """Packed WaveNet residual stack (pwgb_wnstack_*): the residual stream and the conditioning stay in the
     tensor core's operand layout (bf16 hi/lo) between the fused one-kernel layers.  Holds the two ping-pong
     stream buffers (zero halos, allocated once per (B, T)) and the packed conditioning."""
 
-    def __init__(self, B, T, R, G, S, A, K, max_dilation, device):
+    def __init__(self, B, T, R, G, S, A, K, max_dilation, device, causal=False):
         self.desc = capi.WnStackDesc(batch=B, t=T, residual_channels=R, gate_channels=G, skip_channels=S, aux_channels=A,
-                                     kernel=K, halo=(K - 1) // 2 * int(max_dilation))
+                                     kernel=K, halo=_wn_halo(K, max_dilation, causal), causal=int(bool(causal)))
         L = capi.lib()
         if not L.pwgb_wnstack_supported(C.byref(self.desc)):
             raise PwgbError("wnstack: configuration not supported by the fused tensor-core layer")
@@ -468,9 +481,9 @@ class WnStack:
         self.S, self.A = S, A
 
     @staticmethod
-    def supported(B, T, R, G, S, A, K, max_dilation):
+    def supported(B, T, R, G, S, A, K, max_dilation, causal=False):
         d = capi.WnStackDesc(batch=B, t=T, residual_channels=R, gate_channels=G, skip_channels=S, aux_channels=A, kernel=K,
-                             halo=(K - 1) // 2 * int(max_dilation))
+                             halo=_wn_halo(K, max_dilation, causal), causal=int(bool(causal)))
         return ENGINE != "simt" and bool(capi.lib().pwgb_wnstack_supported(C.byref(d)))
 
     def pack_c(self, c):
@@ -526,7 +539,7 @@ class WnStack:
             self.cur = 1 - self.cur
 
 
-def wavenet_packed_weights(w_conv, w_aux, w_skip, w_out, b_skip, b_out, aux_real, cache=None, key=None):
+def wavenet_packed_weights(w_conv, w_aux, w_skip, w_out, b_skip, b_out, aux_real, cache=None, key=None, causal=False):
     """Operand images of one WaveNet layer (pwgb_wavenet_pack, conditioning weight padded to a multiple of 32
     input channels) + concat(b_skip, b_out); cached under ``key`` (see param_key)."""
     ent = cache.get("wnp") if (cache is not None and key is not None) else None
@@ -535,7 +548,8 @@ def wavenet_packed_weights(w_conv, w_aux, w_skip, w_out, b_skip, b_out, aux_real
     G, R, K = w_conv.shape
     S = w_skip.shape[0]
     aux_pad = (aux_real + 31) // 32 * 32
-    d = capi.WaveNetDesc(batch=1, t=128, residual_channels=R, gate_channels=G, skip_channels=S, aux_channels=aux_pad, kernel=K, dilation=1)
+    d = capi.WaveNetDesc(batch=1, t=128, residual_channels=R, gate_channels=G, skip_channels=S, aux_channels=aux_pad, kernel=K, dilation=1,
+                         causal=int(bool(causal)))
     L = capi.lib()
     nbytes = L.pwgb_wavenet_packed_bytes(C.byref(d))
     if nbytes == 0:
