@@ -305,6 +305,21 @@ PWGB_API int pwgb_wnstack_first_conv(const pwgb_wnstack_desc* d, const float* z,
 PWGB_API int pwgb_wnstack_layer_forward(const pwgb_wnstack_desc* d, int dilation, const void* xpk_in, const void* cpk,
                                const void* packed_w, const float* b_conv, const float* b_skip_out, void* xpk_out,
                                float* skips, int skips_init, void* stream);
+/* Streaming a causal stack chunk by chunk.  A causal layer reads only the (kernel-1)*dilation rows in front of sample 0,
+ * so those rows of its input buffer may hold the previous chunk's last samples instead of zeros: the unchanged layer
+ * then computes the chunk exactly as the whole-signal forward would.  Relaxed contract for such streaming buffers
+ * (causal only): the left halo rows may hold history; the right halo and every row past t stay zero.  Buffers that
+ * are not streamed keep the contract above.
+ * A layer's history h = (kernel-1)*dilation is a state tensor laid out like the stream, [batch][hi|lo][R/8][h][8] bf16
+ * (batch * 2 * residual_channels * h * 2 bytes), all zero for a fresh signal (the whole-signal zero padding).
+ * pwgb_wnstack_carry() runs between layer l and layer l+1, before layer l+1 writes into the buffer layer l read:
+ *   save: rows [t - h_save, t) of xpk_save (layer l's input) -> hist_save; rows before 0 come from the left halo, so
+ *         for t < h_save the previous history shifts through;
+ *   load: hist_load -> rows [-h_load, 0) of xpk_load (layer l+1's input).
+ * The halves touch disjoint memory; either may be absent (h = 0: load only before layer 0, save only after the last
+ * layer).  h_save, h_load <= halo.  A plain copy: deterministic. */
+PWGB_API int pwgb_wnstack_carry(const pwgb_wnstack_desc* d, const void* xpk_save, void* hist_save, int h_save, void* xpk_load,
+                       const void* hist_load, int h_load, void* stream);
 
 /* ------------------------------------------------------------------------
  * One stage of the PWG conditioning upsampler (layers/upsample.py:112-128): nearest repeat
@@ -321,6 +336,12 @@ PWGB_API int pwgb_upsample_fir_forward(int rows, int rows_per_batch, int t_in, i
  * so output frame j only meets input frames j-2, j-1, j.  Same arguments and layout as the centred pair. */
 PWGB_API int pwgb_upsample_fir_causal_forward(int rows, int rows_per_batch, int t_in, int scale, const float* x, const float* fir,
                                      float* y, long long y_batch_stride, void* stream);
+/* The causal stage of a stream: input frames -2 and -1 come from hist_in (rows x 2 fp32, oldest first) instead of zero,
+ * and hist_out (rows x 2, not aliasing hist_in) receives the last two frames of [hist_in | x].  Every output is the same
+ * fp32 expression as in pwgb_upsample_fir_causal_forward, so chunked runs equal the whole-signal stage bit for bit. */
+PWGB_API int pwgb_upsample_fir_causal_stream_forward(int rows, int rows_per_batch, int t_in, int scale, const float* x,
+                                            const float* fir, float* y, long long y_batch_stride, const float* hist_in,
+                                            float* hist_out, void* stream);
 PWGB_API int pwgb_upsample_fir_causal_backward(int rows, int rows_per_batch, int t_in, int scale, const float* x, const float* fir,
                                       const float* gy, long long gy_batch_stride, float* gx, float* dfir, void* stream);
 

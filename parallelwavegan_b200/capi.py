@@ -138,6 +138,8 @@ def lib():
     L.pwgb_wnstack_first_conv.argtypes = [C.POINTER(WnStackDesc), vp, C.c_int, vp, vp, vp, vp]
     L.pwgb_wnstack_layer_forward.restype = C.c_int
     L.pwgb_wnstack_layer_forward.argtypes = [C.POINTER(WnStackDesc), C.c_int, vp, vp, vp, vp, vp, vp, vp, C.c_int, vp]
+    L.pwgb_wnstack_carry.restype = C.c_int
+    L.pwgb_wnstack_carry.argtypes = [C.POINTER(WnStackDesc), vp, vp, C.c_int, vp, vp, C.c_int, vp]
     L.pwgb_collate_crop.restype = C.c_int
     L.pwgb_collate_crop.argtypes = [vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp]
     L.pwgb_prep_features.restype = C.c_int
@@ -154,6 +156,8 @@ def lib():
     for fn in (L.pwgb_upsample_fir_forward, L.pwgb_upsample_fir_causal_forward):
         fn.restype = C.c_int
         fn.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_longlong, vp]
+    L.pwgb_upsample_fir_causal_stream_forward.restype = C.c_int
+    L.pwgb_upsample_fir_causal_stream_forward.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_longlong, vp, vp, vp]
     L.pwgb_mr_stft_loss_workspace.restype = C.c_size_t
     L.pwgb_mr_stft_loss_workspace.argtypes = [C.POINTER(StftDesc), C.c_int]
     L.pwgb_mr_stft_loss_forward.restype = C.c_int
@@ -280,7 +284,8 @@ EXPORTED_SYMBOLS = [
     "pwgb_wavenet_pack", "pwgb_wavenet_layer_forward", "pwgb_upsample_fir_forward", "pwgb_upsample_fir_causal_forward",
     "pwgb_s2d_forward", "pwgb_s2d_backward", "pwgb_mt_clip_coef", "pwgb_mt_adam_step", "pwgb_prep_features", "pwgb_pcm16_forward", "pwgb_collate_crop",
     "pwgb_wnstack_supported", "pwgb_wnstack_x_bytes", "pwgb_wnstack_c_bytes", "pwgb_wnstack_pack_x", "pwgb_wnstack_unpack_x",
-    "pwgb_wnstack_pack_c", "pwgb_wnstack_first_conv", "pwgb_wnstack_layer_forward",
+    "pwgb_wnstack_pack_c", "pwgb_wnstack_first_conv", "pwgb_wnstack_layer_forward", "pwgb_wnstack_carry",
+    "pwgb_upsample_fir_causal_stream_forward",
     "pwgb_mr_stft_loss_workspace", "pwgb_mr_stft_loss_forward", "pwgb_stft_amplitude_forward",
     "pwgb_mel_project_forward", "pwgb_reduce_mean_forward", "pwgb_avg_pool1d_forward",
     "pwgb_conv1d_wgrad_workspace", "pwgb_conv1d_wgrad", "pwgb_conv1d_wgrad_tc_supported",

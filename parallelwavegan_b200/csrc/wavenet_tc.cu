@@ -381,6 +381,24 @@ static int wn_plan(const pwgb_wnstack_desc* d, WnK& p, size_t& smem_bytes) {
   return 1;
 }
 
+// History carry of a streamed causal stack: blockIdx.y is one ([batch][hi|lo][8-channel group]) plane, blockIdx.z picks
+// the half.  z = 0 saves rows [t - h_save, t) of xs (halo-relative) into hs; z = 1 loads hl into rows [-h_load, 0) of
+// xl.  hs / hl are laid out like the stream with h rows per plane, so each row is one 16-byte copy.
+__global__ void wn_carry_kernel(const uint4* __restrict__ xs, uint4* __restrict__ hs, int h_save, uint4* __restrict__ xl,
+                                const uint4* __restrict__ hl, int h_load, int Tp, int halo, int t) {
+  const long long pl = blockIdx.y;
+  const int step = gridDim.x * blockDim.x;
+  if (blockIdx.z == 0) {
+    const uint4* src = xs + pl * Tp + halo + t - h_save;
+    uint4* dst = hs + pl * h_save;
+    for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < h_save; r += step) dst[r] = src[r];
+  } else {
+    const uint4* src = hl + pl * h_load;
+    uint4* dst = xl + pl * Tp + halo - h_load;
+    for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < h_load; r += step) dst[r] = src[r];
+  }
+}
+
 }  // namespace pwgb
 
 using namespace pwgb;
@@ -488,4 +506,27 @@ extern "C" int pwgb_wnstack_layer_forward(const pwgb_wnstack_desc* d, int dilati
   wavenet_fused_kernel<<<(unsigned)grid, WN_THREADS, bytes, (cudaStream_t)stream>>>(
       p, tm_x, tm_c, (const unsigned*)xpk_in, (const unsigned char*)packed_w, b_conv, b_skip_out, (unsigned*)xpk_out, skips);
   return check_launch("wavenet_fused_kernel");
+}
+
+extern "C" int pwgb_wnstack_carry(const pwgb_wnstack_desc* d, const void* xpk_save, void* hist_save, int h_save, void* xpk_load,
+                                  const void* hist_load, int h_load, void* stream) {
+  WnK p;
+  size_t bytes;
+  PWGB_UNSUPPORTED_IF(!wn_plan(d, p, bytes), "wnstack: configuration not supported");
+  PWGB_CHECK_ARG(d->causal, "wnstack_carry: only a causal stack reads its history from the left halo");
+  PWGB_CHECK_ARG(h_save >= 0 && h_save <= d->halo && h_load >= 0 && h_load <= d->halo,
+                 "wnstack_carry: history lengths %d / %d must lie in [0, halo = %d]", h_save, h_load, d->halo);
+  PWGB_CHECK_ARG(!h_save || (xpk_save && hist_save), "wnstack_carry: null save buffer");
+  PWGB_CHECK_ARG(!h_load || (xpk_load && hist_load), "wnstack_carry: null load buffer");
+  PWGB_CHECK_ARG(!((reinterpret_cast<uintptr_t>(xpk_save) | reinterpret_cast<uintptr_t>(hist_save) | reinterpret_cast<uintptr_t>(xpk_load) |
+                    reinterpret_cast<uintptr_t>(hist_load)) & 15),
+                 "wnstack_carry: buffers must be 16-byte aligned");
+  if (p.B == 0 || (h_save == 0 && h_load == 0)) return PWGB_OK;
+  const long long planes = 2LL * p.B * p.ngx;
+  PWGB_UNSUPPORTED_IF(planes > 65535, "wnstack_carry: batch too large");
+  const int hmax = h_save > h_load ? h_save : h_load;
+  const dim3 grid((unsigned)(ceil_div(hmax, 256) < 8 ? ceil_div(hmax, 256) : 8), (unsigned)planes, 2);
+  wn_carry_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const uint4*)xpk_save, (uint4*)hist_save, h_save, (uint4*)xpk_load,
+                                                          (const uint4*)hist_load, h_load, p.Tp, p.halo, p.T);
+  return check_launch("wn_carry_kernel");
 }

@@ -367,6 +367,28 @@ def upsample_fir(x, fir, scale, out=None, out_channels=None, causal=False):
     return out
 
 
+def upsample_fir_causal_stream(x, fir, scale, hist_in, hist_out, out_channels=None):
+    """The causal upsampler stage of a stream (pwgb_upsample_fir_causal_stream_forward): ``upsample_fir(..., causal=True)``
+    with input frames -2 and -1 read from ``hist_in`` (B*C, 2) instead of the zero padding; ``hist_out`` (B*C, 2)
+    receives the last two frames of [hist_in | x].  Bit-identical to the whole-signal stage on the concatenation."""
+    x = _dev(x, "x")
+    fir = _dev(fir, "fir").reshape(-1)
+    hist_in, hist_out = _dev(hist_in, "hist_in"), _dev(hist_out, "hist_out")
+    B, Cc, T = x.shape
+    if fir.numel() != 2 * scale + 1:
+        raise PwgbError("upsample_fir: filter must have 2*scale+1 taps")
+    if tuple(hist_in.shape) != (B * Cc, 2) or tuple(hist_out.shape) != (B * Cc, 2):
+        raise PwgbError(f"upsample_fir_causal_stream: histories must be ({B * Cc}, 2)")
+    oc = Cc if out_channels is None else int(out_channels)
+    out = (torch.zeros if oc != Cc else torch.empty)((B, oc, T * scale), device=x.device, dtype=torch.float32)
+    prof = _Prof("upsample_fir", 2.0 * B * Cc * T * scale * (2 * scale + 1), 4.0 * (x.numel() + B * Cc * T * scale), f"B{B} C{Cc} T{T} s{scale}")
+    rc = capi.lib().pwgb_upsample_fir_causal_stream_forward(B * Cc, Cc, T, int(scale), _p(x), _p(fir), _p(out), oc * T * scale,
+                                                            _p(hist_in), _p(hist_out), _stream())
+    capi.check(rc, "pwgb_upsample_fir_causal_stream_forward")
+    prof.done()
+    return out
+
+
 class WaveNetLayerWeights:
     """Device-side operand images of one WaveNetResidualBlock for pwgb_wavenet_layer_forward."""
 
@@ -477,6 +499,7 @@ class WnStack:
         self.x = [torch.zeros(nx // 4, device=device, dtype=torch.int32) for _ in range(2)]  # zero halos: written once
         self.c = torch.empty(nc // 4, device=device, dtype=torch.int32)
         self.cur = 0
+        self.prev = None  # the buffer the last layer() read
         self.shape = (B, R, T)
         self.S, self.A = S, A
 
@@ -535,8 +558,29 @@ class WnStack:
                                                    _p(b_conv), _p(b_skip_out), _p(nxt), _p(skips), int(bool(skips_init)), _stream())
         capi.check(rc, "pwgb_wnstack_layer_forward")
         prof.done()
+        self.prev = self.x[self.cur]
         if write_x:
             self.cur = 1 - self.cur
+
+    def hist_numel(self, h):
+        """int32 elements of one layer's history state of ``h`` rows ([B][hi|lo][R/8][h][8] bf16)"""
+        B, R, _ = self.shape
+        return B * R * h
+
+    def carry(self, save=None, load=None):
+        """History carry of a streamed causal stack (pwgb_wnstack_carry).  ``save`` = (hist, h): rows [t - h, t) of the
+        buffer the last layer() read -> hist; ``load`` = (hist, h): hist -> the h rows in front of sample 0 of the
+        current buffer (the next layer's input).  Run it before the next layer() writes into the buffer that was read."""
+        hs, ns = save if save is not None else (None, 0)
+        hl, nl = load if load is not None else (None, 0)
+        for h, n in ((hs, ns), (hl, nl)):
+            if h is not None and (not h.is_cuda or h.dtype != torch.int32 or not h.is_contiguous() or h.numel() != self.hist_numel(n)):
+                raise PwgbError(f"wnstack.carry: a history of {n} rows must be a contiguous int32 CUDA tensor of {self.hist_numel(n)} elements")
+        if ns and self.prev is None:
+            raise PwgbError("wnstack.carry: nothing to save before the first layer")
+        rc = capi.lib().pwgb_wnstack_carry(C.byref(self.desc), _p(self.prev) if ns else None, _p(hs), int(ns),
+                                           _p(self.x[self.cur]) if nl else None, _p(hl), int(nl), _stream())
+        capi.check(rc, "pwgb_wnstack_carry")
 
 
 def wavenet_packed_weights(w_conv, w_aux, w_skip, w_out, b_skip, b_out, aux_real, cache=None, key=None, causal=False):
