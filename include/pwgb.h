@@ -41,7 +41,8 @@ typedef enum pwgb_status {
   PWGB_CUDA_ERROR = -3   /* launch failed; message holds cudaGetErrorString */
 } pwgb_status;
 
-enum { PWGB_PAD_ZERO = 0, PWGB_PAD_REFLECT = 1, PWGB_PAD_REPLICATE = 2 };
+/* PWGB_PAD_HISTORY: rows before sample 0 come from a caller-owned history (the stream entry points only) */
+enum { PWGB_PAD_ZERO = 0, PWGB_PAD_REFLECT = 1, PWGB_PAD_REPLICATE = 2, PWGB_PAD_HISTORY = 3 };
 enum { PWGB_ACT_NONE = 0, PWGB_ACT_TANH = 1, PWGB_ACT_LRELU = 2 };
 
 PWGB_API const char* pwgb_last_error(void);
@@ -158,6 +159,42 @@ PWGB_API int pwgb_conv1d_tc_pack_weight_grouped(const float* w, int cin_per_grou
 PWGB_API int pwgb_conv1d_tc_supported(const pwgb_conv1d_desc* d);
 PWGB_API int pwgb_conv1d_tc_forward(const pwgb_conv1d_desc* d, const float* x, const void* packed_w, const float* bias,
                            const float* residual, float* y, void* stream);
+
+/* ------------------------------------------------------------------------
+ * Streaming a causal conv stack chunk by chunk (layers/causal_conv.py under a chunked driver): history padding.
+ * pwgb_conv1d_stream_forward (FFMA) and pwgb_conv1d_tc_stream_forward (tensor cores, packed weights as for
+ * pwgb_conv1d_tc_forward) compute pwgb_conv1d_forward / pwgb_conv1d_tc_forward in every respect (pre-activation,
+ * epilogue, residual, out_scale, accumulate) except for the input rows t < 0 in front of sample 0:
+ *   t in [-hist_len, 0): hist[b, c, hist_len + t], hist (batch, cin, hist_len) fp32; or x[b, c, 0] where replicate[b] != 0
+ *                        (replicate: DEVICE array of batch int32, or NULL) -- ReplicationPad1d for a fresh signal;
+ *   t < -hist_len:       zero.
+ * History rows are input rows: the pre-activation applies to them.  d->pad_mode must be PWGB_PAD_HISTORY (accepted by
+ * these entry points only) with d->pad_left the conv's left padding; the scope is stride 1, groups 1, period 1, no
+ * pre_gate, one source (anything else: PWGB_INVALID or PWGB_UNSUPPORTED).  pwgb_conv1d_tc_supported() answers for such a
+ * descriptor as for any other.  The FFMA entry always runs the generic kernel, whose sum order does not depend on
+ * where a sample sits, so a chunked run is bit-identical to the whole-signal conv on cat(hist, x) when that takes the same
+ * kernel.  On the tensor cores the history launch stages activations with per-element copies (never TMA rows); the sum
+ * order is the same as for the other plans.
+ * ---------------------------------------------------------------------- */
+PWGB_API int pwgb_conv1d_stream_forward(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len,
+                                        const int* replicate, const float* w, const float* bias, const float* residual,
+                                        float* y, void* stream);
+PWGB_API int pwgb_conv1d_tc_stream_forward(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len,
+                                           const int* replicate, const void* packed_w, const float* bias,
+                                           const float* residual, float* y, void* stream);
+/* The causal conv-transpose of a stream (CausalConvTranspose1d, layers/causal_conv.py:46-79, with its one-frame
+ * ReplicationPad1d): d describes the conv-transpose on cat(h, x) along time, so d->t_in = frames of x + 1 and
+ * d->padding == d->stride (dense, plain); h[b] = replicate[b] ? x[b, :, 0] : hist[b, :, 0], hist (batch, cin, 1).  The
+ * result is bit-identical to pwgb_conv_transpose1d_forward(d) on that concatenation, which is never materialised.  ws:
+ * pwgb_conv_transpose1d_workspace(d) bytes. */
+PWGB_API int pwgb_conv_transpose1d_stream_forward(const pwgb_convtr1d_desc* d, const float* x, const float* hist,
+                                                  const int* replicate, const float* w, const float* bias, float* y, void* ws,
+                                                  size_t ws_bytes, void* stream);
+/* History carry of a stream, many signals in one launch.  table: DEVICE array of n_entries rows {x*, hist*, rows, n, H}
+ * (5 x int64): x (rows, n) fp32 is this chunk of a signal, hist (rows, H) fp32 its history; afterwards hist holds the
+ * last H samples of [hist | x] per row (also for n < H).  Every read of an entry happens before that entry's writes;
+ * entries must not overlap each other.  A plain copy: deterministic. */
+PWGB_API int pwgb_stream_carry(const void* table, int n_entries, void* stream);
 
 /* ------------------------------------------------------------------------
  * One HiFi-GAN ResBlock conv pair (layers/residual_block.py:243-258, non-causal, additional convs) in one

@@ -10,6 +10,8 @@ namespace pwgb {
 
 void set_error(const char* fmt, ...);
 void count_launch(int n = 1);
+// argument check shared by the two history conv entry points (api.cu)
+int conv1d_stream_check(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len, const float* y);
 
 #define PWGB_CHECK_ARG(cond, ...)          \
   do {                                     \

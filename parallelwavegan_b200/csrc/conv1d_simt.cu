@@ -34,13 +34,19 @@ struct ConvK {
   int shuffle, shuffle_pad, shuffle_tout;
   long long xbs, ybs, rbs, xcs;
   int CI_T, XW, tiles_per_group;
+  // history launches: input rows [-hist_len, 0) come from hist (B, Cin, hist_len), or from sample 0 of x for an item whose
+  // rep flag is set
+  const float* hist;
+  const int* rep;
+  int hist_len;
 };
 
-template <int RCO, int WARPS_CO, int RT>
-__global__ void __launch_bounds__(256) conv1d_fwd_kernel(const ConvK p, const float* __restrict__ x,
-                                                          const float* __restrict__ w,
-                                                          const float* __restrict__ bias,
-                                                          const float* __restrict__ res, float* __restrict__ y) {
+// HIST: the history padding policy (pwgb_conv1d_stream_forward, groups 1, period 1) in the input staging loop; a template
+// argument so that the kernels without it keep their code and registers
+template <int RCO, int WARPS_CO, int RT, bool HIST>
+__global__ void __launch_bounds__(256) conv1d_fwd_kernel(const ConvK p, const float* __restrict__ x, const float* __restrict__ w,
+                                                const float* __restrict__ bias, const float* __restrict__ res,
+                                                float* __restrict__ y) {
   constexpr int WARPS_T = 8 / WARPS_CO;
   constexpr int CO_T = RCO * WARPS_CO;
   constexpr int TT = WARPS_T * 32 * RT;
@@ -92,6 +98,18 @@ __global__ void __launch_bounds__(256) conv1d_fwd_kernel(const ConvK p, const fl
       int r = idx - ci * p.XW;
       long long li = row0 * p.P + r;
       float v = 0.f;
+      if constexpr (HIST) {
+        // rows [-hist_len, 0) from the history (or sample 0 of a replicated item), earlier rows and rows past the input zero
+        const int ch = ci0 + ci;
+        const float* src = nullptr;
+        if (li >= 0 && li < p.Lin)
+          src = xb + (long long)ch * p.xcs + li;
+        else if (li < 0 && li >= -p.hist_len)
+          src = p.rep && p.rep[b] ? xb + (long long)ch * p.xcs : p.hist + ((long long)b * p.Cin + ch) * p.hist_len + (p.hist_len + li);
+        if (src) v = lrelu(__ldg(src), p.pre_slope);
+        xs[idx] = v;
+        continue;
+      }
       bool ok = true;
       if (li < 0 || li >= p.Lin) {
         if (p.pad_mode == PWGB_PAD_ZERO) {
@@ -196,7 +214,7 @@ __global__ void __launch_bounds__(256) conv1d_fwd_kernel(const ConvK p, const fl
   }
 }
 
-template <int RCO, int WARPS_CO, int RT>
+template <int RCO, int WARPS_CO, int RT, bool HIST>
 static int launch_conv_rt(ConvK p, const float* x, const float* w, const float* bias, const float* res, float* y,
                        cudaStream_t st) {
   constexpr int WARPS_T = 8 / WARPS_CO;
@@ -220,7 +238,7 @@ static int launch_conv_rt(ConvK p, const float* x, const float* w, const float* 
   p.CI_T = ci_t;
   p.XW = (int)XW;
   p.tiles_per_group = ceil_div(p.Cout_g, CO_T);
-  auto kern = conv1d_fwd_kernel<RCO, WARPS_CO, RT>;
+  auto kern = conv1d_fwd_kernel<RCO, WARPS_CO, RT, HIST>;
   if (bytes > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (e != cudaSuccess) {
@@ -380,17 +398,18 @@ __global__ void __launch_bounds__(256) conv1d_fewcout_long_kernel(const ConvK p,
 }
 
 // short sequences (discriminator tails, 10-50 positions per item): 1 position per lane instead of 4
-template <int RCO, int WARPS_CO>
+template <int RCO, int WARPS_CO, bool HIST = false>
 static int launch_conv(ConvK p, const float* x, const float* w, const float* bias, const float* res, float* y,
                        cudaStream_t st) {
   constexpr int WARPS_T = 8 / WARPS_CO;
-  if (p.Lout <= 40 * WARPS_T) return launch_conv_rt<RCO, WARPS_CO, 1>(p, x, w, bias, res, y, st);
-  return launch_conv_rt<RCO, WARPS_CO, 4>(p, x, w, bias, res, y, st);
+  if (p.Lout <= 40 * WARPS_T) return launch_conv_rt<RCO, WARPS_CO, 1, HIST>(p, x, w, bias, res, y, st);
+  return launch_conv_rt<RCO, WARPS_CO, 4, HIST>(p, x, w, bias, res, y, st);
 }
 
-int conv1d_forward_simt(const pwgb_conv1d_desc* d, const float* x, const float* w, const float* bias,
-                        const float* residual, float* y, cudaStream_t st) {
-  ConvK p;
+static void conv_params(const pwgb_conv1d_desc* d, ConvK& p) {
+  p.hist = nullptr;
+  p.rep = nullptr;
+  p.hist_len = 0;
   p.B = d->batch;
   p.Cin = d->cin;
   p.Cout = d->cout;
@@ -423,6 +442,12 @@ int conv1d_forward_simt(const pwgb_conv1d_desc* d, const float* x, const float* 
   const long long ylen = d->shuffle > 1 ? (long long)(d->cout / d->shuffle) * d->shuffle_tout * p.P : (long long)d->cout * p.Lout;
   p.ybs = d->y_batch_stride ? d->y_batch_stride : ylen;
   p.rbs = d->r_batch_stride ? d->r_batch_stride : (long long)d->cout * p.Lout;
+}
+
+int conv1d_forward_simt(const pwgb_conv1d_desc* d, const float* x, const float* w, const float* bias,
+                        const float* residual, float* y, cudaStream_t st) {
+  ConvK p;
+  conv_params(d, p);
   if (p.B == 0 || p.Lout == 0) return PWGB_OK;
   if (p.Cout <= 4 && p.groups == 1 && p.Cin >= 64 && p.pad_mode == PWGB_PAD_ZERO && !p.pre_gate && !residual &&
       !p.accumulate && p.shuffle <= 1 && (long long)p.Lout * p.B <= 65536 && p.B <= 65535) {
@@ -452,6 +477,25 @@ int conv1d_forward_simt(const pwgb_conv1d_desc* d, const float* x, const float* 
   if (cg >= 8) return launch_conv<8, 1>(p, x, w, bias, residual, y, st);
   if (cg >= 4) return launch_conv<4, 1>(p, x, w, bias, residual, y, st);
   return launch_conv<1, 1>(p, x, w, bias, residual, y, st);
+}
+
+// History launches (pad_mode PWGB_PAD_HISTORY, groups 1, period 1) always take the generic kernel: the few-channel
+// kernels above sum in an order that depends on where a sample sits in the sequence, which a stream cannot reproduce.
+int conv1d_stream_simt(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len, const int* rep,
+                       const float* w, const float* bias, const float* residual, float* y, cudaStream_t st) {
+  ConvK p;
+  conv_params(d, p);
+  p.hist = hist;
+  p.rep = rep;
+  p.hist_len = hist_len;
+  if (p.B == 0 || p.Lout == 0) return PWGB_OK;
+  const int cg = p.Cout_g;
+  if (cg >= 64) return launch_conv<8, 8, true>(p, x, w, bias, residual, y, st);
+  if (cg >= 32) return launch_conv<8, 4, true>(p, x, w, bias, residual, y, st);
+  if (cg >= 16) return launch_conv<8, 2, true>(p, x, w, bias, residual, y, st);
+  if (cg >= 8) return launch_conv<8, 1, true>(p, x, w, bias, residual, y, st);
+  if (cg >= 4) return launch_conv<4, 1, true>(p, x, w, bias, residual, y, st);
+  return launch_conv<1, 1, true>(p, x, w, bias, residual, y, st);
 }
 
 }  // namespace pwgb

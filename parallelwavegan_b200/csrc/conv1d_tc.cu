@@ -66,6 +66,11 @@ struct TcK {
   int variant;           // debug (pwgb_debug_set(1, v)): bit 1 stages activations with cp.async instead of TMA,
                          // bit 2 keeps the register epilogue
   int staged;            // plain epilogue through a shared-memory tile per consumer warpgroup (tc_plan)
+  // history launches (conv1d_tc_hist_kernel, pad_mode PWGB_PAD_HISTORY): input rows [-hist_len, 0) come from hist
+  // (B, Cin, hist_len), or from sample 0 of x for an item whose rep flag is set
+  const float* hist;
+  const int* rep;
+  int hist_len;
 };
 
 // Staged epilogue: one tile (fp32 [col][stage_ld(MT)], tc_common.cuh) per consumer warpgroup.  Tile shapes compiled with
@@ -182,14 +187,16 @@ __device__ __forceinline__ void tile_origin(const TcK& p, int tile, int TT, int&
 
 // Input sample of operand row r of a main chunk in the tile starting at t0: the row's window and tap (win_mode) or its
 // place in the contiguous halo tile, then the padding policy.  ok = false: a zero-padding row.
-__device__ __forceinline__ long long src_sample(const TcK& p, int t0, int TT, int r, bool& ok) {
-  long long ts;
+__device__ __forceinline__ long long tile_sample(const TcK& p, int t0, int TT, int r) {
   if (p.win_mode) {
     const int k = r / TT;
-    ts = (long long)t0 - p.padL + (long long)k * p.D + (r - k * TT);
-  } else {
-    ts = (long long)t0 - p.padL + r;
+    return (long long)t0 - p.padL + (long long)k * p.D + (r - k * TT);
   }
+  return (long long)t0 - p.padL + r;
+}
+
+__device__ __forceinline__ long long src_sample(const TcK& p, int t0, int TT, int r, bool& ok) {
+  long long ts = tile_sample(p, t0, TT, r);
   ok = true;
   if (ts < 0 || ts >= p.T_in) {
     if (p.pad_mode == PWGB_PAD_ZERO) {
@@ -204,9 +211,27 @@ __device__ __forceinline__ long long src_sample(const TcK& p, int t0, int TT, in
   return ts;
 }
 
-// stage one activation chunk (KC channels x R rows) into the operand layout
+// The history padding policy (one more policy of src_sample, for history launches): the source of operand row r of main
+// chunk c of batch item b.  Rows [-hist_len, 0) read hist[b, c * KC + j, hist_len + ts], or x[b, c * KC + j, 0] when the
+// item's rep flag is set; rows before -hist_len and from T_in on are zero padding (ok = false).  Returns channel j = 0's
+// sample; ld: the channel stride.
+__device__ __forceinline__ const float* hist_sample(const TcK& p, const float* xc, int b, int c, int t0, int TT, int r, bool& ok,
+                                                    long long& ld) {
+  const long long ts = tile_sample(p, t0, TT, r);
+  ld = p.T_in;
+  ok = ts >= -p.hist_len && ts < p.T_in;
+  if (!ok) return xc;
+  if (ts >= 0) return xc + ts;
+  if (p.rep && p.rep[b]) return xc;
+  ld = p.hist_len;
+  return p.hist + ((long long)b * p.Cin + (long long)c * KC) * p.hist_len + (p.hist_len + ts);
+}
+
+// stage one activation chunk (KC channels x R rows) into the operand layout; HIST: with the history padding policy
+// (chunk c of batch item b)
+template <bool HIST>
 __device__ __forceinline__ void fill_main_chunk(const TcK& p, const float* __restrict__ xc, int t0, int TT,
-                                                unsigned char* dst, int tid) {
+                                                unsigned char* dst, int tid, int b, int c) {
   auto store_row = [&](const float (&v)[KC], int r) {
 #pragma unroll
     for (int g = 0; g < KC / 8; ++g) {
@@ -216,7 +241,7 @@ __device__ __forceinline__ void fill_main_chunk(const TcK& p, const float* __res
       store_split8(dst, p.R, r, g, u);
     }
   };
-  if (p.pre_gate) {
+  if (!HIST && p.pre_gate) {
     const float* xg = xc + (long long)p.Cin * p.T_in;
     for (int r = tid; r < p.R; r += NPROD) {
       bool ok;
@@ -235,10 +260,17 @@ __device__ __forceinline__ void fill_main_chunk(const TcK& p, const float* __res
   }
   for (int r = tid; r < p.R; r += NPROD) {
     bool ok;
-    const long long ts = src_sample(p, t0, TT, r, ok);
     float v[KC];
+    if constexpr (HIST) {
+      long long ld;
+      const float* s = hist_sample(p, xc, b, c, t0, TT, r, ok, ld);
 #pragma unroll
-    for (int j = 0; j < KC; ++j) v[j] = ok ? __ldg(xc + (long long)j * p.T_in + ts) : 0.f;
+      for (int j = 0; j < KC; ++j) v[j] = ok ? __ldg(s + (long long)j * ld) : 0.f;
+    } else {
+      const long long ts = src_sample(p, t0, TT, r, ok);
+#pragma unroll
+      for (int j = 0; j < KC; ++j) v[j] = ok ? __ldg(xc + (long long)j * p.T_in + ts) : 0.f;
+    }
 #pragma unroll
     for (int j = 0; j < KC; ++j) v[j] = lrelu(v[j], p.pre_slope);
     store_row(v, r);
@@ -246,12 +278,13 @@ __device__ __forceinline__ void fill_main_chunk(const TcK& p, const float* __res
 }
 
 // MT (64-row blocks per warpgroup) and NB16 (16-column blocks, Cout = 16 * NB16) are compile-time constants, so the
-// consumers issue a fixed wgmma sequence into fixed accumulator registers (tc_launch picks the instantiation).
-template <int MT, int NB16>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-    conv1d_tc_kernel(const TcK p, const float* __restrict__ x, const float* __restrict__ x2,
-                     const uint4* __restrict__ wpk, const float* __restrict__ bias, const float* __restrict__ res,
-                     float* __restrict__ y, float* __restrict__ y2) {
+// consumers issue a fixed wgmma sequence into fixed accumulator registers (tc_launch picks the instantiation).  HIST: the
+// history padding policy on the element-addressed producers (cp.async-staged and direct; history launches never take
+// the TMA activation path).  It is a template argument so that the kernels without it keep their code.
+template <int MT, int NB16, bool HIST>
+__device__ __forceinline__ void conv1d_tc_body(const TcK& p, const float* __restrict__ x, const float* __restrict__ x2,
+                                               const uint4* __restrict__ wpk, const float* __restrict__ bias,
+                                               const float* __restrict__ res, float* __restrict__ y, float* __restrict__ y2) {
   extern __shared__ __align__(128) unsigned char smem[];
   // layout: A[na] | B[nb] | raw staging[ns] | epilogue tiles[2 if staged] | barriers | bias
   constexpr int SLD = stage_ld(MT);
@@ -303,7 +336,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     bias_s[i] = bias ? __ldg(bias + (p.shuffle > 1 ? (p.co_off + i) / p.shuffle : p.co_off + i)) : 0.f;
   __syncthreads();
 
-  if (warp < W_CONS0 && p.tma_act) {
+  if (warp < W_CONS0 && !HIST && p.tma_act) {
     // ===================== A producers, TMA-staged =====================
     // Warp W_LDA streams the raw fp32 rows of chunk q + ns - 1 into shared memory with bulk copies
     // (no LSU instructions, no registers); these 8 warps only convert landed stages to the bf16 hi/lo
@@ -349,13 +382,23 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         const float* xc = main_src(p, x, x2, b, c, MC ? (long long)((tile / pct) / p.cpg) * p.xgs : 0);
         for (int r = tid; r < p.R; r += NPROD) {
           bool ok;
-          const long long ts = src_sample(p, t0, TT, r, ok);
-          const float* src = ok ? xc + ts : xc;
-          const unsigned nbytes = ok ? 4u : 0u;
-          unsigned dq = raw + (unsigned)r * 4u;
-          const unsigned dstep = (unsigned)p.R * 4u;
+          if constexpr (HIST) {
+            long long ld;
+            const float* src = hist_sample(p, xc, b, c, t0, TT, r, ok, ld);
+            const unsigned nbytes = ok ? 4u : 0u;
+            unsigned dq = raw + (unsigned)r * 4u;
+            const unsigned dstep = (unsigned)p.R * 4u;
 #pragma unroll 8
-          for (int j = 0; j < KC; ++j, src += p.T_in, dq += dstep) cp_async4(dq, src, nbytes);
+            for (int j = 0; j < KC; ++j, src += ld, dq += dstep) cp_async4(dq, src, nbytes);
+          } else {
+            const long long ts = src_sample(p, t0, TT, r, ok);
+            const float* src = ok ? xc + ts : xc;
+            const unsigned nbytes = ok ? 4u : 0u;
+            unsigned dq = raw + (unsigned)r * 4u;
+            const unsigned dstep = (unsigned)p.R * 4u;
+#pragma unroll 8
+            for (int j = 0; j < KC; ++j, src += p.T_in, dq += dstep) cp_async4(dq, src, nbytes);
+          }
         }
       } else {
         const float* xc = x2 + ((long long)b * p.C2 + (long long)(c - p.nchunks) * KC) * p.T_out;
@@ -405,7 +448,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         mbar_wait(A_EMPTY(buf), ((ca / p.na) & 1) ^ 1);
         unsigned char* dst = a_buf + (size_t)buf * p.a_bytes;
         if (c < p.nchunks) {
-          fill_main_chunk(p, xb + (long long)(c * KC) * p.T_in, t0, TT, dst, tid);
+          fill_main_chunk<HIST>(p, xb + (long long)(c * KC) * p.T_in, t0, TT, dst, tid, b, c);
         } else {
           // auxiliary 1x1 source: TT rows aligned with the output tile, no padding shift, no activation
           const float* xc = x2 + ((long long)b * p.C2 + (long long)(c - p.nchunks) * KC) * p.T_out;
@@ -568,7 +611,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     }
   } else if (warp == W_LDA) {
     // ===================== raw activation loader (TMA bulk row copies) =====================
-    if (p.tma_act) {
+    if (!HIST && p.tma_act) {
       int s = 0, ph = 0;
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
         int b, t0;
@@ -601,6 +644,23 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   }
 }
 
+template <int MT, int NB16>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+    conv1d_tc_kernel(const TcK p, const float* __restrict__ x, const float* __restrict__ x2,
+                     const uint4* __restrict__ wpk, const float* __restrict__ bias, const float* __restrict__ res,
+                     float* __restrict__ y, float* __restrict__ y2) {
+  conv1d_tc_body<MT, NB16, false>(p, x, x2, wpk, bias, res, y, y2);
+}
+
+// history launches (pwgb_conv1d_tc_stream_forward, the causal conv-transpose of a stream): x2 is unused
+template <int MT, int NB16>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+    conv1d_tc_hist_kernel(const TcK p, const float* __restrict__ x, const float* __restrict__ x2,
+                          const uint4* __restrict__ wpk, const float* __restrict__ bias, const float* __restrict__ res,
+                          float* __restrict__ y, float* __restrict__ y2) {
+  conv1d_tc_body<MT, NB16, true>(p, x, x2, wpk, bias, res, y, y2);
+}
+
 static int g_tc_variant = 0;
 // the plan of the last conv1d_tc_kernel launch, for pwgb_debug_get(1, ...); the first five fields are the original
 // readout, so a caller that asks for five ints keeps working
@@ -621,6 +681,9 @@ static WtPlanInfo g_wt_last = {};
 static int tc_plan(const pwgb_conv1d_desc* d, TcK& p, size_t& smem_bytes, int aux_c2 = 0, int split = 0, int nco_bias = 1,
                    int has_res = 0) {
   p.variant = g_tc_variant;
+  p.hist = nullptr;
+  p.rep = nullptr;
+  p.hist_len = 0;
   p.co_off = 0;
   p.nco = 1;
   p.cpg = 1;
@@ -750,11 +813,16 @@ static const TcKernel tc_kernels[12] = {conv1d_tc_kernel<1, 1>, conv1d_tc_kernel
                                         conv1d_tc_kernel<1, 4>, conv1d_tc_kernel<1, 5>, conv1d_tc_kernel<1, 6>,
                                         conv1d_tc_kernel<1, 7>, conv1d_tc_kernel<1, 8>, conv1d_tc_kernel<2, 1>,
                                         conv1d_tc_kernel<2, 2>, conv1d_tc_kernel<2, 3>, conv1d_tc_kernel<2, 4>};
-static TcKernel tc_kernel_for(int mt, int cout) {
+static const TcKernel tc_hist_kernels[12] = {
+    conv1d_tc_hist_kernel<1, 1>, conv1d_tc_hist_kernel<1, 2>, conv1d_tc_hist_kernel<1, 3>, conv1d_tc_hist_kernel<1, 4>,
+    conv1d_tc_hist_kernel<1, 5>, conv1d_tc_hist_kernel<1, 6>, conv1d_tc_hist_kernel<1, 7>, conv1d_tc_hist_kernel<1, 8>,
+    conv1d_tc_hist_kernel<2, 1>, conv1d_tc_hist_kernel<2, 2>, conv1d_tc_hist_kernel<2, 3>, conv1d_tc_hist_kernel<2, 4>};
+static TcKernel tc_kernel_for(int mt, int cout, bool hist) {
   if (cout % 16 != 0) return nullptr;
+  const TcKernel* table = hist ? tc_hist_kernels : tc_kernels;
   const int nb16 = cout / 16;
-  if (mt == 1 && nb16 >= 1 && nb16 <= 8) return tc_kernels[nb16 - 1];
-  if (mt == 2 && nb16 >= 1 && nb16 <= 4) return tc_kernels[8 + nb16 - 1];
+  if (mt == 1 && nb16 >= 1 && nb16 <= 8) return table[nb16 - 1];
+  if (mt == 2 && nb16 >= 1 && nb16 <= 4) return table[8 + nb16 - 1];
   return nullptr;
 }
 
@@ -762,13 +830,16 @@ static int tc_launch(TcK& p, size_t bytes, const float* x, const void* packed_w,
                      const float* residual, float* y, cudaStream_t st, const float* x2 = nullptr,
                      float* y2 = nullptr) {
   if (p.B == 0 || p.T_out == 0) return PWGB_OK;
-  const TcKernel kernel = tc_kernel_for(p.MT, p.Cout);
+  const bool hist = p.pad_mode == PWGB_PAD_HISTORY;
+  const TcKernel kernel = tc_kernel_for(p.MT, p.Cout, hist);
   if (!kernel) {
     set_error("conv1d_tc: no kernel instantiation for MT = %d, Cout = %d", p.MT, p.Cout);
     return PWGB_UNSUPPORTED;
   }
-  static bool smem_set = false;
-  if (const int rc = smem_opt_in(smem_set, tc_kernels, (int)TC_SMEM_STAGED, "conv1d_tc")) return rc;
+  static bool smem_set = false, smem_set_hist = false;
+  if (const int rc = hist ? smem_opt_in(smem_set_hist, tc_hist_kernels, (int)TC_SMEM_STAGED, "conv1d_tc")
+                          : smem_opt_in(smem_set, tc_kernels, (int)TC_SMEM_STAGED, "conv1d_tc"))
+    return rc;
   const int num_sms = tc_num_sms();
   if ((long long)p.B * p.tiles_per_seq > 0x7fffffffLL) {
     set_error("conv1d_tc: too many tiles");
@@ -786,12 +857,20 @@ static int tc_launch(TcK& p, size_t bytes, const float* x, const void* packed_w,
 
 // Internal entry for N-chunked callers (conv_transpose): runs output channels
 // [co_off, co_off + d->cout) of a conv whose full output has cout_total channels.  cin1 > 0: the input is
-// cat(x (B, cin1, T), x2 (B, d->cin - cin1, T)) along channels (cin1 a multiple of KC).
+// cat(x (B, cin1, T), x2 (B, d->cin - cin1, T)) along channels (cin1 a multiple of KC).  d->pad_mode ==
+// PWGB_PAD_HISTORY: a history launch reading rows before sample 0 from hist / rep (one source only).
 int conv1d_tc_chunk(const pwgb_conv1d_desc* d, int co_off, int cout_total, const float* x, const void* packed_w,
-                    const float* bias, float* y, cudaStream_t st, int nco, const float* x2, int cin1) {
+                    const float* bias, float* y, cudaStream_t st, int nco, const float* x2, int cin1, const float* hist,
+                    const int* rep, int hist_len) {
   TcK p;
   size_t bytes = 0;
   if (!tc_plan(d, p, bytes)) return PWGB_UNSUPPORTED;
+  if (d->pad_mode == PWGB_PAD_HISTORY) {
+    if (cin1 > 0) return PWGB_UNSUPPORTED;
+    p.hist = hist;
+    p.rep = rep;
+    p.hist_len = hist_len;
+  }
   if (cin1 > 0) {
     // the direct register path (ns == 0) reads one source
     if (!x2 || cin1 % KC || cin1 >= d->cin || p.ns == 0) return PWGB_UNSUPPORTED;
@@ -897,6 +976,8 @@ static int tc_cout_chunk(int cout) {
 // channel slice (pointer offsets, batch strides of the full tensors).
 extern "C" int pwgb_conv1d_tc_supported(const pwgb_conv1d_desc* d) {
   if (!d || d->cout <= 0 || d->groups <= 0 || d->cin % d->groups || d->cout % d->groups) return 0;
+  // history padding: plain dense convs only (pwgb_conv1d_tc_stream_forward)
+  if (d->pad_mode == PWGB_PAD_HISTORY && (d->groups != 1 || d->pre_gate || d->shuffle > 1)) return 0;
   const int G = d->groups;
   if (G > 1 && (d->shuffle > 1 || d->pre_gate || G > 64)) return 0;
   const int chunk = tc_cout_chunk(d->cout / G);
@@ -911,9 +992,8 @@ extern "C" int pwgb_conv1d_tc_supported(const pwgb_conv1d_desc* d) {
   return tc_plan(&c, p, bytes, 0, 0, G * ((d->cout / G) / chunk));
 }
 
-extern "C" int pwgb_conv1d_tc_forward(const pwgb_conv1d_desc* d, const float* x, const void* packed_w,
-                                      const float* bias, const float* residual, float* y, void* stream) {
-  PWGB_CHECK_ARG(d && x && packed_w && y, "conv1d_tc: null argument");
+static int tc_forward(const pwgb_conv1d_desc* d, const float* x, const void* packed_w, const float* bias, const float* residual,
+                      float* y, void* stream, const float* hist, const int* rep, int hist_len) {
   PWGB_UNSUPPORTED_IF(!pwgb_conv1d_tc_supported(d), "conv1d_tc: configuration not supported by the tensor-core path");
   const int G = d->groups, cin_g = d->cin / G, cout_g = d->cout / G;
   const int chunk = tc_cout_chunk(cout_g);
@@ -944,7 +1024,25 @@ extern "C" int pwgb_conv1d_tc_forward(const pwgb_conv1d_desc* d, const float* x,
     p.xgs = G > 1 ? (long long)cin_g * d->t_in : 0;
     p.total_tiles *= nco;
   }
+  p.hist = hist;
+  p.rep = rep;
+  p.hist_len = hist_len;
   return tc_launch(p, bytes, x, packed_w, bias, residual, y, (cudaStream_t)stream);
+}
+
+extern "C" int pwgb_conv1d_tc_forward(const pwgb_conv1d_desc* d, const float* x, const void* packed_w,
+                                      const float* bias, const float* residual, float* y, void* stream) {
+  PWGB_CHECK_ARG(d && x && packed_w && y, "conv1d_tc: null argument");
+  PWGB_CHECK_ARG(d->pad_mode != PWGB_PAD_HISTORY, "conv1d_tc: PWGB_PAD_HISTORY is served by pwgb_conv1d_tc_stream_forward");
+  return tc_forward(d, x, packed_w, bias, residual, y, stream, nullptr, nullptr, 0);
+}
+
+extern "C" int pwgb_conv1d_tc_stream_forward(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len,
+                                             const int* replicate, const void* packed_w, const float* bias, const float* residual,
+                                             float* y, void* stream) {
+  PWGB_CHECK_ARG(packed_w, "conv1d_tc_stream: null argument");
+  if (const int rc = conv1d_stream_check(d, x, hist, hist_len, y)) return rc;
+  return tc_forward(d, x, packed_w, bias, residual, y, stream, hist, replicate, hist_len);
 }
 
 // ======================================================================================

@@ -10,7 +10,10 @@ namespace pwgb {
 int conv1d_forward_simt(const pwgb_conv1d_desc* d, const float* x, const float* w, const float* bias,
                         const float* residual, float* y, cudaStream_t st);
 int conv1d_tc_chunk(const pwgb_conv1d_desc* d, int co_off, int cout_total, const float* x, const void* packed_w,
-                    const float* bias, float* y, cudaStream_t st, int nco, const float* x2 = nullptr, int cin1 = 0);
+                    const float* bias, float* y, cudaStream_t st, int nco, const float* x2 = nullptr, int cin1 = 0,
+                    const float* hist = nullptr, const int* rep = nullptr, int hist_len = 0);
+int conv1d_stream_simt(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len, const int* rep,
+                       const float* w, const float* bias, const float* residual, float* y, cudaStream_t st);
 int conv1d_tc_plan_ok(const pwgb_conv1d_desc* d, int* raw_staged = nullptr);
 void tc_pack_weight(const float* w, int cin, int cout, int kernel, void* packed, cudaStream_t st);
 
@@ -99,9 +102,12 @@ static int convtr_tc_chunk(const pwgb_conv1d_desc& c, bool two_source) {
   return chunk;
 }
 
-// x2 / cin1: the second source of a two-source input (cin1 > 0 only on the tensor-core path)
+// x2 / cin1: the second source of a two-source input (cin1 > 0 only on the tensor-core path).  hist_mode: d describes the
+// conv-transpose on cat(h, x) along time, x holds its last t_in - 1 frames and frame 0 is hist[b] (or x[b, :, 0] where
+// rep[b] is set): the virtual conv runs on x with that frame as a one-row history.
 static int convtr_forward(const pwgb_convtr1d_desc* d, const float* x, const float* x2, int cin1, const float* w,
-                          const float* bias, float* y, void* ws, size_t ws_bytes, void* stream) {
+                          const float* bias, float* y, void* ws, size_t ws_bytes, void* stream, bool hist_mode = false,
+                          const float* hist = nullptr, const int* rep = nullptr) {
   const int s = d->stride, K = d->kernel, M = ceil_div(K, s);
   const int G = d->groups > 1 ? d->groups : 1;
   const size_t need = pwgb_conv_transpose1d_workspace(d);
@@ -114,7 +120,13 @@ static int convtr_forward(const pwgb_convtr1d_desc* d, const float* x, const flo
   convtr_weight_kernel<<<blocks, 256, 0, st>>>(w, wv, d->cin, d->cout, K, s, M, G);
   int rc = check_launch("convtr_weight_kernel");
   if (rc) return rc;
-  const pwgb_conv1d_desc c = convtr_virtual_desc(d);
+  pwgb_conv1d_desc c = convtr_virtual_desc(d);
+  if (hist_mode) {
+    c.t_in -= 1;
+    c.t_valid = c.t_in;
+    c.pad_left += 1;
+    c.pad_mode = PWGB_PAD_HISTORY;
+  }
   const int chunk = convtr_tc_chunk(c, cin1 > 0);
   if (chunk) {
     pwgb_conv1d_desc cc = c;
@@ -128,8 +140,10 @@ static int convtr_forward(const pwgb_convtr1d_desc* d, const float* x, const flo
       rc = check_launch("tc_pack_weight_kernel");
       if (rc) return rc;
     }
+    if (hist_mode) return conv1d_tc_chunk(&cc, 0, c.cout, x, pk, bias, y, st, c.cout / chunk, nullptr, 0, hist, rep, 1);
     return conv1d_tc_chunk(&cc, 0, c.cout, x, pk, bias, y, st, c.cout / chunk, x2, cin1);
   }
+  if (hist_mode) return conv1d_stream_simt(&c, x, hist, 1, rep, wv, bias, nullptr, y, st);
   if (cin1 > 0) {
     set_error("conv_transpose1d_cat: configuration not supported by the tensor-core path");
     return PWGB_UNSUPPORTED;
@@ -161,4 +175,16 @@ extern "C" int pwgb_conv_transpose1d_cat_forward(const pwgb_convtr1d_desc* d, in
   PWGB_UNSUPPORTED_IF(!pwgb_conv_transpose1d_cat_supported(d, cin1),
                       "conv_transpose1d_cat: configuration not supported by the two-source tensor-core path");
   return convtr_forward(d, x1, x2, cin1, w, bias, y, ws, ws_bytes, stream);
+}
+
+extern "C" int pwgb_conv_transpose1d_stream_forward(const pwgb_convtr1d_desc* d, const float* x, const float* hist,
+                                                    const int* replicate, const float* w, const float* bias, float* y, void* ws,
+                                                    size_t ws_bytes, void* stream) {
+  PWGB_CHECK_ARG(d && x && hist && w && y, "conv_transpose1d_stream: null argument");
+  const int rc = convtr_desc_ok(d);
+  if (rc) return rc;
+  PWGB_CHECK_ARG(d->t_in >= 2, "conv_transpose1d_stream: t_in counts the history frame and at least one input frame");
+  PWGB_UNSUPPORTED_IF(d->groups > 1 || d->period > 1 || d->padding != d->stride,
+                      "conv_transpose1d_stream: the causal conv-transpose is dense, plain and has padding == stride");
+  return convtr_forward(d, x, nullptr, 0, w, bias, y, ws, ws_bytes, stream, true, hist, replicate);
 }

@@ -1,0 +1,78 @@
+// Streaming a causal conv stack chunk by chunk: the history conv entry point of the FFMA engine, the argument check both
+// engines share, and the multi-tensor history carry.
+#include "common.cuh"
+
+namespace pwgb {
+
+int conv1d_stream_simt(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len, const int* rep,
+                       const float* w, const float* bias, const float* residual, float* y, cudaStream_t st);
+
+int conv1d_stream_check(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len, const float* y) {
+  PWGB_CHECK_ARG(d && x && y, "conv1d_stream: null argument");
+  PWGB_CHECK_ARG(d->batch >= 0 && d->cin > 0 && d->cout > 0 && d->t_in > 0 && d->t_out >= 0, "conv1d_stream: bad sizes");
+  PWGB_CHECK_ARG(d->kernel > 0 && d->stride > 0 && d->dilation > 0 && d->groups > 0 && d->pad_left >= 0,
+                 "conv1d_stream: bad kernel geometry");
+  PWGB_CHECK_ARG(d->pad_mode == PWGB_PAD_HISTORY, "conv1d_stream: pad_mode must be PWGB_PAD_HISTORY");
+  PWGB_CHECK_ARG(hist_len >= 0 && (hist_len == 0 || hist), "conv1d_stream: bad history (hist_len %d)", hist_len);
+  PWGB_UNSUPPORTED_IF(d->stride != 1 || d->groups != 1 || d->period > 1 || d->pre_gate || d->shuffle > 1,
+                      "conv1d_stream: history padding serves plain stride-1 convs (groups 1, period 1, no pre_gate, one source)");
+  PWGB_UNSUPPORTED_IF(d->x_batch_stride || d->y_batch_stride || d->r_batch_stride || (d->t_valid > 0 && d->t_valid != d->t_in),
+                      "conv1d_stream: strided or reflect-extended inputs are not supported");
+  const long long need = (long long)(d->t_out - 1) + (long long)(d->kernel - 1) * d->dilation + 1 - d->pad_left;
+  PWGB_CHECK_ARG(d->t_out == 0 || need <= (long long)d->t_in, "conv1d_stream: t_out too large for t_in");
+  return PWGB_OK;
+}
+
+// One block per (entry, group of whole rows): the rows of a block are disjoint from every other block's, and within a
+// block every pass reads all its sources before any thread writes.  A pass covers ascending flat indices r * H + j of
+// its rows and element j reads index j + n of [hist | x], which is never below an index an earlier pass wrote, so the
+// in-place shift of a history longer than the chunk reads no overwritten sample.
+__global__ void __launch_bounds__(256) stream_carry_kernel(const long long* __restrict__ table, int n_entries) {
+  const long long* e = table + 5LL * blockIdx.y;
+  const float* x = reinterpret_cast<const float*>(e[0]);
+  float* hist = reinterpret_cast<float*>(e[1]);
+  const long long rows = e[2], n = e[3];
+  const int H = (int)e[4];
+  if (H <= 0) return;
+  const int rpb = H >= 256 ? 1 : 256 / H;  // rows per block group
+  const long long ngroups = (rows + rpb - 1) / rpb;
+  for (long long g = blockIdx.x; g < ngroups; g += gridDim.x) {
+    const long long r0 = g * rpb;
+    const long long nel = ((rows - r0 < rpb) ? rows - r0 : rpb) * (long long)H;
+    for (long long base = 0; base < nel; base += 256) {
+      const long long i = base + threadIdx.x;
+      float v = 0.f;
+      long long r = 0, j = 0;
+      if (i < nel) {
+        r = r0 + i / H;
+        j = i % H;
+        const long long s = j + n;  // index into [hist | x] of row r
+        v = s < H ? hist[r * H + s] : __ldg(x + r * n + (s - H));
+      }
+      __syncthreads();
+      if (i < nel) hist[r * H + j] = v;
+      __syncthreads();
+    }
+  }
+}
+
+}  // namespace pwgb
+
+using namespace pwgb;
+
+extern "C" int pwgb_conv1d_stream_forward(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len,
+                                          const int* replicate, const float* w, const float* bias, const float* residual,
+                                          float* y, void* stream) {
+  PWGB_CHECK_ARG(w, "conv1d_stream: null argument");
+  if (const int rc = conv1d_stream_check(d, x, hist, hist_len, y)) return rc;
+  return conv1d_stream_simt(d, x, hist, hist_len, replicate, w, bias, residual, y, (cudaStream_t)stream);
+}
+
+extern "C" int pwgb_stream_carry(const void* table, int n_entries, void* stream) {
+  PWGB_CHECK_ARG(n_entries >= 0 && n_entries <= 65535, "stream_carry: bad entry count %d", n_entries);
+  if (n_entries == 0) return PWGB_OK;
+  PWGB_CHECK_ARG(table, "stream_carry: null table");
+  // a fixed number of blocks per entry, each looping over its row groups: the table stays on the device
+  stream_carry_kernel<<<dim3(64, (unsigned)n_entries), 256, 0, (cudaStream_t)stream>>>((const long long*)table, n_entries);
+  return check_launch("stream_carry_kernel");
+}

@@ -389,6 +389,138 @@ def upsample_fir_causal_stream(x, fir, scale, hist_in, hist_out, out_channels=No
     return out
 
 
+def conv1d_stream(x, hist, w, bias=None, *, pad_left, dilation=1, replicate=None, pre_slope=1.0, post_act=None, post_slope=0.0,
+                  residual=None, out_scale=1.0, out=None, accumulate=False):
+    """conv1d with history padding (pwgb_conv1d_stream_forward / pwgb_conv1d_tc_stream_forward): of the ``pad_left`` rows
+    in front of x, the last H read ``hist`` (B, cin, H) -- or x[:, :, 0] for the items whose ``replicate`` (B,) int32 flag
+    is set -- and the earlier ones are zero; no right padding.  Everything else is conv1d's, and so is the engine choice
+    (including the 16-column and 32-channel paddings of conv1d), so a chunked run equals conv1d on the whole signal."""
+    x, w = _dev(x, "x"), _dev(w, "w")
+    B, cin, L = x.shape
+    cout, cin_w, K = w.shape
+    if hist is None:
+        hist = x.new_zeros((B, cin, 0))
+    hist = _dev(hist, "hist")
+    if cin_w != cin or hist.dim() != 3 or tuple(hist.shape[:2]) != (B, cin):
+        raise PwgbError(f"conv1d_stream: x {tuple(x.shape)}, hist {tuple(hist.shape)} and weight {tuple(w.shape)} do not match")
+    if replicate is not None and (replicate.dtype != torch.int32 or not replicate.is_cuda or replicate.numel() != B):
+        raise PwgbError(f"conv1d_stream: replicate must be {B} int32 flags on the device")
+    kw = dict(pad_left=pad_left, dilation=dilation, replicate=replicate, pre_slope=pre_slope, post_act=post_act, post_slope=post_slope)
+    if ENGINE != "simt" and cout < 16 and cin >= 256 and cin % 32 == 0 and residual is None and out is None and not accumulate:
+        # as _conv1d_fewcout: the weight padded to 16 output channels for the tensor cores
+        b16 = torch.nn.functional.pad(bias, (0, 16 - cout)) if bias is not None else None
+        y = conv1d_stream(x, hist, torch.nn.functional.pad(w, (0, 0, 0, 0, 0, 16 - cout)), b16, **kw)
+        return y[:, :cout].contiguous()
+    if ENGINE != "simt" and cin % 32 and cin >= 48 and cout % 16 == 0:
+        # as _conv1d_padcin: input channels zero-padded to a multiple of 32
+        padc = (cin + 31) // 32 * 32 - cin
+        pc = (0, 0, 0, padc)
+        return conv1d_stream(torch.nn.functional.pad(x, pc), torch.nn.functional.pad(hist, pc), torch.nn.functional.pad(w, pc),
+                             bias, residual=residual, out_scale=out_scale, out=out, accumulate=accumulate, **kw)
+    t_out = L + pad_left - dilation * (K - 1)
+    if t_out < 0:
+        raise PwgbError("conv1d_stream: input shorter than the receptive field")
+    shape = (B, cout, t_out)
+    if out is None:
+        if accumulate:
+            raise PwgbError("conv1d_stream: accumulate needs `out`")
+        out = torch.empty(shape, device=x.device, dtype=torch.float32)
+    elif tuple(out.shape) != shape or not out.is_contiguous():
+        raise PwgbError(f"conv1d_stream: out has shape {tuple(out.shape)}, expected {shape}")
+    if residual is not None:
+        residual = _dev(residual, "residual")
+        if residual.numel() != out.numel() or residual.data_ptr() == out.data_ptr():
+            raise PwgbError("conv1d_stream: residual must match out and not alias it")
+    if out.numel() == 0:
+        return out
+    if bias is not None:
+        bias = _dev(bias, "bias")
+    H = hist.shape[-1]
+    dkey = ("stream", B, cin, cout, L, t_out, K, dilation, pad_left, float(pre_slope), post_act, float(post_slope), float(out_scale),
+            bool(accumulate))
+    d = _DESC_CACHE.get(dkey)
+    if d is None:
+        if len(_DESC_CACHE) > 4096:
+            _DESC_CACHE.clear()
+        d = _DESC_CACHE[dkey] = capi.Conv1dDesc(
+            batch=B, cin=cin, cout=cout, t_in=L, t_out=t_out, kernel=K, stride=1, dilation=dilation, groups=1, pad_left=pad_left,
+            pad_mode=capi.PAD_HISTORY, period=1, t_valid=L, pre_slope=float(pre_slope), pre_gate=0, post_act=_ACT[post_act],
+            post_slope=float(post_slope), out_scale=float(out_scale), accumulate=int(bool(accumulate)))
+    prof = _Prof("conv1d_stream", 2.0 * B * cout * t_out * cin * K,
+                 4.0 * (x.numel() + out.numel() * (2 if accumulate else 1) + (residual.numel() if residual is not None else 0)),
+                 f"B{B} cin{cin} cout{cout} k{K} d{dilation} T{t_out} H{H}" if PROFILE is not None else "")
+    lib = capi.lib()
+    if ENGINE != "simt" and lib.pwgb_conv1d_tc_supported(C.byref(d)):
+        prof.name = "conv1d_tc_stream"
+        rc = lib.pwgb_conv1d_tc_stream_forward(C.byref(d), _p(x), _p(hist), H, _p(replicate), _p(packed_weight(w)), _p(bias),
+                                               _p(residual), _p(out), _stream())
+        capi.check(rc, "pwgb_conv1d_tc_stream_forward")
+    else:
+        rc = lib.pwgb_conv1d_stream_forward(C.byref(d), _p(x), _p(hist), H, _p(replicate), _p(w), _p(bias), _p(residual), _p(out),
+                                            _stream())
+        capi.check(rc, "pwgb_conv1d_stream_forward")
+    prof.done()
+    return out
+
+
+def conv_transpose1d_stream(x, hist, w, bias=None, *, stride, replicate=None, pre_slope=1.0, out=None):
+    """The causal conv-transpose of a stream (pwgb_conv_transpose1d_stream_forward): conv_transpose1d(cat(h, x), w, bias,
+    stride=stride, padding=stride, pre_slope=pre_slope) along time with h[b] = x[b, :, :1] where ``replicate`` (B,) int32
+    is set, else hist[b] ((B, cin, 1)); the concatenation is never materialised.  Bit-identical to that call."""
+    x, w, hist = _dev(x, "x"), _dev(w, "w"), _dev(hist, "hist")
+    B, cin, n = x.shape
+    if w.shape[0] != cin or tuple(hist.shape) != (B, cin, 1):
+        raise PwgbError(f"conv_transpose1d_stream: x {tuple(x.shape)}, hist {tuple(hist.shape)} and weight {tuple(w.shape)} do not match")
+    if replicate is not None and (replicate.dtype != torch.int32 or not replicate.is_cuda or replicate.numel() != B):
+        raise PwgbError(f"conv_transpose1d_stream: replicate must be {B} int32 flags on the device")
+    cout, K = w.shape[1], w.shape[2]
+    t_out = n * stride - 2 * stride + K
+    if bias is not None:
+        bias = _dev(bias, "bias")
+    d = capi.ConvTr1dDesc(batch=B, cin=cin, cout=cout, t_in=n + 1, t_out=t_out, kernel=K, stride=stride, padding=stride,
+                          pre_slope=float(pre_slope), groups=1, period=1)
+    lib = capi.lib()
+    nbytes = lib.pwgb_conv_transpose1d_workspace(C.byref(d))
+    ws = torch.empty((nbytes + 3) // 4, device=x.device, dtype=torch.float32)
+    y = torch.empty((B, cout, t_out), device=x.device, dtype=torch.float32) if out is None else out
+    if tuple(y.shape) != (B, cout, t_out) or not y.is_contiguous() or y.dtype != torch.float32:
+        raise PwgbError(f"conv_transpose1d_stream: out must be a contiguous float32 {(B, cout, t_out)} tensor")
+    if y.numel() == 0:
+        return y
+    prof = _Prof("conv_transpose1d_stream", 2.0 * B * cout * t_out * cin * ((K + stride - 1) // stride), 4.0 * (x.numel() + y.numel()),
+                 f"B{B} cin{cin} cout{cout} k{K} s{stride} T{t_out}")
+    rc = lib.pwgb_conv_transpose1d_stream_forward(C.byref(d), _p(x), _p(hist), _p(replicate), _p(w), _p(bias), _p(y), _p(ws),
+                                                  C.c_size_t(nbytes), _stream())
+    capi.check(rc, "pwgb_conv_transpose1d_stream_forward")
+    prof.done()
+    return y
+
+
+def stream_carry_table(entries, device):
+    """Device table of pwgb_stream_carry for ``entries`` = [(x, hist), ...]: x (..., n) is a chunk of a signal and hist
+    (..., H) its history, both contiguous fp32 with the same leading shape.  The table holds the tensors' addresses, so
+    they must stay allocated (and in place) while it is used."""
+    rows = []
+    for x, hist in entries:
+        for t, name in ((x, "x"), (hist, "hist")):
+            if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
+                raise PwgbError(f"stream_carry: {name} must be a contiguous float32 CUDA tensor")
+        if tuple(x.shape[:-1]) != tuple(hist.shape[:-1]):
+            raise PwgbError(f"stream_carry: x {tuple(x.shape)} and hist {tuple(hist.shape)} do not have the same rows")
+        rows.append([x.data_ptr(), hist.data_ptr(), x.numel() // max(x.shape[-1], 1), x.shape[-1], hist.shape[-1]])
+    return torch.tensor(rows, dtype=torch.int64).reshape(-1, 5).to(device)
+
+
+def stream_carry(table):
+    """pwgb_stream_carry: every entry's hist becomes the last H samples of [hist | x]."""
+    if table.dtype != torch.int64 or not table.is_cuda or table.dim() != 2 or table.shape[1] != 5:
+        raise PwgbError("stream_carry: the table must be an (entries, 5) int64 CUDA tensor")
+    prof = _Prof("stream_carry", 0.0, 0.0, f"entries{table.shape[0]}")
+    rc = capi.lib().pwgb_stream_carry(_p(table), table.shape[0], _stream())
+    capi.check(rc, "pwgb_stream_carry")
+    prof.done()
+
+
 class WaveNetLayerWeights:
     """Device-side operand images of one WaveNetResidualBlock for pwgb_wavenet_layer_forward."""
 

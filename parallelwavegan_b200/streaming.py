@@ -1,4 +1,5 @@
-"""Chunked synthesis with a causal Parallel WaveGAN: mel frames in, waveform out, while the frames are still arriving.
+"""Chunked synthesis with the causal generators: mel frames in, waveform out, while the frames are still arriving.
+``CausalPWGStream`` streams a causal Parallel WaveGAN, ``CausalHiFiGANStream`` a causal HiFi-GAN.
 
 A causal generator's output for frame j depends only on frames <= j, so it can be synthesised as soon as frame j
 exists.  ``CausalPWGStream`` carries, per batch slot, everything the whole-utterance forward would read from before
@@ -34,15 +35,79 @@ def _layer_weights(f, A):
                                       cache=f._cache, key=k, causal=True)
 
 
-class CausalPWGStream:
+class _ChunkStream:
+    """Plumbing shared by the streams: slot validation, one cached entry per chunk length (at most
+    ``MAX_CHUNK_LENGTHS``), and one CUDA graph per chunk length captured after an eager warm-up whose state changes are
+    undone.  A subclass provides ``_state()`` (the tensors a push advances), ``_new_entry(n)`` and ``_step(*inputs)``."""
+
+    MAX_CHUNK_LENGTHS = 8
+
+    def _setup(self, model, batch, use_graphs):
+        self._check_eval(model)
+        self.model = model
+        self.dev = next(model.parameters()).device
+        if self.dev.type != "cuda":
+            raise PwgbError(f"{type(self).__name__}: the model must live on a CUDA device (no CPU fallback)")
+        self.B = int(batch)
+        if self.B < 1:
+            raise PwgbError(f"{type(self).__name__}: batch must be >= 1")
+        self.use_graphs = bool(use_graphs)
+        self._entries = {}  # chunk frames -> per-length data and "graph"; a graph lives and dies with its entry
+
+    def _check_eval(self, model):
+        if model.training:
+            raise PwgbError(f"{type(self).__name__}: the model is in train mode; call model.eval() (dropout would apply)")
+
+    def _slots(self, items):
+        """``items`` (an index, an iterable of indices or None for every slot) as a checked list"""
+        items = range(self.B) if items is None else ([items] if isinstance(items, int) else list(items))
+        for b in items:
+            if not 0 <= b < self.B:
+                raise PwgbError(f"{type(self).__name__}.reset: slot {b} out of range [0, {self.B})")
+        return items
+
+    def _entry(self, n):
+        ent = self._entries.get(n)
+        if ent is None:
+            if len(self._entries) >= self.MAX_CHUNK_LENGTHS:
+                self._entries.clear()
+            ent = self._entries[n] = self._new_entry(n)
+        return ent
+
+    def _replay(self, n, inputs):
+        ent = self._entry(n)
+        if "graph" not in ent:
+            static = [t.clone() for t in inputs]
+            # one eager warm-up (packs weights, sets kernel attributes, fills the per-shape caches) advances the state:
+            # it is restored before the capture, which itself runs nothing
+            snap = [t.clone() for t in self._state()]
+            side = torch.cuda.Stream()
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):
+                self._step(*static)
+            torch.cuda.current_stream().wait_stream(side)
+            for t, s in zip(self._state(), snap):
+                t.copy_(s)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                out = self._step(*static)
+            ent.update(graph=graph, inputs=static, out=out)
+        for s, t in zip(ent["inputs"], inputs):
+            s.copy_(t)
+        ent["graph"].replay()
+        return ent["out"].clone()
+
+    def _run(self, n, *inputs):
+        return self._replay(n, inputs) if self.use_graphs else self._step(*inputs)
+
+
+class CausalPWGStream(_ChunkStream):
     """Streams a causal ``ParallelWaveGANGenerator`` chunk by chunk for ``batch`` independent slots.
 
     ``push(c, z)`` takes the next n >= 1 frames of every slot and returns their n * hop samples; n may change from
     push to push.  For every slot, the concatenated outputs equal ``model.inference(c=all_frames, x=all_noise)``.
     There is no lookahead and no flush.  With ``use_graphs`` each chunk length is captured once into a CUDA graph and
     replayed.  The model's weights must not change while a stream uses them (the graphs hold the packed images)."""
-
-    MAX_CHUNK_LENGTHS = 8
 
     def __init__(self, model, batch=1, seed=None, use_graphs=True):
         from .models import MelGANGenerator, ParallelWaveGANGenerator
@@ -58,14 +123,7 @@ class CausalPWGStream:
             raise PwgbError("CausalPWGStream: upsample_net='MelGANGenerator' is not supported")
         if isinstance(up, UpsampleNetwork) and model.aux_context_window:
             raise PwgbError("CausalPWGStream: UpsampleNetwork with aux_context_window > 0 has no whole-utterance inference to match")
-        self._check_eval(model)
-        self.model = model
-        self.dev = next(model.parameters()).device
-        if self.dev.type != "cuda":
-            raise PwgbError("CausalPWGStream: the model must live on a CUDA device (no CPU fallback)")
-        self.B = int(batch)
-        if self.B < 1:
-            raise PwgbError("CausalPWGStream: batch must be >= 1")
+        self._setup(model, batch, use_graphs)
         self.conv_in = up.conv_in if isinstance(up, ConvInUpsampleNetwork) else None
         fir_net = up.upsample if isinstance(up, ConvInUpsampleNetwork) else up
         self.scales = list(fir_net.upsample_scales)
@@ -87,16 +145,9 @@ class CausalPWGStream:
         self.fir_next = [torch.zeros((B * A, 2), device=dev, dtype=torch.float32) for _ in self.scales]
         self.wn_hist = [torch.zeros(B * self.R * h, device=dev, dtype=torch.int32) for h in self.H]
         self._fresh = [True] * B
-        self.use_graphs = bool(use_graphs)
-        self._entries = {}  # chunk frames -> {"stack": WnStack, "graph": ...}; a graph lives and dies with its stack
         self.gen = torch.Generator(device=dev)
         if seed is not None:
             self.gen.manual_seed(int(seed))
-
-    @staticmethod
-    def _check_eval(model):
-        if model.training:
-            raise PwgbError("CausalPWGStream: the model is in train mode; call model.eval() (dropout would apply)")
 
     # ---------------------------------------------------------------------------------------------------- state
     def _state(self):
@@ -105,11 +156,8 @@ class CausalPWGStream:
     def reset(self, items=None):
         """Restart slots ``items`` (an index or an iterable of indices; None: every slot) as fresh signals.  The other
         slots continue unaffected."""
-        items = range(self.B) if items is None else ([items] if isinstance(items, int) else list(items))
         A = self.A
-        for b in items:
-            if not 0 <= b < self.B:
-                raise PwgbError(f"CausalPWGStream.reset: slot {b} out of range [0, {self.B})")
+        for b in self._slots(items):
             if self.cin_hist is not None:
                 self.cin_hist[b].zero_()
             for h in self.fir_hist:
@@ -119,14 +167,8 @@ class CausalPWGStream:
             self._fresh[b] = True
 
     # ---------------------------------------------------------------------------------------------------- compute
-    def _entry(self, n):
-        ent = self._entries.get(n)
-        if ent is None:
-            if len(self._entries) >= self.MAX_CHUNK_LENGTHS:
-                self._entries.clear()
-            ent = self._entries[n] = {"stack": ops.WnStack(self.B, n * self.hop, self.R, self.G, self.S, self.A, self.K, self.dmax,
-                                                           self.dev, True)}
-        return ent
+    def _new_entry(self, n):
+        return {"stack": ops.WnStack(self.B, n * self.hop, self.R, self.G, self.S, self.A, self.K, self.dmax, self.dev, True)}
 
     def _step(self, z, c):
         """One chunk: z (B, in_channels, n * hop), c (B, aux, n) -> (B, out_channels, n * hop).  Advances the state."""
@@ -163,29 +205,6 @@ class CausalPWGStream:
         h = ops.conv1d(skips, effective_weight(l1) * m._skip_scale, l1.bias, pre_slope=0.0)
         return ops.conv1d(h, effective_weight(l3), l3.bias, pre_slope=0.0)
 
-    def _replay(self, z, c):
-        ent = self._entry(c.shape[-1])
-        if "graph" not in ent:
-            static_z, static_c = z.clone(), c.clone()
-            # one eager warm-up (packs weights, sets kernel attributes, fills the per-shape caches) advances the state:
-            # it is restored before the capture, which itself runs nothing
-            snap = [t.clone() for t in self._state()]
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                self._step(static_z, static_c)
-            torch.cuda.current_stream().wait_stream(side)
-            for t, s in zip(self._state(), snap):
-                t.copy_(s)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                out = self._step(static_z, static_c)
-            ent.update(graph=graph, z=static_z, c=static_c, out=out)
-        ent["z"].copy_(z)
-        ent["c"].copy_(c)
-        ent["graph"].replay()
-        return ent["out"].clone()
-
     @torch.no_grad()
     def push(self, c, z=None, normalize_before=False):
         """c: (B, n, aux) mel frames ((n, aux) when batch == 1); z: optional (B, in_channels, n * hop) noise, drawn from
@@ -214,4 +233,186 @@ class CausalPWGStream:
                 if self._fresh[b]:
                     self.cin_hist[b].copy_(c[b, :, :1].expand(-1, self.acw))
         self._fresh = [False] * self.B
-        return self._replay(z, c) if self.use_graphs else self._step(z, c)
+        return self._run(n, z, c)
+
+
+class CausalHiFiGANStream(_ChunkStream):
+    """Streams a causal ``HiFiGANGenerator`` (``use_causal_conv=True``) chunk by chunk for ``batch`` independent slots.
+
+    ``push(c)`` takes the next n >= 1 mel frames of every slot and returns their n * hop samples; n may change from push
+    to push.  For every slot, the concatenated outputs equal ``model.inference(all_frames)``.  There is no lookahead and
+    no flush.  Every conv of the causal generator pads only on the left, so the stream keeps, per slot, the samples in
+    front of the chunk that the whole-utterance forward would read, one history per signal (convs that read the same
+    tensor share a buffer sized by the largest of their histories):
+
+    * the input conv: the last kernel_size - 1 mel frames; it runs as a valid conv on [history | chunk];
+    * each conv-transpose: the last frame of its input, replicated from the first frame for a fresh slot
+      (``ReplicationPad1d``, pwgb_conv_transpose1d_stream_forward with the per-slot replicate flags);
+    * each level's input, read by the first dilated conv of every block: max_j (k_j - 1) * d_j0 samples;
+    * each ResBlock's later dilated-conv inputs ((k - 1) * d) and second-conv inputs (k - 1);
+    * the output conv: its last kernel_size - 1 input samples.
+
+    The convs read their histories in their loaders (pwgb_conv1d_stream_forward / pwgb_conv1d_tc_stream_forward), so no
+    [history | chunk] concatenation is made at the waveform rate.  After a ResBlock's last conv one pwgb_stream_carry
+    launch updates every history it read; the intermediate signals of each chunk length live in buffers allocated once,
+    so the carry tables are built once too.  With ``use_graphs`` each chunk length is captured once into a CUDA graph
+    and replayed.  The weights are read when the stream is built and must not change while it is used."""
+
+    def __init__(self, model, batch=1, use_graphs=True):
+        from .models import HiFiGANGenerator
+
+        if not isinstance(model, HiFiGANGenerator):
+            raise PwgbError("CausalHiFiGANStream: expected a HiFiGANGenerator")
+        if not model.use_causal_conv:
+            raise PwgbError("CausalHiFiGANStream: the model is not causal (use_causal_conv=False); a centred model needs lookahead")
+        self._setup(model, batch, use_graphs)
+        dev, B = self.dev, self.B
+
+        def wb(conv):
+            return effective_weight(conv).detach().contiguous(), (conv.bias.detach() if conv.bias is not None else None)
+
+        def zeros(*shape):
+            return torch.zeros(shape, device=dev, dtype=torch.float32)
+
+        m = model
+        self.slope, self.nb = m.slope, m.num_blocks
+        ic = m.input_conv
+        self.w_in = wb(ic.conv)
+        self.in_channels = ic.conv.in_channels
+        self.cin_hist = zeros(B, self.in_channels, ic.left)
+        self.hop = 1
+        self.levels = []
+        for i in range(m.num_upsamples):
+            up = m.upsamples[i][1]
+            cin, cout = up.deconv.in_channels, up.deconv.out_channels
+            self.hop *= up.stride
+            blocks = []
+            for j in range(self.nb):
+                blk = m.blocks[i * self.nb + j]
+                k, dils = blk.kernel_size, blk.dilations
+                convs = []
+                for idx, d in enumerate(dils):
+                    c1 = blk.convs1[idx][1].conv
+                    c2 = blk.convs2[idx][1].conv if blk.use_additional_convs else None
+                    convs.append(dict(d=d, w1=wb(c1), w2=wb(c2) if c2 is not None else None,
+                                      # the input of the dilated conv (idx 0: the level input, shared) and of the second conv
+                                      x_hist=zeros(B, cout, (k - 1) * d) if idx > 0 else None,
+                                      xt_hist=zeros(B, cout, k - 1) if c2 is not None else None))
+                blocks.append(dict(k=k, convs=convs))
+            hl = max((b["k"] - 1) * b["convs"][0]["d"] for b in blocks)
+            self.levels.append(dict(stride=up.stride, channels=cout, w=wb(up.deconv), up_hist=zeros(B, cin, 1),
+                                    lvl_hist=zeros(B, cout, hl), blocks=blocks))
+        oc = m.output_conv[1]
+        self.w_out = wb(oc.conv)
+        self.out_hist = zeros(B, oc.conv.in_channels, oc.left)
+        self.out_channels = oc.conv.out_channels
+        self.rep = torch.ones(B, device=dev, dtype=torch.int32)  # replicate flags of the conv-transposes: fresh slots
+
+    # ---------------------------------------------------------------------------------------------------- state
+    def _state(self):
+        hs = [self.cin_hist, self.out_hist, self.rep]
+        for lv in self.levels:
+            hs += [lv["up_hist"], lv["lvl_hist"]]
+            for blk in lv["blocks"]:
+                hs += [h for cv in blk["convs"] for h in (cv["x_hist"], cv["xt_hist"]) if h is not None]
+        return hs
+
+    def state_bytes(self):
+        """bytes of carried state per slot"""
+        return sum(t.numel() * t.element_size() for t in self._state() if t is not self.rep) // self.B
+
+    def reset(self, items=None):
+        """Restart slots ``items`` (an index or an iterable of indices; None: every slot) as fresh signals.  The other
+        slots continue unaffected."""
+        for b in self._slots(items):
+            for h in self._state():
+                if h is not self.rep:
+                    h[b].zero_()
+            self.rep[b] = 1
+
+    # ---------------------------------------------------------------------------------------------------- compute
+    def _new_entry(self, n):
+        """The buffers of every intermediate signal of an n-frame chunk, and the carry tables over them."""
+        dev, B = self.dev, self.B
+
+        def empty(*shape):
+            return torch.empty(shape, device=dev, dtype=torch.float32)
+
+        K_in = self.cin_hist.shape[-1]
+        ent = dict(xin=empty(B, self.in_channels, K_in + n), h0=empty(B, self.levels[0]["w"][0].shape[0], n), levels=[])
+        t, prev = n, ent["h0"]
+        for i, lv in enumerate(self.levels):
+            t *= lv["stride"]
+            C = lv["channels"]
+            nd = max(len(b["convs"]) for b in lv["blocks"])
+            buf = dict(u=empty(B, C, t), cs=empty(B, C, t), x=[empty(B, C, t) for _ in range(nd - 1)], xt=[empty(B, C, t) for _ in range(nd)])
+            tables = []
+            for j, blk in enumerate(lv["blocks"]):
+                entries = []
+                for idx, cv in enumerate(blk["convs"]):
+                    if cv["x_hist"] is not None:
+                        entries.append((buf["x"][idx - 1], cv["x_hist"]))
+                    if cv["xt_hist"] is not None:
+                        entries.append((buf["xt"][idx], cv["xt_hist"]))
+                if j == len(lv["blocks"]) - 1:  # the level's shared signals, after their last reader
+                    entries += [(prev, lv["up_hist"]), (buf["u"], lv["lvl_hist"])]
+                    if i == 0:
+                        entries.append((ent["xin"], self.cin_hist))  # the last frames of [history | chunk] are the chunk's
+                tables.append(ops.stream_carry_table(entries, dev))
+            buf["tables"] = tables
+            ent["levels"].append(buf)
+            prev = buf["cs"]
+        ent["y"] = empty(B, self.out_channels, t)
+        ent["out_table"] = ops.stream_carry_table([(prev, self.out_hist)], dev)
+        return ent
+
+    def _step(self, c):
+        """One chunk: c (B, in_channels, n) -> (B, out_channels, n * hop).  Advances the state."""
+        ent = self._entry(c.shape[-1])
+        K_in = self.cin_hist.shape[-1]
+        xin = ent["xin"]
+        xin[:, :, :K_in].copy_(self.cin_hist)
+        xin[:, :, K_in:].copy_(c)
+        h = ops.conv1d(xin, self.w_in[0], self.w_in[1], out=ent["h0"])
+        slope = self.slope
+        for lv, buf in zip(self.levels, ent["levels"]):
+            u = ops.conv_transpose1d_stream(h, lv["up_hist"], lv["w"][0], lv["w"][1], stride=lv["stride"], replicate=self.rep,
+                                            pre_slope=slope, out=buf["u"])
+            cs = buf["cs"]
+            for j, blk in enumerate(lv["blocks"]):
+                k, convs = blk["k"], blk["convs"]
+                x = u
+                for idx, cv in enumerate(convs):
+                    d = cv["d"]
+                    last = idx == len(convs) - 1
+                    tail = dict(out=cs, accumulate=j > 0, out_scale=1.0 / self.nb) if last else dict(out=buf["x"][idx])
+                    hx = lv["lvl_hist"] if idx == 0 else cv["x_hist"]
+                    if cv["w2"] is not None:
+                        xt = ops.conv1d_stream(x, hx, *cv["w1"], pad_left=(k - 1) * d, dilation=d, pre_slope=slope, out=buf["xt"][idx])
+                        x = ops.conv1d_stream(xt, cv["xt_hist"], *cv["w2"], pad_left=k - 1, pre_slope=slope, residual=x, **tail)
+                    else:
+                        x = ops.conv1d_stream(x, hx, *cv["w1"], pad_left=(k - 1) * d, dilation=d, pre_slope=slope, residual=x, **tail)
+                ops.stream_carry(buf["tables"][j])
+            h = cs
+        y = ops.conv1d_stream(h, self.out_hist, *self.w_out, pad_left=self.out_hist.shape[-1], pre_slope=0.01, post_act="tanh",
+                              out=ent["y"])
+        ops.stream_carry(ent["out_table"])
+        self.rep.zero_()
+        return y
+
+    @torch.no_grad()
+    def push(self, c, normalize_before=False):
+        """c: (B, n, in_channels) mel frames ((n, in_channels) when batch == 1).  Returns (B, out_channels, n * hop) on the
+        device."""
+        m = self.model
+        self._check_eval(m)
+        c = torch.as_tensor(c, dtype=torch.float32, device=self.dev)
+        if c.dim() == 2 and self.B == 1:
+            c = c.unsqueeze(0)
+        if c.dim() != 3 or c.shape[0] != self.B or c.shape[2] != self.in_channels or c.shape[1] < 1:
+            raise PwgbError(f"CausalHiFiGANStream.push: c must be ({self.B}, n >= 1, {self.in_channels}), got {tuple(c.shape)}")
+        if normalize_before:
+            c = (c - m.mean) / m.scale
+        c = c.transpose(1, 2).contiguous()
+        y = self._run(c.shape[-1], c)
+        return y if self.use_graphs else y.clone()
