@@ -41,8 +41,9 @@ typedef enum pwgb_status {
   PWGB_CUDA_ERROR = -3   /* launch failed; message holds cudaGetErrorString */
 } pwgb_status;
 
-/* PWGB_PAD_HISTORY: rows before sample 0 come from a caller-owned history (the stream entry points only) */
-enum { PWGB_PAD_ZERO = 0, PWGB_PAD_REFLECT = 1, PWGB_PAD_REPLICATE = 2, PWGB_PAD_HISTORY = 3 };
+/* PWGB_PAD_HISTORY: rows before sample 0 come from a caller-owned history (the stream entry points only);
+ * PWGB_PAD_HISTORY_REFLECT: the same, except that a flagged slot reflects instead of replicating */
+enum { PWGB_PAD_ZERO = 0, PWGB_PAD_REFLECT = 1, PWGB_PAD_REPLICATE = 2, PWGB_PAD_HISTORY = 3, PWGB_PAD_HISTORY_REFLECT = 4 };
 enum { PWGB_ACT_NONE = 0, PWGB_ACT_TANH = 1, PWGB_ACT_LRELU = 2 };
 
 PWGB_API const char* pwgb_last_error(void);
@@ -175,6 +176,11 @@ PWGB_API int pwgb_conv1d_tc_forward(const pwgb_conv1d_desc* d, const float* x, c
  * where a sample sits, so a chunked run is bit-identical to the whole-signal conv on cat(hist, x) when that takes the same
  * kernel.  On the tensor cores the history launch stages activations with per-element copies (never TMA rows); the sum
  * order is the same as for the other plans.
+ * d->pad_mode == PWGB_PAD_HISTORY_REFLECT (these entry points only) is the same policy, except that for a slot whose
+ * flag is set (the same array, now a fresh-signal flag) row t in [-hist_len, 0) reads x[b, c, -t] -- ReflectionPad1d for a
+ * fresh signal; it needs d->pad_left < d->t_in and hist_len <= d->pad_left (else PWGB_INVALID).  With hist_len ==
+ * pad_left a flagged slot is bit-identical to the whole-signal conv with PWGB_PAD_REFLECT on x when that takes the same
+ * kernel.
  * ---------------------------------------------------------------------- */
 PWGB_API int pwgb_conv1d_stream_forward(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len,
                                         const int* replicate, const float* w, const float* bias, const float* residual,
@@ -190,6 +196,20 @@ PWGB_API int pwgb_conv1d_tc_stream_forward(const pwgb_conv1d_desc* d, const floa
 PWGB_API int pwgb_conv_transpose1d_stream_forward(const pwgb_convtr1d_desc* d, const float* x, const float* hist,
                                                   const int* replicate, const float* w, const float* bias, float* y, void* ws,
                                                   size_t ws_bytes, void* stream);
+/* A window of a conv-transpose over a streamed signal (PQMF synthesis, layers/pqmf.py:133-149, under a chunked driver).
+ * d describes the conv-transpose of one chunk (stride s, kernel K, padding p; groups 1, period 1): d->t_in = n rows of
+ * x and d->t_out = n * s.  hist (batch, cin, hist_len) holds the signal's rows in front of the chunk (earlier rows read as
+ * zero; hist_len >= ceil(K / s) - 1 covers the whole receptive field).  With the chunk starting at row T0 of the signal,
+ * y[b, :, j] is output sample T0 * s - p + j of pwgb_conv_transpose1d_forward on the whole signal (any output_padding):
+ * the window lags the input by p samples, so it never reads a row after the chunk.  fresh (DEVICE array of batch int32,
+ * or NULL): a flagged slot is at the start of its signal (T0 = 0), and its y[b, :, j] for j < p (samples before 0) is
+ * written as zero (a flagged slot's window must hold them all: d->t_out >= p).  flush != 0: x is not read (may be NULL) and the chunk's rows are zero -- the signal has ended, and
+ * the window computes its last samples against the zero right padding.  It always runs the generic FFMA kernel, so it is
+ * bit-identical to the whole-signal call when that runs the same kernel (cin not a multiple of 32, e.g. 4 subbands ->
+ * 1).  ws: pwgb_conv_transpose1d_workspace(d) bytes. */
+PWGB_API int pwgb_conv_transpose1d_window_stream_forward(const pwgb_convtr1d_desc* d, const float* x, const float* hist,
+                                                         int hist_len, const int* fresh, int flush, const float* w,
+                                                         const float* bias, float* y, void* ws, size_t ws_bytes, void* stream);
 /* History carry of a stream, many signals in one launch.  table: DEVICE array of n_entries rows {x*, hist*, rows, n, H}
  * (5 x int64): x (rows, n) fp32 is this chunk of a signal, hist (rows, H) fp32 its history; afterwards hist holds the
  * last H samples of [hist | x] per row (also for n < H).  Every read of an entry happens before that entry's writes;

@@ -5,7 +5,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_lib", "libpwgb.so")
 
-PAD_ZERO, PAD_REFLECT, PAD_REPLICATE, PAD_HISTORY = 0, 1, 2, 3
+PAD_ZERO, PAD_REFLECT, PAD_REPLICATE, PAD_HISTORY, PAD_HISTORY_REFLECT = 0, 1, 2, 3, 4
 ACT_NONE, ACT_TANH, ACT_LRELU = 0, 1, 2
 
 
@@ -111,6 +111,9 @@ def lib():
     L.pwgb_conv1d_tc_stream_forward.argtypes = [C.POINTER(Conv1dDesc), vp, vp, C.c_int, vp, vp, vp, vp, vp, vp]
     L.pwgb_conv_transpose1d_stream_forward.restype = C.c_int
     L.pwgb_conv_transpose1d_stream_forward.argtypes = [C.POINTER(ConvTr1dDesc), vp, vp, vp, vp, vp, vp, vp, C.c_size_t, vp]
+    L.pwgb_conv_transpose1d_window_stream_forward.restype = C.c_int
+    L.pwgb_conv_transpose1d_window_stream_forward.argtypes = [C.POINTER(ConvTr1dDesc), vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp,
+                                                             C.c_size_t, vp]
     L.pwgb_stream_carry.restype = C.c_int
     L.pwgb_stream_carry.argtypes = [vp, C.c_int, vp]
     L.pwgb_debug_set.restype = None
@@ -287,7 +290,8 @@ EXPORTED_SYMBOLS = [
     "pwgb_conv1d_tc_packed_weight_bytes", "pwgb_conv1d_tc_pack_weight", "pwgb_conv1d_tc_pack_weight_grouped",
     "pwgb_conv1d_tc_supported",
     "pwgb_conv1d_tc_forward", "pwgb_debug_set", "pwgb_debug_get",
-    "pwgb_conv1d_stream_forward", "pwgb_conv1d_tc_stream_forward", "pwgb_conv_transpose1d_stream_forward", "pwgb_stream_carry",
+    "pwgb_conv1d_stream_forward", "pwgb_conv1d_tc_stream_forward", "pwgb_conv_transpose1d_stream_forward",
+    "pwgb_conv_transpose1d_window_stream_forward", "pwgb_stream_carry",
     "pwgb_resblock_pair_supported", "pwgb_resblock_pair_plan", "pwgb_resblock_pair_forward",
     "pwgb_wavenet_supported", "pwgb_wavenet_packed_bytes",
     "pwgb_wavenet_pack", "pwgb_wavenet_layer_forward", "pwgb_upsample_fir_forward", "pwgb_upsample_fir_causal_forward",

@@ -41,6 +41,11 @@ inline int check_launch(const char* what) {
 
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
+// the two history padding policies of the stream entry points (flagged slots replicate or reflect)
+__host__ __device__ inline bool is_history_pad(int pad_mode) {
+  return pad_mode == PWGB_PAD_HISTORY || pad_mode == PWGB_PAD_HISTORY_REFLECT;
+}
+
 __device__ __forceinline__ float lrelu(float v, float slope) { return v > 0.f ? v : v * slope; }
 
 // Accurate-enough transcendental helpers: tanhf/expf from libdevice (<= 2 ulp);

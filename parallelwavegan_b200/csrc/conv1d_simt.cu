@@ -35,10 +35,13 @@ struct ConvK {
   long long xbs, ybs, rbs, xcs;
   int CI_T, XW, tiles_per_group;
   // history launches: input rows [-hist_len, 0) come from hist (B, Cin, hist_len), or from sample 0 of x for an item whose
-  // rep flag is set
+  // rep flag is set (x[-t] under PWGB_PAD_HISTORY_REFLECT).  A shuffled history launch writes zero to output rows below
+  // zero_rows of an item whose zero_flag is set (the samples before 0 of a conv-transpose window).
   const float* hist;
   const int* rep;
   int hist_len;
+  const int* zero_flag;
+  int zero_rows;
 };
 
 // HIST: the history padding policy (pwgb_conv1d_stream_forward, groups 1, period 1) in the input staging loop; a template
@@ -99,13 +102,15 @@ __global__ void __launch_bounds__(256) conv1d_fwd_kernel(const ConvK p, const fl
       long long li = row0 * p.P + r;
       float v = 0.f;
       if constexpr (HIST) {
-        // rows [-hist_len, 0) from the history (or sample 0 of a replicated item), earlier rows and rows past the input zero
+        // rows [-hist_len, 0) from the history (or sample 0 of a replicated item, sample -li of a reflected one), earlier
+        // rows and rows past the input zero
         const int ch = ci0 + ci;
         const float* src = nullptr;
         if (li >= 0 && li < p.Lin)
           src = xb + (long long)ch * p.xcs + li;
         else if (li < 0 && li >= -p.hist_len)
-          src = p.rep && p.rep[b] ? xb + (long long)ch * p.xcs : p.hist + ((long long)b * p.Cin + ch) * p.hist_len + (p.hist_len + li);
+          src = p.rep && p.rep[b] ? xb + (long long)ch * p.xcs + (p.pad_mode == PWGB_PAD_HISTORY_REFLECT ? -li : 0)
+                                  : p.hist + ((long long)b * p.Cin + ch) * p.hist_len + (p.hist_len + li);
         if (src) v = lrelu(__ldg(src), p.pre_slope);
         xs[idx] = v;
         continue;
@@ -203,6 +208,12 @@ __global__ void __launch_bounds__(256) conv1d_fwd_kernel(const ConvK p, const fl
         const int of = to * p.shuffle + ph - p.shuffle_pad;  // output row
         if (of < 0 || of >= p.shuffle_tout) continue;
         yi = (long long)b * p.ybs + ((long long)cof * p.shuffle_tout + of) * p.P + jj;
+        if constexpr (HIST) {
+          if (of < p.zero_rows && p.zero_flag && p.zero_flag[b]) {
+            y[yi] = 0.f;
+            continue;
+          }
+        }
       } else {
         yi = (long long)b * p.ybs + (long long)co * p.Lout + o;
       }
@@ -410,6 +421,8 @@ static void conv_params(const pwgb_conv1d_desc* d, ConvK& p) {
   p.hist = nullptr;
   p.rep = nullptr;
   p.hist_len = 0;
+  p.zero_flag = nullptr;
+  p.zero_rows = 0;
   p.B = d->batch;
   p.Cin = d->cin;
   p.Cout = d->cout;
@@ -481,13 +494,17 @@ int conv1d_forward_simt(const pwgb_conv1d_desc* d, const float* x, const float* 
 
 // History launches (pad_mode PWGB_PAD_HISTORY, groups 1, period 1) always take the generic kernel: the few-channel
 // kernels above sum in an order that depends on where a sample sits in the sequence, which a stream cannot reproduce.
+// zero_flag / zero_rows: see ConvK (shuffled launches only).
 int conv1d_stream_simt(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len, const int* rep,
-                       const float* w, const float* bias, const float* residual, float* y, cudaStream_t st) {
+                       const float* w, const float* bias, const float* residual, float* y, cudaStream_t st,
+                       const int* zero_flag, int zero_rows) {
   ConvK p;
   conv_params(d, p);
   p.hist = hist;
   p.rep = rep;
   p.hist_len = hist_len;
+  p.zero_flag = zero_flag;
+  p.zero_rows = zero_rows;
   if (p.B == 0 || p.Lout == 0) return PWGB_OK;
   const int cg = p.Cout_g;
   if (cg >= 64) return launch_conv<8, 8, true>(p, x, w, bias, residual, y, st);

@@ -213,8 +213,8 @@ __device__ __forceinline__ long long src_sample(const TcK& p, int t0, int TT, in
 
 // The history padding policy (one more policy of src_sample, for history launches): the source of operand row r of main
 // chunk c of batch item b.  Rows [-hist_len, 0) read hist[b, c * KC + j, hist_len + ts], or x[b, c * KC + j, 0] when the
-// item's rep flag is set; rows before -hist_len and from T_in on are zero padding (ok = false).  Returns channel j = 0's
-// sample; ld: the channel stride.
+// item's rep flag is set (x[b, c * KC + j, -ts] under PWGB_PAD_HISTORY_REFLECT); rows before -hist_len and from T_in on
+// are zero padding (ok = false).  Returns channel j = 0's sample; ld: the channel stride.
 __device__ __forceinline__ const float* hist_sample(const TcK& p, const float* xc, int b, int c, int t0, int TT, int r, bool& ok,
                                                     long long& ld) {
   const long long ts = tile_sample(p, t0, TT, r);
@@ -222,7 +222,7 @@ __device__ __forceinline__ const float* hist_sample(const TcK& p, const float* x
   ok = ts >= -p.hist_len && ts < p.T_in;
   if (!ok) return xc;
   if (ts >= 0) return xc + ts;
-  if (p.rep && p.rep[b]) return xc;
+  if (p.rep && p.rep[b]) return p.pad_mode == PWGB_PAD_HISTORY_REFLECT ? xc - ts : xc;
   ld = p.hist_len;
   return p.hist + ((long long)b * p.Cin + (long long)c * KC) * p.hist_len + (p.hist_len + ts);
 }
@@ -830,7 +830,7 @@ static int tc_launch(TcK& p, size_t bytes, const float* x, const void* packed_w,
                      const float* residual, float* y, cudaStream_t st, const float* x2 = nullptr,
                      float* y2 = nullptr) {
   if (p.B == 0 || p.T_out == 0) return PWGB_OK;
-  const bool hist = p.pad_mode == PWGB_PAD_HISTORY;
+  const bool hist = is_history_pad(p.pad_mode);
   const TcKernel kernel = tc_kernel_for(p.MT, p.Cout, hist);
   if (!kernel) {
     set_error("conv1d_tc: no kernel instantiation for MT = %d, Cout = %d", p.MT, p.Cout);
@@ -865,7 +865,7 @@ int conv1d_tc_chunk(const pwgb_conv1d_desc* d, int co_off, int cout_total, const
   TcK p;
   size_t bytes = 0;
   if (!tc_plan(d, p, bytes)) return PWGB_UNSUPPORTED;
-  if (d->pad_mode == PWGB_PAD_HISTORY) {
+  if (is_history_pad(d->pad_mode)) {
     if (cin1 > 0) return PWGB_UNSUPPORTED;
     p.hist = hist;
     p.rep = rep;
@@ -977,7 +977,7 @@ static int tc_cout_chunk(int cout) {
 extern "C" int pwgb_conv1d_tc_supported(const pwgb_conv1d_desc* d) {
   if (!d || d->cout <= 0 || d->groups <= 0 || d->cin % d->groups || d->cout % d->groups) return 0;
   // history padding: plain dense convs only (pwgb_conv1d_tc_stream_forward)
-  if (d->pad_mode == PWGB_PAD_HISTORY && (d->groups != 1 || d->pre_gate || d->shuffle > 1)) return 0;
+  if (is_history_pad(d->pad_mode) && (d->groups != 1 || d->pre_gate || d->shuffle > 1)) return 0;
   const int G = d->groups;
   if (G > 1 && (d->shuffle > 1 || d->pre_gate || G > 64)) return 0;
   const int chunk = tc_cout_chunk(d->cout / G);
@@ -1033,7 +1033,7 @@ static int tc_forward(const pwgb_conv1d_desc* d, const float* x, const void* pac
 extern "C" int pwgb_conv1d_tc_forward(const pwgb_conv1d_desc* d, const float* x, const void* packed_w,
                                       const float* bias, const float* residual, float* y, void* stream) {
   PWGB_CHECK_ARG(d && x && packed_w && y, "conv1d_tc: null argument");
-  PWGB_CHECK_ARG(d->pad_mode != PWGB_PAD_HISTORY, "conv1d_tc: PWGB_PAD_HISTORY is served by pwgb_conv1d_tc_stream_forward");
+  PWGB_CHECK_ARG(!is_history_pad(d->pad_mode), "conv1d_tc: history padding is served by pwgb_conv1d_tc_stream_forward");
   return tc_forward(d, x, packed_w, bias, residual, y, stream, nullptr, nullptr, 0);
 }
 

@@ -13,7 +13,8 @@ int conv1d_tc_chunk(const pwgb_conv1d_desc* d, int co_off, int cout_total, const
                     const float* bias, float* y, cudaStream_t st, int nco, const float* x2 = nullptr, int cin1 = 0,
                     const float* hist = nullptr, const int* rep = nullptr, int hist_len = 0);
 int conv1d_stream_simt(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len, const int* rep,
-                       const float* w, const float* bias, const float* residual, float* y, cudaStream_t st);
+                       const float* w, const float* bias, const float* residual, float* y, cudaStream_t st,
+                       const int* zero_flag = nullptr, int zero_rows = 0);
 int conv1d_tc_plan_ok(const pwgb_conv1d_desc* d, int* raw_staged = nullptr);
 void tc_pack_weight(const float* w, int cin, int cout, int kernel, void* packed, cudaStream_t st);
 
@@ -187,4 +188,52 @@ extern "C" int pwgb_conv_transpose1d_stream_forward(const pwgb_convtr1d_desc* d,
   PWGB_UNSUPPORTED_IF(d->groups > 1 || d->period > 1 || d->padding != d->stride,
                       "conv_transpose1d_stream: the causal conv-transpose is dense, plain and has padding == stride");
   return convtr_forward(d, x, nullptr, 0, w, bias, y, ws, ws_bytes, stream, true, hist, replicate);
+}
+
+// The window of virtual positions [T0, T0 + n) of the whole signal's virtual conv, all phases: the virtual conv runs on x
+// (no rows with flush) with hist as its left history, and the pixel shuffle writes phase ph of position i to i * s + ph,
+// which is whole-signal sample T0 * s - padding + that.  The generic FFMA kernel sums in the same order at any position.
+extern "C" int pwgb_conv_transpose1d_window_stream_forward(const pwgb_convtr1d_desc* d, const float* x, const float* hist,
+                                                           int hist_len, const int* fresh, int flush, const float* w,
+                                                           const float* bias, float* y, void* ws, size_t ws_bytes,
+                                                           void* stream) {
+  PWGB_CHECK_ARG(d && (x || flush) && w && y && (hist || hist_len == 0), "conv_transpose1d_window_stream: null argument");
+  PWGB_CHECK_ARG(d->batch >= 0 && d->cin > 0 && d->cout > 0 && d->t_in > 0 && d->kernel > 0 && d->stride > 0 && d->padding >= 0 &&
+                     hist_len >= 0,
+                 "conv_transpose1d_window_stream: bad descriptor");
+  PWGB_CHECK_ARG((long long)d->t_out == (long long)d->t_in * d->stride,
+                 "conv_transpose1d_window_stream: t_out (%d) must be t_in (%d) * stride (%d)", d->t_out, d->t_in, d->stride);
+  PWGB_UNSUPPORTED_IF(d->groups > 1 || d->period > 1 || d->stride < 2,
+                      "conv_transpose1d_window_stream: dense, plain conv-transposes of stride >= 2 only");
+  const int s = d->stride, K = d->kernel, M = ceil_div(K, s);
+  const size_t need = pwgb_conv_transpose1d_workspace(d);
+  PWGB_CHECK_ARG(ws && ws_bytes >= need, "conv_transpose1d_window_stream: workspace too small (%zu < %zu)", ws_bytes, need);
+  cudaStream_t st = (cudaStream_t)stream;
+  float* wv = (float*)ws;
+  const long long n = (long long)d->cout * s * d->cin * M;
+  int blocks = (int)((n + 255) / 256);
+  if (blocks > 4096) blocks = 4096;
+  convtr_weight_kernel<<<blocks, 256, 0, st>>>(w, wv, d->cin, d->cout, K, s, M, 1);
+  if (const int rc = check_launch("convtr_weight_kernel")) return rc;
+  pwgb_conv1d_desc c = {};
+  c.batch = d->batch;
+  c.cin = d->cin;
+  c.cout = d->cout * s;
+  c.t_in = flush ? 0 : d->t_in;  // a flush reads no input row: every row of the chunk is zero
+  c.t_out = d->t_in;
+  c.kernel = M;
+  c.stride = 1;
+  c.dilation = 1;
+  c.groups = 1;
+  c.pad_left = M - 1;
+  c.pad_mode = PWGB_PAD_HISTORY;
+  c.period = 1;
+  c.t_valid = c.t_in;
+  c.pre_slope = d->pre_slope;
+  c.post_act = PWGB_ACT_NONE;
+  c.out_scale = 1.f;
+  c.shuffle = s;
+  c.shuffle_pad = 0;
+  c.shuffle_tout = d->t_out;
+  return conv1d_stream_simt(&c, x, hist, hist_len, nullptr, wv, bias, nullptr, y, st, fresh, d->padding);
 }

@@ -5,15 +5,20 @@
 namespace pwgb {
 
 int conv1d_stream_simt(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len, const int* rep,
-                       const float* w, const float* bias, const float* residual, float* y, cudaStream_t st);
+                       const float* w, const float* bias, const float* residual, float* y, cudaStream_t st,
+                       const int* zero_flag = nullptr, int zero_rows = 0);
 
 int conv1d_stream_check(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len, const float* y) {
   PWGB_CHECK_ARG(d && x && y, "conv1d_stream: null argument");
   PWGB_CHECK_ARG(d->batch >= 0 && d->cin > 0 && d->cout > 0 && d->t_in > 0 && d->t_out >= 0, "conv1d_stream: bad sizes");
   PWGB_CHECK_ARG(d->kernel > 0 && d->stride > 0 && d->dilation > 0 && d->groups > 0 && d->pad_left >= 0,
                  "conv1d_stream: bad kernel geometry");
-  PWGB_CHECK_ARG(d->pad_mode == PWGB_PAD_HISTORY, "conv1d_stream: pad_mode must be PWGB_PAD_HISTORY");
+  PWGB_CHECK_ARG(is_history_pad(d->pad_mode), "conv1d_stream: pad_mode must be PWGB_PAD_HISTORY or PWGB_PAD_HISTORY_REFLECT");
   PWGB_CHECK_ARG(hist_len >= 0 && (hist_len == 0 || hist), "conv1d_stream: bad history (hist_len %d)", hist_len);
+  // a reflected row -t reads sample t <= pad_left of the chunk itself
+  PWGB_CHECK_ARG(d->pad_mode != PWGB_PAD_HISTORY_REFLECT || (d->pad_left < d->t_in && hist_len <= d->pad_left),
+                 "conv1d_stream: reflect needs pad_left (%d) < t_in (%d) and hist_len (%d) <= pad_left", d->pad_left, d->t_in,
+                 hist_len);
   PWGB_UNSUPPORTED_IF(d->stride != 1 || d->groups != 1 || d->period > 1 || d->pre_gate || d->shuffle > 1,
                       "conv1d_stream: history padding serves plain stride-1 convs (groups 1, period 1, no pre_gate, one source)");
   PWGB_UNSUPPORTED_IF(d->x_batch_stride || d->y_batch_stride || d->r_batch_stride || (d->t_valid > 0 && d->t_valid != d->t_in),

@@ -389,12 +389,14 @@ def upsample_fir_causal_stream(x, fir, scale, hist_in, hist_out, out_channels=No
     return out
 
 
-def conv1d_stream(x, hist, w, bias=None, *, pad_left, dilation=1, replicate=None, pre_slope=1.0, post_act=None, post_slope=0.0,
-                  residual=None, out_scale=1.0, out=None, accumulate=False):
+def conv1d_stream(x, hist, w, bias=None, *, pad_left, dilation=1, replicate=None, reflect=False, pre_slope=1.0, post_act=None,
+                  post_slope=0.0, residual=None, out_scale=1.0, out=None, accumulate=False):
     """conv1d with history padding (pwgb_conv1d_stream_forward / pwgb_conv1d_tc_stream_forward): of the ``pad_left`` rows
     in front of x, the last H read ``hist`` (B, cin, H) -- or x[:, :, 0] for the items whose ``replicate`` (B,) int32 flag
-    is set -- and the earlier ones are zero; no right padding.  Everything else is conv1d's, and so is the engine choice
-    (including the 16-column and 32-channel paddings of conv1d), so a chunked run equals conv1d on the whole signal."""
+    is set -- and the earlier ones are zero; no right padding.  With ``reflect`` a flagged item reads row -t from x[:, :, t]
+    instead (ReflectionPad1d for a fresh signal, PWGB_PAD_HISTORY_REFLECT; needs pad_left < x's length).  Everything else
+    is conv1d's, and so is the engine choice (including the 16-column and 32-channel paddings of conv1d), so a chunked run
+    equals conv1d on the whole signal."""
     x, w = _dev(x, "x"), _dev(w, "w")
     B, cin, L = x.shape
     cout, cin_w, K = w.shape
@@ -405,7 +407,8 @@ def conv1d_stream(x, hist, w, bias=None, *, pad_left, dilation=1, replicate=None
         raise PwgbError(f"conv1d_stream: x {tuple(x.shape)}, hist {tuple(hist.shape)} and weight {tuple(w.shape)} do not match")
     if replicate is not None and (replicate.dtype != torch.int32 or not replicate.is_cuda or replicate.numel() != B):
         raise PwgbError(f"conv1d_stream: replicate must be {B} int32 flags on the device")
-    kw = dict(pad_left=pad_left, dilation=dilation, replicate=replicate, pre_slope=pre_slope, post_act=post_act, post_slope=post_slope)
+    kw = dict(pad_left=pad_left, dilation=dilation, replicate=replicate, reflect=reflect, pre_slope=pre_slope, post_act=post_act,
+              post_slope=post_slope)
     if ENGINE != "simt" and cout < 16 and cin >= 256 and cin % 32 == 0 and residual is None and out is None and not accumulate:
         # as _conv1d_fewcout: the weight padded to 16 output channels for the tensor cores
         b16 = torch.nn.functional.pad(bias, (0, 16 - cout)) if bias is not None else None
@@ -436,15 +439,15 @@ def conv1d_stream(x, hist, w, bias=None, *, pad_left, dilation=1, replicate=None
     if bias is not None:
         bias = _dev(bias, "bias")
     H = hist.shape[-1]
-    dkey = ("stream", B, cin, cout, L, t_out, K, dilation, pad_left, float(pre_slope), post_act, float(post_slope), float(out_scale),
-            bool(accumulate))
+    dkey = ("stream", B, cin, cout, L, t_out, K, dilation, pad_left, bool(reflect), float(pre_slope), post_act, float(post_slope),
+            float(out_scale), bool(accumulate))
     d = _DESC_CACHE.get(dkey)
     if d is None:
         if len(_DESC_CACHE) > 4096:
             _DESC_CACHE.clear()
         d = _DESC_CACHE[dkey] = capi.Conv1dDesc(
             batch=B, cin=cin, cout=cout, t_in=L, t_out=t_out, kernel=K, stride=1, dilation=dilation, groups=1, pad_left=pad_left,
-            pad_mode=capi.PAD_HISTORY, period=1, t_valid=L, pre_slope=float(pre_slope), pre_gate=0, post_act=_ACT[post_act],
+            pad_mode=capi.PAD_HISTORY_REFLECT if reflect else capi.PAD_HISTORY, period=1, t_valid=L, pre_slope=float(pre_slope), pre_gate=0, post_act=_ACT[post_act],
             post_slope=float(post_slope), out_scale=float(out_scale), accumulate=int(bool(accumulate)))
     prof = _Prof("conv1d_stream", 2.0 * B * cout * t_out * cin * K,
                  4.0 * (x.numel() + out.numel() * (2 if accumulate else 1) + (residual.numel() if residual is not None else 0)),
@@ -492,6 +495,51 @@ def conv_transpose1d_stream(x, hist, w, bias=None, *, stride, replicate=None, pr
     rc = lib.pwgb_conv_transpose1d_stream_forward(C.byref(d), _p(x), _p(hist), _p(replicate), _p(w), _p(bias), _p(y), _p(ws),
                                                   C.c_size_t(nbytes), _stream())
     capi.check(rc, "pwgb_conv_transpose1d_stream_forward")
+    prof.done()
+    return y
+
+
+def conv_transpose1d_window_stream(x, hist, w, bias=None, *, stride, padding, fresh=None, flush_rows=0, out=None):
+    """A window of conv_transpose1d over a streamed signal (pwgb_conv_transpose1d_window_stream_forward): x (B, cin, n) is
+    the signal's next chunk and hist (B, cin, H) its rows in front of it (H >= ceil(K / stride) - 1).  Returns (B, cout,
+    n * stride): the whole-signal conv_transpose1d(..., stride, padding) samples from chunk_start * stride - padding on,
+    so the window lags its input by ``padding`` samples.  Items whose ``fresh`` (B,) int32 flag is set are at the start of
+    their signal and get zeros for the ``padding`` samples before 0.  ``flush_rows`` > 0 (x None): the signal has ended,
+    and the window runs over that many zero rows.  Always the FFMA kernel: bit-identical to the whole-signal call when that
+    takes the FFMA kernel too (the PQMF synthesis, 4 -> 1 channels)."""
+    w, hist = _dev(w, "w"), _dev(hist, "hist")
+    if w.dim() != 3 or hist.dim() != 3 or hist.shape[1] != w.shape[0]:
+        raise PwgbError(f"conv_transpose1d_window_stream: hist {tuple(hist.shape)} and weight {tuple(w.shape)} do not match")
+    B, cin, H = hist.shape
+    if flush_rows:
+        if x is not None:
+            raise PwgbError("conv_transpose1d_window_stream: a flush reads no input (x must be None)")
+        n = int(flush_rows)
+    else:
+        x = _dev(x, "x")
+        if x.dim() != 3 or tuple(x.shape[:2]) != (B, cin):
+            raise PwgbError(f"conv_transpose1d_window_stream: x {tuple(x.shape)} does not match hist {tuple(hist.shape)}")
+        n = x.shape[-1]
+    if fresh is not None and (fresh.dtype != torch.int32 or not fresh.is_cuda or fresh.numel() != B):
+        raise PwgbError(f"conv_transpose1d_window_stream: fresh must be {B} int32 flags on the device")
+    cout, K = w.shape[1], w.shape[2]
+    if bias is not None:
+        bias = _dev(bias, "bias")
+    d = capi.ConvTr1dDesc(batch=B, cin=cin, cout=cout, t_in=n, t_out=n * stride, kernel=K, stride=stride, padding=padding,
+                          pre_slope=1.0, groups=1, period=1)
+    lib = capi.lib()
+    nbytes = lib.pwgb_conv_transpose1d_workspace(C.byref(d))
+    ws = torch.empty((nbytes + 3) // 4, device=w.device, dtype=torch.float32)
+    y = torch.empty((B, cout, n * stride), device=w.device, dtype=torch.float32) if out is None else out
+    if tuple(y.shape) != (B, cout, n * stride) or not y.is_contiguous() or y.dtype != torch.float32:
+        raise PwgbError(f"conv_transpose1d_window_stream: out must be a contiguous float32 {(B, cout, n * stride)} tensor")
+    if y.numel() == 0:
+        return y
+    prof = _Prof("conv_transpose1d_window_stream", 2.0 * B * cout * n * stride * cin * ((K + stride - 1) // stride),
+                 4.0 * (B * cin * n + y.numel()), f"B{B} cin{cin} cout{cout} k{K} s{stride} n{n}")
+    rc = lib.pwgb_conv_transpose1d_window_stream_forward(C.byref(d), _p(x), _p(hist) if H else None, H, _p(fresh), int(bool(flush_rows)),
+                                                         _p(w), _p(bias), _p(y), _p(ws), C.c_size_t(nbytes), _stream())
+    capi.check(rc, "pwgb_conv_transpose1d_window_stream_forward")
     prof.done()
     return y
 

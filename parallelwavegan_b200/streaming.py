@@ -1,5 +1,6 @@
 """Chunked synthesis with the causal generators: mel frames in, waveform out, while the frames are still arriving.
-``CausalPWGStream`` streams a causal Parallel WaveGAN, ``CausalHiFiGANStream`` a causal HiFi-GAN.
+``CausalPWGStream`` streams a causal Parallel WaveGAN, ``CausalHiFiGANStream`` a causal HiFi-GAN, ``CausalMelGANStream``
+a causal (multi-band) MelGAN.
 
 A causal generator's output for frame j depends only on frames <= j, so it can be synthesised as soon as frame j
 exists.  ``CausalPWGStream`` carries, per batch slot, everything the whole-utterance forward would read from before
@@ -416,3 +417,236 @@ class CausalHiFiGANStream(_ChunkStream):
         c = c.transpose(1, 2).contiguous()
         y = self._run(c.shape[-1], c)
         return y if self.use_graphs else y.clone()
+
+
+class CausalMelGANStream(_ChunkStream):
+    """Streams a causal ``MelGANGenerator`` (``use_causal_conv=True``), full-band or multi-band with ``model.pqmf``, chunk
+    by chunk for ``batch`` independent slots.
+
+    ``push(c)`` takes the next n mel frames of every slot and returns their n * hop * subbands samples; n may change from
+    push to push.  ``flush(items)`` returns the ``delay`` samples the slots still hold and restarts them.  For every slot,
+    the concatenated pushes and flush equal ``[zeros(delay) | model.inference(all_frames)]``.  Without PQMF ``delay`` is
+    0; with it the centred synthesis filter reads ``taps // 2`` samples ahead, so the stream lags by that many samples
+    and the flush computes the tail against the zero right padding.
+
+    Every conv pads only on the left, with the model's pad (reflect, replicate or zero ``ConstantPad1d``).  A reflected
+    row -t is sample t of the same signal, so the first push after a reset must hold every such sample:
+    ``min_first_frames`` frames (7 for the recipes' kernel-7 input conv; 1 for the other pads).  The stream keeps, per
+    slot, one history per signal:
+
+    * the input conv: the last kernel_size - 1 mel frames; a fresh slot starts from what the pad would read (frames
+      P .. 1 for reflect, frame 0 repeated for replicate, zeros); it runs as a valid conv on [history | chunk];
+    * each conv-transpose: the last frame of its input, replicated from the first frame for a fresh slot;
+    * each ResidualStack: its last (k - 1) * d input samples (the two 1x1 convs need none); with replicate padding a
+      chunk shorter than that first sets a fresh slot's history to its first sample, since the carry keeps those rows;
+    * the output conv: its last kernel_size - 1 input samples;
+    * with PQMF: the last ceil((taps + 1) / subbands) - 1 subband samples of the synthesis input.
+
+    The dilated convs read their histories in their loaders (pwgb_conv1d_stream_forward / pwgb_conv1d_tc_stream_forward),
+    reflecting or replicating for the slots whose fresh flag is set; the synthesis is a window of the conv-transpose
+    (pwgb_conv_transpose1d_window_stream_forward) that writes zeros before sample 0 of a fresh slot.  One
+    pwgb_stream_carry launch per push updates every history, and the fresh flags are cleared inside the same captured
+    work.  With ``use_graphs`` each chunk length is captured once into a CUDA graph and replayed.  The weights are read
+    when the stream is built and must not change while it is used."""
+
+    def __init__(self, model, batch=1, use_graphs=True):
+        from .layers import CausalConv1d, CausalConvTranspose1d, ResidualStack
+        from .models import MelGANGenerator
+
+        if not isinstance(model, MelGANGenerator):
+            raise PwgbError("CausalMelGANStream: expected a MelGANGenerator")
+        mods = list(model.melgan)
+        if not isinstance(mods[0], CausalConv1d):
+            raise PwgbError("CausalMelGANStream: the model is not causal (use_causal_conv=False); a centred model needs lookahead")
+        self._setup(model, batch, use_graphs)
+        dev, B = self.dev, self.B
+
+        def wb(conv):
+            return effective_weight(conv).detach().contiguous(), (conv.bias.detach() if conv.bias is not None else None)
+
+        def zeros(*shape):
+            return torch.zeros(shape, device=dev, dtype=torch.float32)
+
+        self.slope, self.pad = model.slope, model.pad_mode
+        ic = mods[0]
+        self.w_in = wb(ic.conv)
+        self.in_channels = ic.conv.in_channels
+        self.cin_hist = zeros(B, self.in_channels, ic.left)
+        reflect_need = [(ic.left, 1)]  # (left padding, input samples per frame) of every conv the pad applies to
+        self.hop, self.levels, oc = 1, [], None
+        for m in mods[1:]:
+            if isinstance(m, CausalConvTranspose1d):
+                if not isinstance(m.pad, torch.nn.ReplicationPad1d):
+                    raise PwgbError("CausalMelGANStream: only the ReplicationPad1d conv-transpose of MelGANGenerator is supported")
+                self.hop *= m.stride
+                self.levels.append(dict(stride=m.stride, channels=m.deconv.out_channels, w=wb(m.deconv),
+                                        up_hist=zeros(B, m.deconv.in_channels, 1), rate=self.hop, stacks=[]))
+            elif isinstance(m, ResidualStack):
+                k, d = m.kernel_size, m.dilation
+                C = m.skip_layer.in_channels
+                self.levels[-1]["stacks"].append(dict(k=k, d=d, w1=wb(m.stack[1].conv), w2=wb(m.stack[3]), ws=wb(m.skip_layer),
+                                                      hist=zeros(B, C, (k - 1) * d)))
+                reflect_need.append(((k - 1) * d, self.hop))
+            elif isinstance(m, CausalConv1d):
+                oc = m
+        self.w_out = wb(oc.conv)
+        self.out_hist = zeros(B, oc.conv.in_channels, oc.left)
+        self.out_channels = oc.conv.out_channels
+        self.post_act = "tanh" if model.use_final_nonlinear_activation else None
+        reflect_need.append((oc.left, self.hop))
+        # the smallest first push after a reset for which every reflected row lies inside the chunk
+        self.min_first_frames = max(P // rate + 1 for P, rate in reflect_need) if self.pad == "reflect" else 1
+        pq = model.pqmf
+        if pq is not None:
+            N = pq.subbands
+            if self.out_channels != N:
+                raise PwgbError(f"CausalMelGANStream: {self.out_channels} output channels for a {N}-band PQMF")
+            # PQMF.synthesis's transposed FIR, computed as there
+            self.w_syn = (pq.synthesis_filter[0].flip(-1) * float(N)).unsqueeze(1).contiguous()
+            self.subbands, self.delay = N, pq.taps // 2
+            self.pq_hist = zeros(B, N, -(-(pq.taps + 1) // N) - 1)
+            # a fresh slot's first window also holds the delay's zeros before sample 0
+            self.min_first_frames = max(self.min_first_frames, -(-self.delay // (self.hop * N)))
+        else:
+            self.subbands, self.delay, self.pq_hist = 1, 0, None
+        self.fresh = torch.ones(B, device=dev, dtype=torch.int32)  # per-slot flags: the slot's signal starts in this push
+        self._fresh = [True] * B  # the same, on the host (the input conv's history is filled in push)
+
+    # ---------------------------------------------------------------------------------------------------- state
+    def _state(self):
+        hs = [self.cin_hist, self.out_hist, self.fresh]
+        for lv in self.levels:
+            hs += [lv["up_hist"]] + [st["hist"] for st in lv["stacks"]]
+        return hs + ([self.pq_hist] if self.pq_hist is not None else [])
+
+    def state_bytes(self):
+        """bytes of carried state per slot"""
+        return sum(t.numel() * t.element_size() for t in self._state() if t is not self.fresh) // self.B
+
+    def reset(self, items=None):
+        """Restart slots ``items`` (an index or an iterable of indices; None: every slot) as fresh signals.  The other
+        slots continue unaffected."""
+        for b in self._slots(items):
+            for h in self._state():
+                if h is not self.fresh:
+                    h[b].zero_()
+            self.fresh[b] = 1
+            self._fresh[b] = True
+
+    # ---------------------------------------------------------------------------------------------------- compute
+    def _pad_kw(self, P, rate, n):
+        """the history policy of a conv with left padding P over an input of ``rate`` samples per frame"""
+        if self.pad == "replicate":
+            return dict(replicate=self.fresh)
+        if self.pad == "reflect" and P < n * rate:
+            # a chunk too short to reflect in never holds a fresh slot (push refuses it)
+            return dict(replicate=self.fresh, reflect=True)
+        return {}
+
+    def _new_entry(self, n):
+        """The buffers of every intermediate signal of an n-frame chunk, and the carry table over them."""
+        dev, B = self.dev, self.B
+
+        def empty(*shape):
+            return torch.empty(shape, device=dev, dtype=torch.float32)
+
+        K_in = self.cin_hist.shape[-1]
+        ent = dict(xin=empty(B, self.in_channels, K_in + n), h0=empty(B, self.levels[0]["w"][0].shape[0], n), levels=[])
+        entries = [(ent["xin"], self.cin_hist)]
+        t, prev = n, ent["h0"]
+        for lv in self.levels:
+            t *= lv["stride"]
+            C = lv["channels"]
+            buf = dict(u=empty(B, C, t), h=empty(B, C, t), s=empty(B, C, t), x=[empty(B, C, t) for _ in lv["stacks"]])
+            entries.append((prev, lv["up_hist"]))
+            x = buf["u"]
+            for j, st in enumerate(lv["stacks"]):
+                entries.append((x, st["hist"]))
+                x = buf["x"][j]
+            ent["levels"].append(buf)
+            prev = x
+        entries.append((prev, self.out_hist))
+        ent["y"] = empty(B, self.out_channels, t)
+        if self.pq_hist is not None:
+            entries.append((ent["y"], self.pq_hist))
+            ent["wave"] = empty(B, 1, t * self.subbands)
+        # every history is read before this one carry, at the end of the push
+        ent["table"] = ops.stream_carry_table(entries, dev)
+        return ent
+
+    def _step(self, c):
+        """One chunk: c (B, in_channels, n) -> (B, 1, n * hop * subbands).  Advances the state."""
+        n = c.shape[-1]
+        ent = self._entry(n)
+        K_in = self.cin_hist.shape[-1]
+        xin = ent["xin"]
+        xin[:, :, :K_in].copy_(self.cin_hist)
+        xin[:, :, K_in:].copy_(c)
+        h = ops.conv1d(xin, self.w_in[0], self.w_in[1], out=ent["h0"])
+        slope = self.slope
+        for lv, buf in zip(self.levels, ent["levels"]):
+            x = ops.conv_transpose1d_stream(h, lv["up_hist"], lv["w"][0], lv["w"][1], stride=lv["stride"], replicate=self.fresh,
+                                            pre_slope=slope, out=buf["u"])
+            for j, st in enumerate(lv["stacks"]):
+                P = (st["k"] - 1) * st["d"]
+                if self.pad == "replicate" and n * lv["rate"] < P:
+                    # the carry keeps rows in front of a chunk shorter than the history: a fresh slot's must be its pad
+                    torch.where(self.fresh.bool()[:, None, None], x[:, :, :1], st["hist"], out=st["hist"])
+                hh = ops.conv1d_stream(x, st["hist"], *st["w1"], pad_left=P, dilation=st["d"], pre_slope=slope, out=buf["h"],
+                                       **self._pad_kw(P, lv["rate"], n))
+                s = ops.conv1d(x, *st["ws"], out=buf["s"])
+                x = ops.conv1d(hh, *st["w2"], pre_slope=slope, residual=s, out=buf["x"][j])
+            h = x
+        P = self.out_hist.shape[-1]
+        y = ops.conv1d_stream(h, self.out_hist, *self.w_out, pad_left=P, pre_slope=slope, post_act=self.post_act, out=ent["y"],
+                              **self._pad_kw(P, self.hop, n))
+        if self.pq_hist is not None:
+            y = ops.conv_transpose1d_window_stream(y, self.pq_hist, self.w_syn, None, stride=self.subbands, padding=self.delay,
+                                                   fresh=self.fresh, out=ent["wave"])
+        ops.stream_carry(ent["table"])
+        self.fresh.zero_()
+        return y
+
+    @torch.no_grad()
+    def push(self, c, normalize_before=False):
+        """c: (B, n, in_channels) mel frames ((n, in_channels) when batch == 1); n >= ``min_first_frames`` for a slot's
+        first push after a reset.  Returns (B, 1, n * hop * subbands) on the device."""
+        m = self.model
+        self._check_eval(m)
+        c = torch.as_tensor(c, dtype=torch.float32, device=self.dev)
+        if c.dim() == 2 and self.B == 1:
+            c = c.unsqueeze(0)
+        if c.dim() != 3 or c.shape[0] != self.B or c.shape[2] != self.in_channels or c.shape[1] < 1:
+            raise PwgbError(f"CausalMelGANStream.push: c must be ({self.B}, n >= 1, {self.in_channels}), got {tuple(c.shape)}")
+        n = c.shape[1]
+        fresh = [b for b in range(self.B) if self._fresh[b]]
+        if fresh and n < self.min_first_frames:
+            raise PwgbError(f"CausalMelGANStream.push: the first push after a reset needs at least {self.min_first_frames} frames "
+                            f"(the reflect padding reads that far into the signal), got {n} for slots {fresh}")
+        if normalize_before:
+            c = (c - m.mean) / m.scale
+        c = c.transpose(1, 2).contiguous()
+        P = self.cin_hist.shape[-1]
+        for b in fresh:  # the input conv's pad for a fresh slot (zero: the reset's zeros)
+            if self.pad == "reflect":
+                self.cin_hist[b].copy_(c[b, :, 1:P + 1].flip(-1))
+            elif self.pad == "replicate":
+                self.cin_hist[b].copy_(c[b, :, :1].expand(-1, P))
+        self._fresh = [False] * self.B
+        y = self._run(n, c)
+        return y if self.use_graphs else y.clone()
+
+    @torch.no_grad()
+    def flush(self, items=None):
+        """The last ``delay`` samples of slots ``items`` (an index, an iterable of indices or None for every slot), computed
+        against the zero right padding, as (len(items), 1, delay); the slots are then reset."""
+        items = self._slots(items)
+        if self.pq_hist is None:
+            y = torch.zeros((len(items), 1, 0), device=self.dev, dtype=torch.float32)
+        else:
+            rows = -(-self.delay // self.subbands)
+            y = ops.conv_transpose1d_window_stream(None, self.pq_hist, self.w_syn, None, stride=self.subbands, padding=self.delay,
+                                                   fresh=self.fresh, flush_rows=rows)
+            y = y[list(items), :, :self.delay].contiguous()
+        self.reset(items)
+        return y
