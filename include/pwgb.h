@@ -393,12 +393,12 @@ PWGB_API int pwgb_upsample_fir_forward(int rows, int rows_per_batch, int t_in, i
  * so output frame j only meets input frames j-2, j-1, j.  Same arguments and layout as the centred pair. */
 PWGB_API int pwgb_upsample_fir_causal_forward(int rows, int rows_per_batch, int t_in, int scale, const float* x, const float* fir,
                                      float* y, long long y_batch_stride, void* stream);
-/* The causal stage of a stream: input frames -2 and -1 come from hist_in (rows x 2 fp32, oldest first) instead of zero,
- * and hist_out (rows x 2, not aliasing hist_in) receives the last two frames of [hist_in | x].  Every output is the same
- * fp32 expression as in pwgb_upsample_fir_causal_forward, so chunked runs equal the whole-signal stage bit for bit. */
+/* The causal stage of a stream: input frames -2 and -1 come from hist_in (rows x 2 fp32, oldest first) instead of zero;
+ * hist_in is only read (the caller carries it, e.g. with pwgb_stream_carry).  Every output is the same fp32 expression
+ * as in pwgb_upsample_fir_causal_forward, so chunked runs equal the whole-signal stage bit for bit. */
 PWGB_API int pwgb_upsample_fir_causal_stream_forward(int rows, int rows_per_batch, int t_in, int scale, const float* x,
                                             const float* fir, float* y, long long y_batch_stride, const float* hist_in,
-                                            float* hist_out, void* stream);
+                                            void* stream);
 PWGB_API int pwgb_upsample_fir_causal_backward(int rows, int rows_per_batch, int t_in, int scale, const float* x, const float* fir,
                                       const float* gy, long long gy_batch_stride, float* gx, float* dfir, void* stream);
 

@@ -168,7 +168,7 @@ def lib():
         fn.restype = C.c_int
         fn.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_longlong, vp]
     L.pwgb_upsample_fir_causal_stream_forward.restype = C.c_int
-    L.pwgb_upsample_fir_causal_stream_forward.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_longlong, vp, vp, vp]
+    L.pwgb_upsample_fir_causal_stream_forward.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_longlong, vp, vp]
     L.pwgb_mr_stft_loss_workspace.restype = C.c_size_t
     L.pwgb_mr_stft_loss_workspace.argtypes = [C.POINTER(StftDesc), C.c_int]
     L.pwgb_mr_stft_loss_forward.restype = C.c_int

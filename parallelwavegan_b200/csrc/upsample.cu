@@ -4,7 +4,7 @@
 // same FIR with its tap origin at 2s instead of s: every output meets the input frames one frame earlier.  `lag` is
 // that shift in frames (0 centred, 1 causal); the per-phase coefficients do not depend on it.
 // The streaming form of the causal stage (HIST) takes frames -2 and -1 from a carried state instead of the zero
-// padding, and hands the last two frames of [state | x] on, so that a chunked run equals the whole-signal stage.
+// padding, so that a chunked run equals the whole-signal stage; the caller carries the state from chunk to chunk.
 #include "common.cuh"
 
 namespace pwgb {
@@ -13,12 +13,12 @@ namespace pwgb {
 // taps pre-summed per phase (A: taps that land in frame j-1, ...).  One thread per input frame writes its s outputs
 // (one 16-byte store per 4): 3 FMAs per output instead of 2s+1 taps with an integer division each (the tap loop ran
 // at 1/12 of the HBM rate: 13 % of the Parallel WaveGAN forward).
-// HIST (causal, lag 1): frames j-2 and j-1 below 0 are hist_in[r][j] and hist_in[r][1] (rows x 2, oldest first); the
-// thread of the last frame writes frames t_in-2, t_in-1 of [hist_in | x] to hist_out.  Same three-FMA expression.
+// HIST (causal, lag 1): frames j-2 and j-1 below 0 are hist_in[r][j] and hist_in[r][1] (rows x 2, oldest first).  Same
+// three-FMA expression.
 template <bool HIST>
 __global__ void upsample_fir_kernel(int rows, int rows_per_batch, int t_in, int s, int lag, const float* __restrict__ x,
                                     const float* __restrict__ fir, float* __restrict__ y, long long ybs,
-                                    const float* __restrict__ hist_in, float* __restrict__ hist_out) {
+                                    const float* __restrict__ hist_in) {
   extern __shared__ float coef[];  // [3][s]
   for (int ph = threadIdx.x; ph < s; ph += blockDim.x) {
     float a = 0.f, bsum = 0.f, c = 0.f;
@@ -49,10 +49,6 @@ __global__ void upsample_fir_kernel(int rows, int rows_per_batch, int t_in, int 
       xm = j >= 2 ? __ldg(xr + j - 2) : __ldg(hr + j);
       x0 = j >= 1 ? __ldg(xr + j - 1) : __ldg(hr + 1);
       xp = __ldg(xr + j);
-      if (j == t_in - 1) {
-        hist_out[2 * (long long)r] = x0;
-        hist_out[2 * (long long)r + 1] = xp;
-      }
     } else {
       const int jc = j - lag;
       xm = jc > 0 ? __ldg(xr + jc - 1) : 0.f;
@@ -80,8 +76,7 @@ __global__ void upsample_fir_kernel(int rows, int rows_per_batch, int t_in, int 
 using namespace pwgb;
 
 static int upsample_fir_forward(int rows, int rows_per_batch, int t_in, int scale, int lag, const float* x, const float* fir,
-                                float* y, long long y_batch_stride, void* stream, const float* hist_in = nullptr,
-                                float* hist_out = nullptr) {
+                                float* y, long long y_batch_stride, void* stream, const float* hist_in = nullptr) {
   PWGB_CHECK_ARG(x && fir && y, "upsample_fir: null argument");
   PWGB_CHECK_ARG(rows >= 0 && rows_per_batch > 0 && t_in > 0 && scale > 0 && rows % rows_per_batch == 0,
                  "upsample_fir: bad sizes");
@@ -93,10 +88,10 @@ static int upsample_fir_forward(int rows, int rows_per_batch, int t_in, int scal
   const size_t smem = 3 * scale * sizeof(float);
   if (hist_in)
     upsample_fir_kernel<true><<<grid, 256, smem, (cudaStream_t)stream>>>(rows, rows_per_batch, t_in, scale, lag, x, fir, y, ybs,
-                                                                         hist_in, hist_out);
+                                                                         hist_in);
   else
     upsample_fir_kernel<false><<<grid, 256, smem, (cudaStream_t)stream>>>(rows, rows_per_batch, t_in, scale, lag, x, fir, y, ybs,
-                                                                          nullptr, nullptr);
+                                                                          nullptr);
   return check_launch("upsample_fir_kernel");
 }
 
@@ -112,8 +107,7 @@ extern "C" int pwgb_upsample_fir_causal_forward(int rows, int rows_per_batch, in
 
 extern "C" int pwgb_upsample_fir_causal_stream_forward(int rows, int rows_per_batch, int t_in, int scale, const float* x,
                                                        const float* fir, float* y, long long y_batch_stride, const float* hist_in,
-                                                       float* hist_out, void* stream) {
-  PWGB_CHECK_ARG(hist_in && hist_out, "upsample_fir_causal_stream: null history");
-  PWGB_CHECK_ARG(hist_in != hist_out, "upsample_fir_causal_stream: hist_out must not alias hist_in");
-  return upsample_fir_forward(rows, rows_per_batch, t_in, scale, 1, x, fir, y, y_batch_stride, stream, hist_in, hist_out);
+                                                       void* stream) {
+  PWGB_CHECK_ARG(hist_in, "upsample_fir_causal_stream: null history");
+  return upsample_fir_forward(rows, rows_per_batch, t_in, scale, 1, x, fir, y, y_batch_stride, stream, hist_in);
 }

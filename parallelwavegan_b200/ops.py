@@ -367,23 +367,28 @@ def upsample_fir(x, fir, scale, out=None, out_channels=None, causal=False):
     return out
 
 
-def upsample_fir_causal_stream(x, fir, scale, hist_in, hist_out, out_channels=None):
+def upsample_fir_causal_stream(x, fir, scale, hist, out=None, out_channels=None):
     """The causal upsampler stage of a stream (pwgb_upsample_fir_causal_stream_forward): ``upsample_fir(..., causal=True)``
-    with input frames -2 and -1 read from ``hist_in`` (B*C, 2) instead of the zero padding; ``hist_out`` (B*C, 2)
-    receives the last two frames of [hist_in | x].  Bit-identical to the whole-signal stage on the concatenation."""
+    with input frames -2 and -1 read from ``hist`` ((B, C, 2) or (B*C, 2), contiguous) instead of the zero padding.  The
+    history is only read; the caller carries it (``stream_carry``).  ``out`` and ``out_channels`` as in ``upsample_fir``:
+    a given ``out`` with more than C channels must hold zeros in the others.  Bit-identical to the whole-signal stage on
+    the concatenation."""
     x = _dev(x, "x")
     fir = _dev(fir, "fir").reshape(-1)
-    hist_in, hist_out = _dev(hist_in, "hist_in"), _dev(hist_out, "hist_out")
+    hist = _dev(hist, "hist")
     B, Cc, T = x.shape
     if fir.numel() != 2 * scale + 1:
         raise PwgbError("upsample_fir: filter must have 2*scale+1 taps")
-    if tuple(hist_in.shape) != (B * Cc, 2) or tuple(hist_out.shape) != (B * Cc, 2):
-        raise PwgbError(f"upsample_fir_causal_stream: histories must be ({B * Cc}, 2)")
+    if hist.numel() != B * Cc * 2 or hist.shape[-1] != 2 or not hist.is_contiguous():
+        raise PwgbError(f"upsample_fir_causal_stream: the history must be a contiguous ({B}, {Cc}, 2) tensor")
     oc = Cc if out_channels is None else int(out_channels)
-    out = (torch.zeros if oc != Cc else torch.empty)((B, oc, T * scale), device=x.device, dtype=torch.float32)
+    if out is None:
+        out = (torch.zeros if oc != Cc else torch.empty)((B, oc, T * scale), device=x.device, dtype=torch.float32)
+    elif tuple(out.shape) != (B, oc, T * scale) or not out.is_contiguous() or out.dtype != torch.float32:
+        raise PwgbError(f"upsample_fir_causal_stream: out must be a contiguous float32 {(B, oc, T * scale)} tensor")
     prof = _Prof("upsample_fir", 2.0 * B * Cc * T * scale * (2 * scale + 1), 4.0 * (x.numel() + B * Cc * T * scale), f"B{B} C{Cc} T{T} s{scale}")
     rc = capi.lib().pwgb_upsample_fir_causal_stream_forward(B * Cc, Cc, T, int(scale), _p(x), _p(fir), _p(out), oc * T * scale,
-                                                            _p(hist_in), _p(hist_out), _stream())
+                                                            _p(hist), _stream())
     capi.check(rc, "pwgb_upsample_fir_causal_stream_forward")
     prof.done()
     return out

@@ -9,7 +9,8 @@ the current chunk:
 * conv_in (ConvInUpsampleNetwork): the last ``aux_context_window`` mel frames.  A fresh slot starts from its first
   frame replicated, as ``ReplicationPad1d`` does in ``inference``; conv_in then runs as a valid conv on
   [history | chunk];
-* every causal FIR stage of the upsampler: its last two input frames (pwgb_upsample_fir_causal_stream_forward);
+* every causal FIR stage of the upsampler: its last two input frames, read by pwgb_upsample_fir_causal_stream_forward;
+  these and the conv_in history are updated by one pwgb_stream_carry after the last FIR stage;
 * every WaveNet layer l: its last H_l = (kernel - 1) * dilation_l input samples, in the packed residual stream's
   operand layout.  A causal layer reads only those rows in front of sample 0, so one copy per layer boundary
   (pwgb_wnstack_carry) puts the history where the whole-utterance forward has the previous samples, and the unchanged
@@ -36,14 +37,30 @@ def _layer_weights(f, A):
                                       cache=f._cache, key=k, causal=True)
 
 
+def wb(conv):
+    """(weight, bias) of a conv container, read once when a stream is built"""
+    return effective_weight(conv).detach().contiguous(), (conv.bias.detach() if conv.bias is not None else None)
+
+
 class _ChunkStream:
-    """Plumbing shared by the streams: slot validation, one cached entry per chunk length (at most
-    ``MAX_CHUNK_LENGTHS``), and one CUDA graph per chunk length captured after an eager warm-up whose state changes are
-    undone.  A subclass provides ``_state()`` (the tensors a push advances), ``_new_entry(n)`` and ``_step(*inputs)``."""
+    """Plumbing shared by the streams:
+
+    * slot validation, and ``reset`` / ``state_bytes`` over the batch-leading state tensors of ``_state()``;
+    * the mel frames of a push, checked, normalised if asked and laid out as (B, C, n);
+    * the input conv's history of ``history`` frames: a fresh slot's is filled as the model's pad (``"zero"``,
+      ``"replicate"`` or ``"reflect"``) would fill it, and ``_input`` copies [history | chunk] into the entry's ``xin``
+      buffer, which the subclass's carry table carries into the history;
+    * the fresh slots: a host list, and with ``flags`` the same as device int32 flags (``fresh``) for the kernels that
+      read them; the subclass clears those inside the captured push;
+    * one cached entry per chunk length (at most ``MAX_CHUNK_LENGTHS``), and one CUDA graph per chunk length captured
+      after an eager warm-up whose state changes are undone; the result is cloned once, in ``_run``.
+
+    A subclass provides ``_state()`` (the tensors a push advances, including ``cin_hist``), ``_new_entry(n, xin)`` and
+    ``_step(*inputs)``, which writes into the entry's buffers."""
 
     MAX_CHUNK_LENGTHS = 8
 
-    def _setup(self, model, batch, use_graphs):
+    def _setup(self, model, batch, use_graphs, in_channels, history, pad, flags=False):
         self._check_eval(model)
         self.model = model
         self.dev = next(model.parameters()).device
@@ -54,6 +71,16 @@ class _ChunkStream:
             raise PwgbError(f"{type(self).__name__}: batch must be >= 1")
         self.use_graphs = bool(use_graphs)
         self._entries = {}  # chunk frames -> per-length data and "graph"; a graph lives and dies with its entry
+        self.in_channels, self.pad = in_channels, pad
+        self.cin_hist = self._zeros(self.B, in_channels, history)
+        self._fresh = [True] * self.B
+        self.fresh = torch.ones(self.B, device=self.dev, dtype=torch.int32) if flags else None
+
+    def _zeros(self, *shape):
+        return torch.zeros(shape, device=self.dev, dtype=torch.float32)
+
+    def _empty(self, *shape):
+        return torch.empty(shape, device=self.dev, dtype=torch.float32)
 
     def _check_eval(self, model):
         if model.training:
@@ -67,27 +94,74 @@ class _ChunkStream:
                 raise PwgbError(f"{type(self).__name__}.reset: slot {b} out of range [0, {self.B})")
         return items
 
+    def state_bytes(self):
+        """bytes of carried state per slot"""
+        return sum(t.numel() * t.element_size() for t in self._state()) // self.B
+
+    def reset(self, items=None):
+        """Restart slots ``items`` (an index or an iterable of indices; None: every slot) as fresh signals.  The other
+        slots continue unaffected."""
+        for b in self._slots(items):
+            for h in self._state():
+                h[b].zero_()
+            self._fresh[b] = True
+            if self.fresh is not None:
+                self.fresh[b] = 1
+
+    def _frames(self, c, normalize_before):
+        """c: (B, n, C) mel frames ((n, C) when batch == 1) -> (B, C, n) contiguous on the device"""
+        m = self.model
+        self._check_eval(m)
+        c = torch.as_tensor(c, dtype=torch.float32, device=self.dev)
+        if c.dim() == 2 and self.B == 1:
+            c = c.unsqueeze(0)
+        if c.dim() != 3 or c.shape[0] != self.B or c.shape[2] != self.in_channels or c.shape[1] < 1:
+            raise PwgbError(f"{type(self).__name__}.push: c must be ({self.B}, n >= 1, {self.in_channels}), got {tuple(c.shape)}")
+        if normalize_before:
+            c = (c - m.mean) / m.scale
+        return c.transpose(1, 2).contiguous()
+
+    def _start(self, c):
+        """Fill the input-conv history of the fresh slots from their first chunk c (B, C, n) as the pad would: frames
+        P .. 1 (reflect), frame 0 repeated (replicate) or the reset's zeros."""
+        P = self.cin_hist.shape[-1]
+        for b in range(self.B):
+            if self._fresh[b] and P and self.pad != "zero":
+                self.cin_hist[b].copy_(c[b, :, 1:P + 1].flip(-1) if self.pad == "reflect" else c[b, :, :1].expand(-1, P))
+        self._fresh = [False] * self.B
+
+    def _input(self, ent, c):
+        """[history | chunk] in the entry's xin buffer, the input of the input conv"""
+        P = self.cin_hist.shape[-1]
+        xin = ent["xin"]
+        xin[:, :, :P].copy_(self.cin_hist)
+        xin[:, :, P:].copy_(c)
+        return xin
+
     def _entry(self, n):
         ent = self._entries.get(n)
         if ent is None:
             if len(self._entries) >= self.MAX_CHUNK_LENGTHS:
                 self._entries.clear()
-            ent = self._entries[n] = self._new_entry(n)
+            xin = self._empty(self.B, self.in_channels, self.cin_hist.shape[-1] + n)
+            ent = self._entries[n] = self._new_entry(n, xin)
+            ent["xin"] = xin
         return ent
 
     def _replay(self, n, inputs):
         ent = self._entry(n)
         if "graph" not in ent:
             static = [t.clone() for t in inputs]
-            # one eager warm-up (packs weights, sets kernel attributes, fills the per-shape caches) advances the state:
-            # it is restored before the capture, which itself runs nothing
-            snap = [t.clone() for t in self._state()]
+            # one eager warm-up (packs weights, sets kernel attributes, fills the per-shape caches) advances the state
+            # and clears the flags: both are restored before the capture, which itself runs nothing
+            carried = self._state() + ([self.fresh] if self.fresh is not None else [])
+            snap = [t.clone() for t in carried]
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
                 self._step(*static)
             torch.cuda.current_stream().wait_stream(side)
-            for t, s in zip(self._state(), snap):
+            for t, s in zip(carried, snap):
                 t.copy_(s)
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
@@ -96,10 +170,12 @@ class _ChunkStream:
         for s, t in zip(ent["inputs"], inputs):
             s.copy_(t)
         ent["graph"].replay()
-        return ent["out"].clone()
+        return ent["out"]
 
     def _run(self, n, *inputs):
-        return self._replay(n, inputs) if self.use_graphs else self._step(*inputs)
+        """One push; the result is the caller's own tensor (the graph's output and the entry's buffers are reused)"""
+        y = self._replay(n, inputs) if self.use_graphs else self._step(*inputs)
+        return y.clone()
 
 
 class CausalPWGStream(_ChunkStream):
@@ -108,7 +184,7 @@ class CausalPWGStream(_ChunkStream):
     ``push(c, z)`` takes the next n >= 1 frames of every slot and returns their n * hop samples; n may change from
     push to push.  For every slot, the concatenated outputs equal ``model.inference(c=all_frames, x=all_noise)``.
     There is no lookahead and no flush.  With ``use_graphs`` each chunk length is captured once into a CUDA graph and
-    replayed.  The model's weights must not change while a stream uses them (the graphs hold the packed images)."""
+    replayed.  The weights are read when the stream is built and must not change while it is used."""
 
     def __init__(self, model, batch=1, seed=None, use_graphs=True):
         from .models import MelGANGenerator, ParallelWaveGANGenerator
@@ -124,14 +200,15 @@ class CausalPWGStream(_ChunkStream):
             raise PwgbError("CausalPWGStream: upsample_net='MelGANGenerator' is not supported")
         if isinstance(up, UpsampleNetwork) and model.aux_context_window:
             raise PwgbError("CausalPWGStream: UpsampleNetwork with aux_context_window > 0 has no whole-utterance inference to match")
-        self._setup(model, batch, use_graphs)
-        self.conv_in = up.conv_in if isinstance(up, ConvInUpsampleNetwork) else None
-        fir_net = up.upsample if isinstance(up, ConvInUpsampleNetwork) else up
-        self.scales = list(fir_net.upsample_scales)
-        self.firs = [fir_net.up_layers[2 * i + 1] for i in range(len(self.scales))]
-        self.hop = model.upsample_factor
-        self.acw = model.aux_context_window if self.conv_in is not None else 0
+        conv_in = up.conv_in if isinstance(up, ConvInUpsampleNetwork) else None
         self.A = model.aux_channels
+        # ReplicationPad1d of inference: a fresh slot's conv_in history is its first frame
+        self._setup(model, batch, use_graphs, self.A, model.aux_context_window if conv_in is not None else 0, "replicate")
+        fir_net = up.upsample if conv_in is not None else up
+        self.scales = list(fir_net.upsample_scales)
+        self.w_in = wb(conv_in)[0] if conv_in is not None else None
+        self.firs = [wb(fir_net.up_layers[2 * i + 1])[0] for i in range(len(self.scales))]
+        self.hop = model.upsample_factor
         l0 = model.conv_layers[0]
         self.R, self.G, self.K = l0.conv.in_channels, l0.conv.out_channels, l0.conv.kernel_size[0]
         self.S = l0.conv1x1_skip.out_channels
@@ -140,60 +217,57 @@ class CausalPWGStream(_ChunkStream):
         if not ops.WnStack.supported(self.B, self.hop, self.R, self.G, self.S, self.A, self.K, self.dmax, True):
             raise PwgbError("CausalPWGStream: the fused packed WaveNet stack does not support this configuration "
                             f"(residual {self.R}, gate {self.G}, skip {self.S}, aux {self.A} channels, kernel {self.K})")
+        self.w_first = wb(model.first_conv)
+        # the output head as in ParallelWaveGANGenerator.forward: sqrt(1/layers) folded into the first 1x1 conv
+        w1, b1 = wb(model.last_conv_layers[1])
+        self.w_l1, self.w_l3 = (w1 * model._skip_scale, b1), wb(model.last_conv_layers[3])
         dev, B, A = self.dev, self.B, self.A
-        self.cin_hist = torch.zeros((B, A, self.acw), device=dev, dtype=torch.float32) if self.acw else None
-        self.fir_hist = [torch.zeros((B * A, 2), device=dev, dtype=torch.float32) for _ in self.scales]
-        self.fir_next = [torch.zeros((B * A, 2), device=dev, dtype=torch.float32) for _ in self.scales]
-        self.wn_hist = [torch.zeros(B * self.R * h, device=dev, dtype=torch.int32) for h in self.H]
-        self._fresh = [True] * B
+        self.fir_hist = [self._zeros(B, A, 2) for _ in self.scales]
+        self.wn_hist = [torch.zeros((B, self.R * h), device=dev, dtype=torch.int32) for h in self.H]
         self.gen = torch.Generator(device=dev)
         if seed is not None:
             self.gen.manual_seed(int(seed))
 
-    # ---------------------------------------------------------------------------------------------------- state
     def _state(self):
-        return ([self.cin_hist] if self.cin_hist is not None else []) + self.fir_hist + self.wn_hist
+        return [self.cin_hist] + self.fir_hist + self.wn_hist
 
-    def reset(self, items=None):
-        """Restart slots ``items`` (an index or an iterable of indices; None: every slot) as fresh signals.  The other
-        slots continue unaffected."""
-        A = self.A
-        for b in self._slots(items):
-            if self.cin_hist is not None:
-                self.cin_hist[b].zero_()
-            for h in self.fir_hist:
-                h[b * A:(b + 1) * A].zero_()
-            for h in self.wn_hist:
-                h.view(self.B, -1)[b].zero_()
-            self._fresh[b] = True
-
-    # ---------------------------------------------------------------------------------------------------- compute
-    def _new_entry(self, n):
-        return {"stack": ops.WnStack(self.B, n * self.hop, self.R, self.G, self.S, self.A, self.K, self.dmax, self.dev, True)}
+    def _new_entry(self, n, xin):
+        """The conditioning's buffers for an n-frame chunk, the carry table of the conv_in and FIR histories over them,
+        and the packed WaveNet stack."""
+        dev, B, A = self.dev, self.B, self.A
+        ent = dict(stack=ops.WnStack(B, n * self.hop, self.R, self.G, self.S, A, self.K, self.dmax, dev, True),
+                   skips=self._empty(B, self.S, n * self.hop))
+        ent["cin"] = self._empty(B, A, n) if self.w_in is not None else xin
+        entries, x, t = [(xin, self.cin_hist)], ent["cin"], n
+        ent["fir"] = []
+        for i, s in enumerate(self.scales):
+            entries.append((x, self.fir_hist[i]))
+            t *= s
+            # the last stage writes the first A of the stack's aux_pad channels; the others stay zero
+            x = self._zeros(B, self.model._aux_pad, t) if i == len(self.scales) - 1 else self._empty(B, A, t)
+            ent["fir"].append(x)
+        ent["table"] = ops.stream_carry_table(entries, dev)
+        return ent
 
     def _step(self, z, c):
         """One chunk: z (B, in_channels, n * hop), c (B, aux, n) -> (B, out_channels, n * hop).  Advances the state."""
         m = self.model
-        n = c.shape[-1]
-        # conditioning: conv_in on [history | chunk], then the causal FIR stages with their carried frames
-        if self.conv_in is not None:
-            x = c
-            if self.acw:
-                x = torch.cat([self.cin_hist, c], -1)
-                self.cin_hist.copy_(x[:, :, n:])
-            c = ops.conv1d(x, effective_weight(self.conv_in), None)
-        last = len(self.scales) - 1
+        ent = self._entry(c.shape[-1])
+        # conditioning: conv_in on [history | chunk], then the causal FIR stages reading their histories; one carry after
+        # the last of them updates every history they read
+        x = self._input(ent, c)
+        if self.w_in is not None:
+            x = ops.conv1d(x, self.w_in, None, out=ent["cin"])
         for i, s in enumerate(self.scales):
-            c = ops.upsample_fir_causal_stream(c, effective_weight(self.firs[i]), s, self.fir_hist[i], self.fir_next[i],
-                                               out_channels=m._aux_pad if i == last else None)
-            self.fir_hist[i].copy_(self.fir_next[i])
+            x = ops.upsample_fir_causal_stream(x, self.firs[i], s, self.fir_hist[i], out=ent["fir"][i],
+                                               out_channels=ent["fir"][i].shape[1])
+        ops.stream_carry(ent["table"])
         # the residual stack on the packed stream; each layer's history is carried between the layer launches
-        st = self._entry(n)["stack"]
+        st = ent["stack"]
         st.cur, st.prev = 0, None
-        st.pack_c(c)
-        fc = m.first_conv
-        st.first_conv(z, effective_weight(fc), fc.bias)
-        skips = torch.empty((self.B, self.S, z.shape[-1]), device=z.device, dtype=torch.float32)
+        st.pack_c(x)
+        st.first_conv(z, *self.w_first)
+        skips = ent["skips"]
         layers = m.conv_layers
         L = len(layers)
         st.carry(load=(self.wn_hist[0], self.H[0]))
@@ -201,27 +275,17 @@ class CausalPWGStream(_ChunkStream):
             packed, bso = _layer_weights(f, self.A)
             st.layer(packed, f.conv.bias, bso, f.dilation, skips, skips_init=(i == 0), write_x=(i < L - 1))
             st.carry(save=(self.wn_hist[i], self.H[i]), load=(self.wn_hist[i + 1], self.H[i + 1]) if i + 1 < L else None)
-        # the output head as in ParallelWaveGANGenerator.forward: sqrt(1/layers) folded into the first 1x1 conv
-        l1, l3 = m.last_conv_layers[1], m.last_conv_layers[3]
-        h = ops.conv1d(skips, effective_weight(l1) * m._skip_scale, l1.bias, pre_slope=0.0)
-        return ops.conv1d(h, effective_weight(l3), l3.bias, pre_slope=0.0)
+        h = ops.conv1d(skips, *self.w_l1, pre_slope=0.0)
+        # into a fresh tensor, as in inference: given out=, a wide few-channel output conv would not take _conv1d_fewcout
+        return ops.conv1d(h, *self.w_l3, pre_slope=0.0)
 
     @torch.no_grad()
     def push(self, c, z=None, normalize_before=False):
         """c: (B, n, aux) mel frames ((n, aux) when batch == 1); z: optional (B, in_channels, n * hop) noise, drawn from
         the stream's generator when omitted.  Returns (B, out_channels, n * hop) on the device."""
         m = self.model
-        self._check_eval(m)
-        c = torch.as_tensor(c, dtype=torch.float32, device=self.dev)
-        if c.dim() == 2 and self.B == 1:
-            c = c.unsqueeze(0)
-        if c.dim() != 3 or c.shape[0] != self.B or c.shape[2] != self.A or c.shape[1] < 1:
-            raise PwgbError(f"CausalPWGStream.push: c must be ({self.B}, n >= 1, {self.A}), got {tuple(c.shape)}")
-        if normalize_before:
-            c = (c - m.mean) / m.scale
-        c = c.transpose(1, 2).contiguous()
-        n = c.shape[-1]
-        T = n * self.hop
+        c = self._frames(c, normalize_before)
+        T = c.shape[-1] * self.hop
         if z is None:
             z = torch.randn((self.B, m.in_channels, T), device=self.dev, generator=self.gen)
         else:
@@ -229,12 +293,8 @@ class CausalPWGStream(_ChunkStream):
             if tuple(z.shape) != (self.B, m.in_channels, T):
                 raise PwgbError(f"CausalPWGStream.push: z must be ({self.B}, {m.in_channels}, {T}), got {tuple(z.shape)}")
             z = z.contiguous()
-        if self.acw and any(self._fresh):  # ReplicationPad1d: a fresh slot's history is its first frame
-            for b in range(self.B):
-                if self._fresh[b]:
-                    self.cin_hist[b].copy_(c[b, :, :1].expand(-1, self.acw))
-        self._fresh = [False] * self.B
-        return self._run(n, z, c)
+        self._start(c)
+        return self._run(c.shape[-1], z, c)
 
 
 class CausalHiFiGANStream(_ChunkStream):
@@ -266,21 +326,13 @@ class CausalHiFiGANStream(_ChunkStream):
             raise PwgbError("CausalHiFiGANStream: expected a HiFiGANGenerator")
         if not model.use_causal_conv:
             raise PwgbError("CausalHiFiGANStream: the model is not causal (use_causal_conv=False); a centred model needs lookahead")
-        self._setup(model, batch, use_graphs)
-        dev, B = self.dev, self.B
-
-        def wb(conv):
-            return effective_weight(conv).detach().contiguous(), (conv.bias.detach() if conv.bias is not None else None)
-
-        def zeros(*shape):
-            return torch.zeros(shape, device=dev, dtype=torch.float32)
-
+        ic = model.input_conv
+        # the fresh slots' flags are the conv-transposes' replicate flags
+        self._setup(model, batch, use_graphs, ic.conv.in_channels, ic.left, "zero", flags=True)
+        B, zeros = self.B, self._zeros
         m = model
         self.slope, self.nb = m.slope, m.num_blocks
-        ic = m.input_conv
         self.w_in = wb(ic.conv)
-        self.in_channels = ic.conv.in_channels
-        self.cin_hist = zeros(B, self.in_channels, ic.left)
         self.hop = 1
         self.levels = []
         for i in range(m.num_upsamples):
@@ -307,40 +359,21 @@ class CausalHiFiGANStream(_ChunkStream):
         self.w_out = wb(oc.conv)
         self.out_hist = zeros(B, oc.conv.in_channels, oc.left)
         self.out_channels = oc.conv.out_channels
-        self.rep = torch.ones(B, device=dev, dtype=torch.int32)  # replicate flags of the conv-transposes: fresh slots
 
     # ---------------------------------------------------------------------------------------------------- state
     def _state(self):
-        hs = [self.cin_hist, self.out_hist, self.rep]
+        hs = [self.cin_hist, self.out_hist]
         for lv in self.levels:
             hs += [lv["up_hist"], lv["lvl_hist"]]
             for blk in lv["blocks"]:
                 hs += [h for cv in blk["convs"] for h in (cv["x_hist"], cv["xt_hist"]) if h is not None]
         return hs
 
-    def state_bytes(self):
-        """bytes of carried state per slot"""
-        return sum(t.numel() * t.element_size() for t in self._state() if t is not self.rep) // self.B
-
-    def reset(self, items=None):
-        """Restart slots ``items`` (an index or an iterable of indices; None: every slot) as fresh signals.  The other
-        slots continue unaffected."""
-        for b in self._slots(items):
-            for h in self._state():
-                if h is not self.rep:
-                    h[b].zero_()
-            self.rep[b] = 1
-
     # ---------------------------------------------------------------------------------------------------- compute
-    def _new_entry(self, n):
+    def _new_entry(self, n, xin):
         """The buffers of every intermediate signal of an n-frame chunk, and the carry tables over them."""
-        dev, B = self.dev, self.B
-
-        def empty(*shape):
-            return torch.empty(shape, device=dev, dtype=torch.float32)
-
-        K_in = self.cin_hist.shape[-1]
-        ent = dict(xin=empty(B, self.in_channels, K_in + n), h0=empty(B, self.levels[0]["w"][0].shape[0], n), levels=[])
+        dev, B, empty = self.dev, self.B, self._empty
+        ent = dict(h0=empty(B, self.levels[0]["w"][0].shape[0], n), levels=[])
         t, prev = n, ent["h0"]
         for i, lv in enumerate(self.levels):
             t *= lv["stride"]
@@ -358,7 +391,7 @@ class CausalHiFiGANStream(_ChunkStream):
                 if j == len(lv["blocks"]) - 1:  # the level's shared signals, after their last reader
                     entries += [(prev, lv["up_hist"]), (buf["u"], lv["lvl_hist"])]
                     if i == 0:
-                        entries.append((ent["xin"], self.cin_hist))  # the last frames of [history | chunk] are the chunk's
+                        entries.append((xin, self.cin_hist))  # the last frames of [history | chunk] are the chunk's
                 tables.append(ops.stream_carry_table(entries, dev))
             buf["tables"] = tables
             ent["levels"].append(buf)
@@ -370,14 +403,10 @@ class CausalHiFiGANStream(_ChunkStream):
     def _step(self, c):
         """One chunk: c (B, in_channels, n) -> (B, out_channels, n * hop).  Advances the state."""
         ent = self._entry(c.shape[-1])
-        K_in = self.cin_hist.shape[-1]
-        xin = ent["xin"]
-        xin[:, :, :K_in].copy_(self.cin_hist)
-        xin[:, :, K_in:].copy_(c)
-        h = ops.conv1d(xin, self.w_in[0], self.w_in[1], out=ent["h0"])
+        h = ops.conv1d(self._input(ent, c), *self.w_in, out=ent["h0"])
         slope = self.slope
         for lv, buf in zip(self.levels, ent["levels"]):
-            u = ops.conv_transpose1d_stream(h, lv["up_hist"], lv["w"][0], lv["w"][1], stride=lv["stride"], replicate=self.rep,
+            u = ops.conv_transpose1d_stream(h, lv["up_hist"], lv["w"][0], lv["w"][1], stride=lv["stride"], replicate=self.fresh,
                                             pre_slope=slope, out=buf["u"])
             cs = buf["cs"]
             for j, blk in enumerate(lv["blocks"]):
@@ -398,25 +427,16 @@ class CausalHiFiGANStream(_ChunkStream):
         y = ops.conv1d_stream(h, self.out_hist, *self.w_out, pad_left=self.out_hist.shape[-1], pre_slope=0.01, post_act="tanh",
                               out=ent["y"])
         ops.stream_carry(ent["out_table"])
-        self.rep.zero_()
+        self.fresh.zero_()
         return y
 
     @torch.no_grad()
     def push(self, c, normalize_before=False):
         """c: (B, n, in_channels) mel frames ((n, in_channels) when batch == 1).  Returns (B, out_channels, n * hop) on the
         device."""
-        m = self.model
-        self._check_eval(m)
-        c = torch.as_tensor(c, dtype=torch.float32, device=self.dev)
-        if c.dim() == 2 and self.B == 1:
-            c = c.unsqueeze(0)
-        if c.dim() != 3 or c.shape[0] != self.B or c.shape[2] != self.in_channels or c.shape[1] < 1:
-            raise PwgbError(f"CausalHiFiGANStream.push: c must be ({self.B}, n >= 1, {self.in_channels}), got {tuple(c.shape)}")
-        if normalize_before:
-            c = (c - m.mean) / m.scale
-        c = c.transpose(1, 2).contiguous()
-        y = self._run(c.shape[-1], c)
-        return y if self.use_graphs else y.clone()
+        c = self._frames(c, normalize_before)
+        self._start(c)
+        return self._run(c.shape[-1], c)
 
 
 class CausalMelGANStream(_ChunkStream):
@@ -458,20 +478,11 @@ class CausalMelGANStream(_ChunkStream):
         mods = list(model.melgan)
         if not isinstance(mods[0], CausalConv1d):
             raise PwgbError("CausalMelGANStream: the model is not causal (use_causal_conv=False); a centred model needs lookahead")
-        self._setup(model, batch, use_graphs)
-        dev, B = self.dev, self.B
-
-        def wb(conv):
-            return effective_weight(conv).detach().contiguous(), (conv.bias.detach() if conv.bias is not None else None)
-
-        def zeros(*shape):
-            return torch.zeros(shape, device=dev, dtype=torch.float32)
-
-        self.slope, self.pad = model.slope, model.pad_mode
         ic = mods[0]
+        self._setup(model, batch, use_graphs, ic.conv.in_channels, ic.left, model.pad_mode, flags=True)
+        B, zeros = self.B, self._zeros
+        self.slope = model.slope
         self.w_in = wb(ic.conv)
-        self.in_channels = ic.conv.in_channels
-        self.cin_hist = zeros(B, self.in_channels, ic.left)
         reflect_need = [(ic.left, 1)]  # (left padding, input samples per frame) of every conv the pad applies to
         self.hop, self.levels, oc = 1, [], None
         for m in mods[1:]:
@@ -509,29 +520,13 @@ class CausalMelGANStream(_ChunkStream):
             self.min_first_frames = max(self.min_first_frames, -(-self.delay // (self.hop * N)))
         else:
             self.subbands, self.delay, self.pq_hist = 1, 0, None
-        self.fresh = torch.ones(B, device=dev, dtype=torch.int32)  # per-slot flags: the slot's signal starts in this push
-        self._fresh = [True] * B  # the same, on the host (the input conv's history is filled in push)
 
     # ---------------------------------------------------------------------------------------------------- state
     def _state(self):
-        hs = [self.cin_hist, self.out_hist, self.fresh]
+        hs = [self.cin_hist, self.out_hist]
         for lv in self.levels:
             hs += [lv["up_hist"]] + [st["hist"] for st in lv["stacks"]]
         return hs + ([self.pq_hist] if self.pq_hist is not None else [])
-
-    def state_bytes(self):
-        """bytes of carried state per slot"""
-        return sum(t.numel() * t.element_size() for t in self._state() if t is not self.fresh) // self.B
-
-    def reset(self, items=None):
-        """Restart slots ``items`` (an index or an iterable of indices; None: every slot) as fresh signals.  The other
-        slots continue unaffected."""
-        for b in self._slots(items):
-            for h in self._state():
-                if h is not self.fresh:
-                    h[b].zero_()
-            self.fresh[b] = 1
-            self._fresh[b] = True
 
     # ---------------------------------------------------------------------------------------------------- compute
     def _pad_kw(self, P, rate, n):
@@ -543,16 +538,11 @@ class CausalMelGANStream(_ChunkStream):
             return dict(replicate=self.fresh, reflect=True)
         return {}
 
-    def _new_entry(self, n):
+    def _new_entry(self, n, xin):
         """The buffers of every intermediate signal of an n-frame chunk, and the carry table over them."""
-        dev, B = self.dev, self.B
-
-        def empty(*shape):
-            return torch.empty(shape, device=dev, dtype=torch.float32)
-
-        K_in = self.cin_hist.shape[-1]
-        ent = dict(xin=empty(B, self.in_channels, K_in + n), h0=empty(B, self.levels[0]["w"][0].shape[0], n), levels=[])
-        entries = [(ent["xin"], self.cin_hist)]
+        dev, B, empty = self.dev, self.B, self._empty
+        ent = dict(h0=empty(B, self.levels[0]["w"][0].shape[0], n), levels=[])
+        entries = [(xin, self.cin_hist)]
         t, prev = n, ent["h0"]
         for lv in self.levels:
             t *= lv["stride"]
@@ -578,11 +568,7 @@ class CausalMelGANStream(_ChunkStream):
         """One chunk: c (B, in_channels, n) -> (B, 1, n * hop * subbands).  Advances the state."""
         n = c.shape[-1]
         ent = self._entry(n)
-        K_in = self.cin_hist.shape[-1]
-        xin = ent["xin"]
-        xin[:, :, :K_in].copy_(self.cin_hist)
-        xin[:, :, K_in:].copy_(c)
-        h = ops.conv1d(xin, self.w_in[0], self.w_in[1], out=ent["h0"])
+        h = ops.conv1d(self._input(ent, c), *self.w_in, out=ent["h0"])
         slope = self.slope
         for lv, buf in zip(self.levels, ent["levels"]):
             x = ops.conv_transpose1d_stream(h, lv["up_hist"], lv["w"][0], lv["w"][1], stride=lv["stride"], replicate=self.fresh,
@@ -611,30 +597,14 @@ class CausalMelGANStream(_ChunkStream):
     def push(self, c, normalize_before=False):
         """c: (B, n, in_channels) mel frames ((n, in_channels) when batch == 1); n >= ``min_first_frames`` for a slot's
         first push after a reset.  Returns (B, 1, n * hop * subbands) on the device."""
-        m = self.model
-        self._check_eval(m)
-        c = torch.as_tensor(c, dtype=torch.float32, device=self.dev)
-        if c.dim() == 2 and self.B == 1:
-            c = c.unsqueeze(0)
-        if c.dim() != 3 or c.shape[0] != self.B or c.shape[2] != self.in_channels or c.shape[1] < 1:
-            raise PwgbError(f"CausalMelGANStream.push: c must be ({self.B}, n >= 1, {self.in_channels}), got {tuple(c.shape)}")
-        n = c.shape[1]
+        c = self._frames(c, normalize_before)
+        n = c.shape[-1]
         fresh = [b for b in range(self.B) if self._fresh[b]]
         if fresh and n < self.min_first_frames:
             raise PwgbError(f"CausalMelGANStream.push: the first push after a reset needs at least {self.min_first_frames} frames "
                             f"(the reflect padding reads that far into the signal), got {n} for slots {fresh}")
-        if normalize_before:
-            c = (c - m.mean) / m.scale
-        c = c.transpose(1, 2).contiguous()
-        P = self.cin_hist.shape[-1]
-        for b in fresh:  # the input conv's pad for a fresh slot (zero: the reset's zeros)
-            if self.pad == "reflect":
-                self.cin_hist[b].copy_(c[b, :, 1:P + 1].flip(-1))
-            elif self.pad == "replicate":
-                self.cin_hist[b].copy_(c[b, :, :1].expand(-1, P))
-        self._fresh = [False] * self.B
-        y = self._run(n, c)
-        return y if self.use_graphs else y.clone()
+        self._start(c)
+        return self._run(n, c)
 
     @torch.no_grad()
     def flush(self, items=None):

@@ -143,33 +143,33 @@ def test_carry_kernel_bit_for_bit(dev, t, h_save, h_load):
 
 
 @pytest.mark.parametrize("n,scale,oc", [(1, 4, None), (2, 4, None), (37, 4, 96), (300, 8, None), (5, 3, None)])
-def test_stream_fir_bit_for_bit(dev, n, scale, oc):
+def test_stream_fir_and_carry_bit_for_bit(dev, n, scale, oc):
     """pwgb_upsample_fir_causal_stream_forward against the whole-signal causal stage on [history | x] with its first
-    two frames' outputs dropped, and the history it hands on against the last two frames"""
+    two frames' outputs dropped, and the history the stream's carry hands on against the last two frames"""
     from parallelwavegan_b200 import ops
 
     B, Cc = 2, 80
     g = torch.Generator(device=dev).manual_seed(n * 10 + scale)
     x = torch.randn((B, Cc, n), device=dev, generator=g)
-    hist = torch.randn((B * Cc, 2), device=dev, generator=g)
+    hist = torch.randn((B, Cc, 2), device=dev, generator=g)
     fir = torch.randn(2 * scale + 1, device=dev, generator=g)
-    nxt = torch.full((B * Cc, 2), float("nan"), device=dev)
-    y = ops.upsample_fir_causal_stream(x, fir, scale, hist, nxt, out_channels=oc)
-    xc = torch.cat([hist.view(B, Cc, 2), x], -1)
+    y = ops.upsample_fir_causal_stream(x, fir, scale, hist, out_channels=oc)
+    xc = torch.cat([hist, x], -1)
     ref = ops.upsample_fir(xc, fir, scale, causal=True)[:, :, 2 * scale:]
     assert torch.equal(y[:, :Cc], ref)
     if oc:
         assert not y[:, Cc:].any()
-    assert torch.equal(nxt, xc[:, :, -2:].reshape(B * Cc, 2))
+    ops.stream_carry(ops.stream_carry_table([(x, hist)], dev))
+    assert torch.equal(hist, xc[:, :, -2:])
 
 
-def test_stream_fir_zero_history_is_the_causal_stage(dev):
+def test_stream_fir_zero_history_equals_the_causal_stage(dev):
     from parallelwavegan_b200 import ops
 
     g = torch.Generator(device=dev).manual_seed(5)
     x = torch.randn((3, 80, 50), device=dev, generator=g)
     fir = torch.randn(9, device=dev, generator=g)
-    y = ops.upsample_fir_causal_stream(x, fir, 4, torch.zeros((240, 2), device=dev), torch.empty((240, 2), device=dev))
+    y = ops.upsample_fir_causal_stream(x, fir, 4, torch.zeros((240, 2), device=dev))
     assert torch.equal(y, ops.upsample_fir(x, fir, 4, causal=True))
 
 
@@ -184,6 +184,10 @@ def test_batch_slots_are_independent(dev):
     y = _stream(st, c.to(dev), z.to(dev), SCHEDULES["mixed"], m.upsample_factor)
     for b in range(4):
         assert torch.equal(y[b], ref[b]), b
+    # fp32 conv_in and FIR histories, and (K-1)*d packed hi/lo bf16 rows of R channels per WaveNet layer
+    A, R = m.aux_channels, m.conv_layers[0].conv.in_channels
+    wn = sum(R * (f.conv.kernel_size[0] - 1) * f.dilation for f in m.conv_layers)
+    assert st.state_bytes() == 4 * (A * m.aux_context_window + 2 * A * len(m.upsample_net.upsample.upsample_scales) + wn)
 
 
 def test_reset_one_slot_mid_stream(dev):

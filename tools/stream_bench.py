@@ -1,0 +1,208 @@
+"""Per-push latency of the causal streams (parallelwavegan_b200.streaming) with synthetic weights, weight norm removed,
+for batch sizes B, chunks of 1, 4, 16 and 64 frames, CUDA graphs off and on.  MODEL is
+
+* pwg: the causal PWG v1 generator (CausalPWGStream), hop 256;
+* hifigan: the causal HiFi-GAN v1 generator (CausalHiFiGANStream), hop 256;
+* melgan_v1: the causal MelGAN v1 (512 channels, scales [8, 8, 2, 2], 3 stacks; CausalMelGANStream);
+* mb_melgan_v2: the causal multi-band MelGAN v2 (384 channels, scales [8, 4, 2], 4 stacks, 4-band PQMF), 256 output
+  samples per frame like the others.
+
+PWG and HiFi-GAN stream a 256-frame utterance (65536 samples per item); the MelGANs stream a 263-frame one, a 7-frame
+opening push (their min_first_frames) then 256 frames, and flush.  Each configuration streams its utterance PASSES
+times.  A push is timed with CUDA events recorded around it and a synchronise after it, so a latency includes the
+host's launch work whenever the GPU waits for it.  Reported: median / min / max latency of the chunk pushes, the
+streamed real-time factor (GPU time of all pushes, and the flush, over the audio's duration at 22050 Hz: below 1 is
+faster than real time), the libpwgb kernel launches of one steady-state eager push (the few torch copies are not
+counted), and the whole-utterance forward of the same audio (one call on the B utterances; for MB-MelGAN with the PQMF
+synthesis) for comparison.
+
+Every timed stream is checked against ``model.inference`` of each item in the same run:
+
+* pwg: bit for bit while a push has at most 65536 samples in all (B x chunk x 256), so that its 64 -> 1 output conv
+  takes conv1d_small_cout_kernel as the per-item inference does; above that the push's output conv takes
+  conv1d_fewcout_long_kernel, which sums in another order, and the check is rel-L2 <= 1e-6;
+* hifigan: the per-item inference's 32 -> 1 output conv has 65536 output samples and takes conv1d_fewcout_long_kernel,
+  which sums in another order than the generic kernel every stream conv takes, so the check is rel-L2 <= 1e-6 (bit
+  identity holds up to 15 frames, tests/test_gpu_hifigan_stream.py);
+* melgan_v1, mb_melgan_v2: after the PQMF delay, the per-item inference's output conv has 67328 output samples and
+  takes conv1d_fewcout_long_kernel too, so the check is rel-L2 <= 1e-6 (bit identity holds below 4096 output-conv
+  samples, tests/test_gpu_melgan_stream.py).
+
+Prints the card name and power limit of the same run, as one JSON document.
+
+    python tools/stream_bench.py [MODEL] [B ...]        # default: every model at B = 1 16"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import torch  # noqa: E402
+import torch.nn.functional as F  # noqa: E402
+
+from parallelwavegan_b200 import capi, models  # noqa: E402
+from parallelwavegan_b200 import synth_weights as synth  # noqa: E402
+from parallelwavegan_b200.layers import PQMF  # noqa: E402
+from parallelwavegan_b200.streaming import CausalHiFiGANStream, CausalMelGANStream, CausalPWGStream  # noqa: E402
+
+MELGAN = {
+    "melgan_v1": dict(in_channels=80, out_channels=1, kernel_size=7, channels=512, upsample_scales=[8, 8, 2, 2], stacks=3,
+                      use_causal_conv=True),
+    "mb_melgan_v2": dict(in_channels=80, out_channels=4, kernel_size=7, channels=384, upsample_scales=[8, 4, 2], stacks=4,
+                         use_causal_conv=True),
+}
+MODELS = ("pwg", "hifigan", *MELGAN)
+FRAMES = 256
+CHUNKS = (1, 4, 16, 64)
+PASSES = 2
+SR = 22050
+
+
+def card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
+    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name(0)
+
+
+def stats(v):
+    v = sorted(v)
+    return {"ms_median": v[len(v) // 2], "ms_min": v[0], "ms_max": v[-1], "pushes": len(v)}
+
+
+def timed(fn):
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    y = fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return y, e0.elapsed_time(e1)
+
+
+def build(name, dev):
+    if name == "pwg":
+        m, scale = models.ParallelWaveGANGenerator(use_causal_conv=True), 1.0
+    elif name == "hifigan":
+        m, scale = models.HiFiGANGenerator(use_causal_conv=True), 1.15
+    else:
+        m, scale = models.MelGANGenerator(**MELGAN[name]), 1.0
+    m.load_state_dict(synth.synth_state_dict([(k, tuple(v.shape)) for k, v in m.state_dict().items()], 31, scale))
+    m.remove_weight_norm()
+    m = m.eval().to(dev)
+    if name in MELGAN and MELGAN[name]["out_channels"] > 1:
+        m.pqmf = PQMF(MELGAN[name]["out_channels"]).to(dev)
+    return m
+
+
+class Workload:
+    """One model's utterance: its inputs, reference, whole-utterance forward, streams and pushes"""
+
+    def __init__(self, name, m, B, dev):
+        self.name, self.m = name, m
+        self.melgan = name in MELGAN
+        self.open = 7 if self.melgan else 0
+        self.frames = self.open + FRAMES
+        g = torch.Generator().manual_seed(B)
+        c = self.c = torch.randn(B, self.frames, 80, generator=g).to(dev)
+        cw = c.transpose(1, 2).contiguous()
+        self.delay = 0
+        if name == "pwg":
+            hop = self.hop = m.upsample_factor
+            z = self.z = torch.randn(B, 1, FRAMES * hop, generator=g).to(dev)
+            self.ref = torch.stack([m.inference(c=c[b], x=z[b].t()).t() for b in range(B)])
+            # the inference input: edge-padded by aux_context_window
+            acw = m.aux_context_window
+            cw = cw[:, :, torch.arange(-acw, FRAMES + acw, device=dev).clamp(0, FRAMES - 1)].contiguous()
+            self.whole = lambda: m(z, cw)
+        elif name == "hifigan":
+            self.ref = torch.stack([m.inference(c[b]).t() for b in range(B)])
+            self.whole = lambda: m(cw)
+        else:
+            probe = CausalMelGANStream(m, batch=B, use_graphs=False)
+            assert probe.min_first_frames == self.open, probe.min_first_frames
+            self.delay = probe.delay
+            self.ref = F.pad(torch.stack([m.inference(c[b]).t() for b in range(B)]), (self.delay, 0))
+            self.whole = lambda: m.pqmf.synthesis(m(cw)) if m.pqmf is not None else m(cw)
+        self.samples = self.ref.shape[-1] - self.delay
+
+    def stream(self, B, graphs):
+        cls = {"pwg": CausalPWGStream, "hifigan": CausalHiFiGANStream}.get(self.name, CausalMelGANStream)
+        return cls(self.m, batch=B, use_graphs=graphs)
+
+    def push(self, st, j, n):
+        if self.name == "pwg":
+            return st.push(self.c[:, j:j + n], self.z[:, :, j * self.hop:(j + n) * self.hop])
+        return st.push(self.c[:, j:j + n])
+
+    def check(self, s, B, n):
+        if self.name == "pwg" and B * n * self.hop <= 65536:
+            assert s["bit_identical_to_inference"], (self.name, B, n)
+        else:
+            assert s["rel_l2_vs_inference"] <= 1e-6, (self.name, B, n, s["rel_l2_vs_inference"])
+
+
+def bench_model(name, Bs, dev):
+    m = build(name, dev)
+    res = {}
+    for B in Bs:
+        w = Workload(name, m, B, dev)
+        res.update(frames=w.frames, opening_push_frames=w.open)
+        for _ in range(3):
+            w.whole()
+        row = {"samples_per_item": w.samples, "delay_samples": w.delay,
+               "whole_utterance_forward": stats([timed(w.whole)[1] for _ in range(5)])}
+        audio_s = w.samples / SR
+        for graphs in (False, True):
+            for n in CHUNKS:
+                st = w.stream(B, graphs)
+                if w.open:  # warm-up: caches, weight packing, graph capture of every length
+                    w.push(st, 0, w.open)
+                w.push(st, w.open, n)
+                capi.reset_launch_count()
+                w.push(st, w.open + n, n)
+                launches = capi.launch_count()  # a steady-state push (0 with graphs: the replay launches nothing)
+                lat, total = [], 0.0
+                for _ in range(PASSES):
+                    st.reset()
+                    ys = []
+                    if w.open:
+                        y, t = timed(lambda: w.push(st, 0, w.open))
+                        ys.append(y)
+                        total += t
+                    for j in range(w.open, w.frames, n):
+                        y, t = timed(lambda: w.push(st, j, n))
+                        lat.append(t)
+                        total += t
+                        ys.append(y)
+                    if w.melgan:
+                        y, t = timed(st.flush)
+                        total += t
+                        ys.append(y)
+                y = torch.cat(ys, -1)
+                s = stats(lat)
+                s["rtf"] = total / PASSES / 1e3 / audio_s
+                if not graphs:
+                    s["libpwgb_launches_per_push"] = launches
+                s["bit_identical_to_inference"] = torch.equal(y, w.ref)
+                s["rel_l2_vs_inference"] = float((y - w.ref).double().norm() / w.ref.double().norm())
+                row[f"{'graph' if graphs else 'eager'}_chunk{n}"] = s
+                w.check(s, B, n)
+        res[f"B{B}"] = row
+    return res
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0], formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("model", nargs="?", choices=MODELS, help="the model to stream (default: every one)")
+    ap.add_argument("batch", nargs="*", type=int, default=[1, 16], help="batch sizes (default: 1 16)")
+    a = ap.parse_args()
+    dev = torch.device("cuda:0")
+    out = {"card": card(), "sample_rate_for_rtf": SR}
+    with torch.no_grad():
+        for name in [a.model] if a.model else MODELS:
+            out[name] = bench_model(name, a.batch, dev)
+    print(json.dumps(out, indent=1))
+
+
+if __name__ == "__main__":
+    main()
