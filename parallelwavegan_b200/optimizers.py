@@ -63,7 +63,8 @@ class _FusedBase(torch.optim.Optimizer):
         ent = self._tables.get(ids)
         if ent is None or ent[0] != key:  # first use, or an address changed (gradients re-allocated by zero_grad(set_to_none=True))
             t_host = torch.tensor(rows, dtype=torch.int64).pin_memory()
-            c_host = torch.tensor(chunks, dtype=torch.int32).reshape(-1, 2).pin_memory()
+            # only empty tensors: no chunk to launch, but the kernels' entry points still want a non-null chunk table
+            c_host = torch.tensor(chunks or [(0, 0)], dtype=torch.int32).reshape(-1, 2).pin_memory()
             if ent is None and len(self._tables) >= 8:
                 self._tables.clear()
             ent = (key, t_host.to(dev, non_blocking=True), c_host.to(dev, non_blocking=True), len(chunks),
