@@ -215,6 +215,39 @@ PWGB_API int pwgb_conv_transpose1d_window_stream_forward(const pwgb_convtr1d_des
  * last H samples of [hist | x] per row (also for n < H).  Every read of an entry happens before that entry's writes;
  * entries must not overlap each other.  A plain copy: deterministic. */
 PWGB_API int pwgb_stream_carry(const void* table, int n_entries, void* stream);
+/* Streaming a centred conv stack with a fixed lookahead.  A centred conv over [history | chunk] is the history conv
+ * above with its output labelled pad samples earlier, so each signal of such a stream runs in "delayed time": output row
+ * t of a chunk is signal sample frame[b] * rate - lookahead + t.  Two extensions of the history launches serve it:
+ *   mask (frame != NULL): frame and end are DEVICE arrays of batch int32, the frames a slot has pushed before this chunk
+ *     and its end frame (INT32_MAX while the signal is open); an output sample outside [0, end[b] * rate) is stored as
+ *     +0.0 (also with accumulate), which is the zero padding the whole-signal conv reads there.  rate >= 1; lookahead >= 0.
+ *   delayed residual (res_delay > 0 or res_hist_len > 0): output row t adds row t - res_delay of [res_hist | residual],
+ *     res_hist (batch, cout, res_hist_len) fp32; needs a residual and 0 <= res_delay <= res_hist_len.
+ * Every other value is computed exactly as by the entry point without the extension; with ext == NULL (or all fields
+ * zero) the call is that entry point.  A tensor-core launch with an extension keeps the register epilogue (same values
+ * as the staged one). */
+typedef struct pwgb_stream_ext {
+  const int* frame;
+  const int* end;
+  int rate;
+  int lookahead;
+  const float* res_hist;
+  int res_hist_len;
+  int res_delay;
+} pwgb_stream_ext;
+PWGB_API int pwgb_conv1d_stream_ext_forward(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len,
+                                            const int* replicate, const float* w, const float* bias, const float* residual,
+                                            const pwgb_stream_ext* ext, float* y, void* stream);
+PWGB_API int pwgb_conv1d_tc_stream_ext_forward(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len,
+                                               const int* replicate, const void* packed_w, const float* bias,
+                                               const float* residual, const pwgb_stream_ext* ext, float* y, void* stream);
+/* pwgb_conv_transpose1d_stream_forward with the mask of ext (no residual fields).  For a centred layer (kernel 2s,
+ * padding p) the window of cat(h, x) is whole-signal samples [a * s - p, (a + n) * s - p) when x starts at input sample
+ * a and h is sample a - 1 (zero for a fresh slot: pass no replicate flags), so lookahead = s * (input lookahead) + p. */
+PWGB_API int pwgb_conv_transpose1d_stream_ext_forward(const pwgb_convtr1d_desc* d, const float* x, const float* hist,
+                                                      const int* replicate, const float* w, const float* bias,
+                                                      const pwgb_stream_ext* ext, float* y, void* ws, size_t ws_bytes,
+                                                      void* stream);
 
 /* ------------------------------------------------------------------------
  * One HiFi-GAN ResBlock conv pair (layers/residual_block.py:243-258, non-causal, additional convs) in one

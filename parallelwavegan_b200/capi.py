@@ -33,6 +33,13 @@ class ConvTr1dDesc(C.Structure):
     ]
 
 
+class StreamExt(C.Structure):
+    _fields_ = [
+        ("frame", C.c_void_p), ("end", C.c_void_p), ("rate", C.c_int32), ("lookahead", C.c_int32),
+        ("res_hist", C.c_void_p), ("res_hist_len", C.c_int32), ("res_delay", C.c_int32),
+    ]
+
+
 class WaveNetDesc(C.Structure):
     _fields_ = [
         ("batch", C.c_int32), ("t", C.c_int32), ("residual_channels", C.c_int32), ("gate_channels", C.c_int32),
@@ -116,6 +123,14 @@ def lib():
                                                              C.c_size_t, vp]
     L.pwgb_stream_carry.restype = C.c_int
     L.pwgb_stream_carry.argtypes = [vp, C.c_int, vp]
+    L.pwgb_conv1d_stream_ext_forward.restype = C.c_int
+    L.pwgb_conv1d_stream_ext_forward.argtypes = [C.POINTER(Conv1dDesc), vp, vp, C.c_int, vp, vp, vp, vp, C.POINTER(StreamExt), vp, vp]
+    L.pwgb_conv1d_tc_stream_ext_forward.restype = C.c_int
+    L.pwgb_conv1d_tc_stream_ext_forward.argtypes = [C.POINTER(Conv1dDesc), vp, vp, C.c_int, vp, vp, vp, vp, C.POINTER(StreamExt), vp,
+                                                    vp]
+    L.pwgb_conv_transpose1d_stream_ext_forward.restype = C.c_int
+    L.pwgb_conv_transpose1d_stream_ext_forward.argtypes = [C.POINTER(ConvTr1dDesc), vp, vp, vp, vp, vp, C.POINTER(StreamExt), vp, vp,
+                                                           C.c_size_t, vp]
     L.pwgb_debug_set.restype = None
     L.pwgb_debug_set.argtypes = [C.c_int, C.c_int]
     L.pwgb_debug_get.restype = C.c_int
@@ -291,7 +306,8 @@ EXPORTED_SYMBOLS = [
     "pwgb_conv1d_tc_supported",
     "pwgb_conv1d_tc_forward", "pwgb_debug_set", "pwgb_debug_get",
     "pwgb_conv1d_stream_forward", "pwgb_conv1d_tc_stream_forward", "pwgb_conv_transpose1d_stream_forward",
-    "pwgb_conv_transpose1d_window_stream_forward", "pwgb_stream_carry",
+    "pwgb_conv_transpose1d_window_stream_forward", "pwgb_stream_carry", "pwgb_conv1d_stream_ext_forward",
+    "pwgb_conv1d_tc_stream_ext_forward", "pwgb_conv_transpose1d_stream_ext_forward",
     "pwgb_resblock_pair_supported", "pwgb_resblock_pair_plan", "pwgb_resblock_pair_forward",
     "pwgb_wavenet_supported", "pwgb_wavenet_packed_bytes",
     "pwgb_wavenet_pack", "pwgb_wavenet_layer_forward", "pwgb_upsample_fir_forward", "pwgb_upsample_fir_causal_forward",

@@ -12,6 +12,8 @@ void set_error(const char* fmt, ...);
 void count_launch(int n = 1);
 // argument check shared by the two history conv entry points (api.cu)
 int conv1d_stream_check(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len, const float* y);
+// argument check of a pwgb_stream_ext (NULL passes); residual: whether the launch has one
+int stream_ext_check(const pwgb_stream_ext* e, const float* residual);
 
 #define PWGB_CHECK_ARG(cond, ...)          \
   do {                                     \
@@ -47,6 +49,12 @@ __host__ __device__ inline bool is_history_pad(int pad_mode) {
 }
 
 __device__ __forceinline__ float lrelu(float v, float slope) { return v > 0.f ? v : v * slope; }
+
+// The mask of a pwgb_stream_ext launch: output row `row` of item b lies outside its signal
+__device__ __forceinline__ bool stream_outside(const int* frame, const int* end, int rate, int lookahead, int b, long long row) {
+  const long long pos = (long long)__ldg(frame + b) * rate - lookahead + row;
+  return pos < 0 || pos >= (long long)__ldg(end + b) * rate;
+}
 
 // Accurate-enough transcendental helpers: tanhf/expf from libdevice (<= 2 ulp);
 // the parity bar is 1e-3 relative so these are never the limiting error.

@@ -12,6 +12,8 @@
 #include <stdarg.h>
 #include <string.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace pwgb {
@@ -44,10 +46,25 @@ struct ConvK {
   int zero_rows;
 };
 
-// HIST: the history padding policy (pwgb_conv1d_stream_forward, groups 1, period 1) in the input staging loop; a template
-// argument so that the kernels without it keep their code and registers
-template <int RCO, int WARPS_CO, int RT, bool HIST>
-__global__ void __launch_bounds__(256) conv1d_fwd_kernel(const ConvK p, const float* __restrict__ x, const float* __restrict__ w,
+// The parameters of an EXT history launch (pwgb_stream_ext): the mask (output row o, of for a shuffled launch, is signal
+// sample mframe[b] * mrate - mlook + o; outside the signal it stores +0.0) and the delayed residual (row o adds row
+// o - rdelay of [rhist | rres]; the kernel's res argument is null).  A separate struct, so that the kernels without EXT
+// keep their parameters and code.
+struct ConvKExt : ConvK {
+  const int* mframe;
+  const int* mend;
+  int mrate, mlook;
+  const float* rres;
+  const float* rhist;
+  int rhist_len, rdelay;
+};
+
+// HIST: the history padding policy (pwgb_conv1d_stream_forward, groups 1, period 1) in the input staging loop; EXT (with
+// HIST only): the mask and the delayed residual of pwgb_conv1d_stream_ext_forward in the epilogue.  Template arguments so
+// that the kernels without them keep their code and registers.
+template <int RCO, int WARPS_CO, int RT, bool HIST, bool EXT = false>
+__global__ void __launch_bounds__(256) conv1d_fwd_kernel(const std::conditional_t<EXT, ConvKExt, ConvK> p,
+                                                const float* __restrict__ x, const float* __restrict__ w,
                                                 const float* __restrict__ bias, const float* __restrict__ res,
                                                 float* __restrict__ y) {
   constexpr int WARPS_T = 8 / WARPS_CO;
@@ -217,6 +234,19 @@ __global__ void __launch_bounds__(256) conv1d_fwd_kernel(const ConvK p, const fl
       } else {
         yi = (long long)b * p.ybs + (long long)co * p.Lout + o;
       }
+      if constexpr (EXT) {
+        // the mask sees the output row (of for a shuffled launch; period 1); the delayed residual is p.rres (res is null)
+        const int orow = p.shuffle > 1 ? o * p.shuffle + (co - (co / p.shuffle) * p.shuffle) - p.shuffle_pad : o;
+        if (p.mframe && stream_outside(p.mframe, p.mend, p.mrate, p.mlook, b, orow)) {
+          y[yi] = 0.f;
+          continue;
+        }
+        if (p.rres) {
+          const int ro = o - p.rdelay;
+          v += ro >= 0 ? __ldg(p.rres + (long long)b * p.rbs + (long long)co * p.Lout + ro)
+                       : __ldg(p.rhist + ((long long)b * p.Cout + co) * p.rhist_len + (p.rhist_len + ro));
+        }
+      }
       if (res) v += __ldg(res + (long long)b * p.rbs + (long long)co * p.Lout + o);
       v *= p.out_scale;
       if (p.accumulate) v += y[yi];
@@ -225,8 +255,8 @@ __global__ void __launch_bounds__(256) conv1d_fwd_kernel(const ConvK p, const fl
   }
 }
 
-template <int RCO, int WARPS_CO, int RT, bool HIST>
-static int launch_conv_rt(ConvK p, const float* x, const float* w, const float* bias, const float* res, float* y,
+template <int RCO, int WARPS_CO, int RT, bool HIST, bool EXT, class P>
+static int launch_conv_rt(P p, const float* x, const float* w, const float* bias, const float* res, float* y,
                        cudaStream_t st) {
   constexpr int WARPS_T = 8 / WARPS_CO;
   constexpr int CO_T = RCO * WARPS_CO;
@@ -249,7 +279,7 @@ static int launch_conv_rt(ConvK p, const float* x, const float* w, const float* 
   p.CI_T = ci_t;
   p.XW = (int)XW;
   p.tiles_per_group = ceil_div(p.Cout_g, CO_T);
-  auto kern = conv1d_fwd_kernel<RCO, WARPS_CO, RT, HIST>;
+  auto kern = conv1d_fwd_kernel<RCO, WARPS_CO, RT, HIST, EXT>;
   if (bytes > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (e != cudaSuccess) {
@@ -409,12 +439,12 @@ __global__ void __launch_bounds__(256) conv1d_fewcout_long_kernel(const ConvK p,
 }
 
 // short sequences (discriminator tails, 10-50 positions per item): 1 position per lane instead of 4
-template <int RCO, int WARPS_CO, bool HIST = false>
-static int launch_conv(ConvK p, const float* x, const float* w, const float* bias, const float* res, float* y,
+template <int RCO, int WARPS_CO, bool HIST = false, bool EXT = false, class P = ConvK>
+static int launch_conv(P p, const float* x, const float* w, const float* bias, const float* res, float* y,
                        cudaStream_t st) {
   constexpr int WARPS_T = 8 / WARPS_CO;
-  if (p.Lout <= 40 * WARPS_T) return launch_conv_rt<RCO, WARPS_CO, 1, HIST>(p, x, w, bias, res, y, st);
-  return launch_conv_rt<RCO, WARPS_CO, 4, HIST>(p, x, w, bias, res, y, st);
+  if (p.Lout <= 40 * WARPS_T) return launch_conv_rt<RCO, WARPS_CO, 1, HIST, EXT>(p, x, w, bias, res, y, st);
+  return launch_conv_rt<RCO, WARPS_CO, 4, HIST, EXT>(p, x, w, bias, res, y, st);
 }
 
 static void conv_params(const pwgb_conv1d_desc* d, ConvK& p) {
@@ -494,11 +524,11 @@ int conv1d_forward_simt(const pwgb_conv1d_desc* d, const float* x, const float* 
 
 // History launches (pad_mode PWGB_PAD_HISTORY, groups 1, period 1) always take the generic kernel: the few-channel
 // kernels above sum in an order that depends on where a sample sits in the sequence, which a stream cannot reproduce.
-// zero_flag / zero_rows: see ConvK (shuffled launches only).
+// zero_flag / zero_rows: see ConvK (shuffled launches only); ext: the mask and the delayed residual (pwgb_stream_ext).
 int conv1d_stream_simt(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len, const int* rep,
                        const float* w, const float* bias, const float* residual, float* y, cudaStream_t st,
-                       const int* zero_flag, int zero_rows) {
-  ConvK p;
+                       const int* zero_flag, int zero_rows, const pwgb_stream_ext* ext) {
+  ConvKExt p;
   conv_params(d, p);
   p.hist = hist;
   p.rep = rep;
@@ -507,12 +537,30 @@ int conv1d_stream_simt(const pwgb_conv1d_desc* d, const float* x, const float* h
   p.zero_rows = zero_rows;
   if (p.B == 0 || p.Lout == 0) return PWGB_OK;
   const int cg = p.Cout_g;
-  if (cg >= 64) return launch_conv<8, 8, true>(p, x, w, bias, residual, y, st);
-  if (cg >= 32) return launch_conv<8, 4, true>(p, x, w, bias, residual, y, st);
-  if (cg >= 16) return launch_conv<8, 2, true>(p, x, w, bias, residual, y, st);
-  if (cg >= 8) return launch_conv<8, 1, true>(p, x, w, bias, residual, y, st);
-  if (cg >= 4) return launch_conv<4, 1, true>(p, x, w, bias, residual, y, st);
-  return launch_conv<1, 1, true>(p, x, w, bias, residual, y, st);
+  if (ext) {
+    // the EXT instantiations: without an extension the launch keeps the HIST kernels of the causal streams
+    p.mframe = ext->frame;
+    p.mend = ext->end;
+    p.mrate = ext->rate;
+    p.mlook = ext->lookahead;
+    p.rhist = ext->res_hist;
+    p.rhist_len = ext->res_hist_len;
+    p.rdelay = ext->res_delay;
+    p.rres = residual;
+    if (cg >= 64) return launch_conv<8, 8, true, true>(p, x, w, bias, nullptr, y, st);
+    if (cg >= 32) return launch_conv<8, 4, true, true>(p, x, w, bias, nullptr, y, st);
+    if (cg >= 16) return launch_conv<8, 2, true, true>(p, x, w, bias, nullptr, y, st);
+    if (cg >= 8) return launch_conv<8, 1, true, true>(p, x, w, bias, nullptr, y, st);
+    if (cg >= 4) return launch_conv<4, 1, true, true>(p, x, w, bias, nullptr, y, st);
+    return launch_conv<1, 1, true, true>(p, x, w, bias, nullptr, y, st);
+  }
+  const ConvK& q = p;
+  if (cg >= 64) return launch_conv<8, 8, true>(q, x, w, bias, residual, y, st);
+  if (cg >= 32) return launch_conv<8, 4, true>(q, x, w, bias, residual, y, st);
+  if (cg >= 16) return launch_conv<8, 2, true>(q, x, w, bias, residual, y, st);
+  if (cg >= 8) return launch_conv<8, 1, true>(q, x, w, bias, residual, y, st);
+  if (cg >= 4) return launch_conv<4, 1, true>(q, x, w, bias, residual, y, st);
+  return launch_conv<1, 1, true>(q, x, w, bias, residual, y, st);
 }
 
 }  // namespace pwgb

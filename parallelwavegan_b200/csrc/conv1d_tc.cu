@@ -73,6 +73,19 @@ struct TcK {
   int hist_len;
 };
 
+// The parameters of an EXT history launch (conv1d_tc_ext_kernel, pwgb_stream_ext; register epilogue only): the mask
+// (output row t, or the shuffled row, is signal sample mframe[b] * mrate - mlook + t; outside the signal it stores +0.0)
+// and the delayed residual (row t adds row t - rdelay of [rhist | res], rhist (B, total cout, rhist_len)).  A separate
+// struct, so that the kernels without EXT keep their parameters and code.
+struct TcKExt : TcK {
+  const int* mframe;
+  const int* mend;
+  int mrate, mlook;
+  const float* rhist;
+  int rhist_len, rdelay;
+  long long rhbs;
+};
+
 // Staged epilogue: one tile (fp32 [col][stage_ld(MT)], tc_common.cuh) per consumer warpgroup.  Tile shapes compiled with
 // it: at MT = 2 and more than 32 columns it made ptxas spill, and its tiles would not fit beside the pipeline there anyway.
 __host__ __device__ constexpr bool stage_shape(int mt, int cout) { return mt == 1 || cout <= 32; }
@@ -125,8 +138,8 @@ void tc_pack_rows(const float* w, void* packed, int cin_real, int cin_pad, int r
 // (EPI_SHUFFLE: p.shuffle > 1, EPI_WAVENET: p.wavenet, else EPI_PLAIN) is a template argument so the consumers branch on
 // it once per 64-row block, not per element.
 enum { EPI_PLAIN, EPI_SHUFFLE, EPI_WAVENET };
-template <int MODE>
-__device__ __forceinline__ void epi_store(const TcK& p, float a, int b, int t, int col, int co_base, const float* __restrict__ bias,
+template <int MODE, bool EXT, class P>
+__device__ __forceinline__ void epi_store(const P& p, float a, int b, int t, int col, int co_base, const float* __restrict__ bias,
                                           const float* bias_s, const float* __restrict__ res, float* __restrict__ y,
                                           float* __restrict__ y2) {
   const long long st = p.T_out;
@@ -138,6 +151,14 @@ __device__ __forceinline__ void epi_store(const TcK& p, float a, int b, int t, i
     else if (p.post_act == PWGB_ACT_LRELU)
       v = lrelu(v, p.post_slope);
     const int of = t * p.shuffle + (co - cof * p.shuffle) - p.shuffle_pad;
+    if constexpr (EXT) {
+      if (of >= 0 && of < p.shuffle_tout) {
+        v *= p.out_scale;
+        if (p.mframe && stream_outside(p.mframe, p.mend, p.mrate, p.mlook, b, of)) v = 0.f;
+        y[(long long)b * p.ybs + (long long)cof * p.shuffle_tout + of] = v;
+      }
+      return;
+    }
     if (of >= 0 && of < p.shuffle_tout) y[(long long)b * p.ybs + (long long)cof * p.shuffle_tout + of] = v * p.out_scale;
   } else if constexpr (MODE == EPI_WAVENET) {
     // WaveNet split epilogue (residual_block.py:131-138): columns [0, split) are the skip 1x1
@@ -155,10 +176,21 @@ __device__ __forceinline__ void epi_store(const TcK& p, float a, int b, int t, i
     const long long off = (long long)(co_base + col) * st + t;
     float v = a + bias_s[co_base - p.co_off + col];
     if (p.post_act != PWGB_ACT_NONE) v = p.post_act == PWGB_ACT_TANH ? tanhf(v) : lrelu(v, p.post_slope);
-    if (res) v += __ldg(res + (long long)b * p.rbs + off);
+    if constexpr (EXT) {
+      if (res) {
+        const int ro = t - p.rdelay;
+        v += ro >= 0 ? __ldg(res + (long long)b * p.rbs + off - p.rdelay)
+                     : __ldg(p.rhist + (long long)b * p.rhbs + (long long)(co_base + col) * p.rhist_len + (p.rhist_len + ro));
+      }
+    } else {
+      if (res) v += __ldg(res + (long long)b * p.rbs + off);
+    }
     v *= p.out_scale;
     float* q = y + (long long)b * p.ybs + off;
     if (p.accumulate) v += *q;
+    if constexpr (EXT) {
+      if (p.mframe && stream_outside(p.mframe, p.mend, p.mrate, p.mlook, b, t)) v = 0.f;
+    }
     *q = v;
   }
 }
@@ -280,9 +312,11 @@ __device__ __forceinline__ void fill_main_chunk(const TcK& p, const float* __res
 // MT (64-row blocks per warpgroup) and NB16 (16-column blocks, Cout = 16 * NB16) are compile-time constants, so the
 // consumers issue a fixed wgmma sequence into fixed accumulator registers (tc_launch picks the instantiation).  HIST: the
 // history padding policy on the element-addressed producers (cp.async-staged and direct; history launches never take
-// the TMA activation path).  It is a template argument so that the kernels without it keep their code.
-template <int MT, int NB16, bool HIST>
-__device__ __forceinline__ void conv1d_tc_body(const TcK& p, const float* __restrict__ x, const float* __restrict__ x2,
+// the TMA activation path).  EXT (with HIST only): the mask and the delayed residual of a pwgb_stream_ext launch in the
+// register epilogue, with the parameters of TcKExt.  They are template arguments so that the kernels without them keep
+// their code.
+template <int MT, int NB16, bool HIST, bool EXT = false>
+__device__ __forceinline__ void conv1d_tc_body(const std::conditional_t<EXT, TcKExt, TcK>& p, const float* __restrict__ x, const float* __restrict__ x2,
                                                const uint4* __restrict__ wpk, const float* __restrict__ bias,
                                                const float* __restrict__ res, float* __restrict__ y, float* __restrict__ y2) {
   extern __shared__ __align__(128) unsigned char smem[];
@@ -568,7 +602,7 @@ __device__ __forceinline__ void conv1d_tc_body(const TcK& p, const float* __rest
         for (int i = 0; i < NACC; ++i) {
           const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
           const int t = t0 + (wg * MT + mb) * 64 + wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
-          if (t < p.T_out) epi_store<decltype(mode)::value>(p, ab[i], b, t, col, co_base, bias, bias_s, res, y, y2);
+          if (t < p.T_out) epi_store<decltype(mode)::value, EXT>(p, ab[i], b, t, col, co_base, bias, bias_s, res, y, y2);
         }
       };
 #pragma unroll
@@ -659,6 +693,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
                           const uint4* __restrict__ wpk, const float* __restrict__ bias, const float* __restrict__ res,
                           float* __restrict__ y, float* __restrict__ y2) {
   conv1d_tc_body<MT, NB16, true>(p, x, x2, wpk, bias, res, y, y2);
+}
+
+// history launches with a pwgb_stream_ext (pwgb_conv1d_tc_stream_ext_forward, the masked stream conv-transpose)
+template <int MT, int NB16>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+    conv1d_tc_ext_kernel(const TcKExt p, const float* __restrict__ x, const float* __restrict__ x2,
+                         const uint4* __restrict__ wpk, const float* __restrict__ bias, const float* __restrict__ res,
+                         float* __restrict__ y, float* __restrict__ y2) {
+  conv1d_tc_body<MT, NB16, true, true>(p, x, x2, wpk, bias, res, y, y2);
 }
 
 static int g_tc_variant = 0;
@@ -817,6 +860,18 @@ static const TcKernel tc_hist_kernels[12] = {
     conv1d_tc_hist_kernel<1, 1>, conv1d_tc_hist_kernel<1, 2>, conv1d_tc_hist_kernel<1, 3>, conv1d_tc_hist_kernel<1, 4>,
     conv1d_tc_hist_kernel<1, 5>, conv1d_tc_hist_kernel<1, 6>, conv1d_tc_hist_kernel<1, 7>, conv1d_tc_hist_kernel<1, 8>,
     conv1d_tc_hist_kernel<2, 1>, conv1d_tc_hist_kernel<2, 2>, conv1d_tc_hist_kernel<2, 3>, conv1d_tc_hist_kernel<2, 4>};
+using TcKernelExt = void (*)(const TcKExt, const float*, const float*, const uint4*, const float*, const float*, float*, float*);
+static const TcKernelExt tc_ext_kernels[12] = {
+    conv1d_tc_ext_kernel<1, 1>, conv1d_tc_ext_kernel<1, 2>, conv1d_tc_ext_kernel<1, 3>, conv1d_tc_ext_kernel<1, 4>,
+    conv1d_tc_ext_kernel<1, 5>, conv1d_tc_ext_kernel<1, 6>, conv1d_tc_ext_kernel<1, 7>, conv1d_tc_ext_kernel<1, 8>,
+    conv1d_tc_ext_kernel<2, 1>, conv1d_tc_ext_kernel<2, 2>, conv1d_tc_ext_kernel<2, 3>, conv1d_tc_ext_kernel<2, 4>};
+static TcKernelExt tc_ext_kernel_for(int mt, int cout) {
+  if (cout % 16 != 0) return nullptr;
+  const int nb16 = cout / 16;
+  if (mt == 1 && nb16 >= 1 && nb16 <= 8) return tc_ext_kernels[nb16 - 1];
+  if (mt == 2 && nb16 >= 1 && nb16 <= 4) return tc_ext_kernels[8 + nb16 - 1];
+  return nullptr;
+}
 static TcKernel tc_kernel_for(int mt, int cout, bool hist) {
   if (cout % 16 != 0) return nullptr;
   const TcKernel* table = hist ? tc_hist_kernels : tc_kernels;
@@ -826,20 +881,31 @@ static TcKernel tc_kernel_for(int mt, int cout, bool hist) {
   return nullptr;
 }
 
-static int tc_launch(TcK& p, size_t bytes, const float* x, const void* packed_w, const float* bias,
+// P: TcK, or TcKExt for the EXT kernels of a pwgb_stream_ext launch
+template <class P>
+static int tc_launch(P& p, size_t bytes, const float* x, const void* packed_w, const float* bias,
                      const float* residual, float* y, cudaStream_t st, const float* x2 = nullptr,
                      float* y2 = nullptr) {
   if (p.B == 0 || p.T_out == 0) return PWGB_OK;
+  constexpr bool ext = std::is_same<P, TcKExt>::value;
   const bool hist = is_history_pad(p.pad_mode);
-  const TcKernel kernel = tc_kernel_for(p.MT, p.Cout, hist);
+  std::conditional_t<ext, TcKernelExt, TcKernel> kernel;
+  if constexpr (ext)
+    kernel = tc_ext_kernel_for(p.MT, p.Cout);
+  else
+    kernel = tc_kernel_for(p.MT, p.Cout, hist);
   if (!kernel) {
     set_error("conv1d_tc: no kernel instantiation for MT = %d, Cout = %d", p.MT, p.Cout);
     return PWGB_UNSUPPORTED;
   }
   static bool smem_set = false, smem_set_hist = false;
-  if (const int rc = hist ? smem_opt_in(smem_set_hist, tc_hist_kernels, (int)TC_SMEM_STAGED, "conv1d_tc")
-                          : smem_opt_in(smem_set, tc_kernels, (int)TC_SMEM_STAGED, "conv1d_tc"))
-    return rc;
+  if constexpr (ext) {
+    if (const int rc = smem_opt_in(smem_set, tc_ext_kernels, (int)TC_SMEM_STAGED, "conv1d_tc")) return rc;
+  } else {
+    if (const int rc = hist ? smem_opt_in(smem_set_hist, tc_hist_kernels, (int)TC_SMEM_STAGED, "conv1d_tc")
+                            : smem_opt_in(smem_set, tc_kernels, (int)TC_SMEM_STAGED, "conv1d_tc"))
+      return rc;
+  }
   const int num_sms = tc_num_sms();
   if ((long long)p.B * p.tiles_per_seq > 0x7fffffffLL) {
     set_error("conv1d_tc: too many tiles");
@@ -855,13 +921,27 @@ static int tc_launch(TcK& p, size_t bytes, const float* x, const void* packed_w,
   return check_launch("conv1d_tc_kernel");
 }
 
+// The pwgb_stream_ext of a history launch, for the EXT kernels.  Their epilogue reads residual rows one by one and masks each
+// store, so the launch keeps the register epilogue, which computes the staged epilogue's values.
+static void tc_apply_ext(TcKExt& p, const pwgb_stream_ext* e, int cout_total) {
+  p.mframe = e->frame;
+  p.mend = e->end;
+  p.mrate = e->rate;
+  p.mlook = e->lookahead;
+  p.rhist = e->res_hist;
+  p.rhist_len = e->res_hist_len;
+  p.rdelay = e->res_delay;
+  p.rhbs = (long long)cout_total * e->res_hist_len;
+  p.staged = 0;
+}
+
 // Internal entry for N-chunked callers (conv_transpose): runs output channels
 // [co_off, co_off + d->cout) of a conv whose full output has cout_total channels.  cin1 > 0: the input is
 // cat(x (B, cin1, T), x2 (B, d->cin - cin1, T)) along channels (cin1 a multiple of KC).  d->pad_mode ==
 // PWGB_PAD_HISTORY: a history launch reading rows before sample 0 from hist / rep (one source only).
 int conv1d_tc_chunk(const pwgb_conv1d_desc* d, int co_off, int cout_total, const float* x, const void* packed_w,
                     const float* bias, float* y, cudaStream_t st, int nco, const float* x2, int cin1, const float* hist,
-                    const int* rep, int hist_len) {
+                    const int* rep, int hist_len, const pwgb_stream_ext* ext) {
   TcK p;
   size_t bytes = 0;
   if (!tc_plan(d, p, bytes)) return PWGB_UNSUPPORTED;
@@ -884,6 +964,12 @@ int conv1d_tc_chunk(const pwgb_conv1d_desc* d, int co_off, int cout_total, const
     if (d->shuffle <= 1 || (long long)p.total_tiles * nco > 0x7fffffffLL) return PWGB_UNSUPPORTED;
     p.nco = nco;
     p.total_tiles *= nco;
+  }
+  if (ext && is_history_pad(d->pad_mode)) {
+    TcKExt px;
+    static_cast<TcK&>(px) = p;
+    tc_apply_ext(px, ext, cout_total);
+    return tc_launch(px, bytes, x, packed_w, bias, nullptr, y, st);
   }
   return tc_launch(p, bytes, x, packed_w, bias, nullptr, y, st, cin1 > 0 ? x2 : nullptr);
 }
@@ -993,7 +1079,8 @@ extern "C" int pwgb_conv1d_tc_supported(const pwgb_conv1d_desc* d) {
 }
 
 static int tc_forward(const pwgb_conv1d_desc* d, const float* x, const void* packed_w, const float* bias, const float* residual,
-                      float* y, void* stream, const float* hist, const int* rep, int hist_len) {
+                      float* y, void* stream, const float* hist, const int* rep, int hist_len,
+                      const pwgb_stream_ext* ext = nullptr) {
   PWGB_UNSUPPORTED_IF(!pwgb_conv1d_tc_supported(d), "conv1d_tc: configuration not supported by the tensor-core path");
   const int G = d->groups, cin_g = d->cin / G, cout_g = d->cout / G;
   const int chunk = tc_cout_chunk(cout_g);
@@ -1027,6 +1114,12 @@ static int tc_forward(const pwgb_conv1d_desc* d, const float* x, const void* pac
   p.hist = hist;
   p.rep = rep;
   p.hist_len = hist_len;
+  if (ext) {
+    TcKExt px;
+    static_cast<TcK&>(px) = p;
+    tc_apply_ext(px, ext, d->cout);
+    return tc_launch(px, bytes, x, packed_w, bias, residual, y, (cudaStream_t)stream);
+  }
   return tc_launch(p, bytes, x, packed_w, bias, residual, y, (cudaStream_t)stream);
 }
 
@@ -1043,6 +1136,15 @@ extern "C" int pwgb_conv1d_tc_stream_forward(const pwgb_conv1d_desc* d, const fl
   PWGB_CHECK_ARG(packed_w, "conv1d_tc_stream: null argument");
   if (const int rc = conv1d_stream_check(d, x, hist, hist_len, y)) return rc;
   return tc_forward(d, x, packed_w, bias, residual, y, stream, hist, replicate, hist_len);
+}
+
+extern "C" int pwgb_conv1d_tc_stream_ext_forward(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len,
+                                                 const int* replicate, const void* packed_w, const float* bias,
+                                                 const float* residual, const pwgb_stream_ext* ext, float* y, void* stream) {
+  PWGB_CHECK_ARG(packed_w, "conv1d_tc_stream: null argument");
+  if (const int rc = conv1d_stream_check(d, x, hist, hist_len, y)) return rc;
+  if (const int rc = stream_ext_check(ext, residual)) return rc;
+  return tc_forward(d, x, packed_w, bias, residual, y, stream, hist, replicate, hist_len, ext);
 }
 
 // ======================================================================================

@@ -11,10 +11,11 @@ int conv1d_forward_simt(const pwgb_conv1d_desc* d, const float* x, const float* 
                         const float* residual, float* y, cudaStream_t st);
 int conv1d_tc_chunk(const pwgb_conv1d_desc* d, int co_off, int cout_total, const float* x, const void* packed_w,
                     const float* bias, float* y, cudaStream_t st, int nco, const float* x2 = nullptr, int cin1 = 0,
-                    const float* hist = nullptr, const int* rep = nullptr, int hist_len = 0);
+                    const float* hist = nullptr, const int* rep = nullptr, int hist_len = 0,
+                    const pwgb_stream_ext* ext = nullptr);
 int conv1d_stream_simt(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len, const int* rep,
                        const float* w, const float* bias, const float* residual, float* y, cudaStream_t st,
-                       const int* zero_flag = nullptr, int zero_rows = 0);
+                       const int* zero_flag = nullptr, int zero_rows = 0, const pwgb_stream_ext* ext = nullptr);
 int conv1d_tc_plan_ok(const pwgb_conv1d_desc* d, int* raw_staged = nullptr);
 void tc_pack_weight(const float* w, int cin, int cout, int kernel, void* packed, cudaStream_t st);
 
@@ -108,7 +109,7 @@ static int convtr_tc_chunk(const pwgb_conv1d_desc& c, bool two_source) {
 // rep[b] is set): the virtual conv runs on x with that frame as a one-row history.
 static int convtr_forward(const pwgb_convtr1d_desc* d, const float* x, const float* x2, int cin1, const float* w,
                           const float* bias, float* y, void* ws, size_t ws_bytes, void* stream, bool hist_mode = false,
-                          const float* hist = nullptr, const int* rep = nullptr) {
+                          const float* hist = nullptr, const int* rep = nullptr, const pwgb_stream_ext* ext = nullptr) {
   const int s = d->stride, K = d->kernel, M = ceil_div(K, s);
   const int G = d->groups > 1 ? d->groups : 1;
   const size_t need = pwgb_conv_transpose1d_workspace(d);
@@ -141,10 +142,10 @@ static int convtr_forward(const pwgb_convtr1d_desc* d, const float* x, const flo
       rc = check_launch("tc_pack_weight_kernel");
       if (rc) return rc;
     }
-    if (hist_mode) return conv1d_tc_chunk(&cc, 0, c.cout, x, pk, bias, y, st, c.cout / chunk, nullptr, 0, hist, rep, 1);
+    if (hist_mode) return conv1d_tc_chunk(&cc, 0, c.cout, x, pk, bias, y, st, c.cout / chunk, nullptr, 0, hist, rep, 1, ext);
     return conv1d_tc_chunk(&cc, 0, c.cout, x, pk, bias, y, st, c.cout / chunk, x2, cin1);
   }
-  if (hist_mode) return conv1d_stream_simt(&c, x, hist, 1, rep, wv, bias, nullptr, y, st);
+  if (hist_mode) return conv1d_stream_simt(&c, x, hist, 1, rep, wv, bias, nullptr, y, st, nullptr, 0, ext);
   if (cin1 > 0) {
     set_error("conv_transpose1d_cat: configuration not supported by the tensor-core path");
     return PWGB_UNSUPPORTED;
@@ -188,6 +189,20 @@ extern "C" int pwgb_conv_transpose1d_stream_forward(const pwgb_convtr1d_desc* d,
   PWGB_UNSUPPORTED_IF(d->groups > 1 || d->period > 1 || d->padding != d->stride,
                       "conv_transpose1d_stream: the causal conv-transpose is dense, plain and has padding == stride");
   return convtr_forward(d, x, nullptr, 0, w, bias, y, ws, ws_bytes, stream, true, hist, replicate);
+}
+
+extern "C" int pwgb_conv_transpose1d_stream_ext_forward(const pwgb_convtr1d_desc* d, const float* x, const float* hist,
+                                                        const int* replicate, const float* w, const float* bias,
+                                                        const pwgb_stream_ext* ext, float* y, void* ws, size_t ws_bytes,
+                                                        void* stream) {
+  PWGB_CHECK_ARG(d && x && hist && w && y, "conv_transpose1d_stream: null argument");
+  const int rc = convtr_desc_ok(d);
+  if (rc) return rc;
+  PWGB_CHECK_ARG(d->t_in >= 2, "conv_transpose1d_stream: t_in counts the history frame and at least one input frame");
+  PWGB_UNSUPPORTED_IF(d->groups > 1 || d->period > 1 || d->padding != d->stride,
+                      "conv_transpose1d_stream: the stream conv-transpose is dense, plain and has padding == stride");
+  if (const int rc2 = stream_ext_check(ext, nullptr)) return rc2;
+  return convtr_forward(d, x, nullptr, 0, w, bias, y, ws, ws_bytes, stream, true, hist, replicate, ext);
 }
 
 // The window of virtual positions [T0, T0 + n) of the whole signal's virtual conv, all phases: the virtual conv runs on x

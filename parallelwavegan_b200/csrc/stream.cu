@@ -6,7 +6,18 @@ namespace pwgb {
 
 int conv1d_stream_simt(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len, const int* rep,
                        const float* w, const float* bias, const float* residual, float* y, cudaStream_t st,
-                       const int* zero_flag = nullptr, int zero_rows = 0);
+                       const int* zero_flag = nullptr, int zero_rows = 0, const pwgb_stream_ext* ext = nullptr);
+
+int stream_ext_check(const pwgb_stream_ext* e, const float* residual) {
+  if (!e) return PWGB_OK;
+  PWGB_CHECK_ARG(!e->frame || (e->end && e->rate >= 1 && e->lookahead >= 0),
+                 "stream_ext: a mask needs end flags, rate >= 1 and lookahead >= 0 (rate %d, lookahead %d)", e->rate, e->lookahead);
+  PWGB_CHECK_ARG(e->res_hist_len >= 0 && e->res_delay >= 0 && e->res_delay <= e->res_hist_len &&
+                     (e->res_hist_len == 0 || e->res_hist),
+                 "stream_ext: bad residual history (res_hist_len %d, res_delay %d)", e->res_hist_len, e->res_delay);
+  PWGB_CHECK_ARG(residual || e->res_hist_len == 0, "stream_ext: a residual history needs a residual");
+  return PWGB_OK;
+}
 
 int conv1d_stream_check(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len, const float* y) {
   PWGB_CHECK_ARG(d && x && y, "conv1d_stream: null argument");
@@ -71,6 +82,15 @@ extern "C" int pwgb_conv1d_stream_forward(const pwgb_conv1d_desc* d, const float
   PWGB_CHECK_ARG(w, "conv1d_stream: null argument");
   if (const int rc = conv1d_stream_check(d, x, hist, hist_len, y)) return rc;
   return conv1d_stream_simt(d, x, hist, hist_len, replicate, w, bias, residual, y, (cudaStream_t)stream);
+}
+
+extern "C" int pwgb_conv1d_stream_ext_forward(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len,
+                                              const int* replicate, const float* w, const float* bias, const float* residual,
+                                              const pwgb_stream_ext* ext, float* y, void* stream) {
+  PWGB_CHECK_ARG(w, "conv1d_stream: null argument");
+  if (const int rc = conv1d_stream_check(d, x, hist, hist_len, y)) return rc;
+  if (const int rc = stream_ext_check(ext, residual)) return rc;
+  return conv1d_stream_simt(d, x, hist, hist_len, replicate, w, bias, residual, y, (cudaStream_t)stream, nullptr, 0, ext);
 }
 
 extern "C" int pwgb_stream_carry(const void* table, int n_entries, void* stream) {

@@ -394,14 +394,38 @@ def upsample_fir_causal_stream(x, fir, scale, hist, out=None, out_channels=None)
     return out
 
 
+def _stream_ext(B, cout, mask, res_hist, res_delay):
+    """The pwgb_stream_ext of a stream launch, or None when it has neither a mask nor a delayed residual"""
+    if mask is None and res_hist is None and not res_delay:
+        return None
+    frame, end, rate, lookahead = mask if mask is not None else (None, None, 1, 0)
+    for t, name in ((frame, "frame"), (end, "end")):
+        if mask is not None and (t.dtype != torch.int32 or not t.is_cuda or t.numel() != B or not t.is_contiguous()):
+            raise PwgbError(f"stream mask: {name} must be {B} contiguous int32 counters on the device")
+    H = 0
+    if res_hist is not None:
+        res_hist = _dev(res_hist, "res_hist")
+        if res_hist.dim() != 3 or tuple(res_hist.shape[:2]) != (B, cout):
+            raise PwgbError(f"stream residual: res_hist must be ({B}, {cout}, H), got {tuple(res_hist.shape)}")
+        H = res_hist.shape[-1]
+    return capi.StreamExt(frame=_p(frame), end=_p(end), rate=int(rate), lookahead=int(lookahead),
+                          res_hist=_p(res_hist) if H else None, res_hist_len=H, res_delay=int(res_delay))
+
+
 def conv1d_stream(x, hist, w, bias=None, *, pad_left, dilation=1, replicate=None, reflect=False, pre_slope=1.0, post_act=None,
-                  post_slope=0.0, residual=None, out_scale=1.0, out=None, accumulate=False):
+                  post_slope=0.0, residual=None, out_scale=1.0, out=None, accumulate=False, t_out=None, mask=None, res_hist=None,
+                  res_delay=0):
     """conv1d with history padding (pwgb_conv1d_stream_forward / pwgb_conv1d_tc_stream_forward): of the ``pad_left`` rows
     in front of x, the last H read ``hist`` (B, cin, H) -- or x[:, :, 0] for the items whose ``replicate`` (B,) int32 flag
     is set -- and the earlier ones are zero; no right padding.  With ``reflect`` a flagged item reads row -t from x[:, :, t]
     instead (ReflectionPad1d for a fresh signal, PWGB_PAD_HISTORY_REFLECT; needs pad_left < x's length).  Everything else
     is conv1d's, and so is the engine choice (including the 16-column and 32-channel paddings of conv1d), so a chunked run
-    equals conv1d on the whole signal."""
+    equals conv1d on the whole signal.
+
+    The extensions of a lookahead stream (pwgb_*_stream_ext_forward): ``t_out`` fewer output rows than the input allows
+    (the later input rows are not read); ``mask`` = (frame, end, rate, lookahead): (B,) int32 device counters, output row
+    t of item b is signal sample frame[b] * rate - lookahead + t, stored as +0.0 outside [0, end[b] * rate);
+    ``res_hist`` (B, cout, Hr) / ``res_delay``: row t adds row t - res_delay of [res_hist | residual]."""
     x, w = _dev(x, "x"), _dev(w, "w")
     B, cin, L = x.shape
     cout, cin_w, K = w.shape
@@ -413,7 +437,7 @@ def conv1d_stream(x, hist, w, bias=None, *, pad_left, dilation=1, replicate=None
     if replicate is not None and (replicate.dtype != torch.int32 or not replicate.is_cuda or replicate.numel() != B):
         raise PwgbError(f"conv1d_stream: replicate must be {B} int32 flags on the device")
     kw = dict(pad_left=pad_left, dilation=dilation, replicate=replicate, reflect=reflect, pre_slope=pre_slope, post_act=post_act,
-              post_slope=post_slope)
+              post_slope=post_slope, t_out=t_out, mask=mask)
     if ENGINE != "simt" and cout < 16 and cin >= 256 and cin % 32 == 0 and residual is None and out is None and not accumulate:
         # as _conv1d_fewcout: the weight padded to 16 output channels for the tensor cores
         b16 = torch.nn.functional.pad(bias, (0, 16 - cout)) if bias is not None else None
@@ -424,10 +448,16 @@ def conv1d_stream(x, hist, w, bias=None, *, pad_left, dilation=1, replicate=None
         padc = (cin + 31) // 32 * 32 - cin
         pc = (0, 0, 0, padc)
         return conv1d_stream(torch.nn.functional.pad(x, pc), torch.nn.functional.pad(hist, pc), torch.nn.functional.pad(w, pc),
-                             bias, residual=residual, out_scale=out_scale, out=out, accumulate=accumulate, **kw)
-    t_out = L + pad_left - dilation * (K - 1)
-    if t_out < 0:
+                             bias, residual=residual, out_scale=out_scale, out=out, accumulate=accumulate, res_hist=res_hist,
+                             res_delay=res_delay, **kw)
+    t_full = L + pad_left - dilation * (K - 1)
+    if t_full < 0:
         raise PwgbError("conv1d_stream: input shorter than the receptive field")
+    if t_out is None:
+        t_out = t_full
+    elif not 0 <= t_out <= t_full:
+        raise PwgbError(f"conv1d_stream: t_out {t_out} outside [0, {t_full}]")
+    ext = _stream_ext(B, cout, mask, res_hist, res_delay)
     shape = (B, cout, t_out)
     if out is None:
         if accumulate:
@@ -460,21 +490,30 @@ def conv1d_stream(x, hist, w, bias=None, *, pad_left, dilation=1, replicate=None
     lib = capi.lib()
     if ENGINE != "simt" and lib.pwgb_conv1d_tc_supported(C.byref(d)):
         prof.name = "conv1d_tc_stream"
-        rc = lib.pwgb_conv1d_tc_stream_forward(C.byref(d), _p(x), _p(hist), H, _p(replicate), _p(packed_weight(w)), _p(bias),
-                                               _p(residual), _p(out), _stream())
+        if ext is not None:
+            rc = lib.pwgb_conv1d_tc_stream_ext_forward(C.byref(d), _p(x), _p(hist), H, _p(replicate), _p(packed_weight(w)), _p(bias),
+                                                       _p(residual), C.byref(ext), _p(out), _stream())
+        else:
+            rc = lib.pwgb_conv1d_tc_stream_forward(C.byref(d), _p(x), _p(hist), H, _p(replicate), _p(packed_weight(w)), _p(bias),
+                                                   _p(residual), _p(out), _stream())
         capi.check(rc, "pwgb_conv1d_tc_stream_forward")
     else:
-        rc = lib.pwgb_conv1d_stream_forward(C.byref(d), _p(x), _p(hist), H, _p(replicate), _p(w), _p(bias), _p(residual), _p(out),
-                                            _stream())
+        if ext is not None:
+            rc = lib.pwgb_conv1d_stream_ext_forward(C.byref(d), _p(x), _p(hist), H, _p(replicate), _p(w), _p(bias), _p(residual),
+                                                    C.byref(ext), _p(out), _stream())
+        else:
+            rc = lib.pwgb_conv1d_stream_forward(C.byref(d), _p(x), _p(hist), H, _p(replicate), _p(w), _p(bias), _p(residual),
+                                                _p(out), _stream())
         capi.check(rc, "pwgb_conv1d_stream_forward")
     prof.done()
     return out
 
 
-def conv_transpose1d_stream(x, hist, w, bias=None, *, stride, replicate=None, pre_slope=1.0, out=None):
+def conv_transpose1d_stream(x, hist, w, bias=None, *, stride, replicate=None, pre_slope=1.0, out=None, mask=None):
     """The causal conv-transpose of a stream (pwgb_conv_transpose1d_stream_forward): conv_transpose1d(cat(h, x), w, bias,
     stride=stride, padding=stride, pre_slope=pre_slope) along time with h[b] = x[b, :, :1] where ``replicate`` (B,) int32
-    is set, else hist[b] ((B, cin, 1)); the concatenation is never materialised.  Bit-identical to that call."""
+    is set, else hist[b] ((B, cin, 1)); the concatenation is never materialised.  Bit-identical to that call.  ``mask``
+    as in conv1d_stream (pwgb_conv_transpose1d_stream_ext_forward)."""
     x, w, hist = _dev(x, "x"), _dev(w, "w"), _dev(hist, "hist")
     B, cin, n = x.shape
     if w.shape[0] != cin or tuple(hist.shape) != (B, cin, 1):
@@ -497,8 +536,13 @@ def conv_transpose1d_stream(x, hist, w, bias=None, *, stride, replicate=None, pr
         return y
     prof = _Prof("conv_transpose1d_stream", 2.0 * B * cout * t_out * cin * ((K + stride - 1) // stride), 4.0 * (x.numel() + y.numel()),
                  f"B{B} cin{cin} cout{cout} k{K} s{stride} T{t_out}")
-    rc = lib.pwgb_conv_transpose1d_stream_forward(C.byref(d), _p(x), _p(hist), _p(replicate), _p(w), _p(bias), _p(y), _p(ws),
-                                                  C.c_size_t(nbytes), _stream())
+    if mask is not None:
+        rc = lib.pwgb_conv_transpose1d_stream_ext_forward(C.byref(d), _p(x), _p(hist), _p(replicate), _p(w), _p(bias),
+                                                          C.byref(_stream_ext(B, cout, mask, None, 0)), _p(y), _p(ws),
+                                                          C.c_size_t(nbytes), _stream())
+    else:
+        rc = lib.pwgb_conv_transpose1d_stream_forward(C.byref(d), _p(x), _p(hist), _p(replicate), _p(w), _p(bias), _p(y), _p(ws),
+                                                      C.c_size_t(nbytes), _stream())
     capi.check(rc, "pwgb_conv_transpose1d_stream_forward")
     prof.done()
     return y

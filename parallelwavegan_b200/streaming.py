@@ -1,6 +1,6 @@
-"""Chunked synthesis with the causal generators: mel frames in, waveform out, while the frames are still arriving.
-``CausalPWGStream`` streams a causal Parallel WaveGAN, ``CausalHiFiGANStream`` a causal HiFi-GAN, ``CausalMelGANStream``
-a causal (multi-band) MelGAN.
+"""Chunked synthesis: mel frames in, waveform out, while the frames are still arriving.  ``CausalPWGStream`` streams a
+causal Parallel WaveGAN, ``CausalHiFiGANStream`` a causal HiFi-GAN, ``CausalMelGANStream`` a causal (multi-band) MelGAN,
+and ``HiFiGANLookaheadStream`` a centred HiFi-GAN with a fixed lookahead and a flush.
 
 A causal generator's output for frame j depends only on frames <= j, so it can be synthesised as soon as frame j
 exists.  ``CausalPWGStream`` carries, per batch slot, everything the whole-utterance forward would read from before
@@ -297,71 +297,85 @@ class CausalPWGStream(_ChunkStream):
         return self._run(c.shape[-1], z, c)
 
 
-class CausalHiFiGANStream(_ChunkStream):
-    """Streams a causal ``HiFiGANGenerator`` (``use_causal_conv=True``) chunk by chunk for ``batch`` independent slots.
+class _HiFiGANStream(_ChunkStream):
+    """The level, block and carry tables of a streamed ``HiFiGANGenerator``, shared by the causal stream and the centred
+    one with lookahead.  Both keep, per slot, one history per signal (convs that read the same tensor share a buffer sized
+    by the largest of their histories):
 
-    ``push(c)`` takes the next n >= 1 mel frames of every slot and returns their n * hop samples; n may change from push
-    to push.  For every slot, the concatenated outputs equal ``model.inference(all_frames)``.  There is no lookahead and
-    no flush.  Every conv of the causal generator pads only on the left, so the stream keeps, per slot, the samples in
-    front of the chunk that the whole-utterance forward would read, one history per signal (convs that read the same
-    tensor share a buffer sized by the largest of their histories):
-
-    * the input conv: the last kernel_size - 1 mel frames; it runs as a valid conv on [history | chunk];
-    * each conv-transpose: the last frame of its input, replicated from the first frame for a fresh slot
-      (``ReplicationPad1d``, pwgb_conv_transpose1d_stream_forward with the per-slot replicate flags);
-    * each level's input, read by the first dilated conv of every block: max_j (k_j - 1) * d_j0 samples;
+    * the input conv: the last kernel_size - 1 mel frames; it runs on [history | chunk];
+    * each conv-transpose: the last frame of its input;
+    * each level's input, read by the first dilated conv of every block: max_j (delta_j + (k_j - 1) * d_j0) samples;
     * each ResBlock's later dilated-conv inputs ((k - 1) * d) and second-conv inputs (k - 1);
     * the output conv: its last kernel_size - 1 input samples.
 
     The convs read their histories in their loaders (pwgb_conv1d_stream_forward / pwgb_conv1d_tc_stream_forward), so no
     [history | chunk] concatenation is made at the waveform rate.  After a ResBlock's last conv one pwgb_stream_carry
     launch updates every history it read; the intermediate signals of each chunk length live in buffers allocated once,
-    so the carry tables are built once too.  With ``use_graphs`` each chunk length is captured once into a CUDA graph
-    and replayed.  The weights are read when the stream is built and must not change while it is used."""
+    so the carry tables are built once too.
 
-    def __init__(self, model, batch=1, use_graphs=True):
-        from .models import HiFiGANGenerator
+    A centred conv over [history | chunk] is the causal conv of the stream with its output labelled pad samples earlier,
+    so the centred stream runs every signal in "delayed time", ``look`` samples (at the signal's rate) behind the frames
+    pushed.  The causal stream is the case where every lookahead and every delay is zero: ``look*`` 0, ``delta`` 0 and
+    ``rdelay`` 0 for every conv, and no mask."""
 
-        if not isinstance(model, HiFiGANGenerator):
-            raise PwgbError("CausalHiFiGANStream: expected a HiFiGANGenerator")
-        if not model.use_causal_conv:
-            raise PwgbError("CausalHiFiGANStream: the model is not causal (use_causal_conv=False); a centred model needs lookahead")
-        ic = model.input_conv
-        # the fresh slots' flags are the conv-transposes' replicate flags
-        self._setup(model, batch, use_graphs, ic.conv.in_channels, ic.left, "zero", flags=True)
+    def _build(self, model, centred):
         B, zeros = self.B, self._zeros
         m = model
         self.slope, self.nb = m.slope, m.num_blocks
-        self.w_in = wb(ic.conv)
+        ic = m.input_conv if centred else m.input_conv.conv
+        self.w_in = wb(ic)
+        look = (ic.kernel_size[0] - 1) // 2 if centred else 0  # lookahead of the current signal, in its samples
+        self.look_in = look
         self.hop = 1
         self.levels = []
         for i in range(m.num_upsamples):
             up = m.upsamples[i][1]
-            cin, cout = up.deconv.in_channels, up.deconv.out_channels
-            self.hop *= up.stride
+            deconv = up if centred else up.deconv
+            cin, cout = deconv.in_channels, deconv.out_channels
+            s = deconv.stride[0]
+            self.hop *= s
+            # the window of cat(h, x) is the centred layer's samples from a * s - padding on
+            look = look * s + deconv.padding[0] if centred else 0
+            look_u = look
             blocks = []
             for j in range(self.nb):
                 blk = m.blocks[i * self.nb + j]
                 k, dils = blk.kernel_size, blk.dilations
                 convs = []
                 for idx, d in enumerate(dils):
-                    c1 = blk.convs1[idx][1].conv
-                    c2 = blk.convs2[idx][1].conv if blk.use_additional_convs else None
-                    convs.append(dict(d=d, w1=wb(c1), w2=wb(c2) if c2 is not None else None,
+                    c1 = blk.convs1[idx][1] if centred else blk.convs1[idx][1].conv
+                    c2 = (blk.convs2[idx][1] if centred else blk.convs2[idx][1].conv) if blk.use_additional_convs else None
+                    p1 = (k - 1) * d // 2 if centred else 0
+                    q = p1 + ((k - 1) // 2 if c2 is not None and centred else 0)  # the branch's lag behind its input
+                    convs.append(dict(d=d, w1=wb(c1), w2=wb(c2) if c2 is not None else None, p1=p1, q=q,
                                       # the input of the dilated conv (idx 0: the level input, shared) and of the second conv
                                       x_hist=zeros(B, cout, (k - 1) * d) if idx > 0 else None,
                                       xt_hist=zeros(B, cout, k - 1) if c2 is not None else None))
-                blocks.append(dict(k=k, convs=convs))
-            hl = max((b["k"] - 1) * b["convs"][0]["d"] for b in blocks)
-            self.levels.append(dict(stride=up.stride, channels=cout, w=wb(up.deconv), up_hist=zeros(B, cin, 1),
-                                    lvl_hist=zeros(B, cout, hl), blocks=blocks))
-        oc = m.output_conv[1]
-        self.w_out = wb(oc.conv)
-        self.out_hist = zeros(B, oc.conv.in_channels, oc.left)
-        self.out_channels = oc.conv.out_channels
+                blocks.append(dict(k=k, convs=convs, lag=sum(cv["q"] for cv in convs)))
+            # block j reads the level input delta_j samples later, so that every block ends at the same lookahead
+            lag = max(b["lag"] for b in blocks)
+            for b in blocks:
+                b["delta"] = lag - b["lag"]
+                cur = look_u + b["delta"]
+                for idx, cv in enumerate(b["convs"]):
+                    # mask lookaheads of the dilated conv's output and of the block step's output; the residual is the
+                    # step's input, q (and, for the level input, delta_j) rows back
+                    cv["look1"], cv["look2"] = cur + cv["p1"], cur + cv["q"]
+                    cv["rdelay"] = cv["q"] + (b["delta"] if idx == 0 else 0)
+                    cur += cv["q"]
+            look = look_u + lag
+            hl = max(b["delta"] + (b["k"] - 1) * b["convs"][0]["d"] for b in blocks)
+            self.levels.append(dict(stride=s, channels=cout, w=wb(deconv), up_hist=zeros(B, cin, 1), lvl_hist=zeros(B, cout, hl),
+                                    blocks=blocks, rate=self.hop, look_u=look_u))
+        oc = m.output_conv[1] if centred else m.output_conv[1].conv
+        self.w_out = wb(oc)
+        K_out = oc.kernel_size[0]
+        self.out_hist = zeros(B, oc.in_channels, K_out - 1)
+        self.out_channels = oc.out_channels
+        self.delay = look + (K_out - 1) // 2 if centred else 0
 
     # ---------------------------------------------------------------------------------------------------- state
-    def _state(self):
+    def _histories(self):
         hs = [self.cin_hist, self.out_hist]
         for lv in self.levels:
             hs += [lv["up_hist"], lv["lvl_hist"]]
@@ -400,14 +414,18 @@ class CausalHiFiGANStream(_ChunkStream):
         ent["out_table"] = ops.stream_carry_table([(prev, self.out_hist)], dev)
         return ent
 
-    def _step(self, c):
-        """One chunk: c (B, in_channels, n) -> (B, out_channels, n * hop).  Advances the state."""
-        ent = self._entry(c.shape[-1])
-        h = ops.conv1d(self._input(ent, c), *self.w_in, out=ent["h0"])
+    def _mask(self, rate, look):
+        """the stream_ext mask of a signal with ``rate`` samples per frame and lookahead ``look`` (None: causal)"""
+        return None
+
+    def _levels(self, h, ent, replicate):
+        """the conv-transposes and the MRF blocks of one chunk, from the input conv's output h"""
         slope = self.slope
         for lv, buf in zip(self.levels, ent["levels"]):
-            u = ops.conv_transpose1d_stream(h, lv["up_hist"], lv["w"][0], lv["w"][1], stride=lv["stride"], replicate=self.fresh,
-                                            pre_slope=slope, out=buf["u"])
+            rate = lv["rate"]
+            u = ops.conv_transpose1d_stream(h, lv["up_hist"], lv["w"][0], lv["w"][1], stride=lv["stride"], replicate=replicate,
+                                            pre_slope=slope, out=buf["u"], mask=self._mask(rate, lv["look_u"]))
+            t = u.shape[-1]
             cs = buf["cs"]
             for j, blk in enumerate(lv["blocks"]):
                 k, convs = blk["k"], blk["convs"]
@@ -417,16 +435,59 @@ class CausalHiFiGANStream(_ChunkStream):
                     last = idx == len(convs) - 1
                     tail = dict(out=cs, accumulate=j > 0, out_scale=1.0 / self.nb) if last else dict(out=buf["x"][idx])
                     hx = lv["lvl_hist"] if idx == 0 else cv["x_hist"]
+                    # block j's first conv reads the level input delta_j rows early: rows [-(P + delta_j), t - delta_j)
+                    P = (k - 1) * d + (blk["delta"] if idx == 0 else 0)
+                    res = dict(residual=x, res_hist=hx if cv["rdelay"] else None, res_delay=cv["rdelay"])
                     if cv["w2"] is not None:
-                        xt = ops.conv1d_stream(x, hx, *cv["w1"], pad_left=(k - 1) * d, dilation=d, pre_slope=slope, out=buf["xt"][idx])
-                        x = ops.conv1d_stream(xt, cv["xt_hist"], *cv["w2"], pad_left=k - 1, pre_slope=slope, residual=x, **tail)
+                        xt = ops.conv1d_stream(x, hx, *cv["w1"], pad_left=P, dilation=d, pre_slope=slope, out=buf["xt"][idx], t_out=t,
+                                               mask=self._mask(rate, cv["look1"]))
+                        x = ops.conv1d_stream(xt, cv["xt_hist"], *cv["w2"], pad_left=k - 1, pre_slope=slope,
+                                              mask=self._mask(rate, cv["look2"]), **res, **tail)
                     else:
-                        x = ops.conv1d_stream(x, hx, *cv["w1"], pad_left=(k - 1) * d, dilation=d, pre_slope=slope, residual=x, **tail)
+                        x = ops.conv1d_stream(x, hx, *cv["w1"], pad_left=P, dilation=d, pre_slope=slope, t_out=t,
+                                              mask=self._mask(rate, cv["look2"]), **res, **tail)
                 ops.stream_carry(buf["tables"][j])
             h = cs
+        return h
+
+    def _output(self, h, ent):
         y = ops.conv1d_stream(h, self.out_hist, *self.w_out, pad_left=self.out_hist.shape[-1], pre_slope=0.01, post_act="tanh",
-                              out=ent["y"])
+                              out=ent["y"], mask=self._mask(self.hop, self.delay))
         ops.stream_carry(ent["out_table"])
+        return y
+
+
+class CausalHiFiGANStream(_HiFiGANStream):
+    """Streams a causal ``HiFiGANGenerator`` (``use_causal_conv=True``) chunk by chunk for ``batch`` independent slots.
+
+    ``push(c)`` takes the next n >= 1 mel frames of every slot and returns their n * hop samples; n may change from push
+    to push.  For every slot, the concatenated outputs equal ``model.inference(all_frames)``.  There is no lookahead and
+    no flush.  Every conv of the causal generator pads only on the left, so the histories of ``_HiFiGANStream`` hold
+    exactly what the whole-utterance forward reads in front of the chunk: zeros for a fresh slot, except that each
+    conv-transpose's history replicates its first frame (``ReplicationPad1d``, pwgb_conv_transpose1d_stream_forward with
+    the per-slot replicate flags).  With ``use_graphs`` each chunk length is captured once into a CUDA graph and replayed.
+    The weights are read when the stream is built and must not change while it is used."""
+
+    def __init__(self, model, batch=1, use_graphs=True):
+        from .models import HiFiGANGenerator
+
+        if not isinstance(model, HiFiGANGenerator):
+            raise PwgbError("CausalHiFiGANStream: expected a HiFiGANGenerator")
+        if not model.use_causal_conv:
+            raise PwgbError("CausalHiFiGANStream: the model is not causal (use_causal_conv=False); a centred model needs lookahead")
+        ic = model.input_conv
+        # the fresh slots' flags are the conv-transposes' replicate flags
+        self._setup(model, batch, use_graphs, ic.conv.in_channels, ic.left, "zero", flags=True)
+        self._build(model, centred=False)
+
+    def _state(self):
+        return self._histories()
+
+    def _step(self, c):
+        """One chunk: c (B, in_channels, n) -> (B, out_channels, n * hop).  Advances the state."""
+        ent = self._entry(c.shape[-1])
+        h = ops.conv1d(self._input(ent, c), *self.w_in, out=ent["h0"])
+        y = self._output(self._levels(h, ent, self.fresh), ent)
         self.fresh.zero_()
         return y
 
@@ -437,6 +498,96 @@ class CausalHiFiGANStream(_ChunkStream):
         c = self._frames(c, normalize_before)
         self._start(c)
         return self._run(c.shape[-1], c)
+
+
+class HiFiGANLookaheadStream(_HiFiGANStream):
+    """Streams a centred ``HiFiGANGenerator`` (``use_causal_conv=False``, the published checkpoints) chunk by chunk for
+    ``batch`` independent slots, with a fixed lookahead of ``delay`` output samples.
+
+    ``push(c)`` takes the next n >= 1 mel frames of every slot and returns n * hop samples: the whole-utterance samples
+    from t0 * hop - delay on (t0: the frames pushed before), with zeros before sample 0.  ``flush(items)`` returns the
+    last ``delay`` samples of those slots and restarts them; the other slots continue as if no flush had happened.  For
+    every slot, the concatenated pushes and flush equal ``[zeros(delay) | model.inference(all_frames)]``.
+
+    ``delay`` is the sum of the centred paddings along the generator (DESIGN.md §3.8), derived from the module: 3258
+    samples (12.7 frames) for HiFi-GAN v1.  Each signal runs in delayed time behind the frames pushed; every conv is the
+    causal stream's history conv on [history | chunk], and:
+
+    * every launch masks the samples outside its signal to +0.0 (pwgb_stream_ext: a device frame counter per slot,
+      advanced inside the captured push, and an end frame set by the flush), which is the zero padding the
+      whole-utterance forward reads there;
+    * a ResBlock step x + branch(x) adds its input q samples back (q: the branch's lag), read from the step's history;
+    * block j of a level reads the level input delta_j samples later, so that every block ends at the same lookahead and
+      the MRF sum accumulates as in ``inference``;
+    * the conv-transposes' one-frame histories are zero for a fresh slot (no replication);
+    * the flush pushes ceil(delay / hop) zero frames with the slots' end frames set: the mask gives every layer its right
+      zero padding, so it is one more push through a cached entry.
+
+    With ``use_graphs`` each chunk length is captured once into a CUDA graph and replayed.  The weights are read when the
+    stream is built and must not change while it is used."""
+
+    OPEN = 2 ** 31 - 1  # the end frame of a slot whose signal has not ended
+
+    def __init__(self, model, batch=1, use_graphs=True):
+        from .models import HiFiGANGenerator
+
+        if not isinstance(model, HiFiGANGenerator):
+            raise PwgbError("HiFiGANLookaheadStream: expected a HiFiGANGenerator")
+        if model.use_causal_conv:
+            raise PwgbError("HiFiGANLookaheadStream: the model is causal (use_causal_conv=True); stream it with CausalHiFiGANStream, "
+                            "which has no lookahead")
+        ic = model.input_conv
+        self._setup(model, batch, use_graphs, ic.in_channels, ic.kernel_size[0] - 1, "zero")
+        self._build(model, centred=True)
+        self.frame = torch.zeros(self.B, device=self.dev, dtype=torch.int32)
+        self.end = torch.full((self.B,), self.OPEN, device=self.dev, dtype=torch.int32)
+        self._nohist = self._zeros(self.B, ic.in_channels, 0)
+
+    def _state(self):
+        return self._histories() + [self.frame, self.end]
+
+    def reset(self, items=None):
+        super().reset(items)
+        for b in self._slots(items):
+            self.end[b] = self.OPEN
+
+    def _mask(self, rate, look):
+        return (self.frame, self.end, rate, look)
+
+    def _step(self, c):
+        """One chunk: c (B, in_channels, n) -> (B, out_channels, n * hop).  Advances the state."""
+        ent = self._entry(c.shape[-1])
+        # the centred input conv on [history | chunk]: frames t0 - 3 .. t0 + n - 4 for kernel 7
+        h = ops.conv1d_stream(self._input(ent, c), self._nohist, *self.w_in, pad_left=0, out=ent["h0"], mask=self._mask(1, self.look_in))
+        y = self._output(self._levels(h, ent, None), ent)
+        self.frame += c.shape[-1]
+        return y
+
+    @torch.no_grad()
+    def push(self, c, normalize_before=False):
+        """c: (B, n, in_channels) mel frames ((n, in_channels) when batch == 1).  Returns (B, out_channels, n * hop) on the
+        device: samples [t0 * hop - delay, (t0 + n) * hop - delay) of each slot's utterance."""
+        c = self._frames(c, normalize_before)
+        self._start(c)
+        return self._run(c.shape[-1], c)
+
+    @torch.no_grad()
+    def flush(self, items=None):
+        """The last ``delay`` samples of slots ``items`` (an index, an iterable of indices or None for every slot), computed
+        against the zero right padding, as (len(items), out_channels, delay); the slots are then reset.  The other slots'
+        state is restored around the flush push, so they continue exactly as if it had not happened.  The flush push covers
+        every slot, so ending one slot costs a ceil(delay / hop)-frame batch push (DESIGN.md §3.8)."""
+        items = list(self._slots(items))
+        keep = [b for b in range(self.B) if b not in items]
+        snap = [t[keep].clone() for t in self._state()] if keep else []
+        sel = torch.tensor(items, device=self.dev, dtype=torch.long)
+        self.end[sel] = self.frame[sel]
+        n = -(-self.delay // self.hop)
+        y = self._run(n, self._zeros(self.B, self.in_channels, n))[sel, :, :self.delay].contiguous()
+        for t, s in zip(self._state(), snap):
+            t[keep] = s
+        self.reset(items)
+        return y
 
 
 class CausalMelGANStream(_ChunkStream):

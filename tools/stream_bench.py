@@ -3,17 +3,19 @@ for batch sizes B, chunks of 1, 4, 16 and 64 frames, CUDA graphs off and on.  MO
 
 * pwg: the causal PWG v1 generator (CausalPWGStream), hop 256;
 * hifigan: the causal HiFi-GAN v1 generator (CausalHiFiGANStream), hop 256;
+* hifigan_centred: the centred HiFi-GAN v1 generator (HiFiGANLookaheadStream), hop 256, with its 3258-sample lookahead;
 * melgan_v1: the causal MelGAN v1 (512 channels, scales [8, 8, 2, 2], 3 stacks; CausalMelGANStream);
 * mb_melgan_v2: the causal multi-band MelGAN v2 (384 channels, scales [8, 4, 2], 4 stacks, 4-band PQMF), 256 output
   samples per frame like the others.
 
-PWG and HiFi-GAN stream a 256-frame utterance (65536 samples per item); the MelGANs stream a 263-frame one, a 7-frame
-opening push (their min_first_frames) then 256 frames, and flush.  Each configuration streams its utterance PASSES
+PWG and HiFi-GAN stream a 256-frame utterance (65536 samples per item), the centred HiFi-GAN then flushes; the MelGANs
+stream a 263-frame one, a 7-frame opening push (their min_first_frames) then 256 frames, and flush.  Each configuration streams its utterance PASSES
 times.  A push is timed with CUDA events recorded around it and a synchronise after it, so a latency includes the
 host's launch work whenever the GPU waits for it.  Reported: median / min / max latency of the chunk pushes, the
-streamed real-time factor (GPU time of all pushes, and the flush, over the audio's duration at 22050 Hz: below 1 is
+streamed real-time factor (GPU time of all pushes, and the flush, whose own latency is reported too, over the audio's duration at 22050 Hz: below 1 is
 faster than real time), the libpwgb kernel launches of one steady-state eager push (the few torch copies are not
-counted), and the whole-utterance forward of the same audio (one call on the B utterances; for MB-MelGAN with the PQMF
+counted), the stream's state_bytes() and algorithmic latency (delay plus one chunk, in ms at 22050 Hz), and the
+whole-utterance forward of the same audio (one call on the B utterances; for MB-MelGAN with the PQMF
 synthesis) for comparison.
 
 Every timed stream is checked against ``model.inference`` of each item in the same run:
@@ -21,7 +23,7 @@ Every timed stream is checked against ``model.inference`` of each item in the sa
 * pwg: bit for bit while a push has at most 65536 samples in all (B x chunk x 256), so that its 64 -> 1 output conv
   takes conv1d_small_cout_kernel as the per-item inference does; above that the push's output conv takes
   conv1d_fewcout_long_kernel, which sums in another order, and the check is rel-L2 <= 1e-6;
-* hifigan: the per-item inference's 32 -> 1 output conv has 65536 output samples and takes conv1d_fewcout_long_kernel,
+* hifigan, hifigan_centred (after its delay): the per-item inference's 32 -> 1 output conv has 65536 output samples and takes conv1d_fewcout_long_kernel,
   which sums in another order than the generic kernel every stream conv takes, so the check is rel-L2 <= 1e-6 (bit
   identity holds up to 15 frames, tests/test_gpu_hifigan_stream.py);
 * melgan_v1, mb_melgan_v2: after the PQMF delay, the per-item inference's output conv has 67328 output samples and
@@ -45,7 +47,7 @@ import torch.nn.functional as F  # noqa: E402
 from parallelwavegan_b200 import capi, models  # noqa: E402
 from parallelwavegan_b200 import synth_weights as synth  # noqa: E402
 from parallelwavegan_b200.layers import PQMF  # noqa: E402
-from parallelwavegan_b200.streaming import CausalHiFiGANStream, CausalMelGANStream, CausalPWGStream  # noqa: E402
+from parallelwavegan_b200.streaming import CausalHiFiGANStream, CausalMelGANStream, CausalPWGStream, HiFiGANLookaheadStream  # noqa: E402
 
 MELGAN = {
     "melgan_v1": dict(in_channels=80, out_channels=1, kernel_size=7, channels=512, upsample_scales=[8, 8, 2, 2], stacks=3,
@@ -53,7 +55,7 @@ MELGAN = {
     "mb_melgan_v2": dict(in_channels=80, out_channels=4, kernel_size=7, channels=384, upsample_scales=[8, 4, 2], stacks=4,
                          use_causal_conv=True),
 }
-MODELS = ("pwg", "hifigan", *MELGAN)
+MODELS = ("pwg", "hifigan", "hifigan_centred", *MELGAN)
 FRAMES = 256
 CHUNKS = (1, 4, 16, 64)
 PASSES = 2
@@ -84,6 +86,8 @@ def build(name, dev):
         m, scale = models.ParallelWaveGANGenerator(use_causal_conv=True), 1.0
     elif name == "hifigan":
         m, scale = models.HiFiGANGenerator(use_causal_conv=True), 1.15
+    elif name == "hifigan_centred":
+        m, scale = models.HiFiGANGenerator(use_causal_conv=False), 1.15
     else:
         m, scale = models.MelGANGenerator(**MELGAN[name]), 1.0
     m.load_state_dict(synth.synth_state_dict([(k, tuple(v.shape)) for k, v in m.state_dict().items()], 31, scale))
@@ -100,6 +104,7 @@ class Workload:
     def __init__(self, name, m, B, dev):
         self.name, self.m = name, m
         self.melgan = name in MELGAN
+        self.flushes = self.melgan or name == "hifigan_centred"
         self.open = 7 if self.melgan else 0
         self.frames = self.open + FRAMES
         g = torch.Generator().manual_seed(B)
@@ -117,6 +122,10 @@ class Workload:
         elif name == "hifigan":
             self.ref = torch.stack([m.inference(c[b]).t() for b in range(B)])
             self.whole = lambda: m(cw)
+        elif name == "hifigan_centred":
+            self.delay = HiFiGANLookaheadStream(m, batch=B, use_graphs=False).delay
+            self.ref = F.pad(torch.stack([m.inference(c[b]).t() for b in range(B)]), (self.delay, 0))
+            self.whole = lambda: m(cw)
         else:
             probe = CausalMelGANStream(m, batch=B, use_graphs=False)
             assert probe.min_first_frames == self.open, probe.min_first_frames
@@ -126,7 +135,8 @@ class Workload:
         self.samples = self.ref.shape[-1] - self.delay
 
     def stream(self, B, graphs):
-        cls = {"pwg": CausalPWGStream, "hifigan": CausalHiFiGANStream}.get(self.name, CausalMelGANStream)
+        cls = {"pwg": CausalPWGStream, "hifigan": CausalHiFiGANStream, "hifigan_centred": HiFiGANLookaheadStream}.get(self.name,
+                                                                                                                 CausalMelGANStream)
         return cls(self.m, batch=B, use_graphs=graphs)
 
     def push(self, st, j, n):
@@ -161,7 +171,8 @@ def bench_model(name, Bs, dev):
                 capi.reset_launch_count()
                 w.push(st, w.open + n, n)
                 launches = capi.launch_count()  # a steady-state push (0 with graphs: the replay launches nothing)
-                lat, total = [], 0.0
+                row["state_bytes_per_slot"] = st.state_bytes()
+                lat, flushes, total = [], [], 0.0
                 for _ in range(PASSES):
                     st.reset()
                     ys = []
@@ -174,13 +185,17 @@ def bench_model(name, Bs, dev):
                         lat.append(t)
                         total += t
                         ys.append(y)
-                    if w.melgan:
+                    if w.flushes:
                         y, t = timed(st.flush)
+                        flushes.append(t)
                         total += t
                         ys.append(y)
                 y = torch.cat(ys, -1)
                 s = stats(lat)
                 s["rtf"] = total / PASSES / 1e3 / audio_s
+                s["algorithmic_latency_ms"] = (w.delay + n * 256) / SR * 1e3
+                if flushes:
+                    s["flush_ms"] = sorted(flushes)[len(flushes) // 2]  # every slot at once; the upper median of the passes
                 if not graphs:
                     s["libpwgb_launches_per_push"] = launches
                 s["bit_identical_to_inference"] = torch.equal(y, w.ref)
