@@ -248,6 +248,9 @@ PWGB_API int pwgb_conv_transpose1d_stream_ext_forward(const pwgb_convtr1d_desc* 
                                                       const int* replicate, const float* w, const float* bias,
                                                       const pwgb_stream_ext* ext, float* y, void* ws, size_t ws_bytes,
                                                       void* stream);
+/* y (batch, rows, t) fp32 in place: every sample outside the signal of ext's mask (rows of item b: frame[b], end[b],
+ * rate, lookahead as above) is set to +0.0.  ext must hold a mask; its residual fields are ignored. */
+PWGB_API int pwgb_stream_mask(float* y, int batch, int rows, int t, const pwgb_stream_ext* ext, void* stream);
 
 /* ------------------------------------------------------------------------
  * One HiFi-GAN ResBlock conv pair (layers/residual_block.py:243-258, non-causal, additional convs) in one
@@ -398,7 +401,7 @@ PWGB_API int pwgb_wnstack_layer_forward(const pwgb_wnstack_desc* d, int dilation
 /* Streaming a causal stack chunk by chunk.  A causal layer reads only the (kernel-1)*dilation rows in front of sample 0,
  * so those rows of its input buffer may hold the previous chunk's last samples instead of zeros: the unchanged layer
  * then computes the chunk exactly as the whole-signal forward would.  Relaxed contract for such streaming buffers
- * (causal only): the left halo rows may hold history; the right halo and every row past t stay zero.  Buffers that
+ * (causal, or a centred stack streamed with lookahead, below): the left halo rows may hold history; the right halo and every row past t stay zero.  Buffers that
  * are not streamed keep the contract above.
  * A layer's history h = (kernel-1)*dilation is a state tensor laid out like the stream, [batch][hi|lo][R/8][h][8] bf16
  * (batch * 2 * residual_channels * h * 2 bytes), all zero for a fresh signal (the whole-signal zero padding).
@@ -410,6 +413,28 @@ PWGB_API int pwgb_wnstack_layer_forward(const pwgb_wnstack_desc* d, int dilation
  * layer).  h_save, h_load <= halo.  A plain copy: deterministic. */
 PWGB_API int pwgb_wnstack_carry(const pwgb_wnstack_desc* d, const void* xpk_save, void* hist_save, int h_save, void* xpk_load,
                        const void* hist_load, int h_load, void* stream);
+/* Streaming a centred stack with a fixed lookahead (desc.causal = 0, halo >= (kernel-1) * largest dilation).  In delayed
+ * time (see pwgb_stream_ext) a centred layer over [history | chunk] is the causal tap pattern with its output labelled
+ * (kernel-1)/2 * dilation rows earlier; its input buffer's left halo holds the (kernel-1) * dilation history rows, carried
+ * with pwgb_wnstack_carry exactly as for a causal stack.  pwgb_wnstack_layer_stream_ext_forward is
+ * pwgb_wnstack_layer_forward with:
+ *   - taps t - (kernel-1-j) * dilation, and the residual of output row t read at input row t - (kernel-1)/2 * dilation
+ *     (from the halo or the chunk);
+ *   - the conditioning of output row t read at row c_row0 + t of cpk, laid out as pwgb_wnstack_pack_c writes it with
+ *     c_rows rows per plane ([batch][hi|lo][ceil(aux/8)][c_rows][8] bf16, c_rows >= c_row0 + t);
+ *   - the skip of output row t at skips[(b * skip_channels + ch) * skip_row_stride + skip_col0 + t];
+ *   - x' rows outside the signal of ext's mask (rate = samples per frame, lookahead = the output's) stored as zero, the
+ *     next layer's zero padding.  ext must be a mask without residual fields.
+ * Every value is the same fp32 expression as in pwgb_wnstack_layer_forward of the centred stack, so a chunked run equals
+ * the whole signal bit for bit.  pwgb_wnstack_first_conv_stream_ext is pwgb_wnstack_first_conv on z rows z_row_stride
+ * floats apart (z_row_stride >= t), with the rows outside ext's mask stored as zero. */
+PWGB_API int pwgb_wnstack_first_conv_stream_ext(const pwgb_wnstack_desc* d, const float* z, long long z_row_stride, int in_channels,
+                                                const float* w, const float* bias, const pwgb_stream_ext* ext, void* xpk, void* stream);
+PWGB_API int pwgb_wnstack_layer_stream_ext_forward(const pwgb_wnstack_desc* d, int dilation, const void* xpk_in, const void* cpk,
+                                                   int c_rows, int c_row0, const void* packed_w, const float* b_conv,
+                                                   const float* b_skip_out, void* xpk_out, float* skips, int skip_col0,
+                                                   long long skip_row_stride, int skips_init, const pwgb_stream_ext* ext,
+                                                   void* stream);
 
 /* ------------------------------------------------------------------------
  * One stage of the PWG conditioning upsampler (layers/upsample.py:112-128): nearest repeat
@@ -432,6 +457,14 @@ PWGB_API int pwgb_upsample_fir_causal_forward(int rows, int rows_per_batch, int 
 PWGB_API int pwgb_upsample_fir_causal_stream_forward(int rows, int rows_per_batch, int t_in, int scale, const float* x,
                                             const float* fir, float* y, long long y_batch_stride, const float* hist_in,
                                             void* stream);
+/* The centred stage of a lookahead stream: on [2 history frames | chunk] output frame j reads input frames j-2, j-1, j,
+ * i.e. it is the centred stage's output frame j-1 (lookahead <- scale * lookahead + scale).  hist_in as in
+ * pwgb_upsample_fir_causal_stream_forward; every output is the same fp32 expression as in pwgb_upsample_fir_forward, and
+ * the outputs outside the signal of ext's mask (rate: output samples per input frame of the whole upsampler so far)
+ * are stored as +0.0.  ext must be a mask without residual fields. */
+PWGB_API int pwgb_upsample_fir_stream_ext_forward(int rows, int rows_per_batch, int t_in, int scale, const float* x, const float* fir,
+                                                  float* y, long long y_batch_stride, const float* hist_in, const pwgb_stream_ext* ext,
+                                                  void* stream);
 PWGB_API int pwgb_upsample_fir_causal_backward(int rows, int rows_per_batch, int t_in, int scale, const float* x, const float* fir,
                                       const float* gy, long long gy_batch_stride, float* gx, float* dfir, void* stream);
 

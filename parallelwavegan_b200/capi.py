@@ -131,6 +131,8 @@ def lib():
     L.pwgb_conv_transpose1d_stream_ext_forward.restype = C.c_int
     L.pwgb_conv_transpose1d_stream_ext_forward.argtypes = [C.POINTER(ConvTr1dDesc), vp, vp, vp, vp, vp, C.POINTER(StreamExt), vp, vp,
                                                            C.c_size_t, vp]
+    L.pwgb_stream_mask.restype = C.c_int
+    L.pwgb_stream_mask.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.POINTER(StreamExt), vp]
     L.pwgb_debug_set.restype = None
     L.pwgb_debug_set.argtypes = [C.c_int, C.c_int]
     L.pwgb_debug_get.restype = C.c_int
@@ -164,6 +166,11 @@ def lib():
     L.pwgb_wnstack_first_conv.argtypes = [C.POINTER(WnStackDesc), vp, C.c_int, vp, vp, vp, vp]
     L.pwgb_wnstack_layer_forward.restype = C.c_int
     L.pwgb_wnstack_layer_forward.argtypes = [C.POINTER(WnStackDesc), C.c_int, vp, vp, vp, vp, vp, vp, vp, C.c_int, vp]
+    L.pwgb_wnstack_first_conv_stream_ext.restype = C.c_int
+    L.pwgb_wnstack_first_conv_stream_ext.argtypes = [C.POINTER(WnStackDesc), vp, C.c_longlong, C.c_int, vp, vp, C.POINTER(StreamExt), vp, vp]
+    L.pwgb_wnstack_layer_stream_ext_forward.restype = C.c_int
+    L.pwgb_wnstack_layer_stream_ext_forward.argtypes = [C.POINTER(WnStackDesc), C.c_int, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp,
+                                                        C.c_int, C.c_longlong, C.c_int, C.POINTER(StreamExt), vp]
     L.pwgb_wnstack_carry.restype = C.c_int
     L.pwgb_wnstack_carry.argtypes = [C.POINTER(WnStackDesc), vp, vp, C.c_int, vp, vp, C.c_int, vp]
     L.pwgb_collate_crop.restype = C.c_int
@@ -184,6 +191,9 @@ def lib():
         fn.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_longlong, vp]
     L.pwgb_upsample_fir_causal_stream_forward.restype = C.c_int
     L.pwgb_upsample_fir_causal_stream_forward.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_longlong, vp, vp]
+    L.pwgb_upsample_fir_stream_ext_forward.restype = C.c_int
+    L.pwgb_upsample_fir_stream_ext_forward.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_longlong, vp,
+                                                       C.POINTER(StreamExt), vp]
     L.pwgb_mr_stft_loss_workspace.restype = C.c_size_t
     L.pwgb_mr_stft_loss_workspace.argtypes = [C.POINTER(StftDesc), C.c_int]
     L.pwgb_mr_stft_loss_forward.restype = C.c_int
@@ -314,7 +324,8 @@ EXPORTED_SYMBOLS = [
     "pwgb_s2d_forward", "pwgb_s2d_backward", "pwgb_mt_clip_coef", "pwgb_mt_adam_step", "pwgb_prep_features", "pwgb_pcm16_forward", "pwgb_collate_crop",
     "pwgb_wnstack_supported", "pwgb_wnstack_x_bytes", "pwgb_wnstack_c_bytes", "pwgb_wnstack_pack_x", "pwgb_wnstack_unpack_x",
     "pwgb_wnstack_pack_c", "pwgb_wnstack_first_conv", "pwgb_wnstack_layer_forward", "pwgb_wnstack_carry",
-    "pwgb_upsample_fir_causal_stream_forward",
+    "pwgb_upsample_fir_causal_stream_forward", "pwgb_upsample_fir_stream_ext_forward", "pwgb_stream_mask",
+    "pwgb_wnstack_first_conv_stream_ext", "pwgb_wnstack_layer_stream_ext_forward",
     "pwgb_mr_stft_loss_workspace", "pwgb_mr_stft_loss_forward", "pwgb_stft_amplitude_forward",
     "pwgb_mel_project_forward", "pwgb_reduce_mean_forward", "pwgb_avg_pool1d_forward",
     "pwgb_conv1d_wgrad_workspace", "pwgb_conv1d_wgrad", "pwgb_conv1d_wgrad_tc_supported",

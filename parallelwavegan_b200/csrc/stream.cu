@@ -72,9 +72,28 @@ __global__ void __launch_bounds__(256) stream_carry_kernel(const long long* __re
   }
 }
 
+// y (batch, rows, t) in place: samples outside the signal of the pwgb_stream_ext mask become +0.0
+__global__ void stream_mask_kernel(float* __restrict__ y, int rows, int t, const int* __restrict__ frame, const int* __restrict__ end,
+                                   int rate, int look) {
+  const int b = blockIdx.z;
+  float* yr = y + ((long long)b * rows + blockIdx.y) * t;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < t; i += gridDim.x * blockDim.x)
+    if (stream_outside(frame, end, rate, look, b, i)) yr[i] = 0.f;
+}
+
 }  // namespace pwgb
 
 using namespace pwgb;
+
+extern "C" int pwgb_stream_mask(float* y, int batch, int rows, int t, const pwgb_stream_ext* ext, void* stream) {
+  PWGB_CHECK_ARG(ext && ext->frame && ext->end && ext->rate >= 1 && ext->lookahead >= 0, "stream_mask: ext must hold a mask");
+  PWGB_CHECK_ARG(batch >= 0 && batch <= 65535 && rows >= 0 && rows <= 65535 && t >= 0, "stream_mask: bad sizes");
+  if (batch == 0 || rows == 0 || t == 0) return PWGB_OK;
+  PWGB_CHECK_ARG(y, "stream_mask: null argument");
+  stream_mask_kernel<<<dim3((unsigned)(ceil_div(t, 256) < 64 ? ceil_div(t, 256) : 64), (unsigned)rows, (unsigned)batch), 256, 0,
+                       (cudaStream_t)stream>>>(y, rows, t, ext->frame, ext->end, ext->rate, ext->lookahead);
+  return check_launch("stream_mask_kernel");
+}
 
 extern "C" int pwgb_conv1d_stream_forward(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len,
                                           const int* replicate, const float* w, const float* bias, const float* residual,

@@ -15,10 +15,13 @@ namespace pwgb {
 // at 1/12 of the HBM rate: 13 % of the Parallel WaveGAN forward).
 // HIST (causal, lag 1): frames j-2 and j-1 below 0 are hist_in[r][j] and hist_in[r][1] (rows x 2, oldest first).  Same
 // three-FMA expression.
-template <bool HIST>
-__global__ void upsample_fir_kernel(int rows, int rows_per_batch, int t_in, int s, int lag, const float* __restrict__ x,
-                                    const float* __restrict__ fir, float* __restrict__ y, long long ybs,
-                                    const float* __restrict__ hist_in) {
+// EXT (with HIST): the stage of a lookahead stream (pwgb_upsample_fir_stream_ext_forward); the same expression, with the
+// outputs outside the signal (the pwgb_stream_ext mask) stored as +0.0.
+template <bool HIST, bool EXT>
+__device__ __forceinline__ void upsample_fir_body(int rows, int rows_per_batch, int t_in, int s, int lag, const float* __restrict__ x,
+                                                  const float* __restrict__ fir, float* __restrict__ y, long long ybs,
+                                                  const float* __restrict__ hist_in, const int* frame, const int* end, int rate,
+                                                  int look) {
   extern __shared__ float coef[];  // [3][s]
   for (int ph = threadIdx.x; ph < s; ph += blockDim.x) {
     float a = 0.f, bsum = 0.f, c = 0.f;
@@ -56,6 +59,16 @@ __global__ void upsample_fir_kernel(int rows, int rows_per_batch, int t_in, int 
       xp = jc + 1 < t_in ? __ldg(xr + jc + 1) : 0.f;
     }
     float* dst = yr + (long long)j * s;
+    if constexpr (EXT) {
+      // signal sample of output o = j * s + ph; the chunk's outputs are contiguous, so the mask is one interval per frame
+      const long long pos0 = (long long)__ldg(frame + r / rows_per_batch) * rate - look + (long long)j * s;
+      const long long lim = (long long)__ldg(end + r / rows_per_batch) * rate;
+      for (int ph = 0; ph < s; ++ph) {
+        const float v = fmaf(coef[2 * s + ph], xp, fmaf(coef[s + ph], x0, coef[ph] * xm));
+        dst[ph] = (pos0 + ph < 0 || pos0 + ph >= lim) ? 0.f : v;
+      }
+      continue;
+    }
     if (vec) {
       for (int ph = 0; ph < s; ph += 4) {
         float4 v;
@@ -69,6 +82,20 @@ __global__ void upsample_fir_kernel(int rows, int rows_per_batch, int t_in, int 
       for (int ph = 0; ph < s; ++ph) dst[ph] = fmaf(coef[2 * s + ph], xp, fmaf(coef[s + ph], x0, coef[ph] * xm));
     }
   }
+}
+
+template <bool HIST>
+__global__ void upsample_fir_kernel(int rows, int rows_per_batch, int t_in, int s, int lag, const float* __restrict__ x,
+                                    const float* __restrict__ fir, float* __restrict__ y, long long ybs,
+                                    const float* __restrict__ hist_in) {
+  upsample_fir_body<HIST, false>(rows, rows_per_batch, t_in, s, lag, x, fir, y, ybs, hist_in, nullptr, nullptr, 1, 0);
+}
+
+__global__ void upsample_fir_stream_ext_kernel(int rows, int rows_per_batch, int t_in, int s, const float* __restrict__ x,
+                                               const float* __restrict__ fir, float* __restrict__ y, long long ybs,
+                                               const float* __restrict__ hist_in, const int* __restrict__ frame,
+                                               const int* __restrict__ end, int rate, int look) {
+  upsample_fir_body<true, true>(rows, rows_per_batch, t_in, s, 1, x, fir, y, ybs, hist_in, frame, end, rate, look);
 }
 
 }  // namespace pwgb
@@ -110,4 +137,21 @@ extern "C" int pwgb_upsample_fir_causal_stream_forward(int rows, int rows_per_ba
                                                        void* stream) {
   PWGB_CHECK_ARG(hist_in, "upsample_fir_causal_stream: null history");
   return upsample_fir_forward(rows, rows_per_batch, t_in, scale, 1, x, fir, y, y_batch_stride, stream, hist_in);
+}
+
+extern "C" int pwgb_upsample_fir_stream_ext_forward(int rows, int rows_per_batch, int t_in, int scale, const float* x, const float* fir,
+                                                    float* y, long long y_batch_stride, const float* hist_in,
+                                                    const pwgb_stream_ext* ext, void* stream) {
+  PWGB_CHECK_ARG(x && fir && y && hist_in, "upsample_fir_stream_ext: null argument");
+  PWGB_CHECK_ARG(ext && ext->frame && ext->end && ext->rate >= 1 && ext->lookahead >= 0 && !ext->res_hist_len && !ext->res_delay,
+                 "upsample_fir_stream_ext: ext must be a mask (frame, end, rate >= 1, lookahead >= 0) without residual fields");
+  PWGB_CHECK_ARG(rows >= 0 && rows_per_batch > 0 && t_in > 0 && scale > 0 && rows % rows_per_batch == 0,
+                 "upsample_fir_stream_ext: bad sizes");
+  PWGB_UNSUPPORTED_IF(rows > 65535, "upsample_fir_stream_ext: too many rows");
+  if (rows == 0) return PWGB_OK;
+  const long long ybs = y_batch_stride ? y_batch_stride : (long long)rows_per_batch * t_in * scale;
+  dim3 grid(ceil_div(t_in, 256) < 64 ? ceil_div(t_in, 256) : 64, rows);
+  upsample_fir_stream_ext_kernel<<<grid, 256, 3 * scale * sizeof(float), (cudaStream_t)stream>>>(
+      rows, rows_per_batch, t_in, scale, x, fir, y, ybs, hist_in, ext->frame, ext->end, ext->rate, ext->lookahead);
+  return check_launch("upsample_fir_stream_ext_kernel");
 }

@@ -50,6 +50,18 @@ struct WnK {
   int write_x, skip_init;
 };
 
+// The parameters of a lookahead-stream layer (wavenet_fused_ext_kernel, pwgb_wnstack_layer_stream_ext_forward): the
+// causal tap pattern over [history | chunk] with the output labelled (K-1)/2 * D rows earlier, so the residual is input
+// row t - rdelay; the conditioning of output row t is row c_row0 + t of cpk; the skip of output row t goes to column
+// skip_col0 + t of rows skip_rs floats apart; x' rows outside the signal (the pwgb_stream_ext mask) are stored as zero.
+struct WnKExt : WnK {
+  int rdelay, c_row0, skip_col0;
+  long long skip_rs;
+  const int* frame;
+  const int* end;
+  int rate, look;
+};
+
 __device__ __forceinline__ float ex2_approx(float v) {
   float r;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(v));
@@ -93,10 +105,12 @@ __device__ __forceinline__ void gate_to_z(const float* acc, const float* bias1, 
   }
 }
 
-__global__ void __launch_bounds__(WN_THREADS, 1)
-    wavenet_fused_kernel(const WnK p, const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_c,
-                         const unsigned* __restrict__ xin, const unsigned char* __restrict__ wpk, const float* __restrict__ b_conv,
-                         const float* __restrict__ b_so, unsigned* __restrict__ xout, float* __restrict__ skips) {
+// EXT: the lookahead-stream layer (P = WnKExt); the centred and causal layers are EXT = false (P = WnK)
+template <bool EXT, class P>
+__device__ __forceinline__ void wavenet_fused_body(const P& p, const CUtensorMap* tm_x, const CUtensorMap* tm_c,
+                                                   const unsigned* __restrict__ xin, const unsigned char* __restrict__ wpk,
+                                                   const float* __restrict__ b_conv, const float* __restrict__ b_so,
+                                                   unsigned* __restrict__ xout, float* __restrict__ skips) {
   extern __shared__ __align__(128) unsigned char smem[];
   // layout: ring[nslot] (A 16 KB | B) | resident skip/out weights | z images (one per warpgroup) | barriers | bias
   unsigned char* ring = smem;
@@ -135,8 +149,8 @@ __global__ void __launch_bounds__(WN_THREADS, 1)
   if (warp == WN_W_TMA) {
     // ===================== TMA loader: activation windows + weight stages
     if (lane == 0) {
-      tma_prefetch_desc(&tm_x);
-      tma_prefetch_desc(&tm_c);
+      tma_prefetch_desc(tm_x);
+      tma_prefetch_desc(tm_c);
       // skip / out weights stay resident for the whole kernel
       mbar_expect_tx(WSO_FULL, (unsigned)p.wso_bytes);
       for (int sc = 0; sc < p.nsc; ++sc)
@@ -159,9 +173,11 @@ __global__ void __launch_bounds__(WN_THREADS, 1)
           const unsigned full = FULL(s);
           mbar_expect_tx(full, (unsigned)(p.a_bytes + p.b_bytes));
           if (is_x)
-            tma_load_3d(dstA, &tm_x, 2 * (p.halo + t0 + (tap - p.tap0) * p.D), chunk * 4, 2 * b, full);
+            tma_load_3d(dstA, tm_x, 2 * (p.halo + t0 + (tap - p.tap0) * p.D), chunk * 4, 2 * b, full);
+          else if constexpr (EXT)
+            tma_load_3d(dstA, tm_c, 2 * (p.c_row0 + t0), chunk * 4, 2 * b, full);
           else
-            tma_load_3d(dstA, &tm_c, 2 * t0, chunk * 4, 2 * b, full);
+            tma_load_3d(dstA, tm_c, 2 * t0, chunk * 4, 2 * b, full);
           const unsigned char* wsrc = is_x ? wpk + (size_t)j * p.b_bytes : w_aux + (size_t)chunk * p.b_bytes;
           bulk_g2s(dstA + (unsigned)p.a_bytes, wsrc, (unsigned)p.b_bytes, full);
         }
@@ -246,14 +262,27 @@ __global__ void __launch_bounds__(WN_THREADS, 1)
         const bool tv = t < p.T;
         if (col < S) {
           if (tv) {
-            float* q = skips + ((long long)b * S + col) * p.T + t;
-            const float v0 = acc[e] + bias2[col], v1 = acc[e + 1] + bias2[col + 1];
-            if (p.skip_init) {
-              q[0] = v0;
-              q[p.T] = v1;
+            if constexpr (EXT) {
+              const long long rs = p.skip_rs;
+              float* q = skips + ((long long)b * S + col) * rs + p.skip_col0 + t;
+              const float v0 = acc[e] + bias2[col], v1 = acc[e + 1] + bias2[col + 1];
+              if (p.skip_init) {
+                q[0] = v0;
+                q[rs] = v1;
+              } else {
+                q[0] = v0 + q[0];
+                q[rs] = v1 + q[rs];
+              }
             } else {
-              q[0] = v0 + q[0];
-              q[p.T] = v1 + q[p.T];
+              float* q = skips + ((long long)b * S + col) * p.T + t;
+              const float v0 = acc[e] + bias2[col], v1 = acc[e + 1] + bias2[col + 1];
+              if (p.skip_init) {
+                q[0] = v0;
+                q[p.T] = v1;
+              } else {
+                q[0] = v0 + q[0];
+                q[p.T] = v1 + q[p.T];
+              }
             }
           }
         } else if (p.write_x) {
@@ -262,9 +291,15 @@ __global__ void __launch_bounds__(WN_THREADS, 1)
           const long long hi_i = (((long long)(b * 2) * p.ngx + (ch >> 3)) * p.Tp + p.halo + t) * 4 + ((ch & 7) >> 1);
           const long long lo_i = hi_i + (long long)p.ngx * p.Tp * 4;
           unsigned hi = 0, lo = 0;  // rows past the end of the sequence stay zero (the next layer's padding)
-          if (tv) {
+          bool keep = tv;
+          long long r_off = 0;  // the residual's row, relative to the output row (EXT: the delayed residual)
+          if constexpr (EXT) {
+            keep = tv && !stream_outside(p.frame, p.end, p.rate, p.look, b, t);
+            r_off = -4LL * p.rdelay;
+          }
+          if (keep) {
             float fh[2], fl[2];
-            const unsigned xh = __ldg(xin + hi_i), xl = __ldg(xin + lo_i);
+            const unsigned xh = __ldg(xin + hi_i + r_off), xl = __ldg(xin + lo_i + r_off);
             fh[0] = __uint_as_float(xh << 16), fh[1] = __uint_as_float(xh & 0xFFFF0000u);
             fl[0] = __uint_as_float(xl << 16), fl[1] = __uint_as_float(xl & 0xFFFF0000u);
             const float u0 = ((acc[e] + bias2[col]) + fh[0] + fl[0]) * rs;
@@ -277,6 +312,20 @@ __global__ void __launch_bounds__(WN_THREADS, 1)
       }
     }
   }
+}
+
+__global__ void __launch_bounds__(WN_THREADS, 1)
+    wavenet_fused_kernel(const WnK p, const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_c,
+                         const unsigned* __restrict__ xin, const unsigned char* __restrict__ wpk, const float* __restrict__ b_conv,
+                         const float* __restrict__ b_so, unsigned* __restrict__ xout, float* __restrict__ skips) {
+  wavenet_fused_body<false>(p, &tm_x, &tm_c, xin, wpk, b_conv, b_so, xout, skips);
+}
+
+__global__ void __launch_bounds__(WN_THREADS, 1)
+    wavenet_fused_ext_kernel(const WnKExt p, const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_c,
+                             const unsigned* __restrict__ xin, const unsigned char* __restrict__ wpk, const float* __restrict__ b_conv,
+                             const float* __restrict__ b_so, unsigned* __restrict__ xout, float* __restrict__ skips) {
+  wavenet_fused_body<true>(p, &tm_x, &tm_c, xin, wpk, b_conv, b_so, xout, skips);
 }
 
 // ------------------------------------------------------------------ layout helpers (HBM-bound, one pass)
@@ -312,24 +361,41 @@ __global__ void wn_unpack_kernel(const uint4* __restrict__ pk, int ng, int rows,
   }
 }
 
-// first_conv (Conv1d1x1 in_channels -> R, parallel_wavegan.py:155) writing the packed residual stream directly
-__global__ void wn_first_conv_kernel(const float* __restrict__ z, int cin, const float* __restrict__ w, const float* __restrict__ bias,
-                                     int T, uint4* __restrict__ pk, int ng, int rows, int row0) {
+// first_conv (Conv1d1x1 in_channels -> R, parallel_wavegan.py:155) writing the packed residual stream directly.
+// EXT (lookahead stream): z rows are zs floats apart, and rows outside the signal (the pwgb_stream_ext mask) are zero.
+template <bool EXT>
+__device__ __forceinline__ void wn_first_conv_body(const float* __restrict__ z, int cin, const float* __restrict__ w,
+                                                   const float* __restrict__ bias, int T, uint4* __restrict__ pk, int ng, int rows,
+                                                   int row0, long long zs, const int* frame, const int* end, int rate, int look) {
   const int b = blockIdx.z, g = blockIdx.y;
   for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < T; t += gridDim.x * blockDim.x) {
     float u[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) u[j] = bias ? __ldg(bias + g * 8 + j) : 0.f;
     for (int ci = 0; ci < cin; ++ci) {
-      const float zv = __ldg(z + ((long long)b * cin + ci) * T + t);
+      const float zv = __ldg(z + ((long long)b * cin + ci) * (EXT ? zs : T) + t);
 #pragma unroll
       for (int j = 0; j < 8; ++j) u[j] = fmaf(__ldg(w + (long long)(g * 8 + j) * cin + ci), zv, u[j]);
     }
     uint4 hi, lo;
     split8(u, hi, lo);
+    if constexpr (EXT) {
+      if (stream_outside(frame, end, rate, look, b, t)) hi = lo = make_uint4(0u, 0u, 0u, 0u);
+    }
     pk[((long long)(b * 2 + 0) * ng + g) * rows + row0 + t] = hi;
     pk[((long long)(b * 2 + 1) * ng + g) * rows + row0 + t] = lo;
   }
+}
+
+__global__ void wn_first_conv_kernel(const float* __restrict__ z, int cin, const float* __restrict__ w, const float* __restrict__ bias,
+                                     int T, uint4* __restrict__ pk, int ng, int rows, int row0) {
+  wn_first_conv_body<false>(z, cin, w, bias, T, pk, ng, rows, row0, T, nullptr, nullptr, 1, 0);
+}
+
+__global__ void wn_first_conv_ext_kernel(const float* __restrict__ z, long long zs, int cin, const float* __restrict__ w,
+                                         const float* __restrict__ bias, int T, uint4* __restrict__ pk, int ng, int rows, int row0,
+                                         const int* __restrict__ frame, const int* __restrict__ end, int rate, int look) {
+  wn_first_conv_body<true>(z, cin, w, bias, T, pk, ng, rows, row0, zs, frame, end, rate, look);
 }
 
 
@@ -508,12 +574,86 @@ extern "C" int pwgb_wnstack_layer_forward(const pwgb_wnstack_desc* d, int dilati
   return check_launch("wavenet_fused_kernel");
 }
 
+static int wn_check_mask(const pwgb_stream_ext* e, const char* what) {
+  PWGB_CHECK_ARG(e && e->frame && e->end && e->rate >= 1 && e->lookahead >= 0 && !e->res_hist && !e->res_hist_len && !e->res_delay,
+                 "%s: ext must be a mask (frame, end, rate >= 1, lookahead >= 0) without residual fields", what);
+  return PWGB_OK;
+}
+
+extern "C" int pwgb_wnstack_first_conv_stream_ext(const pwgb_wnstack_desc* d, const float* z, long long z_row_stride, int in_channels,
+                                                  const float* w, const float* bias, const pwgb_stream_ext* ext, void* xpk, void* stream) {
+  WnK p;
+  size_t bytes;
+  PWGB_UNSUPPORTED_IF(!wn_plan(d, p, bytes), "wnstack: configuration not supported");
+  PWGB_CHECK_ARG(in_channels > 0 && z_row_stride >= p.T, "wnstack_first_conv_stream_ext: bad argument");
+  if (const int rc = wn_check_mask(ext, "wnstack_first_conv_stream_ext")) return rc;
+  if (p.B == 0) return PWGB_OK;
+  PWGB_CHECK_ARG(z && w && xpk, "wnstack_first_conv_stream_ext: bad argument");
+  wn_first_conv_ext_kernel<<<wn_grid(p.T, p.ngx, p.B), 256, 0, (cudaStream_t)stream>>>(
+      z, z_row_stride, in_channels, w, bias, p.T, (uint4*)xpk, p.ngx, p.Tp, p.halo, ext->frame, ext->end, ext->rate, ext->lookahead);
+  return check_launch("wn_first_conv_ext_kernel");
+}
+
+extern "C" int pwgb_wnstack_layer_stream_ext_forward(const pwgb_wnstack_desc* d, int dilation, const void* xpk_in, const void* cpk,
+                                                     int c_rows, int c_row0, const void* packed_w, const float* b_conv,
+                                                     const float* b_skip_out, void* xpk_out, float* skips, int skip_col0,
+                                                     long long skip_row_stride, int skips_init, const pwgb_stream_ext* ext,
+                                                     void* stream) {
+  WnKExt p;
+  size_t bytes = 0;
+  PWGB_UNSUPPORTED_IF(!wn_plan(d, p, bytes), "wnstack: configuration not supported by the fused tensor-core layer");
+  PWGB_CHECK_ARG(!d->causal, "wnstack_layer_stream_ext: the lookahead layer streams a centred stack (causal = 0)");
+  PWGB_CHECK_ARG(dilation > 0 && (long long)(p.K - 1) * dilation <= d->halo,
+                 "wnstack_layer_stream_ext: (kernel - 1) * dilation %d exceeds the halo %d of the packed stream", (p.K - 1) * dilation,
+                 d->halo);
+  PWGB_CHECK_ARG(c_row0 >= 0 && c_rows >= c_row0 + p.T, "wnstack_layer_stream_ext: conditioning rows [%d, %d) outside the %d rows of cpk",
+                 c_row0, c_row0 + p.T, c_rows);
+  PWGB_CHECK_ARG(skip_col0 >= 0 && skip_row_stride >= (long long)skip_col0 + p.T, "wnstack_layer_stream_ext: bad skip columns");
+  if (const int rc = wn_check_mask(ext, "wnstack_layer_stream_ext")) return rc;
+  if (p.B == 0) return PWGB_OK;
+  PWGB_CHECK_ARG(xpk_in && cpk && packed_w && skips, "wnstack_layer_stream_ext: null argument");
+  PWGB_CHECK_ARG(xpk_in != xpk_out, "wnstack_layer_stream_ext: xpk_out must not alias xpk_in (other tiles read the halo)");
+  PWGB_CHECK_ARG(!((reinterpret_cast<uintptr_t>(xpk_in) | reinterpret_cast<uintptr_t>(cpk) | reinterpret_cast<uintptr_t>(packed_w) |
+                    reinterpret_cast<uintptr_t>(xpk_out)) & 15),
+                 "wnstack_layer_stream_ext: packed buffers must be 16-byte aligned");
+  p.tap0 = p.K - 1;  // the causal tap pattern; the output is labelled (K-1)/2 * dilation rows earlier
+  p.D = dilation;
+  p.write_x = xpk_out != nullptr;
+  p.skip_init = skips_init != 0;
+  p.rdelay = (p.K - 1) / 2 * dilation;
+  p.c_row0 = c_row0;
+  p.skip_col0 = skip_col0;
+  p.skip_rs = skip_row_stride;
+  p.frame = ext->frame;
+  p.end = ext->end;
+  p.rate = ext->rate;
+  p.look = ext->lookahead;
+  static bool smem_set = false;
+  if (const int rc = smem_opt_in(smem_set, {wavenet_fused_ext_kernel}, 227 * 1024, "wnstack_layer_stream_ext")) return rc;
+  const int num_sms = tc_num_sms();
+  const int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
+  CUtensorMap tm_x, tm_c;
+  {
+    const unsigned long long dx[3] = {2ull * p.Tp, (unsigned long long)p.ngx, 2ull * p.B};
+    const unsigned long long dc[3] = {2ull * c_rows, (unsigned long long)p.ngc, 2ull * p.B};
+    const unsigned box[3] = {2u * WN_TT, 4u, 2u};
+    int rc = tma_make(&tm_x, CU_TENSOR_MAP_DATA_TYPE_UINT64, 8, 3, xpk_in, dx, box);
+    if (rc) return rc;
+    rc = tma_make(&tm_c, CU_TENSOR_MAP_DATA_TYPE_UINT64, 8, 3, cpk, dc, box);
+    if (rc) return rc;
+  }
+  wavenet_fused_ext_kernel<<<(unsigned)grid, WN_THREADS, bytes, (cudaStream_t)stream>>>(
+      p, tm_x, tm_c, (const unsigned*)xpk_in, (const unsigned char*)packed_w, b_conv, b_skip_out, (unsigned*)xpk_out, skips);
+  return check_launch("wavenet_fused_ext_kernel");
+}
+
 extern "C" int pwgb_wnstack_carry(const pwgb_wnstack_desc* d, const void* xpk_save, void* hist_save, int h_save, void* xpk_load,
                                   const void* hist_load, int h_load, void* stream) {
   WnK p;
   size_t bytes;
   PWGB_UNSUPPORTED_IF(!wn_plan(d, p, bytes), "wnstack: configuration not supported");
-  PWGB_CHECK_ARG(d->causal, "wnstack_carry: only a causal stack reads its history from the left halo");
+  // a causal stack, or a centred one streamed with lookahead (pwgb_wnstack_layer_stream_ext_forward): both read their
+  // history from the left halo
   PWGB_CHECK_ARG(h_save >= 0 && h_save <= d->halo && h_load >= 0 && h_load <= d->halo,
                  "wnstack_carry: history lengths %d / %d must lie in [0, halo = %d]", h_save, h_load, d->halo);
   PWGB_CHECK_ARG(!h_save || (xpk_save && hist_save), "wnstack_carry: null save buffer");

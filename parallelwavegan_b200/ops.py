@@ -367,12 +367,16 @@ def upsample_fir(x, fir, scale, out=None, out_channels=None, causal=False):
     return out
 
 
-def upsample_fir_causal_stream(x, fir, scale, hist, out=None, out_channels=None):
+def upsample_fir_causal_stream(x, fir, scale, hist, out=None, out_channels=None, mask=None):
     """The causal upsampler stage of a stream (pwgb_upsample_fir_causal_stream_forward): ``upsample_fir(..., causal=True)``
     with input frames -2 and -1 read from ``hist`` ((B, C, 2) or (B*C, 2), contiguous) instead of the zero padding.  The
     history is only read; the caller carries it (``stream_carry``).  ``out`` and ``out_channels`` as in ``upsample_fir``:
     a given ``out`` with more than C channels must hold zeros in the others.  Bit-identical to the whole-signal stage on
-    the concatenation."""
+    the concatenation.
+
+    With ``mask`` = (frame, end, rate, lookahead) as in conv1d_stream: the centred stage of a lookahead stream
+    (pwgb_upsample_fir_stream_ext_forward), the same three frames labelled one frame earlier, with the outputs outside
+    the signal stored as +0.0; bit-identical to the centred whole-signal stage ``upsample_fir``."""
     x = _dev(x, "x")
     fir = _dev(fir, "fir").reshape(-1)
     hist = _dev(hist, "hist")
@@ -387,9 +391,15 @@ def upsample_fir_causal_stream(x, fir, scale, hist, out=None, out_channels=None)
     elif tuple(out.shape) != (B, oc, T * scale) or not out.is_contiguous() or out.dtype != torch.float32:
         raise PwgbError(f"upsample_fir_causal_stream: out must be a contiguous float32 {(B, oc, T * scale)} tensor")
     prof = _Prof("upsample_fir", 2.0 * B * Cc * T * scale * (2 * scale + 1), 4.0 * (x.numel() + B * Cc * T * scale), f"B{B} C{Cc} T{T} s{scale}")
-    rc = capi.lib().pwgb_upsample_fir_causal_stream_forward(B * Cc, Cc, T, int(scale), _p(x), _p(fir), _p(out), oc * T * scale,
-                                                            _p(hist), _stream())
-    capi.check(rc, "pwgb_upsample_fir_causal_stream_forward")
+    if mask is not None:
+        ext = _stream_ext(B, Cc, mask, None, 0)
+        rc = capi.lib().pwgb_upsample_fir_stream_ext_forward(B * Cc, Cc, T, int(scale), _p(x), _p(fir), _p(out), oc * T * scale,
+                                                             _p(hist), C.byref(ext), _stream())
+        capi.check(rc, "pwgb_upsample_fir_stream_ext_forward")
+    else:
+        rc = capi.lib().pwgb_upsample_fir_causal_stream_forward(B * Cc, Cc, T, int(scale), _p(x), _p(fir), _p(out), oc * T * scale,
+                                                                _p(hist), _stream())
+        capi.check(rc, "pwgb_upsample_fir_causal_stream_forward")
     prof.done()
     return out
 
@@ -593,6 +603,16 @@ def conv_transpose1d_window_stream(x, hist, w, bias=None, *, stride, padding, fr
     return y
 
 
+def stream_mask(y, mask):
+    """pwgb_stream_mask: y (B, C, T) contiguous fp32, in place: the samples outside the signal of ``mask`` = (frame, end,
+    rate, lookahead) (as in conv1d_stream) become +0.0.  Returns y."""
+    y = _dev(y, "y")
+    B, Cc, T = y.shape
+    rc = capi.lib().pwgb_stream_mask(_p(y), B, Cc, T, C.byref(_stream_ext(B, Cc, mask, None, 0)), _stream())
+    capi.check(rc, "pwgb_stream_mask")
+    return y
+
+
 def stream_carry_table(entries, device):
     """Device table of pwgb_stream_carry for ``entries`` = [(x, hist), ...]: x (..., n) is a chunk of a signal and hist
     (..., H) its history, both contiguous fp32 with the same leading shape.  The table holds the tensors' addresses, so
@@ -717,9 +737,11 @@ class WnStack:
     tensor core's operand layout (bf16 hi/lo) between the fused one-kernel layers.  Holds the two ping-pong
     stream buffers (zero halos, allocated once per (B, T)) and the packed conditioning."""
 
-    def __init__(self, B, T, R, G, S, A, K, max_dilation, device, causal=False):
+    def __init__(self, B, T, R, G, S, A, K, max_dilation, device, causal=False, lookahead=False):
+        # a centred stack streamed with lookahead keeps its layers' histories in the left halo, as a causal one does
+        halo = _wn_halo(K, max_dilation, causal or lookahead)
         self.desc = capi.WnStackDesc(batch=B, t=T, residual_channels=R, gate_channels=G, skip_channels=S, aux_channels=A,
-                                     kernel=K, halo=_wn_halo(K, max_dilation, causal), causal=int(bool(causal)))
+                                     kernel=K, halo=halo, causal=int(bool(causal)))
         L = capi.lib()
         if not L.pwgb_wnstack_supported(C.byref(self.desc)):
             raise PwgbError("wnstack: configuration not supported by the fused tensor-core layer")
@@ -748,6 +770,25 @@ class WnStack:
         rc = capi.lib().pwgb_wnstack_pack_c(C.byref(self.desc), _p(c), Cs * T, _p(self.c), _stream())
         capi.check(rc, "pwgb_wnstack_pack_c")
         prof.done()
+
+    def pack_c_window(self, c):
+        """Pack c (B, >= A, L), a conditioning window of L >= T samples, as pwgb_wnstack_pack_c does for a stack of L
+        samples, into a buffer kept by the stack (allocated on first use).  Returns (cpk, rows per plane)."""
+        c = _dev(c, "c")
+        B, Cs, L = c.shape
+        if B != self.shape[0] or L < self.shape[2] or Cs < self.A:
+            raise PwgbError(f"wnstack.pack_c_window: conditioning shape {tuple(c.shape)} does not match the stack")
+        d = self.__dict__.get("cw_desc")
+        if d is None or d.t != L:
+            dd = self.desc
+            d = capi.WnStackDesc(batch=B, t=L, residual_channels=dd.residual_channels, gate_channels=dd.gate_channels,
+                                 skip_channels=dd.skip_channels, aux_channels=dd.aux_channels, kernel=dd.kernel, halo=0, causal=dd.causal)
+            nc = capi.lib().pwgb_wnstack_c_bytes(C.byref(d))
+            self.cw_desc, self.cw = d, torch.empty(nc // 4, device=c.device, dtype=torch.int32)
+            self.cw_rows = nc // (B * 2 * ((self.A + 7) // 8) * 16)
+        rc = capi.lib().pwgb_wnstack_pack_c(C.byref(d), _p(c), Cs * L, _p(self.cw), _stream())
+        capi.check(rc, "pwgb_wnstack_pack_c")
+        return self.cw, self.cw_rows
 
     def pack_x(self, x):
         x = _dev(x, "x")
@@ -786,6 +827,41 @@ class WnStack:
         rc = capi.lib().pwgb_wnstack_layer_forward(C.byref(self.desc), int(dilation), _p(self.x[self.cur]), _p(self.c), _p(packed),
                                                    _p(b_conv), _p(b_skip_out), _p(nxt), _p(skips), int(bool(skips_init)), _stream())
         capi.check(rc, "pwgb_wnstack_layer_forward")
+        prof.done()
+        self.prev = self.x[self.cur]
+        if write_x:
+            self.cur = 1 - self.cur
+
+    def first_conv_stream(self, z, w, bias, mask):
+        """first_conv of a lookahead stream (pwgb_wnstack_first_conv_stream_ext): z (B, in_channels, >= T), its first T
+        samples per row; rows outside the signal of ``mask`` are stored as zero."""
+        z = _dev(z, "z")
+        w = _dev(w, "w").reshape(w.shape[0], -1)
+        B, cin, Tz = z.shape
+        if B != self.shape[0] or Tz < self.shape[2] or w.shape != (self.shape[1], cin):
+            raise PwgbError("wnstack.first_conv_stream: shape mismatch")
+        ext = _stream_ext(B, self.shape[1], mask, None, 0)
+        rc = capi.lib().pwgb_wnstack_first_conv_stream_ext(C.byref(self.desc), _p(z), Tz, cin, _p(w), _p(bias), C.byref(ext),
+                                                           _p(self.x[self.cur]), _stream())
+        capi.check(rc, "pwgb_wnstack_first_conv_stream_ext")
+
+    def layer_stream(self, packed, b_conv, b_skip_out, dilation, cpk, c_rows, c_row0, skips, skip_col0, mask, skips_init=False,
+                     write_x=True):
+        """One layer of a lookahead stream (pwgb_wnstack_layer_stream_ext_forward) on the current buffer: the conditioning
+        of output row t is row c_row0 + t of ``cpk`` (c_rows rows per plane); its skip goes to column skip_col0 + t of
+        ``skips`` (B, S, W) contiguous fp32; x' rows outside the signal of ``mask`` are zero."""
+        B, R, T = self.shape
+        if skips.dim() != 3 or tuple(skips.shape[:2]) != (B, self.S) or not skips.is_contiguous():
+            raise PwgbError(f"wnstack.layer_stream: skips must be a contiguous ({B}, {self.S}, W) tensor")
+        nxt = self.x[1 - self.cur] if write_x else None
+        ext = _stream_ext(B, R, mask, None, 0)
+        prof = _Prof("wavenet_fused_tc", 2.0 * B * T * (self.desc.gate_channels * R * self.desc.kernel + self.desc.gate_channels * self.A +
+                                                         (self.S + R) * (self.desc.gate_channels // 2)), 0.0, f"B{B} d{dilation} T{T} stream")
+        rc = capi.lib().pwgb_wnstack_layer_stream_ext_forward(C.byref(self.desc), int(dilation), _p(self.x[self.cur]), _p(cpk), int(c_rows),
+                                                              int(c_row0), _p(packed), _p(b_conv), _p(b_skip_out), _p(nxt), _p(skips),
+                                                              int(skip_col0), skips.shape[-1], int(bool(skips_init)), C.byref(ext),
+                                                              _stream())
+        capi.check(rc, "pwgb_wnstack_layer_stream_ext_forward")
         prof.done()
         self.prev = self.x[self.cur]
         if write_x:

@@ -1,6 +1,7 @@
 """Chunked synthesis: mel frames in, waveform out, while the frames are still arriving.  ``CausalPWGStream`` streams a
 causal Parallel WaveGAN, ``CausalHiFiGANStream`` a causal HiFi-GAN, ``CausalMelGANStream`` a causal (multi-band) MelGAN,
-and ``HiFiGANLookaheadStream`` a centred HiFi-GAN with a fixed lookahead and a flush.
+and ``HiFiGANLookaheadStream`` and ``PWGLookaheadStream`` a centred HiFi-GAN and a centred Parallel WaveGAN with a fixed
+lookahead and a flush.
 
 A causal generator's output for frame j depends only on frames <= j, so it can be synthesised as soon as frame j
 exists.  ``CausalPWGStream`` carries, per batch slot, everything the whole-utterance forward would read from before
@@ -26,7 +27,7 @@ from .capi import PwgbError
 from .layers import ConvInUpsampleNetwork, UpsampleNetwork, effective_weight
 
 
-def _layer_weights(f, A):
+def _layer_weights(f, A, causal=True):
     """The packed operand image of one WaveNet layer, shared with ParallelWaveGANGenerator._forward_packed's cache."""
     k = ops.param_key(f.conv, f.conv1x1_aux, f.conv1x1_skip, f.conv1x1_out)
     ent = f._cache.get("wnp")
@@ -34,7 +35,7 @@ def _layer_weights(f, A):
         return ent[1], ent[2]
     return ops.wavenet_packed_weights(effective_weight(f.conv), effective_weight(f.conv1x1_aux), effective_weight(f.conv1x1_skip),
                                       effective_weight(f.conv1x1_out), f.conv1x1_skip.bias, f.conv1x1_out.bias, A,
-                                      cache=f._cache, key=k, causal=True)
+                                      cache=f._cache, key=k, causal=causal)
 
 
 def wb(conv):
@@ -295,6 +296,218 @@ class CausalPWGStream(_ChunkStream):
             z = z.contiguous()
         self._start(c)
         return self._run(c.shape[-1], z, c)
+
+
+class PWGLookaheadStream(_ChunkStream):
+    """Streams a centred ``ParallelWaveGANGenerator`` (``use_causal_conv=False``, the published checkpoints) chunk by chunk
+    for ``batch`` independent slots, with a fixed lookahead of ``delay`` output samples.
+
+    ``push(c, z)`` takes the next n >= 1 mel frames and their n * hop noise samples of every slot and returns n * hop
+    samples: the whole-utterance samples from t0 * hop - delay on (t0: the frames pushed before), with zeros before sample
+    0.  ``flush(items)`` returns the last ``delay`` samples of those slots and restarts them; the other slots continue as
+    if no flush had happened.  For every slot, the concatenated pushes and flush equal ``[zeros(delay) |
+    model.inference(all_frames, all_noise)]``.
+
+    Each signal runs in delayed time behind the frames pushed (DESIGN.md §3.9, oracle/ref_pwg_lookahead_stream.py):
+
+    * conv_in (kernel 2 acw + 1) runs on [the last 2 acw frames | chunk], acw frames behind; a fresh slot's history is its
+      first frame replicated, and the flush pushes its last frame replicated (both edges of ``ReplicationPad1d``);
+    * each FIR stage (scale s) reads [2 history frames | chunk] and is one frame behind its input
+      (pwgb_upsample_fir_stream_ext_forward): lookahead look_c = 852 samples for v1 ([4, 4, 4, 4], acw 2);
+    * the conditioning enters each WaveNet layer after its dilated conv, so the residual stream runs look_x = look_c -
+      (K - 1) / 2 * d_0 behind: the noise goes through a look_x-sample delay line into first_conv;
+    * WaveNet layer l is the causal tap pattern over the (K - 1) d_l history rows of the packed stream's left halo
+      (pwgb_wnstack_layer_stream_ext_forward), look_x + D_l behind (D_l = sum_{j <= l} (K - 1) / 2 d_j), with its
+      residual read (K - 1) / 2 d_l rows back, its conditioning read from a window that keeps the last off_L rows, and its
+      skip added into an (off_L + T)-column accumulator at the columns of its output positions; layer 0 initialises them
+      and the others add in layer order, as in ``inference``;
+    * every signal a later layer reads is masked to +0.0 outside [0, end) (pwgb_stream_ext: device frame counters and end
+      frames), the whole-utterance zero padding, and so is the output before sample 0.
+
+    ``delay`` = look_x + D_L: 3920 samples (15.3 frames) for v1, the lookahead autograd measures on the model.  With
+    ``use_graphs`` each chunk length is captured once into a CUDA graph and replayed.  The weights are read when the stream
+    is built and must not change while it is used."""
+
+    OPEN = 2 ** 31 - 1  # the end frame of a slot whose signal has not ended
+
+    def __init__(self, model, batch=1, seed=None, use_graphs=True):
+        from .models import MelGANGenerator, ParallelWaveGANGenerator
+
+        if not isinstance(model, ParallelWaveGANGenerator):
+            raise PwgbError("PWGLookaheadStream: expected a ParallelWaveGANGenerator")
+        if model.use_causal_conv:
+            raise PwgbError("PWGLookaheadStream: the model is causal (use_causal_conv=True); stream it with CausalPWGStream, "
+                            "which has no lookahead")
+        up = model.upsample_net
+        if up is None:
+            raise PwgbError("PWGLookaheadStream: upsample_conditional_features=False is not supported")
+        if isinstance(up, MelGANGenerator):
+            raise PwgbError("PWGLookaheadStream: upsample_net='MelGANGenerator' is not supported")
+        if isinstance(up, UpsampleNetwork) and model.aux_context_window:
+            raise PwgbError("PWGLookaheadStream: UpsampleNetwork with aux_context_window > 0 has no whole-utterance inference to match")
+        conv_in = up.conv_in if isinstance(up, ConvInUpsampleNetwork) else None
+        acw = model.aux_context_window if conv_in is not None else 0
+        self.A = model.aux_channels
+        # ReplicationPad1d of inference: a fresh slot's conv_in history is its first frame
+        self._setup(model, batch, use_graphs, self.A, 2 * acw, "replicate")
+        fir_net = up.upsample if conv_in is not None else up
+        self.scales = list(fir_net.upsample_scales)
+        self.w_in = wb(conv_in)[0] if conv_in is not None else None
+        self.firs = [wb(fir_net.up_layers[2 * i + 1])[0] for i in range(len(self.scales))]
+        self.hop = model.upsample_factor
+        l0 = model.conv_layers[0]
+        self.R, self.G, self.K = l0.conv.in_channels, l0.conv.out_channels, l0.conv.kernel_size[0]
+        self.S = l0.conv1x1_skip.out_channels
+        self.dmax = max(f.dilation for f in model.conv_layers)
+        self.H = [(self.K - 1) * f.dilation for f in model.conv_layers]
+        if not ops.WnStack.supported(self.B, self.hop, self.R, self.G, self.S, self.A, self.K, self.dmax, False):
+            raise PwgbError("PWGLookaheadStream: the fused packed WaveNet stack does not support this configuration "
+                            f"(residual {self.R}, gate {self.G}, skip {self.S}, aux {self.A} channels, kernel {self.K})")
+        # the plan: lookaheads of conv_in (frames), of each FIR stage's output, of first_conv's output and of each layer's
+        look, self.looks = acw, []
+        self.look_in = acw
+        for s in self.scales:
+            look = look * s + s
+            self.looks.append(look)
+        self.look_c = look
+        self.D, acc = [], 0
+        for f in model.conv_layers:
+            acc += (self.K - 1) // 2 * f.dilation
+            self.D.append(acc)
+        self.look_x = max(self.look_c - self.D[0], 0)
+        self.off = [self.look_x + d - self.look_c for d in self.D]  # conditioning rows behind the newest, per layer
+        self.W = self.off[-1]
+        self.delay = self.look_x + self.D[-1]
+        self.w_first = wb(model.first_conv)
+        # the output head as in ParallelWaveGANGenerator.forward: sqrt(1/layers) folded into the first 1x1 conv
+        w1, b1 = wb(model.last_conv_layers[1])
+        self.w_l1, self.w_l3 = (w1 * model._skip_scale, b1), wb(model.last_conv_layers[3])
+        dev, B, A = self.dev, self.B, self.A
+        self.fir_hist = [self._zeros(B, A, 2) for _ in self.scales]
+        self.z_hist = self._zeros(B, model.in_channels, self.look_x)
+        self.c_hist = self._zeros(B, A, self.W)
+        self.skip_hist = self._zeros(B, self.S, self.W)
+        self.wn_hist = [torch.zeros((B, self.R * h), device=dev, dtype=torch.int32) for h in self.H]
+        self.frame = torch.zeros(B, device=dev, dtype=torch.int32)
+        self.end = torch.full((B,), self.OPEN, device=dev, dtype=torch.int32)
+        self._nohist = self._zeros(B, A, 0)
+        self.gen = torch.Generator(device=dev)
+        if seed is not None:
+            self.gen.manual_seed(int(seed))
+
+    def _state(self):
+        return [self.cin_hist] + self.fir_hist + [self.z_hist, self.c_hist, self.skip_hist] + self.wn_hist + [self.frame, self.end]
+
+    def reset(self, items=None):
+        super().reset(items)
+        for b in self._slots(items):
+            self.end[b] = self.OPEN
+
+    def _mask(self, rate, look):
+        return (self.frame, self.end, rate, look)
+
+    def _new_entry(self, n, xin):
+        """The buffers of an n-frame chunk (conditioning stages, the noise, conditioning and skip windows), the packed
+        WaveNet stack, and the carry table of every history but the WaveNet layers'."""
+        dev, B, A, T = self.dev, self.B, self.A, n * self.hop
+        ent = dict(stack=ops.WnStack(B, T, self.R, self.G, self.S, A, self.K, self.dmax, dev, causal=False, lookahead=True),
+                   zw=self._empty(B, self.model.in_channels, self.look_x + T), cw=self._empty(B, A, self.W + T),
+                   sw=self._zeros(B, self.S, self.W + T), skips=self._empty(B, self.S, T))
+        ent["cin"] = self._empty(B, A, n) if self.w_in is not None else xin
+        entries, x, t = [(xin, self.cin_hist)], ent["cin"], n
+        ent["fir"] = []
+        for i, s in enumerate(self.scales):
+            entries.append((x, self.fir_hist[i]))
+            t *= s
+            x = self._empty(B, A, t)
+            ent["fir"].append(x)
+        entries += [(ent["zw"], self.z_hist), (ent["cw"], self.c_hist), (ent["sw"], self.skip_hist)]
+        ent["table"] = ops.stream_carry_table(entries, dev)
+        return ent
+
+    def _step(self, z, c):
+        """One chunk: z (B, in_channels, n * hop), c (B, aux, n) -> (B, out_channels, n * hop).  Advances the state."""
+        m = self.model
+        n = c.shape[-1]
+        ent = self._entry(n)
+        W, lx, hop = self.W, self.look_x, self.hop
+        # conditioning: the masked conv_in on [history | chunk], then the masked FIR stages reading their histories
+        x = self._input(ent, c)
+        if self.w_in is not None:
+            x = ops.conv1d_stream(x, self._nohist, self.w_in, None, pad_left=0, out=ent["cin"], mask=self._mask(1, self.look_in))
+        rate = 1
+        for i, s in enumerate(self.scales):
+            rate *= s
+            x = ops.upsample_fir_causal_stream(x, self.firs[i], s, self.fir_hist[i], out=ent["fir"][i], mask=self._mask(rate, self.looks[i]))
+        # the windows [history | chunk] of the conditioning, the noise delay line and the skip accumulator
+        cw, zw, sw = ent["cw"], ent["zw"], ent["sw"]
+        cw[:, :, :W].copy_(self.c_hist)
+        cw[:, :, W:].copy_(x)
+        zw[:, :, :lx].copy_(self.z_hist)
+        zw[:, :, lx:].copy_(z)
+        sw[:, :, :W].copy_(self.skip_hist)
+        # the residual stack on the packed stream; each layer's history is carried between the layer launches
+        st = ent["stack"]
+        st.cur, st.prev = 0, None
+        cpk, c_rows = st.pack_c_window(cw)
+        st.first_conv_stream(zw, *self.w_first, mask=self._mask(hop, lx))
+        layers = m.conv_layers
+        L = len(layers)
+        st.carry(load=(self.wn_hist[0], self.H[0]))
+        for i, f in enumerate(layers):
+            packed, bso = _layer_weights(f, self.A, causal=False)
+            col = W - self.off[i]
+            st.layer_stream(packed, f.conv.bias, bso, f.dilation, cpk, c_rows, col, sw, col, self._mask(hop, lx + self.D[i]),
+                            skips_init=(i == 0), write_x=(i < L - 1))
+            st.carry(save=(self.wn_hist[i], self.H[i]), load=(self.wn_hist[i + 1], self.H[i + 1]) if i + 1 < L else None)
+        skips = ent["skips"]
+        skips.copy_(sw[:, :, :skips.shape[-1]])
+        ops.stream_carry(ent["table"])
+        h = ops.conv1d(skips, *self.w_l1, pre_slope=0.0)
+        # into a fresh tensor, as in inference: given out=, a wide few-channel output conv would not take _conv1d_fewcout
+        y = ops.stream_mask(ops.conv1d(h, *self.w_l3, pre_slope=0.0), self._mask(hop, self.delay))
+        self.frame += n
+        return y
+
+    @torch.no_grad()
+    def push(self, c, z=None, normalize_before=False):
+        """c: (B, n, aux) mel frames ((n, aux) when batch == 1); z: optional (B, in_channels, n * hop) noise of those
+        frames, drawn from the stream's generator when omitted.  Returns (B, out_channels, n * hop) on the device: samples
+        [t0 * hop - delay, (t0 + n) * hop - delay) of each slot's utterance."""
+        m = self.model
+        c = self._frames(c, normalize_before)
+        T = c.shape[-1] * self.hop
+        if z is None:
+            z = torch.randn((self.B, m.in_channels, T), device=self.dev, generator=self.gen)
+        else:
+            z = torch.as_tensor(z, dtype=torch.float32, device=self.dev)
+            if tuple(z.shape) != (self.B, m.in_channels, T):
+                raise PwgbError(f"PWGLookaheadStream.push: z must be ({self.B}, {m.in_channels}, {T}), got {tuple(z.shape)}")
+            z = z.contiguous()
+        self._start(c)
+        return self._run(c.shape[-1], z, c)
+
+    @torch.no_grad()
+    def flush(self, items=None):
+        """The last ``delay`` samples of slots ``items`` (an index, an iterable of indices or None for every slot), as
+        (len(items), out_channels, delay); the slots are then reset.  The flush push repeats each slot's last frame (the
+        right edge of ReplicationPad1d) with zero noise, and the end frames mask everything past the signal.  The other
+        slots' state is restored around it, so they continue exactly as if it had not happened; ending one slot costs a
+        ceil(delay / hop)-frame batch push (DESIGN.md §3.9)."""
+        items = list(self._slots(items))
+        keep = [b for b in range(self.B) if b not in items]
+        snap = [t[keep].clone() for t in self._state()] if keep else []
+        sel = torch.tensor(items, device=self.dev, dtype=torch.long)
+        self.end[sel] = self.frame[sel]
+        n = -(-self.delay // self.hop)
+        P = self.cin_hist.shape[-1]
+        c = self.cin_hist[:, :, P - 1:].expand(-1, -1, n).contiguous() if P else self._zeros(self.B, self.in_channels, n)
+        z = self._zeros(self.B, self.model.in_channels, n * self.hop)
+        y = self._run(n, z, c)[sel, :, :self.delay].contiguous()
+        for t, s in zip(self._state(), snap):
+            t[keep] = s
+        self.reset(items)
+        return y
 
 
 class _HiFiGANStream(_ChunkStream):

@@ -4,11 +4,12 @@ for batch sizes B, chunks of 1, 4, 16 and 64 frames, CUDA graphs off and on.  MO
 * pwg: the causal PWG v1 generator (CausalPWGStream), hop 256;
 * hifigan: the causal HiFi-GAN v1 generator (CausalHiFiGANStream), hop 256;
 * hifigan_centred: the centred HiFi-GAN v1 generator (HiFiGANLookaheadStream), hop 256, with its 3258-sample lookahead;
+* pwg_centred: the centred PWG v1 generator (PWGLookaheadStream), hop 256, with its 3920-sample lookahead;
 * melgan_v1: the causal MelGAN v1 (512 channels, scales [8, 8, 2, 2], 3 stacks; CausalMelGANStream);
 * mb_melgan_v2: the causal multi-band MelGAN v2 (384 channels, scales [8, 4, 2], 4 stacks, 4-band PQMF), 256 output
   samples per frame like the others.
 
-PWG and HiFi-GAN stream a 256-frame utterance (65536 samples per item), the centred HiFi-GAN then flushes; the MelGANs
+PWG and HiFi-GAN stream a 256-frame utterance (65536 samples per item), the centred ones then flush; the MelGANs
 stream a 263-frame one, a 7-frame opening push (their min_first_frames) then 256 frames, and flush.  Each configuration streams its utterance PASSES
 times.  A push is timed with CUDA events recorded around it and a synchronise after it, so a latency includes the
 host's launch work whenever the GPU waits for it.  Reported: median / min / max latency of the chunk pushes, the
@@ -20,9 +21,10 @@ synthesis) for comparison.
 
 Every timed stream is checked against ``model.inference`` of each item in the same run:
 
-* pwg: bit for bit while a push has at most 65536 samples in all (B x chunk x 256), so that its 64 -> 1 output conv
-  takes conv1d_small_cout_kernel as the per-item inference does; above that the push's output conv takes
-  conv1d_fewcout_long_kernel, which sums in another order, and the check is rel-L2 <= 1e-6;
+* pwg, pwg_centred: bit for bit while a push (for pwg_centred also its 16-frame flush push) has at most 65536 samples
+  in all (B x chunk x 256), so that its 64 -> 1 output conv takes conv1d_small_cout_kernel as the per-item inference
+  does; above that the push's output conv takes conv1d_fewcout_long_kernel, which sums in another order, and the check
+  is rel-L2 <= 1e-6;
 * hifigan, hifigan_centred (after its delay): the per-item inference's 32 -> 1 output conv has 65536 output samples and takes conv1d_fewcout_long_kernel,
   which sums in another order than the generic kernel every stream conv takes, so the check is rel-L2 <= 1e-6 (bit
   identity holds up to 15 frames, tests/test_gpu_hifigan_stream.py);
@@ -47,7 +49,8 @@ import torch.nn.functional as F  # noqa: E402
 from parallelwavegan_b200 import capi, models  # noqa: E402
 from parallelwavegan_b200 import synth_weights as synth  # noqa: E402
 from parallelwavegan_b200.layers import PQMF  # noqa: E402
-from parallelwavegan_b200.streaming import CausalHiFiGANStream, CausalMelGANStream, CausalPWGStream, HiFiGANLookaheadStream  # noqa: E402
+from parallelwavegan_b200.streaming import (CausalHiFiGANStream, CausalMelGANStream, CausalPWGStream, HiFiGANLookaheadStream,  # noqa: E402
+                                            PWGLookaheadStream)
 
 MELGAN = {
     "melgan_v1": dict(in_channels=80, out_channels=1, kernel_size=7, channels=512, upsample_scales=[8, 8, 2, 2], stacks=3,
@@ -55,7 +58,7 @@ MELGAN = {
     "mb_melgan_v2": dict(in_channels=80, out_channels=4, kernel_size=7, channels=384, upsample_scales=[8, 4, 2], stacks=4,
                          use_causal_conv=True),
 }
-MODELS = ("pwg", "hifigan", "hifigan_centred", *MELGAN)
+MODELS = ("pwg", "pwg_centred", "hifigan", "hifigan_centred", *MELGAN)
 FRAMES = 256
 CHUNKS = (1, 4, 16, 64)
 PASSES = 2
@@ -84,6 +87,8 @@ def timed(fn):
 def build(name, dev):
     if name == "pwg":
         m, scale = models.ParallelWaveGANGenerator(use_causal_conv=True), 1.0
+    elif name == "pwg_centred":
+        m, scale = models.ParallelWaveGANGenerator(use_causal_conv=False), 1.0
     elif name == "hifigan":
         m, scale = models.HiFiGANGenerator(use_causal_conv=True), 1.15
     elif name == "hifigan_centred":
@@ -104,17 +109,20 @@ class Workload:
     def __init__(self, name, m, B, dev):
         self.name, self.m = name, m
         self.melgan = name in MELGAN
-        self.flushes = self.melgan or name == "hifigan_centred"
+        self.flushes = self.melgan or name.endswith("_centred")
         self.open = 7 if self.melgan else 0
         self.frames = self.open + FRAMES
         g = torch.Generator().manual_seed(B)
         c = self.c = torch.randn(B, self.frames, 80, generator=g).to(dev)
         cw = c.transpose(1, 2).contiguous()
         self.delay = 0
-        if name == "pwg":
+        if name in ("pwg", "pwg_centred"):
             hop = self.hop = m.upsample_factor
             z = self.z = torch.randn(B, 1, FRAMES * hop, generator=g).to(dev)
             self.ref = torch.stack([m.inference(c=c[b], x=z[b].t()).t() for b in range(B)])
+            if name == "pwg_centred":
+                self.delay = PWGLookaheadStream(m, batch=B, use_graphs=False).delay
+                self.ref = F.pad(self.ref, (self.delay, 0))
             # the inference input: edge-padded by aux_context_window
             acw = m.aux_context_window
             cw = cw[:, :, torch.arange(-acw, FRAMES + acw, device=dev).clamp(0, FRAMES - 1)].contiguous()
@@ -135,17 +143,18 @@ class Workload:
         self.samples = self.ref.shape[-1] - self.delay
 
     def stream(self, B, graphs):
-        cls = {"pwg": CausalPWGStream, "hifigan": CausalHiFiGANStream, "hifigan_centred": HiFiGANLookaheadStream}.get(self.name,
-                                                                                                                 CausalMelGANStream)
+        cls = {"pwg": CausalPWGStream, "pwg_centred": PWGLookaheadStream, "hifigan": CausalHiFiGANStream,
+               "hifigan_centred": HiFiGANLookaheadStream}.get(self.name, CausalMelGANStream)
         return cls(self.m, batch=B, use_graphs=graphs)
 
     def push(self, st, j, n):
-        if self.name == "pwg":
+        if self.name in ("pwg", "pwg_centred"):
             return st.push(self.c[:, j:j + n], self.z[:, :, j * self.hop:(j + n) * self.hop])
         return st.push(self.c[:, j:j + n])
 
     def check(self, s, B, n):
-        if self.name == "pwg" and B * n * self.hop <= 65536:
+        flush_frames = -(-self.delay // self.hop) if self.name == "pwg_centred" else 0
+        if self.name in ("pwg", "pwg_centred") and B * max(n, flush_frames) * self.hop <= 65536:
             assert s["bit_identical_to_inference"], (self.name, B, n)
         else:
             assert s["rel_l2_vs_inference"] <= 1e-6, (self.name, B, n, s["rel_l2_vs_inference"])
