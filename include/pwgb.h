@@ -223,9 +223,20 @@ PWGB_API int pwgb_stream_carry(const void* table, int n_entries, void* stream);
  *     +0.0 (also with accumulate), which is the zero padding the whole-signal conv reads there.  rate >= 1; lookahead >= 0.
  *   delayed residual (res_delay > 0 or res_hist_len > 0): output row t adds row t - res_delay of [res_hist | residual],
  *     res_hist (batch, cout, res_hist_len) fp32; needs a residual and 0 <= res_delay <= res_hist_len.
+ *   edge policy (edge != PWGB_PAD_ZERO; the conv entry points only, with a mask and d->pad_mode == PWGB_PAD_HISTORY):
+ *     input row r in [-hist_len, t_in) is signal sample u = frame[b] * rate - in_lookahead + r (the same rate and end as
+ *     the mask: a stride-1 conv).  A row with u outside [0, end[b] * rate) reads instead the row of [hist | x] that holds
+ *     the reflected sample (edge PWGB_PAD_REFLECT: -u before the start, 2 (L - 1) - u after the end L = end[b] * rate)
+ *     or the replicated one (PWGB_PAD_REPLICATE: 0 or L - 1), and zero when that row lies outside [-hist_len, t_in).  The
+ *     pre-activation applies to it as to any input row.  For a centred conv with padding p over [history (K-1) d |
+ *     chunk], in_lookahead = the input signal's lookahead and output lookahead = in_lookahead - p + (K-1) d, every
+ *     sample such a pad reads for an output inside the signal lies in the launch's window, so every output inside the
+ *     signal is bit-identical to the whole-signal conv with PWGB_PAD_REFLECT / PWGB_PAD_REPLICATE (when that takes the
+ *     same kernel); outputs outside it are masked.  The reflect case needs p < L, as ReflectionPad1d does.
  * Every other value is computed exactly as by the entry point without the extension; with ext == NULL (or all fields
  * zero) the call is that entry point.  A tensor-core launch with an extension keeps the register epilogue (same values
- * as the staged one). */
+ * as the staged one).  edge and in_lookahead were appended to the struct; a zero-initialised struct keeps the meaning it
+ * had before them. */
 typedef struct pwgb_stream_ext {
   const int* frame;
   const int* end;
@@ -234,6 +245,8 @@ typedef struct pwgb_stream_ext {
   const float* res_hist;
   int res_hist_len;
   int res_delay;
+  int edge;
+  int in_lookahead;
 } pwgb_stream_ext;
 PWGB_API int pwgb_conv1d_stream_ext_forward(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len,
                                             const int* replicate, const float* w, const float* bias, const float* residual,
@@ -241,7 +254,7 @@ PWGB_API int pwgb_conv1d_stream_ext_forward(const pwgb_conv1d_desc* d, const flo
 PWGB_API int pwgb_conv1d_tc_stream_ext_forward(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len,
                                                const int* replicate, const void* packed_w, const float* bias,
                                                const float* residual, const pwgb_stream_ext* ext, float* y, void* stream);
-/* pwgb_conv_transpose1d_stream_forward with the mask of ext (no residual fields).  For a centred layer (kernel 2s,
+/* pwgb_conv_transpose1d_stream_forward with the mask of ext (no residual fields, edge 0).  For a centred layer (kernel 2s,
  * padding p) the window of cat(h, x) is whole-signal samples [a * s - p, (a + n) * s - p) when x starts at input sample
  * a and h is sample a - 1 (zero for a fresh slot: pass no replicate flags), so lookahead = s * (input lookahead) + p. */
 PWGB_API int pwgb_conv_transpose1d_stream_ext_forward(const pwgb_convtr1d_desc* d, const float* x, const float* hist,

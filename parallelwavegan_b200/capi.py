@@ -37,6 +37,7 @@ class StreamExt(C.Structure):
     _fields_ = [
         ("frame", C.c_void_p), ("end", C.c_void_p), ("rate", C.c_int32), ("lookahead", C.c_int32),
         ("res_hist", C.c_void_p), ("res_hist_len", C.c_int32), ("res_delay", C.c_int32),
+        ("edge", C.c_int32), ("in_lookahead", C.c_int32),
     ]
 
 

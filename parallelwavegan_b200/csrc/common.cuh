@@ -12,8 +12,9 @@ void set_error(const char* fmt, ...);
 void count_launch(int n = 1);
 // argument check shared by the two history conv entry points (api.cu)
 int conv1d_stream_check(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len, const float* y);
-// argument check of a pwgb_stream_ext (NULL passes); residual: whether the launch has one
-int stream_ext_check(const pwgb_stream_ext* e, const float* residual);
+// argument check of a pwgb_stream_ext (NULL passes); residual: whether the launch has one; pad_mode: the conv's (an edge
+// policy needs PWGB_PAD_HISTORY), -1 for an entry point without an edge policy
+int stream_ext_check(const pwgb_stream_ext* e, const float* residual, int pad_mode = -1);
 
 #define PWGB_CHECK_ARG(cond, ...)          \
   do {                                     \

@@ -59,14 +59,33 @@ struct ConvKExt : ConvK {
   int rhist_len, rdelay;
 };
 
+// The edge policy of an EDGE launch (pwgb_stream_ext.edge != 0): input row r is signal sample mframe[b] * mrate - in_look
+// + r, and a row outside [0, mend[b] * mrate) reads the row holding the reflected (edge PWGB_PAD_REFLECT) or replicated
+// (PWGB_PAD_REPLICATE) sample.
+struct ConvKEdge : ConvKExt {
+  int edge, in_look;
+};
+
+template <bool EXT, bool EDGE>
+using ConvKOf = std::conditional_t<EDGE, ConvKEdge, std::conditional_t<EXT, ConvKExt, ConvK>>;
+
+// The input row of [hist | x] that an EDGE launch reads for row li (outside [-hist_len, Lin) reads zero)
+__device__ __forceinline__ long long edge_row(const ConvKEdge& p, int b, long long li) {
+  const long long u = (long long)__ldg(p.mframe + b) * p.mrate - p.in_look + li;
+  const long long L = (long long)__ldg(p.mend + b) * p.mrate;
+  if (u >= 0 && u < L) return li;
+  const long long v = p.edge == PWGB_PAD_REFLECT ? (u < 0 ? -u : 2 * (L - 1) - u) : (u < 0 ? 0 : L - 1);
+  return li + (v - u);
+}
+
 // HIST: the history padding policy (pwgb_conv1d_stream_forward, groups 1, period 1) in the input staging loop; EXT (with
-// HIST only): the mask and the delayed residual of pwgb_conv1d_stream_ext_forward in the epilogue.  Template arguments so
-// that the kernels without them keep their code and registers.
-template <int RCO, int WARPS_CO, int RT, bool HIST, bool EXT = false>
-__global__ void __launch_bounds__(256) conv1d_fwd_kernel(const std::conditional_t<EXT, ConvKExt, ConvK> p,
-                                                const float* __restrict__ x, const float* __restrict__ w,
-                                                const float* __restrict__ bias, const float* __restrict__ res,
-                                                float* __restrict__ y) {
+// HIST only): the mask and the delayed residual of pwgb_conv1d_stream_ext_forward in the epilogue; EDGE (with EXT): the
+// edge policy in the staging loop.  Template arguments of one body so that the kernels without them keep their code and
+// registers.
+template <int RCO, int WARPS_CO, int RT, bool HIST, bool EXT, bool EDGE>
+__device__ __forceinline__ void conv1d_fwd_body(const ConvKOf<EXT, EDGE> p, const float* __restrict__ x,
+                                                const float* __restrict__ w, const float* __restrict__ bias,
+                                                const float* __restrict__ res, float* __restrict__ y) {
   constexpr int WARPS_T = 8 / WARPS_CO;
   constexpr int CO_T = RCO * WARPS_CO;
   constexpr int TT = WARPS_T * 32 * RT;
@@ -123,6 +142,9 @@ __global__ void __launch_bounds__(256) conv1d_fwd_kernel(const std::conditional_
         // rows and rows past the input zero
         const int ch = ci0 + ci;
         const float* src = nullptr;
+        if constexpr (EDGE) {
+          if (p.edge) li = edge_row(p, b, li);
+        }
         if (li >= 0 && li < p.Lin)
           src = xb + (long long)ch * p.xcs + li;
         else if (li < 0 && li >= -p.hist_len)
@@ -255,6 +277,22 @@ __global__ void __launch_bounds__(256) conv1d_fwd_kernel(const std::conditional_
   }
 }
 
+template <int RCO, int WARPS_CO, int RT, bool HIST, bool EXT = false>
+__global__ void __launch_bounds__(256) conv1d_fwd_kernel(const std::conditional_t<EXT, ConvKExt, ConvK> p,
+                                                const float* __restrict__ x, const float* __restrict__ w,
+                                                const float* __restrict__ bias, const float* __restrict__ res,
+                                                float* __restrict__ y) {
+  conv1d_fwd_body<RCO, WARPS_CO, RT, HIST, EXT, false>(p, x, w, bias, res, y);
+}
+
+// history launches with an edge policy (pwgb_conv1d_stream_ext_forward with edge != 0)
+template <int RCO, int WARPS_CO, int RT>
+__global__ void __launch_bounds__(256) conv1d_fwd_edge_kernel(const ConvKEdge p, const float* __restrict__ x,
+                                                              const float* __restrict__ w, const float* __restrict__ bias,
+                                                              const float* __restrict__ res, float* __restrict__ y) {
+  conv1d_fwd_body<RCO, WARPS_CO, RT, true, true, true>(p, x, w, bias, res, y);
+}
+
 template <int RCO, int WARPS_CO, int RT, bool HIST, bool EXT, class P>
 static int launch_conv_rt(P p, const float* x, const float* w, const float* bias, const float* res, float* y,
                        cudaStream_t st) {
@@ -279,7 +317,12 @@ static int launch_conv_rt(P p, const float* x, const float* w, const float* bias
   p.CI_T = ci_t;
   p.XW = (int)XW;
   p.tiles_per_group = ceil_div(p.Cout_g, CO_T);
-  auto kern = conv1d_fwd_kernel<RCO, WARPS_CO, RT, HIST, EXT>;
+  auto kern = [] {
+    if constexpr (std::is_same<P, ConvKEdge>::value)
+      return conv1d_fwd_edge_kernel<RCO, WARPS_CO, RT>;
+    else
+      return conv1d_fwd_kernel<RCO, WARPS_CO, RT, HIST, EXT>;
+  }();
   if (bytes > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (e != cudaSuccess) {
@@ -528,7 +571,7 @@ int conv1d_forward_simt(const pwgb_conv1d_desc* d, const float* x, const float* 
 int conv1d_stream_simt(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len, const int* rep,
                        const float* w, const float* bias, const float* residual, float* y, cudaStream_t st,
                        const int* zero_flag, int zero_rows, const pwgb_stream_ext* ext) {
-  ConvKExt p;
+  ConvKEdge p;
   conv_params(d, p);
   p.hist = hist;
   p.rep = rep;
@@ -547,12 +590,24 @@ int conv1d_stream_simt(const pwgb_conv1d_desc* d, const float* x, const float* h
     p.rhist_len = ext->res_hist_len;
     p.rdelay = ext->res_delay;
     p.rres = residual;
-    if (cg >= 64) return launch_conv<8, 8, true, true>(p, x, w, bias, nullptr, y, st);
-    if (cg >= 32) return launch_conv<8, 4, true, true>(p, x, w, bias, nullptr, y, st);
-    if (cg >= 16) return launch_conv<8, 2, true, true>(p, x, w, bias, nullptr, y, st);
-    if (cg >= 8) return launch_conv<8, 1, true, true>(p, x, w, bias, nullptr, y, st);
-    if (cg >= 4) return launch_conv<4, 1, true, true>(p, x, w, bias, nullptr, y, st);
-    return launch_conv<1, 1, true, true>(p, x, w, bias, nullptr, y, st);
+    if (ext->edge) {
+      // the EDGE instantiations: only a launch with an edge policy takes them
+      p.edge = ext->edge;
+      p.in_look = ext->in_lookahead;
+      if (cg >= 64) return launch_conv<8, 8, true, true>(p, x, w, bias, nullptr, y, st);
+      if (cg >= 32) return launch_conv<8, 4, true, true>(p, x, w, bias, nullptr, y, st);
+      if (cg >= 16) return launch_conv<8, 2, true, true>(p, x, w, bias, nullptr, y, st);
+      if (cg >= 8) return launch_conv<8, 1, true, true>(p, x, w, bias, nullptr, y, st);
+      if (cg >= 4) return launch_conv<4, 1, true, true>(p, x, w, bias, nullptr, y, st);
+      return launch_conv<1, 1, true, true>(p, x, w, bias, nullptr, y, st);
+    }
+    const ConvKExt& e = p;
+    if (cg >= 64) return launch_conv<8, 8, true, true>(e, x, w, bias, nullptr, y, st);
+    if (cg >= 32) return launch_conv<8, 4, true, true>(e, x, w, bias, nullptr, y, st);
+    if (cg >= 16) return launch_conv<8, 2, true, true>(e, x, w, bias, nullptr, y, st);
+    if (cg >= 8) return launch_conv<8, 1, true, true>(e, x, w, bias, nullptr, y, st);
+    if (cg >= 4) return launch_conv<4, 1, true, true>(e, x, w, bias, nullptr, y, st);
+    return launch_conv<1, 1, true, true>(e, x, w, bias, nullptr, y, st);
   }
   const ConvK& q = p;
   if (cg >= 64) return launch_conv<8, 8, true>(q, x, w, bias, residual, y, st);

@@ -86,6 +86,16 @@ struct TcKExt : TcK {
   long long rhbs;
 };
 
+// The edge policy of an EDGE history launch (conv1d_tc_edge_kernel, pwgb_stream_ext.edge != 0): input row r is signal
+// sample mframe[b] * mrate - in_look + r, and a row outside [0, mend[b] * mrate) reads the row of [hist | x] holding the
+// reflected (edge PWGB_PAD_REFLECT) or replicated (PWGB_PAD_REPLICATE) sample.
+struct TcKEdge : TcKExt {
+  int edge, in_look;
+};
+
+template <bool EXT, bool EDGE>
+using TcKOf = std::conditional_t<EDGE, TcKEdge, std::conditional_t<EXT, TcKExt, TcK>>;
+
 // Staged epilogue: one tile (fp32 [col][stage_ld(MT)], tc_common.cuh) per consumer warpgroup.  Tile shapes compiled with
 // it: at MT = 2 and more than 32 columns it made ptxas spill, and its tiles would not fit beside the pipeline there anyway.
 __host__ __device__ constexpr bool stage_shape(int mt, int cout) { return mt == 1 || cout <= 32; }
@@ -259,11 +269,30 @@ __device__ __forceinline__ const float* hist_sample(const TcK& p, const float* x
   return p.hist + ((long long)b * p.Cin + (long long)c * KC) * p.hist_len + (p.hist_len + ts);
 }
 
+// hist_sample under the edge policy of TcKEdge: the row is first moved to the one holding its reflected or replicated
+// sample, which is then read like any row of [hist | x] (zero outside [-hist_len, T_in))
+__device__ __forceinline__ const float* hist_sample_edge(const TcKEdge& p, const float* xc, int b, int c, int t0, int TT, int r,
+                                                         bool& ok, long long& ld) {
+  long long ts = tile_sample(p, t0, TT, r);
+  if (p.edge) {
+    const long long u = (long long)__ldg(p.mframe + b) * p.mrate - p.in_look + ts;
+    const long long L = (long long)__ldg(p.mend + b) * p.mrate;
+    if (u < 0 || u >= L) ts += (p.edge == PWGB_PAD_REFLECT ? (u < 0 ? -u : 2 * (L - 1) - u) : (u < 0 ? 0 : L - 1)) - u;
+  }
+  ld = p.T_in;
+  ok = ts >= -p.hist_len && ts < p.T_in;
+  if (!ok) return xc;
+  if (ts >= 0) return xc + ts;
+  if (p.rep && p.rep[b]) return p.pad_mode == PWGB_PAD_HISTORY_REFLECT ? xc - ts : xc;
+  ld = p.hist_len;
+  return p.hist + ((long long)b * p.Cin + (long long)c * KC) * p.hist_len + (p.hist_len + ts);
+}
+
 // stage one activation chunk (KC channels x R rows) into the operand layout; HIST: with the history padding policy
-// (chunk c of batch item b)
-template <bool HIST>
-__device__ __forceinline__ void fill_main_chunk(const TcK& p, const float* __restrict__ xc, int t0, int TT,
-                                                unsigned char* dst, int tid, int b, int c) {
+// (chunk c of batch item b); EDGE: with the edge policy as well
+template <bool HIST, bool EDGE = false>
+__device__ __forceinline__ void fill_main_chunk(const std::conditional_t<EDGE, TcKEdge, TcK>& p, const float* __restrict__ xc,
+                                                int t0, int TT, unsigned char* dst, int tid, int b, int c) {
   auto store_row = [&](const float (&v)[KC], int r) {
 #pragma unroll
     for (int g = 0; g < KC / 8; ++g) {
@@ -295,7 +324,11 @@ __device__ __forceinline__ void fill_main_chunk(const TcK& p, const float* __res
     float v[KC];
     if constexpr (HIST) {
       long long ld;
-      const float* s = hist_sample(p, xc, b, c, t0, TT, r, ok, ld);
+      const float* s;
+      if constexpr (EDGE)
+        s = hist_sample_edge(p, xc, b, c, t0, TT, r, ok, ld);
+      else
+        s = hist_sample(p, xc, b, c, t0, TT, r, ok, ld);
 #pragma unroll
       for (int j = 0; j < KC; ++j) v[j] = ok ? __ldg(s + (long long)j * ld) : 0.f;
     } else {
@@ -313,10 +346,10 @@ __device__ __forceinline__ void fill_main_chunk(const TcK& p, const float* __res
 // consumers issue a fixed wgmma sequence into fixed accumulator registers (tc_launch picks the instantiation).  HIST: the
 // history padding policy on the element-addressed producers (cp.async-staged and direct; history launches never take
 // the TMA activation path).  EXT (with HIST only): the mask and the delayed residual of a pwgb_stream_ext launch in the
-// register epilogue, with the parameters of TcKExt.  They are template arguments so that the kernels without them keep
-// their code.
-template <int MT, int NB16, bool HIST, bool EXT = false>
-__device__ __forceinline__ void conv1d_tc_body(const std::conditional_t<EXT, TcKExt, TcK>& p, const float* __restrict__ x, const float* __restrict__ x2,
+// register epilogue, with the parameters of TcKExt.  EDGE (with EXT): the edge policy of TcKEdge in the history
+// producers' row addressing.  They are template arguments so that the kernels without them keep their code.
+template <int MT, int NB16, bool HIST, bool EXT = false, bool EDGE = false>
+__device__ __forceinline__ void conv1d_tc_body(const TcKOf<EXT, EDGE>& p, const float* __restrict__ x, const float* __restrict__ x2,
                                                const uint4* __restrict__ wpk, const float* __restrict__ bias,
                                                const float* __restrict__ res, float* __restrict__ y, float* __restrict__ y2) {
   extern __shared__ __align__(128) unsigned char smem[];
@@ -418,7 +451,11 @@ __device__ __forceinline__ void conv1d_tc_body(const std::conditional_t<EXT, TcK
           bool ok;
           if constexpr (HIST) {
             long long ld;
-            const float* src = hist_sample(p, xc, b, c, t0, TT, r, ok, ld);
+            const float* src;
+            if constexpr (EDGE)
+              src = hist_sample_edge(p, xc, b, c, t0, TT, r, ok, ld);
+            else
+              src = hist_sample(p, xc, b, c, t0, TT, r, ok, ld);
             const unsigned nbytes = ok ? 4u : 0u;
             unsigned dq = raw + (unsigned)r * 4u;
             const unsigned dstep = (unsigned)p.R * 4u;
@@ -482,7 +519,7 @@ __device__ __forceinline__ void conv1d_tc_body(const std::conditional_t<EXT, TcK
         mbar_wait(A_EMPTY(buf), ((ca / p.na) & 1) ^ 1);
         unsigned char* dst = a_buf + (size_t)buf * p.a_bytes;
         if (c < p.nchunks) {
-          fill_main_chunk<HIST>(p, xb + (long long)(c * KC) * p.T_in, t0, TT, dst, tid, b, c);
+          fill_main_chunk<HIST, EDGE>(p, xb + (long long)(c * KC) * p.T_in, t0, TT, dst, tid, b, c);
         } else {
           // auxiliary 1x1 source: TT rows aligned with the output tile, no padding shift, no activation
           const float* xc = x2 + ((long long)b * p.C2 + (long long)(c - p.nchunks) * KC) * p.T_out;
@@ -704,6 +741,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   conv1d_tc_body<MT, NB16, true, true>(p, x, x2, wpk, bias, res, y, y2);
 }
 
+// history launches with a pwgb_stream_ext edge policy (pwgb_conv1d_tc_stream_ext_forward with edge != 0)
+template <int MT, int NB16>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+    conv1d_tc_edge_kernel(const TcKEdge p, const float* __restrict__ x, const float* __restrict__ x2,
+                          const uint4* __restrict__ wpk, const float* __restrict__ bias, const float* __restrict__ res,
+                          float* __restrict__ y, float* __restrict__ y2) {
+  conv1d_tc_body<MT, NB16, true, true, true>(p, x, x2, wpk, bias, res, y, y2);
+}
+
 static int g_tc_variant = 0;
 // the plan of the last conv1d_tc_kernel launch, for pwgb_debug_get(1, ...); the first five fields are the original
 // readout, so a caller that asks for five ints keeps working
@@ -872,6 +918,18 @@ static TcKernelExt tc_ext_kernel_for(int mt, int cout) {
   if (mt == 2 && nb16 >= 1 && nb16 <= 4) return tc_ext_kernels[8 + nb16 - 1];
   return nullptr;
 }
+using TcKernelEdge = void (*)(const TcKEdge, const float*, const float*, const uint4*, const float*, const float*, float*, float*);
+static const TcKernelEdge tc_edge_kernels[12] = {
+    conv1d_tc_edge_kernel<1, 1>, conv1d_tc_edge_kernel<1, 2>, conv1d_tc_edge_kernel<1, 3>, conv1d_tc_edge_kernel<1, 4>,
+    conv1d_tc_edge_kernel<1, 5>, conv1d_tc_edge_kernel<1, 6>, conv1d_tc_edge_kernel<1, 7>, conv1d_tc_edge_kernel<1, 8>,
+    conv1d_tc_edge_kernel<2, 1>, conv1d_tc_edge_kernel<2, 2>, conv1d_tc_edge_kernel<2, 3>, conv1d_tc_edge_kernel<2, 4>};
+static TcKernelEdge tc_edge_kernel_for(int mt, int cout) {
+  if (cout % 16 != 0) return nullptr;
+  const int nb16 = cout / 16;
+  if (mt == 1 && nb16 >= 1 && nb16 <= 8) return tc_edge_kernels[nb16 - 1];
+  if (mt == 2 && nb16 >= 1 && nb16 <= 4) return tc_edge_kernels[8 + nb16 - 1];
+  return nullptr;
+}
 static TcKernel tc_kernel_for(int mt, int cout, bool hist) {
   if (cout % 16 != 0) return nullptr;
   const TcKernel* table = hist ? tc_hist_kernels : tc_kernels;
@@ -881,16 +939,19 @@ static TcKernel tc_kernel_for(int mt, int cout, bool hist) {
   return nullptr;
 }
 
-// P: TcK, or TcKExt for the EXT kernels of a pwgb_stream_ext launch
+// P: TcK, or TcKExt / TcKEdge for the EXT / EDGE kernels of a pwgb_stream_ext launch
 template <class P>
 static int tc_launch(P& p, size_t bytes, const float* x, const void* packed_w, const float* bias,
                      const float* residual, float* y, cudaStream_t st, const float* x2 = nullptr,
                      float* y2 = nullptr) {
   if (p.B == 0 || p.T_out == 0) return PWGB_OK;
   constexpr bool ext = std::is_same<P, TcKExt>::value;
+  constexpr bool edge = std::is_same<P, TcKEdge>::value;
   const bool hist = is_history_pad(p.pad_mode);
-  std::conditional_t<ext, TcKernelExt, TcKernel> kernel;
-  if constexpr (ext)
+  std::conditional_t<edge, TcKernelEdge, std::conditional_t<ext, TcKernelExt, TcKernel>> kernel;
+  if constexpr (edge)
+    kernel = tc_edge_kernel_for(p.MT, p.Cout);
+  else if constexpr (ext)
     kernel = tc_ext_kernel_for(p.MT, p.Cout);
   else
     kernel = tc_kernel_for(p.MT, p.Cout, hist);
@@ -899,7 +960,9 @@ static int tc_launch(P& p, size_t bytes, const float* x, const void* packed_w, c
     return PWGB_UNSUPPORTED;
   }
   static bool smem_set = false, smem_set_hist = false;
-  if constexpr (ext) {
+  if constexpr (edge) {
+    if (const int rc = smem_opt_in(smem_set, tc_edge_kernels, (int)TC_SMEM_STAGED, "conv1d_tc")) return rc;
+  } else if constexpr (ext) {
     if (const int rc = smem_opt_in(smem_set, tc_ext_kernels, (int)TC_SMEM_STAGED, "conv1d_tc")) return rc;
   } else {
     if (const int rc = hist ? smem_opt_in(smem_set_hist, tc_hist_kernels, (int)TC_SMEM_STAGED, "conv1d_tc")
@@ -1114,6 +1177,14 @@ static int tc_forward(const pwgb_conv1d_desc* d, const float* x, const void* pac
   p.hist = hist;
   p.rep = rep;
   p.hist_len = hist_len;
+  if (ext && ext->edge) {
+    TcKEdge px;
+    static_cast<TcK&>(px) = p;
+    tc_apply_ext(px, ext, d->cout);
+    px.edge = ext->edge;
+    px.in_look = ext->in_lookahead;
+    return tc_launch(px, bytes, x, packed_w, bias, residual, y, (cudaStream_t)stream);
+  }
   if (ext) {
     TcKExt px;
     static_cast<TcK&>(px) = p;
@@ -1143,7 +1214,7 @@ extern "C" int pwgb_conv1d_tc_stream_ext_forward(const pwgb_conv1d_desc* d, cons
                                                  const float* residual, const pwgb_stream_ext* ext, float* y, void* stream) {
   PWGB_CHECK_ARG(packed_w, "conv1d_tc_stream: null argument");
   if (const int rc = conv1d_stream_check(d, x, hist, hist_len, y)) return rc;
-  if (const int rc = stream_ext_check(ext, residual)) return rc;
+  if (const int rc = stream_ext_check(ext, residual, d->pad_mode)) return rc;
   return tc_forward(d, x, packed_w, bias, residual, y, stream, hist, replicate, hist_len, ext);
 }
 

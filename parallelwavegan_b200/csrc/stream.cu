@@ -8,8 +8,14 @@ int conv1d_stream_simt(const pwgb_conv1d_desc* d, const float* x, const float* h
                        const float* w, const float* bias, const float* residual, float* y, cudaStream_t st,
                        const int* zero_flag = nullptr, int zero_rows = 0, const pwgb_stream_ext* ext = nullptr);
 
-int stream_ext_check(const pwgb_stream_ext* e, const float* residual) {
+int stream_ext_check(const pwgb_stream_ext* e, const float* residual, int pad_mode) {
   if (!e) return PWGB_OK;
+  PWGB_CHECK_ARG(e->edge == PWGB_PAD_ZERO || e->edge == PWGB_PAD_REFLECT || e->edge == PWGB_PAD_REPLICATE,
+                 "stream_ext: edge must be PWGB_PAD_ZERO, PWGB_PAD_REFLECT or PWGB_PAD_REPLICATE (got %d)", e->edge);
+  PWGB_CHECK_ARG(e->edge == PWGB_PAD_ZERO || pad_mode >= 0, "stream_ext: this entry point has no edge policy (edge must be 0)");
+  PWGB_CHECK_ARG(e->edge == PWGB_PAD_ZERO || e->frame, "stream_ext: an edge policy needs the mask (frame and end)");
+  PWGB_CHECK_ARG(e->edge == PWGB_PAD_ZERO || pad_mode == PWGB_PAD_HISTORY, "stream_ext: an edge policy needs pad_mode PWGB_PAD_HISTORY");
+  PWGB_CHECK_ARG(e->in_lookahead >= 0, "stream_ext: in_lookahead must be >= 0 (got %d)", e->in_lookahead);
   PWGB_CHECK_ARG(!e->frame || (e->end && e->rate >= 1 && e->lookahead >= 0),
                  "stream_ext: a mask needs end flags, rate >= 1 and lookahead >= 0 (rate %d, lookahead %d)", e->rate, e->lookahead);
   PWGB_CHECK_ARG(e->res_hist_len >= 0 && e->res_delay >= 0 && e->res_delay <= e->res_hist_len &&
@@ -108,7 +114,7 @@ extern "C" int pwgb_conv1d_stream_ext_forward(const pwgb_conv1d_desc* d, const f
                                               const pwgb_stream_ext* ext, float* y, void* stream) {
   PWGB_CHECK_ARG(w, "conv1d_stream: null argument");
   if (const int rc = conv1d_stream_check(d, x, hist, hist_len, y)) return rc;
-  if (const int rc = stream_ext_check(ext, residual)) return rc;
+  if (const int rc = stream_ext_check(ext, residual, d->pad_mode)) return rc;
   return conv1d_stream_simt(d, x, hist, hist_len, replicate, w, bias, residual, y, (cudaStream_t)stream, nullptr, 0, ext);
 }
 

@@ -404,10 +404,17 @@ def upsample_fir_causal_stream(x, fir, scale, hist, out=None, out_channels=None,
     return out
 
 
-def _stream_ext(B, cout, mask, res_hist, res_delay):
+_EDGE = {None: capi.PAD_ZERO, "zero": capi.PAD_ZERO, "reflect": capi.PAD_REFLECT, "replicate": capi.PAD_REPLICATE}
+
+
+def _stream_ext(B, cout, mask, res_hist, res_delay, edge=None, in_lookahead=0):
     """The pwgb_stream_ext of a stream launch, or None when it has neither a mask nor a delayed residual"""
     if mask is None and res_hist is None and not res_delay:
+        if edge not in (None, "zero"):
+            raise PwgbError("stream edge: an edge policy needs the mask")
         return None
+    if edge not in _EDGE:
+        raise PwgbError(f"stream edge: edge must be 'reflect', 'replicate', 'zero' or None, got {edge!r}")
     frame, end, rate, lookahead = mask if mask is not None else (None, None, 1, 0)
     for t, name in ((frame, "frame"), (end, "end")):
         if mask is not None and (t.dtype != torch.int32 or not t.is_cuda or t.numel() != B or not t.is_contiguous()):
@@ -419,12 +426,13 @@ def _stream_ext(B, cout, mask, res_hist, res_delay):
             raise PwgbError(f"stream residual: res_hist must be ({B}, {cout}, H), got {tuple(res_hist.shape)}")
         H = res_hist.shape[-1]
     return capi.StreamExt(frame=_p(frame), end=_p(end), rate=int(rate), lookahead=int(lookahead),
-                          res_hist=_p(res_hist) if H else None, res_hist_len=H, res_delay=int(res_delay))
+                          res_hist=_p(res_hist) if H else None, res_hist_len=H, res_delay=int(res_delay), edge=_EDGE[edge],
+                          in_lookahead=int(in_lookahead))
 
 
 def conv1d_stream(x, hist, w, bias=None, *, pad_left, dilation=1, replicate=None, reflect=False, pre_slope=1.0, post_act=None,
                   post_slope=0.0, residual=None, out_scale=1.0, out=None, accumulate=False, t_out=None, mask=None, res_hist=None,
-                  res_delay=0):
+                  res_delay=0, edge=None, in_lookahead=0):
     """conv1d with history padding (pwgb_conv1d_stream_forward / pwgb_conv1d_tc_stream_forward): of the ``pad_left`` rows
     in front of x, the last H read ``hist`` (B, cin, H) -- or x[:, :, 0] for the items whose ``replicate`` (B,) int32 flag
     is set -- and the earlier ones are zero; no right padding.  With ``reflect`` a flagged item reads row -t from x[:, :, t]
@@ -435,7 +443,10 @@ def conv1d_stream(x, hist, w, bias=None, *, pad_left, dilation=1, replicate=None
     The extensions of a lookahead stream (pwgb_*_stream_ext_forward): ``t_out`` fewer output rows than the input allows
     (the later input rows are not read); ``mask`` = (frame, end, rate, lookahead): (B,) int32 device counters, output row
     t of item b is signal sample frame[b] * rate - lookahead + t, stored as +0.0 outside [0, end[b] * rate);
-    ``res_hist`` (B, cout, Hr) / ``res_delay``: row t adds row t - res_delay of [res_hist | residual]."""
+    ``res_hist`` (B, cout, Hr) / ``res_delay``: row t adds row t - res_delay of [res_hist | residual]; ``edge`` ("reflect"
+    or "replicate", with a mask) / ``in_lookahead``: input row r of [hist | x] is signal sample frame[b] * rate -
+    in_lookahead + r, and a row outside [0, end[b] * rate) reads the row holding the reflected or replicated sample, so
+    every output inside the signal equals the whole-signal conv with that pad."""
     x, w = _dev(x, "x"), _dev(w, "w")
     B, cin, L = x.shape
     cout, cin_w, K = w.shape
@@ -447,7 +458,7 @@ def conv1d_stream(x, hist, w, bias=None, *, pad_left, dilation=1, replicate=None
     if replicate is not None and (replicate.dtype != torch.int32 or not replicate.is_cuda or replicate.numel() != B):
         raise PwgbError(f"conv1d_stream: replicate must be {B} int32 flags on the device")
     kw = dict(pad_left=pad_left, dilation=dilation, replicate=replicate, reflect=reflect, pre_slope=pre_slope, post_act=post_act,
-              post_slope=post_slope, t_out=t_out, mask=mask)
+              post_slope=post_slope, t_out=t_out, mask=mask, edge=edge, in_lookahead=in_lookahead)
     if ENGINE != "simt" and cout < 16 and cin >= 256 and cin % 32 == 0 and residual is None and out is None and not accumulate:
         # as _conv1d_fewcout: the weight padded to 16 output channels for the tensor cores
         b16 = torch.nn.functional.pad(bias, (0, 16 - cout)) if bias is not None else None
@@ -467,7 +478,7 @@ def conv1d_stream(x, hist, w, bias=None, *, pad_left, dilation=1, replicate=None
         t_out = t_full
     elif not 0 <= t_out <= t_full:
         raise PwgbError(f"conv1d_stream: t_out {t_out} outside [0, {t_full}]")
-    ext = _stream_ext(B, cout, mask, res_hist, res_delay)
+    ext = _stream_ext(B, cout, mask, res_hist, res_delay, edge, in_lookahead)
     shape = (B, cout, t_out)
     if out is None:
         if accumulate:

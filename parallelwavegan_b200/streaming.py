@@ -1,7 +1,7 @@
 """Chunked synthesis: mel frames in, waveform out, while the frames are still arriving.  ``CausalPWGStream`` streams a
 causal Parallel WaveGAN, ``CausalHiFiGANStream`` a causal HiFi-GAN, ``CausalMelGANStream`` a causal (multi-band) MelGAN,
-and ``HiFiGANLookaheadStream`` and ``PWGLookaheadStream`` a centred HiFi-GAN and a centred Parallel WaveGAN with a fixed
-lookahead and a flush.
+and ``HiFiGANLookaheadStream``, ``PWGLookaheadStream`` and ``MelGANLookaheadStream`` a centred HiFi-GAN, a centred Parallel
+WaveGAN and a centred (multi-band) MelGAN with a fixed lookahead and a flush.
 
 A causal generator's output for frame j depends only on frames <= j, so it can be synthesised as soon as frame j
 exists.  ``CausalPWGStream`` carries, per batch slot, everything the whole-utterance forward would read from before
@@ -803,7 +803,96 @@ class HiFiGANLookaheadStream(_HiFiGANStream):
         return y
 
 
-class CausalMelGANStream(_ChunkStream):
+class _MelGANStream(_ChunkStream):
+    """The levels, stacks, histories and carry table of a streamed ``MelGANGenerator`` (full-band, or multi-band with
+    ``model.pqmf``), shared by the causal stream and the centred one with lookahead.  Both keep, per slot, one history
+    per signal:
+
+    * the input conv: the last kernel_size - 1 mel frames; it runs on [history | chunk];
+    * each conv-transpose: the last frame of its input;
+    * each ResidualStack: its last (k - 1) * d input samples (the two 1x1 convs need none of their own);
+    * the output conv: its last kernel_size - 1 input samples;
+    * with PQMF: the last ceil((taps + 1) / subbands) - 1 subband samples of the synthesis input.
+
+    The dilated convs read their histories in their loaders (pwgb_conv1d_stream_forward / pwgb_conv1d_tc_stream_forward),
+    and one pwgb_stream_carry launch at the end of a push updates every history."""
+
+    def _build(self, model, centred):
+        from .layers import CausalConv1d, CausalConvTranspose1d, ResidualStack
+
+        B, zeros = self.B, self._zeros
+        self.slope = model.slope
+        mods = list(model.melgan)
+        convs = [m for m in mods if isinstance(m, torch.nn.Conv1d if centred else CausalConv1d)]
+        ic, oc = convs[0], convs[-1]
+        self.w_in = wb(ic if centred else ic.conv)
+        self.hop, self.levels = 1, []
+        for m in mods[1:]:
+            if isinstance(m, torch.nn.ConvTranspose1d if centred else CausalConvTranspose1d):
+                if not centred and not isinstance(m.pad, torch.nn.ReplicationPad1d):
+                    raise PwgbError("CausalMelGANStream: only the ReplicationPad1d conv-transpose of MelGANGenerator is supported")
+                deconv = m if centred else m.deconv
+                self.hop *= deconv.stride[0]
+                self.levels.append(dict(stride=deconv.stride[0], channels=deconv.out_channels, w=wb(deconv),
+                                        up_hist=zeros(B, deconv.in_channels, 1), rate=self.hop, stacks=[]))
+            elif isinstance(m, ResidualStack):
+                k, d = m.kernel_size, m.dilation
+                C = m.skip_layer.in_channels
+                c1, c2 = (m.stack[2], m.stack[4]) if centred else (m.stack[1].conv, m.stack[3])
+                self.levels[-1]["stacks"].append(dict(k=k, d=d, w1=wb(c1), w2=wb(c2), ws=wb(m.skip_layer), hist=zeros(B, C, (k - 1) * d)))
+        oconv = oc if centred else oc.conv
+        self.w_out = wb(oconv)
+        self.out_hist = zeros(B, oconv.in_channels, oconv.kernel_size[0] - 1)
+        self.out_channels = oconv.out_channels
+        self.post_act = "tanh" if model.use_final_nonlinear_activation else None
+        pq = model.pqmf
+        if pq is not None:
+            N = pq.subbands
+            if self.out_channels != N:
+                raise PwgbError(f"{type(self).__name__}: {self.out_channels} output channels for a {N}-band PQMF")
+            # PQMF.synthesis's transposed FIR, computed as there; its window lags its input by taps // 2 samples
+            self.w_syn = (pq.synthesis_filter[0].flip(-1) * float(N)).unsqueeze(1).contiguous()
+            self.subbands, self.pq_pad = N, pq.taps // 2
+            self.pq_hist = zeros(B, N, -(-(pq.taps + 1) // N) - 1)
+        else:
+            self.subbands, self.pq_hist = 1, None
+
+    # ---------------------------------------------------------------------------------------------------- state
+    def _histories(self):
+        hs = [self.cin_hist, self.out_hist]
+        for lv in self.levels:
+            hs += [lv["up_hist"]] + [st["hist"] for st in lv["stacks"]]
+        return hs + ([self.pq_hist] if self.pq_hist is not None else [])
+
+    # ---------------------------------------------------------------------------------------------------- compute
+    def _new_entry(self, n, xin):
+        """The buffers of every intermediate signal of an n-frame chunk, and the carry table over them."""
+        dev, B, empty = self.dev, self.B, self._empty
+        ent = dict(h0=empty(B, self.levels[0]["w"][0].shape[0], n), levels=[])
+        entries = [(xin, self.cin_hist)]
+        t, prev = n, ent["h0"]
+        for lv in self.levels:
+            t *= lv["stride"]
+            C = lv["channels"]
+            buf = dict(u=empty(B, C, t), h=empty(B, C, t), s=empty(B, C, t), x=[empty(B, C, t) for _ in lv["stacks"]])
+            entries.append((prev, lv["up_hist"]))
+            x = buf["u"]
+            for j, st in enumerate(lv["stacks"]):
+                entries.append((x, st["hist"]))
+                x = buf["x"][j]
+            ent["levels"].append(buf)
+            prev = x
+        entries.append((prev, self.out_hist))
+        ent["y"] = empty(B, self.out_channels, t)
+        if self.pq_hist is not None:
+            entries.append((ent["y"], self.pq_hist))
+            ent["wave"] = empty(B, 1, t * self.subbands)
+        # every history is read before this one carry, at the end of the push
+        ent["table"] = ops.stream_carry_table(entries, dev)
+        return ent
+
+
+class CausalMelGANStream(_MelGANStream):
     """Streams a causal ``MelGANGenerator`` (``use_causal_conv=True``), full-band or multi-band with ``model.pqmf``, chunk
     by chunk for ``batch`` independent slots.
 
@@ -834,7 +923,7 @@ class CausalMelGANStream(_ChunkStream):
     when the stream is built and must not change while it is used."""
 
     def __init__(self, model, batch=1, use_graphs=True):
-        from .layers import CausalConv1d, CausalConvTranspose1d, ResidualStack
+        from .layers import CausalConv1d
         from .models import MelGANGenerator
 
         if not isinstance(model, MelGANGenerator):
@@ -844,53 +933,21 @@ class CausalMelGANStream(_ChunkStream):
             raise PwgbError("CausalMelGANStream: the model is not causal (use_causal_conv=False); a centred model needs lookahead")
         ic = mods[0]
         self._setup(model, batch, use_graphs, ic.conv.in_channels, ic.left, model.pad_mode, flags=True)
-        B, zeros = self.B, self._zeros
-        self.slope = model.slope
-        self.w_in = wb(ic.conv)
-        reflect_need = [(ic.left, 1)]  # (left padding, input samples per frame) of every conv the pad applies to
-        self.hop, self.levels, oc = 1, [], None
-        for m in mods[1:]:
-            if isinstance(m, CausalConvTranspose1d):
-                if not isinstance(m.pad, torch.nn.ReplicationPad1d):
-                    raise PwgbError("CausalMelGANStream: only the ReplicationPad1d conv-transpose of MelGANGenerator is supported")
-                self.hop *= m.stride
-                self.levels.append(dict(stride=m.stride, channels=m.deconv.out_channels, w=wb(m.deconv),
-                                        up_hist=zeros(B, m.deconv.in_channels, 1), rate=self.hop, stacks=[]))
-            elif isinstance(m, ResidualStack):
-                k, d = m.kernel_size, m.dilation
-                C = m.skip_layer.in_channels
-                self.levels[-1]["stacks"].append(dict(k=k, d=d, w1=wb(m.stack[1].conv), w2=wb(m.stack[3]), ws=wb(m.skip_layer),
-                                                      hist=zeros(B, C, (k - 1) * d)))
-                reflect_need.append(((k - 1) * d, self.hop))
-            elif isinstance(m, CausalConv1d):
-                oc = m
-        self.w_out = wb(oc.conv)
-        self.out_hist = zeros(B, oc.conv.in_channels, oc.left)
-        self.out_channels = oc.conv.out_channels
-        self.post_act = "tanh" if model.use_final_nonlinear_activation else None
-        reflect_need.append((oc.left, self.hop))
+        self._build(model, centred=False)
+        # (left padding, input samples per frame) of every conv the pad applies to
+        reflect_need = [(ic.left, 1)] + [((st["k"] - 1) * st["d"], lv["rate"]) for lv in self.levels for st in lv["stacks"]]
+        reflect_need.append((self.out_hist.shape[-1], self.hop))
         # the smallest first push after a reset for which every reflected row lies inside the chunk
         self.min_first_frames = max(P // rate + 1 for P, rate in reflect_need) if self.pad == "reflect" else 1
-        pq = model.pqmf
-        if pq is not None:
-            N = pq.subbands
-            if self.out_channels != N:
-                raise PwgbError(f"CausalMelGANStream: {self.out_channels} output channels for a {N}-band PQMF")
-            # PQMF.synthesis's transposed FIR, computed as there
-            self.w_syn = (pq.synthesis_filter[0].flip(-1) * float(N)).unsqueeze(1).contiguous()
-            self.subbands, self.delay = N, pq.taps // 2
-            self.pq_hist = zeros(B, N, -(-(pq.taps + 1) // N) - 1)
+        if self.pq_hist is not None:
+            self.delay = self.pq_pad
             # a fresh slot's first window also holds the delay's zeros before sample 0
-            self.min_first_frames = max(self.min_first_frames, -(-self.delay // (self.hop * N)))
+            self.min_first_frames = max(self.min_first_frames, -(-self.delay // (self.hop * self.subbands)))
         else:
-            self.subbands, self.delay, self.pq_hist = 1, 0, None
+            self.delay = 0
 
-    # ---------------------------------------------------------------------------------------------------- state
     def _state(self):
-        hs = [self.cin_hist, self.out_hist]
-        for lv in self.levels:
-            hs += [lv["up_hist"]] + [st["hist"] for st in lv["stacks"]]
-        return hs + ([self.pq_hist] if self.pq_hist is not None else [])
+        return self._histories()
 
     # ---------------------------------------------------------------------------------------------------- compute
     def _pad_kw(self, P, rate, n):
@@ -901,32 +958,6 @@ class CausalMelGANStream(_ChunkStream):
             # a chunk too short to reflect in never holds a fresh slot (push refuses it)
             return dict(replicate=self.fresh, reflect=True)
         return {}
-
-    def _new_entry(self, n, xin):
-        """The buffers of every intermediate signal of an n-frame chunk, and the carry table over them."""
-        dev, B, empty = self.dev, self.B, self._empty
-        ent = dict(h0=empty(B, self.levels[0]["w"][0].shape[0], n), levels=[])
-        entries = [(xin, self.cin_hist)]
-        t, prev = n, ent["h0"]
-        for lv in self.levels:
-            t *= lv["stride"]
-            C = lv["channels"]
-            buf = dict(u=empty(B, C, t), h=empty(B, C, t), s=empty(B, C, t), x=[empty(B, C, t) for _ in lv["stacks"]])
-            entries.append((prev, lv["up_hist"]))
-            x = buf["u"]
-            for j, st in enumerate(lv["stacks"]):
-                entries.append((x, st["hist"]))
-                x = buf["x"][j]
-            ent["levels"].append(buf)
-            prev = x
-        entries.append((prev, self.out_hist))
-        ent["y"] = empty(B, self.out_channels, t)
-        if self.pq_hist is not None:
-            entries.append((ent["y"], self.pq_hist))
-            ent["wave"] = empty(B, 1, t * self.subbands)
-        # every history is read before this one carry, at the end of the push
-        ent["table"] = ops.stream_carry_table(entries, dev)
-        return ent
 
     def _step(self, c):
         """One chunk: c (B, in_channels, n) -> (B, 1, n * hop * subbands).  Advances the state."""
@@ -982,5 +1013,150 @@ class CausalMelGANStream(_ChunkStream):
             y = ops.conv_transpose1d_window_stream(None, self.pq_hist, self.w_syn, None, stride=self.subbands, padding=self.delay,
                                                    fresh=self.fresh, flush_rows=rows)
             y = y[list(items), :, :self.delay].contiguous()
+        self.reset(items)
+        return y
+
+
+class MelGANLookaheadStream(_MelGANStream):
+    """Streams a centred ``MelGANGenerator`` (``use_causal_conv=False``, the published checkpoints), full-band or
+    multi-band with ``model.pqmf``, chunk by chunk for ``batch`` independent slots, with a fixed lookahead of ``delay``
+    output samples.
+
+    ``push(c)`` takes the next n >= 1 mel frames of every slot and returns n * hop * subbands samples: the whole-utterance
+    samples from t0 * hop * subbands - delay on (t0: the frames pushed before), with zeros before sample 0.
+    ``flush(items)`` returns the last ``delay`` samples of those slots and restarts them; the other slots continue as if
+    no flush had happened.  For every slot, the concatenated pushes and flush equal ``[zeros(delay) |
+    model.inference(all_frames)]``.
+
+    Each signal runs in delayed time behind the frames pushed, as in ``HiFiGANLookaheadStream`` (DESIGN.md §3.10,
+    oracle/ref_melgan_lookahead_stream.py): every conv is a history conv on [history | chunk] whose output is labelled
+    its padding earlier, and every launch masks the samples outside its signal to +0.0 (pwgb_stream_ext), the zero padding
+    the conv-transposes and the PQMF synthesis read.  The model's pad (reflect, replicate or zero ``ConstantPad1d``) sits
+    at both ends of every signal a ResidualStack, the input conv or the output conv reads; those convs take the stream
+    edge policy instead (pwgb_stream_ext.edge): an input row outside the signal reads the row of [history | chunk] that
+    holds its reflected or replicated sample, which for every output inside the signal is in the window.  The lookaheads:
+    (K - 1) / 2 frames after the input conv; s * look + s // 2 + s % 2 after a conv-transpose; + (k - 1) / 2 * d after a
+    ResidualStack, whose 1x1 skip reads the stack input that many rows back from the stack's history; + (K - 1) / 2 after
+    the output conv; with PQMF ``delay`` = subbands * look + taps // 2.  1425 samples for MelGAN v1, 2719 for multi-band
+    MelGAN v2 ([8, 4, 2]).
+
+    ``ReflectionPad1d`` needs its padding below the signal's length, so ``inference`` needs ``min_frames`` frames (4 for
+    the recipes' [8, 8, 2, 2] and [8, 4, 2] models, 6 for [5, 5, 3]; 1 for the other pads), and ``flush`` refuses a slot
+    with fewer.  With ``use_graphs`` each chunk length is captured once into a CUDA graph and replayed.  The weights are
+    read when the stream is built and must not change while it is used."""
+
+    OPEN = 2 ** 31 - 1  # the end frame of a slot whose signal has not ended
+
+    def __init__(self, model, batch=1, use_graphs=True):
+        from .layers import CausalConv1d
+        from .models import MelGANGenerator
+
+        if not isinstance(model, MelGANGenerator):
+            raise PwgbError("MelGANLookaheadStream: expected a MelGANGenerator")
+        mods = list(model.melgan)
+        if isinstance(mods[0], CausalConv1d):
+            raise PwgbError("MelGANLookaheadStream: the model is causal (use_causal_conv=True); stream it with CausalMelGANStream, "
+                            "which has no lookahead")
+        ic = mods[1]
+        # a fresh slot's input-conv history stays zero: those frames lie before the signal, where the edge policy reads
+        self._setup(model, batch, use_graphs, ic.in_channels, ic.kernel_size[0] - 1, "zero")
+        self._build(model, centred=True)
+        self.edge = model.pad_mode
+        # the plan: lookahead of each signal, in its own samples
+        K_out = self.out_hist.shape[-1] + 1
+        look = self.look_in = (ic.kernel_size[0] - 1) // 2
+        need = [(look, 1)]  # (padding, input samples per frame) of every conv the pad applies to
+        for lv in self.levels:
+            s = lv["stride"]
+            look = lv["look_u"] = look * s + s // 2 + s % 2
+            for st in lv["stacks"]:
+                st["P"] = (st["k"] - 1) // 2 * st["d"]
+                st["look"] = look
+                look += st["P"]
+                need.append((st["P"], lv["rate"]))
+        self.look_last = look
+        self.look_sub = look + (K_out - 1) // 2
+        need.append(((K_out - 1) // 2, self.hop))
+        self.min_frames = max(P // rate + 1 for P, rate in need) if self.edge == "reflect" else 1
+        self.delay = self.subbands * self.look_sub + self.pq_pad if self.pq_hist is not None else self.look_sub
+        self.frame = torch.zeros(self.B, device=self.dev, dtype=torch.int32)
+        self.end = torch.full((self.B,), self.OPEN, device=self.dev, dtype=torch.int32)
+        self._count = [0] * self.B  # frames pushed per slot, on the host
+
+    def _state(self):
+        return self._histories() + [self.frame, self.end]
+
+    def reset(self, items=None):
+        super().reset(items)
+        for b in self._slots(items):
+            self.end[b] = self.OPEN
+            self._count[b] = 0
+
+    def _mask(self, rate, look):
+        return (self.frame, self.end, rate, look)
+
+    def _step(self, c):
+        """One chunk: c (B, in_channels, n) -> (B, out_channels or 1, n * hop * subbands).  Advances the state."""
+        n = c.shape[-1]
+        ent = self._entry(n)
+        slope, edge = self.slope, self.edge
+        xin = self._input(ent, c)
+        # the input conv on [history | chunk]: input row r is frame t0 - (K - 1) + r
+        h = ops.conv1d_stream(xin, None, *self.w_in, pad_left=0, out=ent["h0"], mask=self._mask(1, self.look_in), edge=edge,
+                              in_lookahead=xin.shape[-1] - n)
+        for lv, buf in zip(self.levels, ent["levels"]):
+            rate = lv["rate"]
+            x = ops.conv_transpose1d_stream(h, lv["up_hist"], lv["w"][0], lv["w"][1], stride=lv["stride"], pre_slope=slope,
+                                            out=buf["u"], mask=self._mask(rate, lv["look_u"]))
+            for j, st in enumerate(lv["stacks"]):
+                P, look, m = st["P"], st["look"], self._mask(rate, st["look"] + st["P"])
+                hh = ops.conv1d_stream(x, st["hist"], *st["w1"], pad_left=(st["k"] - 1) * st["d"], dilation=st["d"], pre_slope=slope,
+                                       out=buf["h"], mask=m, edge=edge, in_lookahead=look)
+                # the skip reads the stack input P rows back, as h lags it
+                s = ops.conv1d_stream(x, st["hist"], *st["ws"], pad_left=P, t_out=x.shape[-1], out=buf["s"])
+                x = ops.conv1d_stream(hh, None, *st["w2"], pad_left=0, pre_slope=slope, residual=s, out=buf["x"][j], mask=m)
+            h = x
+        y = ops.conv1d_stream(h, self.out_hist, *self.w_out, pad_left=self.out_hist.shape[-1], pre_slope=slope, post_act=self.post_act,
+                              out=ent["y"], mask=self._mask(self.hop, self.look_sub), edge=edge, in_lookahead=self.look_last)
+        if self.pq_hist is not None:
+            y = ops.conv_transpose1d_window_stream(y, self.pq_hist, self.w_syn, None, stride=self.subbands, padding=self.pq_pad,
+                                                   out=ent["wave"])
+            ops.stream_mask(y, self._mask(self.hop * self.subbands, self.delay))
+        ops.stream_carry(ent["table"])
+        self.frame += n
+        return y
+
+    @torch.no_grad()
+    def push(self, c, normalize_before=False):
+        """c: (B, n, in_channels) mel frames ((n, in_channels) when batch == 1).  Returns (B, 1, n * hop * subbands) on
+        the device (out_channels rows for a multi-band model without PQMF): samples [t0 * hop * subbands - delay,
+        (t0 + n) * hop * subbands - delay) of each slot's utterance."""
+        c = self._frames(c, normalize_before)
+        self._start(c)
+        n = c.shape[-1]
+        y = self._run(n, c)
+        self._count = [k + n for k in self._count]
+        return y
+
+    @torch.no_grad()
+    def flush(self, items=None):
+        """The last ``delay`` samples of slots ``items`` (an index, an iterable of indices or None for every slot), as
+        (len(items), 1, delay); the slots are then reset.  The flush push covers ceil(delay / (hop * subbands)) zero frames
+        with the slots' end frames set, so every conv reads its pad about the signal's last sample.  The other slots'
+        state is restored around it, so they continue exactly as if it had not happened; ending one slot costs a batch
+        push (DESIGN.md §3.10).  A slot with fewer than ``min_frames`` frames raises, with nothing changed."""
+        items = list(self._slots(items))
+        short = [b for b in items if self._count[b] < self.min_frames]
+        if short:
+            raise PwgbError(f"MelGANLookaheadStream.flush: slots {short} hold fewer than {self.min_frames} frames "
+                            f"({[self._count[b] for b in short]}); inference needs that many for the reflect padding")
+        keep = [b for b in range(self.B) if b not in items]
+        snap = [t[keep].clone() for t in self._state()] if keep else []
+        sel = torch.tensor(items, device=self.dev, dtype=torch.long)
+        self.end[sel] = self.frame[sel]
+        n = -(-self.delay // (self.hop * self.subbands))
+        y = self._run(n, self._zeros(self.B, self.in_channels, n))[sel, :, :self.delay].contiguous()
+        for t, s in zip(self._state(), snap):
+            t[keep] = s
         self.reset(items)
         return y

@@ -7,10 +7,13 @@ for batch sizes B, chunks of 1, 4, 16 and 64 frames, CUDA graphs off and on.  MO
 * pwg_centred: the centred PWG v1 generator (PWGLookaheadStream), hop 256, with its 3920-sample lookahead;
 * melgan_v1: the causal MelGAN v1 (512 channels, scales [8, 8, 2, 2], 3 stacks; CausalMelGANStream);
 * mb_melgan_v2: the causal multi-band MelGAN v2 (384 channels, scales [8, 4, 2], 4 stacks, 4-band PQMF), 256 output
-  samples per frame like the others.
+  samples per frame like the others;
+* melgan_v1_centred, mb_melgan_v2_centred: the same two models centred (MelGANLookaheadStream), with their 1425- and
+  2719-sample lookaheads.
 
 PWG and HiFi-GAN stream a 256-frame utterance (65536 samples per item), the centred ones then flush; the MelGANs
-stream a 263-frame one, a 7-frame opening push (their min_first_frames) then 256 frames, and flush.  Each configuration streams its utterance PASSES
+stream a 263-frame one, a 7-frame opening push (their min_first_frames) then 256 frames, and flush; the centred
+MelGANs stream 256 frames and flush.  Each configuration streams its utterance PASSES
 times.  A push is timed with CUDA events recorded around it and a synchronise after it, so a latency includes the
 host's launch work whenever the GPU waits for it.  Reported: median / min / max latency of the chunk pushes, the
 streamed real-time factor (GPU time of all pushes, and the flush, whose own latency is reported too, over the audio's duration at 22050 Hz: below 1 is
@@ -28,7 +31,7 @@ Every timed stream is checked against ``model.inference`` of each item in the sa
 * hifigan, hifigan_centred (after its delay): the per-item inference's 32 -> 1 output conv has 65536 output samples and takes conv1d_fewcout_long_kernel,
   which sums in another order than the generic kernel every stream conv takes, so the check is rel-L2 <= 1e-6 (bit
   identity holds up to 15 frames, tests/test_gpu_hifigan_stream.py);
-* melgan_v1, mb_melgan_v2: after the PQMF delay, the per-item inference's output conv has 67328 output samples and
+* melgan_v1, mb_melgan_v2 and their centred forms: after the delay, the per-item inference's output conv has 67328 output samples and
   takes conv1d_fewcout_long_kernel too, so the check is rel-L2 <= 1e-6 (bit identity holds below 4096 output-conv
   samples, tests/test_gpu_melgan_stream.py).
 
@@ -50,7 +53,7 @@ from parallelwavegan_b200 import capi, models  # noqa: E402
 from parallelwavegan_b200 import synth_weights as synth  # noqa: E402
 from parallelwavegan_b200.layers import PQMF  # noqa: E402
 from parallelwavegan_b200.streaming import (CausalHiFiGANStream, CausalMelGANStream, CausalPWGStream, HiFiGANLookaheadStream,  # noqa: E402
-                                            PWGLookaheadStream)
+                                            MelGANLookaheadStream, PWGLookaheadStream)
 
 MELGAN = {
     "melgan_v1": dict(in_channels=80, out_channels=1, kernel_size=7, channels=512, upsample_scales=[8, 8, 2, 2], stacks=3,
@@ -58,6 +61,7 @@ MELGAN = {
     "mb_melgan_v2": dict(in_channels=80, out_channels=4, kernel_size=7, channels=384, upsample_scales=[8, 4, 2], stacks=4,
                          use_causal_conv=True),
 }
+MELGAN.update({f"{k}_centred": dict(v, use_causal_conv=False) for k, v in list(MELGAN.items())})
 MODELS = ("pwg", "pwg_centred", "hifigan", "hifigan_centred", *MELGAN)
 FRAMES = 256
 CHUNKS = (1, 4, 16, 64)
@@ -110,7 +114,7 @@ class Workload:
         self.name, self.m = name, m
         self.melgan = name in MELGAN
         self.flushes = self.melgan or name.endswith("_centred")
-        self.open = 7 if self.melgan else 0
+        self.open = 7 if self.melgan and MELGAN[name]["use_causal_conv"] else 0
         self.frames = self.open + FRAMES
         g = torch.Generator().manual_seed(B)
         c = self.c = torch.randn(B, self.frames, 80, generator=g).to(dev)
@@ -135,8 +139,8 @@ class Workload:
             self.ref = F.pad(torch.stack([m.inference(c[b]).t() for b in range(B)]), (self.delay, 0))
             self.whole = lambda: m(cw)
         else:
-            probe = CausalMelGANStream(m, batch=B, use_graphs=False)
-            assert probe.min_first_frames == self.open, probe.min_first_frames
+            probe = self.stream(B, False)
+            assert not self.open or probe.min_first_frames == self.open, probe.min_first_frames
             self.delay = probe.delay
             self.ref = F.pad(torch.stack([m.inference(c[b]).t() for b in range(B)]), (self.delay, 0))
             self.whole = lambda: m.pqmf.synthesis(m(cw)) if m.pqmf is not None else m(cw)
@@ -144,7 +148,9 @@ class Workload:
 
     def stream(self, B, graphs):
         cls = {"pwg": CausalPWGStream, "pwg_centred": PWGLookaheadStream, "hifigan": CausalHiFiGANStream,
-               "hifigan_centred": HiFiGANLookaheadStream}.get(self.name, CausalMelGANStream)
+               "hifigan_centred": HiFiGANLookaheadStream}.get(self.name)
+        if cls is None:
+            cls = CausalMelGANStream if MELGAN[self.name]["use_causal_conv"] else MelGANLookaheadStream
         return cls(self.m, batch=B, use_graphs=graphs)
 
     def push(self, st, j, n):
