@@ -265,6 +265,39 @@ PWGB_API int pwgb_conv_transpose1d_stream_ext_forward(const pwgb_convtr1d_desc* 
  * rate, lookahead as above) is set to +0.0.  ext must hold a mask; its residual fields are ignored. */
 PWGB_API int pwgb_stream_mask(float* y, int batch, int rows, int t, const pwgb_stream_ext* ext, void* stream);
 
+/* The strided convs of a stream (the encoder of a centred U-Net HiFi-GAN).
+ *
+ * pwgb_s2d_stream_forward: pwgb_s2d_forward (groups 1, period 1, pad_left 0) on the window [hist | x] without building it:
+ * x (batch, channels, rows_in), hist (batch, channels, hist_len) -> y (batch, cgo, rows_out), channel r * channels + c
+ * of row u = window row stride * u + r of channel c (zero past the window, and in channels >= stride * channels; cgo 0
+ * means stride * channels).  A stream keeps the window starting on a stride boundary of the whole signal's padded
+ * input, so its rows are the whole-signal gather's and the stride-1 conv that follows (pwgb_conv1d_tc_stream_ext_forward
+ * with the mask) is bit-identical to the whole-signal strided conv's tensor-core route.
+ *
+ * pwgb_conv1d_strided_stream_ext_forward: pwgb_conv1d_stream_ext_forward (FFMA) for a stride >= 1 conv: input rows
+ * [-hist_len, 0) come from hist (pad_left >= hist_len, earlier rows zero), groups 1, period 1, no residual, no edge
+ * policy, d->pad_mode PWGB_PAD_HISTORY; output row o reads input rows o * stride - pad_left + k * dilation.  The mask of
+ * ext applies to the output rows (rate: the output's samples per frame).  Bit-identical to pwgb_conv1d_forward with the
+ * same stride on the explicit window when that takes the generic kernel (not conv1d_small_cout_kernel or
+ * conv1d_fewcout_long_kernel). */
+PWGB_API int pwgb_s2d_stream_forward(const float* x, const float* hist, int hist_len, float* y, int batch, int channels, long long rows_in,
+                                     int stride, long long rows_out, int cgo, void* stream);
+PWGB_API int pwgb_conv1d_strided_stream_ext_forward(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len,
+                                                    const float* w, const float* bias, const pwgb_stream_ext* ext, float* y,
+                                                    void* stream);
+/* The two-source stream conv-transpose of a U-Net decoder level: pwgb_conv_transpose1d_stream_ext_forward on
+ * cat(x1, x2) along channels (d->cin = cin1 + cin2, d->t_in = n + 1 counting the history frame), where each source has
+ * its own history: source 1 is [hist1 (batch, cin1, 1) | x1 (batch, cin1, n)], source 2 is read delay2 rows back from
+ * [hist2 (batch, cin2, hist2_len) | x2 (batch, cin2, n)] (hist2_len >= delay2 + 1), so that its row j is row j - delay2.
+ * One gather launch builds the window in ws, then the single-source stream conv-transpose runs on it (tensor cores or
+ * FFMA as that entry picks); the result is bit-identical to pwgb_conv_transpose1d_cat_forward / the single-source entry
+ * on the explicit windows.  ws: pwgb_conv_transpose1d_cat_stream_workspace(d) bytes. */
+PWGB_API size_t pwgb_conv_transpose1d_cat_stream_workspace(const pwgb_convtr1d_desc* d);
+PWGB_API int pwgb_conv_transpose1d_cat_stream_ext_forward(const pwgb_convtr1d_desc* d, int cin1, const float* x1, const float* hist1,
+                                                          const float* x2, const float* hist2, int hist2_len, int delay2,
+                                                          const float* w, const float* bias, const pwgb_stream_ext* ext, float* y,
+                                                          void* ws, size_t ws_bytes, void* stream);
+
 /* ------------------------------------------------------------------------
  * One HiFi-GAN ResBlock conv pair (layers/residual_block.py:243-258, non-causal, additional convs) in one
  * tensor-core launch; the intermediate stays in shared memory:

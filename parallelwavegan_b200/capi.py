@@ -134,6 +134,15 @@ def lib():
                                                            C.c_size_t, vp]
     L.pwgb_stream_mask.restype = C.c_int
     L.pwgb_stream_mask.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.POINTER(StreamExt), vp]
+    L.pwgb_s2d_stream_forward.restype = C.c_int
+    L.pwgb_s2d_stream_forward.argtypes = [vp, vp, C.c_int, vp, C.c_int, C.c_int, C.c_longlong, C.c_int, C.c_longlong, C.c_int, vp]
+    L.pwgb_conv1d_strided_stream_ext_forward.restype = C.c_int
+    L.pwgb_conv1d_strided_stream_ext_forward.argtypes = [C.POINTER(Conv1dDesc), vp, vp, C.c_int, vp, vp, C.POINTER(StreamExt), vp, vp]
+    L.pwgb_conv_transpose1d_cat_stream_workspace.restype = C.c_size_t
+    L.pwgb_conv_transpose1d_cat_stream_workspace.argtypes = [C.POINTER(ConvTr1dDesc)]
+    L.pwgb_conv_transpose1d_cat_stream_ext_forward.restype = C.c_int
+    L.pwgb_conv_transpose1d_cat_stream_ext_forward.argtypes = [C.POINTER(ConvTr1dDesc), C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp,
+                                                               C.POINTER(StreamExt), vp, vp, C.c_size_t, vp]
     L.pwgb_debug_set.restype = None
     L.pwgb_debug_set.argtypes = [C.c_int, C.c_int]
     L.pwgb_debug_get.restype = C.c_int
@@ -326,6 +335,8 @@ EXPORTED_SYMBOLS = [
     "pwgb_wnstack_supported", "pwgb_wnstack_x_bytes", "pwgb_wnstack_c_bytes", "pwgb_wnstack_pack_x", "pwgb_wnstack_unpack_x",
     "pwgb_wnstack_pack_c", "pwgb_wnstack_first_conv", "pwgb_wnstack_layer_forward", "pwgb_wnstack_carry",
     "pwgb_upsample_fir_causal_stream_forward", "pwgb_upsample_fir_stream_ext_forward", "pwgb_stream_mask",
+    "pwgb_s2d_stream_forward", "pwgb_conv1d_strided_stream_ext_forward", "pwgb_conv_transpose1d_cat_stream_workspace",
+    "pwgb_conv_transpose1d_cat_stream_ext_forward",
     "pwgb_wnstack_first_conv_stream_ext", "pwgb_wnstack_layer_stream_ext_forward",
     "pwgb_mr_stft_loss_workspace", "pwgb_mr_stft_loss_forward", "pwgb_stft_amplitude_forward",
     "pwgb_mel_project_forward", "pwgb_reduce_mean_forward", "pwgb_avg_pool1d_forward",

@@ -37,6 +37,31 @@ __global__ void convtr_weight_kernel(const float* __restrict__ w, float* __restr
   }
 }
 
+// The [history | chunk] window of cat(x1, x2) for a two-source stream conv-transpose: xw (B, cin1 + cin2, n), hw (B,
+// cin1 + cin2, 1).  Source 1 row j is x1 row j (row -1: hist1); source 2 row j is row j - delay2 of [hist2 | x2].
+__global__ void convtr_cat_window_kernel(const float* __restrict__ x1, const float* __restrict__ hist1, const float* __restrict__ x2,
+                                         const float* __restrict__ hist2, int hist2_len, int delay2, float* __restrict__ xw,
+                                         float* __restrict__ hw, int cin1, int cin, int n, long long total) {
+  const int cin2 = cin - cin1;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int j = (int)(i % (n + 1)) - 1;  // row of the chunk, -1 the history frame
+    const long long t = i / (n + 1);
+    const int c = (int)(t % cin);
+    const long long b = t / cin;
+    float v;
+    if (c < cin1) {
+      v = j < 0 ? __ldg(hist1 + b * cin1 + c) : __ldg(x1 + (b * cin1 + c) * n + j);
+    } else {
+      const int c2 = c - cin1, r = j - delay2;
+      v = r >= 0 ? __ldg(x2 + (b * cin2 + c2) * n + r) : __ldg(hist2 + (b * cin2 + c2) * hist2_len + (hist2_len + r));
+    }
+    if (j < 0)
+      hw[b * cin + c] = v;
+    else
+      xw[(b * cin + c) * n + j] = v;
+  }
+}
+
 }  // namespace pwgb
 
 using namespace pwgb;
@@ -251,4 +276,42 @@ extern "C" int pwgb_conv_transpose1d_window_stream_forward(const pwgb_convtr1d_d
   c.shuffle_pad = 0;
   c.shuffle_tout = d->t_out;
   return conv1d_stream_simt(&c, x, hist, hist_len, nullptr, wv, bias, nullptr, y, st, fresh, d->padding);
+}
+
+// the window buffers follow the conv-transpose's own workspace, 256-byte aligned
+static size_t convtr_cat_window_offset(const pwgb_convtr1d_desc* d) { return (pwgb_conv_transpose1d_workspace(d) + 255) / 256 * 256; }
+
+extern "C" size_t pwgb_conv_transpose1d_cat_stream_workspace(const pwgb_convtr1d_desc* d) {
+  if (!d || d->stride <= 0 || d->batch < 0 || d->cin <= 0 || d->t_in <= 0) return 0;
+  return convtr_cat_window_offset(d) + (size_t)d->batch * d->cin * d->t_in * sizeof(float);
+}
+
+extern "C" int pwgb_conv_transpose1d_cat_stream_ext_forward(const pwgb_convtr1d_desc* d, int cin1, const float* x1, const float* hist1,
+                                                            const float* x2, const float* hist2, int hist2_len, int delay2,
+                                                            const float* w, const float* bias, const pwgb_stream_ext* ext, float* y,
+                                                            void* ws, size_t ws_bytes, void* stream) {
+  PWGB_CHECK_ARG(d && x1 && hist1 && x2 && hist2 && w && y, "conv_transpose1d_cat_stream: null argument");
+  const int rc = convtr_desc_ok(d);
+  if (rc) return rc;
+  PWGB_CHECK_ARG(d->t_in >= 2, "conv_transpose1d_cat_stream: t_in counts the history frame and at least one input frame");
+  PWGB_UNSUPPORTED_IF(d->groups > 1 || d->period > 1 || d->padding != d->stride,
+                      "conv_transpose1d_cat_stream: the stream conv-transpose is dense, plain and has padding == stride");
+  PWGB_CHECK_ARG(cin1 > 0 && cin1 < d->cin, "conv_transpose1d_cat_stream: cin1 %d outside (0, %d)", cin1, d->cin);
+  PWGB_CHECK_ARG(delay2 >= 0 && hist2_len >= delay2 + 1, "conv_transpose1d_cat_stream: source 2 needs delay2 + 1 history rows (delay2 %d, "
+                 "hist2_len %d)", delay2, hist2_len);
+  const size_t need = pwgb_conv_transpose1d_cat_stream_workspace(d);
+  PWGB_CHECK_ARG(ws && ws_bytes >= need, "conv_transpose1d_cat_stream: workspace too small (%zu < %zu)", ws_bytes, need);
+  if (const int rc2 = stream_ext_check(ext, nullptr)) return rc2;
+  if (d->batch == 0) return PWGB_OK;
+  const int n = d->t_in - 1;
+  float* xw = (float*)((unsigned char*)ws + convtr_cat_window_offset(d));
+  float* hw = xw + (size_t)d->batch * d->cin * n;
+  const long long total = (long long)d->batch * d->cin * (n + 1);
+  const int blocks = (int)((total + 255) / 256 < 4096 ? (total + 255) / 256 : 4096);
+  convtr_cat_window_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(x1, hist1, x2, hist2, hist2_len, delay2, xw, hw, cin1, d->cin, n,
+                                                                      total);
+  if (const int rc3 = check_launch("convtr_cat_window_kernel")) return rc3;
+  // the single-source stream conv-transpose on the gathered window: pwgb_conv_transpose1d_cat_forward is bit-identical to
+  // the single-source entry on the concatenation, so this is too
+  return convtr_forward(d, xw, nullptr, 0, w, bias, y, ws, pwgb_conv_transpose1d_workspace(d), stream, true, hw, nullptr, ext);
 }

@@ -118,6 +118,27 @@ extern "C" int pwgb_conv1d_stream_ext_forward(const pwgb_conv1d_desc* d, const f
   return conv1d_stream_simt(d, x, hist, hist_len, replicate, w, bias, residual, y, (cudaStream_t)stream, nullptr, 0, ext);
 }
 
+extern "C" int pwgb_conv1d_strided_stream_ext_forward(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len,
+                                                      const float* w, const float* bias, const pwgb_stream_ext* ext, float* y,
+                                                      void* stream) {
+  PWGB_CHECK_ARG(d && x && y && w, "conv1d_strided_stream: null argument");
+  PWGB_CHECK_ARG(d->batch >= 0 && d->cin > 0 && d->cout > 0 && d->t_in > 0 && d->t_out >= 0 && d->kernel > 0 && d->stride > 0 &&
+                     d->dilation > 0 && d->pad_left >= 0,
+                 "conv1d_strided_stream: bad descriptor");
+  PWGB_CHECK_ARG(d->pad_mode == PWGB_PAD_HISTORY, "conv1d_strided_stream: pad_mode must be PWGB_PAD_HISTORY");
+  PWGB_CHECK_ARG(hist_len >= 0 && hist_len <= d->pad_left && (hist_len == 0 || hist), "conv1d_strided_stream: bad history (hist_len %d)",
+                 hist_len);
+  PWGB_UNSUPPORTED_IF(d->groups != 1 || d->period > 1 || d->pre_gate || d->shuffle > 1 || d->accumulate || d->x_batch_stride ||
+                          d->y_batch_stride || d->r_batch_stride || (d->t_valid > 0 && d->t_valid != d->t_in),
+                      "conv1d_strided_stream: plain dense convs only (groups 1, period 1, no pre_gate, no accumulate, one source)");
+  const long long need = (long long)(d->t_out - 1) * d->stride + (long long)(d->kernel - 1) * d->dilation + 1 - d->pad_left;
+  PWGB_CHECK_ARG(d->t_out == 0 || need <= (long long)d->t_in, "conv1d_strided_stream: t_out too large for t_in");
+  if (const int rc = stream_ext_check(ext, nullptr, d->pad_mode)) return rc;
+  PWGB_CHECK_ARG(!ext || ext->edge == PWGB_PAD_ZERO, "conv1d_strided_stream: no edge policy");
+  // the generic FFMA body is written for any stride: the EXT instantiations of pwgb_conv1d_stream_ext_forward serve it
+  return conv1d_stream_simt(d, x, hist, hist_len, nullptr, w, bias, nullptr, y, (cudaStream_t)stream, nullptr, 0, ext);
+}
+
 extern "C" int pwgb_stream_carry(const void* table, int n_entries, void* stream) {
   PWGB_CHECK_ARG(n_entries >= 0 && n_entries <= 65535, "stream_carry: bad entry count %d", n_entries);
   if (n_entries == 0) return PWGB_OK;

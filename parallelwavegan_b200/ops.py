@@ -614,6 +614,104 @@ def conv_transpose1d_window_stream(x, hist, w, bias=None, *, stride, padding, fr
     return y
 
 
+def s2d_stream(x, hist, stride, rows_out, cgo=0, out=None):
+    """The space-to-depth of a stream window [hist | x] (pwgb_s2d_stream_forward): x (B, C, n), hist (B, C, H) -> (B, cgo
+    or stride * C, rows_out), row u holding window rows stride * u .. stride * u + stride - 1; ``s2d_raw`` on the
+    concatenation with no padding, read in place."""
+    x, hist = _dev(x, "x"), _dev(hist, "hist")
+    B, Cc, n = x.shape
+    if hist.dim() != 3 or tuple(hist.shape[:2]) != (B, Cc):
+        raise PwgbError(f"s2d_stream: x {tuple(x.shape)} and hist {tuple(hist.shape)} do not match")
+    co = int(cgo) if cgo else Cc * int(stride)
+    shape = (B, co, int(rows_out))
+    y = torch.empty(shape, device=x.device, dtype=torch.float32) if out is None else out
+    if tuple(y.shape) != shape or not y.is_contiguous() or y.dtype != torch.float32:
+        raise PwgbError(f"s2d_stream: out must be a contiguous float32 {shape} tensor")
+    H = hist.shape[-1]
+    prof = _Prof("s2d_stream", 0.0, 4.0 * (x.numel() + hist.numel() + y.numel()), f"B{B} C{Cc} n{n} H{H} s{stride}")
+    rc = capi.lib().pwgb_s2d_stream_forward(_p(x), _p(hist) if H else None, H, _p(y), B, Cc, n, int(stride), int(rows_out), int(cgo),
+                                            _stream())
+    capi.check(rc, "pwgb_s2d_stream_forward")
+    prof.done()
+    return y
+
+
+def conv1d_strided_stream(x, hist, w, bias=None, *, stride, pad_left, post_act=None, post_slope=0.0, t_out=None, out=None,
+                          mask=None):
+    """A strided history conv on the FFMA engine (pwgb_conv1d_strided_stream_ext_forward): of the ``pad_left`` rows in
+    front of x (B, cin, n), the last H read ``hist`` (B, cin, H) and the earlier ones are zero; output row o reads input
+    rows o * stride - pad_left + k.  ``t_out`` defaults to every row the input allows; ``mask`` as in conv1d_stream.
+    Bit-identical to ``conv1d_raw`` with that stride on the explicit window (the generic FFMA kernel)."""
+    x, w, hist = _dev(x, "x"), _dev(w, "w"), _dev(hist, "hist")
+    B, cin, L = x.shape
+    cout, cin_w, K = w.shape
+    if cin_w != cin or hist.dim() != 3 or tuple(hist.shape[:2]) != (B, cin):
+        raise PwgbError(f"conv1d_strided_stream: x {tuple(x.shape)}, hist {tuple(hist.shape)} and weight {tuple(w.shape)} do not match")
+    t_full = (L + pad_left - K) // stride + 1
+    t_out = t_full if t_out is None else int(t_out)
+    if not 0 <= t_out <= t_full:
+        raise PwgbError(f"conv1d_strided_stream: t_out {t_out} outside [0, {t_full}]")
+    shape = (B, cout, t_out)
+    y = torch.empty(shape, device=x.device, dtype=torch.float32) if out is None else out
+    if tuple(y.shape) != shape or not y.is_contiguous() or y.dtype != torch.float32:
+        raise PwgbError(f"conv1d_strided_stream: out must be a contiguous float32 {shape} tensor")
+    if y.numel() == 0:
+        return y
+    if bias is not None:
+        bias = _dev(bias, "bias")
+    d = capi.Conv1dDesc(batch=B, cin=cin, cout=cout, t_in=L, t_out=t_out, kernel=K, stride=int(stride), dilation=1, groups=1,
+                        pad_left=int(pad_left), pad_mode=capi.PAD_HISTORY, period=1, t_valid=L, pre_slope=1.0, pre_gate=0,
+                        post_act=_ACT[post_act], post_slope=float(post_slope), out_scale=1.0, accumulate=0)
+    ext = _stream_ext(B, cout, mask, None, 0)
+    H = hist.shape[-1]
+    prof = _Prof("conv1d_strided_stream", 2.0 * B * cout * t_out * cin * K, 4.0 * (x.numel() + y.numel()),
+                 f"B{B} cin{cin} cout{cout} k{K} s{stride} T{t_out} H{H}")
+    rc = capi.lib().pwgb_conv1d_strided_stream_ext_forward(C.byref(d), _p(x), _p(hist) if H else None, H, _p(w), _p(bias),
+                                                            C.byref(ext) if ext is not None else None, _p(y), _stream())
+    capi.check(rc, "pwgb_conv1d_strided_stream_ext_forward")
+    prof.done()
+    return y
+
+
+def conv_transpose1d_cat_stream(x1, hist1, x2, hist2, delay2, w, bias=None, *, stride, pre_slope=1.0, out=None, mask=None):
+    """The two-source stream conv-transpose (pwgb_conv_transpose1d_cat_stream_ext_forward): conv_transpose1d_stream on
+    cat(x1, x2) along channels, source 1 with its one-frame history hist1 (B, cin1, 1), source 2 read ``delay2`` rows
+    back from [hist2 (B, cin2, H2 >= delay2 + 1) | x2].  ``mask`` as in conv1d_stream.  Bit-identical to
+    conv_transpose1d_cat_raw(cat(hist1, x1), rows [-(delay2 + 1), n - delay2) of [hist2 | x2], w, bias, stride=stride,
+    padding=stride, pre_slope=pre_slope)."""
+    x1, x2, w = _dev(x1, "x1"), _dev(x2, "x2"), _dev(w, "w")
+    hist1, hist2 = _dev(hist1, "hist1"), _dev(hist2, "hist2")
+    B, cin1, n = x1.shape
+    cin2 = x2.shape[1]
+    if (x2.dim() != 3 or tuple(x2.shape) != (B, cin2, n) or tuple(hist1.shape) != (B, cin1, 1) or hist2.dim() != 3
+            or tuple(hist2.shape[:2]) != (B, cin2) or w.shape[0] != cin1 + cin2):
+        raise PwgbError(f"conv_transpose1d_cat_stream: x1 {tuple(x1.shape)}, hist1 {tuple(hist1.shape)}, x2 {tuple(x2.shape)}, "
+                        f"hist2 {tuple(hist2.shape)} and weight {tuple(w.shape)} do not match")
+    cout, K = w.shape[1], w.shape[2]
+    t_out = n * stride - 2 * stride + K
+    if bias is not None:
+        bias = _dev(bias, "bias")
+    d = capi.ConvTr1dDesc(batch=B, cin=cin1 + cin2, cout=cout, t_in=n + 1, t_out=t_out, kernel=K, stride=stride, padding=stride,
+                          pre_slope=float(pre_slope), groups=1, period=1)
+    lib = capi.lib()
+    nbytes = lib.pwgb_conv_transpose1d_cat_stream_workspace(C.byref(d))
+    ws = torch.empty((nbytes + 3) // 4, device=x1.device, dtype=torch.float32)
+    y = torch.empty((B, cout, t_out), device=x1.device, dtype=torch.float32) if out is None else out
+    if tuple(y.shape) != (B, cout, t_out) or not y.is_contiguous() or y.dtype != torch.float32:
+        raise PwgbError(f"conv_transpose1d_cat_stream: out must be a contiguous float32 {(B, cout, t_out)} tensor")
+    if y.numel() == 0:
+        return y
+    ext = _stream_ext(B, cout, mask, None, 0)
+    prof = _Prof("conv_transpose1d_cat_stream", 2.0 * B * cout * t_out * (cin1 + cin2) * ((K + stride - 1) // stride),
+                 4.0 * (x1.numel() + x2.numel() + y.numel()), f"B{B} cin{cin1}+{cin2} cout{cout} k{K} s{stride} T{t_out} d{delay2}")
+    rc = lib.pwgb_conv_transpose1d_cat_stream_ext_forward(C.byref(d), cin1, _p(x1), _p(hist1), _p(x2), _p(hist2), hist2.shape[-1],
+                                                          int(delay2), _p(w), _p(bias), C.byref(ext) if ext is not None else None,
+                                                          _p(y), _p(ws), C.c_size_t(nbytes), _stream())
+    capi.check(rc, "pwgb_conv_transpose1d_cat_stream_ext_forward")
+    prof.done()
+    return y
+
+
 def stream_mask(y, mask):
     """pwgb_stream_mask: y (B, C, T) contiguous fp32, in place: the samples outside the signal of ``mask`` = (frame, end,
     rate, lookahead) (as in conv1d_stream) become +0.0.  Returns y."""
@@ -1233,6 +1331,23 @@ def s2d_backward_raw(gy, x_shape, groups, stride, pad_left, period=1, cgo=0):
     return gx
 
 
+def s2d_weight(w, stride, cgo):
+    """The weight of the stride-1 conv that follows the space-to-depth of a strided conv: (cout, cin_g, K[, 1]) ->
+    (cout, cgo, ceil(K / stride)[, 1]), taps zero-extended to a multiple of the stride and cgo - stride * cin_g zero
+    input channels appended."""
+    cout, cin_g, K = w.shape[0], w.shape[1], w.shape[2]
+    Kp = (K + stride - 1) // stride
+    w3 = w.reshape(cout, cin_g, K)
+    if Kp * stride != K:
+        w3 = torch.nn.functional.pad(w3, (0, Kp * stride - K))
+    w2 = w3.reshape(cout, cin_g, Kp, stride).permute(0, 3, 1, 2).reshape(cout, stride * cin_g, Kp)
+    if cgo != stride * cin_g:  # zero weight columns for the zero channels the re-layout appends to every group
+        w2 = torch.nn.functional.pad(w2, (0, 0, 0, cgo - stride * cin_g))
+    if w.dim() == 4:
+        w2 = w2.unsqueeze(-1)
+    return w2
+
+
 def _conv1d_s2d(x, w, bias, kw):
     """Strided conv on the tensor-core path: space-to-depth + a stride-1 conv with ceil(K/s) taps and s x the
     input channels (pwgb_s2d_forward).  Returns None when the configuration does not qualify.  The weight
@@ -1265,14 +1380,7 @@ def _conv1d_s2d(x, w, bias, kw):
         return None
     Kp = (K + stride - 1) // stride
     rows_out = t_out + Kp - 1
-    w3 = w.reshape(cout, cin_g, K)
-    if Kp * stride != K:
-        w3 = torch.nn.functional.pad(w3, (0, Kp * stride - K))
-    w2 = w3.reshape(cout, cin_g, Kp, stride).permute(0, 3, 1, 2).reshape(cout, stride * cin_g, Kp)
-    if cgo != stride * cin_g:  # zero weight columns for the zero channels the re-layout appends to every group
-        w2 = torch.nn.functional.pad(w2, (0, 0, 0, cgo - stride * cin_g))
-    if w.dim() == 4:
-        w2 = w2.unsqueeze(-1)
+    w2 = s2d_weight(w, stride, cgo)
     if _needs_grad(x):
         from . import autograd as ag
 

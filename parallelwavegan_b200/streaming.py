@@ -1,7 +1,8 @@
 """Chunked synthesis: mel frames in, waveform out, while the frames are still arriving.  ``CausalPWGStream`` streams a
 causal Parallel WaveGAN, ``CausalHiFiGANStream`` a causal HiFi-GAN, ``CausalMelGANStream`` a causal (multi-band) MelGAN,
-and ``HiFiGANLookaheadStream``, ``PWGLookaheadStream`` and ``MelGANLookaheadStream`` a centred HiFi-GAN, a centred Parallel
-WaveGAN and a centred (multi-band) MelGAN with a fixed lookahead and a flush.
+and ``HiFiGANLookaheadStream``, ``PWGLookaheadStream``, ``MelGANLookaheadStream`` and ``UHiFiGANLookaheadStream`` a centred
+HiFi-GAN, a centred Parallel WaveGAN, a centred (multi-band) MelGAN and a centred U-Net HiFi-GAN (excitation pushed with
+its frames) with a fixed lookahead and a flush.
 
 A causal generator's output for frame j depends only on frames <= j, so it can be synthesised as soon as frame j
 exists.  ``CausalPWGStream`` carries, per batch slot, everything the whole-utterance forward would read from before
@@ -179,6 +180,39 @@ class _ChunkStream:
         return y.clone()
 
 
+class _Lookahead:
+    """The frame / end counters of a stream with a fixed lookahead, shared by the centred streams: the mask of every launch
+    (``_mask``), ``reset`` reopening a slot's end, and ``_flush`` (a push with the flushed slots' end frames set, the other
+    slots' state restored around it, then the flushed slots reset).  Mixed in before the stream's base class."""
+
+    OPEN = 2 ** 31 - 1  # the end frame of a slot whose signal has not ended
+
+    def _counters(self):
+        self.frame = torch.zeros(self.B, device=self.dev, dtype=torch.int32)
+        self.end = torch.full((self.B,), self.OPEN, device=self.dev, dtype=torch.int32)
+
+    def reset(self, items=None):
+        super().reset(items)
+        for b in self._slots(items):
+            self.end[b] = self.OPEN
+
+    def _mask(self, rate, look):
+        return (self.frame, self.end, rate, look)
+
+    def _flush(self, items, inputs):
+        """The first ``delay`` samples of the flush push ``inputs()`` (the arguments of ``_run``) for slots ``items`` (a
+        checked list); the other slots continue exactly as if it had not happened."""
+        keep = [b for b in range(self.B) if b not in items]
+        snap = [t[keep].clone() for t in self._state()] if keep else []
+        sel = torch.tensor(items, device=self.dev, dtype=torch.long)
+        self.end[sel] = self.frame[sel]
+        y = self._run(*inputs())[sel, :, :self.delay].contiguous()
+        for t, s in zip(self._state(), snap):
+            t[keep] = s
+        self.reset(items)
+        return y
+
+
 class CausalPWGStream(_ChunkStream):
     """Streams a causal ``ParallelWaveGANGenerator`` chunk by chunk for ``batch`` independent slots.
 
@@ -298,7 +332,7 @@ class CausalPWGStream(_ChunkStream):
         return self._run(c.shape[-1], z, c)
 
 
-class PWGLookaheadStream(_ChunkStream):
+class PWGLookaheadStream(_Lookahead, _ChunkStream):
     """Streams a centred ``ParallelWaveGANGenerator`` (``use_causal_conv=False``, the published checkpoints) chunk by chunk
     for ``batch`` independent slots, with a fixed lookahead of ``delay`` output samples.
 
@@ -327,8 +361,6 @@ class PWGLookaheadStream(_ChunkStream):
     ``delay`` = look_x + D_L: 3920 samples (15.3 frames) for v1, the lookahead autograd measures on the model.  With
     ``use_graphs`` each chunk length is captured once into a CUDA graph and replayed.  The weights are read when the stream
     is built and must not change while it is used."""
-
-    OPEN = 2 ** 31 - 1  # the end frame of a slot whose signal has not ended
 
     def __init__(self, model, batch=1, seed=None, use_graphs=True):
         from .models import MelGANGenerator, ParallelWaveGANGenerator
@@ -388,8 +420,7 @@ class PWGLookaheadStream(_ChunkStream):
         self.c_hist = self._zeros(B, A, self.W)
         self.skip_hist = self._zeros(B, self.S, self.W)
         self.wn_hist = [torch.zeros((B, self.R * h), device=dev, dtype=torch.int32) for h in self.H]
-        self.frame = torch.zeros(B, device=dev, dtype=torch.int32)
-        self.end = torch.full((B,), self.OPEN, device=dev, dtype=torch.int32)
+        self._counters()
         self._nohist = self._zeros(B, A, 0)
         self.gen = torch.Generator(device=dev)
         if seed is not None:
@@ -397,14 +428,6 @@ class PWGLookaheadStream(_ChunkStream):
 
     def _state(self):
         return [self.cin_hist] + self.fir_hist + [self.z_hist, self.c_hist, self.skip_hist] + self.wn_hist + [self.frame, self.end]
-
-    def reset(self, items=None):
-        super().reset(items)
-        for b in self._slots(items):
-            self.end[b] = self.OPEN
-
-    def _mask(self, rate, look):
-        return (self.frame, self.end, rate, look)
 
     def _new_entry(self, n, xin):
         """The buffers of an n-frame chunk (conditioning stages, the noise, conditioning and skip windows), the packed
@@ -494,20 +517,14 @@ class PWGLookaheadStream(_ChunkStream):
         right edge of ReplicationPad1d) with zero noise, and the end frames mask everything past the signal.  The other
         slots' state is restored around it, so they continue exactly as if it had not happened; ending one slot costs a
         ceil(delay / hop)-frame batch push (DESIGN.md §3.9)."""
-        items = list(self._slots(items))
-        keep = [b for b in range(self.B) if b not in items]
-        snap = [t[keep].clone() for t in self._state()] if keep else []
-        sel = torch.tensor(items, device=self.dev, dtype=torch.long)
-        self.end[sel] = self.frame[sel]
         n = -(-self.delay // self.hop)
         P = self.cin_hist.shape[-1]
-        c = self.cin_hist[:, :, P - 1:].expand(-1, -1, n).contiguous() if P else self._zeros(self.B, self.in_channels, n)
-        z = self._zeros(self.B, self.model.in_channels, n * self.hop)
-        y = self._run(n, z, c)[sel, :, :self.delay].contiguous()
-        for t, s in zip(self._state(), snap):
-            t[keep] = s
-        self.reset(items)
-        return y
+
+        def inputs():
+            c = self.cin_hist[:, :, P - 1:].expand(-1, -1, n).contiguous() if P else self._zeros(self.B, self.in_channels, n)
+            return n, self._zeros(self.B, self.model.in_channels, n * self.hop), c
+
+        return self._flush(list(self._slots(items)), inputs)
 
 
 class _HiFiGANStream(_ChunkStream):
@@ -550,35 +567,8 @@ class _HiFiGANStream(_ChunkStream):
             # the window of cat(h, x) is the centred layer's samples from a * s - padding on
             look = look * s + deconv.padding[0] if centred else 0
             look_u = look
-            blocks = []
-            for j in range(self.nb):
-                blk = m.blocks[i * self.nb + j]
-                k, dils = blk.kernel_size, blk.dilations
-                convs = []
-                for idx, d in enumerate(dils):
-                    c1 = blk.convs1[idx][1] if centred else blk.convs1[idx][1].conv
-                    c2 = (blk.convs2[idx][1] if centred else blk.convs2[idx][1].conv) if blk.use_additional_convs else None
-                    p1 = (k - 1) * d // 2 if centred else 0
-                    q = p1 + ((k - 1) // 2 if c2 is not None and centred else 0)  # the branch's lag behind its input
-                    convs.append(dict(d=d, w1=wb(c1), w2=wb(c2) if c2 is not None else None, p1=p1, q=q,
-                                      # the input of the dilated conv (idx 0: the level input, shared) and of the second conv
-                                      x_hist=zeros(B, cout, (k - 1) * d) if idx > 0 else None,
-                                      xt_hist=zeros(B, cout, k - 1) if c2 is not None else None))
-                blocks.append(dict(k=k, convs=convs, lag=sum(cv["q"] for cv in convs)))
-            # block j reads the level input delta_j samples later, so that every block ends at the same lookahead
-            lag = max(b["lag"] for b in blocks)
-            for b in blocks:
-                b["delta"] = lag - b["lag"]
-                cur = look_u + b["delta"]
-                for idx, cv in enumerate(b["convs"]):
-                    # mask lookaheads of the dilated conv's output and of the block step's output; the residual is the
-                    # step's input, q (and, for the level input, delta_j) rows back
-                    cv["look1"], cv["look2"] = cur + cv["p1"], cur + cv["q"]
-                    cv["rdelay"] = cv["q"] + (b["delta"] if idx == 0 else 0)
-                    cur += cv["q"]
-            look = look_u + lag
-            hl = max(b["delta"] + (b["k"] - 1) * b["convs"][0]["d"] for b in blocks)
-            self.levels.append(dict(stride=s, channels=cout, w=wb(deconv), up_hist=zeros(B, cin, 1), lvl_hist=zeros(B, cout, hl),
+            blocks, lvl_hist, look = self._mrf_level([m.blocks[i * self.nb + j] for j in range(self.nb)], cout, look_u, centred)
+            self.levels.append(dict(stride=s, channels=cout, w=wb(deconv), up_hist=zeros(B, cin, 1), lvl_hist=lvl_hist,
                                     blocks=blocks, rate=self.hop, look_u=look_u))
         oc = m.output_conv[1] if centred else m.output_conv[1].conv
         self.w_out = wb(oc)
@@ -586,6 +576,38 @@ class _HiFiGANStream(_ChunkStream):
         self.out_hist = zeros(B, oc.in_channels, K_out - 1)
         self.out_channels = oc.out_channels
         self.delay = look + (K_out - 1) // 2 if centred else 0
+
+    def _mrf_level(self, blks, cout, look_u, centred):
+        """The block tables of one MRF level (ResidualBlocks ``blks`` on ``cout`` channels) whose input has lookahead
+        ``look_u``: returns (blocks, the level input's history, the lookahead of the MRF's output)."""
+        B, zeros = self.B, self._zeros
+        blocks = []
+        for blk in blks:
+            k, dils = blk.kernel_size, blk.dilations
+            convs = []
+            for idx, d in enumerate(dils):
+                c1 = blk.convs1[idx][1] if centred else blk.convs1[idx][1].conv
+                c2 = (blk.convs2[idx][1] if centred else blk.convs2[idx][1].conv) if blk.use_additional_convs else None
+                p1 = (k - 1) * d // 2 if centred else 0
+                q = p1 + ((k - 1) // 2 if c2 is not None and centred else 0)  # the branch's lag behind its input
+                convs.append(dict(d=d, w1=wb(c1), w2=wb(c2) if c2 is not None else None, p1=p1, q=q,
+                                  # the input of the dilated conv (idx 0: the level input, shared) and of the second conv
+                                  x_hist=zeros(B, cout, (k - 1) * d) if idx > 0 else None,
+                                  xt_hist=zeros(B, cout, k - 1) if c2 is not None else None))
+            blocks.append(dict(k=k, convs=convs, lag=sum(cv["q"] for cv in convs)))
+        # block j reads the level input delta_j samples later, so that every block ends at the same lookahead
+        lag = max(b["lag"] for b in blocks)
+        for b in blocks:
+            b["delta"] = lag - b["lag"]
+            cur = look_u + b["delta"]
+            for idx, cv in enumerate(b["convs"]):
+                # mask lookaheads of the dilated conv's output and of the block step's output; the residual is the
+                # step's input, q (and, for the level input, delta_j) rows back
+                cv["look1"], cv["look2"] = cur + cv["p1"], cur + cv["q"]
+                cv["rdelay"] = cv["q"] + (b["delta"] if idx == 0 else 0)
+                cur += cv["q"]
+        hl = max(b["delta"] + (b["k"] - 1) * b["convs"][0]["d"] for b in blocks)
+        return blocks, zeros(B, cout, hl), look_u + lag
 
     # ---------------------------------------------------------------------------------------------------- state
     def _histories(self):
@@ -597,6 +619,28 @@ class _HiFiGANStream(_ChunkStream):
         return hs
 
     # ---------------------------------------------------------------------------------------------------- compute
+    def _mrf_buffers(self, lv, t, before, after=(), u=None):
+        """The buffers of one MRF level over t samples (``u``: its input, allocated when None) and its carry tables, one
+        per block; the last block's also carries ``before``, the level input and ``after``."""
+        dev, B, empty = self.dev, self.B, self._empty
+        C = lv["channels"]
+        nd = max(len(b["convs"]) for b in lv["blocks"])
+        buf = dict(u=empty(B, C, t) if u is None else u, cs=empty(B, C, t), x=[empty(B, C, t) for _ in range(nd - 1)],
+                   xt=[empty(B, C, t) for _ in range(nd)])
+        tables = []
+        for j, blk in enumerate(lv["blocks"]):
+            entries = []
+            for idx, cv in enumerate(blk["convs"]):
+                if cv["x_hist"] is not None:
+                    entries.append((buf["x"][idx - 1], cv["x_hist"]))
+                if cv["xt_hist"] is not None:
+                    entries.append((buf["xt"][idx], cv["xt_hist"]))
+            if j == len(lv["blocks"]) - 1:
+                entries += list(before) + [(buf["u"], lv["lvl_hist"])] + list(after)
+            tables.append(ops.stream_carry_table(entries, dev))
+        buf["tables"] = tables
+        return buf
+
     def _new_entry(self, n, xin):
         """The buffers of every intermediate signal of an n-frame chunk, and the carry tables over them."""
         dev, B, empty = self.dev, self.B, self._empty
@@ -604,23 +648,9 @@ class _HiFiGANStream(_ChunkStream):
         t, prev = n, ent["h0"]
         for i, lv in enumerate(self.levels):
             t *= lv["stride"]
-            C = lv["channels"]
-            nd = max(len(b["convs"]) for b in lv["blocks"])
-            buf = dict(u=empty(B, C, t), cs=empty(B, C, t), x=[empty(B, C, t) for _ in range(nd - 1)], xt=[empty(B, C, t) for _ in range(nd)])
-            tables = []
-            for j, blk in enumerate(lv["blocks"]):
-                entries = []
-                for idx, cv in enumerate(blk["convs"]):
-                    if cv["x_hist"] is not None:
-                        entries.append((buf["x"][idx - 1], cv["x_hist"]))
-                    if cv["xt_hist"] is not None:
-                        entries.append((buf["xt"][idx], cv["xt_hist"]))
-                if j == len(lv["blocks"]) - 1:  # the level's shared signals, after their last reader
-                    entries += [(prev, lv["up_hist"]), (buf["u"], lv["lvl_hist"])]
-                    if i == 0:
-                        entries.append((xin, self.cin_hist))  # the last frames of [history | chunk] are the chunk's
-                tables.append(ops.stream_carry_table(entries, dev))
-            buf["tables"] = tables
+            # the level's shared signals are carried after their last reader; the last frames of [history | chunk] are
+            # the chunk's
+            buf = self._mrf_buffers(lv, t, [(prev, lv["up_hist"])], [(xin, self.cin_hist)] if i == 0 else [])
             ent["levels"].append(buf)
             prev = buf["cs"]
         ent["y"] = empty(B, self.out_channels, t)
@@ -638,30 +668,33 @@ class _HiFiGANStream(_ChunkStream):
             rate = lv["rate"]
             u = ops.conv_transpose1d_stream(h, lv["up_hist"], lv["w"][0], lv["w"][1], stride=lv["stride"], replicate=replicate,
                                             pre_slope=slope, out=buf["u"], mask=self._mask(rate, lv["look_u"]))
-            t = u.shape[-1]
-            cs = buf["cs"]
-            for j, blk in enumerate(lv["blocks"]):
-                k, convs = blk["k"], blk["convs"]
-                x = u
-                for idx, cv in enumerate(convs):
-                    d = cv["d"]
-                    last = idx == len(convs) - 1
-                    tail = dict(out=cs, accumulate=j > 0, out_scale=1.0 / self.nb) if last else dict(out=buf["x"][idx])
-                    hx = lv["lvl_hist"] if idx == 0 else cv["x_hist"]
-                    # block j's first conv reads the level input delta_j rows early: rows [-(P + delta_j), t - delta_j)
-                    P = (k - 1) * d + (blk["delta"] if idx == 0 else 0)
-                    res = dict(residual=x, res_hist=hx if cv["rdelay"] else None, res_delay=cv["rdelay"])
-                    if cv["w2"] is not None:
-                        xt = ops.conv1d_stream(x, hx, *cv["w1"], pad_left=P, dilation=d, pre_slope=slope, out=buf["xt"][idx], t_out=t,
-                                               mask=self._mask(rate, cv["look1"]))
-                        x = ops.conv1d_stream(xt, cv["xt_hist"], *cv["w2"], pad_left=k - 1, pre_slope=slope,
-                                              mask=self._mask(rate, cv["look2"]), **res, **tail)
-                    else:
-                        x = ops.conv1d_stream(x, hx, *cv["w1"], pad_left=P, dilation=d, pre_slope=slope, t_out=t,
-                                              mask=self._mask(rate, cv["look2"]), **res, **tail)
-                ops.stream_carry(buf["tables"][j])
-            h = cs
+            h = self._mrf(lv, buf, u)
         return h
+
+    def _mrf(self, lv, buf, u):
+        """The MRF blocks of one level on its input u (buf["u"]); returns their average, buf["cs"]"""
+        slope, rate, t, cs = self.slope, lv["rate"], u.shape[-1], buf["cs"]
+        for j, blk in enumerate(lv["blocks"]):
+            k, convs = blk["k"], blk["convs"]
+            x = u
+            for idx, cv in enumerate(convs):
+                d = cv["d"]
+                last = idx == len(convs) - 1
+                tail = dict(out=cs, accumulate=j > 0, out_scale=1.0 / self.nb) if last else dict(out=buf["x"][idx])
+                hx = lv["lvl_hist"] if idx == 0 else cv["x_hist"]
+                # block j's first conv reads the level input delta_j rows early: rows [-(P + delta_j), t - delta_j)
+                P = (k - 1) * d + (blk["delta"] if idx == 0 else 0)
+                res = dict(residual=x, res_hist=hx if cv["rdelay"] else None, res_delay=cv["rdelay"])
+                if cv["w2"] is not None:
+                    xt = ops.conv1d_stream(x, hx, *cv["w1"], pad_left=P, dilation=d, pre_slope=slope, out=buf["xt"][idx], t_out=t,
+                                           mask=self._mask(rate, cv["look1"]))
+                    x = ops.conv1d_stream(xt, cv["xt_hist"], *cv["w2"], pad_left=k - 1, pre_slope=slope,
+                                          mask=self._mask(rate, cv["look2"]), **res, **tail)
+                else:
+                    x = ops.conv1d_stream(x, hx, *cv["w1"], pad_left=P, dilation=d, pre_slope=slope, t_out=t,
+                                          mask=self._mask(rate, cv["look2"]), **res, **tail)
+            ops.stream_carry(buf["tables"][j])
+        return cs
 
     def _output(self, h, ent):
         y = ops.conv1d_stream(h, self.out_hist, *self.w_out, pad_left=self.out_hist.shape[-1], pre_slope=0.01, post_act="tanh",
@@ -713,7 +746,7 @@ class CausalHiFiGANStream(_HiFiGANStream):
         return self._run(c.shape[-1], c)
 
 
-class HiFiGANLookaheadStream(_HiFiGANStream):
+class HiFiGANLookaheadStream(_Lookahead, _HiFiGANStream):
     """Streams a centred ``HiFiGANGenerator`` (``use_causal_conv=False``, the published checkpoints) chunk by chunk for
     ``batch`` independent slots, with a fixed lookahead of ``delay`` output samples.
 
@@ -739,8 +772,6 @@ class HiFiGANLookaheadStream(_HiFiGANStream):
     With ``use_graphs`` each chunk length is captured once into a CUDA graph and replayed.  The weights are read when the
     stream is built and must not change while it is used."""
 
-    OPEN = 2 ** 31 - 1  # the end frame of a slot whose signal has not ended
-
     def __init__(self, model, batch=1, use_graphs=True):
         from .models import HiFiGANGenerator
 
@@ -752,20 +783,11 @@ class HiFiGANLookaheadStream(_HiFiGANStream):
         ic = model.input_conv
         self._setup(model, batch, use_graphs, ic.in_channels, ic.kernel_size[0] - 1, "zero")
         self._build(model, centred=True)
-        self.frame = torch.zeros(self.B, device=self.dev, dtype=torch.int32)
-        self.end = torch.full((self.B,), self.OPEN, device=self.dev, dtype=torch.int32)
+        self._counters()
         self._nohist = self._zeros(self.B, ic.in_channels, 0)
 
     def _state(self):
         return self._histories() + [self.frame, self.end]
-
-    def reset(self, items=None):
-        super().reset(items)
-        for b in self._slots(items):
-            self.end[b] = self.OPEN
-
-    def _mask(self, rate, look):
-        return (self.frame, self.end, rate, look)
 
     def _step(self, c):
         """One chunk: c (B, in_channels, n) -> (B, out_channels, n * hop).  Advances the state."""
@@ -790,17 +812,8 @@ class HiFiGANLookaheadStream(_HiFiGANStream):
         against the zero right padding, as (len(items), out_channels, delay); the slots are then reset.  The other slots'
         state is restored around the flush push, so they continue exactly as if it had not happened.  The flush push covers
         every slot, so ending one slot costs a ceil(delay / hop)-frame batch push (DESIGN.md §3.8)."""
-        items = list(self._slots(items))
-        keep = [b for b in range(self.B) if b not in items]
-        snap = [t[keep].clone() for t in self._state()] if keep else []
-        sel = torch.tensor(items, device=self.dev, dtype=torch.long)
-        self.end[sel] = self.frame[sel]
         n = -(-self.delay // self.hop)
-        y = self._run(n, self._zeros(self.B, self.in_channels, n))[sel, :, :self.delay].contiguous()
-        for t, s in zip(self._state(), snap):
-            t[keep] = s
-        self.reset(items)
-        return y
+        return self._flush(list(self._slots(items)), lambda: (n, self._zeros(self.B, self.in_channels, n)))
 
 
 class _MelGANStream(_ChunkStream):
@@ -1017,7 +1030,7 @@ class CausalMelGANStream(_MelGANStream):
         return y
 
 
-class MelGANLookaheadStream(_MelGANStream):
+class MelGANLookaheadStream(_Lookahead, _MelGANStream):
     """Streams a centred ``MelGANGenerator`` (``use_causal_conv=False``, the published checkpoints), full-band or
     multi-band with ``model.pqmf``, chunk by chunk for ``batch`` independent slots, with a fixed lookahead of ``delay``
     output samples.
@@ -1044,8 +1057,6 @@ class MelGANLookaheadStream(_MelGANStream):
     the recipes' [8, 8, 2, 2] and [8, 4, 2] models, 6 for [5, 5, 3]; 1 for the other pads), and ``flush`` refuses a slot
     with fewer.  With ``use_graphs`` each chunk length is captured once into a CUDA graph and replayed.  The weights are
     read when the stream is built and must not change while it is used."""
-
-    OPEN = 2 ** 31 - 1  # the end frame of a slot whose signal has not ended
 
     def __init__(self, model, batch=1, use_graphs=True):
         from .layers import CausalConv1d
@@ -1079,8 +1090,7 @@ class MelGANLookaheadStream(_MelGANStream):
         need.append(((K_out - 1) // 2, self.hop))
         self.min_frames = max(P // rate + 1 for P, rate in need) if self.edge == "reflect" else 1
         self.delay = self.subbands * self.look_sub + self.pq_pad if self.pq_hist is not None else self.look_sub
-        self.frame = torch.zeros(self.B, device=self.dev, dtype=torch.int32)
-        self.end = torch.full((self.B,), self.OPEN, device=self.dev, dtype=torch.int32)
+        self._counters()
         self._count = [0] * self.B  # frames pushed per slot, on the host
 
     def _state(self):
@@ -1089,11 +1099,7 @@ class MelGANLookaheadStream(_MelGANStream):
     def reset(self, items=None):
         super().reset(items)
         for b in self._slots(items):
-            self.end[b] = self.OPEN
             self._count[b] = 0
-
-    def _mask(self, rate, look):
-        return (self.frame, self.end, rate, look)
 
     def _step(self, c):
         """One chunk: c (B, in_channels, n) -> (B, out_channels or 1, n * hop * subbands).  Advances the state."""
@@ -1150,13 +1156,228 @@ class MelGANLookaheadStream(_MelGANStream):
         if short:
             raise PwgbError(f"MelGANLookaheadStream.flush: slots {short} hold fewer than {self.min_frames} frames "
                             f"({[self._count[b] for b in short]}); inference needs that many for the reflect padding")
-        keep = [b for b in range(self.B) if b not in items]
-        snap = [t[keep].clone() for t in self._state()] if keep else []
-        sel = torch.tensor(items, device=self.dev, dtype=torch.long)
-        self.end[sel] = self.frame[sel]
         n = -(-self.delay // (self.hop * self.subbands))
-        y = self._run(n, self._zeros(self.B, self.in_channels, n))[sel, :, :self.delay].contiguous()
-        for t, s in zip(self._state(), snap):
-            t[keep] = s
-        self.reset(items)
+        return self._flush(items, lambda: (n, self._zeros(self.B, self.in_channels, n)))
+
+
+class UHiFiGANLookaheadStream(_Lookahead, _HiFiGANStream):
+    """Streams a centred ``UHiFiGANGenerator`` (every recipe: opencpop, opensinger, yesno) chunk by chunk for ``batch``
+    independent slots, with a fixed lookahead of ``delay`` output samples.
+
+    ``push(c, excitation)`` takes the next n >= 1 mel frames of every slot and their n * hop excitation samples, and
+    returns n * hop samples: the whole-utterance samples from t0 * hop - delay on (t0: the frames pushed before), with
+    zeros before sample 0.  ``flush(items)`` returns the last ``delay`` samples of those slots and restarts them; the
+    other slots continue as if no flush had happened.  For every slot, the concatenated pushes and flush equal
+    ``[zeros(delay) | model.inference(excitation=all_excitation, c=all_frames)]``.
+
+    Each signal runs in delayed time behind the frames pushed, as in ``HiFiGANLookaheadStream`` (DESIGN.md §3.11,
+    oracle/ref_uhifigan_lookahead_stream.py), and every launch masks the samples outside its signal to +0.0:
+
+    * the encoder: the input conv on [the last K - 1 excitation samples | chunk], then per level the MRF of the HiFi-GAN
+      stream (its block tables, delays and carries, from the level's input) and the strided conv (kernel 2 s, stride s,
+      padding p).  Its output lookahead is the smallest L' for which the push's last output reads only input samples
+      that have arrived, L' = ceil((L + s - p) / s), and it reads a window [the last L' s + p - L input samples | chunk]
+      that starts on a stride boundary of the whole signal's padded input.  It runs as the whole-utterance conv does: the
+      space-to-depth gather reading the history in place (pwgb_s2d_stream_forward) and the masked stride-1 tensor-core
+      conv where ``conv1d`` takes that route, else the masked FFMA strided history conv
+      (pwgb_conv1d_strided_stream_ext_forward);
+    * the bottom: hidden_conv runs at the deepest skip's lookahead, on a history of that many frames plus (K - 1) / 2;
+    * each decoder level: LeakyReLU -> ConvTranspose1d over cat(h, skip), whose two sources have different lookaheads.
+      The skip, which is ahead at every level, is read back by the difference d from a delay line of d + 1 samples by the
+      two-source stream conv-transpose (pwgb_conv_transpose1d_cat_stream_ext_forward); then the MRF.  A model whose
+      decoder state is ahead of its skip is refused;
+    * the output conv as in the HiFi-GAN stream (LeakyReLU 0.01, tanh).
+
+    ``delay`` is the output conv's lookahead: 16231 samples (54.1 frames, 0.68 s at 24 kHz) for the opencpop recipe and
+    5050 (19.7 frames) for yesno's.  It is this large because the bottom level's lag is multiplied by every upsample
+    scale on the way up; it equals the largest lookahead autograd measures over the output phases of a hop (the last
+    frame an output needs, times hop, minus the output's index), so no exact stream can have a smaller one.  With
+    ``use_graphs`` each chunk length is captured once into a CUDA graph and replayed.  The weights and the conv engine
+    (``ops.ENGINE``, which picks each strided conv's route as ``inference`` does) are read when the stream is built and must
+    not change while it is used."""
+
+    def __init__(self, model, batch=1, use_graphs=True):
+        import math
+
+        from .models import UHiFiGANGenerator
+
+        name = "UHiFiGANLookaheadStream"
+        if not isinstance(model, UHiFiGANGenerator):
+            raise PwgbError(f"{name}: expected a UHiFiGANGenerator")
+        self._check_eval(model)
+        if next(model.parameters()).device.type != "cuda":
+            raise PwgbError(f"{name}: the model must live on a CUDA device (no CPU fallback)")
+        if model.use_causal_conv:
+            raise PwgbError(f"{name}: a causal UHiFiGANGenerator cannot be built")
+        if math.prod(model.downsample_scales) != math.prod(model.upsample_scales):
+            raise PwgbError(f"{name}: prod(downsample_scales) {math.prod(model.downsample_scales)} != prod(upsample_scales) "
+                            f"{math.prod(model.upsample_scales)}: a push must give whole samples at every encoder level")
+        for kind, mods in (("downsample", [d[0] for d in model.downsamples]), ("upsample", [u[1] for u in model.upsamples])):
+            for conv in mods:
+                if conv.kernel_size[0] != 2 * conv.stride[0]:
+                    raise PwgbError(f"{name}: a {kind} conv of kernel {conv.kernel_size[0]} and stride {conv.stride[0]}; the stream "
+                                    "needs kernel 2 * stride")
+        hc = model.hidden_conv
+        K = model.kernel_size
+        pk = (K - 1) // 2
+        B = int(batch)
+        self.B = B  # the plan's histories are allocated before _setup, which sizes the mel history from it
+        self.dev = next(model.parameters()).device
+        self.slope, self.nb = model.slope, model.num_blocks
+        self.hop = math.prod(model.upsample_scales)
+        zeros = self._zeros
+        # encoder: the input conv on the excitation, then per level the MRF and the strided conv
+        ic = model.input_conv[0]
+        self.w_in = wb(ic)
+        self.e_hist = zeros(B, 1, K - 1)
+        self.look_in = pk
+        look, rate, self.enc = pk, self.hop, []
+        for i, s in enumerate(model.downsample_scales):
+            conv = model.downsamples[i][0]
+            C = conv.in_channels
+            blocks, lvl_hist, L = self._mrf_level([model.downsamples_mrf[i * self.nb + j] for j in range(self.nb)], C, look, True)
+            p = s // 2 + s % 2
+            Lq = -(-(L + s - p) // s)
+            w, b = wb(conv)
+            cgo = (C * s + 31) // 32 * 32
+            # the whole-utterance conv's route, fixed here: the space-to-depth gather and the stride-1 tensor-core conv
+            # where ops._conv1d_s2d takes them (its channel conditions, the tensor-core engine), else the FFMA strided conv
+            s2d = ops.ENGINE != "simt" and conv.out_channels % 16 == 0 and cgo <= 2 * C * s
+            self.enc.append(dict(stride=s, channels=C, rate=rate, look_u=look, blocks=blocks, lvl_hist=lvl_hist, w=(w, b),
+                                 w2=ops.s2d_weight(w, s, cgo).contiguous() if s2d else None, cgo=cgo, look_d=Lq,
+                                 ds_hist=zeros(B, C, Lq * s + p - L)))
+            rate //= s
+            look = Lq
+        # bottom: the deeper of the mel path and the deepest skip sets the decoder's first lookahead
+        look_h = max(look, pk)
+        self.look_hc = look_h
+        self._setup(model, batch, use_graphs, hc.in_channels, look_h + pk, "zero")
+        self.w_hc = wb(hc)
+        # decoder: cat(h, skip) -> LeakyReLU -> ConvTranspose1d, then the MRF
+        self.levels, rate = [], 1
+        for i, s in enumerate(model.upsample_scales):
+            e = self.enc[-1 - i]
+            up = model.upsamples[i][1]
+            C1 = up.in_channels - 2 * e["channels"]
+            D = max(look_h, e["look_d"])
+            d1, d2 = D - look_h, D - e["look_d"]  # the delay lines of the source ahead
+            if d1:
+                raise PwgbError(f"{name}: decoder level {i}'s skip runs {d1} samples behind its decoder state; the stream reads "
+                                "only the skip through a delay line")
+            rate *= s
+            look_u = D * s + up.padding[0]
+            cout = up.out_channels
+            blocks, lvl_hist, look_h = self._mrf_level([model.upsamples_mrf[i * self.nb + j] for j in range(self.nb)], cout, look_u, True)
+            self.levels.append(dict(stride=s, channels=cout, C1=C1, w=wb(up), rate=rate, look_u=look_u, blocks=blocks,
+                                    lvl_hist=lvl_hist, d1=d1, d2=d2, h1_hist=zeros(B, C1, d1 + 1),
+                                    h2_hist=zeros(B, up.in_channels - C1, d2 + 1)))
+        oc = model.output_conv[1]
+        self.w_out = wb(oc)
+        self.out_hist = zeros(B, oc.in_channels, K - 1)
+        self.out_channels = oc.out_channels
+        self.delay = look_h + pk
+        self._counters()
+        self._nohist = self._zeros(B, hc.in_channels, 0)
+
+    def _state(self):
+        hs = [self.cin_hist, self.out_hist, self.e_hist]
+        for lv in self.enc:
+            hs += [lv["lvl_hist"], lv["ds_hist"]]
+            hs += [h for blk in lv["blocks"] for cv in blk["convs"] for h in (cv["x_hist"], cv["xt_hist"]) if h is not None]
+        for lv in self.levels:
+            hs += [lv["lvl_hist"], lv["h1_hist"], lv["h2_hist"]]
+            hs += [h for blk in lv["blocks"] for cv in blk["convs"] for h in (cv["x_hist"], cv["xt_hist"]) if h is not None]
+        return hs + [self.frame, self.end]
+
+    def _new_entry(self, n, xin):
+        """The buffers of every intermediate signal of an n-frame chunk, and the carry tables over them."""
+        dev, B, empty = self.dev, self.B, self._empty
+        ent = dict(e=empty(B, 1, n * self.hop), enc=[], levels=[])
+        u = empty(B, self.enc[0]["channels"], n * self.hop)
+        misc = [(ent["e"], self.e_hist), (xin, self.cin_hist)]
+        for lv in self.enc:
+            t = n * lv["rate"]
+            buf = self._mrf_buffers(lv, t, [], u=u)
+            s = lv["stride"]
+            if lv["w2"] is not None:
+                buf["xs"] = empty(B, lv["cgo"], t // s + 1)
+            u = buf["d"] = empty(B, 2 * lv["channels"], t // s)
+            misc.append((buf["cs"], lv["ds_hist"]))
+            ent["enc"].append(buf)
+        h = ent["h0"] = empty(B, self.w_hc[0].shape[0], n)
+        t = n
+        for i, lv in enumerate(self.levels):
+            skip = ent["enc"][-1 - i]["d"]
+            buf = self._mrf_buffers(lv, t * lv["stride"], [])
+            misc += [(h, lv["h1_hist"]), (skip, lv["h2_hist"])]
+            ent["levels"].append(buf)
+            t *= lv["stride"]
+            h = buf["cs"]
+        ent["y"] = empty(B, self.out_channels, t)
+        ent["out_table"] = ops.stream_carry_table([(h, self.out_hist)], dev)
+        ent["table"] = ops.stream_carry_table(misc, dev)
+        return ent
+
+    def _strided(self, lv, buf, h):
+        """the level's strided conv on [ds_hist | h], as ``UHiFiGANGenerator.forward`` runs it on the whole signal: the
+        window starts on a stride boundary of the whole signal's padded input, and its outputs are masked"""
+        s, out = lv["stride"], buf["d"]
+        mask = self._mask(lv["rate"] // s, lv["look_d"])
+        if lv["w2"] is not None:
+            xs = ops.s2d_stream(h, lv["ds_hist"], s, out.shape[-1] + 1, lv["cgo"], out=buf["xs"])
+            return ops.conv1d_stream(xs, None, lv["w2"], lv["w"][1], pad_left=0, post_act="lrelu", post_slope=self.slope, out=out,
+                                     mask=mask)
+        return ops.conv1d_strided_stream(h, lv["ds_hist"], *lv["w"], stride=s, pad_left=lv["ds_hist"].shape[-1], post_act="lrelu",
+                                         post_slope=self.slope, t_out=out.shape[-1], out=out, mask=mask)
+
+    def _step(self, c, e):
+        """One chunk: c (B, in_channels, n), e (B, 1, n * hop) -> (B, out_channels, n * hop).  Advances the state."""
+        n = c.shape[-1]
+        ent = self._entry(n)
+        slope = self.slope
+        ent["e"].copy_(e)
+        K = self.e_hist.shape[-1] + 1
+        u = ops.conv1d_stream(ent["e"], self.e_hist, *self.w_in, pad_left=K - 1, post_act="lrelu", post_slope=slope,
+                              out=ent["enc"][0]["u"], mask=self._mask(self.hop, self.look_in))
+        for lv, buf in zip(self.enc, ent["enc"]):
+            u = self._strided(lv, buf, self._mrf(lv, buf, u))
+        # hidden_conv on [the last look_hc + (K - 1) / 2 frames | chunk]: n outputs at the decoder's first lookahead
+        h = ops.conv1d_stream(self._input(ent, c), self._nohist, *self.w_hc, pad_left=0, t_out=n, out=ent["h0"],
+                              mask=self._mask(1, self.look_hc))
+        for i, (lv, buf) in enumerate(zip(self.levels, ent["levels"])):
+            skip = ent["enc"][-1 - i]["d"]
+            # the skip is read d2 samples back from its delay line
+            u = ops.conv_transpose1d_cat_stream(h, lv["h1_hist"], skip, lv["h2_hist"], lv["d2"], *lv["w"], stride=lv["stride"],
+                                                pre_slope=slope, out=buf["u"], mask=self._mask(lv["rate"], lv["look_u"]))
+            h = self._mrf(lv, buf, u)
+        ops.stream_carry(ent["table"])
+        y = self._output(h, ent)
+        self.frame += n
         return y
+
+    @torch.no_grad()
+    def push(self, c, excitation, normalize_before=False):
+        """c: (B, n, in_channels) mel frames ((n, in_channels) when batch == 1); excitation: (B, n * hop) or (B, n, hop)
+        ((n * hop,) or (n, hop) when batch == 1).  ``normalize_before`` normalises c with the model's statistics, as in
+        the other streams.  Returns (B, out_channels, n * hop) on the device: samples [t0 * hop - delay, (t0 + n) * hop
+        - delay) of each slot's utterance."""
+        c = self._frames(c, normalize_before)
+        n = c.shape[-1]
+        e = torch.as_tensor(excitation, dtype=torch.float32, device=self.dev)
+        T = n * self.hop
+        shapes = {(self.B, T), (self.B, n, self.hop)} | ({(T,), (n, self.hop)} if self.B == 1 else set())
+        if tuple(e.shape) not in shapes:
+            raise PwgbError(f"UHiFiGANLookaheadStream.push: excitation must be ({self.B}, {T}) or ({self.B}, {n}, {self.hop}) for "
+                            f"{n} frames, got {tuple(e.shape)}")
+        self._start(c)
+        return self._run(n, c, e.reshape(self.B, 1, T).contiguous())
+
+    @torch.no_grad()
+    def flush(self, items=None):
+        """The last ``delay`` samples of slots ``items`` (an index, an iterable of indices or None for every slot), computed
+        against the zero right padding, as (len(items), out_channels, delay); the slots are then reset.  The flush push
+        covers ceil(delay / hop) zero frames and zero excitation with the slots' end frames set; the other slots' state is
+        restored around it, so they continue exactly as if it had not happened (DESIGN.md §3.11)."""
+        n = -(-self.delay // self.hop)
+        return self._flush(list(self._slots(items)),
+                           lambda: (n, self._zeros(self.B, self.in_channels, n), self._zeros(self.B, 1, n * self.hop)))

@@ -9,7 +9,9 @@ for batch sizes B, chunks of 1, 4, 16 and 64 frames, CUDA graphs off and on.  MO
 * mb_melgan_v2: the causal multi-band MelGAN v2 (384 channels, scales [8, 4, 2], 4 stacks, 4-band PQMF), 256 output
   samples per frame like the others;
 * melgan_v1_centred, mb_melgan_v2_centred: the same two models centred (MelGANLookaheadStream), with their 1425- and
-  2719-sample lookaheads.
+  2719-sample lookaheads;
+* uhifigan_opencpop_centred: the U-Net HiFi-GAN of the opencpop recipe (UHiFiGANLookaheadStream), hop 300 at 24 kHz,
+  excitation pushed with its frames, with its 16231-sample lookahead; 1- and 8-frame chunks.
 
 PWG and HiFi-GAN stream a 256-frame utterance (65536 samples per item), the centred ones then flush; the MelGANs
 stream a 263-frame one, a 7-frame opening push (their min_first_frames) then 256 frames, and flush; the centred
@@ -17,7 +19,7 @@ MelGANs stream 256 frames and flush.  Each configuration streams its utterance P
 times.  A push is timed with CUDA events recorded around it and a synchronise after it, so a latency includes the
 host's launch work whenever the GPU waits for it.  Reported: median / min / max latency of the chunk pushes, the
 streamed real-time factor (GPU time of all pushes, and the flush, whose own latency is reported too, over the audio's duration at 22050 Hz: below 1 is
-faster than real time), the libpwgb kernel launches of one steady-state eager push (the few torch copies are not
+faster than real time; 24000 Hz for the U-Net HiFi-GAN), the libpwgb kernel launches of one steady-state eager push (the few torch copies are not
 counted), the stream's state_bytes() and algorithmic latency (delay plus one chunk, in ms at 22050 Hz), and the
 whole-utterance forward of the same audio (one call on the B utterances; for MB-MelGAN with the PQMF
 synthesis) for comparison.
@@ -33,7 +35,9 @@ Every timed stream is checked against ``model.inference`` of each item in the sa
   identity holds up to 15 frames, tests/test_gpu_hifigan_stream.py);
 * melgan_v1, mb_melgan_v2 and their centred forms: after the delay, the per-item inference's output conv has 67328 output samples and
   takes conv1d_fewcout_long_kernel too, so the check is rel-L2 <= 1e-6 (bit identity holds below 4096 output-conv
-  samples, tests/test_gpu_melgan_stream.py).
+  samples, tests/test_gpu_melgan_stream.py);
+* uhifigan_opencpop_centred: its inference's 32 -> 1 output conv has 76800 samples and takes conv1d_fewcout_long_kernel,
+  so the check is rel-L2 <= 1e-6 (bit identity holds below 4096 samples, tests/test_gpu_uhifigan_lookahead_stream.py).
 
 Prints the card name and power limit of the same run, as one JSON document.
 
@@ -53,7 +57,7 @@ from parallelwavegan_b200 import capi, models  # noqa: E402
 from parallelwavegan_b200 import synth_weights as synth  # noqa: E402
 from parallelwavegan_b200.layers import PQMF  # noqa: E402
 from parallelwavegan_b200.streaming import (CausalHiFiGANStream, CausalMelGANStream, CausalPWGStream, HiFiGANLookaheadStream,  # noqa: E402
-                                            MelGANLookaheadStream, PWGLookaheadStream)
+                                            MelGANLookaheadStream, PWGLookaheadStream, UHiFiGANLookaheadStream)
 
 MELGAN = {
     "melgan_v1": dict(in_channels=80, out_channels=1, kernel_size=7, channels=512, upsample_scales=[8, 8, 2, 2], stacks=3,
@@ -62,11 +66,16 @@ MELGAN = {
                          use_causal_conv=True),
 }
 MELGAN.update({f"{k}_centred": dict(v, use_causal_conv=False) for k, v in list(MELGAN.items())})
-MODELS = ("pwg", "pwg_centred", "hifigan", "hifigan_centred", *MELGAN)
+UHIFIGAN_OPENCPOP = dict(in_channels=80, out_channels=1, channels=32, kernel_size=7, downsample_scales=[5, 5, 4, 3],
+                         downsample_kernel_sizes=[10, 10, 8, 6], upsample_scales=[3, 4, 5, 5], upsample_kernel_sizes=[6, 8, 10, 10],
+                         resblock_kernel_sizes=[3, 7, 11], resblock_dilations=[[1, 3, 5]] * 3)
+MODELS = ("pwg", "pwg_centred", "hifigan", "hifigan_centred", *MELGAN, "uhifigan_opencpop_centred")
 FRAMES = 256
 CHUNKS = (1, 4, 16, 64)
 PASSES = 2
 SR = 22050
+CHUNKS_OF = {"uhifigan_opencpop_centred": (1, 8)}
+SR_OF = {"uhifigan_opencpop_centred": 24000}
 
 
 def card():
@@ -97,6 +106,8 @@ def build(name, dev):
         m, scale = models.HiFiGANGenerator(use_causal_conv=True), 1.15
     elif name == "hifigan_centred":
         m, scale = models.HiFiGANGenerator(use_causal_conv=False), 1.15
+    elif name == "uhifigan_opencpop_centred":
+        m, scale = models.UHiFiGANGenerator(**UHIFIGAN_OPENCPOP), 1.15
     else:
         m, scale = models.MelGANGenerator(**MELGAN[name]), 1.0
     m.load_state_dict(synth.synth_state_dict([(k, tuple(v.shape)) for k, v in m.state_dict().items()], 31, scale))
@@ -119,8 +130,14 @@ class Workload:
         g = torch.Generator().manual_seed(B)
         c = self.c = torch.randn(B, self.frames, 80, generator=g).to(dev)
         cw = c.transpose(1, 2).contiguous()
-        self.delay = 0
-        if name in ("pwg", "pwg_centred"):
+        self.delay, self.hop, self.sr = 0, 256, SR_OF.get(name, SR)
+        if name == "uhifigan_opencpop_centred":
+            hop = self.hop = 300
+            e = self.e = torch.randn(B, FRAMES * hop, generator=g).to(dev) * 0.3
+            self.delay = UHiFiGANLookaheadStream(m, batch=B, use_graphs=False).delay
+            self.ref = F.pad(torch.stack([m.inference(excitation=e[b], c=c[b]).t() for b in range(B)]), (self.delay, 0))
+            self.whole = lambda: m(cw, None, e.unsqueeze(1))
+        elif name in ("pwg", "pwg_centred"):
             hop = self.hop = m.upsample_factor
             z = self.z = torch.randn(B, 1, FRAMES * hop, generator=g).to(dev)
             self.ref = torch.stack([m.inference(c=c[b], x=z[b].t()).t() for b in range(B)])
@@ -148,7 +165,7 @@ class Workload:
 
     def stream(self, B, graphs):
         cls = {"pwg": CausalPWGStream, "pwg_centred": PWGLookaheadStream, "hifigan": CausalHiFiGANStream,
-               "hifigan_centred": HiFiGANLookaheadStream}.get(self.name)
+               "hifigan_centred": HiFiGANLookaheadStream, "uhifigan_opencpop_centred": UHiFiGANLookaheadStream}.get(self.name)
         if cls is None:
             cls = CausalMelGANStream if MELGAN[self.name]["use_causal_conv"] else MelGANLookaheadStream
         return cls(self.m, batch=B, use_graphs=graphs)
@@ -156,6 +173,8 @@ class Workload:
     def push(self, st, j, n):
         if self.name in ("pwg", "pwg_centred"):
             return st.push(self.c[:, j:j + n], self.z[:, :, j * self.hop:(j + n) * self.hop])
+        if self.name == "uhifigan_opencpop_centred":
+            return st.push(self.c[:, j:j + n], self.e[:, j * self.hop:(j + n) * self.hop])
         return st.push(self.c[:, j:j + n])
 
     def check(self, s, B, n):
@@ -176,9 +195,9 @@ def bench_model(name, Bs, dev):
             w.whole()
         row = {"samples_per_item": w.samples, "delay_samples": w.delay,
                "whole_utterance_forward": stats([timed(w.whole)[1] for _ in range(5)])}
-        audio_s = w.samples / SR
+        audio_s = w.samples / w.sr
         for graphs in (False, True):
-            for n in CHUNKS:
+            for n in CHUNKS_OF.get(name, CHUNKS):
                 st = w.stream(B, graphs)
                 if w.open:  # warm-up: caches, weight packing, graph capture of every length
                     w.push(st, 0, w.open)
@@ -208,7 +227,7 @@ def bench_model(name, Bs, dev):
                 y = torch.cat(ys, -1)
                 s = stats(lat)
                 s["rtf"] = total / PASSES / 1e3 / audio_s
-                s["algorithmic_latency_ms"] = (w.delay + n * 256) / SR * 1e3
+                s["algorithmic_latency_ms"] = (w.delay + n * w.hop) / w.sr * 1e3
                 if flushes:
                     s["flush_ms"] = sorted(flushes)[len(flushes) // 2]  # every slot at once; the upper median of the passes
                 if not graphs:
