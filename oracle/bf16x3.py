@@ -107,7 +107,9 @@ def _pad(x, left, right, mode):
 
 
 def _epilogue(acc, bound, g, bias, post_act, post_slope, residual, out_scale, prev):
-    """(act(acc + bias) + residual) * out_scale [+ prev] in fp64, in the kernels' order, and its exactness record"""
+    """(act(acc + bias) + residual) * out_scale [+ prev] in fp64, and its exactness record.  The order is the kernels'
+    (``epilogue_f32`` states it step by step in fp32), but fp64 equals their fp32 result only where every step is
+    exact, which the record guards: on grid data, with power-of-two slopes and scales.  tanh is never exact here."""
     v = acc.clone()
     if bias is not None:
         v = v + bias.double().reshape(1, -1, *([1] * (v.dim() - 2)))
@@ -132,13 +134,20 @@ def _epilogue(acc, bound, g, bias, post_act, post_slope, residual, out_scale, pr
     return v.float(), ex
 
 
-def conv1d_acc(x, w, *, stride=1, padding=(0, 0), dilation=1, groups=1, pad_mode="zero", pre_slope=1.0, lolo=False):
+def _operands(a, bf16x3):
+    """hi / lo parts of the fp32 operand a: its bf16 split, or (a, 0) for the FFMA engine"""
+    return split(a) if bf16x3 else (a.float(), torch.zeros_like(a, dtype=torch.float32))
+
+
+def conv1d_acc(x, w, *, stride=1, padding=(0, 0), dilation=1, groups=1, pad_mode="zero", pre_slope=1.0, lolo=False,
+               bf16x3=True):
     """fp64 accumulator of the bf16x3 conv: sum of x_hi w_hi + x_lo w_hi + x_hi w_lo over (channel, tap) of
     lrelu(x, pre_slope) padded by ``padding`` = (left, right) in ``pad_mode`` (zero / reflect / replicate).
-    ``lolo`` adds the x_lo w_lo term the tensor cores drop (then the result is the fp64 conv of the fp32 operands).
+    ``lolo`` adds the x_lo w_lo term the tensor cores drop (then the result is the fp64 conv of the fp32 operands);
+    ``bf16x3`` False: the FFMA engine's exact products of the fp32 operands.
     Returns (acc, per-element sum of the magnitudes of the terms, their grid)."""
-    xh, xl = split(lrelu(x, pre_slope))
-    wh, wl = split(w)
+    xh, xl = _operands(lrelu(x, pre_slope), bf16x3)
+    wh, wl = _operands(w, bf16x3)
     pl, pr = padding
     xh, xl = (_pad(t.double(), pl, pr, pad_mode) for t in (xh, xl))
     wh, wl = wh.double(), wl.double()
@@ -162,20 +171,26 @@ def conv1d(x, w, bias=None, *, stride=1, padding=(0, 0), dilation=1, groups=1, p
     return _epilogue(acc, bound, g, bias, post_act, post_slope, residual, out_scale, prev)
 
 
-def conv_transpose1d(x, w, bias=None, *, stride, padding=0, output_padding=0, pre_slope=1.0):
-    """ConvTranspose1d (w: (cin, cout, k)) on lrelu(x) with bf16x3 products, + bias.  Returns (y fp32, Exactness)."""
-    xh, xl = (t.double() for t in split(lrelu(x, pre_slope)))
-    wh, wl = (t.double() for t in split(w))
+def conv_transpose1d_acc(x, w, *, stride, padding=0, output_padding=0, pre_slope=1.0, bf16x3=True):
+    """fp64 accumulator of ConvTranspose1d (w: (cin, cout, k)) on lrelu(x) with bf16x3 (or, ``bf16x3`` False, exact
+    fp32) products.  Returns (acc, per-element sum of the magnitudes of the terms, their grid)."""
+    xh, xl = (t.double() for t in _operands(lrelu(x, pre_slope), bf16x3))
+    wh, wl = (t.double() for t in _operands(w, bf16x3))
     kw = dict(stride=stride, padding=padding, output_padding=output_padding)
     acc = F.conv_transpose1d(xh, wh, **kw) + F.conv_transpose1d(xl, wh, **kw) + F.conv_transpose1d(xh, wl, **kw)
     bound = F.conv_transpose1d(xh.abs() + xl.abs(), wh.abs() + wl.abs(), **kw)
-    return _epilogue(acc, bound, _term_grid(xh, xl, wh, wl), bias, None, 1.0, None, 1.0, None)
+    return acc, bound, _term_grid(xh, xl, wh, wl)
 
 
-def conv1d_wgrad(x, gy, kernel, *, pad_left=0, dilation=1, groups=1, x_slope=1.0, g_slope=1.0):
-    """Weight gradient of a stride-1 zero-padded conv: dw[co, ci, k] = sum_{b,t} gy'[b, co, t] x'[b, ci, t + k*D - pad]
-    with gy' = lrelu(gy, g_slope), x' = lrelu(x, x_slope) and bf16x3 products gy_hi x_hi + gy_lo x_hi + gy_hi x_lo.
-    Returns (dw fp32 (cout, cin / groups, kernel), Exactness)."""
+def conv_transpose1d(x, w, bias=None, *, stride, padding=0, output_padding=0, pre_slope=1.0):
+    """ConvTranspose1d (w: (cin, cout, k)) on lrelu(x) with bf16x3 products, + bias.  Returns (y fp32, Exactness)."""
+    acc, bound, g = conv_transpose1d_acc(x, w, stride=stride, padding=padding, output_padding=output_padding,
+                                         pre_slope=pre_slope)
+    return _epilogue(acc, bound, g, bias, None, 1.0, None, 1.0, None)
+
+
+def conv1d_wgrad_acc(x, gy, kernel, *, pad_left=0, dilation=1, groups=1, x_slope=1.0, g_slope=1.0):
+    """fp64 accumulator of ``conv1d_wgrad``: (dw, per-element sum of the magnitudes of the terms, their grid)"""
     gh, gl = (t.double() for t in split(lrelu(gy, g_slope)))
     xh, xl = (t.double() for t in split(lrelu(x, x_slope)))
     B, cout, t_out = gy.shape
@@ -189,7 +204,16 @@ def conv1d_wgrad(x, gy, kernel, *, pad_left=0, dilation=1, groups=1, x_slope=1.0
 
     acc = wg(xh, gh) + wg(xh, gl) + wg(xl, gh)
     bound = wg(xh.abs() + xl.abs(), gh.abs() + gl.abs())
-    return _epilogue(acc, bound, _term_grid(gh, gl, xh, xl), None, None, 1.0, None, 1.0, None)
+    return acc, bound, _term_grid(gh, gl, xh, xl)
+
+
+def conv1d_wgrad(x, gy, kernel, *, pad_left=0, dilation=1, groups=1, x_slope=1.0, g_slope=1.0):
+    """Weight gradient of a stride-1 zero-padded conv: dw[co, ci, k] = sum_{b,t} gy'[b, co, t] x'[b, ci, t + k*D - pad]
+    with gy' = lrelu(gy, g_slope), x' = lrelu(x, x_slope) and bf16x3 products gy_hi x_hi + gy_lo x_hi + gy_hi x_lo.
+    Returns (dw fp32 (cout, cin / groups, kernel), Exactness)."""
+    acc, bound, g = conv1d_wgrad_acc(x, gy, kernel, pad_left=pad_left, dilation=dilation, groups=groups, x_slope=x_slope,
+                                     g_slope=g_slope)
+    return _epilogue(acc, bound, g, None, None, 1.0, None, 1.0, None)
 
 
 def resblock_pair(x, w1, b1, w2, b2, *, kernel_size, dilation, slope, out_scale=1.0, prev=None):
@@ -546,3 +570,215 @@ def gate_bound(d, dilation):
     xo = v * SQRT_HALF
     e = e * SQRT_HALF + U32 * (xo.abs() + e * SQRT_HALF)
     return e_sk, split_bound(xo, e), sk, xo
+
+
+# ---------------------------------------------------------------------------------------------------- rounding on fp32
+# The grid data above make every rounding exact, so they cannot see how a kernel rounds.  Here the operands are
+# arbitrary fp32 values and the weights (or the activations) are one-hot: every output element then receives exactly
+# one non-zero (activation, weight) pair, its terms a_hi w_hi + a_lo w_hi + a_hi w_lo with one operand equal to 1.0
+# (hi = 1, lo = 0), so the accumulator is hi + lo of the other operand.  hi + lo spans at most 17 bits: it is exact in
+# fp32, whatever the order of the (zero) other terms.  The epilogue that follows then has one correct fp32 result for
+# each element, ``epilogue_f32``.  On random data the same emulation gives the value the bound ``conv_bound`` is
+# centred on.
+U_TC = 2.0 ** -23   # tensor-core accumulation: not specified as round-to-nearest (it aligns and truncates), one ulp
+U_FFMA = 2.0 ** -24  # fp32 fma / add, round to nearest
+SUBNORMAL = 2.0 ** -149  # absolute floor of one fp32 rounding (the subnormal spacing)
+BF16_INF_FROM = 0x7F7F8000  # the smallest fp32 magnitude (bits) whose bf16 round to nearest is inf
+
+
+def from_bits(u):
+    """fp32 tensor with the bit patterns of the uint32 numpy array ``u``"""
+    return torch.from_numpy(np.ascontiguousarray(u, dtype=np.uint32).view(np.float32).copy())
+
+
+def fp32_values(shape, seed, special=False):
+    """Arbitrary fp32 values, each element of one class drawn at random, both signs throughout:
+      - "near": random bits with magnitudes in [2^-4, 2^4) (the classes the epilogue mixes most);
+      - "bits": random bit patterns over every normal exponent, below ``BF16_INF_FROM``;
+      - "tie": exact bf16 ties (low 16 bits 0x8000), the kept bit of either parity;
+      - "lo_tie": hi + r with r an exact bf16 tie of the remainder (the lo part's own rounding);
+      - "zero" (+-0) and "sub" (subnormals, which the build does not flush);
+    ``special`` adds "huge" (magnitudes from ``BF16_INF_FROM`` to FLT_MAX, where hi rounds to inf), +-inf and NaN."""
+    rng = np.random.default_rng(seed)
+    n = int(np.prod(shape))
+    classes = ["near"] * 6 + ["bits"] * 3 + ["tie"] * 2 + ["lo_tie"] * 2 + ["zero", "sub"]
+    if special:
+        classes += ["huge", "huge", "inf", "nan"]
+    cls = rng.integers(0, len(classes), n)
+    sign = rng.integers(0, 2, n).astype(np.uint32) << 31
+    mant = rng.integers(0, 1 << 23, n, dtype=np.uint32)
+    out = np.zeros(n, dtype=np.uint32)
+    for i, c in enumerate(classes):
+        m = cls == i
+        k = int(m.sum())
+        if c == "near":
+            e = rng.integers(127 - 4, 127 + 4, k).astype(np.uint32)
+            out[m] = (e << 23) | mant[m]
+        elif c == "bits":
+            e = rng.integers(1, 255, k).astype(np.uint32)
+            out[m] = np.minimum((e << 23) | mant[m], BF16_INF_FROM - 1)
+        elif c == "tie":
+            e = rng.integers(127 - 20, 127 + 20, k).astype(np.uint32)
+            out[m] = (e << 23) | (mant[m] & ~np.uint32(0xFFFF)) | 0x8000
+        elif c == "lo_tie":
+            # hi = 1.m7 * 2^E, r = +-(q + 1/2) 2^(E-16), q in [128, 256): |r| < 2^(E-8) (hi is its bf16), r is a tie
+            e = rng.integers(-20, 20, k)
+            hi = (1.0 + rng.integers(0, 128, k) / 128.0) * np.exp2(e)
+            q = rng.integers(128, 256, k)
+            r = (q + 0.5) * np.exp2(e - 16.0) * np.where(rng.integers(0, 2, k) == 1, 1.0, -1.0)
+            out[m] = (hi + r).astype(np.float32).view(np.uint32)
+        elif c == "zero":
+            out[m] = 0
+        elif c == "sub":
+            out[m] = np.maximum(mant[m], 1)
+        elif c == "huge":
+            out[m] = rng.integers(BF16_INF_FROM, 0x7F7FFFFF, k, endpoint=True, dtype=np.uint32)
+        elif c == "inf":
+            out[m] = 0x7F800000
+        else:
+            out[m] = 0x7FC00000
+    out |= sign
+    return from_bits(out).reshape(shape)
+
+
+def onehot_weight(cout, cin_g, K, offset=0):
+    """the activation probe: w[co, (co + offset) % cin_g, co % K] = 1, every other weight 0 (each column reads one
+    tap); with cout / groups < cin_g, the offsets of ``probe_offsets`` read every input channel between them"""
+    w = torch.zeros(cout, cin_g, K)
+    co = torch.arange(cout)
+    w[co, (co + offset) % cin_g, co % K] = 1.0
+    return w
+
+
+def onehot_weight_transposed(cin, cout, K, stride):
+    """the activation probe of a conv-transpose (w: (cin, cout, K)): for every column co and phase ph < stride one
+    tap k = ph (mod stride) reads channel (co * stride + ph) % cin.  An output row meets the taps of one phase only, so
+    it still reads one non-zero weight, and cout * stride >= cin columns-and-phases read every input channel."""
+    w = torch.zeros(cin, cout, K)
+    for ph in range(stride):
+        taps = list(range(ph, K, stride))
+        if not taps:
+            continue
+        for co in range(cout):
+            w[(co * stride + ph) % cin, co, taps[co % len(taps)]] = 1.0
+    return w
+
+
+def onehot_positions(T, spacing, margin):
+    """the time steps ``onehot_input`` sets"""
+    return range(margin, T - margin, spacing)
+
+
+def onehot_input(B, cin, T, spacing, margin, groups=1, offset=0):
+    """the weight probe: x[b, g cin_g + ci, s] = 1 at s = margin + j * spacing, ci = (j + offset) mod cin_g, 0
+    elsewhere.  With spacing beyond the conv's receptive field every output reads at most one of them, through one
+    tap.  Where fewer steps than cin_g fit, the offsets of ``probe_offsets`` reach the other channels."""
+    x = torch.zeros(B, cin, T)
+    cin_g = cin // groups
+    for j, s in enumerate(onehot_positions(T, spacing, margin)):
+        for g in range(groups):
+            x[:, g * cin_g + (j + offset) % cin_g, s] = 1.0
+    return x
+
+
+def probe_offsets(per_launch, channels):
+    """channel offsets of the launches a probe needs when one launch reads ``per_launch`` consecutive channels of
+    ``channels``: every channel is read by one of them"""
+    return list(range(0, channels, per_launch)) if 0 < per_launch < channels else [0]
+
+
+def pair_count(op, x, w):
+    """the largest number of non-zero (operand, weight) pairs that reach one output element of ``op(x, w)`` (an fp64
+    conv of the non-zero indicators): a one-hot probe is exact when it is at most 1"""
+    return float(op((x != 0).double(), (w != 0).double()).max()) if x.numel() and w.numel() else 0.0
+
+
+def conv1d_acc_ieee(x, w, *, padding, dilation=1, groups=1, pad_mode="zero", pre_slope=1.0, bf16x3=True):
+    """The accumulator of a stride-1 conv with every term formed as the hardware forms it, non-finite values included
+    (0 * inf = NaN, inf - inf = NaN): an explicit fp64 sum over (channel, tap), for small shapes.  Exact for one-hot
+    probes; ``bf16x3`` False is the FFMA engine (fp32 operands, no split)."""
+    a = lrelu(x, pre_slope)
+    a = _pad(a, padding[0], padding[1], pad_mode)
+    cout, cin_g, K = w.shape
+    B, cin, Tp = a.shape
+    t_out = Tp - (K - 1) * dilation
+    win = torch.stack([a[..., k * dilation:k * dilation + t_out] for k in range(K)], -1)  # (B, cin, t_out, K)
+    win = win.reshape(B, groups, cin_g, t_out, K)
+    wg = w.reshape(groups, cout // groups, cin_g, K)
+    with np.errstate(invalid="ignore", over="ignore"):
+        if bf16x3:
+            ah, al = (t.double().numpy() for t in split(win))
+            wh, wl = (t.double().numpy() for t in split(wg))
+            acc = (np.einsum("bgctk,gock->bgot", ah, wh) + np.einsum("bgctk,gock->bgot", al, wh)
+                   + np.einsum("bgctk,gock->bgot", ah, wl))
+        else:
+            acc = np.einsum("bgctk,gock->bgot", win.double().numpy(), wg.double().numpy())
+    return torch.from_numpy(acc).reshape(B, cout, t_out)
+
+
+def epilogue_f32(acc, bias=None, post_act=None, post_slope=0.0, residual=None, out_scale=1.0, prev=None, *, tanh=None,
+                 err=None):
+    """The conv epilogue of every engine, step by step in fp32 (numpy float32, one rounding per step):
+        v = acc + bias (0 without a bias);  v = act(v);  v = v + residual;  v = v * out_scale;  v = v + prev
+    -- epi_store and the staged epilogue of conv1d_tc.cu (the staged accumulate is the bulk copy's fp32 add into y),
+    the FFMA epilogue of conv1d_simt.cu, and conv2 of the fused ResBlock pair (residual = x); conv1 of the pair stops
+    after the bias.  ``acc`` (fp64 or fp32) is rounded to fp32 first, a zero as +0.  act: "lrelu" v > 0 ? v : v * slope, "tanh"
+    ``tanh(v)`` when given (the device's values, to check the other steps around it), else tanh in fp64 rounded to fp32.
+    With ``err`` (per-element bound on |device accumulator - acc|) also returns the bound on |device output - result|:
+    each step adds its input error times the step's slope and two roundings, 2^-24 of its result (device and
+    emulation) plus the subnormal spacing; tanh adds libdevice's 2 ulp.  Returns y (fp32 tensor) [, bound fp64]."""
+    f = np.float32
+    a64 = acc.double().numpy()
+    v = a64.astype(f) + f(0.0)  # every engine's accumulator starts at +0: a zero accumulator is +0
+    shape = (1, -1) + (1,) * (v.ndim - 2)
+    e = None if err is None else err.double().numpy() + np.abs(v.astype(np.float64) - a64)
+
+    def rnd(q, e_in):
+        """error after rounding a step whose exact result is q (fp64) from inputs within e_in"""
+        return e_in * (1 + U_FFMA) + 2 * U_FFMA * np.abs(q) + SUBNORMAL
+
+    with np.errstate(invalid="ignore", over="ignore"):
+        if bias is not None:
+            b = bias.float().numpy().reshape(shape)
+            if e is not None:
+                e = rnd(v.astype(np.float64) + b, e)
+            v = v + b
+        else:
+            v = v + f(0.0)
+        if post_act == "lrelu":
+            s = f(post_slope)
+            if e is not None:
+                e = np.where(v > 0, e, rnd(v.astype(np.float64) * float(s), e))
+            v = np.where(v > 0, v, v * s)
+        elif post_act == "tanh":
+            t = np.tanh(v.astype(np.float64)).astype(f) if tanh is None else np.asarray(tanh, dtype=f)
+            if e is not None:
+                e = e + 2.0 ** -22 * (np.abs(t) + e) + U_FFMA * np.abs(t) + SUBNORMAL
+            v = t
+        elif post_act not in (None, "none"):
+            raise ValueError(post_act)
+        if residual is not None:
+            r = residual.float().numpy()
+            if e is not None:
+                e = rnd(v.astype(np.float64) + r, e)
+            v = v + r
+        s = f(out_scale)
+        if e is not None:
+            e = rnd(v.astype(np.float64) * float(s), e * float(s))
+        v = v * s
+        if prev is not None:
+            p = prev.float().numpy()
+            if e is not None:
+                e = rnd(v.astype(np.float64) + p, e)
+            v = v + p
+    y = torch.from_numpy(np.ascontiguousarray(v, dtype=f))
+    return y if e is None else (y, torch.from_numpy(e))
+
+
+def accumulation_bound(mag, n, u):
+    """gamma_{n-1} sum|terms| with gamma_m = m u / (1 - m u) (+ 2^-52 of it for the fp64 reference sum): the worst
+    error of any order of n - 1 additions, each rounding by at most u of its result (Higham, Accuracy and Stability
+    of Numerical Algorithms, 2nd ed., section 4.2)"""
+    m = (n - 1) * u
+    assert m < 0.5, "accumulation_bound: the sum is too long for the bound"
+    return mag * (m / (1 - m) + 2.0 ** -52)

@@ -270,8 +270,9 @@ __device__ __forceinline__ void conv1d_fwd_body(const ConvKOf<EXT, EDGE> p, cons
         }
       }
       if (res) v += __ldg(res + (long long)b * p.rbs + (long long)co * p.Lout + o);
-      v *= p.out_scale;
-      if (p.accumulate) v += y[yi];
+      // the scale and the accumulate round separately (never one fma), as in the tensor-core epilogues
+      v = __fmul_rn(v, p.out_scale);
+      if (p.accumulate) v = __fadd_rn(v, y[yi]);
       y[yi] = v;
     }
   }

@@ -195,9 +195,10 @@ __device__ __forceinline__ void epi_store(const P& p, float a, int b, int t, int
     } else {
       if (res) v += __ldg(res + (long long)b * p.rbs + off);
     }
-    v *= p.out_scale;
+    // the scale and the accumulate round separately (never one fma), as the staged epilogue's bulk fp32 add does
+    v = __fmul_rn(v, p.out_scale);
     float* q = y + (long long)b * p.ybs + off;
-    if (p.accumulate) v += *q;
+    if (p.accumulate) v = __fadd_rn(v, *q);
     if constexpr (EXT) {
       if (p.mframe && stream_outside(p.mframe, p.mend, p.mrate, p.mlook, b, t)) v = 0.f;
     }
