@@ -170,9 +170,9 @@ PWGB_API int pwgb_conv1d_tc_forward(const pwgb_conv1d_desc* d, const float* x, c
  *                        (replicate: DEVICE array of batch int32, or NULL) -- ReplicationPad1d for a fresh signal;
  *   t < -hist_len:       zero.
  * History rows are input rows: the pre-activation applies to them.  d->pad_mode must be PWGB_PAD_HISTORY (accepted by
- * these entry points only) with d->pad_left the conv's left padding; the scope is stride 1, groups 1, period 1, no
- * pre_gate, one source (anything else: PWGB_INVALID or PWGB_UNSUPPORTED).  pwgb_conv1d_tc_supported() answers for such a
- * descriptor as for any other.  The FFMA entry always runs the generic kernel, whose sum order does not depend on
+ * these entry points only) with d->pad_left the conv's left padding; the scope is stride 1, period 1, no pre_gate, one
+ * source (anything else: PWGB_INVALID or PWGB_UNSUPPORTED); groups as described below pwgb_s2d_stream_grouped_forward.
+ * pwgb_conv1d_tc_supported() answers for such a descriptor as for any other.  The FFMA entry always runs the generic kernel, whose sum order does not depend on
  * where a sample sits, so a chunked run is bit-identical to the whole-signal conv on cat(hist, x) when that takes the same
  * kernel.  On the tensor cores the history launch stages activations with per-element copies (never TMA rows); the sum
  * order is the same as for the other plans.
@@ -275,13 +275,32 @@ PWGB_API int pwgb_stream_mask(float* y, int batch, int rows, int t, const pwgb_s
  * with the mask) is bit-identical to the whole-signal strided conv's tensor-core route.
  *
  * pwgb_conv1d_strided_stream_ext_forward: pwgb_conv1d_stream_ext_forward (FFMA) for a stride >= 1 conv: input rows
- * [-hist_len, 0) come from hist (pad_left >= hist_len, earlier rows zero), groups 1, period 1, no residual, no edge
+ * [-hist_len, 0) come from hist (pad_left >= hist_len, earlier rows zero), any groups, period 1, no residual, no edge
  * policy, d->pad_mode PWGB_PAD_HISTORY; output row o reads input rows o * stride - pad_left + k * dilation.  The mask of
  * ext applies to the output rows (rate: the output's samples per frame).  Bit-identical to pwgb_conv1d_forward with the
  * same stride on the explicit window when that takes the generic kernel (not conv1d_small_cout_kernel or
  * conv1d_fewcout_long_kernel). */
 PWGB_API int pwgb_s2d_stream_forward(const float* x, const float* hist, int hist_len, float* y, int batch, int channels, long long rows_in,
                                      int stride, long long rows_out, int cgo, void* stream);
+/* The grouped strided convs of a stream (the MelGANDiscriminator encoder of a VQ-VAE).
+ *
+ * pwgb_s2d_stream_grouped_forward: pwgb_s2d_forward (groups, period 1, pad_left 0) on the window [hist | x]: y (batch,
+ * groups * group_channels_out, rows_out), channel g * group_channels_out + r * (channels / groups) + c of row u = window
+ * row stride * u + r of input channel g * (channels / groups) + c (zero past the window, and in a group's channels >=
+ * stride * channels / groups; group_channels_out 0 means stride * channels / groups).  pwgb_s2d_stream_forward is this
+ * call with groups 1 (its cgo is group_channels_out).  The stride-1 conv that follows runs with the same groups on
+ * pwgb_conv1d_tc_stream_ext_forward with pad_left 0 and no history: the window carries it.
+ *
+ * Groups in the other stream entry points: pwgb_conv1d_stream_forward / pwgb_conv1d_stream_ext_forward /
+ * pwgb_conv1d_strided_stream_ext_forward (FFMA) take any groups dividing cin and cout, history rows included (hist holds
+ * every input channel).  pwgb_conv1d_tc_stream_forward / pwgb_conv1d_tc_stream_ext_forward take groups > 1 only with
+ * d->pad_left 0 and hist_len 0 (pwgb_conv1d_tc_supported answers 0 for a grouped history descriptor with pad_left > 0,
+ * the entry PWGB_UNSUPPORTED for hist_len > 0); such a launch is the grouped multi-chunk launch of
+ * pwgb_conv1d_tc_forward with the mask, so it is bit-identical to that call on the window when it takes the same tile
+ * shape. */
+PWGB_API int pwgb_s2d_stream_grouped_forward(const float* x, const float* hist, int hist_len, float* y, int batch, int channels,
+                                             int groups, long long rows_in, int stride, long long rows_out, int group_channels_out,
+                                             void* stream);
 PWGB_API int pwgb_conv1d_strided_stream_ext_forward(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len,
                                                     const float* w, const float* bias, const pwgb_stream_ext* ext, float* y,
                                                     void* stream);
@@ -717,6 +736,18 @@ PWGB_API int pwgb_vq_forward(const float* z_e, const float* codebook, int num_co
                              int global_channels, int batch, int dim, int t, void* stream);
 PWGB_API int pwgb_vq_backward(const float* gdec, int batch, int dim, int local_channels, int global_channels, int t, float* gz_e,
                               int accumulate, const long long* g, int num_global, float* d_global_table, void* stream);
+/* The bottleneck of a streamed VQ-VAE: pwgb_vq_forward (search and assembly, the same code) on one chunk of t frames
+ * of z_e (search required, no z_q), with two stream extensions:
+ *   l: row j of the local conditioning is row j of the window [l_hist (B, Cl, l_delay) | l (B, Cl, t)], so l arrives
+ *     l_delay frames before the z_e frames it goes with (the encoder's lookahead in frames);
+ *   ext: a mask at the frame rate (rate 1, no residual, no edge policy): frame j of item b is signal frame
+ *     frame[b] - lookahead + j; outside [0, end[b]) every dec channel is stored as +0.0 and the index as -1.
+ * Inside the signal each frame's index and dec column equal pwgb_vq_forward's on the same z_e column, l column and g
+ * (NaN rules included): the search of a frame does not depend on its place in the launch. */
+PWGB_API int pwgb_vq_stream_forward(const float* z_e, const float* codebook, int num_codes, long long* indices, float* dec,
+                                    const float* l, const float* l_hist, int l_delay, int local_channels, const float* global_table,
+                                    const long long* g, int num_global, int global_channels, const pwgb_stream_ext* ext, int batch,
+                                    int dim, int t, void* stream);
 
 #ifdef __cplusplus
 }

@@ -136,6 +136,9 @@ def lib():
     L.pwgb_stream_mask.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.POINTER(StreamExt), vp]
     L.pwgb_s2d_stream_forward.restype = C.c_int
     L.pwgb_s2d_stream_forward.argtypes = [vp, vp, C.c_int, vp, C.c_int, C.c_int, C.c_longlong, C.c_int, C.c_longlong, C.c_int, vp]
+    L.pwgb_s2d_stream_grouped_forward.restype = C.c_int
+    L.pwgb_s2d_stream_grouped_forward.argtypes = [vp, vp, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_longlong, C.c_int, C.c_longlong,
+                                                  C.c_int, vp]
     L.pwgb_conv1d_strided_stream_ext_forward.restype = C.c_int
     L.pwgb_conv1d_strided_stream_ext_forward.argtypes = [C.POINTER(Conv1dDesc), vp, vp, C.c_int, vp, vp, C.POINTER(StreamExt), vp, vp]
     L.pwgb_conv_transpose1d_cat_stream_workspace.restype = C.c_size_t
@@ -296,6 +299,9 @@ def lib():
     L.pwgb_duration_round.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_float, C.c_int, vp]
     L.pwgb_collate_runlength.restype = C.c_int
     L.pwgb_collate_runlength.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_int, ll, vp]
+    L.pwgb_vq_stream_forward.restype = C.c_int
+    L.pwgb_vq_stream_forward.argtypes = [vp, vp, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, C.c_int,
+                                         C.POINTER(StreamExt), C.c_int, C.c_int, C.c_int, vp]
     L.pwgb_vq_forward.restype = C.c_int
     L.pwgb_vq_forward.argtypes = [vp, vp, C.c_int, vp, vp, vp, vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp]
     L.pwgb_vq_backward.restype = C.c_int
@@ -335,7 +341,7 @@ EXPORTED_SYMBOLS = [
     "pwgb_wnstack_supported", "pwgb_wnstack_x_bytes", "pwgb_wnstack_c_bytes", "pwgb_wnstack_pack_x", "pwgb_wnstack_unpack_x",
     "pwgb_wnstack_pack_c", "pwgb_wnstack_first_conv", "pwgb_wnstack_layer_forward", "pwgb_wnstack_carry",
     "pwgb_upsample_fir_causal_stream_forward", "pwgb_upsample_fir_stream_ext_forward", "pwgb_stream_mask",
-    "pwgb_s2d_stream_forward", "pwgb_conv1d_strided_stream_ext_forward", "pwgb_conv_transpose1d_cat_stream_workspace",
+    "pwgb_s2d_stream_forward", "pwgb_s2d_stream_grouped_forward", "pwgb_conv1d_strided_stream_ext_forward", "pwgb_conv_transpose1d_cat_stream_workspace",
     "pwgb_conv_transpose1d_cat_stream_ext_forward",
     "pwgb_wnstack_first_conv_stream_ext", "pwgb_wnstack_layer_stream_ext_forward",
     "pwgb_mr_stft_loss_workspace", "pwgb_mr_stft_loss_forward", "pwgb_stft_amplitude_forward",
@@ -351,5 +357,5 @@ EXPORTED_SYMBOLS = [
     "pwgb_symbol_embed_forward", "pwgb_symbol_embed_backward_workspace", "pwgb_symbol_embed_backward",
     "pwgb_channel_layernorm_forward", "pwgb_channel_layernorm_backward_workspace", "pwgb_channel_layernorm_backward",
     "pwgb_duration_loss_forward", "pwgb_duration_loss_backward", "pwgb_duration_round", "pwgb_collate_runlength",
-    "pwgb_vq_forward", "pwgb_vq_backward",
+    "pwgb_vq_forward", "pwgb_vq_stream_forward", "pwgb_vq_backward",
 ]

@@ -139,8 +139,8 @@ __device__ __forceinline__ void conv1d_fwd_body(const ConvKOf<EXT, EDGE> p, cons
       float v = 0.f;
       if constexpr (HIST) {
         // rows [-hist_len, 0) from the history (or sample 0 of a replicated item, sample -li of a reflected one), earlier
-        // rows and rows past the input zero
-        const int ch = ci0 + ci;
+        // rows and rows past the input zero; ch: the channel of x and of hist (group g's input channels)
+        const int ch = g * p.Cin_g + ci0 + ci;
         const float* src = nullptr;
         if constexpr (EDGE) {
           if (p.edge) li = edge_row(p, b, li);
@@ -566,7 +566,7 @@ int conv1d_forward_simt(const pwgb_conv1d_desc* d, const float* x, const float* 
   return launch_conv<1, 1>(p, x, w, bias, residual, y, st);
 }
 
-// History launches (pad_mode PWGB_PAD_HISTORY, groups 1, period 1) always take the generic kernel: the few-channel
+// History launches (pad_mode PWGB_PAD_HISTORY, period 1, any groups) always take the generic kernel: the few-channel
 // kernels above sum in an order that depends on where a sample sits in the sequence, which a stream cannot reproduce.
 // zero_flag / zero_rows: see ConvK (shuffled launches only); ext: the mask and the delayed residual (pwgb_stream_ext).
 int conv1d_stream_simt(const pwgb_conv1d_desc* d, const float* x, const float* hist, int hist_len, const int* rep,

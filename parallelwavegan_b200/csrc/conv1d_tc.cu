@@ -1126,8 +1126,9 @@ static int tc_cout_chunk(int cout) {
 // channel slice (pointer offsets, batch strides of the full tensors).
 extern "C" int pwgb_conv1d_tc_supported(const pwgb_conv1d_desc* d) {
   if (!d || d->cout <= 0 || d->groups <= 0 || d->cin % d->groups || d->cout % d->groups) return 0;
-  // history padding: plain dense convs only (pwgb_conv1d_tc_stream_forward)
-  if (is_history_pad(d->pad_mode) && (d->groups != 1 || d->pre_gate || d->shuffle > 1)) return 0;
+  // history padding: one-source convs without pre_gate (pwgb_conv1d_tc_stream_forward); a grouped one reads no row
+  // before sample 0 (pad_left 0: a window that carries its own history, as after pwgb_s2d_stream_grouped_forward)
+  if (is_history_pad(d->pad_mode) && ((d->groups != 1 && d->pad_left != 0) || d->pre_gate || d->shuffle > 1)) return 0;
   const int G = d->groups;
   if (G > 1 && (d->shuffle > 1 || d->pre_gate || G > 64)) return 0;
   const int chunk = tc_cout_chunk(d->cout / G);
@@ -1147,6 +1148,8 @@ static int tc_forward(const pwgb_conv1d_desc* d, const float* x, const void* pac
                       const pwgb_stream_ext* ext = nullptr) {
   PWGB_UNSUPPORTED_IF(!pwgb_conv1d_tc_supported(d), "conv1d_tc: configuration not supported by the tensor-core path");
   const int G = d->groups, cin_g = d->cin / G, cout_g = d->cout / G;
+  // the history loader addresses hist by the chunk within a group: a grouped launch must not read one
+  PWGB_UNSUPPORTED_IF(G > 1 && hist_len > 0, "conv1d_tc_stream: a grouped history launch takes no history rows (hist_len %d)", hist_len);
   const int chunk = tc_cout_chunk(cout_g);
   pwgb_conv1d_desc c = *d;
   c.cout = chunk;

@@ -51,20 +51,23 @@ __global__ void s2d_backward_kernel(const float* __restrict__ gy, float* __restr
   }
 }
 
-// The space-to-depth of one stream window [hist | x] (groups 1, period 1, no padding): y (B, Cgo, rows_out), channel
-// r * C + c of row u is window row s * u + r of channel c; window rows past hist_len + rows_in and channels >= s * C are
-// zero.  The same values pwgb_s2d_forward gives on the concatenation, read in place.
-__global__ void s2d_stream_kernel(const float* __restrict__ x, const float* __restrict__ hist, float* __restrict__ y, int C, int Cgo,
-                                  long long rows_in, int hist_len, int s, long long rows_out, long long total) {
+// The space-to-depth of one stream window [hist | x] (period 1, no padding): y (B, G * Cgo, rows_out), channel
+// g * Cgo + r * Cg + cl of row u is window row s * u + r of input channel g * Cg + cl; window rows past
+// hist_len + rows_in and channels >= s * Cg of a group are zero.  The same values pwgb_s2d_forward gives on the
+// concatenation, read in place.
+__global__ void s2d_stream_kernel(const float* __restrict__ x, const float* __restrict__ hist, float* __restrict__ y, int C, int Cg,
+                                  int Cgo, long long rows_in, int hist_len, int s, long long rows_out, long long total) {
+  const int G = C / Cg;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long u = i % rows_out;
     const long long t = i / rows_out;
-    const int ch = (int)(t % Cgo);
-    const long long b = t / Cgo;
-    const int r = ch / C, c = ch - r * C;
+    const int ch = (int)(t % ((long long)G * Cgo));
+    const long long b = t / ((long long)G * Cgo);
+    const int g = ch / Cgo, rem = ch - g * Cgo;
+    const int r = rem / Cg, c = g * Cg + rem - r * Cg;
     const long long row = (long long)s * u + r - hist_len;  // row of x; below 0: of the history
     float v = 0.f;
-    if (ch < s * C) {
+    if (rem < s * Cg) {
       if (row < 0)
         v = __ldg(hist + (b * C + c) * hist_len + (hist_len + row));
       else if (row < rows_in)
@@ -78,18 +81,26 @@ __global__ void s2d_stream_kernel(const float* __restrict__ x, const float* __re
 
 using namespace pwgb;
 
-extern "C" int pwgb_s2d_stream_forward(const float* x, const float* hist, int hist_len, float* y, int batch, int channels, long long rows_in,
-                                       int stride, long long rows_out, int cgo, void* stream) {
-  PWGB_CHECK_ARG(batch >= 0 && channels > 0 && rows_in > 0 && stride > 0 && rows_out > 0 && hist_len >= 0,
+extern "C" int pwgb_s2d_stream_grouped_forward(const float* x, const float* hist, int hist_len, float* y, int batch, int channels,
+                                               int groups, long long rows_in, int stride, long long rows_out, int group_channels_out,
+                                               void* stream) {
+  PWGB_CHECK_ARG(batch >= 0 && channels > 0 && groups > 0 && channels % groups == 0 && rows_in > 0 && stride > 0 && rows_out > 0 &&
+                     hist_len >= 0,
                  "s2d_stream: bad argument");
-  const int co = cgo ? cgo : channels * stride;
-  PWGB_CHECK_ARG(co >= channels * stride, "s2d_stream: group_channels_out smaller than stride * channels");
+  const int cg = channels / groups;
+  const int cgo = group_channels_out ? group_channels_out : cg * stride;
+  PWGB_CHECK_ARG(cgo >= cg * stride, "s2d_stream: group_channels_out smaller than stride * channels per group");
   PWGB_CHECK_ARG(x && y && (hist_len == 0 || hist), "s2d_stream: null argument");
-  const long long total = (long long)batch * co * rows_out;
+  const long long total = (long long)batch * groups * cgo * rows_out;
   if (total == 0) return PWGB_OK;
   const int blocks = (int)((total + 255) / 256 < 4096 ? (total + 255) / 256 : 4096);
-  s2d_stream_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(x, hist, y, channels, co, rows_in, hist_len, stride, rows_out, total);
+  s2d_stream_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(x, hist, y, channels, cg, cgo, rows_in, hist_len, stride, rows_out, total);
   return check_launch("s2d_stream_kernel");
+}
+
+extern "C" int pwgb_s2d_stream_forward(const float* x, const float* hist, int hist_len, float* y, int batch, int channels, long long rows_in,
+                                       int stride, long long rows_out, int cgo, void* stream) {
+  return pwgb_s2d_stream_grouped_forward(x, hist, hist_len, y, batch, channels, 1, rows_in, stride, rows_out, cgo, stream);
 }
 
 static int s2d_args_ok(int batch, int channels, int groups, long long rows_in, int period, int stride, int pad_left, long long rows_out) {

@@ -36,8 +36,9 @@ int conv1d_stream_check(const pwgb_conv1d_desc* d, const float* x, const float* 
   PWGB_CHECK_ARG(d->pad_mode != PWGB_PAD_HISTORY_REFLECT || (d->pad_left < d->t_in && hist_len <= d->pad_left),
                  "conv1d_stream: reflect needs pad_left (%d) < t_in (%d) and hist_len (%d) <= pad_left", d->pad_left, d->t_in,
                  hist_len);
-  PWGB_UNSUPPORTED_IF(d->stride != 1 || d->groups != 1 || d->period > 1 || d->pre_gate || d->shuffle > 1,
-                      "conv1d_stream: history padding serves plain stride-1 convs (groups 1, period 1, no pre_gate, one source)");
+  PWGB_CHECK_ARG(d->cin % d->groups == 0 && d->cout % d->groups == 0, "conv1d_stream: groups must divide cin and cout");
+  PWGB_UNSUPPORTED_IF(d->stride != 1 || d->period > 1 || d->pre_gate || d->shuffle > 1,
+                      "conv1d_stream: history padding serves plain stride-1 convs (period 1, no pre_gate, one source)");
   PWGB_UNSUPPORTED_IF(d->x_batch_stride || d->y_batch_stride || d->r_batch_stride || (d->t_valid > 0 && d->t_valid != d->t_in),
                       "conv1d_stream: strided or reflect-extended inputs are not supported");
   const long long need = (long long)(d->t_out - 1) + (long long)(d->kernel - 1) * d->dilation + 1 - d->pad_left;
@@ -123,14 +124,14 @@ extern "C" int pwgb_conv1d_strided_stream_ext_forward(const pwgb_conv1d_desc* d,
                                                       void* stream) {
   PWGB_CHECK_ARG(d && x && y && w, "conv1d_strided_stream: null argument");
   PWGB_CHECK_ARG(d->batch >= 0 && d->cin > 0 && d->cout > 0 && d->t_in > 0 && d->t_out >= 0 && d->kernel > 0 && d->stride > 0 &&
-                     d->dilation > 0 && d->pad_left >= 0,
+                     d->dilation > 0 && d->pad_left >= 0 && d->groups > 0 && d->cin % d->groups == 0 && d->cout % d->groups == 0,
                  "conv1d_strided_stream: bad descriptor");
   PWGB_CHECK_ARG(d->pad_mode == PWGB_PAD_HISTORY, "conv1d_strided_stream: pad_mode must be PWGB_PAD_HISTORY");
   PWGB_CHECK_ARG(hist_len >= 0 && hist_len <= d->pad_left && (hist_len == 0 || hist), "conv1d_strided_stream: bad history (hist_len %d)",
                  hist_len);
-  PWGB_UNSUPPORTED_IF(d->groups != 1 || d->period > 1 || d->pre_gate || d->shuffle > 1 || d->accumulate || d->x_batch_stride ||
+  PWGB_UNSUPPORTED_IF(d->period > 1 || d->pre_gate || d->shuffle > 1 || d->accumulate || d->x_batch_stride ||
                           d->y_batch_stride || d->r_batch_stride || (d->t_valid > 0 && d->t_valid != d->t_in),
-                      "conv1d_strided_stream: plain dense convs only (groups 1, period 1, no pre_gate, no accumulate, one source)");
+                      "conv1d_strided_stream: plain convs only (period 1, no pre_gate, no accumulate, one source)");
   const long long need = (long long)(d->t_out - 1) * d->stride + (long long)(d->kernel - 1) * d->dilation + 1 - d->pad_left;
   PWGB_CHECK_ARG(d->t_out == 0 || need <= (long long)d->t_in, "conv1d_strided_stream: t_out too large for t_in");
   if (const int rc = stream_ext_check(ext, nullptr, d->pad_mode)) return rc;

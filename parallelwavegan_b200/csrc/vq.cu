@@ -20,6 +20,13 @@ struct VqArgs {
   const float* gtab;      // (num_g, Cg) or null
   const long long* g;     // (B,) or null
   int B, D, T, K, Cl, Cg, num_g;
+  // the stream launch (pwgb_vq_stream_forward): l row t is row t of [l_hist (B, Cl, l_delay) | l], and frame t of item
+  // b is signal frame mframe[b] - mlook + t, stored as +0.0 (index -1) outside [0, mend[b])
+  const float* l_hist;
+  int l_delay;
+  const int* mframe;
+  const int* mend;
+  int mlook;
 };
 
 // torch.min(dim) order: a NaN distance beats every number and the first NaN wins; otherwise the smaller distance,
@@ -34,8 +41,12 @@ __device__ __forceinline__ bool vq_better(float d, int k, float bd, int bk) {
 // group is XORed with d % 8 so that a warp storing 32 consecutive d of one code hits 8 banks instead of 1
 __device__ __forceinline__ int vq_slot(int d, int kk) { return d * VQ_KC + ((((kk >> 2) ^ (d & 7))) << 2) + (kk & 3); }
 
-// grid (ceil(T / 32), B), 256 threads.  Dynamic shared memory: xs (D x 32) when searching + cs (D x 32).
-__global__ void __launch_bounds__(256) vq_forward_kernel(const VqArgs a) {
+constexpr int VQ_MASKED = -3;  // row[] of a stream frame outside its signal
+
+// grid (ceil(T / 32), B), 256 threads.  Dynamic shared memory: xs (D x 32) when searching + cs (D x 32).  STREAM: the
+// delayed l and the mask of VqArgs (search and assembly otherwise the same code).
+template <bool STREAM>
+__device__ __forceinline__ void vq_forward_body(const VqArgs& a) {
   extern __shared__ __align__(16) float vq_smem[];
   __shared__ float bd_sh[8][VQ_TT];
   __shared__ int bk_sh[8][VQ_TT];
@@ -98,8 +109,9 @@ __global__ void __launch_bounds__(256) vq_forward_kernel(const VqArgs a) {
           best_d = bd_sh[w][lane];
           best_k = bk_sh[w][lane];
         }
-      row[lane] = best_k;
-      if (t0 + lane < T) a.idx[(long long)b * T + t0 + lane] = best_k;
+      const bool masked = STREAM && stream_outside(a.mframe, a.mend, 1, a.mlook, b, t0 + lane);
+      row[lane] = masked ? VQ_MASKED : best_k;
+      if (t0 + lane < T) a.idx[(long long)b * T + t0 + lane] = masked ? -1 : best_k;
     }
   } else if (tid < VQ_TT) {
     int r = 0;
@@ -124,22 +136,29 @@ __global__ void __launch_bounds__(256) vq_forward_kernel(const VqArgs a) {
     const int r = row[tt];
     const float v = r >= 0 ? __ldg(a.cb + (long long)r * D + d) : qnan;
     if (a.z_q) a.z_q[((long long)b * D + d) * T + t] = v;
-    if (a.dec) a.dec[((long long)b * Ct + d) * T + t] = gr == -2 ? qnan : v;
+    if (a.dec) a.dec[((long long)b * Ct + d) * T + t] = (STREAM && r == VQ_MASKED) ? 0.f : gr == -2 ? qnan : v;
   }
   if (!a.dec) return;
   for (int i = tid; i < (a.Cl + a.Cg) * VQ_TT; i += 256) {
     const int c = i / VQ_TT, tt = i % VQ_TT, t = t0 + tt;
     if (t >= T) continue;
     float v;
-    if (gr == -2 || row[tt] < 0)
+    if (STREAM && row[tt] == VQ_MASKED)
+      v = 0.f;
+    else if (gr == -2 || row[tt] < 0)
       v = qnan;
     else if (c < a.Cl)
-      v = a.l[((long long)b * a.Cl + c) * T + t];
+      v = !STREAM ? a.l[((long long)b * a.Cl + c) * T + t]
+          : t < a.l_delay ? a.l_hist[((long long)b * a.Cl + c) * a.l_delay + t]
+                          : a.l[((long long)b * a.Cl + c) * T + (t - a.l_delay)];
     else
       v = __ldg(a.gtab + (long long)gr * a.Cg + (c - a.Cl));
     a.dec[((long long)b * Ct + D + c) * T + t] = v;
   }
 }
+
+__global__ void __launch_bounds__(256) vq_forward_kernel(const VqArgs a) { vq_forward_body<false>(a); }
+__global__ void __launch_bounds__(256) vq_stream_kernel(const VqArgs a) { vq_forward_body<true>(a); }
 
 // straight-through adjoint: gz_e (+)= gdec[:, :D]
 __global__ void vq_st_backward_kernel(const float* __restrict__ gdec, float* __restrict__ gz, int D, int Ct, int T, long long n,
@@ -197,7 +216,8 @@ extern "C" int pwgb_vq_forward(const float* z_e, const float* codebook, int num_
   if (batch == 0 || t == 0) return PWGB_OK;
   PWGB_CHECK_ARG(codebook && indices, "vq_forward: null pointer");
   PWGB_CHECK_ARG(z_e || z_q || dec, "vq_forward: nothing to do");
-  VqArgs a{z_e, codebook, indices, z_q, dec, l, global_table, g, batch, dim, t, num_codes, local_channels, global_channels, num_global};
+  VqArgs a{z_e, codebook, indices, z_q, dec, l, global_table, g, batch, dim, t, num_codes, local_channels, global_channels, num_global,
+           nullptr, 0, nullptr, nullptr, 0};
   const size_t smem = z_e ? (size_t)2 * dim * VQ_TT * sizeof(float) : 0;
   if (smem > 48 * 1024 && cudaFuncSetAttribute(vq_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
     set_error("vq_forward: cannot reserve %zu bytes of shared memory", smem);
@@ -205,6 +225,34 @@ extern "C" int pwgb_vq_forward(const float* z_e, const float* codebook, int num_
   }
   vq_forward_kernel<<<dim3((unsigned)ceil_div(t, VQ_TT), (unsigned)batch), 256, smem, (cudaStream_t)stream>>>(a);
   return check_launch("vq_forward_kernel");
+}
+
+extern "C" int pwgb_vq_stream_forward(const float* z_e, const float* codebook, int num_codes, long long* indices, float* dec,
+                                      const float* l, const float* l_hist, int l_delay, int local_channels, const float* global_table,
+                                      const long long* g, int num_global, int global_channels, const pwgb_stream_ext* ext, int batch,
+                                      int dim, int t, void* stream) {
+  PWGB_CHECK_ARG(batch >= 0 && dim > 0 && t >= 0 && num_codes > 0 && local_channels >= 0 && global_channels >= 0 && l_delay >= 0,
+                 "vq_stream: bad sizes");
+  PWGB_CHECK_ARG(!local_channels == !l && (!local_channels || !l_delay || l_hist) && !global_channels == !global_table &&
+                     !global_table == !g,
+                 "vq_stream: a conditioning tensor and its channel count must come together");
+  PWGB_CHECK_ARG(!g || num_global > 0, "vq_stream: global table without rows");
+  PWGB_CHECK_ARG(ext && ext->frame && ext->end && ext->rate == 1 && ext->lookahead >= 0 && !ext->res_hist_len && !ext->res_delay &&
+                     ext->edge == PWGB_PAD_ZERO,
+                 "vq_stream: ext must hold a frame-rate mask (rate 1) and nothing else");
+  PWGB_UNSUPPORTED_IF(dim > VQ_MAX_D, "vq_stream: embed_dim %d > %d", dim, VQ_MAX_D);
+  PWGB_UNSUPPORTED_IF(batch > 65535, "vq_stream: batch %d > 65535", batch);
+  if (batch == 0 || t == 0) return PWGB_OK;
+  PWGB_CHECK_ARG(z_e && codebook && indices && dec, "vq_stream: null pointer");
+  VqArgs a{z_e, codebook, indices, nullptr, dec, l, global_table, g, batch, dim, t, num_codes, local_channels, global_channels, num_global,
+           l_hist, l_delay, ext->frame, ext->end, ext->lookahead};
+  const size_t smem = (size_t)2 * dim * VQ_TT * sizeof(float);
+  if (smem > 48 * 1024 && cudaFuncSetAttribute(vq_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+    set_error("vq_stream: cannot reserve %zu bytes of shared memory", smem);
+    return PWGB_CUDA_ERROR;
+  }
+  vq_stream_kernel<<<dim3((unsigned)ceil_div(t, VQ_TT), (unsigned)batch), 256, smem, (cudaStream_t)stream>>>(a);
+  return check_launch("vq_stream_kernel");
 }
 
 extern "C" int pwgb_vq_backward(const float* gdec, int batch, int dim, int local_channels, int global_channels, int t, float* gz_e,

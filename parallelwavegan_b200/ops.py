@@ -432,7 +432,7 @@ def _stream_ext(B, cout, mask, res_hist, res_delay, edge=None, in_lookahead=0):
 
 def conv1d_stream(x, hist, w, bias=None, *, pad_left, dilation=1, replicate=None, reflect=False, pre_slope=1.0, post_act=None,
                   post_slope=0.0, residual=None, out_scale=1.0, out=None, accumulate=False, t_out=None, mask=None, res_hist=None,
-                  res_delay=0, edge=None, in_lookahead=0):
+                  res_delay=0, edge=None, in_lookahead=0, groups=1):
     """conv1d with history padding (pwgb_conv1d_stream_forward / pwgb_conv1d_tc_stream_forward): of the ``pad_left`` rows
     in front of x, the last H read ``hist`` (B, cin, H) -- or x[:, :, 0] for the items whose ``replicate`` (B,) int32 flag
     is set -- and the earlier ones are zero; no right padding.  With ``reflect`` a flagged item reads row -t from x[:, :, t]
@@ -446,25 +446,27 @@ def conv1d_stream(x, hist, w, bias=None, *, pad_left, dilation=1, replicate=None
     ``res_hist`` (B, cout, Hr) / ``res_delay``: row t adds row t - res_delay of [res_hist | residual]; ``edge`` ("reflect"
     or "replicate", with a mask) / ``in_lookahead``: input row r of [hist | x] is signal sample frame[b] * rate -
     in_lookahead + r, and a row outside [0, end[b] * rate) reads the row holding the reflected or replicated sample, so
-    every output inside the signal equals the whole-signal conv with that pad."""
+    every output inside the signal equals the whole-signal conv with that pad.  ``groups``: a grouped conv (weight (cout,
+    cin / groups, K)); on the tensor cores only with pad_left 0 and no history (the window after ``s2d_stream``)."""
     x, w = _dev(x, "x"), _dev(w, "w")
     B, cin, L = x.shape
     cout, cin_w, K = w.shape
+    groups = int(groups)
     if hist is None:
         hist = x.new_zeros((B, cin, 0))
     hist = _dev(hist, "hist")
-    if cin_w != cin or hist.dim() != 3 or tuple(hist.shape[:2]) != (B, cin):
+    if cin_w * groups != cin or cout % groups or hist.dim() != 3 or tuple(hist.shape[:2]) != (B, cin):
         raise PwgbError(f"conv1d_stream: x {tuple(x.shape)}, hist {tuple(hist.shape)} and weight {tuple(w.shape)} do not match")
     if replicate is not None and (replicate.dtype != torch.int32 or not replicate.is_cuda or replicate.numel() != B):
         raise PwgbError(f"conv1d_stream: replicate must be {B} int32 flags on the device")
     kw = dict(pad_left=pad_left, dilation=dilation, replicate=replicate, reflect=reflect, pre_slope=pre_slope, post_act=post_act,
               post_slope=post_slope, t_out=t_out, mask=mask, edge=edge, in_lookahead=in_lookahead)
-    if ENGINE != "simt" and cout < 16 and cin >= 256 and cin % 32 == 0 and residual is None and out is None and not accumulate:
+    if ENGINE != "simt" and groups == 1 and cout < 16 and cin >= 256 and cin % 32 == 0 and residual is None and out is None and not accumulate:
         # as _conv1d_fewcout: the weight padded to 16 output channels for the tensor cores
         b16 = torch.nn.functional.pad(bias, (0, 16 - cout)) if bias is not None else None
         y = conv1d_stream(x, hist, torch.nn.functional.pad(w, (0, 0, 0, 0, 0, 16 - cout)), b16, **kw)
         return y[:, :cout].contiguous()
-    if ENGINE != "simt" and cin % 32 and cin >= 48 and cout % 16 == 0:
+    if ENGINE != "simt" and groups == 1 and cin % 32 and cin >= 48 and cout % 16 == 0:
         # as _conv1d_padcin: input channels zero-padded to a multiple of 32
         padc = (cin + 31) // 32 * 32 - cin
         pc = (0, 0, 0, padc)
@@ -496,26 +498,26 @@ def conv1d_stream(x, hist, w, bias=None, *, pad_left, dilation=1, replicate=None
         bias = _dev(bias, "bias")
     H = hist.shape[-1]
     dkey = ("stream", B, cin, cout, L, t_out, K, dilation, pad_left, bool(reflect), float(pre_slope), post_act, float(post_slope),
-            float(out_scale), bool(accumulate))
+            float(out_scale), bool(accumulate), groups)
     d = _DESC_CACHE.get(dkey)
     if d is None:
         if len(_DESC_CACHE) > 4096:
             _DESC_CACHE.clear()
         d = _DESC_CACHE[dkey] = capi.Conv1dDesc(
-            batch=B, cin=cin, cout=cout, t_in=L, t_out=t_out, kernel=K, stride=1, dilation=dilation, groups=1, pad_left=pad_left,
+            batch=B, cin=cin, cout=cout, t_in=L, t_out=t_out, kernel=K, stride=1, dilation=dilation, groups=groups, pad_left=pad_left,
             pad_mode=capi.PAD_HISTORY_REFLECT if reflect else capi.PAD_HISTORY, period=1, t_valid=L, pre_slope=float(pre_slope), pre_gate=0, post_act=_ACT[post_act],
             post_slope=float(post_slope), out_scale=float(out_scale), accumulate=int(bool(accumulate)))
-    prof = _Prof("conv1d_stream", 2.0 * B * cout * t_out * cin * K,
+    prof = _Prof("conv1d_stream", 2.0 * B * cout * t_out * cin_w * K,
                  4.0 * (x.numel() + out.numel() * (2 if accumulate else 1) + (residual.numel() if residual is not None else 0)),
-                 f"B{B} cin{cin} cout{cout} k{K} d{dilation} T{t_out} H{H}" if PROFILE is not None else "")
+                 f"B{B} cin{cin} cout{cout} k{K} d{dilation} g{groups} T{t_out} H{H}" if PROFILE is not None else "")
     lib = capi.lib()
     if ENGINE != "simt" and lib.pwgb_conv1d_tc_supported(C.byref(d)):
         prof.name = "conv1d_tc_stream"
         if ext is not None:
-            rc = lib.pwgb_conv1d_tc_stream_ext_forward(C.byref(d), _p(x), _p(hist), H, _p(replicate), _p(packed_weight(w)), _p(bias),
-                                                       _p(residual), C.byref(ext), _p(out), _stream())
+            rc = lib.pwgb_conv1d_tc_stream_ext_forward(C.byref(d), _p(x), _p(hist), H, _p(replicate), _p(packed_weight(w, groups)),
+                                                       _p(bias), _p(residual), C.byref(ext), _p(out), _stream())
         else:
-            rc = lib.pwgb_conv1d_tc_stream_forward(C.byref(d), _p(x), _p(hist), H, _p(replicate), _p(packed_weight(w)), _p(bias),
+            rc = lib.pwgb_conv1d_tc_stream_forward(C.byref(d), _p(x), _p(hist), H, _p(replicate), _p(packed_weight(w, groups)), _p(bias),
                                                    _p(residual), _p(out), _stream())
         capi.check(rc, "pwgb_conv1d_tc_stream_forward")
     else:
@@ -614,38 +616,42 @@ def conv_transpose1d_window_stream(x, hist, w, bias=None, *, stride, padding, fr
     return y
 
 
-def s2d_stream(x, hist, stride, rows_out, cgo=0, out=None):
-    """The space-to-depth of a stream window [hist | x] (pwgb_s2d_stream_forward): x (B, C, n), hist (B, C, H) -> (B, cgo
-    or stride * C, rows_out), row u holding window rows stride * u .. stride * u + stride - 1; ``s2d_raw`` on the
-    concatenation with no padding, read in place."""
+def s2d_stream(x, hist, stride, rows_out, cgo=0, out=None, groups=1):
+    """The space-to-depth of a stream window [hist | x] (pwgb_s2d_stream_grouped_forward): x (B, C, n), hist (B, C, H) ->
+    (B, groups * (cgo or stride * C / groups), rows_out), row u holding window rows stride * u .. stride * u + stride - 1;
+    ``s2d_raw(window, groups, stride, 0, rows_out, cgo=cgo)`` on the concatenation, read in place."""
     x, hist = _dev(x, "x"), _dev(hist, "hist")
     B, Cc, n = x.shape
     if hist.dim() != 3 or tuple(hist.shape[:2]) != (B, Cc):
         raise PwgbError(f"s2d_stream: x {tuple(x.shape)} and hist {tuple(hist.shape)} do not match")
-    co = int(cgo) if cgo else Cc * int(stride)
+    groups = int(groups)
+    if Cc % groups:
+        raise PwgbError(f"s2d_stream: {groups} groups do not divide {Cc} channels")
+    co = groups * int(cgo) if cgo else Cc * int(stride)
     shape = (B, co, int(rows_out))
     y = torch.empty(shape, device=x.device, dtype=torch.float32) if out is None else out
     if tuple(y.shape) != shape or not y.is_contiguous() or y.dtype != torch.float32:
         raise PwgbError(f"s2d_stream: out must be a contiguous float32 {shape} tensor")
     H = hist.shape[-1]
     prof = _Prof("s2d_stream", 0.0, 4.0 * (x.numel() + hist.numel() + y.numel()), f"B{B} C{Cc} n{n} H{H} s{stride}")
-    rc = capi.lib().pwgb_s2d_stream_forward(_p(x), _p(hist) if H else None, H, _p(y), B, Cc, n, int(stride), int(rows_out), int(cgo),
-                                            _stream())
-    capi.check(rc, "pwgb_s2d_stream_forward")
+    rc = capi.lib().pwgb_s2d_stream_grouped_forward(_p(x), _p(hist) if H else None, H, _p(y), B, Cc, groups, n, int(stride), int(rows_out),
+                                                    int(cgo), _stream())
+    capi.check(rc, "pwgb_s2d_stream_grouped_forward")
     prof.done()
     return y
 
 
 def conv1d_strided_stream(x, hist, w, bias=None, *, stride, pad_left, post_act=None, post_slope=0.0, t_out=None, out=None,
-                          mask=None):
+                          mask=None, groups=1):
     """A strided history conv on the FFMA engine (pwgb_conv1d_strided_stream_ext_forward): of the ``pad_left`` rows in
     front of x (B, cin, n), the last H read ``hist`` (B, cin, H) and the earlier ones are zero; output row o reads input
     rows o * stride - pad_left + k.  ``t_out`` defaults to every row the input allows; ``mask`` as in conv1d_stream.
-    Bit-identical to ``conv1d_raw`` with that stride on the explicit window (the generic FFMA kernel)."""
+    Bit-identical to ``conv1d_raw`` with that stride and ``groups`` on the explicit window (the generic FFMA kernel)."""
     x, w, hist = _dev(x, "x"), _dev(w, "w"), _dev(hist, "hist")
     B, cin, L = x.shape
     cout, cin_w, K = w.shape
-    if cin_w != cin or hist.dim() != 3 or tuple(hist.shape[:2]) != (B, cin):
+    groups = int(groups)
+    if cin_w * groups != cin or cout % groups or hist.dim() != 3 or tuple(hist.shape[:2]) != (B, cin):
         raise PwgbError(f"conv1d_strided_stream: x {tuple(x.shape)}, hist {tuple(hist.shape)} and weight {tuple(w.shape)} do not match")
     t_full = (L + pad_left - K) // stride + 1
     t_out = t_full if t_out is None else int(t_out)
@@ -659,13 +665,13 @@ def conv1d_strided_stream(x, hist, w, bias=None, *, stride, pad_left, post_act=N
         return y
     if bias is not None:
         bias = _dev(bias, "bias")
-    d = capi.Conv1dDesc(batch=B, cin=cin, cout=cout, t_in=L, t_out=t_out, kernel=K, stride=int(stride), dilation=1, groups=1,
+    d = capi.Conv1dDesc(batch=B, cin=cin, cout=cout, t_in=L, t_out=t_out, kernel=K, stride=int(stride), dilation=1, groups=groups,
                         pad_left=int(pad_left), pad_mode=capi.PAD_HISTORY, period=1, t_valid=L, pre_slope=1.0, pre_gate=0,
                         post_act=_ACT[post_act], post_slope=float(post_slope), out_scale=1.0, accumulate=0)
     ext = _stream_ext(B, cout, mask, None, 0)
     H = hist.shape[-1]
-    prof = _Prof("conv1d_strided_stream", 2.0 * B * cout * t_out * cin * K, 4.0 * (x.numel() + y.numel()),
-                 f"B{B} cin{cin} cout{cout} k{K} s{stride} T{t_out} H{H}")
+    prof = _Prof("conv1d_strided_stream", 2.0 * B * cout * t_out * cin_w * K, 4.0 * (x.numel() + y.numel()),
+                 f"B{B} cin{cin} cout{cout} k{K} s{stride} g{groups} T{t_out} H{H}")
     rc = capi.lib().pwgb_conv1d_strided_stream_ext_forward(C.byref(d), _p(x), _p(hist) if H else None, H, _p(w), _p(bias),
                                                             C.byref(ext) if ext is not None else None, _p(y), _stream())
     capi.check(rc, "pwgb_conv1d_strided_stream_ext_forward")
@@ -1687,6 +1693,50 @@ def vq_raw(z_e, codebook, *, indices=None, z_q=True, dec=True, l=None, global_ta
     capi.check(rc, "pwgb_vq_forward")
     prof.done()
     return indices, zq, dc
+
+
+def vq_stream(z_e, codebook, mask, *, l=None, l_hist=None, global_table=None, g=None, indices=None, dec=None):
+    """One pwgb_vq_stream_forward launch on a chunk of n frames -> (indices (B, n) int64, dec (B, D + Cl + Cg, n)): the
+    search and assembly of ``vq_raw`` with ``l`` (B, Cl, n) read E = l_hist.shape[-1] frames late from [l_hist | l],
+    and every frame outside the signal of ``mask`` = (frame, end, 1, lookahead) stored as +0.0 with index -1.
+    ``indices`` / ``dec``: optional output buffers."""
+    z_e, codebook = _dev(z_e, "z_e"), _dev(codebook, "codebook")
+    K, D = codebook.shape
+    if z_e.dim() != 3 or z_e.shape[1] != D:
+        raise PwgbError(f"vq_stream: z_e has shape {tuple(z_e.shape)}, the codebook {D} channels")
+    B, _, T = z_e.shape
+    Cl = Cg = ng = 0
+    E = 0
+    if l is not None:
+        l, l_hist = _dev(l, "l"), _dev(l_hist, "l_hist")
+        if l.dim() != 3 or l.shape[0] != B or l.shape[2] != T or l_hist.dim() != 3 or tuple(l_hist.shape[:2]) != tuple(l.shape[:2]):
+            raise PwgbError(f"vq_stream: l {tuple(l.shape)} / l_hist {tuple(l_hist.shape)} do not match the chunk's (B, T) = {(B, T)}")
+        Cl, E = l.shape[1], l_hist.shape[-1]
+    if g is not None:
+        if global_table is None:
+            raise PwgbError("vq_stream: global ids without a global table")
+        global_table = _dev(global_table, "global_table")
+        g = _long_tensor(g, (B,), "g")
+        ng, Cg = global_table.shape
+    if indices is None:
+        indices = torch.empty((B, T), device=z_e.device, dtype=torch.int64)
+    elif not indices.is_contiguous() or indices.dtype != torch.int64 or tuple(indices.shape) != (B, T):
+        raise PwgbError(f"vq_stream: indices must be a contiguous int64 {(B, T)} tensor")
+    shape = (B, D + Cl + Cg, T)
+    if dec is None:
+        dec = torch.empty(shape, device=z_e.device, dtype=torch.float32)
+    elif tuple(dec.shape) != shape or not dec.is_contiguous() or dec.dtype != torch.float32:
+        raise PwgbError(f"vq_stream: dec must be a contiguous float32 {shape} tensor")
+    if B * T == 0:
+        return indices, dec
+    ext = _stream_ext(B, D, mask, None, 0)
+    prof = _Prof("vq_stream", 2.0 * B * T * K * D, 4.0 * (B * T * D + K * D + dec.numel()), f"B{B} D{D} K{K} T{T} Cl{Cl} Cg{Cg} E{E}")
+    rc = capi.lib().pwgb_vq_stream_forward(_p(z_e), _p(codebook), K, _p(indices), _p(dec), _p(l) if Cl else None,
+                                           _p(l_hist) if Cl and E else None, E, Cl, _p(global_table) if g is not None else None, _p(g),
+                                           ng, Cg, C.byref(ext), B, D, T, _stream())
+    capi.check(rc, "pwgb_vq_stream_forward")
+    prof.done()
+    return indices, dec
 
 
 def vq_backward_raw(gdec, dim, local_channels, g=None, num_global=0, want_gz=True):

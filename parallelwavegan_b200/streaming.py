@@ -2,7 +2,8 @@
 causal Parallel WaveGAN, ``CausalHiFiGANStream`` a causal HiFi-GAN, ``CausalMelGANStream`` a causal (multi-band) MelGAN,
 and ``HiFiGANLookaheadStream``, ``PWGLookaheadStream``, ``MelGANLookaheadStream`` and ``UHiFiGANLookaheadStream`` a centred
 HiFi-GAN, a centred Parallel WaveGAN, a centred (multi-band) MelGAN and a centred U-Net HiFi-GAN (excitation pushed with
-its frames) with a fixed lookahead and a flush.
+its frames) with a fixed lookahead and a flush; ``VQVAELookaheadStream`` streams a VQ-VAE's wav2wav conversion (audio in,
+converted audio out) the same way.
 
 A causal generator's output for frame j depends only on frames <= j, so it can be synthesised as soon as frame j
 exists.  ``CausalPWGStream`` carries, per batch slot, everything the whole-utterance forward would read from before
@@ -1071,9 +1072,20 @@ class MelGANLookaheadStream(_Lookahead, _MelGANStream):
         ic = mods[1]
         # a fresh slot's input-conv history stays zero: those frames lie before the signal, where the edge policy reads
         self._setup(model, batch, use_graphs, ic.in_channels, ic.kernel_size[0] - 1, "zero")
+        self._plan(model)
+        self._counters()
+        self._count = [0] * self.B  # frames pushed per slot, on the host
+
+    # the frames the generator's input runs behind the frame counter (VQVAELookaheadStream's decoder: the encoder's
+    # lookahead); every mask and edge lookahead of the generator grows by that many frames at its rate
+    _shift = 0
+
+    def _plan(self, model):
+        """The generator's histories (``_build``) and its plan: the lookahead of each signal, in its own samples, from an
+        input conv whose [history | chunk] window starts K - 1 frames before the frame counter"""
+        ic = list(model.melgan)[1]
         self._build(model, centred=True)
         self.edge = model.pad_mode
-        # the plan: lookahead of each signal, in its own samples
         K_out = self.out_hist.shape[-1] + 1
         look = self.look_in = (ic.kernel_size[0] - 1) // 2
         need = [(look, 1)]  # (padding, input samples per frame) of every conv the pad applies to
@@ -1090,8 +1102,6 @@ class MelGANLookaheadStream(_Lookahead, _MelGANStream):
         need.append(((K_out - 1) // 2, self.hop))
         self.min_frames = max(P // rate + 1 for P, rate in need) if self.edge == "reflect" else 1
         self.delay = self.subbands * self.look_sub + self.pq_pad if self.pq_hist is not None else self.look_sub
-        self._counters()
-        self._count = [0] * self.B  # frames pushed per slot, on the host
 
     def _state(self):
         return self._histories() + [self.frame, self.end]
@@ -1105,31 +1115,39 @@ class MelGANLookaheadStream(_Lookahead, _MelGANStream):
         """One chunk: c (B, in_channels, n) -> (B, out_channels or 1, n * hop * subbands).  Advances the state."""
         n = c.shape[-1]
         ent = self._entry(n)
-        slope, edge = self.slope, self.edge
-        xin = self._input(ent, c)
+        y = self._generate(ent, self._input(ent, c), n)
+        self.frame += n
+        return y
+
+    def _generate(self, ent, xin, n):
+        """The generator on the window xin = [history | n frames] of the entry; carries its histories, not the counter"""
+        slope, edge, sh = self.slope, self.edge, self._shift
+
+        def mask(rate, look):
+            return self._mask(rate, look + sh * rate)
+
         # the input conv on [history | chunk]: input row r is frame t0 - (K - 1) + r
-        h = ops.conv1d_stream(xin, None, *self.w_in, pad_left=0, out=ent["h0"], mask=self._mask(1, self.look_in), edge=edge,
-                              in_lookahead=xin.shape[-1] - n)
+        h = ops.conv1d_stream(xin, None, *self.w_in, pad_left=0, out=ent["h0"], mask=mask(1, self.look_in), edge=edge,
+                              in_lookahead=xin.shape[-1] - n + sh)
         for lv, buf in zip(self.levels, ent["levels"]):
             rate = lv["rate"]
             x = ops.conv_transpose1d_stream(h, lv["up_hist"], lv["w"][0], lv["w"][1], stride=lv["stride"], pre_slope=slope,
-                                            out=buf["u"], mask=self._mask(rate, lv["look_u"]))
+                                            out=buf["u"], mask=mask(rate, lv["look_u"]))
             for j, st in enumerate(lv["stacks"]):
-                P, look, m = st["P"], st["look"], self._mask(rate, st["look"] + st["P"])
+                P, look, m = st["P"], st["look"], mask(rate, st["look"] + st["P"])
                 hh = ops.conv1d_stream(x, st["hist"], *st["w1"], pad_left=(st["k"] - 1) * st["d"], dilation=st["d"], pre_slope=slope,
-                                       out=buf["h"], mask=m, edge=edge, in_lookahead=look)
+                                       out=buf["h"], mask=m, edge=edge, in_lookahead=look + sh * rate)
                 # the skip reads the stack input P rows back, as h lags it
                 s = ops.conv1d_stream(x, st["hist"], *st["ws"], pad_left=P, t_out=x.shape[-1], out=buf["s"])
                 x = ops.conv1d_stream(hh, None, *st["w2"], pad_left=0, pre_slope=slope, residual=s, out=buf["x"][j], mask=m)
             h = x
         y = ops.conv1d_stream(h, self.out_hist, *self.w_out, pad_left=self.out_hist.shape[-1], pre_slope=slope, post_act=self.post_act,
-                              out=ent["y"], mask=self._mask(self.hop, self.look_sub), edge=edge, in_lookahead=self.look_last)
+                              out=ent["y"], mask=mask(self.hop, self.look_sub), edge=edge, in_lookahead=self.look_last + sh * self.hop)
         if self.pq_hist is not None:
             y = ops.conv_transpose1d_window_stream(y, self.pq_hist, self.w_syn, None, stride=self.subbands, padding=self.pq_pad,
                                                    out=ent["wave"])
             ops.stream_mask(y, self._mask(self.hop * self.subbands, self.delay))
         ops.stream_carry(ent["table"])
-        self.frame += n
         return y
 
     @torch.no_grad()
@@ -1158,6 +1176,260 @@ class MelGANLookaheadStream(_Lookahead, _MelGANStream):
                             f"({[self._count[b] for b in short]}); inference needs that many for the reflect padding")
         n = -(-self.delay // (self.hop * self.subbands))
         return self._flush(items, lambda: (n, self._zeros(self.B, self.in_channels, n)))
+
+
+class VQVAELookaheadStream(MelGANLookaheadStream):
+    """Streams the wav2wav conversion of a ``VQVAE`` (``decode(encode(x), l, g)``, the vctk / yesno ``vq1`` recipes:
+    a ``MelGANDiscriminator`` encoder and a centred ``MelGANGenerator`` decoder) chunk by chunk for ``batch``
+    independent slots, with a fixed lookahead of ``delay`` output samples.
+
+    ``push(x, l, g)`` takes the next n * hop samples of every slot (hop = prod(downsample_scales)), their n local
+    conditioning frames when the model has them, and the slots' target speaker ids when it has a global embedding, and
+    returns n * hop samples: the converted samples from t0 * hop - delay on (t0: the frames pushed before), with zeros
+    before sample 0.  ``flush(items)`` returns the last ``delay`` samples of those slots and restarts them; the other
+    slots continue as if no flush had happened.  For every slot, the concatenated pushes and flush equal ``[zeros(delay)
+    | model.decode(model.encode(all_x), all_l, g)]`` (``encode`` under ``torch.no_grad``, as inference runs it).  A
+    slot's speaker may not change inside a signal.
+
+    Two delayed-time chains (DESIGN.md §3.12, oracle/ref_vqvae_lookahead_stream.py), every launch masked outside its
+    signal (pwgb_stream_ext):
+
+    * the encoder on the audio: the reflect-padded input conv with the edge policy; each grouped strided conv (kernel K,
+      stride s, padding p) at the smallest output lookahead L' = ceil((L + K - p - s) / s) for which the push's last
+      output reads only samples that have arrived, on a window [the last L' s + p - L input samples | chunk] that starts
+      on a stride boundary of the whole signal's padded input; it runs as ``encode`` runs it: the grouped space-to-depth
+      gather read in place (pwgb_s2d_stream_grouped_forward) and the grouped masked stride-1 tensor-core conv where
+      ``conv1d`` takes that route, else the grouped masked FFMA strided history conv; then the two centred stride-1 convs.
+      The encoder's output lookahead is E whole frames (12 for [4, 4, 2, 2]);
+    * the bottleneck, one pwgb_vq_stream_forward per push: the nearest code of each frame (the search of ``encode``),
+      gathered with the local conditioning (after ``local_embed``, run on the pushed frames) read from an E-frame delay
+      line, and the target speaker's embedding;
+    * the decoder: the body of ``MelGANLookaheadStream`` on the frames the bottleneck wrote, E frames behind the frame
+      counter, so ``delay`` = E * hop + the decoder's lookahead: 1305 samples (54 ms at 24 kHz) for the vctk recipes,
+      1098 for yesno, the lookahead autograd measures on the model.
+
+    ``min_frames`` is the decoder's (the reflect padding of ``decode``); ``flush`` refuses a slot with fewer.  With
+    ``use_graphs`` each chunk length is captured once into a CUDA graph and replayed.  The weights and the conv engine
+    (``ops.ENGINE``, which picks each strided conv's route as ``encode`` does) are read when the stream is built and must
+    not change while it is used."""
+
+    def __init__(self, model, batch=1, use_graphs=True):
+        import math
+
+        from .layers import CausalConv1d
+        from .models import VQVAE, MelGANDiscriminator
+
+        name = "VQVAELookaheadStream"
+        if not isinstance(model, VQVAE):
+            raise PwgbError(f"{name}: expected a VQVAE")
+        enc, dec = model.encoder, model.decoder
+        if not isinstance(enc, MelGANDiscriminator):
+            raise PwgbError(f"{name}: the encoder is a {type(enc).__name__}; only MelGANDiscriminator is streamed")
+        mods = list(dec.melgan)
+        if isinstance(mods[0], CausalConv1d):
+            raise PwgbError(f"{name}: the decoder is causal (use_causal_conv=True); only the centred MelGANGenerator is streamed")
+        if dec.pqmf is not None:
+            raise PwgbError(f"{name}: a decoder with PQMF synthesis is not streamed")
+        if model.in_channels != 1:
+            raise PwgbError(f"{name}: in_channels {model.in_channels}; the stream takes one audio channel")
+        layers = list(enc.layers)
+        strided = [q[0] for q in layers[1:-2]]
+        down = math.prod(c.stride[0] for c in strided)
+        up = math.prod(c.stride[0] for c in mods if isinstance(c, torch.nn.ConvTranspose1d))
+        if down != up:
+            raise PwgbError(f"{name}: prod(downsample_scales) {down} != prod(upsample_scales) {up}: a frame of audio must give "
+                            "one frame of codes")
+        self._setup(model, batch, use_graphs, mods[1].in_channels, mods[1].kernel_size[0] - 1, "zero")
+        B, zeros = self.B, self._zeros
+        # encoder: the reflect-padded input conv, the strided convs, the two centred stride-1 convs
+        c0 = [q for q in layers[0] if isinstance(q, torch.nn.Conv1d)][0]
+        self.enc_edge, self.enc_slope = enc.pad_mode, enc.slope
+        self.w_e0 = wb(c0)
+        self.e_hist = zeros(B, 1, c0.kernel_size[0] - 1)
+        look = self.look_e0 = (c0.kernel_size[0] - 1) // 2
+        rate, self.enc = down, []
+        for conv in strided:
+            s, K, p, G = conv.stride[0], conv.kernel_size[0], conv.padding[0], conv.groups
+            Lq = -(-(look + K - p - s) // s)
+            w, b = wb(conv)
+            cin_g = conv.in_channels // G
+            cgo = (cin_g * s + 31) // 32 * 32
+            # the route of ops._conv1d_s2d under no_grad: the grouped space-to-depth and the stride-1 tensor-core conv
+            # (its channel conditions, the tensor-core engine), else the FFMA strided conv
+            s2d = ops.ENGINE != "simt" and (conv.out_channels // G) % 16 == 0 and cgo <= 2 * cin_g * s
+            rate //= s
+            self.enc.append(dict(stride=s, groups=G, kernel=K, w=(w, b), w2=ops.s2d_weight(w, s, cgo).contiguous() if s2d else None,
+                                 cgo=cgo, rate=rate, look=Lq, cout=conv.out_channels, hist=zeros(B, conv.in_channels, Lq * s + p - look)))
+            look = Lq
+        self.tail = []
+        for q in (layers[-2][0], layers[-1]):
+            K, p = q.kernel_size[0], q.padding[0]
+            look += K - 1 - p
+            self.tail.append(dict(w=wb(q), look=look, cout=q.out_channels, hist=zeros(B, q.in_channels, K - 1)))
+        self.E = look
+        # bottleneck
+        self.codebook = model.codebook.embedding.weight.detach()
+        self.local = hasattr(model, "local_embed")
+        self.w_le = wb(model.local_embed) if self.local and model.local_embed is not None else None
+        self.l_in = (model.local_embed.in_channels if self.w_le is not None else None) if self.local else 0
+        self.glob = hasattr(model, "global_embed")
+        self.g_table = model.global_embed.weight.detach() if self.glob else None
+        # decoder: MelGANLookaheadStream's plan and histories, E frames behind the counter
+        self._shift = self.E
+        self._plan(dec)
+        self.dec_delay = self.delay
+        self.delay = self.E * self.hop + self.dec_delay
+        Cl = dec.melgan[1].in_channels - self.codebook.shape[1] - (self.g_table.shape[1] if self.glob else 0)
+        if self.local and self.l_in is None:
+            self.l_in = Cl  # num_local_embeds without local_embed_dim: l goes to the decoder as it is
+        self.l_hist = zeros(B, Cl, self.E) if self.local else None
+        self._counters()
+        self._count = [0] * self.B
+        self._g = [None] * self.B  # the speaker of each slot's signal, on the host
+        self._nog = torch.zeros(self.B, device=self.dev, dtype=torch.int64)
+
+    def _state(self):
+        enc = [self.e_hist] + [lv["hist"] for lv in self.enc] + [t["hist"] for t in self.tail]
+        return self._histories() + enc + ([self.l_hist] if self.local else []) + [self.frame, self.end]
+
+    def reset(self, items=None):
+        super().reset(items)
+        for b in self._slots(items):
+            self._g[b] = None
+
+    def _new_entry(self, n, xin):
+        """The decoder's buffers and carry table (``MelGANLookaheadStream``), the encoder's and the bottleneck's, and the
+        carry table of the encoder's histories and the l delay line"""
+        ent = super()._new_entry(n, xin)
+        B, empty, hop = self.B, self._empty, self.hop
+        ent["e"] = empty(B, 1, n * hop)
+        ent["e0"] = empty(B, self.w_e0[0].shape[0], n * hop)
+        carry, x = [(ent["e"], self.e_hist)], ent["e0"]
+        ent["enc"] = []
+        for lv in self.enc:
+            t = n * lv["rate"]
+            buf = dict(d=empty(B, lv["cout"], t))
+            if lv["w2"] is not None:
+                buf["xs"] = empty(B, lv["groups"] * lv["cgo"], t + -(-lv["kernel"] // lv["stride"]) - 1)
+            carry.append((x, lv["hist"]))
+            x = buf["d"]
+            ent["enc"].append(buf)
+        ent["tail"] = []
+        for t in self.tail:
+            carry.append((x, t["hist"]))
+            x = empty(B, t["cout"], n)
+            ent["tail"].append(x)
+        if self.local:
+            ent["l"] = empty(B, self.l_hist.shape[1], n)
+            carry.append((ent["l"], self.l_hist))
+        ent["idx"] = torch.empty((B, n), device=self.dev, dtype=torch.int64)
+        ent["dec"] = empty(B, xin.shape[1], n)
+        ent["enc_table"] = ops.stream_carry_table(carry, self.dev)
+        return ent
+
+    def _strided(self, lv, buf, h):
+        """a strided conv on [hist | h], as ``MelGANDiscriminator.forward`` runs it on the whole signal: the window starts
+        on a stride boundary of the whole signal's padded input, and its outputs are masked"""
+        s, G, out = lv["stride"], lv["groups"], buf["d"]
+        mask = self._mask(lv["rate"], lv["look"])
+        if lv["w2"] is not None:
+            xs = ops.s2d_stream(h, lv["hist"], s, buf["xs"].shape[-1], lv["cgo"], out=buf["xs"], groups=G)
+            return ops.conv1d_stream(xs, None, lv["w2"], lv["w"][1], pad_left=0, post_act="lrelu", post_slope=self.enc_slope, out=out,
+                                     mask=mask, groups=G)
+        return ops.conv1d_strided_stream(h, lv["hist"], *lv["w"], stride=s, pad_left=lv["hist"].shape[-1], post_act="lrelu",
+                                         post_slope=self.enc_slope, t_out=out.shape[-1], out=out, mask=mask, groups=G)
+
+    def _step(self, e, l, g):
+        """One chunk: e (B, 1, n * hop), l (B, l_in, n), g (B,) -> (B, 1, n * hop).  Advances the state."""
+        n = e.shape[-1] // self.hop
+        ent = self._entry(n)
+        ent["e"].copy_(e)
+        h = ops.conv1d_stream(ent["e"], self.e_hist, *self.w_e0, pad_left=self.e_hist.shape[-1], post_act="lrelu",
+                              post_slope=self.enc_slope, out=ent["e0"], mask=self._mask(self.hop, self.look_e0), edge=self.enc_edge)
+        for lv, buf in zip(self.enc, ent["enc"]):
+            h = self._strided(lv, buf, h)
+        for i, (t, out) in enumerate(zip(self.tail, ent["tail"])):
+            act = dict(post_act="lrelu", post_slope=self.enc_slope) if i == 0 else {}
+            h = ops.conv1d_stream(h, t["hist"], *t["w"], pad_left=t["hist"].shape[-1], out=out, mask=self._mask(1, t["look"]), **act)
+        le = None
+        if self.local:
+            le = ops.conv1d(l, *self.w_le, out=ent["l"]) if self.w_le is not None else ent["l"].copy_(l)
+        _, dec = ops.vq_stream(h, self.codebook, self._mask(1, self.E), l=le, l_hist=self.l_hist, global_table=self.g_table,
+                               g=g if self.glob else None, indices=ent["idx"], dec=ent["dec"])
+        ops.stream_carry(ent["enc_table"])
+        y = self._generate(ent, self._input(ent, dec), n)
+        self.frame += n
+        return y
+
+    @torch.no_grad()
+    def push(self, x, l=None, g=None, return_indices=False):
+        """x: (B, n * hop) or (B, 1, n * hop) audio samples, n >= 1; l: (B, num_local_embeds, n) local conditioning frames
+        (required when the model has them, refused otherwise); g: (B,) target speaker ids (likewise).  Returns (B, 1, n *
+        hop) on the device: samples [t0 * hop - delay, (t0 + n) * hop - delay) of each slot's converted signal; with
+        ``return_indices`` also the (B, n) codes of frames t0 - E .. t0 + n - E - 1 (-1 outside the signal)."""
+        name = "VQVAELookaheadStream.push"
+        self._check_eval(self.model)
+        x = torch.as_tensor(x, dtype=torch.float32, device=self.dev)
+        if x.dim() == 3 and x.shape[1] == 1:
+            x = x[:, 0]
+        T = x.shape[-1] if x.dim() == 2 else 0
+        if x.dim() != 2 or x.shape[0] != self.B or T < self.hop or T % self.hop:
+            raise PwgbError(f"{name}: x must be ({self.B}, n * {self.hop}) or ({self.B}, 1, n * {self.hop}) samples with n >= 1, "
+                            f"got {tuple(x.shape)}")
+        n = T // self.hop
+        if self.local:
+            if l is None:
+                raise PwgbError(f"{name}: the model has local conditioning; l ({self.B}, {self.l_in}, {n}) is required")
+            l = torch.as_tensor(l, dtype=torch.float32, device=self.dev)
+            if tuple(l.shape) != (self.B, self.l_in, n):
+                raise PwgbError(f"{name}: l must be ({self.B}, {self.l_in}, {n}), got {tuple(l.shape)}")
+            l = l.contiguous()
+        elif l is not None:
+            raise PwgbError(f"{name}: the model has no local conditioning; l must be None")
+        else:
+            l = self._zeros(self.B, 0, n)
+        if self.glob:
+            if g is None:
+                raise PwgbError(f"{name}: the model has a global embedding; g ({self.B},) target speaker ids are required")
+            gl = [int(v) for v in torch.as_tensor(g).reshape(-1).tolist()]
+            if len(gl) != self.B:
+                raise PwgbError(f"{name}: g must hold {self.B} speaker ids, got {len(gl)}")
+            moved = [b for b in range(self.B) if self._g[b] is not None and self._g[b] != gl[b]]
+            if moved:
+                raise PwgbError(f"{name}: slots {moved} change speaker inside their signal ({[self._g[b] for b in moved]} -> "
+                                f"{[gl[b] for b in moved]}); reset them first")
+            g = torch.tensor(gl, device=self.dev, dtype=torch.int64)
+        elif g is not None:
+            raise PwgbError(f"{name}: the model has no global embedding; g must be None")
+        else:
+            g = self._nog
+        y = self._run(n, x.reshape(self.B, 1, T).contiguous(), l, g)
+        if self.glob:
+            self._g = gl
+        self._fresh = [False] * self.B
+        self._count = [k + n for k in self._count]
+        return (y, self._entries[n]["idx"].clone()) if return_indices else y
+
+    @torch.no_grad()
+    def flush(self, items=None):
+        """The last ``delay`` samples of slots ``items`` (an index, an iterable of indices or None for every slot), as
+        (len(items), 1, delay); the slots are then reset.  The flush push covers ceil(delay / hop) frames of zero audio and
+        conditioning with the slots' end frames set, so every conv reads its pad about the signal's last sample; the other
+        slots' state is restored around it, so they continue exactly as if it had not happened (DESIGN.md §3.12).  A slot
+        with fewer than ``min_frames`` frames raises, with nothing changed."""
+        items = list(self._slots(items))
+        short = [b for b in items if self._count[b] < self.min_frames]
+        if short:
+            raise PwgbError(f"VQVAELookaheadStream.flush: slots {short} hold fewer than {self.min_frames} frames "
+                            f"({[self._count[b] for b in short]}); decode needs that many for the reflect padding")
+        n = -(-self.delay // self.hop)
+        l_ch = self.l_in if self.local else 0
+
+        def inputs():
+            g = torch.tensor([v or 0 for v in self._g], device=self.dev, dtype=torch.int64) if self.glob else self._nog
+            return n, self._zeros(self.B, 1, n * self.hop), self._zeros(self.B, l_ch, n), g
+
+        return self._flush(items, inputs)
 
 
 class UHiFiGANLookaheadStream(_Lookahead, _HiFiGANStream):

@@ -11,7 +11,10 @@ for batch sizes B, chunks of 1, 4, 16 and 64 frames, CUDA graphs off and on.  MO
 * melgan_v1_centred, mb_melgan_v2_centred: the same two models centred (MelGANLookaheadStream), with their 1425- and
   2719-sample lookaheads;
 * uhifigan_opencpop_centred: the U-Net HiFi-GAN of the opencpop recipe (UHiFiGANLookaheadStream), hop 300 at 24 kHz,
-  excitation pushed with its frames, with its 16231-sample lookahead; 1- and 8-frame chunks.
+  excitation pushed with its frames, with its 16231-sample lookahead; 1- and 8-frame chunks;
+* vqvae_vctk_lg: the wav2wav conversion of the vctk local- and global-conditioned VQ-VAE recipe (VQVAELookaheadStream),
+  hop 64 at 24 kHz, audio and local conditioning pushed together, a target speaker per slot, with its 1305-sample
+  lookahead; 1-, 4- and 16-frame chunks.
 
 PWG and HiFi-GAN stream a 256-frame utterance (65536 samples per item), the centred ones then flush; the MelGANs
 stream a 263-frame one, a 7-frame opening push (their min_first_frames) then 256 frames, and flush; the centred
@@ -37,7 +40,10 @@ Every timed stream is checked against ``model.inference`` of each item in the sa
   takes conv1d_fewcout_long_kernel too, so the check is rel-L2 <= 1e-6 (bit identity holds below 4096 output-conv
   samples, tests/test_gpu_melgan_stream.py);
 * uhifigan_opencpop_centred: its inference's 32 -> 1 output conv has 76800 samples and takes conv1d_fewcout_long_kernel,
-  so the check is rel-L2 <= 1e-6 (bit identity holds below 4096 samples, tests/test_gpu_uhifigan_lookahead_stream.py).
+  so the check is rel-L2 <= 1e-6 (bit identity holds below 4096 samples, tests/test_gpu_uhifigan_lookahead_stream.py);
+* vqvae_vctk_lg: against decode(encode(x), l, g) of the batch, whose 32 -> 1 output conv has 16384 samples per item and
+  takes conv1d_fewcout_long_kernel, so the check is rel-L2 <= 1e-6 (bit identity holds below 4096 samples,
+  tests/test_gpu_vqvae_lookahead_stream.py).
 
 Prints the card name and power limit of the same run, as one JSON document.
 
@@ -57,7 +63,7 @@ from parallelwavegan_b200 import capi, models  # noqa: E402
 from parallelwavegan_b200 import synth_weights as synth  # noqa: E402
 from parallelwavegan_b200.layers import PQMF  # noqa: E402
 from parallelwavegan_b200.streaming import (CausalHiFiGANStream, CausalMelGANStream, CausalPWGStream, HiFiGANLookaheadStream,  # noqa: E402
-                                            MelGANLookaheadStream, PWGLookaheadStream, UHiFiGANLookaheadStream)
+                                            MelGANLookaheadStream, PWGLookaheadStream, UHiFiGANLookaheadStream, VQVAELookaheadStream)
 
 MELGAN = {
     "melgan_v1": dict(in_channels=80, out_channels=1, kernel_size=7, channels=512, upsample_scales=[8, 8, 2, 2], stacks=3,
@@ -69,13 +75,18 @@ MELGAN.update({f"{k}_centred": dict(v, use_causal_conv=False) for k, v in list(M
 UHIFIGAN_OPENCPOP = dict(in_channels=80, out_channels=1, channels=32, kernel_size=7, downsample_scales=[5, 5, 4, 3],
                          downsample_kernel_sizes=[10, 10, 8, 6], upsample_scales=[3, 4, 5, 5], upsample_kernel_sizes=[6, 8, 10, 10],
                          resblock_kernel_sizes=[3, 7, 11], resblock_dilations=[[1, 3, 5]] * 3)
-MODELS = ("pwg", "pwg_centred", "hifigan", "hifigan_centred", *MELGAN, "uhifigan_opencpop_centred")
+# egs/vctk/vq1/conf/local_conditioned_melgan_vae.v3.yaml generator_params
+VQVAE_VCTK_LG = dict(in_channels=1, out_channels=1, num_embeds=512, embed_dim=256, num_local_embeds=2, local_embed_dim=32,
+                     num_global_embeds=128, global_embed_dim=128, encoder_type="MelGANDiscriminator", decoder_type="MelGANGenerator",
+                     encoder_conf={"out_channels": 256, "downsample_scales": [4, 4, 2, 2], "max_downsample_channels": 1024},
+                     decoder_conf={"in_channels": 416, "upsample_scales": [4, 4, 2, 2], "channels": 512, "stacks": 3})
+MODELS = ("pwg", "pwg_centred", "hifigan", "hifigan_centred", *MELGAN, "uhifigan_opencpop_centred", "vqvae_vctk_lg")
 FRAMES = 256
 CHUNKS = (1, 4, 16, 64)
 PASSES = 2
 SR = 22050
-CHUNKS_OF = {"uhifigan_opencpop_centred": (1, 8)}
-SR_OF = {"uhifigan_opencpop_centred": 24000}
+CHUNKS_OF = {"uhifigan_opencpop_centred": (1, 8), "vqvae_vctk_lg": (1, 4, 16)}
+SR_OF = {"uhifigan_opencpop_centred": 24000, "vqvae_vctk_lg": 24000}
 
 
 def card():
@@ -108,6 +119,8 @@ def build(name, dev):
         m, scale = models.HiFiGANGenerator(use_causal_conv=False), 1.15
     elif name == "uhifigan_opencpop_centred":
         m, scale = models.UHiFiGANGenerator(**UHIFIGAN_OPENCPOP), 1.15
+    elif name == "vqvae_vctk_lg":
+        m, scale = models.VQVAE(**VQVAE_VCTK_LG), 1.15
     else:
         m, scale = models.MelGANGenerator(**MELGAN[name]), 1.0
     m.load_state_dict(synth.synth_state_dict([(k, tuple(v.shape)) for k, v in m.state_dict().items()], 31, scale))
@@ -124,7 +137,7 @@ class Workload:
     def __init__(self, name, m, B, dev):
         self.name, self.m = name, m
         self.melgan = name in MELGAN
-        self.flushes = self.melgan or name.endswith("_centred")
+        self.flushes = self.melgan or name.endswith("_centred") or name == "vqvae_vctk_lg"
         self.open = 7 if self.melgan and MELGAN[name]["use_causal_conv"] else 0
         self.frames = self.open + FRAMES
         g = torch.Generator().manual_seed(B)
@@ -137,6 +150,14 @@ class Workload:
             self.delay = UHiFiGANLookaheadStream(m, batch=B, use_graphs=False).delay
             self.ref = F.pad(torch.stack([m.inference(excitation=e[b], c=c[b]).t() for b in range(B)]), (self.delay, 0))
             self.whole = lambda: m(cw, None, e.unsqueeze(1))
+        elif name == "vqvae_vctk_lg":
+            hop = self.hop = 64
+            x = self.x = torch.randn(B, 1, FRAMES * hop, generator=g).to(dev) * 0.5
+            self.l = torch.randn(B, 2, FRAMES, generator=g).to(dev)
+            self.g = torch.arange(B, device=dev) * 7 % 128  # a different target speaker per slot
+            self.delay = VQVAELookaheadStream(m, batch=B, use_graphs=False).delay
+            self.whole = lambda: m.decode(m.encode(x), self.l, self.g)
+            self.ref = F.pad(self.whole(), (self.delay, 0))
         elif name in ("pwg", "pwg_centred"):
             hop = self.hop = m.upsample_factor
             z = self.z = torch.randn(B, 1, FRAMES * hop, generator=g).to(dev)
@@ -165,7 +186,8 @@ class Workload:
 
     def stream(self, B, graphs):
         cls = {"pwg": CausalPWGStream, "pwg_centred": PWGLookaheadStream, "hifigan": CausalHiFiGANStream,
-               "hifigan_centred": HiFiGANLookaheadStream, "uhifigan_opencpop_centred": UHiFiGANLookaheadStream}.get(self.name)
+               "hifigan_centred": HiFiGANLookaheadStream, "uhifigan_opencpop_centred": UHiFiGANLookaheadStream,
+               "vqvae_vctk_lg": VQVAELookaheadStream}.get(self.name)
         if cls is None:
             cls = CausalMelGANStream if MELGAN[self.name]["use_causal_conv"] else MelGANLookaheadStream
         return cls(self.m, batch=B, use_graphs=graphs)
@@ -175,6 +197,8 @@ class Workload:
             return st.push(self.c[:, j:j + n], self.z[:, :, j * self.hop:(j + n) * self.hop])
         if self.name == "uhifigan_opencpop_centred":
             return st.push(self.c[:, j:j + n], self.e[:, j * self.hop:(j + n) * self.hop])
+        if self.name == "vqvae_vctk_lg":
+            return st.push(self.x[..., j * self.hop:(j + n) * self.hop], self.l[..., j:j + n], self.g)
         return st.push(self.c[:, j:j + n])
 
     def check(self, s, B, n):
