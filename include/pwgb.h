@@ -341,6 +341,15 @@ PWGB_API int pwgb_resblock_pair_supported(const pwgb_resblock_desc* d);
 PWGB_API int pwgb_resblock_pair_plan(const pwgb_resblock_desc* d, int* info);
 PWGB_API int pwgb_resblock_pair_forward(const pwgb_resblock_desc* d, const float* x, const void* w1_packed, const float* b1,
                                const void* w2_packed, const float* b2, float* y, void* stream);
+/* The same pair at 128 or 256 channels, where the intermediate does not fit on chip: two tensor-core launches that hand
+ * it over in h_packed, a caller-owned workspace of 4 * batch * channels * t bytes (16-byte aligned), written by the
+ * first launch as the second one's bf16 hi/lo operand image and read by it with tensor copies.  Same arguments and
+ * result as pwgb_resblock_pair_forward, bit-identical to the two pwgb_conv1d_tc_forward calls it replaces.
+ * pwgb_resblock_pair_packed_supported() == 0 (other channel counts, t % 4 != 0, no tile plan in which the second conv
+ * stages its residual in shared memory): use those two calls instead. */
+PWGB_API int pwgb_resblock_pair_packed_supported(const pwgb_resblock_desc* d);
+PWGB_API int pwgb_resblock_pair_packed_forward(const pwgb_resblock_desc* d, const float* x, const void* w1_packed, const float* b1,
+                                               const void* w2_packed, const float* b2, void* h_packed, float* y, void* stream);
 
 /* ------------------------------------------------------------------------
  * Fused WaveNet residual layer of ParallelWaveGANGenerator (layers/residual_block.py:102-140,

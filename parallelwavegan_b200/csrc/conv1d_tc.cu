@@ -26,6 +26,7 @@
 #include <type_traits>
 
 #include "tc_common.cuh"
+#include "tma.cuh"
 
 namespace pwgb {
 
@@ -64,8 +65,14 @@ struct TcK {
   int split;
   int co_off;            // first output channel of this launch (N-chunked callers)
   int variant;           // debug (pwgb_debug_set(1, v)): bit 1 stages activations with cp.async instead of TMA,
-                         // bit 2 keeps the register epilogue
+                         // bit 2 keeps the register epilogue, bit 8 runs the 128- and 256-channel ResBlock pairs as
+                         // two fp32 launches (rb_packed_plan declines)
   int staged;            // plain epilogue through a shared-memory tile per consumer warpgroup (tc_plan)
+  // packed ResBlock intermediate (pk_plane, tc_common.cuh): pk_out, the epilogue writes lrelu(acc + bias, pk_slope) there
+  // as bf16 hi/lo (y: the packed image); pk_in, warp W_LDA lands each chunk's operand image from it with one tensor copy
+  // (tm_a) and the producers have no work
+  int pk_in, pk_out;
+  float pk_slope;
   // history launches (conv1d_tc_hist_kernel, pad_mode PWGB_PAD_HISTORY): input rows [-hist_len, 0) come from hist
   // (B, Cin, hist_len), or from sample 0 of x for an item whose rep flag is set
   const float* hist;
@@ -352,7 +359,8 @@ __device__ __forceinline__ void fill_main_chunk(const std::conditional_t<EDGE, T
 template <int MT, int NB16, bool HIST, bool EXT = false, bool EDGE = false>
 __device__ __forceinline__ void conv1d_tc_body(const TcKOf<EXT, EDGE>& p, const float* __restrict__ x, const float* __restrict__ x2,
                                                const uint4* __restrict__ wpk, const float* __restrict__ bias,
-                                               const float* __restrict__ res, float* __restrict__ y, float* __restrict__ y2) {
+                                               const float* __restrict__ res, float* __restrict__ y, float* __restrict__ y2,
+                                               const CUtensorMap* tm_a) {
   extern __shared__ __align__(128) unsigned char smem[];
   // layout: A[na] | B[nb] | raw staging[ns] | epilogue tiles[2 if staged] | barriers | bias
   constexpr int SLD = stage_ld(MT);
@@ -385,7 +393,7 @@ __device__ __forceinline__ void conv1d_tc_body(const TcKOf<EXT, EDGE>& p, const 
 
   if (tid == 0) {
     for (int i = 0; i < p.na; ++i) {
-      mbar_init(A_FULL(i), NPROD);
+      mbar_init(A_FULL(i), !HIST && p.pk_in ? 1 : NPROD);
       mbar_init(A_EMPTY(i), NCONS / 32);
     }
     for (int i = 0; i < p.nb; ++i) {
@@ -404,7 +412,9 @@ __device__ __forceinline__ void conv1d_tc_body(const TcKOf<EXT, EDGE>& p, const 
     bias_s[i] = bias ? __ldg(bias + (p.shuffle > 1 ? (p.co_off + i) / p.shuffle : p.co_off + i)) : 0.f;
   __syncthreads();
 
-  if (warp < W_CONS0 && !HIST && p.tma_act) {
+  if (warp < W_CONS0 && !HIST && p.pk_in) {
+    // packed activations: warp W_LDA lands the operand images, nothing to convert
+  } else if (warp < W_CONS0 && !HIST && p.tma_act) {
     // ===================== A producers, TMA-staged =====================
     // Warp W_LDA streams the raw fp32 rows of chunk q + ns - 1 into shared memory with bulk copies
     // (no LSU instructions, no registers); these 8 warps only convert landed stages to the bf16 hi/lo
@@ -633,6 +643,36 @@ __device__ __forceinline__ void conv1d_tc_body(const TcKOf<EXT, EDGE>& p, const 
           *sv = v * p.out_scale;
         }
       };
+      // Packed output (128-column tiles, MT = 1): the quad of lanes holding 8 channels of a row (2 each, of rows r and
+      // r + 8 of the fragment) transposes its split halves (two xor-shuffle steps) so that lane q stores one 16-byte run:
+      // hi of row r, lo of row r, hi of row r + 8, lo of row r + 8
+      auto pack_block = [&](const float* ab, int mb) {
+        const int q = lane & 3;
+        const bool q1 = q & 1, q2 = q & 2;
+        const int t = t0 + (wg * MT + mb) * 64 + wq * 16 + (lane >> 2) + (q2 ? 8 : 0);
+        const long long ld = 16LL * p.T_out;  // bytes between planes
+        unsigned char* dst = reinterpret_cast<unsigned char*>(y) + (pk_plane(b, p.Cout * (MC ? p.nco : 1), co_base) +
+                                                                    (q1 ? KC / 8 : 0)) * ld + 16LL * t;
+#pragma unroll
+        for (int n = 0; n < NACC / 4; ++n) {
+          const int col = 8 * n + 2 * q;
+          const float bs0 = bias_s[co_base - p.co_off + col], bs1 = bias_s[co_base - p.co_off + col + 1];
+          unsigned v0, v1, v2, v3;
+          split2(lrelu(ab[4 * n] + bs0, p.pk_slope), lrelu(ab[4 * n + 1] + bs1, p.pk_slope), v0, v1);
+          split2(lrelu(ab[4 * n + 2] + bs0, p.pk_slope), lrelu(ab[4 * n + 3] + bs1, p.pk_slope), v2, v3);
+          unsigned s0 = q2 ? v0 : v2, s1 = q2 ? v1 : v3;
+          s0 = __shfl_xor_sync(0xffffffffu, s0, 2);
+          s1 = __shfl_xor_sync(0xffffffffu, s1, 2);
+          if (q2) { v0 = s0; v1 = s1; } else { v2 = s0; v3 = s1; }
+          s0 = q1 ? v0 : v1;
+          s1 = q1 ? v2 : v3;
+          s0 = __shfl_xor_sync(0xffffffffu, s0, 1);
+          s1 = __shfl_xor_sync(0xffffffffu, s1, 1);
+          if (q1) { v0 = s0; v2 = s1; } else { v1 = s0; v3 = s1; }
+          // 8-channel group n: plane (n / 4) 2 KC / 8 + n % 4 from the tile's first
+          if (t < p.T_out) *reinterpret_cast<uint4*>(dst + ((n >> 2) * (2 * (KC / 8)) + (n & 3)) * ld) = make_uint4(v0, v1, v2, v3);
+        }
+      };
       // one 64-row block at a time, the mode chosen once per block (branching per element, or once for both blocks,
       // made ptxas spill at MT = 2)
       auto store_block = [&](auto mode, const float* ab, int mb) {
@@ -647,6 +687,8 @@ __device__ __forceinline__ void conv1d_tc_body(const TcKOf<EXT, EDGE>& p, const 
       for (int mb = 0; mb < MT; ++mb) {
         if (staged)
           stage_block(acc + mb * NACC, mb);
+        else if (!HIST && MT == 1 && p.pk_out)
+          pack_block(acc + mb * NACC, mb);
         else if (p.shuffle > 1)
           store_block(std::integral_constant<int, EPI_SHUFFLE>{}, acc + mb * NACC, mb);
         else if (p.wavenet)
@@ -683,7 +725,24 @@ __device__ __forceinline__ void conv1d_tc_body(const TcKOf<EXT, EDGE>& p, const 
     }
   } else if (warp == W_LDA) {
     // ===================== raw activation loader (TMA bulk row copies) =====================
-    if (!HIST && p.tma_act) {
+    if (!HIST && p.pk_in) {
+      // packed activations: chunk c of a tile is the box of 8 planes x R rows at its first plane, rows from t0 - padL
+      int buf = 0, ph = 0;
+      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+        int b, t0;
+        tile_origin(p, tile, TT, b, t0);
+        for (int c = 0; c < p.nchunks; ++c) {
+          mbar_wait(A_EMPTY(buf), ph ^ 1);
+          if (elect_one()) {
+            mbar_expect_tx(A_FULL(buf), (unsigned)p.a_bytes);
+            tma_load_3d(smem_u32(a_buf + (size_t)buf * p.a_bytes), tm_a, 0, t0 - p.padL, (int)pk_plane(b, p.Cin, c * KC),
+                        A_FULL(buf));
+          }
+          __syncwarp();
+          if (++buf == p.na) { buf = 0; ph ^= 1; }
+        }
+      }
+    } else if (!HIST && p.tma_act) {
       int s = 0, ph = 0;
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
         int b, t0;
@@ -720,17 +779,17 @@ template <int MT, int NB16>
 __global__ void __launch_bounds__(TC_THREADS, 1)
     conv1d_tc_kernel(const TcK p, const float* __restrict__ x, const float* __restrict__ x2,
                      const uint4* __restrict__ wpk, const float* __restrict__ bias, const float* __restrict__ res,
-                     float* __restrict__ y, float* __restrict__ y2) {
-  conv1d_tc_body<MT, NB16, false>(p, x, x2, wpk, bias, res, y, y2);
+                     float* __restrict__ y, float* __restrict__ y2, const __grid_constant__ CUtensorMap tm_a) {
+  conv1d_tc_body<MT, NB16, false>(p, x, x2, wpk, bias, res, y, y2, &tm_a);
 }
 
-// history launches (pwgb_conv1d_tc_stream_forward, the causal conv-transpose of a stream): x2 is unused
+// history launches (pwgb_conv1d_tc_stream_forward, the causal conv-transpose of a stream): x2 and tm_a are unused
 template <int MT, int NB16>
 __global__ void __launch_bounds__(TC_THREADS, 1)
     conv1d_tc_hist_kernel(const TcK p, const float* __restrict__ x, const float* __restrict__ x2,
                           const uint4* __restrict__ wpk, const float* __restrict__ bias, const float* __restrict__ res,
-                          float* __restrict__ y, float* __restrict__ y2) {
-  conv1d_tc_body<MT, NB16, true>(p, x, x2, wpk, bias, res, y, y2);
+                          float* __restrict__ y, float* __restrict__ y2, const __grid_constant__ CUtensorMap tm_a) {
+  conv1d_tc_body<MT, NB16, true>(p, x, x2, wpk, bias, res, y, y2, nullptr);
 }
 
 // history launches with a pwgb_stream_ext (pwgb_conv1d_tc_stream_ext_forward, the masked stream conv-transpose)
@@ -739,7 +798,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     conv1d_tc_ext_kernel(const TcKExt p, const float* __restrict__ x, const float* __restrict__ x2,
                          const uint4* __restrict__ wpk, const float* __restrict__ bias, const float* __restrict__ res,
                          float* __restrict__ y, float* __restrict__ y2) {
-  conv1d_tc_body<MT, NB16, true, true>(p, x, x2, wpk, bias, res, y, y2);
+  conv1d_tc_body<MT, NB16, true, true>(p, x, x2, wpk, bias, res, y, y2, nullptr);
 }
 
 // history launches with a pwgb_stream_ext edge policy (pwgb_conv1d_tc_stream_ext_forward with edge != 0)
@@ -748,7 +807,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     conv1d_tc_edge_kernel(const TcKEdge p, const float* __restrict__ x, const float* __restrict__ x2,
                           const uint4* __restrict__ wpk, const float* __restrict__ bias, const float* __restrict__ res,
                           float* __restrict__ y, float* __restrict__ y2) {
-  conv1d_tc_body<MT, NB16, true, true, true>(p, x, x2, wpk, bias, res, y, y2);
+  conv1d_tc_body<MT, NB16, true, true, true>(p, x, x2, wpk, bias, res, y, y2, nullptr);
 }
 
 static int g_tc_variant = 0;
@@ -768,9 +827,13 @@ static WtPlanInfo g_wt_last = {};
 // aux_c2: channels of the auxiliary 1x1 source (0 = none, else multiple of KC); split > 0 selects the
 // WaveNet epilogue.  pre_gate: d->cin is the number of gated channels, x holds 2*cin channels.
 // has_res: the launch adds a residual (selects the staged epilogue like an accumulate does).
+// pk_in: the activations are a packed intermediate (pk_plane) landed by tensor copies, with no raw stages.
 static int tc_plan(const pwgb_conv1d_desc* d, TcK& p, size_t& smem_bytes, int aux_c2 = 0, int split = 0, int nco_bias = 1,
-                   int has_res = 0) {
+                   int has_res = 0, int pk_in = 0) {
   p.variant = g_tc_variant;
+  p.pk_in = pk_in;
+  p.pk_out = 0;
+  p.pk_slope = 0.f;
   p.hist = nullptr;
   p.rep = nullptr;
   p.hist_len = 0;
@@ -844,6 +907,7 @@ static int tc_plan(const pwgb_conv1d_desc* d, TcK& p, size_t& smem_bytes, int au
         p.R = d->kernel * 128;
       }
       if (!p.win_mode && halo > 2048) continue;
+      if (pk_in && p.win_mode) continue;
       if (p.win_mode && halo <= p.MT * 128) continue;  // a contiguous tile is never larger in that case
       p.a_bytes = 2 * (KC / 8) * p.R * 16;
       p.R4 = (p.R + 6) & ~3;
@@ -857,8 +921,12 @@ static int tc_plan(const pwgb_conv1d_desc* d, TcK& p, size_t& smem_bytes, int au
       const size_t bias_bytes = 4 * (size_t)(nco_bias > 1 ? nco_bias * d->cout : TC_NMAX);  // bias of every column chunk of the launch
       const size_t A = (size_t)p.a_bytes, Bs = (size_t)p.b_bytes, S = (size_t)p.raw_bytes, slack = 1024 + bias_bytes;
       const size_t E = staged ? 2 * (size_t)d->cout * stage_ld(p.MT) * 4 : 0;
-      if (staged) {
-        if (!stage_shape(p.MT, d->cout)) continue;
+      if (staged && !stage_shape(p.MT, d->cout)) continue;
+      if (pk_in) {
+        // the raw stages' bytes go to weight stages
+        na = 2;
+        if (na * A + 4 * Bs + E + slack > budget) continue;
+      } else if (staged) {
         ns = p.tma_act ? 3 : 2;
         na = 2;
         if (na * A + ns * S + 4 * Bs + E + slack > budget) continue;
@@ -895,7 +963,8 @@ static int tc_plan(const pwgb_conv1d_desc* d, TcK& p, size_t& smem_bytes, int au
   return 0;
 }
 
-using TcKernel = void (*)(const TcK, const float*, const float*, const uint4*, const float*, const float*, float*, float*);
+using TcKernel = void (*)(const TcK, const float*, const float*, const uint4*, const float*, const float*, float*, float*,
+                         const CUtensorMap);
 
 // Every tile shape tc_plan produces: MT = 1 at any width of 16 .. TC_NMAX columns (the first 8), MT = 2 up to
 // TC_NMAX / 2 (the last 4).
@@ -944,7 +1013,7 @@ static TcKernel tc_kernel_for(int mt, int cout, bool hist) {
 template <class P>
 static int tc_launch(P& p, size_t bytes, const float* x, const void* packed_w, const float* bias,
                      const float* residual, float* y, cudaStream_t st, const float* x2 = nullptr,
-                     float* y2 = nullptr) {
+                     float* y2 = nullptr, const CUtensorMap* tm_a = nullptr) {
   if (p.B == 0 || p.T_out == 0) return PWGB_OK;
   constexpr bool ext = std::is_same<P, TcKExt>::value;
   constexpr bool edge = std::is_same<P, TcKEdge>::value;
@@ -981,7 +1050,16 @@ static int tc_launch(P& p, size_t bytes, const float* x, const void* packed_w, c
     p.staged = 0;  // bulk copies need 16-byte aligned rows: the register epilogue (the plan's tiles stay unused)
   g_tc_last = TcPlanInfo{p.MT, p.na, p.nb, p.ns, p.staged, p.tma_act, p.win_mode, p.nco};
   const int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
-  kernel<<<(unsigned)grid, TC_THREADS, bytes, st>>>(p, x, x2, (const uint4*)packed_w, bias, residual, y, y2);
+  if constexpr (edge || ext) {
+    kernel<<<(unsigned)grid, TC_THREADS, bytes, st>>>(p, x, x2, (const uint4*)packed_w, bias, residual, y, y2);
+  } else {
+    CUtensorMap tm;
+    if (tm_a)
+      tm = *tm_a;
+    else
+      memset(&tm, 0, sizeof(tm));
+    kernel<<<(unsigned)grid, TC_THREADS, bytes, st>>>(p, x, x2, (const uint4*)packed_w, bias, residual, y, y2, tm);
+  }
   return check_launch("conv1d_tc_kernel");
 }
 
@@ -1220,6 +1298,80 @@ extern "C" int pwgb_conv1d_tc_stream_ext_forward(const pwgb_conv1d_desc* d, cons
   if (const int rc = conv1d_stream_check(d, x, hist, hist_len, y)) return rc;
   if (const int rc = stream_ext_check(ext, residual, d->pad_mode)) return rc;
   return tc_forward(d, x, packed_w, bias, residual, y, stream, hist, replicate, hist_len, ext);
+}
+
+// ======================================================================================
+// A 128- or 256-channel HiFi-GAN ResBlock conv pair as two conv1d_tc launches that hand the intermediate over packed
+// (pk_plane): conv1's epilogue writes lrelu(conv1 + b1) already split, conv2 lands it with one tensor copy per chunk and
+// spends the raw stages' shared memory on weight stages.  conv2 must take the staged epilogue (the residual x).
+// ======================================================================================
+namespace pwgb {
+
+static int rb_packed_plan(const pwgb_resblock_desc* d, TcK& p1, size_t& bytes1, TcK& p2, size_t& bytes2) {
+  if (!d || (g_tc_variant & 8) || (d->channels != 128 && d->channels != 256) || d->batch < 0 || d->t <= 0 || d->t % 4 ||
+      d->kernel < 1 || d->kernel % 2 == 0 || d->dilation < 1)
+    return 0;
+  const int nco = d->channels / TC_NMAX;
+  pwgb_conv1d_desc c = {};
+  c.batch = d->batch;
+  c.cin = d->channels;
+  c.cout = TC_NMAX;
+  c.t_in = c.t_out = c.t_valid = d->t;
+  c.kernel = d->kernel;
+  c.stride = 1;
+  c.dilation = d->dilation;
+  c.groups = 1;
+  c.pad_left = (d->kernel - 1) / 2 * d->dilation;
+  c.pad_mode = PWGB_PAD_ZERO;
+  c.period = 1;
+  c.pre_slope = d->slope;
+  c.out_scale = 1.f;
+  if (!tc_plan(&c, p1, bytes1, 0, 0, nco) || p1.MT != 1) return 0;  // the packed epilogue: 128-column tiles
+  c.dilation = 1;
+  c.pad_left = (d->kernel - 1) / 2;
+  c.out_scale = d->out_scale;
+  c.accumulate = d->accumulate;
+  if (!tc_plan(&c, p2, bytes2, 0, 0, nco, 1, 1) || !p2.staged || p2.R > 256) return 0;  // one box: at most 256 rows
+  if ((long long)p1.total_tiles * nco > 0x7fffffffLL) return 0;
+  p1.pk_out = 1;
+  p1.pk_slope = d->slope;
+  for (TcK* p : {&p1, &p2}) {
+    p->xbs = p->ybs = p->rbs = (long long)d->channels * d->t;
+    if (nco > 1) {
+      p->nco = p->cpg = nco;
+      p->total_tiles *= nco;
+    }
+  }
+  return 1;
+}
+
+}  // namespace pwgb
+
+extern "C" int pwgb_resblock_pair_packed_supported(const pwgb_resblock_desc* d) {
+  TcK p1, p2;
+  size_t b1, b2;
+  return rb_packed_plan(d, p1, b1, p2, b2);
+}
+
+extern "C" int pwgb_resblock_pair_packed_forward(const pwgb_resblock_desc* d, const float* x, const void* w1_packed,
+                                                 const float* b1, const void* w2_packed, const float* b2, void* h_packed,
+                                                 float* y, void* stream) {
+  PWGB_CHECK_ARG(d && x && w1_packed && w2_packed && h_packed && y, "resblock_pair_packed: null argument");
+  TcK p1, p2;
+  size_t bytes1 = 0, bytes2 = 0;
+  PWGB_UNSUPPORTED_IF(!rb_packed_plan(d, p1, bytes1, p2, bytes2), "resblock_pair_packed: configuration not supported");
+  PWGB_CHECK_ARG(x != y, "resblock_pair_packed: y must not alias x (halo reads)");
+  PWGB_UNSUPPORTED_IF(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(h_packed)) & 15),
+                      "resblock_pair_packed: x, h_packed and y must be 16-byte aligned");
+  if (d->batch == 0) return PWGB_OK;
+  // the packed image as (8 channels, t rows, planes) bf16; a box is one chunk's 8 planes of R rows
+  CUtensorMap tm;
+  const unsigned long long dims[3] = {8ull, (unsigned long long)d->t, (unsigned long long)pk_plane(d->batch, d->channels, 0)};
+  const unsigned box[3] = {8u, (unsigned)p2.R, 2u * (KC / 8)};
+  if (const int rc = tma_make(&tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, 3, h_packed, dims, box)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (const int rc = tc_launch(p1, bytes1, x, w1_packed, b1, nullptr, static_cast<float*>(h_packed), st)) return rc;
+  return tc_launch(p2, bytes2, static_cast<const float*>(h_packed), w2_packed, b2, x, y, st, nullptr, nullptr, &tm);
 }
 
 // ======================================================================================

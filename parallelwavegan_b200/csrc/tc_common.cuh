@@ -136,6 +136,16 @@ __device__ __forceinline__ void store_split8(unsigned char* img, int R, int r, i
   *reinterpret_cast<uint4*>(img + ((size_t)(KC / 8 + g) * R + r) * 16) = lo;
 }
 
+// Packed activation handed from one conv's epilogue to the next conv's operand buffers (the HiFi-GAN ResBlock
+// intermediate): [B][C / KC][hi|lo][KC / 8][T][8] bf16, 4 C T bytes per item, no halo rows.  The 8-channel planes
+// ([T][8], 16 bytes per row) are numbered (b C / KC + c) 2 KC / 8 + hi|lo KC / 8 + g, so one box of 8 planes x R rows
+// from plane pk_plane(b, C, c KC) is exactly the operand image of chunk c (store_split8's layout); rows outside [0, T)
+// read as zero (TMA out-of-bounds fill), the convs' zero padding.  Plane of the hi bf16 of channels co .. co + 7
+// (co % 8 == 0); the lo plane is KC / 8 further.
+__host__ __device__ __forceinline__ long long pk_plane(int b, int C, int co) {
+  return ((long long)b * (C / KC) + co / KC) * (2 * (KC / 8)) + (co % KC) / 8;
+}
+
 // A landed raw fp32 stage (KC channel rows of `ld` floats; operand row r is raw[r + shift] of each) -> rows [0, rows) of
 // the operand image `img` of R rows, as lrelu(v, slope).  MASK: a row whose sample tbase + r is outside [0, tlim) is zero
 // padding (a stage filled by bulk copies holds no sample there); without it the stage already holds the padding.  NTHR

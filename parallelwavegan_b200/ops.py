@@ -195,9 +195,10 @@ def resblock_pair(x, w1, b1, w2, b2, *, kernel_size, dilation, slope, out=None, 
     """One HiFi-GAN ResBlock conv pair in one launch (pwgb_resblock_pair_forward), inference only:
         x' = conv_{k,1}(lrelu(conv_{k,d}(lrelu(x)) + b1)) + b2 + x     ("same" zero padding, LeakyReLU ``slope``)
     returned as ``out_scale * x'``, or written / added into ``out``.  Bit-identical to the two conv1d calls it replaces.
-    Returns None when the fused kernel does not serve the call (autograd, the FFMA engine, channel counts other than
-    32 / 64, t % 4 != 0, a conv1 halo too wide for the shared-memory plan, unaligned tensors): the caller then runs the
-    two convs."""
+    At 128 and 256 channels the pair runs as two launches (pwgb_resblock_pair_packed_forward) that hand the intermediate
+    over as the second conv's packed bf16 hi/lo operand image.  Returns None when neither serves the call (autograd, the
+    FFMA engine, other channel counts, t % 4 != 0, a conv1 halo too wide for the shared-memory plan, unaligned tensors):
+    the caller then runs the two convs."""
     if ENGINE == "simt" or _needs_grad(x, w1, b1, w2, b2):
         return None
     if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 3 and x.is_contiguous()):
@@ -219,7 +220,8 @@ def resblock_pair(x, w1, b1, w2, b2, *, kernel_size, dilation, slope, out=None, 
         d = _DESC_CACHE[dkey] = capi.ResBlockDesc(batch=B, channels=Cc, t=T, kernel=K, dilation=int(dilation), slope=float(slope),
                                                   out_scale=float(out_scale), accumulate=int(bool(accumulate)))
     L = capi.lib()
-    if not L.pwgb_resblock_pair_supported(C.byref(d)):
+    packed = not L.pwgb_resblock_pair_supported(C.byref(d))
+    if packed and not L.pwgb_resblock_pair_packed_supported(C.byref(d)):
         return None
     w1, w2 = _dev(w1, "w1"), _dev(w2, "w2")
     b1 = _dev(b1, "b1") if b1 is not None else None
@@ -229,6 +231,16 @@ def resblock_pair(x, w1, b1, w2, b2, *, kernel_size, dilation, slope, out=None, 
     if out.numel() == 0:
         return out  # an empty batch: nothing to compute (and no device pointers to pass)
     pk1, pk2 = packed_weight(w1), packed_weight(w2)
+    if packed:
+        h = torch.empty_like(x)  # the packed intermediate: 4 bytes per value, as fp32
+        # bytes: x (conv1's input and conv2's residual), the intermediate written and read, out written (and read)
+        prof = _Prof("resblock_pair_packed_tc", 2 * 2.0 * B * Cc * T * Cc * K,
+                     4.0 * (2 * x.numel() + 2 * h.numel() + out.numel() * (2 if accumulate else 1)),
+                     f"B{B} C{Cc} k{K} d{dilation} T{T}" if PROFILE is not None else "")
+        rc = L.pwgb_resblock_pair_packed_forward(C.byref(d), _p(x), _p(pk1), _p(b1), _p(pk2), _p(b2), _p(h), _p(out), _stream())
+        capi.check(rc, "pwgb_resblock_pair_packed_forward")
+        prof.done()
+        return out
     # FLOPs of both convs; bytes: x once, out written (and read too when accumulating), the intermediate stays on chip
     prof = _Prof("resblock_pair_tc", 2 * 2.0 * B * Cc * T * Cc * K, 4.0 * (x.numel() + out.numel() * (2 if accumulate else 1)),
                  f"B{B} C{Cc} k{K} d{dilation} T{T}" if PROFILE is not None else "")

@@ -2,7 +2,8 @@
 last column is the tile plan: MT (64-row blocks per warpgroup), na / nb / ns (operand buffers, weight stages, raw
 activation stages) and whether the epilogue went through the shared-memory tile (staged) or registers.  For fused ResBlock
 pairs (resblock_pair_tc) it is the output / conv rows per tile, conv1 operand buffers, weight stages of both rings and
-raw stages."""
+raw stages.  For the 128- and 256-channel pairs (resblock_pair_packed_tc: conv1 and conv2 with the packed intermediate
+between them) it is conv2's conv1d_tc plan."""
 import ctypes as C
 import os
 import sys
@@ -24,7 +25,7 @@ _done = ops._Prof.done
 
 def _done_with_plan(self):
     _done(self)
-    if ops.PROFILE is not None and self.name == "conv1d_tc":
+    if ops.PROFILE is not None and self.name in ("conv1d_tc", "resblock_pair_packed_tc"):
         v = (C.c_int * 5)()
         if capi.lib().pwgb_debug_get(1, C.cast(v, C.c_void_p), C.sizeof(v)) == 0:
             plans[len(ops.PROFILE) - 1] = f"MT{v[0]} na{v[1]} nb{v[2]} ns{v[3]} {'staged' if v[4] else 'reg'}"
