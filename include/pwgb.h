@@ -705,6 +705,38 @@ PWGB_API int pwgb_symbol_embed_forward(const void* idx, int idx_int64, long long
                                        long long idx_time_stride, const float* table, int num_embs, const float* spk_table,
                                        int num_spk, const long long* durations, int batch, int len, int channels, int t_out,
                                        float* y, void* stream);
+/* The embedding of a stream chunk of n frames (a centred discrete-symbol HiFi-GAN streamed with a fixed lookahead),
+ * written into columns [y_col0, y_col0 + n) of y (batch, channels, y_len): column y_col0 + j of item b is
+ * pwgb_symbol_embed_forward's column for symbol idx[b, 0, j] (same fp32 expression, same NaN rules), with the item's
+ * latched speaker.  spk_latch (batch) int32 holds each item's speaker row (-2: outside the speaker table); an item whose
+ * fresh flag is set takes the speaker of its chunk's first frame, idx[b, 1, 0], and latches it.  frame / end (batch)
+ * int32: frame j of item b is signal frame frame[b] + j, and a frame at or past end[b] is stored as +0.0 (the whole
+ * utterance's zero padding) without reading its index.  Without a speaker table spk_latch and fresh may be null. */
+PWGB_API int pwgb_symbol_embed_stream_forward(const void* idx, int idx_int64, long long idx_batch_stride, long long idx_chan_stride,
+                                              long long idx_time_stride, const float* table, int num_embs, const float* spk_table,
+                                              int num_spk, int* spk_latch, const int* fresh, const int* frame, const int* end, int batch,
+                                              int n, int channels, float* y, long long y_len, int y_col0, void* stream);
+/* The duration stream's per-item queue of (symbol id, duration) entries: ring_id / ring_d (batch, queue_len) int64,
+ * ring_state (batch, 4) int64 {tail, head, hoff, total} (entries [head, tail) queued at ring index i % queue_len, hoff
+ * frames of entry head consumed, total: the sum of every appended duration) and counts (batch, 2) int64 {queued frames,
+ * overflow flag}.
+ *   duration_queue_append: column j of x (batch, m) log-durations is symbol frame[b] - lookahead + j; a symbol inside
+ *     [0, end[b]) is final: its duration max(0, rint(exp(x) - offset)) (pwgb_duration_round's expression) and
+ *     ids[b * ids_ld + j] are appended in column order, and dur_out (batch, m) (may be null) gets the duration or -1.
+ *     A full queue sets the overflow flag and drops the entry.  zero_rule (batch) int32 flags, with m = 0: an item whose
+ *     total is 0 gets duration 1 for every queued entry (the length regulator's all-zero rule for the item alone).
+ *   symbol_regulate_stream_forward: columns [y_col0, y_col0 + n) of y (batch, channels, y_len) are the next n frames
+ *     of each item's queue, each pwgb_symbol_embed_forward's column of its entry's symbol (same fp32 expression, NaN for
+ *     an id outside the table); a frame past the queue, or at or past end[b] of the frame mask (frame j of item b is
+ *     frame[b] + j), is +0.0.  head / hoff and the queued count then advance by the frames consumed, so a symbol's run
+ *     may continue in a later call. */
+PWGB_API int pwgb_duration_queue_append(const float* x, int m, const long long* ids, long long ids_ld, const int* frame, const int* end,
+                                        int lookahead, float offset, const int* zero_rule, long long* ring_id, long long* ring_d,
+                                        int queue_len, long long* ring_state, long long* counts, long long* dur_out, int batch,
+                                        void* stream);
+PWGB_API int pwgb_symbol_regulate_stream_forward(const float* table, int num_embs, const long long* ring_id, const long long* ring_d,
+                                                 int queue_len, long long* ring_state, long long* counts, const int* frame, const int* end,
+                                                 int batch, int n, int channels, float* y, long long y_len, int y_col0, void* stream);
 PWGB_API size_t pwgb_symbol_embed_backward_workspace(int batch, int len, int channels, int num_embs);
 PWGB_API int pwgb_symbol_embed_backward(const float* gy, const float* gsym, const void* idx, int idx_int64, long long idx_batch_stride,
                                         long long idx_chan_stride, long long idx_time_stride, const long long* durations, int batch,

@@ -284,6 +284,14 @@ def lib():
     ll = C.c_longlong
     L.pwgb_symbol_embed_forward.restype = C.c_int
     L.pwgb_symbol_embed_forward.argtypes = [vp, C.c_int, ll, ll, ll, vp, C.c_int, vp, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]
+    L.pwgb_symbol_embed_stream_forward.restype = C.c_int
+    L.pwgb_symbol_embed_stream_forward.argtypes = [vp, C.c_int, ll, ll, ll, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int,
+                                                   C.c_int, vp, ll, C.c_int, vp]
+    L.pwgb_duration_queue_append.restype = C.c_int
+    L.pwgb_duration_queue_append.argtypes = [vp, C.c_int, vp, ll, vp, vp, C.c_int, C.c_float, vp, vp, vp, C.c_int, vp, vp, vp, C.c_int, vp]
+    L.pwgb_symbol_regulate_stream_forward.restype = C.c_int
+    L.pwgb_symbol_regulate_stream_forward.argtypes = [vp, C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, ll,
+                                                      C.c_int, vp]
     L.pwgb_symbol_embed_backward_workspace.restype = C.c_size_t
     L.pwgb_symbol_embed_backward_workspace.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
     L.pwgb_symbol_embed_backward.restype = C.c_int
@@ -359,7 +367,7 @@ EXPORTED_SYMBOLS = [
     "pwgb_tade_gate_backward",
     "pwgb_stft_amplitude_backward", "pwgb_mel_project_backward", "pwgb_gate_forward", "pwgb_gate_backward",
     "pwgb_upsample_fir_backward", "pwgb_upsample_fir_causal_backward", "pwgb_stft_loss_terms", "pwgb_stft_loss_dmag",
-    "pwgb_symbol_embed_forward", "pwgb_symbol_embed_backward_workspace", "pwgb_symbol_embed_backward",
+    "pwgb_symbol_embed_forward", "pwgb_symbol_embed_stream_forward", "pwgb_duration_queue_append", "pwgb_symbol_regulate_stream_forward", "pwgb_symbol_embed_backward_workspace", "pwgb_symbol_embed_backward",
     "pwgb_channel_layernorm_forward", "pwgb_channel_layernorm_backward_workspace", "pwgb_channel_layernorm_backward",
     "pwgb_duration_loss_forward", "pwgb_duration_loss_backward", "pwgb_duration_round", "pwgb_collate_runlength",
     "pwgb_vq_forward", "pwgb_vq_stream_forward", "pwgb_vq_backward",

@@ -57,9 +57,38 @@ struct EmbedArgs {
   float* y;  // (B, C, T_out)
 };
 
+// The (C, nf) tile of one block's frames, written to y[c * ld + f]: row[f] >= 0 is table row row[f] (+ speaker row g when
+// g >= 0), -1 zero, -2 NaN.  Table rows are read along C and the tile is written along time, both coalesced, through
+// the transposing tile in shared memory.  The one fp32 expression of every embed launch.
+__device__ __forceinline__ void embed_store_tile(const float* __restrict__ table, const float* __restrict__ spk, int C, const int* row,
+                                                 int g, float* __restrict__ y, long long ld, int nf, float (*tile)[SE_TT + 1]) {
+  const int tid = threadIdx.x;
+  for (int c0 = 0; c0 < C; c0 += SE_CC) {
+    for (int i = tid; i < SE_TT * SE_CC; i += 256) {
+      const int f = i / SE_CC, ch = i % SE_CC, c = c0 + ch;
+      const int r = row[f];
+      float v = 0.f;
+      if (c < C) {
+        if (r >= 0) {
+          v = __ldg(table + (long long)r * C + c);
+          if (g >= 0) v += __ldg(spk + (long long)g * C + c);
+        } else if (r == -2) {
+          v = __int_as_float(0x7fc00000);
+        }
+      }
+      tile[ch][f] = v;
+    }
+    __syncthreads();
+    for (int i = tid; i < SE_TT * SE_CC; i += 256) {
+      const int ch = i / SE_TT, f = i % SE_TT, c = c0 + ch;
+      if (c < C && f < nf) y[(long long)c * ld + f] = tile[ch][f];
+    }
+    __syncthreads();
+  }
+}
+
 // grid (ceil(T_out / 32), B), 256 threads.  Frame t of row b takes symbol j with prefix[j] <= t < prefix[j] + ds[j]
-// (durations) or j = t (none).  Table rows are read along C and the (C, 32) output tile is written along time, both
-// coalesced, through a transposing tile in shared memory.
+// (durations) or j = t (none).
 __global__ void __launch_bounds__(256) symbol_embed_kernel(const EmbedArgs a) {
   __shared__ int row[SE_TT];  // table row, -1: zero (past the row total), -2: NaN (index outside the table)
   __shared__ int sym[SE_TT];
@@ -100,28 +129,40 @@ __global__ void __launch_bounds__(256) symbol_embed_kernel(const EmbedArgs a) {
     row[tid] = r;
   }
   __syncthreads();
-  for (int c0 = 0; c0 < a.C; c0 += SE_CC) {
-    for (int i = tid; i < SE_TT * SE_CC; i += 256) {
-      const int f = i / SE_CC, ch = i % SE_CC, c = c0 + ch;
-      const int r = row[f];
-      float v = 0.f;
-      if (c < a.C) {
-        if (r >= 0) {
-          v = __ldg(a.table + (long long)r * a.C + c);
-          if (g >= 0) v += __ldg(a.spk + (long long)g * a.C + c);
-        } else if (r == -2) {
-          v = __int_as_float(0x7fc00000);
-        }
-      }
-      tile[ch][f] = v;
+  embed_store_tile(a.table, a.spk, a.C, row, g, a.y + (long long)b * a.C * a.T_out + t0, a.T_out, min(SE_TT, a.T_out - t0), tile);
+}
+
+// grid (ceil(n / 32), B), 256 threads: the chunk's frames t0 .. of item b through the same row table and tile store as
+// symbol_embed_kernel, into y's columns col0 + t (row stride ld)
+__global__ void __launch_bounds__(256, 4) symbol_embed_stream_kernel(const EmbedArgs a, int* __restrict__ latch, const int* __restrict__ fresh,
+                                                                  const int* __restrict__ frame, const int* __restrict__ end, long long ld,
+                                                                  int col0) {
+  __shared__ int row[SE_TT];
+  __shared__ float tile[SE_CC][SE_TT + 1];
+  const int b = blockIdx.y, t0 = blockIdx.x * SE_TT, tid = threadIdx.x;
+  // the speaker of a fresh item is its chunk's first frame's, latched by block 0; the other blocks of a fresh item read
+  // it from the chunk too, so no block reads the latch while it is written
+  int g = -1;
+  if (a.spk) {
+    if (__ldg(fresh + b)) {
+      const long long k = load_index(a.idx, a.idx64, (long long)b * a.ib + a.ic);
+      g = (k >= 0 && k < a.num_spk) ? (int)k : -2;
+      if (blockIdx.x == 0 && tid == 0) latch[b] = g;
+    } else {
+      g = latch[b];
     }
-    __syncthreads();
-    for (int i = tid; i < SE_TT * SE_CC; i += 256) {
-      const int ch = i / SE_TT, f = i % SE_TT, c = c0 + ch, t = t0 + f;
-      if (c < a.C && t < a.T_out) a.y[((long long)b * a.C + c) * a.T_out + t] = tile[ch][f];
-    }
-    __syncthreads();
   }
+  if (tid < SE_TT) {
+    const int j = t0 + tid;
+    int r = -1;
+    if (j < a.S && !stream_outside(frame, end, 1, 0, b, j)) {
+      const long long k = load_index(a.idx, a.idx64, (long long)b * a.ib + (long long)j * a.it);
+      r = (k >= 0 && k < a.num_embs && g != -2) ? (int)k : -2;
+    }
+    row[tid] = r;
+  }
+  __syncthreads();
+  embed_store_tile(a.table, a.spk, a.C, row, g, a.y + (long long)b * a.C * ld + col0 + t0, ld, min(SE_TT, a.S - t0), tile);
 }
 
 // ---- embed backward ------------------------------------------------------------------------------------------------
@@ -404,6 +445,12 @@ __global__ void duration_loss_backward_kernel(const float* __restrict__ x, const
     gx[i] = s * (x[i] - logf((float)d[i] + offset));
 }
 
+// DurationPredictor.inference's rounding of one log-domain duration: max(0, rint(exp(x) - offset))
+__device__ __forceinline__ long long round_duration(float x, float offset) {
+  const float r = rintf(expf(x) - offset);
+  return r > 0.f ? (long long)r : 0LL;
+}
+
 // one block: ds = max(0, rint(exp(x) - offset)) (x given), per-row totals, and with zero_rule the length regulator's
 // rule: when the whole batch sums to zero, rows summing to zero become all ones
 __global__ void __launch_bounds__(256) duration_round_kernel(const float* __restrict__ x, long long* __restrict__ ds,
@@ -419,8 +466,7 @@ __global__ void __launch_bounds__(256) duration_round_kernel(const float* __rest
       const long long o = (long long)b * S + j;
       long long v;
       if (x) {
-        const float r = rintf(expf(x[o]) - offset);
-        v = r > 0.f ? (long long)r : 0LL;
+        v = round_duration(x[o], offset);
         ds[o] = v;
       } else {
         v = ds[o];
@@ -440,6 +486,110 @@ __global__ void __launch_bounds__(256) duration_round_kernel(const float* __rest
     if (totals[b] != 0) continue;  // ds[ds.sum(dim=1).eq(0)] = 1: only rows summing to zero change
     for (int j = lane; j < S; j += 32) ds[(long long)b * S + j] = 1;
     if (lane == 0) totals[b] = S;
+  }
+}
+
+// ---- the duration stream's queue ----------------------------------------------------------------------------------
+// Per item b a ring of Q (symbol id, duration) entries and rs[b] = {tail, head, hoff, total}: entries [head, tail) are
+// queued (ring index i % Q), hoff frames of entry head are consumed, total is the sum of every appended duration;
+// counts[b] = {queued frames, overflow flag}.
+struct DurQueue {
+  long long* ring_id;
+  long long* ring_d;
+  int Q;
+  long long* rs;
+  long long* counts;
+};
+
+// one warp per item.  Column j of x (B, m) is symbol frame[b] - lookahead + j, final when inside [0, end[b]): its
+// rounded duration and ids[b, j] (row stride ids_ld) are appended in order; dur_out[b, j] gets the duration or -1.
+// zero_rule (B) flags (x == null, m == 0): an item whose total is 0 gets duration 1 for every queued entry (the length
+// regulator's rule for an item alone).
+__global__ void duration_queue_append_kernel(const float* __restrict__ x, int m, const long long* __restrict__ ids, long long ids_ld,
+                                             const int* __restrict__ frame, const int* __restrict__ end, int lookahead, float offset,
+                                             const int* __restrict__ zero_rule, DurQueue q, long long* __restrict__ dur_out) {
+  const int b = blockIdx.x;
+  if (threadIdx.x != 0) return;
+  long long* rs = q.rs + 4LL * b;
+  long long* ct = q.counts + 2LL * b;
+  long long tail = rs[0], total = rs[3], queued = ct[0];
+  const long long head = rs[1];
+  if (zero_rule && zero_rule[b] && total == 0) {
+    for (long long i = head; i < tail; ++i) q.ring_d[(long long)b * q.Q + i % q.Q] = 1;
+    queued = total = tail - head;  // no frame was consumed, so hoff is 0
+  }
+  for (int j = 0; j < m; ++j) {
+    const long long s = (long long)frame[b] - lookahead + j;
+    long long d = -1;
+    if (s >= 0 && s < (long long)end[b]) {
+      d = round_duration(x[(long long)b * m + j], offset);
+      if (tail - head >= q.Q) {
+        ct[1] = 1;  // overflow: the entry is dropped and the stream must be reset
+      } else {
+        const long long o = (long long)b * q.Q + tail % q.Q;
+        q.ring_id[o] = ids[(long long)b * ids_ld + j];
+        q.ring_d[o] = d;
+        ++tail;
+        queued += d;
+        total += d;
+      }
+    }
+    if (dur_out) dur_out[(long long)b * m + j] = d;
+  }
+  rs[0] = tail;
+  rs[3] = total;
+  ct[0] = queued;
+}
+
+// one block per item: frames [0, n) of the chunk are the next n frames of the item's queue, written into columns
+// col0 + t of y (B, C, ld) through symbol_embed_kernel's row table and tile store (a frame past the queue, or at or past
+// end[b] of the frame mask, is +0.0); then head / hoff advance by the frames consumed.
+__global__ void __launch_bounds__(256, 4) symbol_regulate_stream_kernel(const float* __restrict__ table, int num_embs, int C, DurQueue q,
+                                                                        const int* __restrict__ frame, const int* __restrict__ end, int n,
+                                                                        float* __restrict__ y, long long ld, int col0) {
+  __shared__ int row[SE_TT];
+  __shared__ float tile[SE_CC][SE_TT + 1];
+  const int b = blockIdx.x, tid = threadIdx.x;
+  long long* rs = q.rs + 4LL * b;
+  const long long tail = rs[0], head = rs[1], hoff = rs[2];
+  const long long* rid = q.ring_id + (long long)b * q.Q;
+  const long long* rd = q.ring_d + (long long)b * q.Q;
+  for (int t0 = 0; t0 < n; t0 += SE_TT) {
+    if (tid < SE_TT) {
+      const int f = t0 + tid;
+      int r = -1;
+      if (f < n && !stream_outside(frame, end, 1, 0, b, f)) {
+        long long rem = hoff + f, i = head;
+        for (; i < tail; ++i) {
+          const long long d = rd[i % q.Q] > 0 ? rd[i % q.Q] : 0;
+          if (rem < d) break;
+          rem -= d;
+        }
+        if (i < tail) {
+          const long long k = rid[i % q.Q];
+          r = (k >= 0 && k < num_embs) ? (int)k : -2;
+        }
+      }
+      row[tid] = r;
+    }
+    __syncthreads();
+    embed_store_tile(table, nullptr, C, row, -1, y + (long long)b * C * ld + col0 + t0, ld, min(SE_TT, n - t0), tile);
+  }
+  if (tid == 0) {
+    long long inside = (long long)end[b] - frame[b];
+    inside = inside < 0 ? 0 : (inside > n ? n : inside);
+    long long* ct = q.counts + 2LL * b;
+    const long long used = inside < ct[0] ? inside : ct[0];
+    long long rem = hoff + used, i = head;
+    while (i < tail) {
+      const long long d = rd[i % q.Q] > 0 ? rd[i % q.Q] : 0;
+      if (rem < d) break;
+      rem -= d;
+      ++i;
+    }
+    rs[1] = i;
+    rs[2] = i < tail ? rem : 0;
+    ct[0] -= used;
   }
 }
 
@@ -503,6 +653,53 @@ extern "C" int pwgb_symbol_embed_forward(const void* idx, int idx_int64, long lo
   dim3 grid((unsigned)ceil_div(t_out, SE_TT), (unsigned)batch);
   symbol_embed_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(a);
   return check_launch("symbol_embed_kernel");
+}
+
+extern "C" int pwgb_symbol_embed_stream_forward(const void* idx, int idx_int64, long long idx_batch_stride, long long idx_chan_stride,
+                                                long long idx_time_stride, const float* table, int num_embs, const float* spk_table,
+                                                int num_spk, int* spk_latch, const int* fresh, const int* frame, const int* end, int batch,
+                                                int n, int channels, float* y, long long y_len, int y_col0, void* stream) {
+  PWGB_CHECK_ARG(batch >= 0 && n >= 0 && channels > 0 && num_embs > 0, "symbol_embed_stream_forward: bad sizes");
+  PWGB_CHECK_ARG(y_col0 >= 0 && (long long)y_col0 + n <= y_len, "symbol_embed_stream_forward: columns [%d, %d) outside a %lld-column y",
+                 y_col0, y_col0 + n, y_len);
+  PWGB_CHECK_ARG(!spk_table || (num_spk > 0 && spk_latch && fresh), "symbol_embed_stream_forward: a speaker table needs rows, the latch and the fresh flags");
+  PWGB_UNSUPPORTED_IF(batch > 65535, "symbol_embed_stream_forward: batch %d > 65535", batch);
+  if (batch == 0 || n == 0) return PWGB_OK;
+  PWGB_CHECK_ARG(idx && table && y && frame && end, "symbol_embed_stream_forward: null pointer");
+  EmbedArgs a{idx, idx_int64, idx_batch_stride, idx_chan_stride, idx_time_stride, table, num_embs, spk_table, num_spk, nullptr,
+              batch, n, channels, n, y};
+  dim3 grid((unsigned)ceil_div(n, SE_TT), (unsigned)batch);
+  symbol_embed_stream_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(a, spk_latch, fresh, frame, end, y_len, y_col0);
+  return check_launch("symbol_embed_stream_kernel");
+}
+
+extern "C" int pwgb_duration_queue_append(const float* x, int m, const long long* ids, long long ids_ld, const int* frame, const int* end,
+                                          int lookahead, float offset, const int* zero_rule, long long* ring_id, long long* ring_d,
+                                          int queue_len, long long* ring_state, long long* counts, long long* dur_out, int batch,
+                                          void* stream) {
+  PWGB_CHECK_ARG(batch >= 0 && m >= 0 && lookahead >= 0 && queue_len > 0, "duration_queue_append: bad sizes");
+  PWGB_UNSUPPORTED_IF(batch > 65535, "duration_queue_append: batch %d > 65535", batch);
+  if (batch == 0) return PWGB_OK;
+  PWGB_CHECK_ARG(ring_id && ring_d && ring_state && counts && frame && end, "duration_queue_append: null pointer");
+  PWGB_CHECK_ARG(m == 0 || (x && ids && ids_ld >= m), "duration_queue_append: null or short input");
+  DurQueue q{ring_id, ring_d, queue_len, ring_state, counts};
+  duration_queue_append_kernel<<<batch, 32, 0, (cudaStream_t)stream>>>(x, m, ids, ids_ld, frame, end, lookahead, offset, zero_rule, q,
+                                                                       dur_out);
+  return check_launch("duration_queue_append_kernel");
+}
+
+extern "C" int pwgb_symbol_regulate_stream_forward(const float* table, int num_embs, const long long* ring_id, const long long* ring_d,
+                                                   int queue_len, long long* ring_state, long long* counts, const int* frame, const int* end,
+                                                   int batch, int n, int channels, float* y, long long y_len, int y_col0, void* stream) {
+  PWGB_CHECK_ARG(batch >= 0 && n >= 0 && channels > 0 && num_embs > 0 && queue_len > 0, "symbol_regulate_stream_forward: bad sizes");
+  PWGB_CHECK_ARG(y_col0 >= 0 && (long long)y_col0 + n <= y_len, "symbol_regulate_stream_forward: columns [%d, %d) outside a %lld-column y",
+                 y_col0, y_col0 + n, y_len);
+  PWGB_UNSUPPORTED_IF(batch > 65535, "symbol_regulate_stream_forward: batch %d > 65535", batch);
+  if (batch == 0 || n == 0) return PWGB_OK;
+  PWGB_CHECK_ARG(table && ring_id && ring_d && ring_state && counts && frame && end && y, "symbol_regulate_stream_forward: null pointer");
+  DurQueue q{const_cast<long long*>(ring_id), const_cast<long long*>(ring_d), queue_len, ring_state, counts};
+  symbol_regulate_stream_kernel<<<batch, 256, 0, (cudaStream_t)stream>>>(table, num_embs, channels, q, frame, end, n, y, y_len, y_col0);
+  return check_launch("symbol_regulate_stream_kernel");
 }
 
 extern "C" size_t pwgb_symbol_embed_backward_workspace(int batch, int len, int channels, int num_embs) {

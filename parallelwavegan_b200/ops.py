@@ -1546,6 +1546,88 @@ def symbol_embed_raw(c, table, spk_table=None, ds=None, t_out=None):
     return y
 
 
+def symbol_embed_stream(c, table, spk_table, latch, fresh, mask, y, col0):
+    """The embedding of a stream chunk, c (B, 1 or 2, n), into columns [col0, col0 + n) of y (B, C, L) --
+    pwgb_symbol_embed_stream_forward: symbol_embed_raw's columns (same fp32 expression and NaN rules) with each item's
+    speaker row from ``latch`` (B,) int32, which the items whose ``fresh`` (B,) int32 flag is set first take from their
+    chunk's first frame.  ``mask`` = (frame, end, ...): chunk frame j of item b is frame frame[b] + j, stored as +0.0 at
+    or past end[b].  Returns y."""
+    c, is64 = _index_tensor(c)
+    table = _dev(table, "table")
+    B, K, n = c.shape
+    frame, end = mask[0], mask[1]
+    ints = [(frame, "frame"), (end, "end")] + ([(latch, "latch"), (fresh, "fresh")] if spk_table is not None else [])
+    for t, name in ints:
+        if t.dtype != torch.int32 or not t.is_cuda or t.numel() != B or not t.is_contiguous():
+            raise PwgbError(f"symbol_embed_stream: {name} must be {B} contiguous int32 values on the device")
+    if spk_table is not None:
+        spk_table = _dev(spk_table, "spk_table")
+        if K < 2:
+            raise PwgbError("symbol_embed_stream: a speaker table needs (B, 2, n) indices")
+    C_ = table.shape[1]
+    if y.dim() != 3 or tuple(y.shape[:2]) != (B, C_) or not y.is_contiguous() or y.dtype != torch.float32:
+        raise PwgbError(f"symbol_embed_stream: y must be a contiguous float32 ({B}, {C_}, L) tensor, got {tuple(y.shape)}")
+    sb, sc, st = c.stride()
+    rc = capi.lib().pwgb_symbol_embed_stream_forward(
+        _p(c) if c.numel() else None, is64, sb, sc, st, _p(table), table.shape[0], _p(spk_table),
+        spk_table.shape[0] if spk_table is not None else 0, _p(latch) if spk_table is not None else None,
+        _p(fresh) if spk_table is not None else None, _p(frame), _p(end), B, n, C_, _p(y), y.shape[-1], int(col0), _stream())
+    capi.check(rc, "pwgb_symbol_embed_stream_forward")
+    return y
+
+
+class DurationQueue:
+    """The duration stream's per-slot device queue of (symbol id, duration) entries (pwgb_duration_queue_append /
+    pwgb_symbol_regulate_stream_forward): ``ring_id`` / ``ring_d`` (B, Q) int64, ``state`` (B, 4) int64 {tail, head, hoff,
+    total} and ``counts`` (B, 2) int64 {queued frames, overflow flag}.  All batch-leading, so a stream resets and
+    snapshots them with the rest of its state."""
+
+    def __init__(self, B, Q, device):
+        z = lambda *s: torch.zeros(s, device=device, dtype=torch.int64)  # noqa: E731
+        self.Q = int(Q)
+        self.ring_id, self.ring_d, self.state, self.counts = z(B, self.Q), z(B, self.Q), z(B, 4), z(B, 2)
+
+    def tensors(self):
+        return [self.ring_id, self.ring_d, self.state, self.counts]
+
+    def _args(self):
+        return _p(self.ring_id), _p(self.ring_d), self.Q, _p(self.state), _p(self.counts)
+
+
+def duration_queue_append(q, x, ids, mask, lookahead, offset, dur_out=None, zero_rule=None):
+    """Append the final symbols of x (B, m) log-durations (column j: symbol frame[b] - lookahead + j, final inside [0,
+    end[b]) of ``mask`` = (frame, end, ...)) with their ids (B, >= m) int64 to the queue ``q``; ``dur_out`` (B, m) int64
+    receives the rounded durations (-1: not final).  ``zero_rule`` (B,) int32 flags with x None: the all-zero rule of the
+    flagged slots whose total is 0.  One launch -- pwgb_duration_queue_append."""
+    frame, end = mask[0], mask[1]
+    B = frame.numel()
+    m = 0
+    if x is not None:
+        x, ids = _dev(x, "x"), ids
+        B, m = x.shape
+        if ids.dtype != torch.int64 or not ids.is_contiguous() or ids.shape[0] != B or ids.shape[1] < m:
+            raise PwgbError(f"duration_queue_append: ids must be a contiguous int64 ({B}, >= {m}) tensor")
+    if dur_out is not None and (dur_out.dtype != torch.int64 or tuple(dur_out.shape) != (B, m) or not dur_out.is_contiguous()):
+        raise PwgbError(f"duration_queue_append: dur_out must be a contiguous int64 {(B, m)} tensor")
+    rc = capi.lib().pwgb_duration_queue_append(_p(x) if m else None, m, _p(ids) if m else None, ids.shape[1] if m else 0, _p(frame), _p(end),
+                                               int(lookahead), float(offset), _p(zero_rule), *q._args(), _p(dur_out), B, _stream())
+    capi.check(rc, "pwgb_duration_queue_append")
+
+
+def symbol_regulate_stream(table, q, mask, y, col0, n):
+    """The next n frames of every slot's queue ``q``, embedded (table rows, channel-major) into columns [col0, col0 + n)
+    of y (B, C, L); frames at or past end[b] of ``mask`` = (frame, end, ...) are +0.0.  Advances the queue heads.  One
+    launch -- pwgb_symbol_regulate_stream_forward."""
+    table = _dev(table, "table")
+    B = y.shape[0]
+    if y.dim() != 3 or y.shape[1] != table.shape[1] or not y.is_contiguous() or y.dtype != torch.float32:
+        raise PwgbError(f"symbol_regulate_stream: y must be a contiguous float32 ({B}, {table.shape[1]}, L) tensor")
+    rc = capi.lib().pwgb_symbol_regulate_stream_forward(_p(table), table.shape[0], *q._args(), _p(mask[0]), _p(mask[1]), B, int(n),
+                                                        table.shape[1], _p(y), y.shape[-1], int(col0), _stream())
+    capi.check(rc, "pwgb_symbol_regulate_stream_forward")
+    return y
+
+
 def symbol_embed_backward_raw(gy, gsym, c, ds, t_out, num_embs, num_spk=0):
     """(d_table, d_spk_table or None) of symbol_embed_raw -- pwgb_symbol_embed_backward (deterministic)."""
     c, is64 = _index_tensor(c)

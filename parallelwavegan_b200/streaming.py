@@ -2,8 +2,10 @@
 causal Parallel WaveGAN, ``CausalHiFiGANStream`` a causal HiFi-GAN, ``CausalMelGANStream`` a causal (multi-band) MelGAN,
 and ``HiFiGANLookaheadStream``, ``PWGLookaheadStream``, ``MelGANLookaheadStream`` and ``UHiFiGANLookaheadStream`` a centred
 HiFi-GAN, a centred Parallel WaveGAN, a centred (multi-band) MelGAN and a centred U-Net HiFi-GAN (excitation pushed with
-its frames) with a fixed lookahead and a flush; ``VQVAELookaheadStream`` streams a VQ-VAE's wav2wav conversion (audio in,
-converted audio out) the same way.
+its frames) with a fixed lookahead and a flush; ``DiscreteSymbolHiFiGANLookaheadStream`` streams a discrete-symbol HiFi-GAN
+(HuBERT units in, audio out), ``DiscreteSymbolDurationLookaheadStream`` its duration model (durations predicted as the
+units arrive) and ``VQVAELookaheadStream`` a VQ-VAE's wav2wav conversion (audio in, converted audio out) the
+same way.
 
 A causal generator's output for frame j depends only on frames <= j, so it can be synthesised as soon as frame j
 exists.  ``CausalPWGStream`` carries, per batch slot, everything the whole-utterance forward would read from before
@@ -815,6 +817,311 @@ class HiFiGANLookaheadStream(_Lookahead, _HiFiGANStream):
         every slot, so ending one slot costs a ceil(delay / hop)-frame batch push (DESIGN.md §3.8)."""
         n = -(-self.delay // self.hop)
         return self._flush(list(self._slots(items)), lambda: (n, self._zeros(self.B, self.in_channels, n)))
+
+
+def _check_dsym_levels(name, model):
+    for i, up in enumerate(model.upsamples):
+        k, s = up[1].kernel_size[0], up[1].stride[0]
+        if k != 2 * s or s % 2:
+            raise PwgbError(f"{name}: upsampling level {i} has kernel {k} and stride {s}; the stream needs kernel 2 * stride "
+                            "and an even stride (padding (k - s) // 2 makes the whole utterance T * s + 1 samples long otherwise)")
+
+
+class DiscreteSymbolHiFiGANLookaheadStream(_Lookahead, _HiFiGANStream):
+    """Streams a ``DiscreteSymbolHiFiGANGenerator`` (HuBERT units in, audio out; the vctk / cvss_c ``hubert_voc1``
+    recipes without durations) chunk by chunk for ``batch`` independent slots, with a fixed lookahead of ``delay`` output
+    samples.
+
+    ``push(c)`` takes the next n >= 1 frames of every slot: (B, n, 2) (symbol, speaker) indices when the model has
+    speakers, else (B, n) or (B, n, 1); int64 or float32 (read as torch's ``c.long()``, NaN as an index outside the table).
+    It returns (B, out_channels, n * hop): the whole-utterance samples [t0 * hop - delay, (t0 + n) * hop - delay).
+    ``flush(items)`` returns the last ``delay`` samples of those slots and restarts them; the other slots continue as if
+    no flush had happened.  For every slot, the concatenated pushes and flush equal ``[zeros(delay) |
+    model.inference(all_frames)]``.
+
+    The body after input_conv is ``HiFiGANLookaheadStream``'s (DESIGN.md §3.8, §3.13).  The front end is one launch,
+    pwgb_symbol_embed_stream_forward, which writes the chunk's embedding into the input conv's [history | chunk] buffer
+    with the fp32 expression of the whole-utterance embed and stores +0.0 at frames past a flushed slot's end.  The
+    whole-utterance forward adds the speaker of an item's first frame to every frame, so each slot latches the speaker
+    of its first pushed frame on the device, inside the captured push, and a reset unlatches it.  Index and speaker
+    values outside their tables give NaN columns, as in the whole utterance.
+
+    ``delay`` comes from the module: 3482 samples (10.9 frames) for the 16 kHz recipes' scales (10, 8, 2, 2) and 4526 for
+    the 24 kHz ones (12, 10, 2, 2).  With ``use_graphs`` each chunk length (and index dtype) is captured once into a CUDA
+    graph and replayed.  The weights are read when the stream is built and must not change while it is used."""
+
+    def __init__(self, model, batch=1, use_graphs=True):
+        from .models import DiscreteSymbolHiFiGANGenerator
+
+        name = "DiscreteSymbolHiFiGANLookaheadStream"
+        if type(model) is not DiscreteSymbolHiFiGANGenerator:
+            raise PwgbError(f"{name}: expected a DiscreteSymbolHiFiGANGenerator, got {type(model).__name__}")
+        self.use_spk = model.num_spk_embs > 0
+        if self.use_spk and model.concat_spk_emb:
+            raise PwgbError(f"{name}: concat_spk_emb=True is not supported (the model's forward fails on it too)")
+        _check_dsym_levels(name, model)
+        ic = model.input_conv
+        self._setup(model, batch, use_graphs, ic.in_channels, ic.kernel_size[0] - 1, "zero", flags=self.use_spk)
+        self._build(model, centred=True)
+        self._counters()
+        self._nohist = self._zeros(self.B, ic.in_channels, 0)
+        self.table = model.emb.weight.detach()
+        self.spk_table = model.spk_emb.weight.detach() if self.use_spk else None
+        # each slot's latched speaker row (-2: outside the speaker table); valid while the slot's fresh flag is clear
+        self.latch = torch.zeros(self.B, device=self.dev, dtype=torch.int32) if self.use_spk else None
+        self._by_dtype = {}  # index dtype -> its chunk-length entries (a captured graph reads its own index buffer)
+
+    def _state(self):
+        return self._histories() + [self.frame, self.end] + ([self.latch] if self.use_spk else [])
+
+    def _step(self, c):
+        """One chunk: c (B, K, n) indices -> (B, out_channels, n * hop).  Advances the state."""
+        n = c.shape[-1]
+        ent = self._entry(n)
+        xin = ent["xin"]
+        P = self.cin_hist.shape[-1]
+        xin[:, :, :P].copy_(self.cin_hist)
+        ops.symbol_embed_stream(c, self.table, self.spk_table, self.latch, self.fresh, self._mask(1, 0), xin, P)
+        if self.use_spk:
+            self.fresh.zero_()
+        h = ops.conv1d_stream(xin, self._nohist, *self.w_in, pad_left=0, out=ent["h0"], mask=self._mask(1, self.look_in))
+        y = self._output(self._levels(h, ent, None), ent)
+        self.frame += n
+        return y
+
+    def _ids(self, c):
+        """(B, n[, K]) indices -> (B, K, n) contiguous on the device, int64 or float32"""
+        c = torch.as_tensor(c, device=self.dev)
+        if c.dtype not in (torch.float32, torch.int64):
+            c = c.long()
+        K = 2 if self.use_spk else 1
+        if c.dim() == 2 and not self.use_spk:
+            c = c.unsqueeze(-1)
+        if c.dim() != 3 or c.shape[0] != self.B or c.shape[1] < 1 or c.shape[2] != K:
+            want = f"({self.B}, n >= 1, 2)" if self.use_spk else f"({self.B}, n >= 1) or ({self.B}, n >= 1, 1)"
+            raise PwgbError(f"DiscreteSymbolHiFiGANLookaheadStream.push: c must be {want}, got {tuple(c.shape)}")
+        return c.transpose(1, 2).contiguous()
+
+    def _run(self, n, c):
+        self._entries = self._by_dtype.setdefault(c.dtype, {})
+        return super()._run(n, c)
+
+    @torch.no_grad()
+    def push(self, c):
+        """c: (B, n, 2) (symbol, speaker) indices, or (B, n) / (B, n, 1) symbols for a model without speakers.  Returns
+        (B, out_channels, n * hop) on the device: samples [t0 * hop - delay, (t0 + n) * hop - delay) of each slot's
+        utterance."""
+        self._check_eval(self.model)
+        c = self._ids(c)
+        return self._run(c.shape[-1], c)
+
+    @torch.no_grad()
+    def flush(self, items=None):
+        """The last ``delay`` samples of slots ``items`` (an index, an iterable of indices or None for every slot), computed
+        against the zero right padding, as (len(items), out_channels, delay); the slots are then reset.  The flush push
+        covers every slot with symbol 0 (the end mask stores the flushed slots' frames as +0.0); the other slots' state,
+        speaker latch and fresh flag included, is restored around it."""
+        items = list(self._slots(items))
+        n = -(-self.delay // self.hop)
+        fresh = self.fresh.clone() if self.use_spk else None
+        ids = torch.zeros((self.B, 2 if self.use_spk else 1, n), device=self.dev, dtype=torch.int64)
+        y = self._flush(items, lambda: (n, ids))
+        if self.use_spk:
+            keep = [b for b in range(self.B) if b not in items]
+            self.fresh[keep] = fresh[keep]
+        return y
+
+
+class DiscreteSymbolDurationLookaheadStream(_Lookahead, _HiFiGANStream):
+    """Streams a ``DiscreteSymbolDurationGenerator`` without speakers (the cvss_c ``hubert_voc1`` recipe: deduplicated
+    HuBERT units in, audio out, durations predicted as the units arrive) for ``batch`` independent slots.
+
+    ``push(c)`` takes the next m >= 1 symbols of every slot, (B, m) int64 or float32 (the deduplicated units ``synthesis``
+    takes), and returns (B, out_channels, n * hop): the next n frames' samples of every slot, n being the fewest frames
+    any slot has queued (all slots share one frame clock; a slot with more keeps them queued).  ``flush(items)`` ends
+    those slots one at a time and returns a list of their remaining samples, (out_channels, L_b) each; the other slots
+    continue as if no flush had happened.  For every slot, the concatenated pushes and flush equal ``[zeros(delay) |
+    model.inference(all_symbols)]``, and the durations finalised by the pushes and the flush (``last_durations`` after
+    each) equal ``synthesis``'s before its all-zero rule.
+
+    One push runs four stages (DESIGN.md §3.13):
+
+    * the duration predictor at symbol rate, in delayed time P = n_layers * (k - 1) / 2 symbols behind the symbols pushed:
+      the symbol embedding (pwgb_symbol_embed_stream_forward, +0.0 past the end) and each conv on [history | chunk]
+      (masked, ReLU epilogue), each LayerNorm masked to +0.0 outside the signal (LayerNorm of a zero column is beta, the
+      next conv's padding is zero), the Linear as the whole utterance runs it;
+    * the final symbols' durations, rounded as pwgb_duration_round rounds them, appended with their ids to a per-slot
+      device queue (pwgb_duration_queue_append), which also keeps the queued frame count and the running total;
+    * one device-to-host read of the B queued counts (the whole utterance synchronises at the same point), then the body
+      advances every slot by n frames in power-of-two pushes (at most log2 captured lengths), each filling the input
+      conv's [history | chunk] buffer from the queues (pwgb_symbol_regulate_stream_forward); a symbol's run may start in
+      one push and end in a later one;
+    * the body is ``HiFiGANLookaheadStream``'s, ``delay`` samples behind.
+
+    The flush of a slot sets its symbol end, pushes P masked symbols, applies the all-zero rule if the slot's total is
+    still 0 (its queued symbols, all kept, get duration 1), drains its queue through the body and runs the body's flush.
+    A slot that never produces frames stalls the others; ``max_queue`` bounds each slot's queue, and a push that would
+    overflow it raises.  The weights are read when the stream is built and must not change while it is used."""
+
+    def __init__(self, model, batch=1, use_graphs=True, max_queue=4096):
+        from .models import DiscreteSymbolDurationGenerator
+
+        name = "DiscreteSymbolDurationLookaheadStream"
+        if type(model) is not DiscreteSymbolDurationGenerator:
+            raise PwgbError(f"{name}: expected a DiscreteSymbolDurationGenerator, got {type(model).__name__}")
+        if model.num_spk_embs > 0:
+            raise PwgbError(f"{name}: a duration model with speakers is not supported (its forward fails too: the predictor "
+                            "is built for in_channels + spk_emb_dim inputs)")
+        _check_dsym_levels(name, model)
+        ic = model.input_conv
+        self._setup(model, batch, use_graphs, ic.in_channels, ic.kernel_size[0] - 1, "zero")
+        self._build(model, centred=True)
+        self._counters()
+        self._nohist = self._zeros(self.B, ic.in_channels, 0)
+        self.table = model.emb.weight.detach()
+        dp = model.duration_predictor
+        self.offset = float(dp.offset)
+        self.pred = []
+        for f in dp.conv:
+            conv, ln = f[0], f[2]
+            if conv.kernel_size[0] % 2 == 0:
+                raise PwgbError(f"{name}: the duration predictor's kernel must be odd")
+            self.pred.append(dict(w=wb(conv), k=conv.kernel_size[0], ln=(ln.weight.detach(), ln.bias.detach(), float(ln.eps)),
+                                  hist=self._zeros(self.B, conv.in_channels, conv.kernel_size[0] - 1)))
+        self.P = sum((L["k"] - 1) // 2 for L in self.pred)
+        lin = dp.linear
+        self.w_lin = (lin.weight.detach().reshape(1, lin.in_features, 1).contiguous(), lin.bias.detach())
+        self.sframe = torch.zeros(self.B, device=self.dev, dtype=torch.int32)
+        self.send = torch.full((self.B,), self.OPEN, device=self.dev, dtype=torch.int32)
+        self.id_hist = torch.zeros((self.B, self.P), device=self.dev, dtype=torch.int64)
+        self.max_queue = int(max_queue)
+        self.queue = ops.DurationQueue(self.B, self.max_queue, self.dev)
+        self._last, self._last_flush = None, None
+        self._len = {}
+
+    def _state(self):
+        return (self._histories() + [self.frame, self.end, self.sframe, self.send, self.id_hist] + [L["hist"] for L in self.pred]
+                + self.queue.tensors())
+
+    def reset(self, items=None):
+        super().reset(items)
+        for b in self._slots(items):
+            self.send[b] = self.OPEN
+
+    # ---------------------------------------------------------------------------------------------------- predictor
+    def _predict(self, ids):
+        """The predictor on m symbols ids (B, 1, m) int64 of every slot; appends the final symbols to the queues and keeps
+        their durations (B, m) (-1: not final) in ``_last``."""
+        m = ids.shape[-1]
+        smask = lambda look: (self.sframe, self.send, 1, look)  # noqa: E731
+        x = self._empty(self.B, self.table.shape[1], m)
+        ops.symbol_embed_stream(ids, self.table, None, None, None, smask(0), x, 0)
+        look = 0
+        for L in self.pred:
+            k, hist = L["k"], L["hist"]
+            look += (k - 1) // 2
+            y = ops.conv1d_stream(x, hist, *L["w"], pad_left=k - 1, post_act="lrelu", post_slope=0.0, mask=smask(look))
+            hist.copy_(torch.cat([hist, x], -1)[:, :, -(k - 1):] if k > 1 else hist)
+            x = ops.stream_mask(ops.channel_layer_norm(y, *L["ln"]), smask(look))
+        logd = ops.conv1d_raw(x, *self.w_lin).reshape(self.B, m)
+        idw = torch.cat([self.id_hist, ids[:, 0]], -1)  # column j: symbol sframe - P + j
+        if self.P:
+            self.id_hist.copy_(idw[:, -self.P:])
+        self._last, self._last_flush = torch.empty((self.B, m), device=self.dev, dtype=torch.int64), None
+        ops.duration_queue_append(self.queue, logd, idw, smask(self.P), self.P, self.offset, dur_out=self._last)
+        self.sframe += m
+
+    def _queued(self, slots=None):
+        """the queued frame counts on the host (one device-to-host read); raises on an overflowed queue"""
+        q = self.queue.counts.cpu()
+        over = [b for b in (range(self.B) if slots is None else slots) if q[b, 1]]
+        if over:
+            raise PwgbError(f"DiscreteSymbolDurationLookaheadStream: the queue of slot(s) {over} overflowed max_queue = {self.max_queue} "
+                            "symbols (a slot stalls while another makes no frames); build the stream with a larger max_queue and "
+                            "reset those slots")
+        return q[:, 0]
+
+    @property
+    def last_durations(self):
+        """the durations finalised by the last push or flush, one int64 tensor per slot (a list: slots finalise different
+        counts while their first P symbols are in flight)"""
+        if self._last_flush is not None:
+            return self._last_flush
+        if self._last is None:
+            return [torch.zeros(0, dtype=torch.int64) for _ in range(self.B)]
+        d = self._last.cpu()
+        return [row[row >= 0] for row in d]
+
+    # ---------------------------------------------------------------------------------------------------- body
+    def _step(self, tn):
+        """n frames of every slot's queue (n: tn's length) -> (B, out_channels, n * hop).  Advances the state."""
+        n = tn.shape[0]
+        ent = self._entry(n)
+        xin = ent["xin"]
+        P = self.cin_hist.shape[-1]
+        xin[:, :, :P].copy_(self.cin_hist)
+        ops.symbol_regulate_stream(self.table, self.queue, self._mask(1, 0), xin, P, n)
+        h = ops.conv1d_stream(xin, self._nohist, *self.w_in, pad_left=0, out=ent["h0"], mask=self._mask(1, self.look_in))
+        y = self._output(self._levels(h, ent, None), ent)
+        self.frame += n
+        return y
+
+    def _body(self, n):
+        """n frames in power-of-two pushes, largest first"""
+        ys = []
+        p = 1 << max(int(n).bit_length() - 1, 0)
+        while n > 0:
+            if p <= n:
+                if p not in self._len:
+                    self._len[p] = torch.empty(p, device=self.dev)
+                ys.append(self._run(p, self._len[p]))
+                n -= p
+            p >>= 1
+        return torch.cat(ys, -1) if ys else self._zeros(self.B, self.out_channels, 0)
+
+    @torch.no_grad()
+    def push(self, c):
+        """c: (B, m) symbols (or (B, m, 1)).  Returns (B, out_channels, n * hop) on the device (n may be 0)."""
+        self._check_eval(self.model)
+        c = torch.as_tensor(c, device=self.dev)
+        if c.dim() == 3 and c.shape[-1] == 1:
+            c = c[..., 0]
+        if c.dim() != 2 or c.shape[0] != self.B or c.shape[1] < 1:
+            raise PwgbError(f"DiscreteSymbolDurationLookaheadStream.push: c must be ({self.B}, m >= 1) symbols, got {tuple(c.shape)}")
+        if c.dtype not in (torch.float32, torch.int64):
+            c = c.long()
+        self._predict(c.unsqueeze(1).contiguous())
+        return self._body(int(self._queued().min()))
+
+    @torch.no_grad()
+    def flush(self, items=None):
+        """The remaining samples of slots ``items`` (an index, an iterable of indices or None for every slot), as a list of
+        (out_channels, L_b) tensors; the slots are then reset.  Each slot is flushed alone, with the other slots' state
+        restored around it; ``last_durations`` then holds the durations the flush finalised."""
+        items = list(self._slots(items))
+        outs, last = [], [torch.zeros(0, dtype=torch.int64) for _ in range(self.B)]
+        for b in items:
+            keep = [i for i in range(self.B) if i != b]
+            snap = [t[keep].clone() for t in self._state()]
+            self.send[b] = self.sframe[b]
+            if self.P:
+                self._predict(torch.zeros((self.B, 1, self.P), device=self.dev, dtype=torch.int64))
+                last[b] = self.last_durations[b]
+            zr = torch.zeros(self.B, device=self.dev, dtype=torch.int32)
+            zr[b] = 1
+            ops.duration_queue_append(self.queue, None, None, (self.frame, self.end), 0, self.offset, zero_rule=zr)
+            ys = [self._body(int(self._queued([b])[b]))]
+            self.end[b] = self.frame[b]
+            n = -(-self.delay // self.hop)
+            if n not in self._len:
+                self._len[n] = torch.empty(n, device=self.dev)
+            ys.append(self._run(n, self._len[n])[:, :, :self.delay])
+            outs.append(torch.cat(ys, -1)[b])
+            for t, sn in zip(self._state(), snap):
+                t[keep] = sn
+            self.reset(b)
+        self._last_flush = last
+        return outs
 
 
 class _MelGANStream(_ChunkStream):

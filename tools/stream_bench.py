@@ -14,7 +14,13 @@ for batch sizes B, chunks of 1, 4, 16 and 64 frames, CUDA graphs off and on.  MO
   excitation pushed with its frames, with its 16231-sample lookahead; 1- and 8-frame chunks;
 * vqvae_vctk_lg: the wav2wav conversion of the vctk local- and global-conditioned VQ-VAE recipe (VQVAELookaheadStream),
   hop 64 at 24 kHz, audio and local conditioning pushed together, a target speaker per slot, with its 1305-sample
-  lookahead; 1-, 4- and 16-frame chunks.
+  lookahead; 1-, 4- and 16-frame chunks;
+* dsym_vctk_centred: the discrete-symbol HiFi-GAN of the vctk hubert_voc1 recipe (DiscreteSymbolHiFiGANLookaheadStream),
+  HuBERT units and a speaker per slot, hop 320 at 16 kHz, with its 3482-sample lookahead; 1-, 4- and 16-frame chunks;
+* dsym_dur_cvss: the duration model of the cvss_c hubert_voc1 recipe (DiscreteSymbolDurationLookaheadStream): 128
+  deduplicated units per item (the predictor's bias set so that durations are 0 .. 4 frames), pushed 1, 4 or 16 units
+  at a time; a push yields however many frames every slot has queued, so its latency is per push of units and the
+  check compares each slot's audio and durations with its own ``synthesis``.
 
 PWG and HiFi-GAN stream a 256-frame utterance (65536 samples per item), the centred ones then flush; the MelGANs
 stream a 263-frame one, a 7-frame opening push (their min_first_frames) then 256 frames, and flush; the centred
@@ -22,7 +28,7 @@ MelGANs stream 256 frames and flush.  Each configuration streams its utterance P
 times.  A push is timed with CUDA events recorded around it and a synchronise after it, so a latency includes the
 host's launch work whenever the GPU waits for it.  Reported: median / min / max latency of the chunk pushes, the
 streamed real-time factor (GPU time of all pushes, and the flush, whose own latency is reported too, over the audio's duration at 22050 Hz: below 1 is
-faster than real time; 24000 Hz for the U-Net HiFi-GAN), the libpwgb kernel launches of one steady-state eager push (the few torch copies are not
+faster than real time; 24000 Hz for the U-Net HiFi-GAN and the VQ-VAE, 16000 Hz for the discrete-symbol HiFi-GAN), the libpwgb kernel launches of one steady-state eager push (the few torch copies are not
 counted), the stream's state_bytes() and algorithmic latency (delay plus one chunk, in ms at 22050 Hz), and the
 whole-utterance forward of the same audio (one call on the B utterances; for MB-MelGAN with the PQMF
 synthesis) for comparison.
@@ -43,7 +49,11 @@ Every timed stream is checked against ``model.inference`` of each item in the sa
   so the check is rel-L2 <= 1e-6 (bit identity holds below 4096 samples, tests/test_gpu_uhifigan_lookahead_stream.py);
 * vqvae_vctk_lg: against decode(encode(x), l, g) of the batch, whose 32 -> 1 output conv has 16384 samples per item and
   takes conv1d_fewcout_long_kernel, so the check is rel-L2 <= 1e-6 (bit identity holds below 4096 samples,
-  tests/test_gpu_vqvae_lookahead_stream.py).
+  tests/test_gpu_vqvae_lookahead_stream.py);
+* dsym_vctk_centred: its inference's 32 -> 1 output conv has 81920 samples and takes conv1d_fewcout_long_kernel, so the
+  check is rel-L2 <= 1e-6 (bit identity holds below 4096 samples, tests/test_gpu_dsym_lookahead_stream.py);
+* dsym_dur_cvss: durations equal ``synthesis``'s exactly, and the audio is within rel-L2 1e-6 of it (its output conv
+  takes conv1d_fewcout_long_kernel at this length).
 
 Prints the card name and power limit of the same run, as one JSON document.
 
@@ -62,8 +72,8 @@ import torch.nn.functional as F  # noqa: E402
 from parallelwavegan_b200 import capi, models  # noqa: E402
 from parallelwavegan_b200 import synth_weights as synth  # noqa: E402
 from parallelwavegan_b200.layers import PQMF  # noqa: E402
-from parallelwavegan_b200.streaming import (CausalHiFiGANStream, CausalMelGANStream, CausalPWGStream, HiFiGANLookaheadStream,  # noqa: E402
-                                            MelGANLookaheadStream, PWGLookaheadStream, UHiFiGANLookaheadStream, VQVAELookaheadStream)
+from parallelwavegan_b200.streaming import (CausalHiFiGANStream, CausalMelGANStream, CausalPWGStream,  # noqa: E402
+                                            DiscreteSymbolHiFiGANLookaheadStream, HiFiGANLookaheadStream, MelGANLookaheadStream, PWGLookaheadStream, UHiFiGANLookaheadStream, VQVAELookaheadStream)
 
 MELGAN = {
     "melgan_v1": dict(in_channels=80, out_channels=1, kernel_size=7, channels=512, upsample_scales=[8, 8, 2, 2], stacks=3,
@@ -80,13 +90,21 @@ VQVAE_VCTK_LG = dict(in_channels=1, out_channels=1, num_embeds=512, embed_dim=25
                      num_global_embeds=128, global_embed_dim=128, encoder_type="MelGANDiscriminator", decoder_type="MelGANGenerator",
                      encoder_conf={"out_channels": 256, "downsample_scales": [4, 4, 2, 2], "max_downsample_channels": 1024},
                      decoder_conf={"in_channels": 416, "upsample_scales": [4, 4, 2, 2], "channels": 512, "stacks": 3})
-MODELS = ("pwg", "pwg_centred", "hifigan", "hifigan_centred", *MELGAN, "uhifigan_opencpop_centred", "vqvae_vctk_lg")
+# egs/vctk/hubert_voc1 generator_params (DiscreteSymbolHiFiGANGenerator)
+DSYM_VCTK = dict(in_channels=512, out_channels=1, channels=512, num_embs=100, num_spk_embs=128, spk_emb_dim=512, kernel_size=7,
+                 upsample_scales=[10, 8, 2, 2], upsample_kernel_sizes=[20, 16, 4, 4], resblock_kernel_sizes=[3, 7, 11],
+                 resblock_dilations=[[1, 3, 5]] * 3)
+DSYM_DUR_CVSS = dict(in_channels=512, out_channels=1, channels=512, num_embs=500, num_spk_embs=0, kernel_size=7,
+                     upsample_scales=[10, 8, 2, 2], upsample_kernel_sizes=[20, 16, 4, 4], resblock_kernel_sizes=[3, 7, 11],
+                     resblock_dilations=[[1, 3, 5]] * 3)
+MODELS = ("pwg", "pwg_centred", "hifigan", "hifigan_centred", *MELGAN, "uhifigan_opencpop_centred", "vqvae_vctk_lg",
+          "dsym_vctk_centred", "dsym_dur_cvss")
 FRAMES = 256
 CHUNKS = (1, 4, 16, 64)
 PASSES = 2
 SR = 22050
-CHUNKS_OF = {"uhifigan_opencpop_centred": (1, 8), "vqvae_vctk_lg": (1, 4, 16)}
-SR_OF = {"uhifigan_opencpop_centred": 24000, "vqvae_vctk_lg": 24000}
+CHUNKS_OF = {"uhifigan_opencpop_centred": (1, 8), "vqvae_vctk_lg": (1, 4, 16), "dsym_vctk_centred": (1, 4, 16)}
+SR_OF = {"uhifigan_opencpop_centred": 24000, "vqvae_vctk_lg": 24000, "dsym_vctk_centred": 16000}
 
 
 def card():
@@ -121,6 +139,8 @@ def build(name, dev):
         m, scale = models.UHiFiGANGenerator(**UHIFIGAN_OPENCPOP), 1.15
     elif name == "vqvae_vctk_lg":
         m, scale = models.VQVAE(**VQVAE_VCTK_LG), 1.15
+    elif name == "dsym_vctk_centred":
+        m, scale = models.DiscreteSymbolHiFiGANGenerator(**DSYM_VCTK), 1.15
     else:
         m, scale = models.MelGANGenerator(**MELGAN[name]), 1.0
     m.load_state_dict(synth.synth_state_dict([(k, tuple(v.shape)) for k, v in m.state_dict().items()], 31, scale))
@@ -158,6 +178,15 @@ class Workload:
             self.delay = VQVAELookaheadStream(m, batch=B, use_graphs=False).delay
             self.whole = lambda: m.decode(m.encode(x), self.l, self.g)
             self.ref = F.pad(self.whole(), (self.delay, 0))
+        elif name == "dsym_vctk_centred":
+            self.hop = 320
+            sym = torch.randint(0, DSYM_VCTK["num_embs"], (B, self.frames), generator=g)
+            spk = (torch.arange(B) * 7 % DSYM_VCTK["num_spk_embs"])[:, None].expand(B, self.frames)  # a speaker per slot
+            c = self.c = torch.stack([sym, spk], -1).to(dev)  # (B, T, 2) units and speaker ids
+            cu = c.transpose(1, 2).contiguous()
+            self.delay = DiscreteSymbolHiFiGANLookaheadStream(m, batch=B, use_graphs=False).delay
+            self.ref = F.pad(torch.stack([m.inference(c[b]).t() for b in range(B)]), (self.delay, 0))
+            self.whole = lambda: m(cu)
         elif name in ("pwg", "pwg_centred"):
             hop = self.hop = m.upsample_factor
             z = self.z = torch.randn(B, 1, FRAMES * hop, generator=g).to(dev)
@@ -187,7 +216,7 @@ class Workload:
     def stream(self, B, graphs):
         cls = {"pwg": CausalPWGStream, "pwg_centred": PWGLookaheadStream, "hifigan": CausalHiFiGANStream,
                "hifigan_centred": HiFiGANLookaheadStream, "uhifigan_opencpop_centred": UHiFiGANLookaheadStream,
-               "vqvae_vctk_lg": VQVAELookaheadStream}.get(self.name)
+               "vqvae_vctk_lg": VQVAELookaheadStream, "dsym_vctk_centred": DiscreteSymbolHiFiGANLookaheadStream}.get(self.name)
         if cls is None:
             cls = CausalMelGANStream if MELGAN[self.name]["use_causal_conv"] else MelGANLookaheadStream
         return cls(self.m, batch=B, use_graphs=graphs)
@@ -264,6 +293,56 @@ def bench_model(name, Bs, dev):
     return res
 
 
+def bench_duration(Bs, dev):
+    """dsym_dur_cvss: push latency per push of units, RTF over the audio the pushes and flush produce"""
+    from parallelwavegan_b200.streaming import DiscreteSymbolDurationLookaheadStream
+
+    m = models.DiscreteSymbolDurationGenerator(**DSYM_DUR_CVSS)
+    m.load_state_dict(synth.synth_state_dict([(k, tuple(v.shape)) for k, v in m.state_dict().items()], 31, 1.15))
+    m.remove_weight_norm()
+    with torch.no_grad():
+        m.duration_predictor.linear.bias.fill_(0.6)
+    m = m.eval().to(dev)
+    res, S, sr = {}, 128, 16000
+    for B in Bs:
+        g = torch.Generator().manual_seed(B)
+        c = torch.randint(0, DSYM_DUR_CVSS["num_embs"], (B, S), generator=g).to(dev)
+        refs = [m.synthesis(c[b:b + 1, None]) for b in range(B)]
+        row = {"units_per_item": S}
+        for graphs in (False, True):
+            for n in (1, 4, 16):
+                st = DiscreteSymbolDurationLookaheadStream(m, batch=B, use_graphs=graphs)
+                for j in range(0, S, n):  # warm-up pass: caches and every captured length
+                    st.push(c[:, j:j + n])
+                st.flush()
+                lat, total, outs, durs = [], 0.0, [[] for _ in range(B)], [[] for _ in range(B)]
+                for j in range(0, S, n):
+                    y, t = timed(lambda: st.push(c[:, j:j + n]))
+                    lat.append(t)
+                    total += t
+                    d = st.last_durations
+                    for b in range(B):
+                        outs[b].append(y[b])
+                        durs[b].append(d[b])
+                fl, t = timed(st.flush)
+                total += t
+                d = st.last_durations
+                err, same = 0.0, True
+                for b in range(B):
+                    y = torch.cat(outs[b] + [fl[b]], -1)[:, st.delay:]
+                    same &= torch.equal(torch.cat(durs[b] + [d[b]]), refs[b][1][0].cpu())
+                    r = refs[b][0][0]
+                    err = max(err, float((y - r).double().norm() / r.double().norm()))
+                assert same and err <= 1e-6, (B, n, same, err)
+                s = stats(lat)
+                audio_s = sum(int(r[1].sum()) for r in refs) / B * 320 / sr
+                s.update(rtf=total / 1e3 / audio_s, flush_ms=t, durations_equal_synthesis=same, rel_l2_vs_synthesis=err,
+                         delay_samples=st.delay, state_bytes_per_slot=st.state_bytes())
+                row[f"{'graph' if graphs else 'eager'}_units{n}"] = s
+        res[f"B{B}"] = row
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0], formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("model", nargs="?", choices=MODELS, help="the model to stream (default: every one)")
@@ -273,7 +352,7 @@ def main():
     out = {"card": card(), "sample_rate_for_rtf": SR}
     with torch.no_grad():
         for name in [a.model] if a.model else MODELS:
-            out[name] = bench_model(name, a.batch, dev)
+            out[name] = bench_duration(a.batch, dev) if name == "dsym_dur_cvss" else bench_model(name, a.batch, dev)
     print(json.dumps(out, indent=1))
 
 
