@@ -350,6 +350,24 @@ PWGB_API int pwgb_resblock_pair_forward(const pwgb_resblock_desc* d, const float
 PWGB_API int pwgb_resblock_pair_packed_supported(const pwgb_resblock_desc* d);
 PWGB_API int pwgb_resblock_pair_packed_forward(const pwgb_resblock_desc* d, const float* x, const void* w1_packed, const float* b1,
                                                const void* w2_packed, const float* b2, void* h_packed, float* y, void* stream);
+/* The two pairs for a batch of signals of different lengths ("ragged" batches): the arguments of the entry point
+ * above plus ext, of which only the mask fields are read (frame, end, rate, lookahead as in pwgb_stream_ext; residual
+ * and edge fields are ignored).  Row t of item b is signal sample frame[b] * rate - lookahead + t; for a batch that
+ * starts every item at sample 0, frame = 0, lookahead = 0 and end[b] * rate = the item's length L_b.  Outside its signal
+ * the intermediate that the second conv reads (the shared-memory h image; the packed h image, whose tensor-copy box is
+ * only clipped at t) is +0.0, which is the zero padding of that conv on the item alone, and so is y.
+ *   precondition: x is zero outside each item's signal (the previous masked layer leaves it so);
+ *   accumulate: y must be zero on entry outside each item's signal; it is +0.0 there afterwards (y + 0.0);
+ *   then every row of item b inside its signal is bit-identical to the entry point above on that item alone with
+ *   t = L_b (or the two pwgb_conv1d_tc_forward calls it replaces, where L_b % 4 != 0).
+ * ext == NULL: the call is the entry point without the mask.  The unmasked kernels are separate instantiations and
+ * keep their code. */
+PWGB_API int pwgb_resblock_pair_ext_forward(const pwgb_resblock_desc* d, const float* x, const void* w1_packed, const float* b1,
+                                            const void* w2_packed, const float* b2, const pwgb_stream_ext* ext, float* y,
+                                            void* stream);
+PWGB_API int pwgb_resblock_pair_packed_ext_forward(const pwgb_resblock_desc* d, const float* x, const void* w1_packed,
+                                                   const float* b1, const void* w2_packed, const float* b2,
+                                                   const pwgb_stream_ext* ext, void* h_packed, float* y, void* stream);
 
 /* ------------------------------------------------------------------------
  * Fused WaveNet residual layer of ParallelWaveGANGenerator (layers/residual_block.py:102-140,

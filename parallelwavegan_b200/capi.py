@@ -160,6 +160,10 @@ def lib():
     L.pwgb_resblock_pair_packed_supported.argtypes = [C.POINTER(ResBlockDesc)]
     L.pwgb_resblock_pair_packed_forward.restype = C.c_int
     L.pwgb_resblock_pair_packed_forward.argtypes = [C.POINTER(ResBlockDesc), vp, vp, vp, vp, vp, vp, vp, vp]
+    L.pwgb_resblock_pair_ext_forward.restype = C.c_int
+    L.pwgb_resblock_pair_ext_forward.argtypes = [C.POINTER(ResBlockDesc), vp, vp, vp, vp, vp, C.POINTER(StreamExt), vp, vp]
+    L.pwgb_resblock_pair_packed_ext_forward.restype = C.c_int
+    L.pwgb_resblock_pair_packed_ext_forward.argtypes = [C.POINTER(ResBlockDesc), vp, vp, vp, vp, vp, C.POINTER(StreamExt), vp, vp, vp]
     L.pwgb_wavenet_supported.restype = C.c_int
     L.pwgb_wavenet_supported.argtypes = [C.POINTER(WaveNetDesc)]
     L.pwgb_wavenet_packed_bytes.restype = C.c_size_t
@@ -347,7 +351,8 @@ EXPORTED_SYMBOLS = [
     "pwgb_conv_transpose1d_window_stream_forward", "pwgb_stream_carry", "pwgb_conv1d_stream_ext_forward",
     "pwgb_conv1d_tc_stream_ext_forward", "pwgb_conv_transpose1d_stream_ext_forward",
     "pwgb_resblock_pair_supported", "pwgb_resblock_pair_plan", "pwgb_resblock_pair_forward",
-    "pwgb_resblock_pair_packed_supported", "pwgb_resblock_pair_packed_forward",
+    "pwgb_resblock_pair_packed_supported", "pwgb_resblock_pair_packed_forward", "pwgb_resblock_pair_ext_forward",
+    "pwgb_resblock_pair_packed_ext_forward",
     "pwgb_wavenet_supported", "pwgb_wavenet_packed_bytes",
     "pwgb_wavenet_pack", "pwgb_wavenet_layer_forward", "pwgb_upsample_fir_forward", "pwgb_upsample_fir_causal_forward",
     "pwgb_s2d_forward", "pwgb_s2d_backward", "pwgb_mt_clip_coef", "pwgb_mt_adam_step", "pwgb_prep_features", "pwgb_pcm16_forward", "pwgb_collate_crop",

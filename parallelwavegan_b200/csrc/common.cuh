@@ -56,6 +56,14 @@ __device__ __forceinline__ bool stream_outside(const int* frame, const int* end,
   const long long pos = (long long)__ldg(frame + b) * rate - lookahead + row;
   return pos < 0 || pos >= (long long)__ldg(end + b) * rate;
 }
+// The rows [lo, hi) of a launch of t rows that lie inside item b's signal in the sense of stream_outside
+__device__ __forceinline__ void stream_signal_rows(const int* frame, const int* end, int rate, int lookahead, int b, int t, int& lo,
+                                                   int& hi) {
+  const long long first = (long long)lookahead - (long long)__ldg(frame + b) * rate;
+  const long long last = first + (long long)__ldg(end + b) * rate;
+  lo = (int)(first < 0 ? 0 : first < t ? first : t);
+  hi = (int)(last < lo ? lo : last < t ? last : t);
+}
 
 // Accurate-enough transcendental helpers: tanhf/expf from libdevice (<= 2 ulp);
 // the parity bar is 1e-3 relative so these are never the limiting error.

@@ -650,6 +650,8 @@ __device__ __forceinline__ void conv1d_tc_body(const TcKOf<EXT, EDGE>& p, const 
         const int q = lane & 3;
         const bool q1 = q & 1, q2 = q & 2;
         const int t = t0 + (wg * MT + mb) * 64 + wq * 16 + (lane >> 2) + (q2 ? 8 : 0);
+        bool outside = false;  // masked launches: row t lies outside the item's signal
+        if constexpr (EXT && !HIST) outside = stream_outside(p.mframe, p.mend, p.mrate, p.mlook, b, t);
         const long long ld = 16LL * p.T_out;  // bytes between planes
         unsigned char* dst = reinterpret_cast<unsigned char*>(y) + (pk_plane(b, p.Cout * (MC ? p.nco : 1), co_base) +
                                                                     (q1 ? KC / 8 : 0)) * ld + 16LL * t;
@@ -669,6 +671,9 @@ __device__ __forceinline__ void conv1d_tc_body(const TcKOf<EXT, EDGE>& p, const 
           s0 = __shfl_xor_sync(0xffffffffu, s0, 1);
           s1 = __shfl_xor_sync(0xffffffffu, s1, 1);
           if (q1) { v0 = s0; v2 = s1; } else { v1 = s0; v3 = s1; }
+          if constexpr (EXT && !HIST) {
+            if (outside) v0 = v1 = v2 = v3 = 0u;  // +0.0, hi and lo
+          }
           // 8-channel group n: plane (n / 4) 2 KC / 8 + n % 4 from the tile's first
           if (t < p.T_out) *reinterpret_cast<uint4*>(dst + ((n >> 2) * (2 * (KC / 8)) + (n & 3)) * ld) = make_uint4(v0, v1, v2, v3);
         }
@@ -680,7 +685,8 @@ __device__ __forceinline__ void conv1d_tc_body(const TcKOf<EXT, EDGE>& p, const 
         for (int i = 0; i < NACC; ++i) {
           const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
           const int t = t0 + (wg * MT + mb) * 64 + wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
-          if (t < p.T_out) epi_store<decltype(mode)::value, EXT>(p, ab[i], b, t, col, co_base, bias, bias_s, res, y, y2);
+          // (the masked launches without history take the staged or the packed epilogue only)
+          if (t < p.T_out) epi_store<decltype(mode)::value, EXT && HIST>(p, ab[i], b, t, col, co_base, bias, bias_s, res, y, y2);
         }
       };
 #pragma unroll
@@ -701,6 +707,22 @@ __device__ __forceinline__ void conv1d_tc_body(const TcKOf<EXT, EDGE>& p, const 
         wg_barrier(wg);
         unsigned row_bytes;
         const long long row_off = row_pos(t0, co_base, row_bytes);
+        if constexpr (EXT && !HIST) {
+          // masked launches: the row's samples outside the item's signal become +0.0 before the store (y + 0.0 with
+          // accumulate), here where the accumulators are dead
+          if (row_owner) {
+            int lo, hi;
+            stream_signal_rows(p.mframe, p.mend, p.mrate, p.mlook, b, p.T_out, lo, hi);
+            const int tw0 = t0 + wg * MT * 64;
+            if (tw0 < lo || tw0 + MT * 64 > hi) {  // a tile inside the signal has nothing to mask
+              float* row = stg + wt * SLD;
+#pragma unroll 1
+              for (int r = 0; r < MT * 64; ++r)
+                if (tw0 + r < lo || tw0 + r >= hi) row[r] = 0.f;
+              fence_proxy_async();  // generic-proxy writes -> visible to this thread's bulk store
+            }
+          }
+        }
         if (row_owner) stage_store_row(y + (long long)b * p.ybs + row_off, smem_u32(stg + wt * SLD), row_bytes, p.accumulate);
         if (row_owner && res && tile + (int)gridDim.x < p.total_tiles) load_res(tile + gridDim.x);
       }
@@ -799,6 +821,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
                          const uint4* __restrict__ wpk, const float* __restrict__ bias, const float* __restrict__ res,
                          float* __restrict__ y, float* __restrict__ y2) {
   conv1d_tc_body<MT, NB16, true, true>(p, x, x2, wpk, bias, res, y, y2, nullptr);
+}
+
+// the two launches of a masked ResBlock pair at 128 / 256 channels (pwgb_resblock_pair_packed_ext_forward): no history,
+// the mask of TcKExt in the packed-output and the staged epilogues
+template <int MT, int NB16>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+    conv1d_tc_mask_kernel(const TcKExt p, const float* __restrict__ x, const float* __restrict__ x2,
+                          const uint4* __restrict__ wpk, const float* __restrict__ bias, const float* __restrict__ res,
+                          float* __restrict__ y, float* __restrict__ y2, const __grid_constant__ CUtensorMap tm_a) {
+  conv1d_tc_body<MT, NB16, false, true>(p, x, x2, wpk, bias, res, y, y2, &tm_a);
 }
 
 // history launches with a pwgb_stream_ext edge policy (pwgb_conv1d_tc_stream_ext_forward with edge != 0)
@@ -1351,6 +1383,62 @@ extern "C" int pwgb_resblock_pair_packed_supported(const pwgb_resblock_desc* d) 
   TcK p1, p2;
   size_t b1, b2;
   return rb_packed_plan(d, p1, b1, p2, b2);
+}
+
+// One masked launch of the packed pair: both are 128-column, one-block tiles (rb_packed_plan)
+static int rb_packed_launch_ext(TcKExt& p, size_t bytes, const float* x, const void* packed_w, const float* bias,
+                                const float* residual, float* y, cudaStream_t st, const CUtensorMap* tm_a) {
+  using Kernel = void (*)(const TcKExt, const float*, const float*, const uint4*, const float*, const float*, float*, float*,
+                          const CUtensorMap);
+  static const Kernel kernels[1] = {conv1d_tc_mask_kernel<1, TC_NMAX / 16>};
+  static bool smem_set = false;
+  if (p.MT != 1 || p.Cout != TC_NMAX || !(p.staged || p.pk_out)) {
+    set_error("resblock_pair_packed_ext: no masked kernel for MT = %d, Cout = %d", p.MT, p.Cout);
+    return PWGB_UNSUPPORTED;
+  }
+  if (const int rc = smem_opt_in(smem_set, kernels, (int)TC_SMEM_STAGED, "resblock_pair_packed_ext")) return rc;
+  CUtensorMap tm;
+  if (tm_a)
+    tm = *tm_a;
+  else
+    memset(&tm, 0, sizeof(tm));
+  const int num_sms = tc_num_sms();
+  const int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
+  kernels[0]<<<(unsigned)grid, TC_THREADS, bytes, st>>>(p, x, nullptr, (const uint4*)packed_w, bias, residual, y, nullptr, tm);
+  return check_launch("conv1d_tc_mask_kernel");
+}
+
+extern "C" int pwgb_resblock_pair_packed_ext_forward(const pwgb_resblock_desc* d, const float* x, const void* w1_packed,
+                                                     const float* b1, const void* w2_packed, const float* b2,
+                                                     const pwgb_stream_ext* ext, void* h_packed, float* y, void* stream) {
+  if (!ext) return pwgb_resblock_pair_packed_forward(d, x, w1_packed, b1, w2_packed, b2, h_packed, y, stream);
+  PWGB_CHECK_ARG(d && x && w1_packed && w2_packed && h_packed && y, "resblock_pair_packed_ext: null argument");
+  PWGB_CHECK_ARG(ext->frame && ext->end && ext->rate >= 1 && ext->lookahead >= 0,
+                 "resblock_pair_packed_ext: ext must hold a mask (frame, end, rate >= 1, lookahead >= 0)");
+  TcKExt p1, p2;
+  size_t bytes1 = 0, bytes2 = 0;
+  PWGB_UNSUPPORTED_IF(!rb_packed_plan(d, p1, bytes1, p2, bytes2), "resblock_pair_packed_ext: configuration not supported");
+  PWGB_CHECK_ARG(x != y, "resblock_pair_packed_ext: y must not alias x (halo reads)");
+  PWGB_UNSUPPORTED_IF(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(h_packed)) & 15),
+                      "resblock_pair_packed_ext: x, h_packed and y must be 16-byte aligned");
+  if (d->batch == 0) return PWGB_OK;
+  for (TcKExt* p : {&p1, &p2}) {
+    p->mframe = ext->frame;
+    p->mend = ext->end;
+    p->mrate = ext->rate;
+    p->mlook = ext->lookahead;
+    p->rhist = nullptr;
+    p->rhist_len = p->rdelay = 0;
+    p->rhbs = 0;
+  }
+  CUtensorMap tm;
+  const unsigned long long dims[3] = {8ull, (unsigned long long)d->t, (unsigned long long)pk_plane(d->batch, d->channels, 0)};
+  const unsigned box[3] = {8u, (unsigned)p2.R, 2u * (KC / 8)};
+  if (const int rc = tma_make(&tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, 3, h_packed, dims, box)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (const int rc = rb_packed_launch_ext(p1, bytes1, x, w1_packed, b1, nullptr, static_cast<float*>(h_packed), st, nullptr))
+    return rc;
+  return rb_packed_launch_ext(p2, bytes2, static_cast<const float*>(h_packed), w2_packed, b2, x, y, st, &tm);
 }
 
 extern "C" int pwgb_resblock_pair_packed_forward(const pwgb_resblock_desc* d, const float* x, const void* w1_packed,

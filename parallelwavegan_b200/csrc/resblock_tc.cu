@@ -23,6 +23,7 @@
 // Each conv owns a weight ring.  A pair whose conv1 halo leaves no room for two rings of RB_MIN_STAGES stages has no
 // plan and runs as the two conv1d_tc launches.
 #include <cstring>
+#include <type_traits>
 
 #include "tc_common.cuh"
 
@@ -50,6 +51,19 @@ struct RbK {
   int na, nb, ns;          // conv1 operand buffers, weight stages (both rings), raw stages
   int a_bytes, b_bytes, raw_bytes, h_bytes;  // per buffer / stage; h_bytes: one 32-channel chunk of the h image
 };
+
+// The mask of a pwgb_resblock_pair_ext_forward launch (the mask fields of pwgb_stream_ext): row t of item b is signal
+// sample mframe[b] * mrate - mlook + t, and the h rows conv2 reads and the y rows outside [0, mend[b] * mrate) are +0.0.
+// A separate struct and kernel (EXT), so that rb_pair_split_kernel keeps its parameters and code.
+struct RbKExt : RbK {
+  const int* mframe;
+  const int* mend;
+  int mrate, mlook;
+};
+
+__device__ __forceinline__ void rb_signal_rows(const RbKExt& p, int b, int& lo, int& hi) {
+  stream_signal_rows(p.mframe, p.mend, p.mrate, p.mlook, b, p.T, lo, hi);
+}
 
 // ===================== A producers: raw fp32 rows -> conv1 operand image =====================
 // RB_NPROD producer threads, this one `tid` of them.  Barrier arguments are the first of each array of 8-byte mbarriers.
@@ -100,17 +114,21 @@ __device__ __forceinline__ void rb_load_raw(const RbK& p, const float* __restric
 }
 
 // h = lrelu(acc + b1) of the warpgroup's conv rows [row_base, row_base + 64 MT) (time th0 + r for fragment row r) as
-// conv2's operand image; rows outside [0, T) are conv2's zero padding
-template <int MT, int NB16>
+// conv2's operand image; rows outside [0, T) are conv2's zero padding (EXT: rows outside the signal's [lo, hi))
+template <int MT, int NB16, bool EXT = false>
 __device__ __forceinline__ void rb_write_h(const float* acc, unsigned char* h_buf, const RbK& p, int row_base, int th0,
-                                           const float* bias1, int lane, int wq) {
+                                           const float* bias1, int lane, int wq, int lo = 0, int hi = 0) {
   constexpr int NACC = 8 * NB16;
 #pragma unroll
   for (int e = 0; e < MT * NACC; e += 2) {
     const int i = e % NACC;
     const int col = 8 * (i >> 2) + 2 * (lane & 3);
     const int r = (e / NACC) * 64 + wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
-    const bool ok = (unsigned)(th0 + r) < (unsigned)p.T;
+    bool ok;
+    if constexpr (EXT)
+      ok = th0 + r >= lo && th0 + r < hi;
+    else
+      ok = (unsigned)(th0 + r) < (unsigned)p.T;
     const float h0 = acc[e] + bias1[col], h1 = acc[e + 1] + bias1[col + 1];
     unsigned hi, lo;
     split2(ok ? lrelu(h0, p.slope) : 0.f, ok ? lrelu(h1, p.slope) : 0.f, hi, lo);
@@ -122,17 +140,25 @@ __device__ __forceinline__ void rb_write_h(const float* acc, unsigned char* h_bu
 }
 
 // staged epilogue in place over the residual rows of the tile `stg` ([channel][stage_ld(MT)]): v = (a + b2 + x) * out_scale
-template <int MT, int NB16>
+// (EXT: +0.0 in the tile rows outside [lo, hi), relative to the tile's first row)
+template <int MT, int NB16, bool EXT = false>
 __device__ __forceinline__ void rb_stage_result(const float* acc, float* stg, const float* bias2, float out_scale, int lane,
-                                                int wq) {
+                                                int wq, int lo = 0, int hi = 0) {
   constexpr int NACC = 8 * NB16, SLD = stage_ld(MT);
 #pragma unroll
   for (int e = 0; e < MT * NACC; ++e) {
     const int i = e % NACC;
     const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
-    float* sv = stg + col * SLD + (e / NACC) * 64 + wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+    const int r = (e / NACC) * 64 + wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+    float* sv = stg + col * SLD + r;
     float v = acc[e] + bias2[col];
     v += *sv;
+    if constexpr (EXT) {
+      if (r < lo || r >= hi) {
+        *sv = 0.f;
+        continue;
+      }
+    }
     *sv = v * out_scale;
   }
 }
@@ -142,11 +168,12 @@ __device__ __forceinline__ void rb_stage_result(const float* acc, float* stg, co
 // i + 1 while warpgroup 1 runs conv2 and the epilogue of tile i; they hand the single h image over through two
 // mbarriers (H_FULL: written, H_FREE: conv2's MMAs have retired).  Weights come in two rings of nb / 2 stages, conv1's
 // and conv2's, both filled by the weight warp.  The residual rows belong to conv2's warpgroup.
-template <int MT, int NB16>
-__global__ void __launch_bounds__(RB_THREADS, 1)
-    rb_pair_split_kernel(const RbK p, const float* __restrict__ x, const unsigned char* __restrict__ w1,
-                         const float* __restrict__ b1, const unsigned char* __restrict__ w2, const float* __restrict__ b2,
-                         float* __restrict__ y) {
+// EXT: the mask of RbKExt in the h write and the staged epilogue.
+template <int MT, int NB16, bool EXT>
+__device__ __forceinline__ void rb_pair_split_body(const std::conditional_t<EXT, RbKExt, RbK>& p, const float* __restrict__ x,
+                                                   const unsigned char* __restrict__ w1, const float* __restrict__ b1,
+                                                   const unsigned char* __restrict__ w2, const float* __restrict__ b2,
+                                                   float* __restrict__ y) {
   extern __shared__ __align__(128) unsigned char smem[];
   constexpr int C = 16 * NB16, NCH = C / KC, NACC = 8 * NB16, SLD = stage_ld(MT);
   const int nr = p.nb / 2;  // stages per weight ring
@@ -238,7 +265,13 @@ __global__ void __launch_bounds__(RB_THREADS, 1)
       release();
       mbar_wait_trap(H_FREE, (n & 1) ^ 1);  // conv2 of the previous tile has read the image
       const int t0 = (tile % p.tiles_per_seq) * p.M2;
-      rb_write_h<MT, NB16>(acc, h_buf, p, 0, t0 - p.p2, bias_s, lane, wq);
+      if constexpr (EXT) {
+        int lo, hi;
+        rb_signal_rows(p, tile / p.tiles_per_seq, lo, hi);
+        rb_write_h<MT, NB16, true>(acc, h_buf, p, 0, t0 - p.p2, bias_s, lane, wq, lo, hi);
+      } else {
+        rb_write_h<MT, NB16>(acc, h_buf, p, 0, t0 - p.p2, bias_s, lane, wq);
+      }
       fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor core
       mbar_arrive(H_FULL);
     }
@@ -293,7 +326,14 @@ __global__ void __launch_bounds__(RB_THREADS, 1)
       mbar_arrive(H_FREE);
       // ---- staged epilogue over the residual row, one bulk store (or fp32 add) per row
       mbar_wait_trap(RES_FULL, n & 1);  // one phase per tile
-      rb_stage_result<MT, NB16>(acc, stg, bias_s + C, p.out_scale, lane, wq);
+      if constexpr (EXT) {
+        const int b = tile / p.tiles_per_seq, t0 = (tile - b * p.tiles_per_seq) * p.M2;
+        int lo, hi;
+        rb_signal_rows(p, b, lo, hi);
+        rb_stage_result<MT, NB16, true>(acc, stg, bias_s + C, p.out_scale, lane, wq, lo - t0, hi - t0);
+      } else {
+        rb_stage_result<MT, NB16>(acc, stg, bias_s + C, p.out_scale, lane, wq);
+      }
       fence_proxy_async();  // generic-proxy writes -> visible to the bulk copies
       wg_barrier(1);
       if (row_owner) {
@@ -339,14 +379,38 @@ __global__ void __launch_bounds__(RB_THREADS, 1)
   }
 }
 
+template <int MT, int NB16>
+__global__ void __launch_bounds__(RB_THREADS, 1)
+    rb_pair_split_kernel(const RbK p, const float* __restrict__ x, const unsigned char* __restrict__ w1,
+                         const float* __restrict__ b1, const unsigned char* __restrict__ w2, const float* __restrict__ b2,
+                         float* __restrict__ y) {
+  rb_pair_split_body<MT, NB16, false>(p, x, w1, b1, w2, b2, y);
+}
+
+// the masked pair (pwgb_resblock_pair_ext_forward)
+template <int MT, int NB16>
+__global__ void __launch_bounds__(RB_THREADS, 1)
+    rb_pair_split_ext_kernel(const RbKExt p, const float* __restrict__ x, const unsigned char* __restrict__ w1,
+                             const float* __restrict__ b1, const unsigned char* __restrict__ w2, const float* __restrict__ b2,
+                             float* __restrict__ y) {
+  rb_pair_split_body<MT, NB16, true>(p, x, w1, b1, w2, b2, y);
+}
+
 using RbKernel = void (*)(const RbK, const float*, const unsigned char*, const float*, const unsigned char*, const float*,
                           float*);
+using RbKernelExt = void (*)(const RbKExt, const float*, const unsigned char*, const float*, const unsigned char*,
+                             const float*, float*);
 
 // Instantiations: 256-row tiles at 32 channels, 128-row tiles at 64 channels (mt: 64-row blocks of a tile)
 RbKernel rb_split_kernel_for(int channels, int* mt) {
   *mt = channels == 32 ? 4 : 2;
   if (channels == 32) return rb_pair_split_kernel<4, 2>;
   if (channels == 64) return rb_pair_split_kernel<2, 4>;
+  return nullptr;
+}
+RbKernelExt rb_split_ext_kernel_for(int channels) {
+  if (channels == 32) return rb_pair_split_ext_kernel<4, 2>;
+  if (channels == 64) return rb_pair_split_ext_kernel<2, 4>;
   return nullptr;
 }
 
@@ -431,6 +495,35 @@ extern "C" int pwgb_resblock_pair_plan(const pwgb_resblock_desc* d, int* info) {
   const int v[5] = {p.M2, 64 * p.MT, p.na, p.nb, p.ns};
   memcpy(info, v, sizeof(v));
   return 1;
+}
+
+extern "C" int pwgb_resblock_pair_ext_forward(const pwgb_resblock_desc* d, const float* x, const void* w1_packed,
+                                              const float* b1, const void* w2_packed, const float* b2,
+                                              const pwgb_stream_ext* ext, float* y, void* stream) {
+  if (!ext) return pwgb_resblock_pair_forward(d, x, w1_packed, b1, w2_packed, b2, y, stream);
+  PWGB_CHECK_ARG(d && x && w1_packed && w2_packed && y, "resblock_pair_ext: null argument");
+  PWGB_CHECK_ARG(ext->frame && ext->end && ext->rate >= 1 && ext->lookahead >= 0,
+                 "resblock_pair_ext: ext must hold a mask (frame, end, rate >= 1, lookahead >= 0)");
+  RbKExt p;
+  size_t bytes = 0;
+  PWGB_UNSUPPORTED_IF(!rb_plan(d, p, bytes), "resblock_pair_ext: configuration not supported by the fused kernel");
+  PWGB_CHECK_ARG(x != y, "resblock_pair_ext: y must not alias x (halo reads)");
+  PWGB_UNSUPPORTED_IF((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(y) & 15),
+                      "resblock_pair_ext: x and y must be 16-byte aligned");
+  if (p.B == 0) return PWGB_OK;
+  p.mframe = ext->frame;
+  p.mend = ext->end;
+  p.mrate = ext->rate;
+  p.mlook = ext->lookahead;
+  static bool smem_set = false;
+  if (const int rc = smem_opt_in(smem_set, {rb_split_ext_kernel_for(32), rb_split_ext_kernel_for(64)}, (int)RB_SMEM,
+                                 "resblock_pair_ext"))
+    return rc;
+  const int num_sms = tc_num_sms();
+  const int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
+  rb_split_ext_kernel_for(p.C)<<<(unsigned)grid, RB_THREADS, bytes, (cudaStream_t)stream>>>(
+      p, x, (const unsigned char*)w1_packed, b1, (const unsigned char*)w2_packed, b2, y);
+  return check_launch("rb_pair_split_ext_kernel");
 }
 
 extern "C" int pwgb_resblock_pair_forward(const pwgb_resblock_desc* d, const float* x, const void* w1_packed,

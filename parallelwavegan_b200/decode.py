@@ -14,7 +14,17 @@ The reference loops utterances one at a time through ``model.inference`` (host n
 ``exact=True`` (default) batches only utterances of EQUAL length, so every waveform equals ``model.inference`` of that
 utterance alone; ``exact=False`` pads a length bucket with zero frames (after normalisation) to a multiple of
 ``bucket_frames`` and crops -- samples within one receptive field of an utterance's end then see the padded tail
-instead of the conv's zero padding."""
+instead of the conv's zero padding.
+
+``ragged=True`` (HiFi-GAN and the discrete-symbol HiFi-GAN) batches utterances of ANY lengths: the batch (sorted by
+length) is padded to a multiple of ``bucket_frames`` and its per-item frame counts go to the device, where every layer
+keeps each item zero past its own end (``HiFiGANGenerator.forward(c, lengths)``).  Every waveform then equals
+``model.inference`` of that utterance alone (bit for bit wherever both take the same kernels, DESIGN.md §3.14).  One CUDA
+graph per (batch, padded length) serves every mix of lengths, which are a static input of the graph.  A causal
+HiFi-GAN needs the padding only.
+
+The discrete-symbol HiFi-GAN decodes units: each input is a (T, 2) (symbol, speaker) or (T, 1) index array, padded
+with symbol 0 past its end (and its own speaker)."""
 import ctypes as C
 
 import numpy as np
@@ -91,17 +101,54 @@ def prep_features(c, out, mean=None, scale=None, pad_left=0, replicate=False):
     return out
 
 
+def ragged_refusal(model):
+    """Why ``Decoder(model, ragged=True)`` cannot batch utterances of different lengths, or None when it can."""
+    from . import models
+
+    t = type(model)
+    if t is models.HiFiGANGenerator or t is models.DiscreteSymbolHiFiGANGenerator:
+        return None
+    reasons = {
+        models.MelGANGenerator: "MelGAN pads its input by reflection at the signal's end (and multi-band MelGAN's PQMF "
+                                "synthesis looks ahead), which a zero-padded batch cannot reproduce per item",
+        models.ParallelWaveGANGenerator: "the fused WaveNet stack of Parallel WaveGAN has no per-item length mask",
+        models.StyleMelGANGenerator: "StyleMelGAN's InstanceNorm takes statistics over the whole signal",
+        models.UHiFiGANGenerator: "the U-Net HiFi-GAN's strided encoder and excitation input have no per-item length mask",
+        models.DiscreteSymbolDurationGenerator: "the duration model's regulated length is only known after its predictor runs",
+        models.VQVAE: "the VQ-VAE converts waveforms and has no per-item length mask",
+    }
+    for cls, why in reasons.items():
+        if isinstance(model, cls):
+            return why
+    return f"{t.__name__} has no per-item length mask"
+
+
 class Decoder:
-    def __init__(self, model, use_graphs=True, max_batch=16, exact=True, bucket_frames=32, rank=0, world=1, seed=None):
+    def __init__(self, model, use_graphs=True, max_batch=16, exact=True, bucket_frames=32, rank=0, world=1, seed=None,
+                 ragged=False):
         from . import models
 
+        self.max_batch, self.exact, self.bucket = int(max_batch), bool(exact), int(bucket_frames)
+        self.ragged = bool(ragged)
+        # a ragged batch passes per-item lengths to the non-causal HiFi-GAN body; a causal one needs the padding only
+        self.masked = False
+        if self.ragged:
+            if self.max_batch < 1 or self.bucket < 1:
+                raise PwgbError(f"Decoder(ragged=True): max_batch ({max_batch}) and bucket_frames ({bucket_frames}) must be positive")
+            why = ragged_refusal(model)
+            if why is not None:
+                raise PwgbError(f"Decoder(ragged=True): {why}")
+            if self.bucket % 4:
+                raise PwgbError(f"Decoder(ragged=True): bucket_frames must be a multiple of 4 (the fused ResBlock pairs need "
+                                f"t % 4 == 0), got {self.bucket}")
+            self.masked = not getattr(model, "use_causal_conv", False)
         self.model = model.eval()
         self.dev = next(model.parameters()).device
         if self.dev.type != "cuda":
             raise PwgbError("Decoder: the model must live on a CUDA device (no CPU fallback)")
         self.kind = ("pwg" if isinstance(model, models.ParallelWaveGANGenerator) else
-                     "style" if isinstance(model, models.StyleMelGANGenerator) else "mel2wav")
-        self.max_batch, self.exact, self.bucket = int(max_batch), bool(exact), int(bucket_frames)
+                     "style" if isinstance(model, models.StyleMelGANGenerator) else
+                     "units" if type(model) is models.DiscreteSymbolHiFiGANGenerator else "mel2wav")
         self.rank, self.world = rank, world
         self.gen = torch.Generator(device=self.dev)
         if seed is not None:
@@ -117,6 +164,14 @@ class Decoder:
         self.ctx = int(getattr(model, "aux_context_window", 0)) if self.kind == "pwg" else 0
 
     def _groups(self, lengths, idxs):
+        """(padded length, [indices]) batches: equal lengths (exact), length buckets, or (ragged) runs of up to max_batch
+        utterances in length order, each padded to a multiple of bucket_frames above its longest"""
+        if self.ragged:
+            order = sorted(idxs, key=lambda i: (lengths[i], i))
+            for k in range(0, len(order), self.max_batch):
+                g = order[k : k + self.max_batch]
+                yield max(-(-lengths[g[-1]] // self.bucket) * self.bucket, self.bucket), g
+            return
         groups = {}
         for i in idxs:
             L = lengths[i]
@@ -140,20 +195,39 @@ class Decoder:
                 y = m.inference(torch.as_tensor(mels[i], dtype=torch.float32, device=self.dev), normalize_before=normalize_before)
                 out[i] = pcm16(y[:, 0]).cpu().numpy() if to_pcm16 else y
             return out
+        units = self.kind == "units"
+        if units and normalize_before:
+            raise PwgbError("Decoder: units are not normalised (normalize_before=False)")
         mean = m.mean if normalize_before else None
         scale = m.scale if normalize_before else None
-        host = [torch.as_tensor(np.asarray(x, dtype=np.float32) if not isinstance(x, torch.Tensor) else x, dtype=torch.float32) for x in (mels[i] for i in idxs)]
+        if units:
+            host = [_unit_rows(x, m.num_spk_embs > 0) for x in (mels[i] for i in idxs)]
+        else:
+            host = [torch.as_tensor(np.asarray(x, dtype=np.float32) if not isinstance(x, torch.Tensor) else x, dtype=torch.float32) for x in (mels[i] for i in idxs)]
         by_idx = dict(zip(idxs, host))
         lengths = {i: by_idx[i].shape[0] for i in idxs}
         out, pending = {}, []
         for Tb, grp in self._groups(lengths, idxs):
             B, Cc = len(grp), by_idx[grp[0]].shape[1]
-            cin = torch.empty((B, Cc, Tb + 2 * self.ctx), device=self.dev, dtype=torch.float32)
-            for b, i in enumerate(grp):
-                src = by_idx[i]
-                src = src.pin_memory() if not src.is_cuda and not src.is_pinned() else src
-                prep_features(src.to(self.dev, non_blocking=True).contiguous(), cin[b], mean, scale, pad_left=self.ctx, replicate=self.ctx > 0)
-            if self.kind == "pwg":
+            if units:
+                # symbol 0 past an item's end (masked before input_conv), the item's own speaker throughout
+                cin = torch.zeros((B, Cc, Tb), dtype=torch.int64)
+                for b, i in enumerate(grp):
+                    u = by_idx[i]
+                    cin[b, :, : u.shape[0]] = u.transpose(0, 1)
+                    if Cc == 2 and u.shape[0]:
+                        cin[b, 1, u.shape[0] :] = u[0, 1]
+                cin = cin.pin_memory().to(self.dev, non_blocking=True)
+            else:
+                cin = torch.empty((B, Cc, Tb + 2 * self.ctx), device=self.dev, dtype=torch.float32)
+                for b, i in enumerate(grp):
+                    src = by_idx[i]
+                    src = src.pin_memory() if not src.is_cuda and not src.is_pinned() else src
+                    prep_features(src.to(self.dev, non_blocking=True).contiguous(), cin[b], mean, scale, pad_left=self.ctx, replicate=self.ctx > 0)
+            if self.masked:
+                lens = torch.tensor([lengths[i] for i in grp], dtype=torch.int32).pin_memory().to(self.dev, non_blocking=True)
+                y = self.runner(cin, lens)
+            elif self.kind == "pwg":
                 hop = m.upsample_factor
                 z = torch.randn((B, 1, Tb * hop), device=self.dev, generator=self.gen)
                 if noises:
@@ -179,6 +253,18 @@ class Decoder:
             for i, hbuf in pending:
                 out[i] = hbuf.numpy()
         return out
+
+
+def _unit_rows(x, speakers):
+    """One utterance of units: (T, 2) (symbol, speaker) or (T, 1) / (T,) symbols -> (T, K) int64 on the host, K = 2 with
+    speakers, else 1 (DiscreteSymbolHiFiGANGenerator.inference's input)"""
+    u = torch.as_tensor(np.asarray(x) if not isinstance(x, torch.Tensor) else x).cpu()
+    if u.dim() == 1:
+        u = u[:, None]
+    if u.dim() != 2 or u.shape[1] not in (1, 2) or (speakers and u.shape[1] != 2):
+        raise PwgbError(f"Decoder: units must be (T, 2) (symbol, speaker){' or (T, 1)' if not speakers else ''}, got {tuple(u.shape)}")
+    u = u.to(torch.int64)
+    return u if speakers else u[:, :1]
 
 
 @torch.no_grad()

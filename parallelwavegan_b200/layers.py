@@ -144,9 +144,16 @@ class HiFiGANResidualBlock(torch.nn.Module):
                     conv2 = torch.nn.Conv1d(channels, channels, kernel_size, dilation=1, bias=bias, padding=(kernel_size - 1) // 2)
                 self.convs2 += [torch.nn.Sequential(act(**nonlinear_activation_params), conv2)]
 
-    def forward(self, x, out=None, accumulate=False, out_scale=1.0):
+    def forward(self, x, out=None, accumulate=False, out_scale=1.0, mask=None):
         """Returns block(x); optionally ``out (+)= out_scale * block(x)`` fused into the last conv
-        (inference only -- under autograd the caller sums the block outputs with ScaledSumFn)."""
+        (inference only -- under autograd the caller sums the block outputs with ScaledSumFn).
+
+        ``mask`` = (frame, end, rate, lookahead) (ops.conv1d_stream; non-causal inference only): a batch of signals of
+        different lengths.  x is zero outside each item's signal, and so is ``out`` with ``accumulate``.  Every tensor a
+        later conv reads is kept zero there too: the fused pairs mask in their epilogues; the two-conv fallback and the
+        single convs take one pwgb_stream_mask after each conv.  Each item's samples then equal the block on it alone."""
+        if mask is not None and self.use_causal_conv:
+            raise PwgbError("HiFiGANResidualBlock: a causal block needs no length mask")
         k = self.kernel_size
         n = len(self.dilations)
         for idx, d in enumerate(self.dilations):
@@ -163,13 +170,19 @@ class HiFiGANResidualBlock(torch.nn.Module):
                 c2 = self.convs2[idx][1]
                 w1, w2 = effective_weight(c1), effective_weight(c2)
                 # inference at 32 / 64 channels: both convs in one launch, the intermediate never leaves the SM
-                y = ops.resblock_pair(x, w1, c1.bias, w2, c2.bias, kernel_size=k, dilation=d, slope=self.slope, **tail)
+                y = ops.resblock_pair(x, w1, c1.bias, w2, c2.bias, kernel_size=k, dilation=d, slope=self.slope, mask=mask, **tail)
                 if y is None:
                     xt = ops.conv1d(x, w1, c1.bias, dilation=d, padding=(k - 1) // 2 * d, pre_slope=self.slope)
+                    if mask is not None:
+                        ops.stream_mask(xt, mask)
                     y = ops.conv1d(xt, w2, c2.bias, padding=(k - 1) // 2, pre_slope=self.slope, residual=x, **tail)
+                    if mask is not None:
+                        ops.stream_mask(y, mask)
                 x = y
             else:
                 x = ops.conv1d(x, effective_weight(c1), c1.bias, dilation=d, padding=(k - 1) // 2 * d, pre_slope=self.slope, residual=x, **tail)
+                if mask is not None:
+                    ops.stream_mask(x, mask)
         return x
 
 

@@ -53,32 +53,69 @@ class _GeneratorBase(torch.nn.Module):
         return c.transpose(1, 0).unsqueeze(0).contiguous()
 
 
-def _mrf_average(blocks, first, nb, h, differentiable):
-    """sum_j blocks[first + j](h) / nb: ScaledSumFn under autograd, else fused into each block's last conv."""
+def _mrf_average(blocks, first, nb, h, differentiable, mask=None):
+    """sum_j blocks[first + j](h) / nb: ScaledSumFn under autograd, else fused into each block's last conv.  ``mask``:
+    the length mask of a ragged batch (inference only); the first block's last conv writes +0.0 outside each item's
+    signal, which the later ones accumulate onto."""
     if differentiable:
+        if mask is not None:
+            raise PwgbError("per-item lengths are an inference feature (no autograd)")
         from .autograd import ScaledSumFn
 
         return ScaledSumFn.apply(1.0 / nb, *[blocks[first + j](h) for j in range(nb)])
     cs = torch.empty_like(h)
     for j in range(nb):
-        blocks[first + j](h, out=cs, accumulate=j > 0, out_scale=1.0 / nb)
+        if mask is None:
+            blocks[first + j](h, out=cs, accumulate=j > 0, out_scale=1.0 / nb)
+        else:
+            blocks[first + j](h, out=cs, accumulate=j > 0, out_scale=1.0 / nb, mask=mask)
     return cs
 
 
-def _hifigan_body(g, c):
+def _length_mask(lengths, B, rate):
+    """The pwgb_stream_ext mask of a ragged batch at ``rate`` samples per frame: item b is [0, lengths[b] * rate)."""
+    if not (isinstance(lengths, torch.Tensor) and lengths.is_cuda and lengths.dtype == torch.int32 and lengths.dim() == 1
+            and lengths.numel() == B and lengths.is_contiguous()):
+        raise PwgbError(f"lengths must be {B} contiguous int32 frame counts on the device")
+    return (torch.zeros_like(lengths), lengths, int(rate), 0)
+
+
+def _masked(c, lengths, rate):
+    """c with the samples past each item's length (``lengths`` frames at ``rate`` samples per frame) set to +0.0"""
+    return c if lengths is None else ops.stream_mask(c, _length_mask(lengths, c.shape[0], rate))
+
+
+def _hifigan_body(g, c, lengths=None):
     """The HiFi-GAN body after input_conv (hifigan.py:182-192, 1023-1029, 1215-1221, 1281-1287): per level LeakyReLU ->
     ConvTranspose1d (fused pre-activation) and the MRF average, then LeakyReLU(0.01) -> output conv -> tanh.  Shared by
     HiFiGANGenerator and the discrete-symbol generators; the conv-transpose padding is read from each module, which
-    is where the two differ.  Inference runs the fused ResBlock pairs, autograd ScaledSumFn."""
+    is where the two differ.  Inference runs the fused ResBlock pairs, autograd ScaledSumFn.
+
+    ``lengths`` ((B,) int32 frame counts on the device, non-causal inference): a ragged batch whose input c is zero past
+    each item's end.  Each conv-transpose output is masked with one pwgb_stream_mask (its kernels are the ones
+    ``inference`` takes, and the mask pass is one read and write of a tensor that the MRF then reads 3 x 3 x 2 times),
+    the MRF pairs mask in their epilogues, and the output conv needs none: nothing reads it.  Every sample of item b
+    before lengths[b] * hop then equals ``forward`` of that item alone wherever both take the same kernels."""
     nb = g.num_blocks
+    rate = 1
     for i in range(g.num_upsamples):
         up = g.upsamples[i][1]
         if g.use_causal_conv:
             c = up(c, pre_slope=g.slope)
         else:
+            t_in = c.shape[-1]
             c = ops.conv_transpose1d(c, effective_weight(up), up.bias, stride=up.stride[0], padding=up.padding[0],
                                      output_padding=up.output_padding[0], pre_slope=g.slope)
-        c = _mrf_average(g.blocks, i * nb, nb, c, torch.is_grad_enabled() and (c.requires_grad or next(g.parameters()).requires_grad))
+        mask = None
+        if lengths is not None:
+            if c.shape[-1] != t_in * up.stride[0]:
+                raise PwgbError(f"per-item lengths: upsampling level {i} maps {t_in} frames to {c.shape[-1]} samples, not "
+                                f"{t_in} x {up.stride[0]}")
+            rate *= up.stride[0]
+            mask = _length_mask(lengths, c.shape[0], rate)
+            ops.stream_mask(c, mask)
+        c = _mrf_average(g.blocks, i * nb, nb, c, torch.is_grad_enabled() and (c.requires_grad or next(g.parameters()).requires_grad),
+                         mask)
     oc = g.output_conv[1]
     if g.use_causal_conv:
         return oc(c, pre_slope=0.01, post_act="tanh")
@@ -157,11 +194,18 @@ class HiFiGANGenerator(_GeneratorBase):
             self.apply_weight_norm()
         self.reset_parameters()
 
-    def forward(self, c):
-        """(B, in_channels, T) -> (B, out_channels, T * prod(upsample_scales))  (hifigan.py:173-192)."""
+    def forward(self, c, lengths=None):
+        """(B, in_channels, T) -> (B, out_channels, T * prod(upsample_scales))  (hifigan.py:173-192).
+
+        ``lengths``: (B,) int32 frame counts on the device, for a batch of utterances of different lengths padded with
+        zero frames (inference).  Item b's first lengths[b] * hop samples are then the forward of its first lengths[b]
+        frames alone (see _hifigan_body); the rest is padding.  A causal generator needs no mask: its outputs never
+        read later frames, so it ignores ``lengths``."""
         ic = self.input_conv
-        c = ic(c) if self.use_causal_conv else ops.conv1d(c, effective_weight(ic), ic.bias, padding=(self.kernel_size - 1) // 2)
-        return _hifigan_body(self, c)
+        if self.use_causal_conv:
+            return _hifigan_body(self, ic(c))
+        c = ops.conv1d(c, effective_weight(ic), ic.bias, padding=(self.kernel_size - 1) // 2)
+        return _hifigan_body(self, _masked(c, lengths, 1), lengths)
 
     def reset_parameters(self):
         def _reset_parameters(m):
@@ -283,13 +327,18 @@ class DiscreteSymbolHiFiGANGenerator(torch.nn.Module):
         spk = self.spk_emb.weight if self.num_spk_embs > 0 else None
         return ops.symbol_embed(c, self.emb.weight, spk, ds=ds, t_out=t_out, symbol_level=symbol_level)
 
-    def _body(self, c):
+    def _body(self, c, lengths=None):
         ic = self.input_conv
-        return _hifigan_body(self, ops.conv1d(c, effective_weight(ic), ic.bias, padding=(self.kernel_size - 1) // 2))
+        c = ops.conv1d(_masked(c, lengths, 1), effective_weight(ic), ic.bias, padding=(self.kernel_size - 1) // 2)
+        return _hifigan_body(self, _masked(c, lengths, 1), lengths)
 
-    def forward(self, c):
-        """c (B, 2, T) (symbol, speaker id) or (B, 1, T) -> (B, out_channels, T * prod(upsample_scales))  (hifigan.py:995-1031)."""
-        return self._body(self._embed(c))
+    def forward(self, c, lengths=None):
+        """c (B, 2, T) (symbol, speaker id) or (B, 1, T) -> (B, out_channels, T * prod(upsample_scales))  (hifigan.py:995-1031).
+
+        ``lengths``: (B,) int32 frame counts on the device (inference), as in HiFiGANGenerator.forward; the embedding of
+        the indices past an item's end (any symbol) is masked to zero before input_conv, and each item's speaker is its
+        own first frame's."""
+        return self._body(self._embed(c), lengths)
 
     def _prep_symbols(self, c, g):
         """inference input plumbing (hifigan.py:1082-1090): (T, 2) or (T, 1) -> (1, K, T) view."""

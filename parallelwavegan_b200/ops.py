@@ -191,14 +191,19 @@ def conv1d_raw(
     return out
 
 
-def resblock_pair(x, w1, b1, w2, b2, *, kernel_size, dilation, slope, out=None, accumulate=False, out_scale=1.0):
+def resblock_pair(x, w1, b1, w2, b2, *, kernel_size, dilation, slope, out=None, accumulate=False, out_scale=1.0, mask=None):
     """One HiFi-GAN ResBlock conv pair in one launch (pwgb_resblock_pair_forward), inference only:
         x' = conv_{k,1}(lrelu(conv_{k,d}(lrelu(x)) + b1)) + b2 + x     ("same" zero padding, LeakyReLU ``slope``)
     returned as ``out_scale * x'``, or written / added into ``out``.  Bit-identical to the two conv1d calls it replaces.
     At 128 and 256 channels the pair runs as two launches (pwgb_resblock_pair_packed_forward) that hand the intermediate
     over as the second conv's packed bf16 hi/lo operand image.  Returns None when neither serves the call (autograd, the
     FFMA engine, other channel counts, t % 4 != 0, a conv1 halo too wide for the shared-memory plan, unaligned tensors):
-    the caller then runs the two convs."""
+    the caller then runs the two convs.
+
+    ``mask`` = (frame, end, rate, lookahead) as in conv1d_stream (pwgb_resblock_pair_ext_forward /
+    pwgb_resblock_pair_packed_ext_forward): the intermediate the second conv reads and the result are +0.0 outside each
+    item's signal.  x must be zero there, and so must ``out`` with ``accumulate``; each item's rows inside its signal
+    are then bit-identical to the pair on that item alone."""
     if ENGINE == "simt" or _needs_grad(x, w1, b1, w2, b2):
         return None
     if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 3 and x.is_contiguous()):
@@ -231,20 +236,28 @@ def resblock_pair(x, w1, b1, w2, b2, *, kernel_size, dilation, slope, out=None, 
     if out.numel() == 0:
         return out  # an empty batch: nothing to compute (and no device pointers to pass)
     pk1, pk2 = packed_weight(w1), packed_weight(w2)
+    ext = _stream_ext(B, Cc, mask, None, 0) if mask is not None else None
     if packed:
         h = torch.empty_like(x)  # the packed intermediate: 4 bytes per value, as fp32
         # bytes: x (conv1's input and conv2's residual), the intermediate written and read, out written (and read)
         prof = _Prof("resblock_pair_packed_tc", 2 * 2.0 * B * Cc * T * Cc * K,
                      4.0 * (2 * x.numel() + 2 * h.numel() + out.numel() * (2 if accumulate else 1)),
                      f"B{B} C{Cc} k{K} d{dilation} T{T}" if PROFILE is not None else "")
-        rc = L.pwgb_resblock_pair_packed_forward(C.byref(d), _p(x), _p(pk1), _p(b1), _p(pk2), _p(b2), _p(h), _p(out), _stream())
+        if ext is not None:
+            rc = L.pwgb_resblock_pair_packed_ext_forward(C.byref(d), _p(x), _p(pk1), _p(b1), _p(pk2), _p(b2), C.byref(ext), _p(h),
+                                                         _p(out), _stream())
+        else:
+            rc = L.pwgb_resblock_pair_packed_forward(C.byref(d), _p(x), _p(pk1), _p(b1), _p(pk2), _p(b2), _p(h), _p(out), _stream())
         capi.check(rc, "pwgb_resblock_pair_packed_forward")
         prof.done()
         return out
     # FLOPs of both convs; bytes: x once, out written (and read too when accumulating), the intermediate stays on chip
     prof = _Prof("resblock_pair_tc", 2 * 2.0 * B * Cc * T * Cc * K, 4.0 * (x.numel() + out.numel() * (2 if accumulate else 1)),
                  f"B{B} C{Cc} k{K} d{dilation} T{T}" if PROFILE is not None else "")
-    rc = L.pwgb_resblock_pair_forward(C.byref(d), _p(x), _p(pk1), _p(b1), _p(pk2), _p(b2), _p(out), _stream())
+    if ext is not None:
+        rc = L.pwgb_resblock_pair_ext_forward(C.byref(d), _p(x), _p(pk1), _p(b1), _p(pk2), _p(b2), C.byref(ext), _p(out), _stream())
+    else:
+        rc = L.pwgb_resblock_pair_forward(C.byref(d), _p(x), _p(pk1), _p(b1), _p(pk2), _p(b2), _p(out), _stream())
     capi.check(rc, "pwgb_resblock_pair_forward")
     prof.done()
     return out
