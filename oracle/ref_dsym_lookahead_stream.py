@@ -16,6 +16,7 @@ import torch.nn.functional as F
 
 from .ref_discrete import dsym_generator
 from .ref_hifigan_lookahead_stream import HiFiGANLookaheadRef
+from .ref_stream import drive
 
 
 def body_cfg(cfg):
@@ -64,13 +65,7 @@ def stream(w, c, cfg, schedule, **kw):
     """Run ``DSymLookaheadRef`` over c (B, K, T) in chunks of ``schedule`` frames (repeated until the utterance is used
     up; the last chunk is cut short), then flush; returns cat(pushes, flush)."""
     ref = DSymLookaheadRef(w, cfg, batch=c.shape[0], **kw)
-    outs, j, k = [], 0, 0
-    while j < c.shape[-1]:
-        n = min(schedule[k % len(schedule)], c.shape[-1] - j)
-        outs.append(ref.push(c[:, :, j:j + n]))
-        j, k = j + n, k + 1
-    outs.append(ref.flush())
-    return torch.cat(outs, -1)
+    return drive(lambda j, n: ref.push(c[:, :, j:j + n]), c.shape[-1], schedule, ref.flush)
 
 
 class DSymDurationLookaheadRef:
@@ -179,10 +174,5 @@ def duration_stream(w, c, cfg, schedule, **kw):
     """Run ``DSymDurationLookaheadRef`` over the symbols c (S,) in pushes of ``schedule`` symbols, then flush; returns
     (cat(pushes, flush), the finalised durations, their log-domain values)."""
     ref = DSymDurationLookaheadRef(w, cfg, **kw)
-    outs, j, k = [], 0, 0
-    while j < len(c):
-        n = min(schedule[k % len(schedule)], len(c) - j)
-        outs.append(ref.push(c[j:j + n]))
-        j, k = j + n, k + 1
-    outs.append(ref.flush())
-    return torch.cat(outs, -1), torch.tensor(ref.durations), torch.tensor(ref.log_durations, dtype=torch.float64)
+    y = drive(lambda j, n: ref.push(c[j:j + n]), len(c), schedule, ref.flush)
+    return y, torch.tensor(ref.durations), torch.tensor(ref.log_durations, dtype=torch.float64)

@@ -33,34 +33,13 @@ import torch
 import torch.nn.functional as F
 
 from .ref_ops import hifigan_generator
+from .ref_stream import conv, drive, keep, rows
+from .ref_stream import measured_lookahead as _measured
 
 
 def whole_utterance(w, c, cfg):
     """``HiFiGANGenerator.inference`` (centred) for a batch of whole utterances c (B, in_channels, T)."""
     return hifigan_generator(w, c, cfg)
-
-
-def _keep(x, h):
-    """the last ``h`` samples of x (zero-extended on the left)"""
-    if h == 0:
-        return x[..., :0]
-    kept = x[..., max(x.shape[-1] - h, 0):]
-    return F.pad(kept, (h - kept.shape[-1], 0))
-
-
-def _rows(hist, x, first, n):
-    """rows [first, first + n) of [hist | x], row 0 being x's first"""
-    xp = torch.cat([hist, x], -1)
-    H = hist.shape[-1]
-    assert 0 <= H + first and H + first + n <= xp.shape[-1], (H, first, n, xp.shape)
-    return xp[..., H + first:H + first + n]
-
-
-def _conv(hist, x, w, b, d, slope, pad_left, n):
-    """n outputs of the conv of lrelu([hist | x]) whose first output reads row -pad_left"""
-    k = w.shape[-1]
-    xs = _rows(hist, x, -pad_left, n + (k - 1) * d)
-    return F.conv1d(F.leaky_relu(xs, slope), w, b, dilation=d)
 
 
 class HiFiGANLookaheadRef:
@@ -119,8 +98,8 @@ class HiFiGANLookaheadRef:
         w, slope = self.w, self.slope
         c = c.to(self.dtype)
         n, K = c.shape[-1], self.K
-        h = self._mask(_conv(self.cin, c, w["input_conv.weight"], w.get("input_conv.bias"), 1, 1.0, K - 1, n), 1, self.look_in)
-        self.cin = _keep(torch.cat([self.cin, c], -1), K - 1)
+        h = self._mask(conv(self.cin, c, w["input_conv.weight"], w.get("input_conv.bias"), 1, 1.0, K - 1, n), 1, self.look_in)
+        self.cin = keep(torch.cat([self.cin, c], -1), K - 1)
         for i, lv in enumerate(self.levels):
             s, rate = lv["s"], lv["rate"]
             # up_replicate: the fresh history is the signal's sample 0 (ReplicationPad1d), held by a first chunk that
@@ -138,23 +117,23 @@ class HiFiGANLookaheadRef:
                 for idx, d in enumerate(ds):
                     hx, extra = (self.lvl[i], lv["delta"][j]) if idx == 0 else (self.xh[i][j][idx - 1], 0)
                     q = lv["q"][j][idx]
-                    xt = _conv(hx, x, w[f"{p}.convs1.{idx}.1.weight"], w.get(f"{p}.convs1.{idx}.1.bias"), d, slope, (k - 1) * d + extra, t)
+                    xt = conv(hx, x, w[f"{p}.convs1.{idx}.1.weight"], w.get(f"{p}.convs1.{idx}.1.bias"), d, slope, (k - 1) * d + extra, t)
                     xt = self._mask(xt, rate, cur + (k - 1) * d // 2)
                     if self.extra:
                         ht = self.xth[i][j][idx]
-                        self.xth[i][j][idx] = _keep(torch.cat([ht, xt], -1), k - 1)
-                        xt = _conv(ht, xt, w[f"{p}.convs2.{idx}.1.weight"], w.get(f"{p}.convs2.{idx}.1.bias"), 1, slope, k - 1, t)
-                    res = x if self.undelayed_res else _rows(hx, x, -(q + extra), t)
+                        self.xth[i][j][idx] = keep(torch.cat([ht, xt], -1), k - 1)
+                        xt = conv(ht, xt, w[f"{p}.convs2.{idx}.1.weight"], w.get(f"{p}.convs2.{idx}.1.bias"), 1, slope, k - 1, t)
+                    res = x if self.undelayed_res else rows(hx, x, -(q + extra), t)
                     if idx > 0:
-                        self.xh[i][j][idx - 1] = _keep(torch.cat([hx, x], -1), hx.shape[-1])
+                        self.xh[i][j][idx - 1] = keep(torch.cat([hx, x], -1), hx.shape[-1])
                     cur += q
                     x = self._mask(xt + res, rate, cur)
                 cs = cs + x
-            self.lvl[i] = _keep(torch.cat([self.lvl[i], u], -1), lv["hl"])
+            self.lvl[i] = keep(torch.cat([self.lvl[i], u], -1), lv["hl"])
             h = cs / self.nb
-        y = torch.tanh(_conv(self.out, h, w["output_conv.1.weight"], w.get("output_conv.1.bias"), 1, 0.01, K - 1, h.shape[-1]))
+        y = torch.tanh(conv(self.out, h, w["output_conv.1.weight"], w.get("output_conv.1.bias"), 1, 0.01, K - 1, h.shape[-1]))
         y = self._mask(y, self.hop, self.delay)
-        self.out = _keep(torch.cat([self.out, h], -1), K - 1)
+        self.out = keep(torch.cat([self.out, h], -1), K - 1)
         self.frame += n
         self.fresh = False
         return y
@@ -172,32 +151,13 @@ def stream(w, c, cfg, schedule, **kw):
     """Run ``HiFiGANLookaheadRef`` over c (B, in_channels, T) in chunks of ``schedule`` frames (repeated until the
     utterance is used up; the last chunk is cut short), then flush; returns cat(pushes, flush)."""
     ref = HiFiGANLookaheadRef(w, cfg, batch=c.shape[0], **kw)
-    outs, j, k = [], 0, 0
-    while j < c.shape[-1]:
-        n = min(schedule[k % len(schedule)], c.shape[-1] - j)
-        outs.append(ref.push(c[:, :, j:j + n]))
-        j, k = j + n, k + 1
-    outs.append(ref.flush())
-    return torch.cat(outs, -1)
+    return drive(lambda j, n: ref.push(c[:, :, j:j + n]), c.shape[-1], schedule, ref.flush)
 
 
 def measured_lookahead(w, cfg, frames):
-    """The true lookahead of the centred generator in output samples, measured by autograd: the largest f * hop - o over
-    output samples o that depend on frame f.  The dependency is shift-invariant by a frame, so frame f = frames - 1 and a
-    binary search for the first output sample that depends on it give it."""
-    hop = math.prod(cfg["upsample_scales"])
+    """The true lookahead of the centred generator in output samples, measured by autograd at the last of ``frames``
+    frames (``ref_stream.measured_lookahead``)."""
     g = torch.Generator().manual_seed(3)
     c = torch.randn(1, cfg["in_channels"], frames, generator=g, dtype=torch.float64, requires_grad=True)
-    y = whole_utterance({k: v.double() for k, v in w.items()}, c, cfg)
-    f = frames - 1
-
-    def depends(o):
-        (gc,) = torch.autograd.grad(y[0, 0, o], c, retain_graph=True)
-        return bool(gc[0, :, f].abs().sum() > 0)
-
-    lo, hi = 0, y.shape[-1] - 1
-    assert depends(hi) and not depends(0)
-    while hi - lo > 1:
-        mid = (lo + hi) // 2
-        lo, hi = (lo, mid) if depends(mid) else (mid, hi)
-    return f * hop - hi
+    wd = {k: v.double() for k, v in w.items()}
+    return _measured(lambda c: whole_utterance(wd, c, cfg), c, frames - 1, math.prod(cfg["upsample_scales"]))

@@ -16,19 +16,12 @@ import torch
 import torch.nn.functional as F
 
 from .ref_ops import hifigan_generator
+from .ref_stream import drive, keep
 
 
 def whole_utterance(w, c, cfg):
     """``HiFiGANGenerator.inference`` for a batch of whole utterances c (B, in_channels, T)."""
     return hifigan_generator(w, c, cfg)
-
-
-def _keep(x, h, short=0):
-    """the last ``h`` samples of x as the history to carry (``short``: that many of the oldest lost, zero instead)"""
-    if h == 0:
-        return x[..., :0]
-    kept = x[..., x.shape[-1] - h + short:]
-    return F.pad(kept, (h - kept.shape[-1], 0))
 
 
 def _causal(x, hist, w, b, d, slope):
@@ -68,7 +61,7 @@ class HiFiGANStreamRef:
         w, slope = self.w, self.slope
         c = c.to(self.dtype)
         h = _causal(c, self.cin, w["input_conv.conv.weight"], w.get("input_conv.conv.bias"), 1, 1.0)
-        self.cin = _keep(torch.cat([self.cin, c], -1), self.cin.shape[-1])
+        self.cin = keep(torch.cat([self.cin, c], -1), self.cin.shape[-1])
         for i, s in enumerate(self.scales):
             hist = h[:, :, :1] if self.fresh and not self.up_zero else self.up[i]
             xp = torch.cat([hist, h], -1)
@@ -82,18 +75,18 @@ class HiFiGANStreamRef:
                 for idx, d in enumerate(ds):
                     hx = self.lvl[i] if idx == 0 else self.xh[i][j][idx - 1]
                     if idx > 0:
-                        self.xh[i][j][idx - 1] = _keep(torch.cat([hx, x], -1), hx.shape[-1], self.dil_short)
+                        self.xh[i][j][idx - 1] = keep(torch.cat([hx, x], -1), hx.shape[-1], self.dil_short)
                     xt = _causal(x, hx, w[f"{p}.convs1.{idx}.1.conv.weight"], w.get(f"{p}.convs1.{idx}.1.conv.bias"), d, slope)
                     if self.extra:
                         ht = self.xth[i][j][idx]
-                        self.xth[i][j][idx] = _keep(torch.cat([ht, xt], -1), k - 1)
+                        self.xth[i][j][idx] = keep(torch.cat([ht, xt], -1), k - 1)
                         xt = _causal(xt, ht, w[f"{p}.convs2.{idx}.1.conv.weight"], w.get(f"{p}.convs2.{idx}.1.conv.bias"), 1, slope)
                     x = xt + x
                 cs = cs + x
-            self.lvl[i] = _keep(torch.cat([self.lvl[i], u], -1), self.lvl[i].shape[-1])
+            self.lvl[i] = keep(torch.cat([self.lvl[i], u], -1), self.lvl[i].shape[-1])
             h = cs / self.nb
         y = torch.tanh(_causal(h, self.out, w["output_conv.1.conv.weight"], w.get("output_conv.1.conv.bias"), 1, 0.01))
-        self.out = _keep(torch.cat([self.out, h], -1), self.out.shape[-1])
+        self.out = keep(torch.cat([self.out, h], -1), self.out.shape[-1])
         self.fresh = False
         return y
 
@@ -102,9 +95,4 @@ def stream(w, c, cfg, schedule, **kw):
     """Run ``HiFiGANStreamRef`` over c (B, in_channels, T) in chunks of ``schedule`` frames (repeated until the utterance is
     used up; the last chunk is cut short) and return the concatenated output."""
     ref = HiFiGANStreamRef(w, cfg, batch=c.shape[0], **kw)
-    outs, j, k = [], 0, 0
-    while j < c.shape[-1]:
-        n = min(schedule[k % len(schedule)], c.shape[-1] - j)
-        outs.append(ref.push(c[:, :, j:j + n]))
-        j, k = j + n, k + 1
-    return torch.cat(outs, -1)
+    return drive(lambda j, n: ref.push(c[:, :, j:j + n]), c.shape[-1], schedule)

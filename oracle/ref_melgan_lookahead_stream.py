@@ -27,6 +27,8 @@ import torch
 import torch.nn.functional as F
 
 from .ref_ops import melgan_layer_index, pqmf_filters, pqmf_synthesis
+from .ref_stream import drive, keep
+from .ref_stream import measured_lookahead as _measured
 
 MODES = {"reflect": "reflect", "replicate": "replicate", "zero": "constant"}
 
@@ -74,14 +76,6 @@ def min_frames(cfg, pad="reflect"):
         need += [((sk - 1) // 2 * sk ** j, rate) for j in range(cfg["stacks"])]
     need.append(((K - 1) // 2, rate))
     return max(P // r + 1 for P, r in need)
-
-
-def _keep(x, h):
-    """the last ``h`` samples of x (zero-extended on the left)"""
-    if h == 0:
-        return x[..., :0]
-    kept = x[..., max(x.shape[-1] - h, 0):]
-    return F.pad(kept, (h - kept.shape[-1], 0))
 
 
 class MelGANLookaheadRef:
@@ -162,7 +156,7 @@ class MelGANLookaheadRef:
         H = (wt.shape[-1] - 1) * d
         hist = self.hist.get(key, x.new_zeros(x.shape[0], x.shape[1], H))
         xp = torch.cat([hist, x], -1)
-        self.hist[key] = _keep(xp, H)
+        self.hist[key] = keep(xp, H)
         xe = self._edge(xp, rate, in_look_x + H)
         return F.conv1d(F.leaky_relu(xe, slope), wt, b, dilation=d), hist
 
@@ -170,7 +164,7 @@ class MelGANLookaheadRef:
         """the synthesis window of subband chunk y (B, N, m): m * N samples from N * (first row) - taps // 2 on"""
         N, H = self.N, self.pq.shape[-1]
         full = torch.cat([self.pq, y], -1)
-        self.pq = _keep(full, H)
+        self.pq = keep(full, H)
         z = torch.zeros(full.shape[0], N, full.shape[-1] * N, dtype=full.dtype)
         z[..., ::N] = full * N
         lead = self.taps - H * N
@@ -227,32 +221,14 @@ def stream(w, c, cfg, schedule, pad="reflect", subbands=None, **kw):
     """Run ``MelGANLookaheadRef`` over c (B, in_channels, T) in chunks of ``schedule`` frames (repeated until the
     utterance is used up; the last chunk is cut short), then flush; returns cat(pushes, flush)."""
     ref = MelGANLookaheadRef(w, cfg, pad=pad, subbands=subbands, batch=c.shape[0], **kw)
-    outs, j, k = [], 0, 0
-    while j < c.shape[-1]:
-        n = min(schedule[k % len(schedule)], c.shape[-1] - j)
-        outs.append(ref.push(c[:, :, j:j + n]))
-        j, k = j + n, k + 1
-    outs.append(ref.flush())
-    return torch.cat(outs, -1)
+    return drive(lambda j, n: ref.push(c[:, :, j:j + n]), c.shape[-1], schedule, ref.flush)
 
 
 def measured_lookahead(w, cfg, frames, pad="reflect", subbands=None):
-    """The true lookahead of the centred generator in output samples, measured by autograd: the largest f * hop - o over
-    output samples o that depend on frame f, found for f = frames - 1 by a binary search for the first output sample
-    that depends on it."""
+    """The true lookahead of the centred generator in output samples, measured by autograd at the last of ``frames``
+    frames (``ref_stream.measured_lookahead``)."""
     hop = math.prod(cfg["upsample_scales"]) * (subbands or 1)
     g = torch.Generator().manual_seed(3)
     c = torch.randn(1, cfg["in_channels"], frames, generator=g, dtype=torch.float64, requires_grad=True)
-    y = whole_utterance({k: v.double() for k, v in w.items()}, c, cfg, pad, subbands)
-    f = frames - 1
-
-    def depends(o):
-        (gc,) = torch.autograd.grad(y[0, 0, o], c, retain_graph=True)
-        return bool(gc[0, :, f].abs().sum() > 0)
-
-    lo, hi = 0, y.shape[-1] - 1
-    assert depends(hi) and not depends(0)
-    while hi - lo > 1:
-        mid = (lo + hi) // 2
-        lo, hi = (lo, mid) if depends(mid) else (mid, hi)
-    return f * hop - hi
+    wd = {k: v.double() for k, v in w.items()}
+    return _measured(lambda c: whole_utterance(wd, c, cfg, pad, subbands), c, frames - 1, hop)

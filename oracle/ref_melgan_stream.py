@@ -21,6 +21,7 @@ import torch
 import torch.nn.functional as F
 
 from .ref_ops import causal_conv_transpose1d, melgan_layer_index, pqmf_filters, pqmf_synthesis
+from .ref_stream import drive, keep
 
 MODES = {"reflect": "reflect", "replicate": "replicate", "zero": "constant"}
 
@@ -53,14 +54,6 @@ def whole_utterance(w, c, cfg, pad="reflect", subbands=None):
     if subbands:
         c = pqmf_synthesis(c, pqmf_filters(subbands)[1].to(c.dtype))
     return c
-
-
-def _keep(x, h, short=0):
-    """the last ``h`` samples of x as the history to carry (``short``: that many of the oldest lost, zero instead)"""
-    if h == 0:
-        return x[..., :0]
-    kept = x[..., x.shape[-1] - h + short:]
-    return F.pad(kept, (h - kept.shape[-1], 0))
 
 
 class MelGANStreamRef:
@@ -96,14 +89,14 @@ class MelGANStreamRef:
         else:
             h = self.hist[key]
         xp = torch.cat([h, x], -1)
-        self.hist[key] = _keep(xp, P, self.stack_short if key[0] == "stack" else 0)
+        self.hist[key] = keep(xp, P, self.stack_short if key[0] == "stack" else 0)
         return F.conv1d(xp, w, b, dilation=d)
 
     def _synth(self, y):
         """the synthesis window of subband chunk y (B, N, m), m * N samples lagging by D"""
         N, H = self.N, self.pq.shape[-1]
         full = torch.cat([self.pq, y], -1)
-        self.pq = _keep(full, H, self.pq_short)
+        self.pq = keep(full, H, self.pq_short)
         z = torch.zeros(full.shape[0], N, full.shape[-1] * N, dtype=full.dtype)
         z[..., ::N] = full * N
         lead = self.taps - H * N  # zero-stuffed samples in front of the oldest history row that the filter still reaches
@@ -154,13 +147,4 @@ def stream(w, c, cfg, schedule, pad="reflect", subbands=None, first=None, **kw):
     frames if given; repeated until the utterance is used up, the last chunk cut short), flush, and return the
     concatenated output"""
     ref = MelGANStreamRef(w, cfg, pad=pad, subbands=subbands, batch=c.shape[0], **kw)
-    outs, j, k = [], 0, 0
-    if first:
-        outs.append(ref.push(c[:, :, :first]))
-        j = first
-    while j < c.shape[-1]:
-        n = min(schedule[k % len(schedule)], c.shape[-1] - j)
-        outs.append(ref.push(c[:, :, j:j + n]))
-        j, k = j + n, k + 1
-    outs.append(ref.flush())
-    return torch.cat(outs, -1)
+    return drive(lambda j, n: ref.push(c[:, :, j:j + n]), c.shape[-1], schedule, ref.flush, first)

@@ -37,6 +37,8 @@ import torch.nn.functional as F
 
 from .ref_pwg_stream import _fir_prefix
 from .ref_pwg_stream import whole_utterance as _whole
+from .ref_stream import drive, keep
+from .ref_stream import measured_lookahead as _measured
 
 
 def whole_utterance(w, z, c, cfg):
@@ -61,11 +63,6 @@ def plan(cfg):
         D.append(acc)
     look_x = max(look - D[0], 0)
     return look_in, looks, look_x, D, look_x + D[-1]
-
-
-def _keep(x, h):
-    """the last ``h`` samples of x"""
-    return x[..., x.shape[-1] - h:] if h else x[..., :0]
 
 
 class PWGLookaheadRef:
@@ -119,7 +116,7 @@ class PWGLookaheadRef:
         W, T = self.off[-1], x.shape[-1]
         H = (K - 1) * d
         xp = torch.cat([self.wn[l], x], -1)
-        self.wn[l] = _keep(xp, H)
+        self.wn[l] = keep(xp, H)
         g = F.conv1d(xp, w[f"{p}.conv.weight"], w.get(f"{p}.conv.bias"), dilation=d)
         c0 = W if self.undelayed_cond else W - self.off[l]
         ca = F.conv1d(cwin[..., c0:c0 + T], w[f"{p}.conv1x1_aux.weight"])
@@ -141,7 +138,7 @@ class PWGLookaheadRef:
             if self.cin is None:
                 self.cin = c[:, :, :1].expand(-1, -1, P).clone()
             x = torch.cat([self.cin, c], -1)
-            self.cin = _keep(x, P)
+            self.cin = keep(x, P)
             c = self._mask(F.conv1d(x, w["upsample_net.conv_in.weight"]), 1, self.look_in)
         prefix = _fir_prefix(cfg)
         for i, s in enumerate(self.scales):
@@ -153,9 +150,9 @@ class PWGLookaheadRef:
             c = self._mask(c, math.prod(self.scales[:i + 1]), self.looks[i])
         T = c.shape[-1]
         cwin = torch.cat([self.ch, c], -1)
-        self.ch = _keep(cwin, self.off[-1])
+        self.ch = keep(cwin, self.off[-1])
         zw = torch.cat([self.zh, z], -1)
-        self.zh = _keep(zw, self.look_x)
+        self.zh = keep(zw, self.look_x)
         zd = z if self.undelayed_noise else zw[..., :T]
         x = self._mask(F.conv1d(zd, w["first_conv.weight"], w["first_conv.bias"]), self.hop, self.look_x)
         sw = torch.cat([self.sk, torch.zeros(self.B, self.sk.shape[1], T, dtype=self.dtype)], -1)
@@ -187,33 +184,15 @@ def stream(w, z, c, cfg, schedule, **kw):
     the utterance is used up; the last chunk is cut short), then flush; returns cat(pushes, flush)."""
     hop = math.prod(cfg["upsample_scales"])
     ref = PWGLookaheadRef(w, cfg, batch=c.shape[0], **kw)
-    outs, j, k = [], 0, 0
-    while j < c.shape[-1]:
-        n = min(schedule[k % len(schedule)], c.shape[-1] - j)
-        outs.append(ref.push(c[:, :, j:j + n], z[:, :, j * hop:(j + n) * hop]))
-        j, k = j + n, k + 1
-    outs.append(ref.flush())
-    return torch.cat(outs, -1)
+    return drive(lambda j, n: ref.push(c[:, :, j:j + n], z[:, :, j * hop:(j + n) * hop]), c.shape[-1], schedule, ref.flush)
 
 
 def measured_lookahead(w, cfg, frames):
-    """The true lookahead of the centred generator in output samples, measured by autograd: the largest f * hop - o over
-    output samples o that depend on frame f.  The dependency is shift-invariant by a frame, so frame f = frames - 1 and a
-    binary search for the first output sample that depends on it give it."""
+    """The true lookahead of the centred generator in output samples, measured by autograd on the mel frames at the last
+    of ``frames`` frames (``ref_stream.measured_lookahead``)."""
     hop = math.prod(cfg["upsample_scales"])
     g = torch.Generator().manual_seed(3)
     c = torch.randn(1, cfg["aux_channels"], frames, generator=g, dtype=torch.float64, requires_grad=True)
     z = torch.randn(1, cfg.get("in_channels", 1), frames * hop, generator=g, dtype=torch.float64)
-    y = whole_utterance({k: v.double() for k, v in w.items()}, z, c, cfg)
-    f = frames - 1
-
-    def depends(o):
-        (gc,) = torch.autograd.grad(y[0, 0, o], c, retain_graph=True)
-        return bool(gc[0, :, f].abs().sum() > 0)
-
-    lo, hi = 0, y.shape[-1] - 1
-    assert depends(hi) and not depends(0)
-    while hi - lo > 1:
-        mid = (lo + hi) // 2
-        lo, hi = (lo, mid) if depends(mid) else (mid, hi)
-    return f * hop - hi
+    wd = {k: v.double() for k, v in w.items()}
+    return _measured(lambda c: whole_utterance(wd, z, c, cfg), c, frames - 1, hop)

@@ -16,6 +16,7 @@ import torch
 import torch.nn.functional as F
 
 from .ref_causal_pwg import wavenet_residual_block
+from .ref_stream import drive, keep
 
 
 def _fir_prefix(cfg):
@@ -54,13 +55,6 @@ class PWGStreamRef:
         self.fir_hist = [torch.zeros(batch, A, 2, dtype=dtype) for _ in self.scales]
         self.wn_hist = [torch.zeros(batch, R, h, dtype=dtype) for h in self.H]
 
-    def _keep(self, x, h):
-        """the last ``h`` samples of x, as the history to carry (one row short if so injected: the oldest is lost)"""
-        if h == 0:
-            return x[..., :0]
-        kept = x[..., x.shape[-1] - h + self.wn_short:]
-        return F.pad(kept, (h - kept.shape[-1], 0))
-
     def push(self, c, z):
         w, cfg = self.w, self.cfg
         c, z = c.to(self.dtype), z.to(self.dtype)
@@ -91,7 +85,8 @@ class PWGStreamRef:
         skips = 0
         for l, (d, h) in enumerate(zip(self.dil, self.H)):
             xp = torch.cat([self.wn_hist[l], x], -1)
-            self.wn_hist[l] = self._keep(xp, h)
+            # wn_short: the oldest rows of the history lost
+            self.wn_hist[l] = keep(xp, h, self.wn_short)
             # the causal layer on [history | chunk]; its outputs over the history rows are discarded
             cp = F.pad(c, (h, 0))
             xo, s = wavenet_residual_block(w, f"conv_layers.{l}", xp, cp, d, cfg["kernel_size"], causal=True)
@@ -106,9 +101,4 @@ def stream(w, z, c, cfg, schedule, **kw):
     the utterance is used up; the last chunk is cut short) and return the concatenated output."""
     hop = math.prod(cfg["upsample_scales"])
     ref = PWGStreamRef(w, cfg, batch=c.shape[0], **kw)
-    outs, j, k = [], 0, 0
-    while j < c.shape[-1]:
-        n = min(schedule[k % len(schedule)], c.shape[-1] - j)
-        outs.append(ref.push(c[:, :, j:j + n], z[:, :, j * hop:(j + n) * hop]))
-        j, k = j + n, k + 1
-    return torch.cat(outs, -1)
+    return drive(lambda j, n: ref.push(c[:, :, j:j + n], z[:, :, j * hop:(j + n) * hop]), c.shape[-1], schedule)

@@ -31,7 +31,7 @@ import math
 import torch
 import torch.nn.functional as F
 
-from .ref_hifigan_lookahead_stream import _conv, _keep, _rows
+from .ref_stream import conv, drive, keep, rows
 from .ref_uhifigan import uhifigan_generator
 
 
@@ -75,19 +75,19 @@ class _MRF:
             for idx, d in enumerate(ds):
                 hx, extra = (self.lvl, self.delta[j]) if idx == 0 else (self.xh[j][idx - 1], 0)
                 q = self.q[j][idx]
-                xt = _conv(hx, x, w[f"{p}.convs1.{idx}.1.weight"], w.get(f"{p}.convs1.{idx}.1.bias"), d, slope, (k - 1) * d + extra, t)
+                xt = conv(hx, x, w[f"{p}.convs1.{idx}.1.weight"], w.get(f"{p}.convs1.{idx}.1.bias"), d, slope, (k - 1) * d + extra, t)
                 xt = ref._mask(xt, rate, cur + (k - 1) * d // 2)
                 if self.extra:
                     ht = self.xth[j][idx]
-                    self.xth[j][idx] = _keep(torch.cat([ht, xt], -1), k - 1)
-                    xt = _conv(ht, xt, w[f"{p}.convs2.{idx}.1.weight"], w.get(f"{p}.convs2.{idx}.1.bias"), 1, slope, k - 1, t)
-                res = _rows(hx, x, -(q + extra), t)
+                    self.xth[j][idx] = keep(torch.cat([ht, xt], -1), k - 1)
+                    xt = conv(ht, xt, w[f"{p}.convs2.{idx}.1.weight"], w.get(f"{p}.convs2.{idx}.1.bias"), 1, slope, k - 1, t)
+                res = rows(hx, x, -(q + extra), t)
                 if idx > 0:
-                    self.xh[j][idx - 1] = _keep(torch.cat([hx, x], -1), hx.shape[-1])
+                    self.xh[j][idx - 1] = keep(torch.cat([hx, x], -1), hx.shape[-1])
                 cur += q
                 x = ref._mask(xt + res, rate, cur)
             cs = cs + x
-        self.lvl = _keep(torch.cat([self.lvl, u], -1), self.hl)
+        self.lvl = keep(torch.cat([self.lvl, u], -1), self.hl)
         return cs / self.nb
 
 
@@ -170,16 +170,16 @@ class UHiFiGANLookaheadRef:
         n = c.shape[-1]
         assert e.shape[-1] == n * self.hop, (e.shape, n)
         # encoder
-        h = _conv(self.ein, e, w["input_conv.0.weight"], w.get("input_conv.0.bias"), 1, 1.0, K - 1, n * self.hop)
+        h = conv(self.ein, e, w["input_conv.0.weight"], w.get("input_conv.0.bias"), 1, 1.0, K - 1, n * self.hop)
         h = self._mask(F.leaky_relu(h, slope), self.hop, self.look_in)
-        self.ein = _keep(torch.cat([self.ein, e], -1), K - 1)
+        self.ein = keep(torch.cat([self.ein, e], -1), K - 1)
         skips = []
         for i, lv in enumerate(self.enc):
             h = lv["mrf"].push(self, h)
             s, H = lv["s"], lv["H"]
             hist = torch.zeros_like(lv["hist"]) if self.s2d_no_hist else lv["hist"]
             xw = torch.cat([hist, h], -1)
-            lv["hist"] = _keep(xw, H)
+            lv["hist"] = keep(xw, H)
             t = n * lv["rate"]
             first = 1 if self.stride_phase else 0
             xw = xw[..., first:first + (t - 1) * s + 2 * s]
@@ -189,25 +189,25 @@ class UHiFiGANLookaheadRef:
             skips.append(h)
         # bottom: hidden_conv at the decoder's first lookahead
         pad_left = K - 1 if self.mel_undelayed else self.cin_len
-        h = _conv(self.cin, c, w["hidden_conv.weight"], w.get("hidden_conv.bias"), 1, 1.0, pad_left, n)
+        h = conv(self.cin, c, w["hidden_conv.weight"], w.get("hidden_conv.bias"), 1, 1.0, pad_left, n)
         h = self._mask(h, 1, self.look_dec0)
-        self.cin = _keep(torch.cat([self.cin, c], -1), self.cin_len)
+        self.cin = keep(torch.cat([self.cin, c], -1), self.cin_len)
         # decoder
         for i, lv in enumerate(self.dec):
             skip = skips[-1 - i]
             s, t = lv["s"], h.shape[-1]
             d2 = 0 if self.skip_undelayed else lv["d2"]
-            x1 = _rows(lv["h1"], h, -(lv["d1"] + 1), t + 1)
-            x2 = _rows(lv["h2"], skip, -(d2 + 1), t + 1)
-            lv["h1"] = _keep(torch.cat([lv["h1"], h], -1), lv["d1"] + 1)
-            lv["h2"] = _keep(torch.cat([lv["h2"], skip], -1), lv["d2"] + 1)
+            x1 = rows(lv["h1"], h, -(lv["d1"] + 1), t + 1)
+            x2 = rows(lv["h2"], skip, -(d2 + 1), t + 1)
+            lv["h1"] = keep(torch.cat([lv["h1"], h], -1), lv["d1"] + 1)
+            lv["h2"] = keep(torch.cat([lv["h2"], skip], -1), lv["d2"] + 1)
             xp = torch.cat([x1, x2], 1)
             u = F.conv_transpose1d(F.leaky_relu(xp, slope), w[f"upsamples.{i}.1.weight"], w.get(f"upsamples.{i}.1.bias"), stride=s)
             u = self._mask(u[:, :, s:u.shape[-1] - s], lv["rate"], lv["look_u"])
             h = lv["mrf"].push(self, u)
-        y = torch.tanh(_conv(self.out, h, w["output_conv.1.weight"], w.get("output_conv.1.bias"), 1, 0.01, K - 1, h.shape[-1]))
+        y = torch.tanh(conv(self.out, h, w["output_conv.1.weight"], w.get("output_conv.1.bias"), 1, 0.01, K - 1, h.shape[-1]))
         y = self._mask(y, self.hop, self.delay)
-        self.out = _keep(torch.cat([self.out, h], -1), K - 1)
+        self.out = keep(torch.cat([self.out, h], -1), K - 1)
         self.frame += n
         return y
 
@@ -225,13 +225,7 @@ def stream(w, e, c, cfg, schedule, **kw):
     (repeated until the utterance is used up; the last chunk is cut short), then flush; returns cat(pushes, flush)."""
     ref = UHiFiGANLookaheadRef(w, cfg, batch=c.shape[0], **kw)
     hop = ref.hop
-    outs, j, k = [], 0, 0
-    while j < c.shape[-1]:
-        n = min(schedule[k % len(schedule)], c.shape[-1] - j)
-        outs.append(ref.push(c[:, :, j:j + n], e[:, :, j * hop:(j + n) * hop]))
-        j, k = j + n, k + 1
-    outs.append(ref.flush())
-    return torch.cat(outs, -1)
+    return drive(lambda j, n: ref.push(c[:, :, j:j + n], e[:, :, j * hop:(j + n) * hop]), c.shape[-1], schedule, ref.flush)
 
 
 def measured_lookahead(w, cfg, frames, first=2):

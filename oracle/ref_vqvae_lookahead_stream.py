@@ -24,7 +24,9 @@ import math
 import torch
 import torch.nn.functional as F
 
-from .ref_melgan_lookahead_stream import MelGANLookaheadRef, _keep
+from .ref_melgan_lookahead_stream import MelGANLookaheadRef
+from .ref_stream import drive, keep
+from .ref_stream import measured_lookahead as _measured
 from .ref_vqvae import _sub, assemble, decoder, encoder, quantize
 
 
@@ -91,7 +93,7 @@ class VQVAELookaheadRef:
     def _window(self, key, x, H):
         hist = self.hist.get(key, x.new_zeros(x.shape[0], x.shape[1], H))
         xp = torch.cat([hist, x], -1)
-        self.hist[key] = _keep(xp, H)
+        self.hist[key] = keep(xp, H)
         return xp
 
     def _conv0(self, x):
@@ -160,14 +162,12 @@ def stream(w, x, cfg, schedule, l=None, g=None, **kw):
     """Run ``VQVAELookaheadRef`` over x (B, 1, T * hop) in chunks of ``schedule`` frames (repeated until the signal is
     used up; the last chunk is cut short), then flush; returns cat(pushes, flush)."""
     ref = VQVAELookaheadRef(w, cfg, batch=x.shape[0], **kw)
-    hop, T = ref.hop, x.shape[-1] // ref.hop
-    outs, j, k = [], 0, 0
-    while j < T:
-        n = min(schedule[k % len(schedule)], T - j)
-        outs.append(ref.push(x[..., j * hop:(j + n) * hop], l[..., j:j + n] if l is not None else None, g))
-        j, k = j + n, k + 1
-    outs.append(ref.flush(l.shape[1] if l is not None else 0, g))
-    return torch.cat(outs, -1), ref
+    hop = ref.hop
+
+    def push(j, n):
+        return ref.push(x[..., j * hop:(j + n) * hop], l[..., j:j + n] if l is not None else None, g)
+
+    return drive(push, x.shape[-1] // hop, schedule, lambda: ref.flush(l.shape[1] if l is not None else 0, g)), ref
 
 
 def measured_lookahead(w, cfg, frames, l=None, g=None):
@@ -182,19 +182,12 @@ def measured_lookahead(w, cfg, frames, l=None, g=None):
     hop = math.prod(_enc_conf(cfg)[0])
     gen = torch.Generator().manual_seed(5)
     x = torch.randn(1, 1, frames * hop, generator=gen, dtype=torch.float64, requires_grad=True)
-    z = encoder(wd, x, cfg)
     cb = wd["codebook.embedding.weight"]
-    zq = _StraightThrough.apply(z, gather(cb, quantize(z, cb)))
-    y = decoder(wd, assemble(wd, zq, l, g), cfg)
-    f = frames - 10  # the outputs read the frame's samples well before the signal's end, and output 0 does not
 
-    def depends(o):
-        (gx,) = torch.autograd.grad(y[0, 0, o], x, retain_graph=True)
-        return bool(gx[0, 0, f * hop:(f + 1) * hop].abs().sum() > 0)
+    def whole(x):
+        z = encoder(wd, x, cfg)
+        zq = _StraightThrough.apply(z, gather(cb, quantize(z, cb)))
+        return decoder(wd, assemble(wd, zq, l, g), cfg)
 
-    lo, hi = 0, f * hop
-    assert depends(hi) and not depends(0)
-    while hi - lo > 1:
-        mid = (lo + hi) // 2
-        lo, hi = (lo, mid) if depends(mid) else (mid, hi)
-    return f * hop - hi
+    # the outputs read the frame's samples well before the signal's end, and output 0 does not
+    return _measured(whole, x, frames - 10, hop, rate=hop)

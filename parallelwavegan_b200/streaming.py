@@ -24,6 +24,8 @@ the current chunk:
 Every kernel computes each output sample with the same fp32 expression as ``model.inference`` on the whole utterance,
 so the concatenated chunks equal it bit for bit as long as both runs take the same kernels (see DESIGN.md).  The
 state is zeros for a fresh signal (the whole-utterance zero padding), so ``reset`` is a memset."""
+import contextlib
+
 import torch
 
 from . import ops
@@ -189,10 +191,13 @@ class _Lookahead:
     slots' state restored around it, then the flushed slots reset).  Mixed in before the stream's base class."""
 
     OPEN = 2 ** 31 - 1  # the end frame of a slot whose signal has not ended
+    subbands = 1  # output samples per frame are hop * subbands (a multi-band MelGAN's PQMF synthesis sets its own)
 
     def _counters(self):
+        """the frame counters, the open end frames, and the empty history of the input conv's launch on [history | chunk]"""
         self.frame = torch.zeros(self.B, device=self.dev, dtype=torch.int32)
         self.end = torch.full((self.B,), self.OPEN, device=self.dev, dtype=torch.int32)
+        self._nohist = self._zeros(self.B, self.in_channels, 0)
 
     def reset(self, items=None):
         super().reset(items)
@@ -202,46 +207,62 @@ class _Lookahead:
     def _mask(self, rate, look):
         return (self.frame, self.end, rate, look)
 
+    def _flush_frames(self):
+        """the frames of a flush push: the fewest whose output covers ``delay`` samples"""
+        return -(-self.delay // (self.hop * self.subbands))
+
+    @contextlib.contextmanager
+    def _keeping_others(self, items):
+        """Restores the state (and the fresh flags) of every slot but ``items`` (a checked list) after the block, so those
+        slots continue exactly as if it had not run."""
+        keep = [b for b in range(self.B) if b not in items]
+        carried = self._state() + ([self.fresh] if self.fresh is not None else [])
+        snap = [t[keep].clone() for t in carried] if keep else []
+        yield
+        for t, s in zip(carried, snap):
+            t[keep] = s
+
     def _flush(self, items, inputs):
         """The first ``delay`` samples of the flush push ``inputs()`` (the arguments of ``_run``) for slots ``items`` (a
         checked list); the other slots continue exactly as if it had not happened."""
-        keep = [b for b in range(self.B) if b not in items]
-        snap = [t[keep].clone() for t in self._state()] if keep else []
         sel = torch.tensor(items, device=self.dev, dtype=torch.long)
-        self.end[sel] = self.frame[sel]
-        y = self._run(*inputs())[sel, :, :self.delay].contiguous()
-        for t, s in zip(self._state(), snap):
-            t[keep] = s
+        with self._keeping_others(items):
+            self.end[sel] = self.frame[sel]
+            y = self._run(*inputs())[sel, :, :self.delay].contiguous()
         self.reset(items)
         return y
 
 
-class CausalPWGStream(_ChunkStream):
-    """Streams a causal ``ParallelWaveGANGenerator`` chunk by chunk for ``batch`` independent slots.
+class _PWGStream(_ChunkStream):
+    """The weights, histories and noise of a streamed ``ParallelWaveGANGenerator``, shared by the causal stream and the
+    centred one with lookahead: the conv_in and FIR weights of the upsampler and one history per FIR stage (its last two
+    input frames), the WaveNet shapes and one packed history per layer (its last (K - 1) * d_l input samples), the output
+    head, and the generator that draws the noise a push is not given."""
 
-    ``push(c, z)`` takes the next n >= 1 frames of every slot and returns their n * hop samples; n may change from
-    push to push.  For every slot, the concatenated outputs equal ``model.inference(c=all_frames, x=all_noise)``.
-    There is no lookahead and no flush.  With ``use_graphs`` each chunk length is captured once into a CUDA graph and
-    replayed.  The weights are read when the stream is built and must not change while it is used."""
-
-    def __init__(self, model, batch=1, seed=None, use_graphs=True):
+    def _build(self, model, batch, use_graphs, seed, causal):
         from .models import MelGANGenerator, ParallelWaveGANGenerator
 
+        name = type(self).__name__
         if not isinstance(model, ParallelWaveGANGenerator):
-            raise PwgbError("CausalPWGStream: expected a ParallelWaveGANGenerator")
-        if not model.use_causal_conv:
-            raise PwgbError("CausalPWGStream: the model is not causal (use_causal_conv=False); a centred model needs lookahead")
+            raise PwgbError(f"{name}: expected a ParallelWaveGANGenerator")
+        if causal and not model.use_causal_conv:
+            raise PwgbError(f"{name}: the model is not causal (use_causal_conv=False); a centred model needs lookahead")
+        if not causal and model.use_causal_conv:
+            raise PwgbError(f"{name}: the model is causal (use_causal_conv=True); stream it with CausalPWGStream, which has no "
+                            "lookahead")
         up = model.upsample_net
         if up is None:
-            raise PwgbError("CausalPWGStream: upsample_conditional_features=False is not supported")
+            raise PwgbError(f"{name}: upsample_conditional_features=False is not supported")
         if isinstance(up, MelGANGenerator):
-            raise PwgbError("CausalPWGStream: upsample_net='MelGANGenerator' is not supported")
+            raise PwgbError(f"{name}: upsample_net='MelGANGenerator' is not supported")
         if isinstance(up, UpsampleNetwork) and model.aux_context_window:
-            raise PwgbError("CausalPWGStream: UpsampleNetwork with aux_context_window > 0 has no whole-utterance inference to match")
+            raise PwgbError(f"{name}: UpsampleNetwork with aux_context_window > 0 has no whole-utterance inference to match")
         conv_in = up.conv_in if isinstance(up, ConvInUpsampleNetwork) else None
+        self.acw = model.aux_context_window if conv_in is not None else 0
         self.A = model.aux_channels
-        # ReplicationPad1d of inference: a fresh slot's conv_in history is its first frame
-        self._setup(model, batch, use_graphs, self.A, model.aux_context_window if conv_in is not None else 0, "replicate")
+        # ReplicationPad1d of inference: a fresh slot's conv_in history is its first frame; the centred conv_in reads acw
+        # frames on either side
+        self._setup(model, batch, use_graphs, self.A, self.acw if causal else 2 * self.acw, "replicate")
         fir_net = up.upsample if conv_in is not None else up
         self.scales = list(fir_net.upsample_scales)
         self.w_in = wb(conv_in)[0] if conv_in is not None else None
@@ -252,8 +273,8 @@ class CausalPWGStream(_ChunkStream):
         self.S = l0.conv1x1_skip.out_channels
         self.dmax = max(f.dilation for f in model.conv_layers)
         self.H = [(self.K - 1) * f.dilation for f in model.conv_layers]
-        if not ops.WnStack.supported(self.B, self.hop, self.R, self.G, self.S, self.A, self.K, self.dmax, True):
-            raise PwgbError("CausalPWGStream: the fused packed WaveNet stack does not support this configuration "
+        if not ops.WnStack.supported(self.B, self.hop, self.R, self.G, self.S, self.A, self.K, self.dmax, causal):
+            raise PwgbError(f"{name}: the fused packed WaveNet stack does not support this configuration "
                             f"(residual {self.R}, gate {self.G}, skip {self.S}, aux {self.A} channels, kernel {self.K})")
         self.w_first = wb(model.first_conv)
         # the output head as in ParallelWaveGANGenerator.forward: sqrt(1/layers) folded into the first 1x1 conv
@@ -265,6 +286,39 @@ class CausalPWGStream(_ChunkStream):
         self.gen = torch.Generator(device=dev)
         if seed is not None:
             self.gen.manual_seed(int(seed))
+
+    def _noise(self, z, T):
+        """z: (B, in_channels, T) noise on the device, drawn from the stream's generator when None"""
+        shape = (self.B, self.model.in_channels, T)
+        if z is None:
+            return torch.randn(shape, device=self.dev, generator=self.gen)
+        z = torch.as_tensor(z, dtype=torch.float32, device=self.dev)
+        if tuple(z.shape) != shape:
+            raise PwgbError(f"{type(self).__name__}.push: z must be {shape}, got {tuple(z.shape)}")
+        return z.contiguous()
+
+    @torch.no_grad()
+    def push(self, c, z=None, normalize_before=False):
+        """c: (B, n, aux) mel frames ((n, aux) when batch == 1); z: optional (B, in_channels, n * hop) noise of those
+        frames, drawn from the stream's generator when omitted.  Returns (B, out_channels, n * hop) on the device: the
+        frames' samples (causal), or samples [t0 * hop - delay, (t0 + n) * hop - delay) of each slot's utterance (with
+        lookahead; t0: the frames pushed before)."""
+        c = self._frames(c, normalize_before)
+        z = self._noise(z, c.shape[-1] * self.hop)
+        self._start(c)
+        return self._run(c.shape[-1], z, c)
+
+
+class CausalPWGStream(_PWGStream):
+    """Streams a causal ``ParallelWaveGANGenerator`` chunk by chunk for ``batch`` independent slots.
+
+    ``push(c, z)`` takes the next n >= 1 frames of every slot and returns their n * hop samples; n may change from
+    push to push.  For every slot, the concatenated outputs equal ``model.inference(c=all_frames, x=all_noise)``.
+    There is no lookahead and no flush.  With ``use_graphs`` each chunk length is captured once into a CUDA graph and
+    replayed.  The weights are read when the stream is built and must not change while it is used."""
+
+    def __init__(self, model, batch=1, seed=None, use_graphs=True):
+        self._build(model, batch, use_graphs, seed, causal=True)
 
     def _state(self):
         return [self.cin_hist] + self.fir_hist + self.wn_hist
@@ -317,25 +371,8 @@ class CausalPWGStream(_ChunkStream):
         # into a fresh tensor, as in inference: given out=, a wide few-channel output conv would not take _conv1d_fewcout
         return ops.conv1d(h, *self.w_l3, pre_slope=0.0)
 
-    @torch.no_grad()
-    def push(self, c, z=None, normalize_before=False):
-        """c: (B, n, aux) mel frames ((n, aux) when batch == 1); z: optional (B, in_channels, n * hop) noise, drawn from
-        the stream's generator when omitted.  Returns (B, out_channels, n * hop) on the device."""
-        m = self.model
-        c = self._frames(c, normalize_before)
-        T = c.shape[-1] * self.hop
-        if z is None:
-            z = torch.randn((self.B, m.in_channels, T), device=self.dev, generator=self.gen)
-        else:
-            z = torch.as_tensor(z, dtype=torch.float32, device=self.dev)
-            if tuple(z.shape) != (self.B, m.in_channels, T):
-                raise PwgbError(f"CausalPWGStream.push: z must be ({self.B}, {m.in_channels}, {T}), got {tuple(z.shape)}")
-            z = z.contiguous()
-        self._start(c)
-        return self._run(c.shape[-1], z, c)
 
-
-class PWGLookaheadStream(_Lookahead, _ChunkStream):
+class PWGLookaheadStream(_Lookahead, _PWGStream):
     """Streams a centred ``ParallelWaveGANGenerator`` (``use_causal_conv=False``, the published checkpoints) chunk by chunk
     for ``batch`` independent slots, with a fixed lookahead of ``delay`` output samples.
 
@@ -366,41 +403,10 @@ class PWGLookaheadStream(_Lookahead, _ChunkStream):
     is built and must not change while it is used."""
 
     def __init__(self, model, batch=1, seed=None, use_graphs=True):
-        from .models import MelGANGenerator, ParallelWaveGANGenerator
-
-        if not isinstance(model, ParallelWaveGANGenerator):
-            raise PwgbError("PWGLookaheadStream: expected a ParallelWaveGANGenerator")
-        if model.use_causal_conv:
-            raise PwgbError("PWGLookaheadStream: the model is causal (use_causal_conv=True); stream it with CausalPWGStream, "
-                            "which has no lookahead")
-        up = model.upsample_net
-        if up is None:
-            raise PwgbError("PWGLookaheadStream: upsample_conditional_features=False is not supported")
-        if isinstance(up, MelGANGenerator):
-            raise PwgbError("PWGLookaheadStream: upsample_net='MelGANGenerator' is not supported")
-        if isinstance(up, UpsampleNetwork) and model.aux_context_window:
-            raise PwgbError("PWGLookaheadStream: UpsampleNetwork with aux_context_window > 0 has no whole-utterance inference to match")
-        conv_in = up.conv_in if isinstance(up, ConvInUpsampleNetwork) else None
-        acw = model.aux_context_window if conv_in is not None else 0
-        self.A = model.aux_channels
-        # ReplicationPad1d of inference: a fresh slot's conv_in history is its first frame
-        self._setup(model, batch, use_graphs, self.A, 2 * acw, "replicate")
-        fir_net = up.upsample if conv_in is not None else up
-        self.scales = list(fir_net.upsample_scales)
-        self.w_in = wb(conv_in)[0] if conv_in is not None else None
-        self.firs = [wb(fir_net.up_layers[2 * i + 1])[0] for i in range(len(self.scales))]
-        self.hop = model.upsample_factor
-        l0 = model.conv_layers[0]
-        self.R, self.G, self.K = l0.conv.in_channels, l0.conv.out_channels, l0.conv.kernel_size[0]
-        self.S = l0.conv1x1_skip.out_channels
-        self.dmax = max(f.dilation for f in model.conv_layers)
-        self.H = [(self.K - 1) * f.dilation for f in model.conv_layers]
-        if not ops.WnStack.supported(self.B, self.hop, self.R, self.G, self.S, self.A, self.K, self.dmax, False):
-            raise PwgbError("PWGLookaheadStream: the fused packed WaveNet stack does not support this configuration "
-                            f"(residual {self.R}, gate {self.G}, skip {self.S}, aux {self.A} channels, kernel {self.K})")
+        self._build(model, batch, use_graphs, seed, causal=False)
         # the plan: lookaheads of conv_in (frames), of each FIR stage's output, of first_conv's output and of each layer's
-        look, self.looks = acw, []
-        self.look_in = acw
+        look, self.looks = self.acw, []
+        self.look_in = self.acw
         for s in self.scales:
             look = look * s + s
             self.looks.append(look)
@@ -413,21 +419,11 @@ class PWGLookaheadStream(_Lookahead, _ChunkStream):
         self.off = [self.look_x + d - self.look_c for d in self.D]  # conditioning rows behind the newest, per layer
         self.W = self.off[-1]
         self.delay = self.look_x + self.D[-1]
-        self.w_first = wb(model.first_conv)
-        # the output head as in ParallelWaveGANGenerator.forward: sqrt(1/layers) folded into the first 1x1 conv
-        w1, b1 = wb(model.last_conv_layers[1])
-        self.w_l1, self.w_l3 = (w1 * model._skip_scale, b1), wb(model.last_conv_layers[3])
-        dev, B, A = self.dev, self.B, self.A
-        self.fir_hist = [self._zeros(B, A, 2) for _ in self.scales]
+        B, A = self.B, self.A
         self.z_hist = self._zeros(B, model.in_channels, self.look_x)
         self.c_hist = self._zeros(B, A, self.W)
         self.skip_hist = self._zeros(B, self.S, self.W)
-        self.wn_hist = [torch.zeros((B, self.R * h), device=dev, dtype=torch.int32) for h in self.H]
         self._counters()
-        self._nohist = self._zeros(B, A, 0)
-        self.gen = torch.Generator(device=dev)
-        if seed is not None:
-            self.gen.manual_seed(int(seed))
 
     def _state(self):
         return [self.cin_hist] + self.fir_hist + [self.z_hist, self.c_hist, self.skip_hist] + self.wn_hist + [self.frame, self.end]
@@ -496,31 +492,13 @@ class PWGLookaheadStream(_Lookahead, _ChunkStream):
         return y
 
     @torch.no_grad()
-    def push(self, c, z=None, normalize_before=False):
-        """c: (B, n, aux) mel frames ((n, aux) when batch == 1); z: optional (B, in_channels, n * hop) noise of those
-        frames, drawn from the stream's generator when omitted.  Returns (B, out_channels, n * hop) on the device: samples
-        [t0 * hop - delay, (t0 + n) * hop - delay) of each slot's utterance."""
-        m = self.model
-        c = self._frames(c, normalize_before)
-        T = c.shape[-1] * self.hop
-        if z is None:
-            z = torch.randn((self.B, m.in_channels, T), device=self.dev, generator=self.gen)
-        else:
-            z = torch.as_tensor(z, dtype=torch.float32, device=self.dev)
-            if tuple(z.shape) != (self.B, m.in_channels, T):
-                raise PwgbError(f"PWGLookaheadStream.push: z must be ({self.B}, {m.in_channels}, {T}), got {tuple(z.shape)}")
-            z = z.contiguous()
-        self._start(c)
-        return self._run(c.shape[-1], z, c)
-
-    @torch.no_grad()
     def flush(self, items=None):
         """The last ``delay`` samples of slots ``items`` (an index, an iterable of indices or None for every slot), as
         (len(items), out_channels, delay); the slots are then reset.  The flush push repeats each slot's last frame (the
         right edge of ReplicationPad1d) with zero noise, and the end frames mask everything past the signal.  The other
         slots' state is restored around it, so they continue exactly as if it had not happened; ending one slot costs a
         ceil(delay / hop)-frame batch push (DESIGN.md §3.9)."""
-        n = -(-self.delay // self.hop)
+        n = self._flush_frames()
         P = self.cin_hist.shape[-1]
 
         def inputs():
@@ -705,6 +683,14 @@ class _HiFiGANStream(_ChunkStream):
         ops.stream_carry(ent["out_table"])
         return y
 
+    def _centred(self, ent, n):
+        """The centred generator of a lookahead stream on the entry's xin = [history | n frames], which its front end has
+        filled: the input conv, the levels and the output conv.  Advances the frame counter."""
+        h = ops.conv1d_stream(ent["xin"], self._nohist, *self.w_in, pad_left=0, out=ent["h0"], mask=self._mask(1, self.look_in))
+        y = self._output(self._levels(h, ent, None), ent)
+        self.frame += n
+        return y
+
 
 class CausalHiFiGANStream(_HiFiGANStream):
     """Streams a causal ``HiFiGANGenerator`` (``use_causal_conv=True``) chunk by chunk for ``batch`` independent slots.
@@ -787,19 +773,17 @@ class HiFiGANLookaheadStream(_Lookahead, _HiFiGANStream):
         self._setup(model, batch, use_graphs, ic.in_channels, ic.kernel_size[0] - 1, "zero")
         self._build(model, centred=True)
         self._counters()
-        self._nohist = self._zeros(self.B, ic.in_channels, 0)
 
     def _state(self):
         return self._histories() + [self.frame, self.end]
 
     def _step(self, c):
         """One chunk: c (B, in_channels, n) -> (B, out_channels, n * hop).  Advances the state."""
-        ent = self._entry(c.shape[-1])
-        # the centred input conv on [history | chunk]: frames t0 - 3 .. t0 + n - 4 for kernel 7
-        h = ops.conv1d_stream(self._input(ent, c), self._nohist, *self.w_in, pad_left=0, out=ent["h0"], mask=self._mask(1, self.look_in))
-        y = self._output(self._levels(h, ent, None), ent)
-        self.frame += c.shape[-1]
-        return y
+        n = c.shape[-1]
+        ent = self._entry(n)
+        # the centred input conv reads [history | chunk]: frames t0 - 3 .. t0 + n - 4 for kernel 7
+        self._input(ent, c)
+        return self._centred(ent, n)
 
     @torch.no_grad()
     def push(self, c, normalize_before=False):
@@ -815,7 +799,7 @@ class HiFiGANLookaheadStream(_Lookahead, _HiFiGANStream):
         against the zero right padding, as (len(items), out_channels, delay); the slots are then reset.  The other slots'
         state is restored around the flush push, so they continue exactly as if it had not happened.  The flush push covers
         every slot, so ending one slot costs a ceil(delay / hop)-frame batch push (DESIGN.md §3.8)."""
-        n = -(-self.delay // self.hop)
+        n = self._flush_frames()
         return self._flush(list(self._slots(items)), lambda: (n, self._zeros(self.B, self.in_channels, n)))
 
 
@@ -864,7 +848,6 @@ class DiscreteSymbolHiFiGANLookaheadStream(_Lookahead, _HiFiGANStream):
         self._setup(model, batch, use_graphs, ic.in_channels, ic.kernel_size[0] - 1, "zero", flags=self.use_spk)
         self._build(model, centred=True)
         self._counters()
-        self._nohist = self._zeros(self.B, ic.in_channels, 0)
         self.table = model.emb.weight.detach()
         self.spk_table = model.spk_emb.weight.detach() if self.use_spk else None
         # each slot's latched speaker row (-2: outside the speaker table); valid while the slot's fresh flag is clear
@@ -884,10 +867,7 @@ class DiscreteSymbolHiFiGANLookaheadStream(_Lookahead, _HiFiGANStream):
         ops.symbol_embed_stream(c, self.table, self.spk_table, self.latch, self.fresh, self._mask(1, 0), xin, P)
         if self.use_spk:
             self.fresh.zero_()
-        h = ops.conv1d_stream(xin, self._nohist, *self.w_in, pad_left=0, out=ent["h0"], mask=self._mask(1, self.look_in))
-        y = self._output(self._levels(h, ent, None), ent)
-        self.frame += n
-        return y
+        return self._centred(ent, n)
 
     def _ids(self, c):
         """(B, n[, K]) indices -> (B, K, n) contiguous on the device, int64 or float32"""
@@ -921,15 +901,9 @@ class DiscreteSymbolHiFiGANLookaheadStream(_Lookahead, _HiFiGANStream):
         against the zero right padding, as (len(items), out_channels, delay); the slots are then reset.  The flush push
         covers every slot with symbol 0 (the end mask stores the flushed slots' frames as +0.0); the other slots' state,
         speaker latch and fresh flag included, is restored around it."""
-        items = list(self._slots(items))
-        n = -(-self.delay // self.hop)
-        fresh = self.fresh.clone() if self.use_spk else None
+        n = self._flush_frames()
         ids = torch.zeros((self.B, 2 if self.use_spk else 1, n), device=self.dev, dtype=torch.int64)
-        y = self._flush(items, lambda: (n, ids))
-        if self.use_spk:
-            keep = [b for b in range(self.B) if b not in items]
-            self.fresh[keep] = fresh[keep]
-        return y
+        return self._flush(list(self._slots(items)), lambda: (n, ids))
 
 
 class DiscreteSymbolDurationLookaheadStream(_Lookahead, _HiFiGANStream):
@@ -977,7 +951,6 @@ class DiscreteSymbolDurationLookaheadStream(_Lookahead, _HiFiGANStream):
         self._setup(model, batch, use_graphs, ic.in_channels, ic.kernel_size[0] - 1, "zero")
         self._build(model, centred=True)
         self._counters()
-        self._nohist = self._zeros(self.B, ic.in_channels, 0)
         self.table = model.emb.weight.detach()
         dp = model.duration_predictor
         self.offset = float(dp.offset)
@@ -1061,10 +1034,7 @@ class DiscreteSymbolDurationLookaheadStream(_Lookahead, _HiFiGANStream):
         P = self.cin_hist.shape[-1]
         xin[:, :, :P].copy_(self.cin_hist)
         ops.symbol_regulate_stream(self.table, self.queue, self._mask(1, 0), xin, P, n)
-        h = ops.conv1d_stream(xin, self._nohist, *self.w_in, pad_left=0, out=ent["h0"], mask=self._mask(1, self.look_in))
-        y = self._output(self._levels(h, ent, None), ent)
-        self.frame += n
-        return y
+        return self._centred(ent, n)
 
     def _body(self, n):
         """n frames in power-of-two pushes, largest first"""
@@ -1100,25 +1070,22 @@ class DiscreteSymbolDurationLookaheadStream(_Lookahead, _HiFiGANStream):
         restored around it; ``last_durations`` then holds the durations the flush finalised."""
         items = list(self._slots(items))
         outs, last = [], [torch.zeros(0, dtype=torch.int64) for _ in range(self.B)]
+        n = self._flush_frames()
         for b in items:
-            keep = [i for i in range(self.B) if i != b]
-            snap = [t[keep].clone() for t in self._state()]
-            self.send[b] = self.sframe[b]
-            if self.P:
-                self._predict(torch.zeros((self.B, 1, self.P), device=self.dev, dtype=torch.int64))
-                last[b] = self.last_durations[b]
-            zr = torch.zeros(self.B, device=self.dev, dtype=torch.int32)
-            zr[b] = 1
-            ops.duration_queue_append(self.queue, None, None, (self.frame, self.end), 0, self.offset, zero_rule=zr)
-            ys = [self._body(int(self._queued([b])[b]))]
-            self.end[b] = self.frame[b]
-            n = -(-self.delay // self.hop)
-            if n not in self._len:
-                self._len[n] = torch.empty(n, device=self.dev)
-            ys.append(self._run(n, self._len[n])[:, :, :self.delay])
-            outs.append(torch.cat(ys, -1)[b])
-            for t, sn in zip(self._state(), snap):
-                t[keep] = sn
+            with self._keeping_others([b]):
+                self.send[b] = self.sframe[b]
+                if self.P:
+                    self._predict(torch.zeros((self.B, 1, self.P), device=self.dev, dtype=torch.int64))
+                    last[b] = self.last_durations[b]
+                zr = torch.zeros(self.B, device=self.dev, dtype=torch.int32)
+                zr[b] = 1
+                ops.duration_queue_append(self.queue, None, None, (self.frame, self.end), 0, self.offset, zero_rule=zr)
+                ys = [self._body(int(self._queued([b])[b]))]
+                self.end[b] = self.frame[b]
+                if n not in self._len:
+                    self._len[n] = torch.empty(n, device=self.dev)
+                ys.append(self._run(n, self._len[n])[:, :, :self.delay])
+                outs.append(torch.cat(ys, -1)[b])
             self.reset(b)
         self._last_flush = last
         return outs
@@ -1481,7 +1448,7 @@ class MelGANLookaheadStream(_Lookahead, _MelGANStream):
         if short:
             raise PwgbError(f"MelGANLookaheadStream.flush: slots {short} hold fewer than {self.min_frames} frames "
                             f"({[self._count[b] for b in short]}); inference needs that many for the reflect padding")
-        n = -(-self.delay // (self.hop * self.subbands))
+        n = self._flush_frames()
         return self._flush(items, lambda: (n, self._zeros(self.B, self.in_channels, n)))
 
 
@@ -1729,7 +1696,7 @@ class VQVAELookaheadStream(MelGANLookaheadStream):
         if short:
             raise PwgbError(f"VQVAELookaheadStream.flush: slots {short} hold fewer than {self.min_frames} frames "
                             f"({[self._count[b] for b in short]}); decode needs that many for the reflect padding")
-        n = -(-self.delay // self.hop)
+        n = self._flush_frames()
         l_ch = self.l_in if self.local else 0
 
         def inputs():
@@ -1856,7 +1823,6 @@ class UHiFiGANLookaheadStream(_Lookahead, _HiFiGANStream):
         self.out_channels = oc.out_channels
         self.delay = look_h + pk
         self._counters()
-        self._nohist = self._zeros(B, hc.in_channels, 0)
 
     def _state(self):
         hs = [self.cin_hist, self.out_hist, self.e_hist]
@@ -1957,6 +1923,6 @@ class UHiFiGANLookaheadStream(_Lookahead, _HiFiGANStream):
         against the zero right padding, as (len(items), out_channels, delay); the slots are then reset.  The flush push
         covers ceil(delay / hop) zero frames and zero excitation with the slots' end frames set; the other slots' state is
         restored around it, so they continue exactly as if it had not happened (DESIGN.md §3.11)."""
-        n = -(-self.delay // self.hop)
+        n = self._flush_frames()
         return self._flush(list(self._slots(items)),
                            lambda: (n, self._zeros(self.B, self.in_channels, n), self._zeros(self.B, 1, n * self.hop)))

@@ -4,7 +4,6 @@ their latch, the end mask, NaN columns), streamed audio followed by the flush is
 inference] for every chunk schedule while the output conv stays on one kernel, slots with different speakers are
 independent across a reset and a partial flush, graphs replay what eager runs compute, and the unsupported models
 raise."""
-import ctypes as C
 import json
 
 import pytest
@@ -12,6 +11,7 @@ import torch
 
 from helpers import REL_TOL, golden_weights, load_golden, rel_l2
 from oracle import synth
+from stream_harness import dev, debug_get  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -22,15 +22,6 @@ SYN24 = dict(in_channels=32, out_channels=1, channels=64, num_embs=50, num_spk_e
              resblock_dilations=[[1, 3, 5]] * 3)
 # whole utterances below 4096 output samples keep the output conv on the generic FFMA kernel on both sides
 FRAMES = {"dsym_small": 12, "dsym_vctk": 12, "syn24": 8}
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    import __graft_entry__
-
-    __graft_entry__.build()
-    return torch.device("cuda:0")
 
 
 def _model(dev, name, weight_norm=True):
@@ -76,14 +67,6 @@ def _expected(m, c, delay):
     with torch.no_grad():
         y = torch.stack([m.inference(c[b].reshape(c.shape[1], -1).to(d)).t() for b in range(c.shape[0])])
     return torch.cat([y.new_zeros(y.shape[:-1] + (delay,)), y], -1)
-
-
-def _debug(key, n):
-    from parallelwavegan_b200 import capi
-
-    v = (C.c_int * n)()
-    assert capi.lib().pwgb_debug_get(key, C.cast(v, C.c_void_p), C.sizeof(v)) == 0
-    return list(v)
 
 
 # ---------------------------------------------------------------------------------------------------- kernel
@@ -153,9 +136,9 @@ def test_stream_equals_inference(dev, name, weight_norm, schedule):
     c = _units(m, 2, FRAMES[name], 71)
     st = DiscreteSymbolHiFiGANLookaheadStream(m, batch=2)
     ref = _expected(m, c, st.delay)
-    assert _debug(3, 6)[0] == 0  # the output conv of the whole utterance took the generic kernel
+    assert debug_get(3, 6)[0] == 0  # the output conv of the whole utterance took the generic kernel
     y = _stream(st, c, SCHEDULES[schedule])
-    assert _debug(3, 6)[0] == 0  # and so did the stream's
+    assert debug_get(3, 6)[0] == 0  # and so did the stream's
     assert torch.equal(y, ref)
 
 
@@ -213,7 +196,7 @@ def test_long_utterance_within_rel_l2(dev):
     c = _units(m, 2, 40, 73)
     st = DiscreteSymbolHiFiGANLookaheadStream(m, batch=2)
     ref = _expected(m, c, st.delay)
-    assert _debug(3, 6)[0] == 2
+    assert debug_get(3, 6)[0] == 2
     y = _stream(st, c, SCHEDULES["mixed"])
     assert rel_l2(y.cpu(), ref.cpu()) <= 1e-6
 

@@ -3,7 +3,6 @@ conv entry points (mask, delayed residual, delayed read) and the masked conv-tra
 entry points on the explicit signal, streamed audio followed by the flush is bit-identical to
 [zeros(delay) | inference] for every chunk schedule, slots are independent (also across a flush), graphs replay what
 eager runs compute, and the unsupported models raise."""
-import ctypes as C
 import json
 
 import pytest
@@ -11,7 +10,7 @@ import torch
 
 from helpers import REL_TOL, golden_weights, load_golden, rel_l2
 from oracle import synth
-from test_gpu_hifigan_stream import KCASES
+from stream_harness import dev, debug_get, KCASES, mels  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -23,15 +22,6 @@ V1 = dict(in_channels=80, out_channels=1, channels=512, kernel_size=7, upsample_
 # whole utterances up to 15 frames: the output conv takes the generic FFMA kernel on both sides (DESIGN.md)
 FRAMES = 15
 GOLDEN = ["hifigan_small", "hifigan_odd", "hifigan_v1"]
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    import __graft_entry__
-
-    __graft_entry__.build()
-    return torch.device("cuda:0")
 
 
 def _golden(dev, name, weight_norm=True):
@@ -75,18 +65,6 @@ def _expected(m, c, delay):
     with torch.no_grad():
         y = torch.stack([m.inference(c[b].to(d)).t() for b in range(c.shape[0])])
     return torch.cat([y.new_zeros(y.shape[:-1] + (delay,)), y], -1)
-
-
-def _debug(key, n):
-    from parallelwavegan_b200 import capi
-
-    v = (C.c_int * n)()
-    assert capi.lib().pwgb_debug_get(key, C.cast(v, C.c_void_p), C.sizeof(v)) == 0
-    return list(v)
-
-
-def _mels(B, T, seed):
-    return synth.randn((B, T, 80), seed)
 
 
 # ---------------------------------------------------------------------------------------------------- kernels
@@ -141,10 +119,10 @@ def test_conv_stream_ext_bit_exact(dev, name):
                 y = ops.conv1d_stream(x, hist, w, b, pad_left=pl + delta, dilation=d, replicate=repl, t_out=t_out,
                                       mask=(frame, end, rate, look), **res, **kw, **extra)
                 if engine == "tc":
-                    p = _debug(1, 8)
+                    p = debug_get(1, 8)
                     assert p[5] == 0 and p[4] == 0, p  # no TMA activation rows, the register epilogue
                 else:
-                    assert _debug(3, 6)[0] == 0
+                    assert debug_get(3, 6)[0] == 0
             else:
                 # the explicit conv computes delta more rows; the residual and the accumulated output are padded to them
                 pad = lambda t: torch.nn.functional.pad(t, (0, delta))  # noqa: E731
@@ -207,12 +185,12 @@ def test_stream_equals_inference(dev, name, weight_norm, schedule):
     from parallelwavegan_b200.streaming import HiFiGANLookaheadStream
 
     m = _model(dev, name, weight_norm)
-    c = _mels(2, FRAMES, 61)
+    c = mels(2, FRAMES, 61)
     st = HiFiGANLookaheadStream(m, batch=2)
     ref = _expected(m, c, st.delay)
-    assert _debug(3, 6)[0] == 0  # the output conv of the whole utterance took the generic kernel
+    assert debug_get(3, 6)[0] == 0  # the output conv of the whole utterance took the generic kernel
     y = _stream(st, c, SCHEDULES[schedule])
-    assert _debug(3, 6)[0] == 0  # and so did the stream's (the flush's, the last FFMA launch)
+    assert debug_get(3, 6)[0] == 0  # and so did the stream's (the flush's, the last FFMA launch)
     assert torch.equal(y, ref)
 
 
@@ -222,7 +200,7 @@ def test_short_utterances_come_from_the_flush(dev, name, frames):
     from parallelwavegan_b200.streaming import HiFiGANLookaheadStream
 
     m = _model(dev, name)
-    c = _mels(2, frames, 62)
+    c = mels(2, frames, 62)
     st = HiFiGANLookaheadStream(m, batch=2)
     assert frames * st.hop < st.delay
     assert torch.equal(_stream(st, c, [1]), _expected(m, c, st.delay))
@@ -257,10 +235,10 @@ def test_long_utterance_within_rel_l2(dev):
     from parallelwavegan_b200.streaming import HiFiGANLookaheadStream
 
     m = _model(dev, "hifigan_small")
-    c = _mels(2, 48, 63)
+    c = mels(2, 48, 63)
     st = HiFiGANLookaheadStream(m, batch=2)
     ref = _expected(m, c, st.delay)
-    assert _debug(3, 6)[0] == 2
+    assert debug_get(3, 6)[0] == 2
     y = _stream(st, c, SCHEDULES["mixed"])
     assert rel_l2(y.cpu(), ref.cpu()) <= 1e-6
 
@@ -271,7 +249,7 @@ def test_batch_slots_reset_flush_and_graphs(dev):
     from parallelwavegan_b200.streaming import HiFiGANLookaheadStream
 
     m = _model(dev, "v1_512")
-    c = _mels(4, FRAMES, 64)
+    c = mels(4, FRAMES, 64)
     y4 = _stream(HiFiGANLookaheadStream(m, batch=4), c, SCHEDULES["mixed"])
     for b in range(4):
         assert torch.equal(y4[b:b + 1], _stream(HiFiGANLookaheadStream(m, batch=1), c[b:b + 1], SCHEDULES["mixed"]))
@@ -280,7 +258,7 @@ def test_batch_slots_reset_flush_and_graphs(dev):
     st = HiFiGANLookaheadStream(m, batch=4)
     first = _stream(st, c[:, :6], [2, 4], flush=False)
     c2 = c.clone()
-    c2[1, 6:] = _mels(1, FRAMES - 6, 65)[0]
+    c2[1, 6:] = mels(1, FRAMES - 6, 65)[0]
     st.reset(1)
     rest = _stream(st, c2[:, 6:], [1, 3, 5])
     y = torch.cat([first, rest], -1)
@@ -308,15 +286,8 @@ def test_more_chunk_lengths_than_cached(dev):
     m = _model(dev, "hifigan_odd")
     st = HiFiGANLookaheadStream(m, batch=2)
     sched = list(range(1, st.MAX_CHUNK_LENGTHS + 3))
-    c = _mels(2, sum(sched), 66)
+    c = mels(2, sum(sched), 66)
     assert torch.equal(_stream(st, c, sched), _expected(m, c, st.delay))
-
-
-def test_state_bytes(dev):
-    from parallelwavegan_b200.streaming import HiFiGANLookaheadStream
-
-    st = HiFiGANLookaheadStream(_model(dev, "hifigan_small"), batch=3)
-    assert st.state_bytes() == sum(t[0].numel() * t.element_size() for t in st._state())
 
 
 def test_unsupported_models_raise(dev):

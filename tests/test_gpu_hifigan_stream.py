@@ -2,7 +2,6 @@
 points, the causal conv-transpose entry and the carry are bit-identical to the existing entry points on the
 concatenated signal, streamed audio is bit-identical to ``inference`` on the whole utterance for every chunk schedule,
 slots are independent, graphs replay what eager runs compute, and the unsupported models raise."""
-import ctypes as C
 import json
 
 import pytest
@@ -10,6 +9,7 @@ import torch
 
 from helpers import REL_TOL, golden_weights, load_golden, rel_l2
 from oracle import synth
+from stream_harness import dev, debug_get, KCASES, mels  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -21,15 +21,6 @@ V1 = dict(in_channels=80, out_channels=1, channels=512, kernel_size=7, upsample_
           use_causal_conv=True)
 # whole utterances up to 15 frames: every few-channel conv takes the generic FFMA kernel on both sides (DESIGN.md)
 FRAMES = 15
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    import __graft_entry__
-
-    __graft_entry__.build()
-    return torch.device("cuda:0")
 
 
 def _golden(dev, weight_norm=True):
@@ -70,32 +61,7 @@ def _inference(m, c):
         return torch.stack([m.inference(c[b].to(d)).t() for b in range(c.shape[0])])
 
 
-def _debug(key, n):
-    from parallelwavegan_b200 import capi
-
-    v = (C.c_int * n)()
-    assert capi.lib().pwgb_debug_get(key, C.cast(v, C.c_void_p), C.sizeof(v)) == 0
-    return list(v)
-
-
-def _mels(B, T, seed):
-    return synth.randn((B, T, 80), seed)
-
-
 # ---------------------------------------------------------------------------------------------------- kernels
-# name: B, cin, cout, K, dilation, n, H, pad_left, replicate flags, epilogue, engine, expected plan
-#   plan (tensor cores, pwgb_debug_get(1)): "cp" cp.async-staged, "direct" register path, "win" win_mode, "nco" column chunks
-KCASES = {
-    "tc_cp_h_eq_pad": (2, 64, 64, 3, 2, 300, 4, 4, None, "plain", "tc", "cp"),
-    "tc_cp_h_lt_pad_rep": (3, 32, 48, 7, 1, 200, 3, 6, [1, 0, 1], "res", "tc", "cp"),
-    "tc_direct_n_lt_h": (2, 32, 32, 3, 176, 100, 352, 352, [0, 1], "acc", "tc", "direct"),
-    "tc_win": (1, 32, 32, 3, 1100, 500, 2200, 2200, None, "plain", "tc", "win"),
-    "tc_nco_staged": (3, 32, 256, 11, 5, 700, 50, 50, [1, 0, 0], "res", "tc", "nco"),
-    "ffma_h_eq_pad": (2, 16, 8, 3, 3, 257, 6, 6, [0, 1], "plain", "simt", None),
-    "ffma_h_lt_pad": (3, 8, 2, 7, 1, 90, 4, 6, [1, 0, 1], "res", "simt", None),
-    "ffma_n_lt_h": (2, 4, 16, 11, 5, 20, 50, 50, None, "acc", "simt", None),
-    "ffma_tanh": (3, 32, 1, 7, 1, 3000, 6, 6, [0, 1, 1], "tanh", "simt", None),
-}
 
 
 @pytest.mark.parametrize("name", list(KCASES))
@@ -132,15 +98,15 @@ def test_conv_stream_bit_exact(dev, name):
             if stream:
                 y = ops.conv1d_stream(x, hist, w, b, pad_left=pl, dilation=d, replicate=repl, **kw, **extra)
                 if engine == "tc":
-                    p = _debug(1, 8)
+                    p = debug_get(1, 8)
                     assert p[5] == 0, p  # no TMA activation rows in a history launch
                     assert {"cp": p[3] > 0 and not p[6], "direct": p[3] == 0, "win": p[6] == 1, "nco": p[7] > 1}[plan], p
                 else:
-                    assert _debug(3, 6)[0] == 0
+                    assert debug_get(3, 6)[0] == 0
             else:
                 y = ops.conv1d_raw(xc, w, b, dilation=d, padding=(pl - H, 0), **kw, **extra)
                 if engine == "simt":
-                    assert _debug(3, 6)[0] == 0
+                    assert debug_get(3, 6)[0] == 0
             outs.append(y)
     finally:
         ops.ENGINE = old
@@ -189,7 +155,7 @@ def test_golden_stream_equals_inference(dev, weight_norm, schedule):
     meta, _, m = _golden(dev, weight_norm)
     c = synth.randn(meta["c_shape"], meta["c_seed"]).transpose(1, 2)[:, :FRAMES].contiguous()
     ref = _inference(m, c)
-    assert _debug(3, 6)[0] == 0  # the output conv of the whole utterance took the generic kernel
+    assert debug_get(3, 6)[0] == 0  # the output conv of the whole utterance took the generic kernel
     y = _stream(CausalHiFiGANStream(m, batch=c.shape[0]), c, SCHEDULES[schedule])
     assert torch.equal(y, ref)
 
@@ -209,7 +175,7 @@ def test_long_utterance_within_rel_l2(dev):
     from parallelwavegan_b200.streaming import CausalHiFiGANStream
 
     _, _, m = _golden(dev)
-    c = _mels(2, 48, 31)
+    c = mels(2, 48, 31)
     ref = _inference(m, c)
     y = _stream(CausalHiFiGANStream(m, batch=2), c, SCHEDULES["mixed"])
     assert rel_l2(y.cpu(), ref.cpu()) <= 1e-6
@@ -221,7 +187,7 @@ def test_v1_stream_equals_inference(dev, variant, schedule):
     from parallelwavegan_b200.streaming import CausalHiFiGANStream
 
     m = _v1(dev, weight_norm=variant == "wn", **({"use_additional_convs": False} if variant == "no_additional_convs" else {}))
-    c = _mels(1, FRAMES, 41)
+    c = mels(1, FRAMES, 41)
     ref = _inference(m, c)
     y = _stream(CausalHiFiGANStream(m), c, SCHEDULES[schedule])
     assert torch.equal(y, ref)
@@ -233,7 +199,7 @@ def test_batch_slots_reset_and_graphs(dev):
     from parallelwavegan_b200.streaming import CausalHiFiGANStream
 
     m = _v1(dev)
-    c = _mels(4, FRAMES, 51)
+    c = mels(4, FRAMES, 51)
     y4 = _stream(CausalHiFiGANStream(m, batch=4), c, SCHEDULES["mixed"])
     for b in range(4):
         assert torch.equal(y4[b:b + 1], _stream(CausalHiFiGANStream(m, batch=1), c[b:b + 1], SCHEDULES["mixed"]))
@@ -242,7 +208,7 @@ def test_batch_slots_reset_and_graphs(dev):
     st = CausalHiFiGANStream(m, batch=4)
     first = _stream(st, c[:, :6], [2, 4])
     c2 = c.clone()
-    c2[1, 6:] = _mels(1, FRAMES - 6, 52)[0]
+    c2[1, 6:] = mels(1, FRAMES - 6, 52)[0]
     st.reset(1)
     rest = _stream(st, c2[:, 6:], [1, 3, 5])
     y = torch.cat([first, rest], -1)

@@ -3,7 +3,6 @@ history convs with the reflect / replicate edge policy are bit-identical to the 
 engines and every tensor-core plan, streamed audio followed by the flush is bit-identical to [zeros(delay) | inference]
 for every chunk schedule and pad, slots are independent (also across a flush), graphs replay what eager runs compute,
 and the unsupported models and too-short flushes raise."""
-import ctypes as C
 import json
 
 import pytest
@@ -11,6 +10,7 @@ import torch
 
 from helpers import REL_TOL, golden_weights, load_golden, rel_l2
 from oracle import synth
+from stream_harness import dev, debug_get, mels  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -23,15 +23,6 @@ MB2_CSMSC = dict(MB2, upsample_scales=[5, 5, 3])
 # below the length from which the whole utterance's output conv takes conv1d_fewcout_long_kernel (4096 samples)
 FRAMES = {"v1": 15, "mb2": 63, "mb2_csmsc": 54}
 GOLDEN = ["melgan_small", "melgan_centred_replicate", "melgan_centred_zero", "mb_melgan_v2", "melgan_centred_mb"]
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    import __graft_entry__
-
-    __graft_entry__.build()
-    return torch.device("cuda:0")
 
 
 def _golden(dev, name, weight_norm=True):
@@ -82,18 +73,6 @@ def _expected(m, c, delay):
     with torch.no_grad():
         y = torch.stack([m.inference(c[b].to(d)).t() for b in range(c.shape[0])])
     return torch.cat([y.new_zeros(y.shape[:-1] + (delay,)), y], -1)
-
-
-def _debug(key, n):
-    from parallelwavegan_b200 import capi
-
-    v = (C.c_int * n)()
-    assert capi.lib().pwgb_debug_get(key, C.cast(v, C.c_void_p), C.sizeof(v)) == 0
-    return list(v)
-
-
-def _mels(B, T, seed):
-    return synth.randn((B, T, 80), seed)
 
 
 # ---------------------------------------------------------------------------------------------------- kernels
@@ -151,10 +130,10 @@ def test_conv_stream_edge_bit_exact(dev, name, pad):
         y = ops.conv1d_stream(x, hist, w, bias, pad_left=H, dilation=d, mask=(frame, end, rate, look_out), edge=pad,
                               in_lookahead=look_in, **res, **kw)
         if engine == "tc":
-            pl = _debug(1, 8)
+            pl = debug_get(1, 8)
             assert pl[5] == 0 and {"cp": pl[3] > 0 and not pl[6], "direct": pl[3] == 0, "win": pl[6] == 1, "nco": pl[7] > 1}[plan], pl
         else:
-            assert _debug(3, 6)[0] == 0
+            assert debug_get(3, 6)[0] == 0
         ref = torch.zeros(B, cout, n)
         for b in range(B):
             o = frames[b] * rate - look_out + torch.arange(n)
@@ -193,7 +172,7 @@ def test_golden_stream_equals_inference(dev, name, weight_norm, schedule):
     from parallelwavegan_b200.streaming import MelGANLookaheadStream
 
     meta, _, m = _golden(dev, name, weight_norm)
-    c = _mels(2, 13, 71)
+    c = mels(2, 13, 71)
     st = MelGANLookaheadStream(m, batch=2)
     ref = _expected(m, c, st.delay)
     y = _stream(st, c, SCHEDULES[schedule])
@@ -208,11 +187,11 @@ def test_stream_equals_inference(dev, kind, pad, schedule):
     from parallelwavegan_b200.streaming import MelGANLookaheadStream
 
     m = _synthetic(dev, kind, pad=pad)
-    c = _mels(1, FRAMES[kind], 72)
+    c = mels(1, FRAMES[kind], 72)
     st = MelGANLookaheadStream(m)
     ref = _expected(m, c, st.delay)
     if kind == "v1":
-        assert _debug(3, 6)[0] == 0  # the output conv of the whole utterance took the generic kernel
+        assert debug_get(3, 6)[0] == 0  # the output conv of the whole utterance took the generic kernel
     assert torch.equal(_stream(st, c, SCHEDULES[schedule]), ref)
 
 
@@ -221,7 +200,7 @@ def test_stream_without_weight_norm(dev, kind):
     from parallelwavegan_b200.streaming import MelGANLookaheadStream
 
     m = _synthetic(dev, kind, weight_norm=False)
-    c = _mels(2, 11, 73)
+    c = mels(2, 11, 73)
     st = MelGANLookaheadStream(m, batch=2)
     assert torch.equal(_stream(st, c, SCHEDULES["mixed"]), _expected(m, c, st.delay))
 
@@ -234,7 +213,7 @@ def test_shortest_utterances_come_from_the_flush(dev, kind, pad):
     m = _synthetic(dev, kind, pad=pad)
     st = MelGANLookaheadStream(m, batch=2)
     assert st.min_frames == ({"v1": 4, "mb2": 4, "mb2_csmsc": 6}[kind] if pad == "reflect" else 1)
-    c = _mels(2, st.min_frames, 74)
+    c = mels(2, st.min_frames, 74)
     for schedule in (SCHEDULES["ones"], SCHEDULES["long"]):
         assert torch.equal(_stream(st, c, schedule), _expected(m, c, st.delay))
 
@@ -264,10 +243,10 @@ def test_long_utterance_within_rel_l2(dev):
     from parallelwavegan_b200.streaming import MelGANLookaheadStream
 
     m = _synthetic(dev, "v1")
-    c = _mels(1, 48, 75)
+    c = mels(1, 48, 75)
     st = MelGANLookaheadStream(m)
     ref = _expected(m, c, st.delay)
-    assert _debug(3, 6)[0] == 2
+    assert debug_get(3, 6)[0] == 2
     assert rel_l2(_stream(st, c, SCHEDULES["mixed"]).cpu(), ref.cpu()) <= 1e-6
 
 
@@ -278,7 +257,7 @@ def test_batch_slots_reset_flush_and_graphs(dev):
 
     m = _synthetic(dev, "mb2")
     T = 30
-    c = _mels(4, T, 76)
+    c = mels(4, T, 76)
     y4 = _stream(MelGANLookaheadStream(m, batch=4), c, SCHEDULES["mixed"])
     for b in range(4):
         assert torch.equal(y4[b:b + 1], _stream(MelGANLookaheadStream(m, batch=1), c[b:b + 1], SCHEDULES["mixed"]))
@@ -287,7 +266,7 @@ def test_batch_slots_reset_flush_and_graphs(dev):
     st = MelGANLookaheadStream(m, batch=4)
     first = _stream(st, c[:, :6], [2, 4], flush=False)
     c2 = c.clone()
-    c2[1, 6:] = _mels(1, T - 6, 77)[0]
+    c2[1, 6:] = mels(1, T - 6, 77)[0]
     st.reset(1)
     rest = _stream(st, c2[:, 6:], [1, 3, 5])
     y = torch.cat([first, rest], -1)
@@ -312,7 +291,7 @@ def test_more_chunk_lengths_than_cached(dev):
     _, _, m = _golden(dev, "melgan_centred_mb")
     st = MelGANLookaheadStream(m, batch=2)
     sched = list(range(1, st.MAX_CHUNK_LENGTHS + 3))
-    c = _mels(2, sum(sched), 78)
+    c = mels(2, sum(sched), 78)
     assert torch.equal(_stream(st, c, sched), _expected(m, c, st.delay))
 
 
@@ -330,7 +309,7 @@ def test_short_flush_raises_and_leaves_state(dev):
 
     m = _synthetic(dev, "mb2_csmsc")
     st = MelGANLookaheadStream(m, batch=2)
-    c = _mels(2, 9, 79)
+    c = mels(2, 9, 79)
     a = st.push(c[:, :5])
     snap = [t.clone() for t in st._state()]
     with pytest.raises(PwgbError, match="fewer than 6 frames"):

@@ -3,7 +3,6 @@ reflect-flag history convs are bit-identical to the reflect-padded whole-signal 
 synthesis window is bit-identical to ``PQMF.synthesis``, streamed audio plus flush is bit-identical to ``inference``
 after the PQMF delay for every pad and chunk schedule, slots are independent, graphs replay what eager runs compute, and
 the unsupported cases raise."""
-import ctypes as C
 import json
 
 import pytest
@@ -12,6 +11,7 @@ import torch.nn.functional as F
 
 from helpers import REL_TOL, golden_weights, load_golden, rel_l2
 from oracle import synth
+from stream_harness import dev, debug_get, mels  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -26,15 +26,6 @@ MB2 = dict(in_channels=80, out_channels=4, kernel_size=7, channels=384, upsample
 # generic FFMA kernel on both sides (DESIGN.md section 3.7)
 FRAMES = {"v1": 15, "mb2": 40}
 GOLDEN = ["melgan_causal", "melgan_causal_replicate", "melgan_causal_zero", "melgan_causal_mb"]
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    import __graft_entry__
-
-    __graft_entry__.build()
-    return torch.device("cuda:0")
 
 
 def _golden(dev, name, weight_norm=True):
@@ -89,18 +80,6 @@ def _inference(m, c, delay=0):
     return F.pad(y, (delay, 0))
 
 
-def _debug(key, n):
-    from parallelwavegan_b200 import capi
-
-    v = (C.c_int * n)()
-    assert capi.lib().pwgb_debug_get(key, C.cast(v, C.c_void_p), C.sizeof(v)) == 0
-    return list(v)
-
-
-def _mels(B, T, seed):
-    return synth.randn((B, T, 80), seed)
-
-
 # ---------------------------------------------------------------------------------------------------- kernels
 # name: B, cin, cout, K, dilation, n, pad_left (== H), fresh flags, epilogue, engine, expected plan
 #   plan (tensor cores, pwgb_debug_get(1)): "cp" cp.async-staged, "direct" register path, "win" win_mode, "nco" column chunks
@@ -139,11 +118,11 @@ def test_reflect_conv_stream_bit_exact(dev, name):
     try:
         y = ops.conv1d_stream(x, hist, w, b, pad_left=pl, dilation=d, replicate=fresh, reflect=True, **kw)
         if engine == "tc":
-            p = _debug(1, 8)
+            p = debug_get(1, 8)
             assert p[5] == 0, p  # no TMA activation rows in a history launch
             assert {"cp": p[3] > 0 and not p[6], "direct": p[3] == 0, "win": p[6] == 1, "nco": p[7] > 1}[plan], p
         else:
-            assert _debug(3, 6)[0] == 0
+            assert debug_get(3, 6)[0] == 0
         ref_reflect = ops.conv1d_raw(x, w, b, dilation=d, padding=(pl, 0), pad_mode="reflect", **kw)
         ref_hist = ops.conv1d_raw(torch.cat([hist, x], -1), w, b, dilation=d, padding=(0, 0), **kw)
     finally:
@@ -173,7 +152,7 @@ def test_synthesis_window_equals_pqmf_synthesis(dev):
     S = synth.randn((3, 4, 80), 61).to(dev)
     w = (pq.synthesis_filter[0].flip(-1) * 4.0).unsqueeze(1).contiguous()
     whole_fresh = pq.synthesis(S[:, :, 30:].contiguous())
-    assert _debug(3, 6)[0] == 0  # the whole-signal synthesis took the generic FFMA kernel
+    assert debug_get(3, 6)[0] == 0  # the whole-signal synthesis took the generic FFMA kernel
     whole_cont = pq.synthesis(S)
     fresh = torch.tensor([1, 0, 1], dtype=torch.int32, device=dev)
     hist = torch.zeros(3, 4, 15, device=dev)
@@ -209,7 +188,7 @@ def test_golden_stream_equals_inference(dev, name, weight_norm, schedule):
     st = CausalMelGANStream(m, batch=c.shape[0])
     assert st.min_first_frames == (7 if name != "melgan_causal_replicate" and name != "melgan_causal_zero" else 1)
     ref = _inference(m, c, st.delay)
-    assert _debug(3, 6)[0] == 0  # the last few-channel conv of the whole utterance took the generic kernel
+    assert debug_get(3, 6)[0] == 0  # the last few-channel conv of the whole utterance took the generic kernel
     assert torch.equal(_stream(st, c, SCHEDULES[schedule]), ref)
 
 
@@ -231,7 +210,7 @@ def test_recipe_shaped_stream_equals_inference(dev, kind, weight_norm, schedule)
     from parallelwavegan_b200.streaming import CausalMelGANStream
 
     m = _synthetic(dev, kind, weight_norm)
-    c = _mels(1, FRAMES[kind], 41)
+    c = mels(1, FRAMES[kind], 41)
     st = CausalMelGANStream(m)
     assert st.min_first_frames == 7 and st.delay == (31 if kind == "mb2" else 0)
     assert torch.equal(_stream(st, c, SCHEDULES[schedule]), _inference(m, c, st.delay))
@@ -243,7 +222,7 @@ def test_mb_pads_stream_equals_inference(dev, pad):
 
     over = dict(pad="ReplicationPad1d") if pad == "replicate" else dict(pad="ConstantPad1d", pad_params={"value": 0.0})
     m = _synthetic(dev, "mb2", **over)
-    c = _mels(2, 20, 43)
+    c = mels(2, 20, 43)
     st = CausalMelGANStream(m, batch=2)
     assert st.min_first_frames == 1
     assert torch.equal(_stream(st, c, SCHEDULES["mixed"]), _inference(m, c, st.delay))
@@ -256,7 +235,7 @@ def test_long_utterance_within_rel_l2(dev, kind):
     from parallelwavegan_b200.streaming import CausalMelGANStream
 
     m = _golden(dev, "melgan_causal")[2] if kind == "golden" else _synthetic(dev, "mb2")
-    c = _mels(2, 300 if kind == "golden" else 80, 31)
+    c = mels(2, 300 if kind == "golden" else 80, 31)
     st = CausalMelGANStream(m, batch=2)
     ref = _inference(m, c, st.delay)
     y = _stream(st, c, [5, 16, 3])
@@ -270,7 +249,7 @@ def test_batch_slots_reset_and_graphs(dev):
 
     m = _synthetic(dev, "mb2")
     T = 24
-    c = _mels(4, T, 51)
+    c = mels(4, T, 51)
     y4 = _stream(CausalMelGANStream(m, batch=4), c, SCHEDULES["mixed"])
     for b in range(4):
         assert torch.equal(y4[b:b + 1], _stream(CausalMelGANStream(m, batch=1), c[b:b + 1], SCHEDULES["mixed"]))
@@ -280,7 +259,7 @@ def test_batch_slots_reset_and_graphs(dev):
     first = _stream(st, c[:, :10], [3], flush=False)
     tail1 = st.flush(1)
     c2 = c.clone()
-    c2[1, 10:] = _mels(1, T - 10, 52)[0]
+    c2[1, 10:] = mels(1, T - 10, 52)[0]
     rest = _stream(st, c2[:, 10:], [1, 3, 5], flush=False)
     end = st.flush()
     y = torch.cat([first, rest, end], -1)
@@ -300,12 +279,12 @@ def test_unsupported_cases_raise(dev):
     small = dict(V1, channels=32, upsample_scales=[4, 4], stacks=2)
     st = CausalMelGANStream(models.MelGANGenerator(**small).to(dev).eval())
     with pytest.raises(PwgbError, match="at least 7 frames"):
-        st.push(_mels(1, 6, 1)[0])
-    st.push(_mels(1, 7, 1)[0])
-    st.push(_mels(1, 1, 2)[0])  # later pushes may be short
+        st.push(mels(1, 6, 1)[0])
+    st.push(mels(1, 7, 1)[0])
+    st.push(mels(1, 1, 2)[0])  # later pushes may be short
     st.reset()
     with pytest.raises(PwgbError, match="at least 7 frames"):
-        st.push(_mels(1, 3, 1)[0])
+        st.push(mels(1, 3, 1)[0])
     with pytest.raises(PwgbError):
         CausalMelGANStream(models.MelGANGenerator(**dict(small, use_causal_conv=False)).to(dev).eval())
     with pytest.raises(PwgbError):

@@ -11,6 +11,7 @@ import torch
 
 from helpers import REL_TOL, golden_weights, load_golden, rel_l2
 from oracle import synth
+from stream_harness import dev  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -18,15 +19,6 @@ SCHEDULES = {"ones": [1], "short": [3], "long": [7], "mixed": [1, 4, 2, 9, 1, 3]
 V1 = dict(in_channels=1, out_channels=1, kernel_size=3, layers=30, stacks=3, residual_channels=64, gate_channels=128,
           skip_channels=64, aux_channels=80, aux_context_window=2, use_causal_conv=False, upsample_conditional_features=True,
           upsample_net="ConvInUpsampleNetwork", upsample_params={"upsample_scales": [4, 4, 4, 4]})
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    import __graft_entry__
-
-    __graft_entry__.build()
-    return torch.device("cuda:0")
 
 
 def _model(dev, weight_norm=True, seed=91, **over):

@@ -10,6 +10,7 @@ import torch
 
 from helpers import REL_TOL, golden_weights, load_golden, rel_l2
 from oracle import synth
+from stream_harness import dev  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -27,15 +28,6 @@ CONFIGS = {
     "upnet": dict(aux_context_window=0, upsample_net="UpsampleNetwork"),
     "k2": dict(kernel_size=2, layers=10, stacks=1, upsample_params={"upsample_scales": [4, 4, 4]}),
 }
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    import __graft_entry__
-
-    __graft_entry__.build()
-    return torch.device("cuda:0")
 
 
 def _model(dev, config="acw2", weight_norm=True, seed=81, **over):

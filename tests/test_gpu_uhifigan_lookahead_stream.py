@@ -13,21 +13,13 @@ import torch
 
 from helpers import golden_weights, load_golden
 from oracle import synth
+from stream_harness import dev  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
 SCHEDULES = {"ones": [1], "short": [3], "mixed": [1, 4, 2, 9, 1, 3]}
 LONG_OUTPUT_CONV = 4096  # whole-utterance output samples from which the output conv sums in another order
 GOLDENS = ["uhifigan_small", "uhifigan_odd", "uhifigan_opencpop"]
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import __graft_entry__
-
-    __graft_entry__.build()
-    return torch.device("cuda:0")
 
 
 @pytest.fixture

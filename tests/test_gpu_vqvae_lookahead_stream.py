@@ -13,19 +13,11 @@ import torch
 from helpers import load_golden, rel_l2
 from oracle import synth
 from test_vqvae_cpu import vq_weights
+from stream_harness import dev, debug_get  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 NAMES = ["vqvae_yesno", "vqvae_vctk_g", "vqvae_vctk_lg"]
 SCHEDULES = {"ones": [1], "short": [3], "long": [17], "mixed": [1, 4, 2, 9, 1, 3]}
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    import __graft_entry__
-
-    __graft_entry__.build()
-    return torch.device("cuda:0")
 
 
 def _model(dev, name, weight_norm=True):
@@ -71,14 +63,6 @@ def _check(m, st, x, l, g, schedule):
 
 
 # ---------------------------------------------------------------------------------------------------- entry points
-def _last(key, n):
-    from parallelwavegan_b200 import capi
-
-    buf = (C.c_int * n)()
-    assert capi.lib().pwgb_debug_get(key, buf, C.sizeof(buf)) == 0
-    return list(buf)
-
-
 # (cin, cout, groups, stride): the strided convs of the yesno and vctk encoders
 STRIDED = [(16, 32, 4, 4), (32, 32, 8, 4), (32, 32, 8, 2), (16, 64, 4, 4), (64, 256, 16, 4), (256, 512, 64, 2), (512, 1024, 128, 2)]
 
@@ -120,9 +104,9 @@ def test_grouped_strided_entry_points(dev, cin, cout, groups, s, n):
     if (cout // groups) % 16 == 0 and cgo <= 2 * cin_g * s:
         w2 = ops.s2d_weight(w, s, cgo).contiguous()
         ref = ops.conv1d_raw(xs, w2, b, groups=groups, post_act="lrelu", post_slope=0.2)
-        plan_whole = _last(1, 8)
+        plan_whole = debug_get(1, 8)
         got = ops.conv1d_stream(xs, None, w2, b, pad_left=0, post_act="lrelu", post_slope=0.2, mask=mask, groups=groups)
-        plan_stream = _last(1, 8)
+        plan_stream = debug_get(1, 8)
         assert plan_whole[0] == plan_stream[0] and plan_whole[7] == plan_stream[7] == groups * ((cout // groups) // min(cout // groups, 128))
         assert torch.equal(got, masked(ref))
 
@@ -176,7 +160,7 @@ def _routes(fn):
     def wrap(k, f):
         def call(*a):
             rc = f(*a)
-            r = _last(names[k], 8 if names[k] == 1 else 6)
+            r = debug_get(names[k], 8 if names[k] == 1 else 6)
             out.append(("tc", r[0]) if names[k] == 1 else ("ffma", r[0], r[1], r[2]))
             return rc
         return call
