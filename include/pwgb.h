@@ -808,6 +808,22 @@ PWGB_API int pwgb_vq_stream_forward(const float* z_e, const float* codebook, int
                                     const long long* g, int num_global, int global_channels, const pwgb_stream_ext* ext, int batch,
                                     int dim, int t, void* stream);
 
+/* ------------------------------------------------------------------------
+ * SineGen excitation (layers/sine.py SineGen.forward, flag_for_pulse=False) for `batch` rows of f0 (batch, t) fp32 at
+ * the sample rate, dim = harmonic_num + 1.  The random draws come from the caller: rand_ini (batch, dim) uniform, of
+ * which column 0 is ignored (the reference zeroes it), and noise_in (batch, t, dim) standard normal.  Writes
+ * sine_waves (batch, t, dim), uv (batch, t) and noise (batch, t, dim); phase (batch, t, dim), the fp32 argument of
+ * sin, is written when non-null.  Every elementwise step is the reference's fp32 operation in its order; the two
+ * prefix sums accumulate in fp64 and round each output to fp32, as CPU torch.cumsum on fp32 does, and equal the
+ * sequential sums while every partial sum is exact in fp64 (DESIGN.md §3.15).  Deterministic: five launches, no
+ * atomics.  ws: pwgb_sine_gen_workspace(batch, t, harmonic_num) bytes of device memory.  batch <= 65535.
+ * ---------------------------------------------------------------------- */
+PWGB_API size_t pwgb_sine_gen_workspace(int batch, long long t, int harmonic_num);
+PWGB_API int pwgb_sine_gen_forward(const float* f0, int batch, long long t, int harmonic_num, float samp_rate, float sine_amp,
+                                   float noise_std, float voiced_threshold, const float* rand_ini, const float* noise_in,
+                                   float* sine_waves, float* uv, float* noise, float* phase, void* ws, size_t ws_bytes,
+                                   void* stream);
+
 #ifdef __cplusplus
 }
 #endif

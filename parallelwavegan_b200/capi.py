@@ -322,6 +322,11 @@ def lib():
     L.pwgb_vq_forward.argtypes = [vp, vp, C.c_int, vp, vp, vp, vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp]
     L.pwgb_vq_backward.restype = C.c_int
     L.pwgb_vq_backward.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, C.c_int, vp, vp]
+    L.pwgb_sine_gen_workspace.restype = C.c_size_t
+    L.pwgb_sine_gen_workspace.argtypes = [C.c_int, ll, C.c_int]
+    L.pwgb_sine_gen_forward.restype = C.c_int
+    L.pwgb_sine_gen_forward.argtypes = [vp, C.c_int, ll, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, vp, vp, vp, vp, vp, vp,
+                                        vp, C.c_size_t, vp]
     _lib = L
     return L
 
@@ -375,5 +380,5 @@ EXPORTED_SYMBOLS = [
     "pwgb_symbol_embed_forward", "pwgb_symbol_embed_stream_forward", "pwgb_duration_queue_append", "pwgb_symbol_regulate_stream_forward", "pwgb_symbol_embed_backward_workspace", "pwgb_symbol_embed_backward",
     "pwgb_channel_layernorm_forward", "pwgb_channel_layernorm_backward_workspace", "pwgb_channel_layernorm_backward",
     "pwgb_duration_loss_forward", "pwgb_duration_loss_backward", "pwgb_duration_round", "pwgb_collate_runlength",
-    "pwgb_vq_forward", "pwgb_vq_stream_forward", "pwgb_vq_backward",
+    "pwgb_vq_forward", "pwgb_vq_stream_forward", "pwgb_vq_backward", "pwgb_sine_gen_workspace", "pwgb_sine_gen_forward",
 ]

@@ -24,7 +24,11 @@ graph per (batch, padded length) serves every mix of lengths, which are a static
 HiFi-GAN needs the padding only.
 
 The discrete-symbol HiFi-GAN decodes units: each input is a (T, 2) (symbol, speaker) or (T, 1) index array, padded
-with symbol 0 past its end (and its own speaker)."""
+with symbol 0 past its end (and its own speaker).
+
+The U-Net HiFi-GAN decodes mels with their excitations (bin/decode.py:156-230): ``decode(mels, excitations=...)``, one
+(T', hop) or (T' * hop,) excitation per utterance, which crosses PCIe once from pinned memory into its batch slot and is
+padded with zero samples where the mels get zero frames.  Mels and excitation are the static inputs of the graph."""
 import ctypes as C
 
 import numpy as np
@@ -126,8 +130,6 @@ def ragged_refusal(model):
 class Decoder:
     def __init__(self, model, use_graphs=True, max_batch=16, exact=True, bucket_frames=32, rank=0, world=1, seed=None,
                  ragged=False):
-        from . import models
-
         self.max_batch, self.exact, self.bucket = int(max_batch), bool(exact), int(bucket_frames)
         self.ragged = bool(ragged)
         # a ragged batch passes per-item lengths to the non-causal HiFi-GAN body; a causal one needs the padding only
@@ -146,9 +148,7 @@ class Decoder:
         self.dev = next(model.parameters()).device
         if self.dev.type != "cuda":
             raise PwgbError("Decoder: the model must live on a CUDA device (no CPU fallback)")
-        self.kind = ("pwg" if isinstance(model, models.ParallelWaveGANGenerator) else
-                     "style" if isinstance(model, models.StyleMelGANGenerator) else
-                     "units" if type(model) is models.DiscreteSymbolHiFiGANGenerator else "mel2wav")
+        self.kind = decoder_kind(model)
         self.rank, self.world = rank, world
         self.gen = torch.Generator(device=self.dev)
         if seed is not None:
@@ -159,8 +159,13 @@ class Decoder:
             y = model(*a)
             return pq.synthesis(y) if pq is not None else y
 
-        self.runner = GraphedGenerator(model, fn=fwd) if use_graphs else fwd
-        self.hop = int(getattr(model, "upsample_factor", 0)) or None
+        def fwd_excitation(c, e):  # the U-Net HiFi-GAN: mels and excitation (its f0 input is unused)
+            return model(c, None, e)
+
+        run = fwd_excitation if self.kind == "uhifigan" else fwd
+        self.runner = GraphedGenerator(model, fn=run) if use_graphs else run
+        self.hop = (int(np.prod(model.upsample_scales)) if self.kind == "uhifigan" else
+                    int(getattr(model, "upsample_factor", 0)) or None)
         self.ctx = int(getattr(model, "aux_context_window", 0)) if self.kind == "pwg" else 0
 
     def _groups(self, lengths, idxs):
@@ -183,12 +188,21 @@ class Decoder:
                 yield key, g[k : k + self.max_batch]
 
     @torch.no_grad()
-    def decode(self, mels, normalize_before=False, to_pcm16=True, noises=None):
+    def decode(self, mels, normalize_before=False, to_pcm16=True, noises=None, excitations=None):
         """mels: list of (T_i, C) arrays / tensors.  Returns {index: waveform}: int16 numpy arrays of shape (samples,)
         (``to_pcm16``) or float32 device tensors (samples, out_channels).  ``noises`` (Parallel WaveGAN only): optional
-        {index: (samples, 1)} noise for reproducibility (``inference(c, x)``)."""
+        {index: (samples, 1)} noise for reproducibility (``inference(c, x)``).  ``excitations`` (the U-Net HiFi-GAN
+        only, and required there): a list aligned with ``mels``, entry i (T_i, hop) or (T_i * hop,)."""
         m = self.model
         idxs = list(sharding.partition(len(mels), self.rank, self.world))
+        exc = None
+        if self.kind == "uhifigan":
+            if normalize_before:
+                raise PwgbError("Decoder: the U-Net HiFi-GAN's inference ignores normalize_before; normalise the mels "
+                                "before decoding (normalize_before=False)")
+            exc = _excitation_rows(excitations, mels, idxs, self.hop)
+        elif excitations is not None:
+            raise PwgbError(f"Decoder: excitations are an input of the U-Net HiFi-GAN only, not of {type(m).__name__}")
         if self.kind == "style":  # batch-1 inference with its own noise / padding protocol (style_melgan.py:226-262)
             out = {}
             for i in idxs:
@@ -236,6 +250,16 @@ class Decoder:
                             nz = torch.as_tensor(noises[i], dtype=torch.float32).to(self.dev).reshape(-1)
                             z[b, 0, : nz.numel()] = nz
                 y = self.runner(z, cin)
+            elif exc is not None:
+                e = torch.empty((B, 1, Tb * self.hop), device=self.dev, dtype=torch.float32)
+                for b, i in enumerate(grp):
+                    src = exc[i]
+                    src = src.pin_memory() if not src.is_cuda and not src.is_pinned() else src
+                    n = src.numel()
+                    e[b, 0, :n].copy_(src, non_blocking=True)
+                    if n < e.shape[-1]:
+                        e[b, 0, n:].zero_()
+                y = self.runner(cin, e)
             else:
                 y = self.runner(cin)
             hop = y.shape[-1] // Tb
@@ -253,6 +277,36 @@ class Decoder:
             for i, hbuf in pending:
                 out[i] = hbuf.numpy()
         return out
+
+
+def decoder_kind(model):
+    """How ``Decoder`` feeds a generator: "pwg" (noise and mels), "style" (per-utterance inference), "units" (the
+    discrete-symbol HiFi-GAN), "uhifigan" (mels and excitation) or "mel2wav" (mels)."""
+    from . import models
+
+    return ("pwg" if isinstance(model, models.ParallelWaveGANGenerator) else
+            "style" if isinstance(model, models.StyleMelGANGenerator) else
+            "units" if type(model) is models.DiscreteSymbolHiFiGANGenerator else
+            "uhifigan" if isinstance(model, models.UHiFiGANGenerator) else "mel2wav")
+
+
+def _excitation_rows(excitations, mels, idxs, hop):
+    """The excitations of utterances ``idxs`` as {i: (T_i * hop,) float32 tensor}, each checked against the frame count
+    of mels[i]"""
+    if excitations is None:
+        raise PwgbError("Decoder: the U-Net HiFi-GAN needs excitations=[...], one per utterance (features.excitation)")
+    if len(excitations) != len(mels):
+        raise PwgbError(f"Decoder: {len(excitations)} excitations for {len(mels)} utterances")
+    rows = {}
+    for i in idxs:
+        x = excitations[i]
+        e = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.asarray(x, dtype=np.float32))
+        e = e.to(torch.float32).reshape(-1)
+        want = int(np.shape(mels[i])[0]) * hop
+        if e.numel() != want:
+            raise PwgbError(f"Decoder: excitation {i} has {e.numel()} samples, its {want // hop} frames need {want} (hop {hop})")
+        rows[i] = e.contiguous()
+    return rows
 
 
 def _unit_rows(x, speakers):

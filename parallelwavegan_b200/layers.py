@@ -653,3 +653,42 @@ class VQCodebook(torch.nn.Module):
         straight through to z_e, and the same codes for the quantisation loss, whose gradient goes to the codebook."""
         z_q_st, z_q, _ = ops.vq(z_e, self.embedding.weight)
         return z_q_st, z_q
+
+
+class SineGen(torch.nn.Module):
+    """layers/sine.py:7-177: the sine excitation of a harmonic-plus-noise source, on the GPU (``ops.sine_gen``).
+
+    ``forward(f0)`` takes f0 (B, T, 1) in Hz at the sample rate (0 on unvoiced samples) and returns ``(sine_waves, uv,
+    noise)`` of shapes (B, T, dim), (B, T, 1), (B, T, dim), dim = harmonic_num + 1, under ``no_grad`` as the
+    reference does.  The initial phases (uniform, none for the fundamental) and the noise (standard normal) are drawn
+    on the device from ``generator`` (torch's default when None), or injected with ``rand_ini=`` (B, dim) and
+    ``noise=`` (B, T, dim) for tests and reproducibility.  ``flag_for_pulse=True`` (the PulseGen variant, used by no
+    recipe) raises ``PwgbError``."""
+
+    def __init__(self, samp_rate, harmonic_num=0, sine_amp=0.1, noise_std=0.003, voiced_threshold=0, flag_for_pulse=False):
+        super().__init__()
+        if flag_for_pulse:
+            raise PwgbError("SineGen(flag_for_pulse=True) is not supported: no recipe uses the PulseGen phase reset")
+        self.sine_amp = sine_amp
+        self.noise_std = noise_std
+        self.harmonic_num = harmonic_num
+        self.dim = self.harmonic_num + 1
+        self.sampling_rate = samp_rate
+        self.voiced_threshold = voiced_threshold
+        self.flag_for_pulse = flag_for_pulse
+
+    @torch.no_grad()
+    def forward(self, f0, generator=None, rand_ini=None, noise=None):
+        if not isinstance(f0, torch.Tensor) or f0.dim() != 3 or f0.shape[2] != 1:
+            raise PwgbError(f"SineGen: f0 must be a (B, T, 1) tensor, got {getattr(f0, 'shape', type(f0))}")
+        B, T = f0.shape[0], f0.shape[1]
+        if not f0.is_cuda:
+            raise PwgbError(f"SineGen: f0 is on {f0.device}; parallelwavegan_b200 only runs on CUDA (no CPU fallback)")
+        if rand_ini is None:
+            rand_ini = torch.rand(B, self.dim, device=f0.device, generator=generator)
+        if noise is None:
+            noise = torch.randn(B, T, self.dim, device=f0.device, generator=generator)
+        rand_ini = torch.as_tensor(rand_ini, dtype=torch.float32, device=f0.device)
+        noise = torch.as_tensor(noise, dtype=torch.float32, device=f0.device)
+        return ops.sine_gen(f0.reshape(B, T).float(), self.harmonic_num, self.sampling_rate, self.sine_amp, self.noise_std,
+                            self.voiced_threshold, rand_ini, noise)

@@ -368,6 +368,32 @@ def dropout(x, p, training):
     return dropout_raw(x, p, seed)
 
 
+def sine_gen(f0, harmonic_num, samp_rate, sine_amp, noise_std, voiced_threshold, rand_ini, noise, phase=False):
+    """SineGen.forward (layers/sine.py, flag_for_pulse=False) -- pwgb_sine_gen_forward.  f0 (B, T) at the sample rate;
+    rand_ini (B, dim) uniform (column 0 ignored) and noise (B, T, dim) standard normal are the random draws, dim =
+    harmonic_num + 1.  Returns (sine_waves (B, T, dim), uv (B, T, 1), noise (B, T, dim)), and the fp32 argument of
+    sin (B, T, dim) last when ``phase``."""
+    f0 = _dev(f0, "f0")
+    rand_ini, noise = _dev(rand_ini, "rand_ini"), _dev(noise, "noise")
+    if f0.dim() != 2:
+        raise PwgbError(f"sine_gen: f0 must be (B, T), got {tuple(f0.shape)}")
+    B, T = f0.shape
+    dim = int(harmonic_num) + 1
+    if harmonic_num < 0 or tuple(rand_ini.shape) != (B, dim) or tuple(noise.shape) != (B, T, dim):
+        raise PwgbError(f"sine_gen: harmonic_num {harmonic_num}, f0 {tuple(f0.shape)}: rand_ini must be {(B, dim)} and noise "
+                        f"{(B, T, dim)}, got {tuple(rand_ini.shape)} and {tuple(noise.shape)}")
+    sine = torch.empty((B, T, dim), device=f0.device, dtype=torch.float32)
+    uv = torch.empty((B, T, 1), device=f0.device, dtype=torch.float32)
+    nz = torch.empty_like(sine)
+    ph = torch.empty_like(sine) if phase else None
+    L = capi.lib()
+    ws = torch.empty(max(int(L.pwgb_sine_gen_workspace(B, T, dim - 1)), 1), device=f0.device, dtype=torch.uint8)
+    rc = L.pwgb_sine_gen_forward(_p(f0), B, T, dim - 1, float(samp_rate), float(sine_amp), float(noise_std), float(voiced_threshold),
+                                 _p(rand_ini), _p(noise), _p(sine), _p(uv), _p(nz), _p(ph), _p(ws), ws.numel(), _stream())
+    capi.check(rc, "pwgb_sine_gen_forward")
+    return (sine, uv, nz, ph) if phase else (sine, uv, nz)
+
+
 def upsample_fir(x, fir, scale, out=None, out_channels=None, causal=False):
     """One stage of the PWG conditioning upsampler (layers/upsample.py:112-128):
     nearest repeat x`scale` + (2*scale+1)-tap FIR, zero padded -- pwgb_upsample_fir_forward; ``causal``: the FIR
