@@ -265,6 +265,30 @@ PWGB_API int pwgb_conv_transpose1d_stream_ext_forward(const pwgb_convtr1d_desc* 
  * rate, lookahead as above) is set to +0.0.  ext must hold a mask; its residual fields are ignored. */
 PWGB_API int pwgb_stream_mask(float* y, int batch, int rows, int t, const pwgb_stream_ext* ext, void* stream);
 
+/* Whole-signal convs over a batch of signals of different lengths ("ragged" batches; the VQ-VAE's encoder and decoder).
+ * d is the descriptor of pwgb_conv1d_forward / pwgb_conv1d_tc_forward over the padded batch (pad_mode PWGB_PAD_ZERO,
+ * PWGB_PAD_REFLECT or PWGB_PAD_REPLICATE; period 1, no pre_gate, contiguous), and ext a mask of pwgb_stream_ext at the
+ * output: frame (DEVICE, all 0 for signals that start at sample 0), end (DEVICE, the item's length at this layer's rate
+ * in units of rate), rate >= 1, lookahead 0, no residual history, in_lookahead 0, and edge == d->pad_mode.  Item b holds
+ * L_b = end[b] * rate valid rows; then for every output row inside [0, L_b):
+ *   zero pad: input rows at or past the item's input length read as zero -- the caller keeps them zero (the previous
+ *     masked layer leaves them so); any stride;
+ *   reflect / replicate pad (stride 1): an input row u >= L_b reads row 2 (L_b - 1) - u (reflect) or L_b - 1
+ *     (replicate) of the same item, rows before 0 likewise -- the edge policy of pwgb_stream_ext, applied to the whole
+ *     signal; ReflectionPad1d needs pad_left < L_b, which the entry cannot read on the host: the caller checks it (an item
+ *     that breaks it reads zeros, never memory outside x);
+ * and its value is bit-identical to the entry point without ext on that item alone with t = L_b, whenever that lone call
+ * takes the same kernel (the FFMA entry always runs the generic kernel, never conv1d_small_cout_kernel or
+ * conv1d_fewcout_long_kernel) and, on the tensor cores, the same tile shape.  Output rows at or past L_b are stored as
+ * +0.0 (also with accumulate).  The launches are the EXT / EDGE instantiations of the stream history entry points with no
+ * history rows.  ext == NULL: the call is pwgb_conv1d_forward / pwgb_conv1d_tc_forward.  A mask without frame and end
+ * counters, an edge other than d->pad_mode, or a reflect / replicate edge with stride > 1 or pad_left >= t_in is
+ * PWGB_INVALID. */
+PWGB_API int pwgb_conv1d_ragged_forward(const pwgb_conv1d_desc* d, const float* x, const float* w, const float* bias,
+                                        const float* residual, const pwgb_stream_ext* ext, float* y, void* stream);
+PWGB_API int pwgb_conv1d_tc_ragged_forward(const pwgb_conv1d_desc* d, const float* x, const void* packed_w, const float* bias,
+                                           const float* residual, const pwgb_stream_ext* ext, float* y, void* stream);
+
 /* The strided convs of a stream (the encoder of a centred U-Net HiFi-GAN).
  *
  * pwgb_s2d_stream_forward: pwgb_s2d_forward (groups 1, period 1, pad_left 0) on the window [hist | x] without building it:

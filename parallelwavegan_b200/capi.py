@@ -132,6 +132,10 @@ def lib():
     L.pwgb_conv_transpose1d_stream_ext_forward.restype = C.c_int
     L.pwgb_conv_transpose1d_stream_ext_forward.argtypes = [C.POINTER(ConvTr1dDesc), vp, vp, vp, vp, vp, C.POINTER(StreamExt), vp, vp,
                                                            C.c_size_t, vp]
+    L.pwgb_conv1d_ragged_forward.restype = C.c_int
+    L.pwgb_conv1d_ragged_forward.argtypes = [C.POINTER(Conv1dDesc), vp, vp, vp, vp, C.POINTER(StreamExt), vp, vp]
+    L.pwgb_conv1d_tc_ragged_forward.restype = C.c_int
+    L.pwgb_conv1d_tc_ragged_forward.argtypes = [C.POINTER(Conv1dDesc), vp, vp, vp, vp, C.POINTER(StreamExt), vp, vp]
     L.pwgb_stream_mask.restype = C.c_int
     L.pwgb_stream_mask.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.POINTER(StreamExt), vp]
     L.pwgb_s2d_stream_forward.restype = C.c_int
@@ -381,4 +385,5 @@ EXPORTED_SYMBOLS = [
     "pwgb_channel_layernorm_forward", "pwgb_channel_layernorm_backward_workspace", "pwgb_channel_layernorm_backward",
     "pwgb_duration_loss_forward", "pwgb_duration_loss_backward", "pwgb_duration_round", "pwgb_collate_runlength",
     "pwgb_vq_forward", "pwgb_vq_stream_forward", "pwgb_vq_backward", "pwgb_sine_gen_workspace", "pwgb_sine_gen_forward",
+    "pwgb_conv1d_ragged_forward", "pwgb_conv1d_tc_ragged_forward",
 ]

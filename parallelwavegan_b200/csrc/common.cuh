@@ -15,6 +15,9 @@ int conv1d_stream_check(const pwgb_conv1d_desc* d, const float* x, const float* 
 // argument check of a pwgb_stream_ext (NULL passes); residual: whether the launch has one; pad_mode: the conv's (an edge
 // policy needs PWGB_PAD_HISTORY), -1 for an entry point without an edge policy
 int stream_ext_check(const pwgb_stream_ext* e, const float* residual, int pad_mode = -1);
+// argument check of the two ragged conv entry points (stream.cu); h: the history descriptor their launch runs
+int conv1d_ragged_check(const pwgb_conv1d_desc* d, const float* x, const pwgb_stream_ext* e, const float* y,
+                        pwgb_conv1d_desc* h);
 
 #define PWGB_CHECK_ARG(cond, ...)          \
   do {                                     \

@@ -1332,6 +1332,17 @@ extern "C" int pwgb_conv1d_tc_stream_ext_forward(const pwgb_conv1d_desc* d, cons
   return tc_forward(d, x, packed_w, bias, residual, y, stream, hist, replicate, hist_len, ext);
 }
 
+extern "C" int pwgb_conv1d_tc_ragged_forward(const pwgb_conv1d_desc* d, const float* x, const void* packed_w, const float* bias,
+                                             const float* residual, const pwgb_stream_ext* ext, float* y, void* stream) {
+  if (!ext) return pwgb_conv1d_tc_forward(d, x, packed_w, bias, residual, y, stream);
+  PWGB_CHECK_ARG(packed_w, "conv1d_tc_ragged: null argument");
+  pwgb_conv1d_desc h;
+  if (const int rc = conv1d_ragged_check(d, x, ext, y, &h)) return rc;
+  // the EXT / EDGE history kernels with no history rows: rows outside [0, t_in) stage as zero unless the edge policy
+  // moves them onto the item's own reflected or replicated sample
+  return tc_forward(&h, x, packed_w, bias, residual, y, stream, nullptr, nullptr, 0, ext);
+}
+
 // ======================================================================================
 // A 128- or 256-channel HiFi-GAN ResBlock conv pair as two conv1d_tc launches that hand the intermediate over packed
 // (pk_plane): conv1's epilogue writes lrelu(conv1 + b1) already split, conv2 lands it with one tensor copy per chunk and

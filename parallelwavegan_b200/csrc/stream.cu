@@ -46,6 +46,36 @@ int conv1d_stream_check(const pwgb_conv1d_desc* d, const float* x, const float* 
   return PWGB_OK;
 }
 
+// The argument check of the two ragged entry points: h becomes the history descriptor (no history rows) whose EXT or EDGE
+// launch computes the whole-signal conv d with each item's pad at its own end
+int conv1d_ragged_check(const pwgb_conv1d_desc* d, const float* x, const pwgb_stream_ext* e, const float* y,
+                        pwgb_conv1d_desc* h) {
+  PWGB_CHECK_ARG(d && x && y && e, "conv1d_ragged: null argument");
+  PWGB_CHECK_ARG(d->batch >= 0 && d->cin > 0 && d->cout > 0 && d->t_in > 0 && d->t_out >= 0, "conv1d_ragged: bad sizes");
+  PWGB_CHECK_ARG(d->kernel > 0 && d->stride > 0 && d->dilation > 0 && d->groups > 0 && d->pad_left >= 0 &&
+                     d->cin % d->groups == 0 && d->cout % d->groups == 0,
+                 "conv1d_ragged: bad kernel geometry");
+  PWGB_CHECK_ARG(d->pad_mode == PWGB_PAD_ZERO || d->pad_mode == PWGB_PAD_REFLECT || d->pad_mode == PWGB_PAD_REPLICATE,
+                 "conv1d_ragged: pad_mode must be PWGB_PAD_ZERO, PWGB_PAD_REFLECT or PWGB_PAD_REPLICATE");
+  PWGB_CHECK_ARG(e->frame && e->end && e->rate >= 1 && e->lookahead == 0,
+                 "conv1d_ragged: ext must be a mask with frame and end counters, rate >= 1 and lookahead 0");
+  PWGB_CHECK_ARG(!e->res_hist && e->res_hist_len == 0 && e->res_delay == 0 && e->in_lookahead == 0,
+                 "conv1d_ragged: no delayed residual and no input lookahead");
+  PWGB_CHECK_ARG(e->edge == d->pad_mode, "conv1d_ragged: ext->edge (%d) must be the conv's pad_mode (%d)", e->edge, d->pad_mode);
+  PWGB_CHECK_ARG(d->pad_mode == PWGB_PAD_ZERO || (d->stride == 1 && d->pad_left < d->t_in),
+                 "conv1d_ragged: a reflect or replicate edge needs stride 1 and pad_left (%d) < t_in (%d)", d->pad_left, d->t_in);
+  PWGB_UNSUPPORTED_IF(d->period > 1 || d->pre_gate || d->shuffle > 1 || d->x_batch_stride || d->y_batch_stride ||
+                          d->r_batch_stride || (d->t_valid > 0 && d->t_valid != d->t_in),
+                      "conv1d_ragged: plain convs only (period 1, no pre_gate, no shuffle, contiguous)");
+  const long long need = (long long)(d->t_out - 1) * d->stride + (long long)(d->kernel - 1) * d->dilation + 1 - d->pad_left;
+  PWGB_CHECK_ARG(d->t_out == 0 || need <= (long long)d->t_in + (d->pad_mode == PWGB_PAD_ZERO ? (1LL << 30) : d->t_in - 1),
+                 "conv1d_ragged: t_out too large for t_in");
+  *h = *d;
+  h->pad_mode = PWGB_PAD_HISTORY;
+  h->t_valid = d->t_in;
+  return PWGB_OK;
+}
+
 // One block per (entry, group of whole rows): the rows of a block are disjoint from every other block's, and within a
 // block every pass reads all its sources before any thread writes.  A pass covers ascending flat indices r * H + j of
 // its rows and element j reads index j + n of [hist | x], which is never below an index an earlier pass wrote, so the
@@ -138,6 +168,17 @@ extern "C" int pwgb_conv1d_strided_stream_ext_forward(const pwgb_conv1d_desc* d,
   PWGB_CHECK_ARG(!ext || ext->edge == PWGB_PAD_ZERO, "conv1d_strided_stream: no edge policy");
   // the generic FFMA body is written for any stride: the EXT instantiations of pwgb_conv1d_stream_ext_forward serve it
   return conv1d_stream_simt(d, x, hist, hist_len, nullptr, w, bias, nullptr, y, (cudaStream_t)stream, nullptr, 0, ext);
+}
+
+extern "C" int pwgb_conv1d_ragged_forward(const pwgb_conv1d_desc* d, const float* x, const float* w, const float* bias,
+                                          const float* residual, const pwgb_stream_ext* ext, float* y, void* stream) {
+  if (!ext) return pwgb_conv1d_forward(d, x, w, bias, residual, y, stream);
+  PWGB_CHECK_ARG(w, "conv1d_ragged: null argument");
+  pwgb_conv1d_desc h;
+  if (const int rc = conv1d_ragged_check(d, x, ext, y, &h)) return rc;
+  // the generic FFMA body of the history launches, for any stride: rows outside [0, t_in) read zero unless the edge
+  // policy moves them onto the item's own reflected or replicated sample
+  return conv1d_stream_simt(&h, x, nullptr, 0, nullptr, w, bias, residual, y, (cudaStream_t)stream, nullptr, 0, ext);
 }
 
 extern "C" int pwgb_stream_carry(const void* table, int n_entries, void* stream) {

@@ -28,7 +28,13 @@ with symbol 0 past its end (and its own speaker).
 
 The U-Net HiFi-GAN decodes mels with their excitations (bin/decode.py:156-230): ``decode(mels, excitations=...)``, one
 (T', hop) or (T' * hop,) excitation per utterance, which crosses PCIe once from pinned memory into its batch slot and is
-padded with zero samples where the mels get zero frames.  Mels and excitation are the static inputs of the graph."""
+padded with zero samples where the mels get zero frames.  Mels and excitation are the static inputs of the graph.
+
+The VQ-VAE converts waveforms (bin/decode.py's VQ-WAV2WAV branch): ``convert(waves, locals, globals)`` runs ``z =
+model.encode(x); y = model.decode(z, l, g)`` per utterance and returns the converted waveform and the code indices.
+With ``ragged=True`` the per-layer lengths of each batch (the encoder's ceil(L / s) chain and the decoder's frames) go
+to the device, where every conv keeps each item zero past its own end and reflects at its own end
+(``VQVAE.encode(x, lengths)`` / ``decode(..., lengths)``, DESIGN.md §3.16)."""
 import ctypes as C
 
 import numpy as np
@@ -36,6 +42,7 @@ import torch
 
 from . import capi, ops, sharding
 from .capi import PAD_REPLICATE, PAD_ZERO, PwgbError
+from .layers import CausalConv1d
 
 
 def _stream():
@@ -110,7 +117,7 @@ def ragged_refusal(model):
     from . import models
 
     t = type(model)
-    if t is models.HiFiGANGenerator or t is models.DiscreteSymbolHiFiGANGenerator:
+    if t is models.HiFiGANGenerator or t is models.DiscreteSymbolHiFiGANGenerator or t is models.VQVAE:
         return None
     reasons = {
         models.MelGANGenerator: "MelGAN pads its input by reflection at the signal's end (and multi-band MelGAN's PQMF "
@@ -119,7 +126,6 @@ def ragged_refusal(model):
         models.StyleMelGANGenerator: "StyleMelGAN's InstanceNorm takes statistics over the whole signal",
         models.UHiFiGANGenerator: "the U-Net HiFi-GAN's strided encoder and excitation input have no per-item length mask",
         models.DiscreteSymbolDurationGenerator: "the duration model's regulated length is only known after its predictor runs",
-        models.VQVAE: "the VQ-VAE converts waveforms and has no per-item length mask",
     }
     for cls, why in reasons.items():
         if isinstance(model, cls):
@@ -149,6 +155,8 @@ class Decoder:
         if self.dev.type != "cuda":
             raise PwgbError("Decoder: the model must live on a CUDA device (no CPU fallback)")
         self.kind = decoder_kind(model)
+        if self.kind == "wav2wav":
+            _check_wav2wav(model)
         self.rank, self.world = rank, world
         self.gen = torch.Generator(device=self.dev)
         if seed is not None:
@@ -162,7 +170,21 @@ class Decoder:
         def fwd_excitation(c, e):  # the U-Net HiFi-GAN: mels and excitation (its f0 input is unused)
             return model(c, None, e)
 
-        run = fwd_excitation if self.kind == "uhifigan" else fwd
+        def fwd_wav2wav(x, *a):  # waveforms, the model's locals and globals, then (ragged) the encoder's layer lengths
+            k = 0
+            l = g = None
+            if hasattr(model, "local_embed"):
+                l, k = a[k], k + 1
+            if hasattr(model, "global_embed"):
+                g, k = a[k], k + 1
+            lens = list(a[k:])
+            if not lens:
+                idx = model.encode(x)
+                return model.decode(idx, l, g), idx
+            idx = model.codebook(model.encoder(x, lens)[-1])
+            return model._decode(idx, l, g, lens[-1]), idx
+
+        run = {"uhifigan": fwd_excitation, "wav2wav": fwd_wav2wav}.get(self.kind, fwd)
         self.runner = GraphedGenerator(model, fn=run) if use_graphs else run
         self.hop = (int(np.prod(model.upsample_scales)) if self.kind == "uhifigan" else
                     int(getattr(model, "upsample_factor", 0)) or None)
@@ -194,6 +216,8 @@ class Decoder:
         {index: (samples, 1)} noise for reproducibility (``inference(c, x)``).  ``excitations`` (the U-Net HiFi-GAN
         only, and required there): a list aligned with ``mels``, entry i (T_i, hop) or (T_i * hop,)."""
         m = self.model
+        if self.kind == "wav2wav":
+            raise PwgbError("Decoder: a VQ-VAE converts waveforms; use Decoder.convert(waves, locals, globals)")
         idxs = list(sharding.partition(len(mels), self.rank, self.world))
         exc = None
         if self.kind == "uhifigan":
@@ -279,15 +303,148 @@ class Decoder:
         return out
 
 
+    @torch.no_grad()
+    def convert(self, waves, locals=None, globals=None, to_pcm16=True):
+        """VQ-VAE wav2wav (bin/decode.py's VQ-WAV2WAV branch): ``z = model.encode(x); y = model.decode(z, l, g)`` for
+        every utterance of this rank's share.  waves: list of (T_i,) or (T_i, 1) arrays / tensors; ``locals`` (models
+        with local conditioning, and required there): one (T'_i, num_local_embeds) array per utterance, T'_i = ceil(T_i
+        / hop); ``globals`` (models with a global embedding, and required there): one speaker id per utterance.
+        Returns {index: (waveform, indices)}: the waveform of T'_i * hop samples as int16 numpy (``to_pcm16``) or a
+        float32 device tensor (T'_i * hop, 1), the indices a (T'_i,) int64 numpy array (the reference's ``text``)."""
+        m = self.model
+        if self.kind != "wav2wav":
+            raise PwgbError(f"Decoder.convert: {type(m).__name__} is not a VQ-VAE; use Decoder.decode(mels)")
+        if m.training:
+            raise PwgbError("Decoder.convert: the model is in train mode; call model.eval() (dropout-free inference)")
+        hop = m.hop
+        idxs = list(sharding.partition(len(waves), self.rank, self.world))
+        xs = {i: _wave_row(waves[i], i) for i in idxs}
+        samples = {i: xs[i].numel() for i in idxs}
+        frames = {i: -(-samples[i] // hop) for i in idxs}
+        least = m.min_ragged_samples()
+        short = [i for i in idxs if samples[i] < least]
+        if short:
+            raise PwgbError(f"Decoder.convert: utterances {short} hold fewer than {least} samples, which the reflect pads of "
+                            f"encode / decode need")
+        ls = _cond_rows(m, locals, len(waves), idxs, frames)
+        gs = _speaker_ids(m, globals, len(waves), idxs)
+        out, pending = {}, []
+        for key, grp in self._groups(samples if self.exact and not self.ragged else frames, idxs):
+            B = len(grp)
+            T = key if self.exact and not self.ragged else key * hop  # padded samples
+            Tf = -(-T // hop)
+            x = torch.zeros((B, 1, T), device=self.dev, dtype=torch.float32)
+            for b, i in enumerate(grp):
+                x[b, 0, : samples[i]].copy_(_pinned(xs[i]), non_blocking=True)
+            args = [x]
+            if ls is not None:
+                l = torch.zeros((B, ls[grp[0]].shape[1], Tf), dtype=torch.float32)
+                for b, i in enumerate(grp):
+                    l[b, :, : frames[i]] = ls[i].transpose(0, 1)
+                args.append(l.pin_memory().to(self.dev, non_blocking=True))
+            if gs is not None:
+                args.append(torch.tensor([gs[i] for i in grp], dtype=torch.int64).pin_memory().to(self.dev, non_blocking=True))
+            if self.ragged:
+                lens = torch.stack(m.encoder.layer_lengths(torch.tensor([samples[i] for i in grp], dtype=torch.int32)))
+                lens = lens.pin_memory().to(self.dev, non_blocking=True)
+                args += list(lens.unbind(0))
+            y, idx = self.runner(*args)
+            q = pcm16(y) if to_pcm16 else None
+            for b, i in enumerate(grp):
+                n = frames[i] * hop
+                ibuf = torch.empty(frames[i], dtype=torch.int64).pin_memory()
+                ibuf.copy_(idx[b, : frames[i]], non_blocking=True)
+                if to_pcm16:
+                    hbuf = torch.empty(n, dtype=torch.int16).pin_memory()
+                    hbuf.copy_(q[b, 0, :n], non_blocking=True)
+                    pending.append((i, hbuf, ibuf))
+                else:
+                    pending.append((i, y[b, :, :n].transpose(1, 0).clone(), ibuf))
+        torch.cuda.current_stream().synchronize()
+        for i, w, ibuf in pending:
+            out[i] = (w.numpy() if to_pcm16 else w, ibuf.numpy())
+        return out
+
+
 def decoder_kind(model):
     """How ``Decoder`` feeds a generator: "pwg" (noise and mels), "style" (per-utterance inference), "units" (the
-    discrete-symbol HiFi-GAN), "uhifigan" (mels and excitation) or "mel2wav" (mels)."""
+    discrete-symbol HiFi-GAN), "uhifigan" (mels and excitation), "wav2wav" (the VQ-VAE: waveforms, ``convert``) or
+    "mel2wav" (mels)."""
     from . import models
 
     return ("pwg" if isinstance(model, models.ParallelWaveGANGenerator) else
             "style" if isinstance(model, models.StyleMelGANGenerator) else
             "units" if type(model) is models.DiscreteSymbolHiFiGANGenerator else
-            "uhifigan" if isinstance(model, models.UHiFiGANGenerator) else "mel2wav")
+            "uhifigan" if isinstance(model, models.UHiFiGANGenerator) else
+            "wav2wav" if isinstance(model, models.VQVAE) else "mel2wav")
+
+
+def _check_wav2wav(model):
+    """The VQ-VAE configurations ``convert`` serves: one audio channel in and out through the MelGAN encoder / decoder"""
+    from . import models
+
+    if not isinstance(model.encoder, models.MelGANDiscriminator) or not isinstance(model.decoder, models.MelGANGenerator):
+        raise PwgbError("Decoder: the VQ-VAE must have a MelGANDiscriminator encoder and a MelGANGenerator decoder")
+    if isinstance(list(model.decoder.melgan)[0], CausalConv1d):
+        raise PwgbError("Decoder: a causal VQ-VAE decoder (use_causal_conv=True) is not converted")
+    if model.decoder.pqmf is not None or [q for q in model.decoder.melgan if isinstance(q, torch.nn.Conv1d)][-1].out_channels > 1:
+        raise PwgbError("Decoder: out_channels > 1 (the reference's PQMF synthesis branch) is not converted")
+    if model.in_channels != 1:
+        raise PwgbError(f"Decoder: in_channels {model.in_channels}; convert takes one audio channel")
+
+
+def _pinned(t):
+    return t.pin_memory() if not t.is_cuda and not t.is_pinned() else t
+
+
+def _wave_row(x, i):
+    """one waveform, (T,) or (T, 1), as a (T,) float32 tensor on the host (or where it already is)"""
+    w = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.asarray(x, dtype=np.float32))
+    if w.dim() == 2 and w.shape[1] == 1:
+        w = w[:, 0]
+    if w.dim() != 1:
+        raise PwgbError(f"Decoder.convert: waveform {i} must be (T,) or (T, 1), got {tuple(w.shape)}")
+    return w.to(torch.float32).contiguous()
+
+
+def _cond_rows(model, locals, n, idxs, frames):
+    """the local conditioning of utterances ``idxs`` as {i: (T'_i, C) float32 host tensor}, or None for a model without"""
+    if not hasattr(model, "local_embed"):
+        if locals is not None:
+            raise PwgbError("Decoder.convert: the model has no local conditioning; locals must be None")
+        return None
+    if locals is None:
+        raise PwgbError("Decoder.convert: the model has local conditioning; locals=[...] (T'_i, num_local_embeds) are required")
+    if len(locals) != n:
+        raise PwgbError(f"Decoder.convert: {len(locals)} local tracks for {n} utterances")
+    C_in = model.local_embed.in_channels if model.local_embed is not None else None
+    rows = {}
+    for i in idxs:
+        l = torch.as_tensor(np.asarray(locals[i], dtype=np.float32) if not isinstance(locals[i], torch.Tensor) else locals[i])
+        l = l.to(torch.float32).cpu()
+        if l.dim() != 2 or l.shape[0] != frames[i] or (C_in is not None and l.shape[1] != C_in):
+            raise PwgbError(f"Decoder.convert: local track {i} is {tuple(l.shape)}; the encoder gives {frames[i]} frames "
+                            f"(ceil(samples / hop)){f' of {C_in} channels' if C_in is not None else ''}")
+        rows[i] = l
+    return rows
+
+
+def _speaker_ids(model, globals, n, idxs):
+    """the target speaker of utterances ``idxs`` as {i: int}, or None for a model without a global embedding"""
+    if not hasattr(model, "global_embed"):
+        if globals is not None:
+            raise PwgbError("Decoder.convert: the model has no global embedding; globals must be None")
+        return None
+    if globals is None:
+        raise PwgbError("Decoder.convert: the model has a global embedding; globals=[...] (one speaker id per utterance) are required")
+    if len(globals) != n:
+        raise PwgbError(f"Decoder.convert: {len(globals)} speaker ids for {n} utterances")
+    num = model.global_embed.num_embeddings
+    ids = {i: int(np.asarray(globals[i]).reshape(-1)[0]) if np.asarray(globals[i]).size == 1 else None for i in idxs}
+    bad = [i for i in idxs if ids[i] is None or not 0 <= ids[i] < num]
+    if bad:
+        raise PwgbError(f"Decoder.convert: utterances {bad} need one speaker id in [0, {num})")
+    return ids
 
 
 def _excitation_rows(excitations, mels, idxs, hop):

@@ -227,17 +227,22 @@ class ResidualStack(torch.nn.Module):
             )
         self.skip_layer = torch.nn.Conv1d(channels, channels, 1, bias=bias)
 
-    def forward(self, c):
+    def forward(self, c, mask=None):
+        """``mask``: the ragged-batch mask of ops.conv1d (centred only): each conv pads and zeroes each item at its end."""
         k, d = self.kernel_size, self.dilation
         sk = self.skip_layer
+        kw = {} if mask is None else {"mask": mask}
         if self.use_causal_conv:
+            if mask is not None:
+                raise PwgbError("ResidualStack: a ragged mask serves the centred stack")
             c2 = self.stack[3]
             h = self.stack[1](c, pre_slope=self.slope)
         else:
             c1, c2 = self.stack[2], self.stack[4]
-            h = ops.conv1d(c, effective_weight(c1), c1.bias, dilation=d, padding=(k - 1) // 2 * d, pad_mode=self.pad_mode, pre_slope=self.slope)
-        s = ops.conv1d(c, effective_weight(sk), sk.bias)
-        return ops.conv1d(h, effective_weight(c2), c2.bias, pre_slope=self.slope, residual=s)
+            h = ops.conv1d(c, effective_weight(c1), c1.bias, dilation=d, padding=(k - 1) // 2 * d, pad_mode=self.pad_mode, pre_slope=self.slope,
+                           **kw)
+        s = ops.conv1d(c, effective_weight(sk), sk.bias, **kw)
+        return ops.conv1d(h, effective_weight(c2), c2.bias, pre_slope=self.slope, residual=s, **kw)
 
 
 def pad_mode_of(pad, pad_params):

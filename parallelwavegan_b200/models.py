@@ -686,13 +686,25 @@ class MelGANGenerator(_GeneratorBase):
         self.reset_parameters()
         self.pqmf = None
 
-    def forward(self, c):
-        """(B, in_channels, T) -> (B, out_channels, T * prod(upsample_scales))  (melgan.py:168-178)."""
+    def forward(self, c, lengths=None):
+        """(B, in_channels, T) -> (B, out_channels, T * prod(upsample_scales))  (melgan.py:168-178).
+
+        ``lengths`` ((B,) int32 frame counts on the device, centred inference): a ragged batch.  Every conv keeps each
+        item +0.0 past its own end and pads it at its own end -- the reflect-padded input, stack and output convs reflect
+        there (pwgb_conv1d_ragged_forward) -- and each conv-transpose output is masked with one pwgb_stream_mask.  Every
+        sample of item b before lengths[b] * hop then equals ``forward`` of that item alone wherever both take the same
+        kernels (DESIGN.md §3.16)."""
         pad = (self.kernel_size - 1) // 2
         mods = list(self.melgan)
         n = len(mods)
         pre = 1.0  # slope of a pending activation, fused into the next conv's loader
         idx = 0
+        mask, rate = None, 1
+        if lengths is not None:
+            if isinstance(mods[0], CausalConv1d):
+                raise PwgbError("MelGANGenerator: per-item lengths serve the centred generator (use_causal_conv=False)")
+            mask = _length_mask(lengths, c.shape[0], rate)
+        kw = {} if mask is None else {"mask": mask}
         while idx < n:
             m = mods[idx]
             if isinstance(m, CausalConvTranspose1d):
@@ -707,13 +719,18 @@ class MelGANGenerator(_GeneratorBase):
                 c = ops.conv_transpose1d(c, effective_weight(m), m.bias, stride=s, padding=m.padding[0],
                                          output_padding=m.output_padding[0], pre_slope=pre)
                 pre = 1.0
+                if mask is not None:
+                    rate *= s
+                    mask = _length_mask(lengths, c.shape[0], rate)
+                    kw = {"mask": mask}
+                    ops.stream_mask(c, mask)
             elif isinstance(m, torch.nn.Conv1d):
                 final = idx >= n - 2
                 c = ops.conv1d(c, effective_weight(m), m.bias, padding=pad, pad_mode=self.pad_mode, pre_slope=pre,
-                               post_act="tanh" if (final and self.use_final_nonlinear_activation) else None)
+                               post_act="tanh" if (final and self.use_final_nonlinear_activation) else None, **kw)
                 pre = 1.0
             elif isinstance(m, ResidualStack):
-                c = m(c)
+                c = m(c, **kw)
             elif isinstance(m, (torch.nn.LeakyReLU, torch.nn.ReLU)):
                 pre = self.slope
             # padding modules and the final Tanh are fused into the neighbouring conv
@@ -1472,20 +1489,37 @@ class MelGANDiscriminator(torch.nn.Module):
         self.layers += [torch.nn.Conv1d(out_chs, out_channels, kernel_sizes[1], padding=(kernel_sizes[1] - 1) // 2, bias=bias)]
         self.reset_parameters()
 
-    def forward(self, x):
+    def forward(self, x, lengths=None):
+        """x (B, in_channels, T) -> the output of every layer.  ``lengths`` (a ragged batch): per-layer (B,) int32 device
+        tensors of each item's valid rows at that layer's output, ``layer_lengths(samples)``; every layer then keeps
+        each item +0.0 past its own end and pads it at its own end (pwgb_conv1d_ragged_forward)."""
         outs = []
+        if lengths is not None and len(lengths) != len(self.layers):
+            raise PwgbError(f"MelGANDiscriminator: {len(lengths)} layer lengths for {len(self.layers)} layers")
         for i, f in enumerate(self.layers):
+            kw = {} if lengths is None else {"mask": _length_mask(lengths[i], x.shape[0], 1)}
             if isinstance(f, torch.nn.Sequential):
                 m = [q for q in f if isinstance(q, torch.nn.Conv1d)][0]
                 first = i == 0
                 x = ops.conv1d(x, effective_weight(m), m.bias, stride=m.stride[0],
                                padding=(m.kernel_size[0] - 1) // 2 if first else m.padding[0],
                                pad_mode=self.pad_mode if first else "zero", groups=m.groups,
-                               post_act="lrelu", post_slope=self.slope)
+                               post_act="lrelu", post_slope=self.slope, **kw)
             else:
-                x = ops.conv1d(x, effective_weight(f), f.bias, padding=f.padding[0])
+                x = ops.conv1d(x, effective_weight(f), f.bias, padding=f.padding[0], **kw)
             outs += [x]
         return outs
+
+    def layer_lengths(self, lengths):
+        """Each item's valid rows after every layer, from its sample counts ``lengths`` (an int tensor on any device):
+        ceil(L / s) after a conv of stride s (output rows (L + 2 * 5s - (10s + 1)) // s + 1), unchanged otherwise."""
+        out, L = [], lengths
+        for f in self.layers:
+            m = [q for q in f if isinstance(q, torch.nn.Conv1d)][0] if isinstance(f, torch.nn.Sequential) else f
+            s = m.stride[0]
+            L = torch.div(L + (s - 1), s, rounding_mode="floor") if s > 1 else L
+            out.append(L)
+        return out
 
     def reset_parameters(self):
         def _reset_parameters(m):
@@ -1684,17 +1718,68 @@ class VQVAE(torch.nn.Module):
         dec, z_q, _ = ops.vq(z_e, self.codebook.embedding.weight, l=l, global_table=gt, g=g)
         return self.decoder(dec), z_e, z_q
 
-    def encode(self, x):
-        """x (B, in_channels, T) -> codebook indices (B, T')  (vqvae.py:112-125)."""
-        return self.codebook(self._encode(x))
+    def encode(self, x, lengths=None):
+        """x (B, in_channels, T) -> codebook indices (B, T')  (vqvae.py:112-125).
 
-    def decode(self, indices, l=None, g=None):
-        """indices (B, T') int64 -> (B, out_channels, T)  (vqvae.py:127-147): gather and assembly only."""
+        ``lengths`` ((B,) int32 sample counts on the device): a ragged batch, x padded past each item's end.  Item b's
+        first ceil(lengths[b] / hop) indices equal ``encode`` of that item alone (DESIGN.md §3.16); the later ones are
+        the codes of zero frames, to be cropped."""
+        if lengths is None:
+            return self.codebook(self._encode(x))
+        self._check_ragged(lengths, x.shape[-1], self.min_ragged_samples(), "encode")
+        return self.codebook(self.encoder(x, self.encoder.layer_lengths(lengths))[-1])
+
+    def decode(self, indices, l=None, g=None, lengths=None):
+        """indices (B, T') int64 -> (B, out_channels, T)  (vqvae.py:127-147): gather and assembly only.
+
+        ``lengths`` ((B,) int32 frame counts on the device): a ragged batch.  Indices past an item's end must still be
+        codes (0 will do); samples before lengths[b] * hop equal ``decode`` of that item alone, the later ones are +0.0."""
+        if lengths is not None:
+            self._check_ragged(lengths, indices.shape[-1], self.min_ragged_frames(), "decode")
+        return self._decode(indices, l, g, lengths)
+
+    def _decode(self, indices, l, g, lengths):
         if l is not None:
             l = self._local(l)
         gt, g = self._global(g)
         _, _, dec = ops.vq_raw(None, self.codebook.embedding.weight, indices=indices, z_q=False, dec=True, l=l, global_table=gt, g=g)
-        return self.decoder(dec)
+        return self.decoder(dec) if lengths is None else self.decoder(dec, lengths)
+
+    @property
+    def hop(self):
+        """Samples per code frame: the encoder's total stride."""
+        return int(np.prod([f[0].stride[0] for f in self.encoder.layers[1:-2]]))
+
+    def min_ragged_frames(self):
+        """The fewest code frames a ragged decode takes: every reflect-padded conv of the decoder needs its pad < the
+        item's length at its rate (ReflectionPad1d)."""
+        dec = self.decoder
+        need, rate = [(dec.kernel_size - 1) // 2 + 1], 1  # the input conv
+        for m in dec.melgan:
+            if isinstance(m, torch.nn.ConvTranspose1d):
+                rate *= m.stride[0]
+            elif isinstance(m, ResidualStack):
+                need.append(-(-((m.kernel_size - 1) // 2 * m.dilation + 1) // rate))
+        need.append(-(-((dec.kernel_size - 1) // 2 + 1) // rate))  # the output conv
+        return max(need)
+
+    def min_ragged_samples(self):
+        """The shortest utterance a ragged batch converts: the encoder's reflect-padded input conv needs its pad < the
+        length, and the decoder ``min_ragged_frames`` frames of ceil(length / hop)."""
+        c0 = [q for q in self.encoder.layers[0] if isinstance(q, torch.nn.Conv1d)][0]
+        return max((c0.kernel_size[0] - 1) // 2 + 1, (self.min_ragged_frames() - 1) * self.hop + 1)
+
+    def _check_ragged(self, lengths, T, least, what):
+        """the argument checks of a ragged encode / decode; the lengths are read on the host outside graph capture"""
+        if not isinstance(self.encoder, MelGANDiscriminator) or not isinstance(self.decoder, MelGANGenerator):
+            raise PwgbError("VQVAE: per-item lengths serve the MelGANDiscriminator encoder and MelGANGenerator decoder")
+        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            raise PwgbError(f"VQVAE.{what}: per-item lengths are an inference feature (run under torch.no_grad)")
+        if torch.cuda.is_current_stream_capturing():
+            return
+        host = [int(v) for v in lengths.tolist()]
+        if any(L < least or L > T for L in host):
+            raise PwgbError(f"VQVAE.{what}: lengths {host} must lie in [{least}, {T}] (the reflect pads need at least {least})")
 
     def apply_weight_norm(self):
         def _apply_weight_norm(m):

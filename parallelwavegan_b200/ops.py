@@ -111,12 +111,18 @@ def conv1d_raw(
     out=None,
     accumulate=False,
     period=1,
+    mask=None,
 ):
     """y = [y +] out_scale * (act(conv(pre(x)) + bias) + residual)   -- pwgb_conv1d_forward.
 
     ``padding``: int or (left, right) rows.  ``period`` > 1 treats x as the
     (B, C, ceil(L/P), P) view of HiFiGANPeriodDiscriminator (reflect-extended to a
-    multiple of P, hifigan.py:365-369) and returns a 4-D tensor."""
+    multiple of P, hifigan.py:365-369) and returns a 4-D tensor.
+
+    ``mask`` = (frame, end, rate, 0) of a ragged batch (pwgb_conv1d_ragged_forward / pwgb_conv1d_tc_ragged_forward):
+    item b holds end[b] * rate valid output rows, its pad is applied at its own end (``pad_mode`` as the edge), and its
+    rows past the end are +0.0.  The zero pad needs x zero past each item's input length; reflect needs padding <
+    every item's length (the caller checks it)."""
     x = _dev(x, "x")
     w = _dev(w, "w")
     if w.dim() == 4:  # Conv2d (k, 1) weights of the period discriminators
@@ -179,13 +185,24 @@ def conv1d_raw(
                  4.0 * (x.numel() + out.numel() * (2 if accumulate else 1) + (residual.numel() if residual is not None else 0)),
                  f"B{B} cin{cin} cout{cout} k{K} d{dilation} s{stride} g{groups} T{t_out}" if PROFILE is not None else "")
     L = capi.lib()
+    ext = None
+    if mask is not None:
+        if P != 1:
+            raise PwgbError("conv1d: a ragged mask needs period 1")
+        ext = _stream_ext(B, cout, mask, None, 0, edge=pad_mode if pad_mode != "zeros" else "zero")
     if ENGINE != "simt" and L.pwgb_conv1d_tc_supported(C.byref(d)):
         pk = packed_weight(w, groups)
         prof.name = "conv1d_tc"
-        rc = L.pwgb_conv1d_tc_forward(C.byref(d), _p(x), _p(pk), _p(bias), _p(residual), _p(out), _stream())
+        if ext is not None:
+            rc = L.pwgb_conv1d_tc_ragged_forward(C.byref(d), _p(x), _p(pk), _p(bias), _p(residual), C.byref(ext), _p(out), _stream())
+        else:
+            rc = L.pwgb_conv1d_tc_forward(C.byref(d), _p(x), _p(pk), _p(bias), _p(residual), _p(out), _stream())
         capi.check(rc, "pwgb_conv1d_tc_forward")
     else:
-        rc = L.pwgb_conv1d_forward(C.byref(d), _p(x), _p(w), _p(bias), _p(residual), _p(out), _stream())
+        if ext is not None:
+            rc = L.pwgb_conv1d_ragged_forward(C.byref(d), _p(x), _p(w), _p(bias), _p(residual), C.byref(ext), _p(out), _stream())
+        else:
+            rc = L.pwgb_conv1d_forward(C.byref(d), _p(x), _p(w), _p(bias), _p(residual), _p(out), _stream())
         capi.check(rc, "pwgb_conv1d_forward")
     prof.done()
     return out
@@ -1496,6 +1513,8 @@ def conv1d(x, w, bias=None, **kw):
     if y is not None:
         return y
     if _needs_grad(x, w, bias, kw.get("residual")):
+        if kw.get("mask") is not None:
+            raise PwgbError("conv1d: a ragged mask has no backward (run under torch.no_grad)")
         from . import autograd as ag
 
         return ag.conv1d(x, w, bias, **kw)
