@@ -24,7 +24,9 @@ graph per (batch, padded length) serves every mix of lengths, which are a static
 HiFi-GAN needs the padding only.
 
 The discrete-symbol HiFi-GAN decodes units: each input is a (T, 2) (symbol, speaker) or (T, 1) index array, padded
-with symbol 0 past its end (and its own speaker).
+with symbol 0 past its end (and its own speaker).  The discrete-symbol StyleMelGAN decodes units one utterance at a
+time through ``inference``, like StyleMelGAN (its InstanceNorm takes statistics over the whole signal, so padding
+would change every item): (T, 2) units, or (T, 1) units with ``speakers=[...]``.
 
 The U-Net HiFi-GAN decodes mels with their excitations (bin/decode.py:156-230): ``decode(mels, excitations=...)``, one
 (T', hop) or (T' * hop,) excitation per utterance, which crosses PCIe once from pinned memory into its batch slot and is
@@ -124,6 +126,7 @@ def ragged_refusal(model):
                                 "synthesis looks ahead), which a zero-padded batch cannot reproduce per item",
         models.ParallelWaveGANGenerator: "the fused WaveNet stack of Parallel WaveGAN has no per-item length mask",
         models.StyleMelGANGenerator: "StyleMelGAN's InstanceNorm takes statistics over the whole signal",
+        models.DiscreteSymbolStyleMelGANGenerator: "StyleMelGAN's InstanceNorm takes statistics over the whole signal",
         models.UHiFiGANGenerator: "the U-Net HiFi-GAN's strided encoder and excitation input have no per-item length mask",
         models.DiscreteSymbolDurationGenerator: "the duration model's regulated length is only known after its predictor runs",
     }
@@ -210,14 +213,19 @@ class Decoder:
                 yield key, g[k : k + self.max_batch]
 
     @torch.no_grad()
-    def decode(self, mels, normalize_before=False, to_pcm16=True, noises=None, excitations=None):
-        """mels: list of (T_i, C) arrays / tensors.  Returns {index: waveform}: int16 numpy arrays of shape (samples,)
-        (``to_pcm16``) or float32 device tensors (samples, out_channels).  ``noises`` (Parallel WaveGAN only): optional
-        {index: (samples, 1)} noise for reproducibility (``inference(c, x)``).  ``excitations`` (the U-Net HiFi-GAN
-        only, and required there): a list aligned with ``mels``, entry i (T_i, hop) or (T_i * hop,)."""
+    def decode(self, mels, normalize_before=False, to_pcm16=True, noises=None, excitations=None, speakers=None):
+        """mels: list of (T_i, C) arrays / tensors (units for the discrete-symbol generators).  Returns {index:
+        waveform}: int16 numpy arrays of shape (samples,) (``to_pcm16``) or float32 device tensors (samples,
+        out_channels).  ``noises`` (Parallel WaveGAN only): optional {index: (samples, 1)} noise for reproducibility
+        (``inference(c, x)``).  ``excitations`` (the U-Net HiFi-GAN only, and required there): a list aligned with
+        ``mels``, entry i (T_i, hop) or (T_i * hop,).  ``speakers`` (the discrete-symbol StyleMelGAN only): a list
+        aligned with ``mels`` of speaker ids, which replace the units' speaker column as ``inference(c, g)`` does;
+        without it every utterance is (T_i, 2) (symbol, speaker)."""
         m = self.model
         if self.kind == "wav2wav":
             raise PwgbError("Decoder: a VQ-VAE converts waveforms; use Decoder.convert(waves, locals, globals)")
+        if speakers is not None and self.kind != "style_units":
+            raise PwgbError(f"Decoder: speakers are an input of the discrete-symbol StyleMelGAN only, not of {type(m).__name__}")
         idxs = list(sharding.partition(len(mels), self.rank, self.world))
         exc = None
         if self.kind == "uhifigan":
@@ -227,6 +235,19 @@ class Decoder:
             exc = _excitation_rows(excitations, mels, idxs, self.hop)
         elif excitations is not None:
             raise PwgbError(f"Decoder: excitations are an input of the U-Net HiFi-GAN only, not of {type(m).__name__}")
+        if self.kind == "style_units":  # batch-1 inference, as the "style" kind, on units
+            if normalize_before:
+                raise PwgbError("Decoder: units are not normalised (normalize_before=False)")
+            if noises is not None:
+                raise PwgbError("Decoder: the discrete-symbol StyleMelGAN draws its noise in inference (style_melgan.py:588-595); "
+                                "noises are an input of Parallel WaveGAN only")
+            spk = _speaker_list(speakers, len(mels), idxs, m.num_spk_embs)
+            out = {}
+            for i in idxs:
+                u = _unit_rows(mels[i], speakers=spk is None).to(self.dev)
+                y = m.inference(u, g=None if spk is None else spk[i])
+                out[i] = pcm16(y[:, 0]).cpu().numpy() if to_pcm16 else y
+            return out
         if self.kind == "style":  # batch-1 inference with its own noise / padding protocol (style_melgan.py:226-262)
             out = {}
             for i in idxs:
@@ -367,12 +388,13 @@ class Decoder:
 
 
 def decoder_kind(model):
-    """How ``Decoder`` feeds a generator: "pwg" (noise and mels), "style" (per-utterance inference), "units" (the
-    discrete-symbol HiFi-GAN), "uhifigan" (mels and excitation), "wav2wav" (the VQ-VAE: waveforms, ``convert``) or
-    "mel2wav" (mels)."""
+    """How ``Decoder`` feeds a generator: "pwg" (noise and mels), "style" (per-utterance inference), "style_units"
+    (per-utterance inference of the discrete-symbol StyleMelGAN on units), "units" (the discrete-symbol HiFi-GAN),
+    "uhifigan" (mels and excitation), "wav2wav" (the VQ-VAE: waveforms, ``convert``) or "mel2wav" (mels)."""
     from . import models
 
     return ("pwg" if isinstance(model, models.ParallelWaveGANGenerator) else
+            "style_units" if isinstance(model, models.DiscreteSymbolStyleMelGANGenerator) else
             "style" if isinstance(model, models.StyleMelGANGenerator) else
             "units" if type(model) is models.DiscreteSymbolHiFiGANGenerator else
             "uhifigan" if isinstance(model, models.UHiFiGANGenerator) else
@@ -437,14 +459,7 @@ def _speaker_ids(model, globals, n, idxs):
         return None
     if globals is None:
         raise PwgbError("Decoder.convert: the model has a global embedding; globals=[...] (one speaker id per utterance) are required")
-    if len(globals) != n:
-        raise PwgbError(f"Decoder.convert: {len(globals)} speaker ids for {n} utterances")
-    num = model.global_embed.num_embeddings
-    ids = {i: int(np.asarray(globals[i]).reshape(-1)[0]) if np.asarray(globals[i]).size == 1 else None for i in idxs}
-    bad = [i for i in idxs if ids[i] is None or not 0 <= ids[i] < num]
-    if bad:
-        raise PwgbError(f"Decoder.convert: utterances {bad} need one speaker id in [0, {num})")
-    return ids
+    return _speaker_list(globals, n, idxs, model.global_embed.num_embeddings, "Decoder.convert")
 
 
 def _excitation_rows(excitations, mels, idxs, hop):
@@ -464,6 +479,20 @@ def _excitation_rows(excitations, mels, idxs, hop):
             raise PwgbError(f"Decoder: excitation {i} has {e.numel()} samples, its {want // hop} frames need {want} (hop {hop})")
         rows[i] = e.contiguous()
     return rows
+
+
+def _speaker_list(speakers, n, idxs, num_spk, who="Decoder"):
+    """The speaker ids of utterances ``idxs`` as {i: int}, each checked against the table size, or None without
+    ``speakers``"""
+    if speakers is None:
+        return None
+    if len(speakers) != n:
+        raise PwgbError(f"{who}: {len(speakers)} speaker ids for {n} utterances")
+    ids = {i: int(np.asarray(speakers[i]).reshape(-1)[0]) if np.asarray(speakers[i]).size == 1 else None for i in idxs}
+    bad = [i for i in idxs if ids[i] is None or not 0 <= ids[i] < num_spk]
+    if bad:
+        raise PwgbError(f"{who}: utterances {bad} need one speaker id in [0, {num_spk})")
+    return ids
 
 
 def _unit_rows(x, speakers):

@@ -781,9 +781,18 @@ class StyleMelGANGenerator(_GeneratorBase):
     ):
         super().__init__()
         self.in_channels = in_channels
+        self._build(aux_channels, channels, out_channels, kernel_size, dilation, bias, noise_upsample_scales, noise_upsample_activation,
+                    noise_upsample_activation_params, upsample_scales, upsample_mode, gated_function)
+        if use_weight_norm:
+            self.apply_weight_norm()
+        self.reset_parameters()
+
+    def _build(self, aux_channels, channels, out_channels, kernel_size, dilation, bias, noise_upsample_scales, noise_upsample_activation,
+               noise_upsample_activation_params, upsample_scales, upsample_mode, gated_function):
+        """noise_upsample, blocks and output_conv (style_melgan.py:62-131), registered in the reference's order."""
         self.noise_slope = activation_slope(noise_upsample_activation, noise_upsample_activation_params)
         noise_upsample = []
-        in_chs = in_channels
+        in_chs = self.in_channels
         for s in noise_upsample_scales:
             noise_upsample += [torch.nn.ConvTranspose1d(in_chs, channels, s * 2, stride=s, padding=s // 2 + s % 2,
                                                         output_padding=s % 2, bias=bias)]
@@ -803,9 +812,6 @@ class StyleMelGANGenerator(_GeneratorBase):
             torch.nn.Conv1d(channels, out_channels, kernel_size, 1, bias=bias, padding=(kernel_size - 1) // 2),
             torch.nn.Tanh(),
         )
-        if use_weight_norm:
-            self.apply_weight_norm()
-        self.reset_parameters()
 
     def _noise_path(self, z):
         """noise_upsample (style_melgan.py:76-98): every LeakyReLU but the last is fused into the next
@@ -818,15 +824,18 @@ class StyleMelGANGenerator(_GeneratorBase):
                 pre = self.noise_slope
         return ops.leaky_relu(x, self.noise_slope, inplace=True)
 
-    def forward(self, c, z=None):
-        """(B, aux_channels, T) [, (B, in_channels, T_z)] -> (B, out_channels, T * prod(upsample_scales))  (style_melgan.py:140-160)."""
-        if z is None:
-            z = torch.randn(c.size(0), self.in_channels, 1).to(device=c.device, dtype=c.dtype)
-        x = self._noise_path(z)
+    def _body(self, x, c):
+        """The TADE blocks and the output conv -> tanh on the noise path's x and the conditioning c (style_melgan.py:155-159)."""
         for block in self.blocks:
             x, c = block(x, c)
         oc = self.output_conv[0]
         return ops.conv1d(x, effective_weight(oc), oc.bias, padding=(self.kernel_size - 1) // 2, post_act="tanh")
+
+    def forward(self, c, z=None):
+        """(B, aux_channels, T) [, (B, in_channels, T_z)] -> (B, out_channels, T * prod(upsample_scales))  (style_melgan.py:140-160)."""
+        if z is None:
+            z = torch.randn(c.size(0), self.in_channels, 1).to(device=c.device, dtype=c.dtype)
+        return self._body(self._noise_path(z), c)
 
     def apply_weight_norm(self):
         def _apply_weight_norm(m):
@@ -853,11 +862,106 @@ class StyleMelGANGenerator(_GeneratorBase):
         total_length = c.size(2) * self.upsample_factor
         if x.size(2) > c.size(2):  # replicate-pad the conditioning up to the noise length (data movement)
             c = torch.cat([c, c[:, :, -1:].expand(-1, -1, x.size(2) - c.size(2))], dim=2).contiguous()
-        for block in self.blocks:
-            x, c = block(x, c)
-        oc = self.output_conv[0]
-        y = ops.conv1d(x, effective_weight(oc), oc.bias, padding=(self.kernel_size - 1) // 2, post_act="tanh")[..., :total_length]
+        y = self._body(x, c)[..., :total_length]
         return y.squeeze(0).transpose(1, 0)
+
+
+class DiscreteSymbolStyleMelGANGenerator(torch.nn.Module):
+    """models/style_melgan.py:364-602: StyleMelGAN over discrete units (HuBERT codes).  The symbol embedding plus the
+    speaker embedding of each item's first frame is the conditioning, written channel-major by one embed launch
+    (pwgb_symbol_embed_forward) that reads the index tensor in place; the noise path and the body are
+    StyleMelGANGenerator's.  ``inference`` crops the upsampled noise to the T frames of the units instead of padding the
+    conditioning, so the first block's InstanceNorm sees exactly T frames, as in the reference.  There is no
+    ``register_stats``, as in the reference."""
+
+    def __init__(
+        self,
+        in_channels=128,
+        aux_channels=128,
+        channels=64,
+        out_channels=1,
+        num_embs=100,
+        num_spk_embs=128,
+        spk_emb_dim=128,
+        concat_spk_emb=False,
+        kernel_size=9,
+        dilation=2,
+        bias=True,
+        noise_upsample_scales=[11, 2, 2, 2],
+        noise_upsample_activation="LeakyReLU",
+        noise_upsample_activation_params={"negative_slope": 0.2},
+        upsample_scales=[2, 2, 2, 2, 2, 2, 2, 2, 1],
+        upsample_mode="nearest",
+        gated_function="softmax",
+        use_weight_norm=True,
+    ):
+        super().__init__()
+        self.in_channels = in_channels
+        self.num_spk_embs = num_spk_embs
+        self.emb = torch.nn.Embedding(num_embeddings=num_embs, embedding_dim=aux_channels)
+        self.spk_emb = torch.nn.Embedding(num_embeddings=num_spk_embs, embedding_dim=spk_emb_dim)
+        self.concat_spk_emb = concat_spk_emb
+        if not concat_spk_emb:
+            assert aux_channels == spk_emb_dim
+        else:
+            aux_channels = aux_channels + spk_emb_dim
+        self._build(aux_channels, channels, out_channels, kernel_size, dilation, bias, noise_upsample_scales, noise_upsample_activation,
+                    noise_upsample_activation_params, upsample_scales, upsample_mode, gated_function)
+        if use_weight_norm:
+            self.apply_weight_norm()
+        self.reset_parameters()
+
+    remove_weight_norm = _GeneratorBase.remove_weight_norm
+    _build = StyleMelGANGenerator._build
+    apply_weight_norm = StyleMelGANGenerator.apply_weight_norm
+    reset_parameters = StyleMelGANGenerator.reset_parameters
+    _noise_path = StyleMelGANGenerator._noise_path
+    _body = StyleMelGANGenerator._body
+    _prep_symbols = DiscreteSymbolHiFiGANGenerator._prep_symbols
+
+    def _check_input(self, c):
+        assert c.size(1) == 2
+        if self.concat_spk_emb:
+            # style_melgan.py:493-495 concatenates the speaker embedding along time, so the first TADE aux conv, built
+            # for aux_channels + spk_emb_dim, receives aux_channels: the reference fails there; so does the mirror
+            raise PwgbError(f"concat_spk_emb=True: the first TADE aux conv expects {self.blocks[0].tade1.aux_conv[0].in_channels} "
+                            f"channels, the embedding has {self.emb.embedding_dim} (the reference concatenates the speaker "
+                            f"embedding along time)")
+
+    def _embed(self, c):
+        """(B, 2, T) symbol and speaker indices of any dtype -> (B, aux_channels, T) conditioning (see ops.symbol_embed)."""
+        return ops.symbol_embed(c, self.emb.weight, self.spk_emb.weight)
+
+    def forward(self, c, z=None):
+        """c (B, 2, T) (symbol, speaker id) [, z (B, in_channels, T_z)] -> (B, out_channels, T * prod(upsample_scales))
+        (style_melgan.py:474-508).  The noise path makes T_z * noise_upsample_factor frames and nothing crops it, so T
+        must equal that (the default z has T_z = 1)."""
+        self._check_input(c)
+        if z is None:
+            z = torch.randn(c.size(0), self.in_channels, 1).to(device=c.device, dtype=torch.float32)
+        if c.size(2) != z.size(2) * self.noise_upsample_factor:
+            raise PwgbError(f"{c.size(2)} frames of units, but the noise path makes {z.size(2) * self.noise_upsample_factor} "
+                            f"({z.size(2)} noise frames x {self.noise_upsample_factor}); forward neither crops nor pads")
+        return self._body(self._noise_path(z), self._embed(c))
+
+    def inference(self, c, g=None, normalize_before=False, noise=None):
+        """(T, 2) indices, or (T, 1) with a speaker id ``g`` -> (T * prod(upsample_scales), out_channels)
+        (style_melgan.py:563-602).  ``noise`` (1, in_channels, (T - 1) // noise_upsample_factor + 1) may be passed for
+        reproducibility; the upsampled noise is cropped to T frames."""
+        assert not normalize_before, "No statistics are used."
+        c = self._prep_symbols(c, g)
+        self._check_input(c)
+        T = c.size(2)
+        n_frames = (T - 1) // self.noise_upsample_factor + 1
+        if noise is None:
+            noise = torch.randn(1, self.in_channels, n_frames, dtype=torch.float).to(c.device)
+        elif tuple(noise.shape) != (1, self.in_channels, n_frames):
+            raise PwgbError(f"inference: noise must be {(1, self.in_channels, n_frames)} for {T} frames, got {tuple(noise.shape)}")
+        e = self._embed(c)
+        x = self._noise_path(noise.contiguous())
+        if x.size(2) > T:  # crop the noise path to the units (data movement)
+            x = x[:, :, :T].contiguous()
+        return self._body(x, e).squeeze(0).transpose(1, 0)
 
 
 class ParallelWaveGANGenerator(_GeneratorBase):

@@ -7,9 +7,13 @@
   the time of the embed kernel alone against the whole forward;
 * one GanTrainStep of the cvss_c duration recipe (egs/cvss_c/hubert_voc1/conf/hifigan_hubert_duration.v1.yaml) at
   its batch (16 x 10240 samples) from the device duration collater: ms per step (host clock around synchronised steps);
+* ``inference`` of the vctk HuBERT StyleMelGAN recipe's generator (egs/vctk/hubert_voc1/conf/style_melgan_hubert.v1.yaml:
+  64 channels, noise scales 7 2 2 2, scales 5 2 2 2 2 2 2 1 1; weight norm removed, eval mode) on one utterance of 250
+  frames (5 s at 16 kHz) with its noise on the device: ms per call from device events with the L2 flushed before each
+  call, and libpwgb launches per call;
 * the card's name and power limit, read in the same call.
 
-    python tools/dsym_bench.py [--steps 10] [--warmup 3]
+    python tools/dsym_bench.py [--steps 10] [--warmup 3] [--cases inference,train,style]
 """
 import argparse
 import json
@@ -33,6 +37,10 @@ VCTK = dict(in_channels=512, out_channels=1, channels=512, num_embs=100, num_spk
 CVSS = dict(in_channels=512, out_channels=1, channels=512, num_embs=500, kernel_size=7, upsample_scales=[10, 8, 2, 2],
             upsample_kernel_sizes=[20, 16, 4, 4], duration_layers=2, duration_chans=384, duration_kernel_size=3, duration_offset=1.0,
             duration_dropout_rate=0.5, num_spk_embs=0, **RES)
+STYLE = dict(in_channels=128, aux_channels=128, channels=64, out_channels=1, num_embs=100, num_spk_embs=128, spk_emb_dim=128,
+             concat_spk_emb=False, kernel_size=9, dilation=2, bias=True, noise_upsample_scales=[7, 2, 2, 2],
+             noise_upsample_activation="LeakyReLU", noise_upsample_activation_params={"negative_slope": 0.2},
+             upsample_scales=[5, 2, 2, 2, 2, 2, 2, 1, 1], upsample_mode="nearest", gated_function="softmax", use_weight_norm=True)
 HOP = 320
 
 
@@ -106,11 +114,38 @@ def train_step(args, dev):
             "ms_per_step": round(ms, 2), "duration_loss": float(stats["duration_loss"]), "generator_loss": float(stats["generator_loss"])}
 
 
+def style_inference(args, dev, flush):
+    from oracle import synth
+    from parallelwavegan_b200 import capi, models
+
+    m = models.DiscreteSymbolStyleMelGANGenerator(**STYLE)
+    m.load_state_dict(synth.synth_state_dict([(k, tuple(v.shape)) for k, v in m.state_dict().items()], 64, 1.0))
+    m.remove_weight_norm()
+    m = m.to(dev).eval()
+    rng = np.random.RandomState(2)
+    F = 250
+    c = np.stack([rng.randint(0, 100, size=F), np.full(F, 7)], axis=1)
+    c = torch.from_numpy(c).to(dev)
+    noise = torch.randn(1, 128, (F - 1) // 56 + 1, generator=torch.Generator().manual_seed(3)).to(dev)
+    with torch.no_grad():
+        m.inference(c, noise=noise)
+        torch.cuda.synchronize()
+        capi.reset_launch_count()
+        m.inference(c, noise=noise)
+        torch.cuda.synchronize()
+        launches = capi.launch_count()
+        (ms,) = timed([lambda: m.inference(c, noise=noise)], args.steps, args.warmup, flush)
+    return {"workload": f"vctk hubert StyleMelGAN inference, one utterance of {F} frames (hop {HOP}), eval, weight norm removed",
+            "ms_per_inference": round(ms, 3), "samples_per_s": round(F * HOP / (ms / 1e3)), "launches_per_inference": launches}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--cases", default="inference,train,style")
     args = ap.parse_args()
+    cases = args.cases.split(",")
     if not torch.cuda.is_available():
         raise SystemExit("dsym_bench: needs a CUDA device (no CPU measurement)")
     import __graft_entry__
@@ -118,10 +153,12 @@ def main():
     __graft_entry__.build()
     dev = torch.device("cuda:0")
     flush = torch.empty(256 * 1024 * 1024 // 4, device=dev)
-    line = {"inference": inference(args, dev, flush), "train": train_step(args, dev),
-            "timing": f"inference: device events, mean of {args.steps} steps after {args.warmup} warm-up, L2 flushed (256 MiB write) "
-                      f"before each; train: host clock over {args.steps} synchronised steps after {args.warmup} warm-up",
-            "gpu": card()}
+    runs = {"inference": lambda: inference(args, dev, flush), "train": lambda: train_step(args, dev),
+            "style": lambda: style_inference(args, dev, flush)}
+    line = {k: runs[k]() for k in cases}
+    line["timing"] = (f"inference, style: device events, mean of {args.steps} steps after {args.warmup} warm-up, L2 flushed (256 MiB "
+                      f"write) before each; train: host clock over {args.steps} synchronised steps after {args.warmup} warm-up")
+    line["gpu"] = card()
     print(json.dumps(line), flush=True)
 
 
