@@ -121,8 +121,9 @@ PWGB_API int pwgb_conv_transpose1d_cat_forward(const pwgb_convtr1d_desc* d, int 
 /* ------------------------------------------------------------------------
  * Dropout in training mode (torch.nn.Dropout(p); models/uhifigan.py input / downsample convs) over n elements.
  * Element e is kept when word e % 4 of Philox4x32-10(counter = (e / 4, offset), key = seed), as a 24-bit uniform in
- * [0, 1), is >= p; kept elements are multiplied by 1 / (1 - p) computed in fp32, the others are 0.  p == 0 is the
- * identity.  The backward recomputes the same mask from (seed, offset): gx = mask * gy / (1 - p).
+ * [0, 1), is >= p; kept elements are multiplied by 1 / (1 - p) computed in fp32, the others are +0.0 (also when the
+ * input is -0.0, +-inf or NaN).  p == 0 is the identity; p == 1 gives all +0.0; p outside [0, 1] or NaN is refused.
+ * The backward recomputes the same mask from (seed, offset): gx = mask * gy / (1 - p).
  * ---------------------------------------------------------------------- */
 PWGB_API int pwgb_dropout_forward(const float* x, float* y, long long n, float p, unsigned long long seed,
                                   unsigned long long offset, void* stream);
@@ -437,7 +438,8 @@ PWGB_API int pwgb_collate_crop(const float* audio, const long long* x_offsets, c
  *   out[ch, u] = (c[u - pad_left, ch] - mean[ch]) / scale[ch]  (mean/scale NULL: no normalisation; hifigan.py:264-265),
  *   frames outside [0, t) zero (pad_mode PWGB_PAD_ZERO) or edge-replicated (PWGB_PAD_REPLICATE,
  *   parallel_wavegan.py:250-251).  `out` is usually one batch slot of the generator input.
- * pwgb_pcm16_forward: lrintf(y * 32767) saturated to int16 -- libsndfile's float -> PCM_16 (decode.py:236-241).
+ * pwgb_pcm16_forward: lrintf(y * 32767) saturated to int16 -- libsndfile's float -> PCM_16 (decode.py:236-241);
+ *   the product in fp32, ties to even, +-inf saturate, NaN -> 0.
  * ---------------------------------------------------------------------- */
 PWGB_API int pwgb_prep_features(const float* c, const float* mean, const float* scale, float* out, int t, int channels, int pad_left,
                        int t_out, int pad_mode, void* stream);

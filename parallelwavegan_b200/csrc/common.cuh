@@ -47,6 +47,22 @@ inline int check_launch(const char* what) {
 
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
+// A kernel may use 48 KB of shared memory, static and dynamic together, unless it opts in to more: opt in to `dyn`
+// dynamic bytes whenever they and the kernel's static arrays together pass 48 KB.
+template <typename Kernel>
+static int allow_dynamic_smem(Kernel kernel, size_t dyn, const char* what) {
+  if (dyn <= 32 * 1024) return PWGB_OK;  // far below the limit: skip the attribute query
+  cudaFuncAttributes a;
+  cudaError_t e = cudaFuncGetAttributes(&a, kernel);
+  if (e == cudaSuccess && dyn + a.sharedSizeBytes > 48 * 1024)
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
+  if (e != cudaSuccess) {
+    set_error("%s: shared memory opt-in: %s", what, cudaGetErrorString(e));
+    return PWGB_CUDA_ERROR;
+  }
+  return PWGB_OK;
+}
+
 // the two history padding policies of the stream entry points (flagged slots replicate or reflect)
 __host__ __device__ inline bool is_history_pad(int pad_mode) {
   return pad_mode == PWGB_PAD_HISTORY || pad_mode == PWGB_PAD_HISTORY_REFLECT;

@@ -37,11 +37,12 @@ __global__ void prep_features_kernel(const float* __restrict__ c, const float* _
 
 // libsndfile's float -> PCM_16 conversion as used by sf.write(..., "PCM_16") (decode.py:236-241): lrintf(y * 32767),
 // saturated to the int16 range (libsndfile wraps out-of-range values unless clipping is enabled; generators end in tanh).
+// The product is one fp32 multiply and rintf rounds half to even.  A NaN sample becomes 0: silence rather than a
+// full-scale click (fmaxf would turn it into -32768), and what libsndfile's lrintf gives once cut to 16 bits on x86-64.
 __global__ void pcm16_kernel(const float* __restrict__ y, short* __restrict__ out, long long n) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    float v = rintf(y[i] * 32767.f);
-    v = fminf(fmaxf(v, -32768.f), 32767.f);
-    out[i] = (short)v;
+    const float v = rintf(y[i] * 32767.f);
+    out[i] = v != v ? (short)0 : (short)fminf(fmaxf(v, -32768.f), 32767.f);
   }
 }
 

@@ -2,6 +2,9 @@
 // counter-based mask: element e is kept when word e % 4 of Philox4x32-10(counter = (e / 4, offset), key = seed),
 // read as a 24-bit uniform in [0, 1), is >= p.  The mask is a pure function of (seed, offset, e), so the backward
 // recomputes it and no mask tensor is stored.  Kept elements are scaled by 1 / (1 - p), computed in fp32.
+// A dropped element is +0.0 whatever its input (-0.0, +-inf and NaN included); a kept one is exactly v * scale, so
+// non-finite inputs stay non-finite and -0.0 stays -0.0.  At p == 1 every element is dropped (u < 1): all +0.0, no NaN.
+// p outside [0, 1] or NaN is refused.
 #include "common.cuh"
 
 namespace pwgb {

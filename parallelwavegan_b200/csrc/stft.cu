@@ -386,22 +386,8 @@ __global__ void stft_loss_dmag_kernel(const float* __restrict__ xm, const float*
   }
 }
 
-// A kernel may use 48 KB of shared memory, static and dynamic together, unless it opts in to more.  The FFT kernels
-// reach that at n_fft = 4096 (stft_pair_kernel<0>: 48 KB dynamic + 96 B static), so they opt in whenever their total
-// would pass 48 KB.
-template <typename Kernel>
-static int allow_dynamic_smem(Kernel kernel, size_t dyn, const char* what) {
-  if (dyn <= 32 * 1024) return PWGB_OK;  // far below the limit: skip the attribute query
-  cudaFuncAttributes a;
-  cudaError_t e = cudaFuncGetAttributes(&a, kernel);
-  if (e == cudaSuccess && dyn + a.sharedSizeBytes > 48 * 1024)
-    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
-  if (e != cudaSuccess) {
-    set_error("%s: shared memory opt-in: %s", what, cudaGetErrorString(e));
-    return PWGB_CUDA_ERROR;
-  }
-  return PWGB_OK;
-}
+// The FFT kernels reach the 48 KB shared-memory limit at n_fft = 4096 (stft_pair_kernel<0>: 48 KB dynamic + 96 B
+// static), so they opt in through allow_dynamic_smem (common.cuh) whenever their total would pass it.
 
 static int fill(const pwgb_stft_desc* d, StftK& p) {
   if (!d || d->batch < 0 || d->t <= 0 || d->n_fft < 16 || d->n_fft > 4096 || (d->n_fft & (d->n_fft - 1)) ||

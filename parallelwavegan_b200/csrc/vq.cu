@@ -219,10 +219,9 @@ extern "C" int pwgb_vq_forward(const float* z_e, const float* codebook, int num_
   VqArgs a{z_e, codebook, indices, z_q, dec, l, global_table, g, batch, dim, t, num_codes, local_channels, global_channels, num_global,
            nullptr, 0, nullptr, nullptr, 0};
   const size_t smem = z_e ? (size_t)2 * dim * VQ_TT * sizeof(float) : 0;
-  if (smem > 48 * 1024 && cudaFuncSetAttribute(vq_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-    set_error("vq_forward: cannot reserve %zu bytes of shared memory", smem);
-    return PWGB_CUDA_ERROR;
-  }
+  // the static bd_sh / bk_sh / row arrays count too: D = 184 .. 192 fit 48 KiB dynamically but not in total
+  const int rc = allow_dynamic_smem(vq_forward_kernel, smem, "vq_forward");
+  if (rc) return rc;
   vq_forward_kernel<<<dim3((unsigned)ceil_div(t, VQ_TT), (unsigned)batch), 256, smem, (cudaStream_t)stream>>>(a);
   return check_launch("vq_forward_kernel");
 }
@@ -247,10 +246,8 @@ extern "C" int pwgb_vq_stream_forward(const float* z_e, const float* codebook, i
   VqArgs a{z_e, codebook, indices, nullptr, dec, l, global_table, g, batch, dim, t, num_codes, local_channels, global_channels, num_global,
            l_hist, l_delay, ext->frame, ext->end, ext->lookahead};
   const size_t smem = (size_t)2 * dim * VQ_TT * sizeof(float);
-  if (smem > 48 * 1024 && cudaFuncSetAttribute(vq_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-    set_error("vq_stream: cannot reserve %zu bytes of shared memory", smem);
-    return PWGB_CUDA_ERROR;
-  }
+  const int rc = allow_dynamic_smem(vq_stream_kernel, smem, "vq_stream");
+  if (rc) return rc;
   vq_stream_kernel<<<dim3((unsigned)ceil_div(t, VQ_TT), (unsigned)batch), 256, smem, (cudaStream_t)stream>>>(a);
   return check_launch("vq_stream_kernel");
 }
